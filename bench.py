@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the hot-path benchmark (contract in the task brief, metric from BASELINE.json).
+"""bench.py -- the hot-path benchmark (metric from BASELINE.json).
 
 Headline (N=1): BASELINE.json configs[1] -- 100 M-row, 8-column synthetic table, 2 predicates ->
 GROUP BY (1e5 keys) SUM/AVG/COUNT, in Mrows/s. The same JSON line carries a `bm25` object for
@@ -9,10 +9,13 @@ Mdocs/s (postings scanned per second) -- because BASELINE.json's metric names bo
   value     whole step with inputs resident in HBM, device-timed on the library's stream
   e2e       the same metric through the public host API with HOST buffers (H2D of the step's inputs
             from pinned memory + D2H of the results inside the timed region)
-  roofline  dominant kernel: algorithmic bytes per launch / CUDA-event duration vs MEASURED_PEAKS.json
+  roofline  dominant kernel: algorithmic bytes per launch / CUDA-event duration vs the HBM peak (MEASURED_PEAKS.json
+            when present, else the H100 SXM data sheet's 3.35 TB/s)
   cpu_baseline / --impl reference
             the CPU oracle (oracle/, a restatement of the reference's operators: the reference itself
             needs clang-21 + DuckDB + Abseil and cannot be built here) on the box's host cores.
+
+--steps K sets the step count of every timed loop; --dump-outputs DIR: see dump_outputs().
 """
 import argparse
 import json
@@ -40,7 +43,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -148,17 +151,6 @@ def merge_clocks(a, b):
             "reasons": sorted(set(a["reasons"]) | set(b["reasons"])), "samples": a["samples"] + b["samples"]}
 
 
-def ncu_traffic(kernel, units):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from the committed `ncu --set full`
-    capture of this command (profiles/traffic.json names the capture); null when the workload size differs
-    from the captured one or no capture is recorded."""
-    try:
-        t = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "traffic.json")))[kernel]
-        return t["dram_bytes"] if int(t["units"]) == int(units) else None
-    except Exception:
-        return None
-
-
 _M64 = (1 << 64) - 1
 
 
@@ -224,6 +216,38 @@ def cpu_bm25(seg, dc, sum_dl, n_docs, queries, threads, mode=2):
     t = time.perf_counter()
     hits, n_out, total, scored = orc.bm25_topk_batch([seg], "OR", qt, TOPK, mode=mode, threads=threads)
     return time.perf_counter() - t, hits, n_out, scored
+
+
+DUMP_BUDGET = 64 << 20   # bytes --dump-outputs may write in all
+
+
+def dump_outputs(out_dir, groups, bm25_keys, k):
+    """Writes the last timed step's results as float32 / float64 .npy files, so that two builds run with the same
+    arguments (the inputs come from fixed seeds) can be compared output for output. groups: the GROUP BY rows (GROUP_DTYPE);
+    bm25_keys: [queries, k] uint64 top-k keys as the device left them (score bits << 32 | ~doc, 0 = empty slot), or None.
+    When the top-k of every query does not fit the budget, a fixed seeded sample of queries is written."""
+    os.makedirs(out_dir, exist_ok=True)
+    out = {"groupby_key": groups["key"].astype(np.float64),
+           "groupby_count": groups["count"].astype(np.float64),
+           "groupby_sum_v": np.array([float((int(h) << 64) | (int(l) & _M64)) for l, h in zip(groups["sum_lo"], groups["sum_hi"])],
+                                     dtype=np.float64),
+           "groupby_sum_w": groups["sum_f64"].astype(np.float64),
+           "groupby_cnt_w": groups["cnt_f64"].astype(np.float64)}
+    if bm25_keys is not None:
+        keys = np.ascontiguousarray(bm25_keys).view(np.uint64).reshape(-1, k)
+        room = DUMP_BUDGET - sum(a.nbytes for a in out.values())
+        per_query = 8 + k * (8 + 4)
+        q = np.arange(len(keys))
+        if len(q) * per_query > room:
+            q = np.sort(np.random.default_rng(0x5EDB2026).choice(len(q), room // per_query, replace=False))
+        keys = np.sort(keys[q], axis=1)[:, ::-1]          # canonical order: score desc, doc asc; empty slots last
+        empty = keys == 0
+        doc = (~keys & np.uint64(0xFFFFFFFF)).astype(np.float64)
+        doc[empty] = -1.0
+        score = (keys >> np.uint64(32)).astype(np.uint32).view(np.float32)
+        out.update(bm25_query=q.astype(np.float64), bm25_doc=doc, bm25_score=np.ascontiguousarray(score))
+    for name, arr in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
 
 
 def host_cores():
@@ -317,6 +341,7 @@ def main():
     ap.add_argument("--cpu-rows", type=int, default=100_000_000)
     ap.add_argument("--cpu-queries", type=int, default=256)
     ap.add_argument("--cpu-threads", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's results to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
@@ -478,7 +503,7 @@ def main():
                 torch.cuda.synchronize()
             return escan.groupby_finalize(key_min, span, d_i64.data_ptr(), d_f64.data_ptr(), span)
 
-        e_steps = max(1, min(args.steps, 5))
+        e_steps = args.steps
         e_raw_ms = None
         for use_packed in (False, True):
             eres = e2e_step(use_packed)
@@ -542,13 +567,14 @@ def main():
                                                            "ms_per_step": round(e_raw_ms, 3), "note": "every column copied as raw 8-byte values"}},
         "gpu_launches": int(gb_launches),
         "roofline": {"bound": "hbm", "achieved": round(gb_ach, 1), "peak": hbm_peak, "unit": "GB/s",
-                     "frac": round(gb_ach / hbm_peak, 4), "traffic": ncu_traffic("filter_groupby_tma_kernel", rows), "kernel": "filter_groupby_tma_kernel",
+                     "frac": round(gb_ach / hbm_peak, 4), "kernel": "filter_groupby_tma_kernel",
                      "kernel_ms": round(gb_kernel_ms, 4), "algorithmic_bytes": gb_alg_bytes, "peak_source": peak_src},
     }
     if cpu_gb:
         line["cpu_baseline"] = cpu_gb
 
     oseg = odc = osdl = None
+    bm_keys = None
     # ------------------------------------------------------------------ BM25 (configs[2])
     if not args.skip_bm25:
         n_docs = args.docs
@@ -589,7 +615,7 @@ def main():
             tot = 0.0
             with ClockSampler(local, rank == 0) as cs:
                 for _ in range(steps):
-                    ctx.flush_l2()        # evict the index between timed steps (the 256-term one is about L2-sized)
+                    ctx.flush_l2()        # evict the index from L2 between timed steps
                     barrier()
                     ctx.timer_start()
                     step()
@@ -604,12 +630,14 @@ def main():
         barrier()
         # headline: shipped configuration (block-max pruning on: lead mode for pairs whose long list can be probed)
         bm_ms, tk_ms, mg_ms, bm_launches, clocks2 = timed_bm25(bm25_step, args.steps, "default")
+        if dist is None:
+            bm_keys = keys.cpu().numpy()   # the last timed step's top-k (timed_bm25 waited for the library's stream)
         hits_p, n_p, tot_pruned = [x.copy() for x in batch.run_host()] if dist is None else (None, None, None)   # run_host reuses its buffers
         # roofline leg: the same batch with pruning off -- every list of every query is decoded, so the touched bytes
         # are exactly the lists' encoded bytes (what the numerator claims)
         ctx.set_wand(0)
         bm25_step()
-        ex_ms, ex_tk_ms, _, _, _ = timed_bm25(bm25_step, max(3, args.steps // 2), "exhaustive")
+        ex_ms, ex_tk_ms, _, _, _ = timed_bm25(bm25_step, args.steps, "exhaustive")
         hits, n_out, total = [x.copy() for x in batch.run_host()] if dist is None else (None, None, None)
         ctx.set_wand(2)
         seen_pct = None if dist is not None else round(100.0 * float(tot_pruned.sum()) / float(total.sum()), 1)
@@ -619,7 +647,7 @@ def main():
         batch.run_host()
         barrier()
         ctx.timer_start()
-        e_steps2 = max(1, min(args.steps, 5))
+        e_steps2 = args.steps
         for _ in range(e_steps2):
             if dist is None:
                 hits, n_out, total_e = batch.run_host()
@@ -639,13 +667,13 @@ def main():
                        "exhaustive_ms_per_step": round(ex_ms, 3),
                        "merge": "none" if world == 1 else ("1 NCCL all-gather per step, enqueued by libsdbg.so on the scan's stream" if via_c
                                                          else "torch.distributed all-gather (fallback)"),
-                       "l2": "256 MB write between timed steps (index ~L2-sized)"},
+                       "l2": "256 MB write between timed steps evicts the index from L2"},
             "e2e": {"value": round(world * postings / (be_ms * 1e-3) / 1e6, 1), "unit": "Mdocs/s",
                     "h2d_bytes_per_step": int(len(batch.off) * 4 + (len(batch.off) - 1) * 2 * 32),
                     "d2h_bytes_per_step": nq * TOPK * 8 + nq * 12, "ms_per_step": round(be_ms, 3)},
             "gpu_launches": int(bm_launches),
             "roofline": {"bound": "hbm", "achieved": round(ex_ach, 1), "peak": hbm_peak, "unit": "GB/s", "frac": round(ex_ach / hbm_peak, 4),
-                         "traffic": ncu_traffic("bm25_merge_kernel", n_docs), "kernel": "bm25_merge_kernel<2> (pruning off: every list decoded)",
+                         "kernel": "bm25_merge_kernel<2> (pruning off: every list decoded)",
                          "kernel_ms": round(ex_tk_ms, 3), "merge_kernel_ms": round(mg_ms, 3), "algorithmic_bytes": alg_bytes, "peak_source": peak_src,
                          "note": "touched bytes = encoded doc+freq blocks of both lists of every query + 1 B norm per posting + 12 B per hit; "
                                  "the kernel is bound by instruction issue (see DESIGN.md 4.3), the HBM fraction is reported as asked"},
@@ -668,7 +696,7 @@ def main():
             hkeys = torch.zeros(len(hq) * TOPK, dtype=torch.int64, device=dev)
             hstep = lambda: hb.run_device(0, hkeys.data_ptr())
             hstep()
-            h_ms, h_tk, _, _, _ = timed_bm25(hstep, 3, "hbm")
+            h_ms, h_tk, _, _, _ = timed_bm25(hstep, args.steps, "hbm")
             # parity of this workload: the new kernels against the round-1 window kernel, bit for bit, on a sample
             sample = hq[:64]
             s_new = sdb.ExecuteTopKBatch(hreader, sample, sdb.OR, scorer, TOPK)
@@ -718,7 +746,7 @@ def main():
         run_int, run_flt = sc1.prepare_count_sum(*q_int), sc1.prepare_count_sum(*q_flt)   # arguments marshalled once
         for _ in range(5):
             run_int(); run_flt()
-        reps = 200
+        reps = args.steps
         ctx.sync()
         t = time.perf_counter()
         for _ in range(reps):
@@ -749,9 +777,9 @@ def main():
             os.environ["SDBG_ZONEMAP"] = zm
             scan.groupby_partial(zp, K, key_min, span, V, W_, d_i64.data_ptr(), d_f64.data_ptr())
             ctx.sync(); ctx.timer_start()
-            for _ in range(10):
+            for _ in range(args.steps):
                 scan.groupby_partial(zp, K, key_min, span, V, W_, d_i64.data_ptr(), d_f64.data_ptr())
-            zms = ctx.timer_stop() / 10
+            zms = ctx.timer_stop() / args.steps
             zres[zm] = (zms, ctx.scan_stats(), scan.groupby_finalize(key_min, span, d_i64.data_ptr(), d_f64.data_ptr(), span))
         os.environ.pop("SDBG_ZONEMAP", None)
         (z_on, (zb, zs), zr_on), (z_off, _, zr_off) = zres["1"], zres["0"]
@@ -776,9 +804,12 @@ def main():
         nq4 = 64
         b4 = sdb.PreparedBatch(reader4, [q4] * nq4, sdb.AND, scorer, TOPK, filt=filt)
         b4.run_host()
-        ctx.flush_l2(); ctx.sync(); ctx.timer_start()
-        h4, n4, t4 = b4.run_host()
-        ms4 = ctx.timer_stop()
+        ms4 = 0.0
+        for _ in range(args.steps):
+            ctx.flush_l2(); ctx.sync(); ctx.timer_start()
+            h4, n4, t4 = b4.run_host()
+            ms4 += ctx.timer_stop()
+        ms4 /= args.steps
         p4 = int(sum(int(dc4[t]) for t in q4))
         oseg4, odc4, osdl4 = orc.synth_segment_mt(n_docs, T4, 5, doc0=0, threads=threads)
         assert np.array_equal(odc4, dc4)
@@ -804,6 +835,8 @@ def main():
         seg4.close()
         line["other_configs"] = other
     if rank == 0:
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, res, bm_keys, TOPK)
         emit_line(line)
     if dist is not None:
         dist.barrier()

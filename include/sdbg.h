@@ -1,4 +1,4 @@
-/* include/sdbg.h -- C ABI of libsdbg.so: the B200 (sm_100a) implementation of SereneDB's
+/* include/sdbg.h -- C ABI of libsdbg.so: the H100 (sm_90a) implementation of SereneDB's
  * query-time hot path. Plain pointers and sizes only; no C++/torch types cross this boundary.
  *
  * What each entry point replaces in the reference (paths relative to /root/reference, "irs/" =

@@ -1,4 +1,4 @@
-"""serenedb_b200 -- B200-native (sm_100a) implementation of SereneDB's query-time hot path:
+"""serenedb_b200 -- H100-native (sm_90a) implementation of SereneDB's query-time hot path:
 IResearch BM25 posting scan + top-k, and the `iresearch_scan` columnar filter -> aggregate.
 
 The package is a thin host layer over libsdbg.so (hand-written CUDA behind the C ABI in

@@ -1,5 +1,5 @@
-"""Builds libsdbg.so (the sm_100a kernels + C ABI) in-tree with nvcc. No JIT cache: the .so lives
-under serenedb_b200/_lib/ so it travels to the GPU box with the repo snapshot."""
+"""Builds libsdbg.so (the sm_90a kernels + C ABI) in-tree with nvcc. No JIT cache: the .so lives
+under serenedb_b200/_lib/, next to the package that loads it."""
 import os
 import shutil
 import subprocess
@@ -12,7 +12,7 @@ SOURCES = [os.path.join(CSRC, "sdbg_abi.cu"), os.path.join(CSRC, "posting_format
 DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("bm25_kernels.cuh", "bm25_stream.cuh", "bm25_merge.cuh", "column_kernels.cuh", "device_common.cuh",
                                                    "posting_format.hpp")] + [
     os.path.join(os.path.dirname(HERE), "include", "sdbg.h")]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared", "-cudart", "static"]
 
 
@@ -31,13 +31,13 @@ def is_stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a. Returns the library path."""
+    """Compile every CUDA source for sm_90a. Returns the library path."""
     if not force and not is_stale():
         return LIB_PATH
     nvcc = nvcc_path()
     if nvcc is None:
         if os.path.exists(LIB_PATH):
-            return LIB_PATH  # GPU box without sources changed: use the shipped build
+            return LIB_PATH  # no compiler here and no source changed since the last build: use that build
         raise RuntimeError("nvcc not found and no prebuilt libsdbg.so")
     os.makedirs(LIB_DIR, exist_ok=True)
     tmp = LIB_PATH + ".tmp"

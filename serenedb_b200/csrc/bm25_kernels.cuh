@@ -1,4 +1,4 @@
-// bm25_kernels.cuh -- sm_100a kernels for the BM25 posting scan + top-k.
+// bm25_kernels.cuh -- sm_90a kernels for the BM25 posting scan + top-k.
 //
 // Reference behaviour being reproduced (paths relative to /root/reference/libs/iresearch/include/iresearch):
 //   decode      formats/posting/format_block_128.hpp:475-636 (ReadTailDelta / ReadTail)

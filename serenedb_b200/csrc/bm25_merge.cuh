@@ -1,9 +1,7 @@
 // bm25_merge.cuh -- the exhaustive form of the warp-autonomous scan (bm25_stream.cuh): every list of a 1..4-term
 // disjunction is streamed and merged, nothing is pruned or probed. Per-term stream state lives in registers (the term
 // count is a template parameter) and there is no probe / block-max code in the loop, which keeps it at the size the
-// 32 KB instruction cache and the 80-register budget allow: this is the fastest shape measured for the merge itself
-// (profiles/r2_stream_history.txt: occupancy 2 / 3 / 4 CTAs per SM, score table on / off, a rolled single copy of the
-// block advance and earlier norm loads were all measured against it). Used when block-max pruning is off or cannot apply yet (the threshold of a query
+// instruction cache and the 80-register budget allow. Used when block-max pruning is off or cannot apply yet (the threshold of a query
 // is still below the bound of its densest list); bm25_stream_kernel takes over once it can (lead list + probes).
 // Helpers (StreamCtl, unpack4s, decode_block_global, warp_first_block, stream_compact / stream_rendezvous) are shared.
 #pragma once

@@ -1,4 +1,4 @@
-// bm25_stream.cuh -- warp-autonomous BM25 scan + score + top-k for disjunctions of 1..4 terms (sm_100a).
+// bm25_stream.cuh -- warp-autonomous BM25 scan + score + top-k for disjunctions of 1..4 terms (sm_90a).
 //
 // Reference behaviour being reproduced (paths relative to /root/reference/libs/iresearch/include/iresearch):
 //   block walk    formats/posting/iterator_doc.hpp:309-430 (Collect / ScoreBlock / ProcessBatch: one 128-posting

@@ -1,4 +1,4 @@
-// column_kernels.cuh -- sm_100a kernels for the columnar filter / aggregate path.
+// column_kernels.cuh -- sm_90a kernels for the columnar filter / aggregate path.
 //
 // Reference behaviour (paths relative to /root/reference):
 //   scan+filter   server/connector/full_scanner.cpp:81-147 (FullScanner::Scan: FilterWindow narrows a
@@ -333,7 +333,7 @@ filter_groupby_kernel(const GroupByParams P) {
 // column tiles into a kStages-deep shared-memory ring with 1-D bulk async copies
 // (cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes -> SASS UBLKCP) signalled through
 // mbarriers, and the consumer warps evaluate predicates from shared memory and issue the REDs. In-flight
-// bytes per SM = CTAs/SM * kStages * tile bytes (2 * 4 * 20 KB = 160 KB), independent of how far the
+// bytes per SM = CTAs/SM * kStages * tile bytes (3 * 3 * 20 KB = 180 KB), independent of how far the
 // consumers have got. Persistent CTAs, tiles handed out round-robin.
 // ------------------------------------------------------------------------------------------
 constexpr int kMaxStreams = 7;   // up to 4 predicate columns + key + sum_int + sum_f64 (deduplicated)
@@ -440,9 +440,8 @@ __device__ __forceinline__ uint32_t range2(const unsigned char* col, uint32_t r,
 
 // kQuad (opt-in, SDBG_GROUPBY_QUAD=1): every accumulator of the slot is an integer (fixed-point SUM(double) or
 // no double sum), and the four words of a row's slot are updated by four adjacent lanes of ONE RED
-// instruction: one L2 request per passing row, sums independent of update order (bit-reproducible). Measured
-// slower than separate REDs on configs[1] (1.04 vs 0.87 ms): the compaction through shared memory and the
-// limb arithmetic cost the consumer warps more than the saved requests (profiles/r1_groupby_red_experiments.txt).
+// instruction: one L2 request per passing row, sums independent of update order (bit-reproducible), at the
+// cost of a compaction through shared memory and limb arithmetic in the consumer warps. Off by default.
 template <int kStages, int kTileRows, int kConsumerWarps, bool kPacked, bool kQuad>
 __global__ void __launch_bounds__((kConsumerWarps + 1) * 32)
 filter_groupby_tma_kernel(const TmaGroupByParams P) {

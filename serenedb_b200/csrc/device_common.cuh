@@ -1,4 +1,4 @@
-// device_common.cuh -- small device helpers shared by the sm_100a kernels.
+// device_common.cuh -- small device helpers shared by the sm_90a kernels.
 #pragma once
 
 #include <cuda_runtime.h>

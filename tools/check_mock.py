@@ -1,6 +1,6 @@
 """Diffs every `//@ref <file>:<first>-<last>` block of serenedb_b200/host/irs_mock.hpp against the cited lines of the
 reference tree: each block's declarations (comments and whitespace stripped) must appear, in order, in those lines.
-Exit code 0 = the mock's tagged surface is the reference's. Usage: check_mock.py [/root/reference]"""
+Exit code 0 = the mock's tagged surface is the reference's. Usage: check_mock.py <SereneDB source tree>"""
 import os, re, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -41,7 +41,7 @@ def check(ref_root, mock_path=os.path.join(ROOT, "serenedb_b200", "host", "irs_m
 
 
 if __name__ == "__main__":
-    ref_root = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+    ref_root = sys.argv[1]
     nb, nd, problems = check(ref_root)
     for p in problems:
         print("MISMATCH", p)

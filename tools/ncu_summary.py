@@ -1,4 +1,4 @@
-"""Prints the metrics the profiles/ summaries quote from an `ncu --page raw --csv` dump (stdin or file)."""
+"""Prints the headline metrics of an `ncu --page raw --csv` dump (stdin or file)."""
 import csv, sys
 rows = list(csv.reader(open(sys.argv[1]) if len(sys.argv) > 1 else sys.stdin))
 hdr, units = rows[0], rows[1]
