@@ -105,6 +105,11 @@ int sdbg_stage_docs_mask(sdbg_segment*, const uint32_t* deleted_docs, size_t n);
    0.75). Block-max pruning is used only for queries whose scorer has the same b -- the check Scorer::equals makes in
    PostingsReaderImpl::WandIterator (formats/posting/reader.hpp:457-501); any other scorer is evaluated exhaustively. */
 int sdbg_segment_set_wand_b(sdbg_segment*, float wand_b);
+/* The average field length the segment's block-max entries were chosen with (the writer's NormReader::GetAvg,
+   norm_reader_impl.hpp:83-88). sdbg_stage_norms sets it from the staged norms (sum / non-zero count), so only a writer
+   that used another average needs this; call it after sdbg_stage_norms. 0 = no norms. Queries score the entries as upper
+   bounds under their own (corpus-wide) average length, so pruning stays exact when the two averages differ. */
+int sdbg_segment_set_wand_avg_dl(sdbg_segment*, float avg_dl);
 /* Zonemap effect of the last GROUP BY scan: 2048-row blocks judged / proven dead from their min-max (never read). */
 int sdbg_scan_stats(sdbg_ctx*, uint64_t* blocks_total, uint64_t* blocks_skipped);
 /* The context a segment was created in (for sdbg_last_error after a failed call that only has segments at hand). */

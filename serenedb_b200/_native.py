@@ -73,6 +73,7 @@ SIGNATURES = {
     "sdbg_bm25_collect": (C.c_int, [C.c_uint64, C.c_uint64, C.c_uint64, C.c_float, C.c_float, C.POINTER(BM25Term)]),
     "sdbg_stage_docs_mask": (C.c_int, [_vp, _vp, _sz]),
     "sdbg_segment_set_wand_b": (C.c_int, [_vp, C.c_float]),
+    "sdbg_segment_set_wand_avg_dl": (C.c_int, [_vp, C.c_float]),
     "sdbg_segment_context": (_vp, [_vp]),
     "sdbg_tfidf_collect": (C.c_int, [C.c_uint64, C.c_uint64, _vp]),
     "sdbg_tfidf_topk_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, C.c_int, _vp, C.c_uint32, C.c_float, _vp, _vp, _vp]),

@@ -43,7 +43,7 @@ struct FilterDev {  // one pushed column predicate for the hybrid path
   double lo_f, hi_f;
 };
 
-struct QTermDev {  // one term of one query, 32 bytes
+struct QTermDev {  // one term of one query over one segment, 40 bytes
   uint32_t blk_begin;  // first BlockDesc of the term
   uint32_t nblk;
   float c0;            // boost*(k1+1)*idf   (bm25.cpp:224)
@@ -52,6 +52,9 @@ struct QTermDev {  // one term of one query, 32 bytes
   uint32_t docs_count;
   uint32_t root_freq, root_norm;   // block-max pair of the whole list (0,0 = unknown); bit 31 of root_freq: the list's blocks
                                    // are bitsets with random-access freqs, i.e. cheap to probe (driver mode is worth it)
+  // norm_const / norm_length for scoring a block-max pair as an upper bound (fill_qterm, sdbg_abi.cu): the pair maximises
+  // BM25 under the segment's own average length, which need not be the query's corpus-wide one
+  float bound_const, bound_length;
 };
 
 constexpr uint32_t kMaxQueryTerms = 16;
@@ -202,6 +205,12 @@ __device__ __forceinline__ float bm25(uint32_t freq, uint32_t norm, float c0, fl
   if (nl != nl) return __fsub_rn(c0, __fdiv_rn(c0, __fadd_rn(1.f, __fdiv_rn(static_cast<float>(freq), nc))));
   const float c1 = __fadd_rn(nc, __fmul_rn(nl, static_cast<float>(norm)));
   return __fsub_rn(c0, __fdiv_rn(__fmul_rn(c0, c1), __fadd_rn(c1, static_cast<float>(freq))));
+}
+
+// Upper bound of the query-time score of every posting that a block-max pair (freq, norm) stands for. Pruning runs
+// only for the BM25 form, so the bound constants are always finite.
+__device__ __forceinline__ float pair_bound(uint32_t freq, uint32_t norm, const QTermDev& qt) {
+  return bm25(freq, norm, qt.c0, qt.bound_const, qt.bound_length);
 }
 
 // The BM25 form alone (bm25.cpp:105-106), for kernels the host only dispatches with k != 0, b != 0 (bm25_merge_kernel,
@@ -450,7 +459,7 @@ bm25_topk_kernel(const TopkParams P) {
     const QTermDev& L = s_qt[T - 1u];
     // driver mode only for a probe-friendly largest list: a probe into a bit-packed block costs a block decode
     s_ubL = (can_drive && (L.root_freq >> 31) && (L.root_freq & 0x7FFFFFFFu) != 0u)
-                ? bm25(L.root_freq & 0x7FFFFFFFu, L.root_norm, L.c0, L.norm_const, L.norm_length)
+                ? pair_bound(L.root_freq & 0x7FFFFFFFu, L.root_norm, L)
                                               : __int_as_float(0x7f800000);
   }
   __syncthreads();
@@ -460,7 +469,8 @@ bm25_topk_kernel(const TopkParams P) {
   // without being handed to the decoders (UpdateWindowScores, max_score_iterator.hpp:437).
   auto plan = [&](uint32_t lo, uint32_t buf) -> uint32_t {
     const float thr = __uint_as_float(uint32_t(s_theta >> 32));
-    if (can_drive && !s_driver && thr > s_ubL) { if (lane == 0) s_driver = 1u; }   // one-way switch (the threshold only rises)
+    // one-way switch (the threshold only rises); every bound test carries the stream kernels' rounding margin
+    if (can_drive && !s_driver && thr > __fmul_rn(s_ubL, 1.000001f)) { if (lane == 0) s_driver = 1u; }
     __syncwarp();
     const bool driver = kDrive && s_driver != 0u;
     const uint32_t Tp = driver ? T - 1u : T;             // lists that get planner lanes
@@ -493,7 +503,7 @@ bm25_topk_kernel(const TopkParams P) {
       if (prune) {
         if (overlap) {
           const uint2 fn = __ldg(P.seg.blk_max + gblk);
-          if (fn.x != 0u) bound = bm25(fn.x, fn.y, s_qt[t].c0, s_qt[t].norm_const, s_qt[t].norm_length);
+          if (fn.x != 0u) bound = pair_bound(fn.x, fn.y, s_qt[t]);
         }
         // per-term window bound = max over the term's blocks that reach into the window (0 if none)
         s_item_bound[buf][lane] = overlap ? bound : 0.f;
@@ -511,7 +521,7 @@ bm25_topk_kernel(const TopkParams P) {
         float sum = 0.f;
         for (uint32_t u = 0; u < Tp; ++u) sum = __fadd_rn(sum, u == t ? bound : s_term_ub[buf][u]);
         if (driver) sum = __fadd_rn(sum, s_ubL);
-        if (overlap && sum < thr) overlap = false;
+        if (overlap && __fmul_rn(sum, 1.000001f) < thr) overlap = false;
         __syncwarp();
       }
       const uint32_t ov = __ballot_sync(kFull, overlap);
@@ -687,7 +697,7 @@ bm25_topk_kernel(const TopkParams P) {
         const uint4 pd = ld_ro_v4(LB + bl);
         if (!(pd.z < d)) continue;
         const uint2 fn = __ldg(P.seg.blk_max + L.blk_begin + bl);
-        if (fn.x != 0u && __fadd_rn(partial, bm25(fn.x, fn.y, L.c0, L.norm_const, L.norm_length)) < thr) {
+        if (fn.x != 0u && __fmul_rn(__fadd_rn(partial, pair_bound(fn.x, fn.y, L)), 1.000001f) < thr) {
           e_doc[e] = kPadDoc;                                             // cannot qualify even with this block's best
           continue;
         }
@@ -733,7 +743,7 @@ bm25_topk_kernel(const TopkParams P) {
           have_blk = bl; have_f = false;
           if (!(pd.z < d && d <= pd.y)) { have_blk = 0xFFFFFFFFu; continue; }   // d falls between blocks: not in L
           const uint2 fn = __ldg(P.seg.blk_max + L.blk_begin + bl);
-          if (fn.x != 0u && __fadd_rn(partial, bm25(fn.x, fn.y, L.c0, L.norm_const, L.norm_length)) < thr) {
+          if (fn.x != 0u && __fmul_rn(__fadd_rn(partial, pair_bound(fn.x, fn.y, L)), 1.000001f) < thr) {
             e_doc[e] = kPadDoc;                                          // cannot qualify even with this block's best
             have_blk = 0xFFFFFFFFu;
             continue;

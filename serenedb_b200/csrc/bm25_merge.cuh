@@ -133,7 +133,7 @@ bm25_merge_kernel(const TopkParams P) {
       float sfx1 = 0.f;
       for (uint32_t t = T; t-- > 1u;) {
         const uint32_t rf = s_qt[t].root_freq & 0x7FFFFFFFu;
-        const float ub = (P.seg.blk_max != nullptr && rf != 0u) ? bm25(rf, s_qt[t].root_norm, s_qt[t].c0, s_qt[t].norm_const, s_qt[t].norm_length)
+        const float ub = (P.seg.blk_max != nullptr && rf != 0u) ? pair_bound(rf, s_qt[t].root_norm, s_qt[t])
                                                                  : __int_as_float(0x7f800000);
         sfx1 = __fadd_rn(sfx1, ub);
       }

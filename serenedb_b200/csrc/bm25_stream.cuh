@@ -436,7 +436,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
     s_sfx[n_terms] = 0.f;
     for (uint32_t t = n_terms; t-- > 0;) {
       const uint32_t rf = s_qt[t].root_freq & 0x7FFFFFFFu;
-      const float ub = (P.wand && P.seg.blk_max != nullptr && rf != 0u) ? bm25(rf, s_qt[t].root_norm, s_qt[t].c0, s_qt[t].norm_const, s_qt[t].norm_length)
+      const float ub = (P.wand && P.seg.blk_max != nullptr && rf != 0u) ? pair_bound(rf, s_qt[t].root_norm, s_qt[t])
                                                                        : __int_as_float(0x7f800000);
       acc = __fadd_rn(acc, ub);
       s_sfx[t] = acc;
@@ -608,7 +608,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
       if (!kAnd && P.wand && !(P.wand & 16) && E == 1u && first + lane < s_qt[0].nblk) {
         const uint2 fn = __ldg(P.seg.blk_max + s_qt[0].blk_begin + first + lane);
         if (fn.x != 0u) {
-          const float bound = bm25(fn.x, fn.y, s_qt[0].c0, s_qt[0].norm_const, s_qt[0].norm_length);
+          const float bound = pair_bound(fn.x, fn.y, s_qt[0]);
           skip = __fmul_rn(__fadd_rn(bound, s_sfx[1]), 1.000001f) < __uint_as_float(theta_hi);
         }
       }

@@ -107,6 +107,9 @@ struct sdbg_segment {
   uint64_t arena_bytes = 0, n_blocks = 0, n_postings = 0;
   bool has_wand = false;
   float wand_b = 0.75f;   // the b the block-max (freq, norm) pairs were chosen for (BM25 default unless told otherwise)
+  // the average field length the pairs were chosen with (PostingWriter::feed); 0 = none: without norms every doc scores
+  // with norm 1, so a pair's order cannot depend on the average length
+  float wand_avg_dl = 0.f;
   // norms
   void* d_norms = nullptr;
   uint32_t norm_width = 0;
@@ -348,6 +351,12 @@ extern "C" int sdbg_segment_set_wand_b(sdbg_segment* s, float wand_b) {
   return SDBG_OK;
 }
 
+extern "C" int sdbg_segment_set_wand_avg_dl(sdbg_segment* s, float avg_dl) {
+  if (!s || !(avg_dl >= 0.f) || avg_dl == std::numeric_limits<float>::infinity()) return SDBG_EINVAL;
+  s->wand_avg_dl = avg_dl;
+  return SDBG_OK;
+}
+
 extern "C" int sdbg_stage_docs_mask(sdbg_segment* s, const uint32_t* deleted_docs, size_t n) {
   if (!s || (!deleted_docs && n)) return SDBG_EINVAL;
   sdbg_ctx* c = s->ctx;
@@ -444,12 +453,21 @@ extern "C" int sdbg_stage_norms(sdbg_segment* s, const uint8_t* bytes, size_t n,
       }
     src = flat.data();
   }
+  // The average length the writer chose the block-max pairs with: NormReader::GetAvg (norm_reader_impl.hpp:83-88), as
+  // PostingWriter computes it. A writer that used another average overrides it with sdbg_segment_set_wand_avg_dl.
+  uint64_t sum = 0, nonzero = 0;
+  for (uint64_t r = 0; r < rows; ++r) {
+    uint32_t v = 0;
+    std::memcpy(&v, src + r * width, width);
+    sum += v; nonzero += v != 0;
+  }
   CU(c, cudaSetDevice(c->device));
   if (s->d_norms) { cudaFree(s->d_norms); s->d_norms = nullptr; }
   CU(c, cudaMalloc(&s->d_norms, rows * width + 16));
   CU(c, cudaMemcpyAsync(s->d_norms, src, rows * width, cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
   s->norm_width = width;
+  s->wand_avg_dl = nonzero ? float(double(sum) / double(nonzero)) : 0.f;
   return SDBG_OK;
 }
 
@@ -692,6 +710,20 @@ int filter_view(sdbg_segment* s, const sdbg_col_pred* f, FilterDev* out) {
 constexpr int kMaxCopyEvents = 16;
 constexpr float kTfidfK1 = -1.f;   // internal selector of the TFIDF scorer (it has no k / b): see sdbg_tfidf_topk_batch
 
+// norm_const / norm_length that turn the segment's block-max pairs into upper bounds for a query whose BM25 constants
+// are nc = k - k*b and nl = k*b / A_q (A_q: the corpus-wide average length). The writer kept the pair (f*, n*) with the
+// largest f / ((1-b) A_s + b n) under the segment's own average A_s. With M = max(A_q, A_s), every posting of the block
+// scores at most the BM25 form at (f*, n*) with nc_b = k (1-b) A_s / M and nl_b = k b / M. In terms of nl and
+// nl_s = k b / A_s: nl_b = min(nl, nl_s) and nc_b = nc * min(1, nl / nl_s). When A_s == A_q these are the query's own
+// constants, bit for bit; only BM25-form queries prune, so only they use the result.
+void bound_consts(const sdbg_segment* s, float k1, float b, float nc, float nl, float& bnc, float& bnl) {
+  bnc = nc; bnl = nl;
+  if (!(s->wand_avg_dl > 0.f)) return;        // no norms: every norm is 1 and the pair order cannot depend on A_s
+  const float nl_s = (k1 * b) / s->wand_avg_dl;
+  if (nl < nl_s) bnc = nc * (nl / nl_s);       // A_q > A_s
+  else bnl = nl_s;                             // A_q <= A_s
+}
+
 // Device-side descriptor of one query term over one segment (the caller has checked the term id).
 void fill_qterm(const sdbg_segment* s, const sdbg_bm25_term& t, float k1, float b, QTermDev& d) {
   d.blk_begin = s->term_blk_begin[t.term];
@@ -705,6 +737,8 @@ void fill_qterm(const sdbg_segment* s, const sdbg_bm25_term& t, float k1, float 
   }
   else if (k1 == 0.f) d.c0 = 0.f;                                       // BM1: Bm1Score without a filter boost scores 0 (bm25.cpp:118-126)
   else if (b == 0.f) d.norm_length = std::numeric_limits<float>::quiet_NaN();   // BM15 form (device-side marker, see bm25())
+  d.bound_const = d.norm_const; d.bound_length = d.norm_length;
+  if (k1 != kTfidfK1 && k1 != 0.f && b != 0.f) bound_consts(s, k1, b, d.norm_const, d.norm_length, d.bound_const, d.bound_length);
   d.docs_count = s->term_docs[t.term];
   d.root_freq = s->term_max[t.term].freq & 0x7FFFFFFFu; d.root_norm = s->term_max[t.term].norm;
   if (t.term < s->term_probe.size() && s->term_probe[t.term]) d.root_freq |= 0x80000000u;   // probe-friendly list (driver mode)
@@ -816,7 +850,9 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
           if (s->term_docs[ta->term] > s->term_docs[tb->term]) std::swap(ta, tb);       // ta = short list
           const MaxPair root = tb->term < s->term_max.size() ? s->term_max[tb->term] : MaxPair{0, 0};
           if (root.freq != 0) {
-            const float c0b = tb->boost * (k1 + 1) * tb->idf, c1b = tb->norm_const + tb->norm_length * float(root.norm);
+            float bnc, bnl;
+            bound_consts(s, k1, b, tb->norm_const, tb->norm_length, bnc, bnl);
+            const float c0b = tb->boost * (k1 + 1) * tb->idf, c1b = bnc + bnl * float(root.norm);
             const float ub_b = c0b - c0b * c1b / (c1b + float(root.freq));
             const float c0a = ta->boost * (k1 + 1) * ta->idf, c1a = ta->norm_const + ta->norm_length * (ta->norm_length > 0.f ? (k1 * b) / ta->norm_length : 1.f);
             const float typ_a = c0a - c0a * c1a / (c1a + 1.f);                           // freq 1 at the average length

@@ -239,6 +239,11 @@ class Segment:
         rg = N.NormRg(byte_width, self.n_docs, 0)
         N.check(N.lib().sdbg_stage_norms(self._h, _ptr(norm_bytes), len(norm_bytes), C.byref(rg), 1), self.ctx._h)
 
+    def set_wand_avg_dl(self, avg_dl):
+        """Average field length the block-max pairs were chosen with, when the writer did not use the staged norms'
+        own average (stage_norms sets that one). Call after stage_norms."""
+        N.check(N.lib().sdbg_segment_set_wand_avg_dl(self._h, float(avg_dl)), self.ctx._h)
+
     def stage_column(self, field, values, validity=None):
         """values: numpy array (int64/float64/int32) or a (host_ptr, dtype, rows) triple of pinned memory."""
         if isinstance(values, tuple):
