@@ -186,6 +186,27 @@ int sdbg_tfidf_topk_batch(sdbg_segment* const* segs, size_t n_segs, int kind, co
 int sdbg_bm25_scan(sdbg_segment*, int kind, const sdbg_bm25_term* terms, size_t n_terms, float k1, float b,
                    const sdbg_col_pred* filt, uint32_t doc_min, uint32_t doc_max, uint32_t* out_docs, float* out_scores,
                    uint64_t cap, uint64_t* n_out);
+/* Excluded terms (`a & b & !c`, `(a | b) & !c`: the exclusion iterator the reference builds for an And with Not children,
+ * irs/search/exclusion.hpp). A query is its positive part (the OR / AND of terms above) minus every doc that occurs in
+ * any list of its excluded terms; the deleted-docs mask and the hybrid filter apply as before. Scores come from the
+ * positive terms only, bit for bit as without exclusions: excluded terms carry only their term id. An excluded id the
+ * segment does not hold (>= its term count, or no postings) excludes nothing there; an excluded term that is also a
+ * positive one empties an AND and leaves an OR the docs of its other terms. A query with no positive term is not
+ * supported. total_matches follows sdbg_bm25_topk: exact with pruning off, a lower bound with it.
+ * sdbg_bm25_topk_batch_excl: terms / term_off as sdbg_bm25_topk_batch; query q excludes
+ * excl_terms[excl_off[q] .. excl_off[q+1]) (0..16 term ids; excl_off has n_queries + 1 entries). k1 = -1 selects TFIDF as
+ * there. An empty set everywhere gives exactly sdbg_bm25_topk_batch's result. More than 16 excluded terms in a query:
+ * SDBG_EUNSUPPORTED; a decreasing excl_off, or NULL excl_terms with a non-empty range: SDBG_EINVAL.
+ * sdbg_bm25_scan_excl: sdbg_bm25_scan minus the docs of excl_terms[0 .. n_excl).
+ * sdbg_bm25_topk_batch_device and sdbg_dist_bm25_topk_batch have no exclusion form yet; they run the same dispatch as
+ * sdbg_bm25_topk_batch, so adding one means passing the exclusion lists through. */
+int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
+                              const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off,
+                              float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in,
+                              sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches);
+int sdbg_bm25_scan_excl(sdbg_segment*, int kind, const sdbg_bm25_term* terms, size_t n_terms,
+                        const uint32_t* excl_terms, size_t n_excl, float k1, float b, const sdbg_col_pred* filt,
+                        uint32_t doc_min, uint32_t doc_max, uint32_t* out_docs, float* out_scores, uint64_t cap, uint64_t* n_out);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

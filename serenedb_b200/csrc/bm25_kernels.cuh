@@ -325,6 +325,11 @@ struct TopkParams {
   float* emit_scores = nullptr;
   unsigned long long* emit_count = nullptr;
   unsigned long long emit_cap = 0;
+  // Excluded terms (the NOT children of an And, irs search/exclusion.hpp): query q rejects every doc that occurs in one
+  // of the lists excl[excl_off[q] .. excl_off[q + 1]), each {first BlockDesc, blocks} in this segment (0 blocks: a term
+  // the segment does not hold). Excluded terms never score. Null: no query of the call excludes anything.
+  const uint2* excl = nullptr;
+  const uint32_t* excl_off = nullptr;
   uint32_t k;
   uint32_t cap;                // candidate buffer capacity, power of two, > k
   int32_t conjunction;         // 0 OR, 1 AND
@@ -391,8 +396,96 @@ __device__ __forceinline__ uint32_t find_block_from(const uint4* LB, uint32_t b0
   return l;
 }
 
-// kDrive compiles the driver-mode code (pruning level 2) in; the default kernel stays free of its registers.
-template <uint32_t kBudget, bool kDrive>
+__device__ __forceinline__ uint32_t svb_value_at(const uint8_t* bytes, uint32_t len, uint32_t idx_or_doc, bool by_doc, bool delta,
+                                                 uint32_t prev, uint32_t* idx_out) {
+  // by_doc: walks the doc stream until the running id reaches idx_or_doc (returns the id found or 0xFFFFFFFF);
+  // else returns value number idx_or_doc.
+  const uint32_t nctl = (len + 3u) >> 2;
+  uint32_t pos = nctl, acc = prev;
+  for (uint32_t i = 0; i < len; ++i) {
+    const uint32_t c = (uint32_t(__ldg(bytes + (i >> 2))) >> (2u * (i & 3u))) & 3u;
+    uint32_t x = 0;
+    for (uint32_t k = 0; k <= c; ++k) x |= uint32_t(__ldg(bytes + pos + k)) << (8u * k);
+    pos += c + 1u;
+    if (by_doc) {
+      acc = delta ? acc + x : x;
+      if (acc >= idx_or_doc) { *idx_out = i; return acc; }
+    } else if (i == idx_or_doc) {
+      return x;
+    }
+  }
+  return 0xFFFFFFFFu;
+}
+
+// Position of doc `d` inside block `desc` (prev_last < d <= last_doc), or false when the block does not hold it.
+__device__ __forceinline__ bool block_find_doc(const PostingsDev& S, const uint4& desc, uint32_t gblk, uint32_t d, uint32_t& idx) {
+  const uint4* p = S.arena + desc.x;
+  const uint32_t enc = desc_doc_enc(desc.w), len = desc_len(desc.w), prev = desc.z;
+  if (enc >= 8u) {                                   // bit-packed gaps: row r = postings 4r .. 4r+3
+    const uint32_t b = enc - 6u;
+    const uint4 an = __ldg(S.anchors + gblk);
+    const uint32_t qd = (d > an.x ? 1u : 0u) + (d > an.y ? 1u : 0u) + (d > an.z ? 1u : 0u);
+    uint32_t acc = qd == 0u ? prev : qd == 1u ? an.x : qd == 2u ? an.y : an.z;
+    const uint32_t mask = (1u << b) - 1u;
+    for (uint32_t r = 8u * qd; r < 8u * qd + 8u; ++r) {
+      const uint32_t bit = r * b, w = bit >> 5, sh = bit & 31u;
+      const uint4 lo = __ldg(p + w), hi = __ldg(p + min(w + 1u, b - 1u));
+      acc += __funnelshift_r(lo.x, hi.x, sh) & mask; if (acc >= d) { idx = 4u * r; return acc == d; }
+      acc += __funnelshift_r(lo.y, hi.y, sh) & mask; if (acc >= d) { idx = 4u * r + 1u; return acc == d; }
+      acc += __funnelshift_r(lo.z, hi.z, sh) & mask; if (acc >= d) { idx = 4u * r + 2u; return acc == d; }
+      acc += __funnelshift_r(lo.w, hi.w, sh) & mask; if (acc >= d) { idx = 4u * r + 3u; return acc == d; }
+    }
+    return false;
+  }
+  if (enc == 4u) return bitset_rank(S.arena, desc, d, idx);
+  if (enc >= 1u && enc <= 3u) {                       // constant gap g: ids prev + g, prev + 2g, ...
+    const uint32_t g = same_value(p, enc);
+    const uint32_t off = d - prev;
+    if (g == 0u || off % g != 0u) return false;
+    idx = off / g - 1u;
+    return idx < len;
+  }
+  if (enc == 0u) {                                    // raw ids
+    const uint32_t* a = reinterpret_cast<const uint32_t*>(p);
+    uint32_t l = 0, r = len;
+    while (l < r) { const uint32_t m = (l + r) >> 1; if (__ldg(a + m) < d) l = m + 1u; else r = m; }
+    idx = l;
+    return l < len && __ldg(a + l) == d;
+  }
+  return svb_value_at(reinterpret_cast<const uint8_t*>(p), len, d, true, enc == 7u, prev, &idx) == d;
+}
+
+// Membership only: does the list {first BlockDesc, blocks} hold doc d? Block search from `hint` (a block index within the
+// list; on return the block that was searched), then the in-block search -- no frequency, no score. Excluded terms.
+__device__ __forceinline__ bool probe_contains(const PostingsDev& S, uint2 list, uint32_t d, uint32_t hint, uint32_t& found_blk) {
+  const uint4* B = S.blocks + list.x;
+  const uint32_t n = list.y;
+  if (n == 0u) { found_blk = 0u; return false; }
+  const uint32_t l = find_block_from(B, 0u, n, min(hint, n - 1u), d);
+  found_blk = min(l, n - 1u);
+  if (l >= n) return false;
+  const uint4 desc = __ldg(B + l);
+  if (d <= desc.z) return false;                       // d lies between two blocks
+  uint32_t idx = 0;
+  return block_find_doc(S, desc, list.x + l, d, idx);
+}
+
+// One thread: does any of the n excluded lists hold doc d (legacy window kernel's emit step)? Each list is searched from
+// its first block. Takes the views by value so that the kernel's parameter block is not copied to local memory.
+__device__ __noinline__ bool excluded_doc(const uint4* arena, const uint4* blocks, const uint4* anchors, const uint2* ex, uint32_t n,
+                                          uint32_t d) {
+  PostingsDev S{};
+  S.arena = arena; S.blocks = blocks; S.anchors = anchors;
+  for (uint32_t x = 0; x < n; ++x) {
+    uint32_t blk = 0;
+    if (probe_contains(S, ex[x], d, 0u, blk)) return true;
+  }
+  return false;
+}
+
+// kDrive compiles the driver-mode code (pruning level 2) in; the default kernel stays free of its registers. kExcl: the
+// queries of the launch exclude terms (TopkParams::excl); likewise kept out of the other instantiations.
+template <uint32_t kBudget, bool kDrive, bool kExcl = false>
 __global__ void __launch_bounds__(kTopkThreads)
 bm25_topk_kernel(const TopkParams P) {
   constexpr uint32_t kEntries = kBudget * 128u;
@@ -420,12 +513,15 @@ bm25_topk_kernel(const TopkParams P) {
   __shared__ uint32_t s_ncand, s_matched;
   __shared__ unsigned long long s_theta;
   __shared__ uint32_t s_hist[258];
+  __shared__ uint2 s_ex[kExcl ? kMaxQueryTerms : 1];   // excluded lists of the query (TopkParams::excl)
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint4 work = P.work[blockIdx.x];
   const uint32_t q = work.x, chunk = work.z;   // work item = {query, first doc, docs, candidate list}
   const uint32_t t0 = P.qterm_off[q];
   const uint32_t T = min(P.qterm_off[q + 1] - t0, kMaxQueryTerms);
+  const uint32_t x0 = kExcl ? P.excl_off[q] : 0u;
+  const uint32_t n_ex = kExcl ? min(P.excl_off[q + 1] - x0, kMaxQueryTerms) : 0u;
   const uint32_t m = max(1u, kBudget / T);                       // block budget per term
   const unsigned long long first64 = work.y;
   const bool chain_empty = first64 > P.seg.n_docs;
@@ -434,6 +530,7 @@ bm25_topk_kernel(const TopkParams P) {
 
   for (uint32_t i = tid; i < P.cap; i += blockDim.x) cand[i] = 0ull;
   if (tid < T) s_qt[tid] = P.qterms[t0 + tid];
+  if (kExcl && tid < n_ex) s_ex[tid] = P.excl[x0 + tid];
   if (tid == 0) { s_ncand = 0u; s_matched = 0u; s_theta = 0ull; }
   __syncthreads();
 
@@ -772,7 +869,7 @@ bm25_topk_kernel(const TopkParams P) {
     const uint32_t n_entries = n_items * 128u;
     const uint32_t emit_begin = P.conjunction ? s_phase[buf][T - 1u] * 128u : 0u;  // AND: only the last term's slots can be complete (never in driver mode)
     bool first_pass = true;
-    const bool plain = !P.conjunction && P.filt.values == nullptr && P.seg.deleted == nullptr;   // disjunction, no table filter, no deletes: 4 entries per lane
+    const bool plain = !P.conjunction && P.filt.values == nullptr && P.seg.deleted == nullptr && !kExcl;   // disjunction, no table filter, no deletes, no exclusions: 4 entries per lane
     for (;;) {
       const unsigned long long theta = s_theta;
       const uint32_t theta_hi = uint32_t(theta >> 32);
@@ -821,6 +918,7 @@ bm25_topk_kernel(const TopkParams P) {
         if (live && P.conjunction) live = e_cnt[e] == T - 1u;
         if (live && P.seg.deleted != nullptr) live = ((__ldg(P.seg.deleted + (d >> 5)) >> (d & 31u)) & 1u) == 0u;   // MaskDocIterator: neither scored nor counted
         if (live && P.filt.values != nullptr) live = filter_pass(P.filt, d);
+        if (kExcl && live) live = !excluded_doc(P.seg.arena, P.seg.blocks, P.seg.anchors, s_ex, n_ex, d);   // neither collected nor counted
         // cheap pre-test on the score bits alone; the full 64-bit key only for the few that may qualify
         const uint32_t sbits = live ? __float_as_uint(e_score[e]) : 0u;
         matched += (live && first_pass) ? 1u : 0u;

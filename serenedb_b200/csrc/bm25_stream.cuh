@@ -216,65 +216,6 @@ __device__ __forceinline__ uint32_t warp_first_block(const uint4* B, uint32_t n,
 //   StreamVByte      scalar walk (tail blocks only)
 // followed by a random-access read of the frequency.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t svb_value_at(const uint8_t* bytes, uint32_t len, uint32_t idx_or_doc, bool by_doc, bool delta,
-                                                 uint32_t prev, uint32_t* idx_out) {
-  // by_doc: walks the doc stream until the running id reaches idx_or_doc (returns the id found or 0xFFFFFFFF);
-  // else returns value number idx_or_doc.
-  const uint32_t nctl = (len + 3u) >> 2;
-  uint32_t pos = nctl, acc = prev;
-  for (uint32_t i = 0; i < len; ++i) {
-    const uint32_t c = (uint32_t(__ldg(bytes + (i >> 2))) >> (2u * (i & 3u))) & 3u;
-    uint32_t x = 0;
-    for (uint32_t k = 0; k <= c; ++k) x |= uint32_t(__ldg(bytes + pos + k)) << (8u * k);
-    pos += c + 1u;
-    if (by_doc) {
-      acc = delta ? acc + x : x;
-      if (acc >= idx_or_doc) { *idx_out = i; return acc; }
-    } else if (i == idx_or_doc) {
-      return x;
-    }
-  }
-  return 0xFFFFFFFFu;
-}
-
-// Position of doc `d` inside block `desc` (prev_last < d <= last_doc), or false when the block does not hold it.
-__device__ __forceinline__ bool block_find_doc(const PostingsDev& S, const uint4& desc, uint32_t gblk, uint32_t d, uint32_t& idx) {
-  const uint4* p = S.arena + desc.x;
-  const uint32_t enc = desc_doc_enc(desc.w), len = desc_len(desc.w), prev = desc.z;
-  if (enc >= 8u) {                                   // bit-packed gaps: row r = postings 4r .. 4r+3
-    const uint32_t b = enc - 6u;
-    const uint4 an = __ldg(S.anchors + gblk);
-    const uint32_t qd = (d > an.x ? 1u : 0u) + (d > an.y ? 1u : 0u) + (d > an.z ? 1u : 0u);
-    uint32_t acc = qd == 0u ? prev : qd == 1u ? an.x : qd == 2u ? an.y : an.z;
-    const uint32_t mask = (1u << b) - 1u;
-    for (uint32_t r = 8u * qd; r < 8u * qd + 8u; ++r) {
-      const uint32_t bit = r * b, w = bit >> 5, sh = bit & 31u;
-      const uint4 lo = __ldg(p + w), hi = __ldg(p + min(w + 1u, b - 1u));
-      acc += __funnelshift_r(lo.x, hi.x, sh) & mask; if (acc >= d) { idx = 4u * r; return acc == d; }
-      acc += __funnelshift_r(lo.y, hi.y, sh) & mask; if (acc >= d) { idx = 4u * r + 1u; return acc == d; }
-      acc += __funnelshift_r(lo.z, hi.z, sh) & mask; if (acc >= d) { idx = 4u * r + 2u; return acc == d; }
-      acc += __funnelshift_r(lo.w, hi.w, sh) & mask; if (acc >= d) { idx = 4u * r + 3u; return acc == d; }
-    }
-    return false;
-  }
-  if (enc == 4u) return bitset_rank(S.arena, desc, d, idx);
-  if (enc >= 1u && enc <= 3u) {                       // constant gap g: ids prev + g, prev + 2g, ...
-    const uint32_t g = same_value(p, enc);
-    const uint32_t off = d - prev;
-    if (g == 0u || off % g != 0u) return false;
-    idx = off / g - 1u;
-    return idx < len;
-  }
-  if (enc == 0u) {                                    // raw ids
-    const uint32_t* a = reinterpret_cast<const uint32_t*>(p);
-    uint32_t l = 0, r = len;
-    while (l < r) { const uint32_t m = (l + r) >> 1; if (__ldg(a + m) < d) l = m + 1u; else r = m; }
-    idx = l;
-    return l < len && __ldg(a + l) == d;
-  }
-  return svb_value_at(reinterpret_cast<const uint8_t*>(p), len, d, true, enc == 7u, prev, &idx) == d;
-}
-
 // One lane: score of doc d in the posting list of `qt`, or false when the list does not contain d. `hint` = a block
 // of the list (index within the term) that is not behind d's block; on return the block that was searched.
 __device__ __forceinline__ bool probe_term(const PostingsDev& S, const QTermDev& qt, uint32_t d, uint32_t hint, uint32_t& found_blk,
@@ -333,6 +274,34 @@ __device__ __noinline__ ProbeResult stream_probe_round(const PostingsDev* S, con
   return r;
 }
 
+// Excluded lists of a CTA's query (TopkParams::excl), in shared memory.
+struct StreamExcl {
+  uint2 list[kMaxQueryTerms];
+  uint32_t n;
+  uint32_t hint[kTopkWarps][kMaxQueryTerms];      // per warp and list: block where the warp's last probe ended
+};
+
+// Exclusion (NOT clauses): false for lanes whose doc occurs in one of the excluded lists, else `alive`. It votes, so all
+// 32 lanes call it, with `alive` as an argument. The hints advance like s_hint in stream_probe_round. Outlined for the
+// same reason as that function.
+__device__ __noinline__ bool stream_excl_pass(const PostingsDev* S, StreamExcl* X, bool alive, uint32_t d) {
+  const uint32_t lane = threadIdx.x & 31u;
+  uint32_t* const hint = X->hint[threadIdx.x >> 5];
+  for (uint32_t x = 0; x < X->n; ++x) {
+    if (!__any_sync(kFull, alive)) break;
+    uint32_t fb = 0u;
+    bool hit = false;
+    if (alive) hit = probe_contains(*S, X->list[x], d, hint[x], fb);
+    const uint32_t who = __ballot_sync(kFull, alive);
+    fb = __shfl_sync(kFull, fb, __ffs(who) - 1);
+    __syncwarp();
+    if (lane == 0) hint[x] = fb;
+    __syncwarp();
+    alive = alive && !hit;
+  }
+  return alive;
+}
+
 // Candidate buffer full: exact radix select keeps the best k and raises the thresholds. Called by every thread of the
 // CTA between two barriers of the rendezvous.
 __device__ __noinline__ void stream_compact(StreamCtl* ctl, unsigned long long* cand, uint32_t cap, uint32_t k,
@@ -371,14 +340,17 @@ __device__ __noinline__ bool stream_rendezvous(StreamCtl* ctl, unsigned long lon
 // kMode: 0 = disjunction, all T lists live at first; 1 = conjunction (kAnd); 2 = disjunction in LEAD mode: only the
 // shortest list is live from the start and every other list is probed -- valid once the query's threshold exceeds the
 // summed bounds of those lists, which the CTA checks when it claims its work item (TopkParams::claim).
+// kExcl: the queries of the launch exclude terms (TopkParams::excl); separate instantiations, so that the others carry
+// none of its code or registers.
 constexpr int kModeOr = 0, kModeAnd = 1, kModeLead = 2;
-template <uint32_t T, bool kLut, int kMinBlocks, int kMode>
+template <uint32_t T, bool kLut, int kMinBlocks, int kMode, bool kExcl = false>
 __global__ void __launch_bounds__(kTopkThreads, kMinBlocks)
 bm25_stream_kernel(const __grid_constant__ TopkParams P) {
   constexpr bool kAnd = kMode == kModeAnd;
   constexpr bool kProbeRest = kMode != kModeOr;        // the query has more terms than live lists
   static_assert(T >= 1 && T <= kStreamMaxTerms, "1..4 live terms");
   static_assert(!kProbeRest || T == 1, "conjunctions and lead mode stream one list");
+  static_assert(!kExcl || kMode != kModeLead, "lead mode has no per-doc checks");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* cand = reinterpret_cast<unsigned long long*>(smem_raw);
   float* lut = reinterpret_cast<float*>(cand + P.cap);
@@ -389,6 +361,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
   __shared__ QTermDev s_qt[kMaxQueryTerms];
   __shared__ float s_sfx[kMaxQueryTerms + 1];          // s_sfx[e] = sum of the list-wide block-max bounds of terms e .. (inf when unknown)
   __shared__ uint32_t s_hint[kTopkWarps][kMaxQueryTerms];   // per warp and probed term: block where the last probe ended
+  __shared__ std::conditional_t<kExcl, StreamExcl, uint32_t> s_x;   // excluded lists (kExcl only)
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   constexpr uint32_t kWarpBytes = T * kStreamTermBytes + (kProbeRest ? 1024u : 0u);
@@ -414,6 +387,13 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
 
   for (uint32_t i = tid; i < P.cap; i += blockDim.x) cand[i] = 0ull;
   if (tid < n_terms) s_qt[tid] = P.qterms[t0 + tid];
+  if constexpr (kExcl) {
+    const uint32_t x0 = P.excl_off[q];
+    const uint32_t n_ex = min(P.excl_off[q + 1] - x0, kMaxQueryTerms);
+    if (tid < n_ex) s_x.list[tid] = P.excl[x0 + tid];
+    if (tid < kTopkWarps * kMaxQueryTerms) (&s_x.hint[0][0])[tid] = 0u;
+    if (tid == 0) s_x.n = n_ex;
+  }
   if (tid == 0) { ctl.ncand = 0u; ctl.matched = 0u; ctl.full = 0u; ctl.active = kTopkWarps; ctl.theta = 0ull; }
   if (lane == 0) {
 #pragma unroll
@@ -461,6 +441,12 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
   // accepted candidates, which is what block-max skipping lives on.
   const uint32_t lim = min(P.cap, (P.k + max(P.k, 256u) + kTopkThreads - 1u) / kTopkThreads * kTopkThreads);
   const bool doc_checks = P.filt.values != nullptr || P.seg.deleted != nullptr;   // hybrid filter / DocumentMask on final docs
+  // Excluded terms: a probe per doc costs a few dependent loads. With pruning and a top-k sink only docs whose final score
+  // passes the threshold pre-test are probed (late): an excluded doc then never enters the candidate buffer, so the
+  // threshold is raised by real results only and pruned == exhaustive, and `matched` counts only docs known to survive (a
+  // lower bound). Otherwise every match is probed before it is counted (early: exact count).
+  const bool excl_late = kExcl && P.wand != 0 && P.emit_docs == nullptr;
+  const bool excl_early = kExcl && !excl_late;
   const uint8_t* const norms_m1 = P.seg.norms ? P.seg.norms - 1 : nullptr;   // row = doc - 1 (1-byte norms: kLut)
 
   if (!warp_empty) {
@@ -508,6 +494,12 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
     auto test_and_append = [&](bool alive, uint32_t dv, float sv) {
       if (P.emit_docs != nullptr) { stream_emit(P.emit_docs, P.emit_scores, P.emit_count, P.emit_cap, alive, dv, sv); return; }
       bool want = alive && __float_as_uint(sv) >= theta_hi;
+      if constexpr (kExcl) {
+        if (excl_late && __any_sync(kFull, want)) {
+          want = stream_excl_pass(&P.seg, &s_x, want, dv);
+          matched += want ? 1u : 0u;
+        }
+      }
       if (__any_sync(kFull, want)) {
         unsigned long long key = 0ull;
         if (want) { key = make_key(sv, P.seg.ordinal_base + dv); want = key > theta; }
@@ -522,7 +514,12 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
       bool alive = r.alive != 0u;
       if (kAnd) {
         if (doc_checks && alive) alive = doc_ok(r.d);
-        matched += alive ? 1u : 0u;
+        if constexpr (kExcl) {
+          if (excl_early) alive = stream_excl_pass(&P.seg, &s_x, alive, r.d);
+          if (!excl_late) matched += alive ? 1u : 0u;
+        } else {
+          matched += alive ? 1u : 0u;
+        }
       }
       test_and_append(alive, r.d, r.s);
     };
@@ -530,7 +527,12 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
     auto finalize_entries = [&](bool alive, uint32_t dv, float sv) {
       if (!kAnd) {
         if (doc_checks && alive) alive = doc_ok(dv);
-        matched += alive ? 1u : 0u;
+        if constexpr (kExcl) {
+          if (excl_early) alive = stream_excl_pass(&P.seg, &s_x, alive, dv);
+          if (!excl_late) matched += alive ? 1u : 0u;
+        } else {
+          matched += alive ? 1u : 0u;
+        }
         if (E == n_terms) { test_and_append(alive, dv, sv); return; }   // nothing left to probe
         // MaxScore: a doc that cannot reach the threshold even with every probed list's bound is dropped unprobed
         if (!(P.wand & 32)) alive = alive && !(__fmul_rn(__fadd_rn(sv, s_sfx[E]), 1.000001f) < __uint_as_float(theta_hi));
@@ -560,7 +562,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
         alive[j] = dv[j] <= limit && 4u * lane + j >= a0[t];       // pads are kNoDoc > limit
         want_any |= alive[j] && __float_as_uint(sv[j]) >= theta_hi;
       }
-      if (!kAnd && E == n_terms && !doc_checks) {
+      if (!kAnd && E == n_terms && !doc_checks && !kExcl) {
         // common case: nothing to probe, nothing to check -- count, and touch the append path only when some score
         // reaches the threshold
 #pragma unroll

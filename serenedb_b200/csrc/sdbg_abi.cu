@@ -744,6 +744,31 @@ void fill_qterm(const sdbg_segment* s, const sdbg_bm25_term& t, float k1, float 
   if (t.term < s->term_probe.size() && s->term_probe[t.term]) d.root_freq |= 0x80000000u;   // probe-friendly list (driver mode)
 }
 
+// Device-side {first BlockDesc, blocks} of an excluded term in a segment: a term id the segment does not hold is an empty
+// list, which excludes nothing.
+uint2 excl_list(const sdbg_segment* s, uint32_t term) {
+  if (size_t(term) + 1 >= s->term_blk_begin.size()) return make_uint2(0u, 0u);
+  return make_uint2(s->term_blk_begin[term], s->term_blk_begin[term + 1] - s->term_blk_begin[term]);
+}
+
+// Dynamic shared memory limit of the kernels that serve queries with excluded terms (top-k and scored scan).
+cudaError_t set_excl_attrs() {
+  const cudaFuncAttribute a = cudaFuncAttributeMaxDynamicSharedMemorySize;
+  const int v = 200 * 1024;
+  cudaError_t e = cudaSuccess;
+  auto set = [&](cudaError_t r) { if (e == cudaSuccess) e = r; };
+  set(cudaFuncSetAttribute(bm25_topk_kernel<16, false, true>, a, v));
+  set(cudaFuncSetAttribute(bm25_topk_kernel<32, false, true>, a, v));
+  set(cudaFuncSetAttribute(bm25_topk_kernel<16, true, true>, a, v));
+  set(cudaFuncSetAttribute(bm25_topk_kernel<32, true, true>, a, v));
+  set(cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeOr, true>, a, v));
+  set(cudaFuncSetAttribute(bm25_stream_kernel<2, false, 3, kModeOr, true>, a, v));
+  set(cudaFuncSetAttribute(bm25_stream_kernel<3, false, 3, kModeOr, true>, a, v));
+  set(cudaFuncSetAttribute(bm25_stream_kernel<4, false, 3, kModeOr, true>, a, v));
+  set(cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeAnd, true>, a, v));
+  return e;
+}
+
 struct TopkPlan {
   uint32_t G, cap, k, budget;
   size_t smem;
@@ -752,8 +777,10 @@ struct TopkPlan {
 // Device-side result of a batch: keys_out[Q][k] (sorted desc, 0 = empty), n_out[Q], total[Q].
 struct TopkDevOut { unsigned long long* keys; uint32_t* n_out; unsigned long long* total; };
 
+// excl_terms / excl_off: query q excludes the term ids excl_terms[excl_off[q] .. excl_off[q + 1]) (NULL excl_off: none).
 int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
-             size_t nq, float k1, const float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, TopkDevOut* dev) {
+             size_t nq, float k1, const float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, TopkDevOut* dev,
+             const uint32_t* excl_terms = nullptr, const uint32_t* excl_off = nullptr) {
   if (!segs || !n_segs || !terms || !term_off || !nq || !k) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   if (k > 8192) return fail(c, SDBG_EUNSUPPORTED, "k > 8192");
@@ -763,6 +790,17 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   for (size_t q = 0; q < nq; ++q) {
     const uint32_t nt = term_off[q + 1] - term_off[q];
     if (nt == 0 || nt > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 terms");
+  }
+  uint32_t total_excl = 0;   // > 0: some query excludes terms
+  if (excl_off) {
+    for (size_t q = 0; q < nq; ++q) {
+      if (excl_off[q + 1] < excl_off[q]) return fail(c, SDBG_EINVAL, "excl_off must be non-decreasing");
+      if (excl_off[q + 1] - excl_off[q] > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
+    }
+    if (excl_off[nq] > excl_off[0]) {
+      if (!excl_terms) return fail(c, SDBG_EINVAL, "excl_terms is NULL");
+      total_excl = excl_off[nq];
+    }
   }
   uint64_t ord = 0;
   uint32_t max_docs = 0;
@@ -802,9 +840,11 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   //   12           the rest of such a query: launched into BOTH the merge kernel and the stream kernel in lead mode
   //                (short list streamed, long list probed per candidate); the first CTA to arrive decides from the
   //                threshold which of the two runs the item (TopkParams::claim)
+  //   kClasses + c class c (0 / 1, 6 .. 10 only) for queries that exclude terms: the kExcl instantiations of the same
+  //                kernels. Never the merge kernel, slices or lead mode, which have no per-doc checks.
   struct WorkItem { uint32_t q, lo, len, list; uint64_t weight; uint32_t cls; };
   constexpr uint32_t kClsMerge = 2, kClsStream = 2 + kStreamMaxTerms, kClsAnd = 2 + 2 * kStreamMaxTerms, kClsSlice = kClsAnd + 1,
-                     kClsLead = kClsAnd + 2, kClasses = kClsAnd + 3;
+                     kClsLead = kClsAnd + 2, kClasses = kClsAnd + 3, kAllClasses = 2 * kClasses;
   const bool level2 = c->wand >= 2 && kind != SDBG_QUERY_AND && k1 != 0.f && k1 != kTfidfK1 && b != 0.f;
   const bool stream_ok = env_int("SDBG_STREAM", 1) != 0 && k1 != 0.f && b != 0.f && k1 != kTfidfK1 &&
                          size_t(pl.cap) * 8 + size_t(kStreamMaxTerms) * (kLutFreqs * 1024 + kTopkWarps * kStreamTermBytes) <= 200 * 1024;
@@ -813,7 +853,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   // wand_writer.hpp:142-175; the order of two pairs does not depend on k); the reference enables WAND only when
   // Scorer::equals matches (PostingsReaderImpl::WandIterator, reader.hpp:457-501). Any other b: exhaustive.
   auto seg_wand = [&](const sdbg_segment* s) { return (c->wand && s->has_wand && k1 != 0.f && k1 != kTfidfK1 && b != 0.f && b == s->wand_b) ? c->wand : 0; };
-  std::vector<std::array<size_t, kClasses>> n_cls(n_segs);
+  std::vector<std::array<size_t, kAllClasses>> n_cls(n_segs);
   for (auto& a : n_cls) a.fill(0);
   std::vector<std::vector<WorkItem>> seg_work(n_segs);
   std::vector<uint32_t> list_off(nq + 1, 0);
@@ -835,11 +875,12 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
       // Driver mode (pruning level 2) pays only when the largest list can be probed without decoding blocks; the
       // other queries run the plain kernel, which is lighter (fewer registers, no probe buffers, level-1 planner).
       const bool drive_q = level2 && wand && nt >= 2 && largest_term < s->term_probe.size() && s->term_probe[largest_term] != 0;
+      const bool excludes = total_excl && excl_off[q + 1] > excl_off[q];
       uint32_t cls = drive_q ? 0u : 1u;
       uint32_t slice_docs = 0;    // > 0: lead candidate
       if (stream_ok && kind == SDBG_QUERY_AND && env_int("SDBG_STREAM_AND", 1) != 0) cls = kClsAnd;
       else if (stream_ok && kind != SDBG_QUERY_AND && nt <= kStreamMaxTerms) {
-        const bool plain = !filt && !s->d_deleted;                  // the merge kernel has no per-doc checks
+        const bool plain = !filt && !s->d_deleted && !excludes;     // the merge kernel has no per-doc checks
         cls = (!plain || (wand && (nt != 2 || !lead_ok))) ? kClsStream + (nt - 1u) : kClsMerge + (nt - 1u);
         if (wand && nt == 2 && lead_ok && plain && uint64_t(largest) >= 4ull * smallest && smallest >= 3u * k) {
           // Lead mode needs the threshold above the long list's bound. That happens when a typical posting of the short
@@ -873,6 +914,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
         ++lists;
         cls = kClsLead;
       }
+      if (excludes) cls += kClasses;
       uint32_t g = uint32_t(std::max<uint64_t>(pl.G, (rest_postings + chain_target - 1) / chain_target));
       // lead mode is latency-bound (dependent loads per probe), not throughput-bound: more, shorter chains
       if (slice_docs) g = std::max(g, std::min<uint32_t>(uint32_t(env_int("SDBG_STREAM_LEAD_CHAINS", 16)), std::max(1u, smallest / 8192u)));
@@ -901,7 +943,11 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   const size_t off_bytes = (nq + 1) * sizeof(uint32_t);
   const size_t work_bytes = total_work * sizeof(uint4);
   const size_t qt_pad = (qt_bytes + off_bytes + 15) & ~size_t(15);   // work items are 16-byte loads
-  int rc = ensure_pinned(c, qt_pad + work_bytes + off_bytes);
+  // excluded lists, when there are any: [uint2 {first block, blocks} x total_excl per segment | excl_off]
+  const size_t x_pos = (qt_pad + work_bytes + off_bytes + 15) & ~size_t(15);
+  const size_t x_lists = size_t(total_excl) * n_segs * sizeof(uint2);
+  const size_t desc_bytes = total_excl ? x_pos + x_lists + off_bytes : qt_pad + work_bytes + off_bytes;
+  int rc = ensure_pinned(c, desc_bytes);
   if (rc) return rc;
   auto* h_qt = static_cast<QTermDev*>(c->h_pinned);
   auto* h_off = reinterpret_cast<uint32_t*>(static_cast<char*>(c->h_pinned) + qt_bytes);
@@ -910,6 +956,12 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
     auto* h_work = reinterpret_cast<uint4*>(static_cast<char*>(c->h_pinned) + qt_pad);
     for (auto& w : seg_work) for (const WorkItem& it : w) *h_work++ = make_uint4(it.q, it.lo, it.len, it.list);
     std::memcpy(static_cast<char*>(c->h_pinned) + qt_pad + work_bytes, list_off.data(), off_bytes);
+  }
+  if (total_excl) {
+    auto* h_x = reinterpret_cast<uint2*>(static_cast<char*>(c->h_pinned) + x_pos);
+    for (size_t si = 0; si < n_segs; ++si)
+      for (uint32_t i = 0; i < total_excl; ++i) h_x[si * total_excl + i] = excl_list(segs[si], excl_terms[i]);
+    std::memcpy(static_cast<char*>(c->h_pinned) + x_pos + x_lists, excl_off, off_bytes);
   }
   for (size_t si = 0; si < n_segs; ++si) {
     const sdbg_segment* s = segs[si];
@@ -926,13 +978,13 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   }
   DevBuf& b_qt = c->scratch[0]; DevBuf& b_theta = c->scratch[1]; DevBuf& b_cand = c->scratch[2];
   DevBuf& b_candn = c->scratch[3]; DevBuf& b_keys = c->scratch[4]; DevBuf& b_small = c->scratch[5];
-  if ((rc = ensure(c, b_qt, qt_pad + work_bytes + off_bytes))) return rc;
+  if ((rc = ensure(c, b_qt, desc_bytes))) return rc;
   if ((rc = ensure(c, b_theta, nq * 16))) return rc;  // theta[nq] | total[nq]
   if ((rc = ensure(c, b_cand, size_t(total_lists) * pl.cap * 8))) return rc;
   if ((rc = ensure(c, b_candn, size_t(total_lists) * 4))) return rc;
   if ((rc = ensure(c, b_keys, nq * size_t(k) * 8))) return rc;
   if ((rc = ensure(c, b_small, nq * 4))) return rc;
-  CU(c, cudaMemcpyAsync(b_qt.p, c->h_pinned, qt_pad + work_bytes + off_bytes, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(b_qt.p, c->h_pinned, desc_bytes, cudaMemcpyHostToDevice, c->stream));
   auto* d_theta = static_cast<unsigned long long*>(b_theta.p);
   auto* d_total = d_theta + nq;
   uint32_t thr_bits; std::memcpy(&thr_bits, &threshold_in, 4);
@@ -964,6 +1016,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
     CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeLead>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, true, 3, kModeLead>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     CU(c, cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CU(c, set_excl_attrs());
     c->topk_attr_set = true;
   }
   // one claim word per work item of class kClsLead (zeroed per call)
@@ -980,7 +1033,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   // and joined back into the context's stream) so that no class waits for another's tail. First slices (class 11) go
   // first, and everything that depends on their thresholds is ordered behind them.
   uint32_t classes_present = 0;
-  for (size_t si = 0; si < n_segs; ++si) for (uint32_t k2 = 0; k2 < kClasses; ++k2) if (n_cls[si][k2]) classes_present |= 1u << k2;
+  for (size_t si = 0; si < n_segs; ++si) for (uint32_t k2 = 0; k2 < kAllClasses; ++k2) if (n_cls[si][k2]) classes_present |= 1u << k2;
   const bool two_lanes = (classes_present & (classes_present - 1u)) != 0u;
   {
     ProfScope ps_(c, kProfTopk);   // one span for all top-k launches of the call
@@ -997,12 +1050,16 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
       P.cand_n = static_cast<uint32_t*>(b_candn.p);
       P.k = k; P.cap = pl.cap; P.conjunction = kind == SDBG_QUERY_AND ? 1 : 0;
       P.claim = nullptr;
+      if (total_excl) {
+        P.excl = reinterpret_cast<const uint2*>(static_cast<const char*>(b_qt.p) + x_pos) + si * total_excl;
+        P.excl_off = reinterpret_cast<const uint32_t*>(static_cast<const char*>(b_qt.p) + x_pos + x_lists);
+      }
       const int wand = seg_wand(s);
       const bool lut = use_lut[si];
       const uint4* const work0 = reinterpret_cast<const uint4*>(static_cast<const char*>(b_qt.p) + qt_pad) + work_done;
       work_done += seg_work[si].size();
-      std::array<size_t, kClasses> cls_off{};
-      { size_t o = 0; for (uint32_t cls = 0; cls < kClasses; ++cls) { cls_off[cls] = o; o += n_cls[si][cls]; } }
+      std::array<size_t, kAllClasses> cls_off{};
+      { size_t o = 0; for (uint32_t cls = 0; cls < kAllClasses; ++cls) { cls_off[cls] = o; o += n_cls[si][cls]; } }
       auto launch_merge = [&](uint32_t T, size_t n, cudaStream_t st) {
         const size_t sm = size_t(pl.cap) * 8 + (lut ? size_t(T) * kLutFreqs * 1024 : 0) + size_t(kTopkWarps) * T * kMergeTermBytes;
 #define SDBG_MERGE_LAUNCH(TT) \
@@ -1026,13 +1083,39 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
         CU(c, cudaEventRecord(c->ev_fork, c->stream));
         CU(c, cudaStreamWaitEvent(c->stream2, c->ev_fork, 0));
       }
-      for (uint32_t cls = 0; cls < kClasses; ++cls) {
+      for (uint32_t cls = 0; cls < kAllClasses; ++cls) {
         const size_t n = n_cls[si][cls];
         if (!n || cls == kClsSlice) continue;
         cudaStream_t st = (two_lanes && (lane_no++ & 1u)) ? c->stream2 : c->stream;
         P.work = work0 + cls_off[cls];
         P.claim = nullptr;
-        if (cls == 0) {
+        if (cls >= kClasses) {
+          // queries with excluded terms: the kExcl instantiations (without the opt-in score table, a speed variant only)
+          const uint32_t cb = cls - kClasses;
+          if (cb == 0) {
+            P.wand = wand;
+            if (pl.budget == 16) bm25_topk_kernel<16, true, true><<<unsigned(n), kTopkThreads, smem_drive, st>>>(P);
+            else bm25_topk_kernel<32, true, true><<<unsigned(n), kTopkThreads, smem_drive, st>>>(P);
+          } else if (cb == 1) {
+            P.wand = std::min(wand, 1);
+            if (pl.budget == 16) bm25_topk_kernel<16, false, true><<<unsigned(n), kTopkThreads, pl.smem, st>>>(P);
+            else bm25_topk_kernel<32, false, true><<<unsigned(n), kTopkThreads, pl.smem, st>>>(P);
+          } else if (cb == kClsAnd) {
+            P.wand = 0;
+            bm25_stream_kernel<1, false, 3, kModeAnd, true><<<unsigned(n), kTopkThreads, stream_smem(1, false, true), st>>>(P);
+          } else {
+            const uint32_t T = cb - kClsStream + 1u;
+            const size_t sm = stream_smem(T, false, false);
+            P.wand = wand ? (wand | (env_int("SDBG_STREAM_DBG", 0) & 0xF0)) : 0;
+            switch (T) {
+              case 1: bm25_stream_kernel<1, false, 3, kModeOr, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); break;
+              case 2: bm25_stream_kernel<2, false, 3, kModeOr, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); break;
+              case 3: bm25_stream_kernel<3, false, 3, kModeOr, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); break;
+              default: bm25_stream_kernel<4, false, 3, kModeOr, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); break;
+            }
+          }
+          ++c->launches;
+        } else if (cls == 0) {
           P.wand = wand;
           if (pl.budget == 16) bm25_topk_kernel<16, true><<<unsigned(n), kTopkThreads, smem_drive, st>>>(P);
           else bm25_topk_kernel<32, true><<<unsigned(n), kTopkThreads, smem_drive, st>>>(P);
@@ -1164,13 +1247,13 @@ extern "C" int sdbg_tfidf_topk_batch(sdbg_segment* const* segs, size_t n_segs, i
                               total_matches);
 }
 
-extern "C" int sdbg_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
-                                    const uint32_t* term_off, size_t nq, float k1, float b, const sdbg_col_pred* filt,
-                                    uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
-                                    uint64_t* total_matches) {
+namespace {
+int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
+                    size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b, const sdbg_col_pred* filt,
+                    uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
   if (!out || !n_out) return SDBG_EINVAL;
   TopkDevOut dev{};
-  int rc = topk_run(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, &dev);
+  int rc = topk_run(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, &dev, excl_terms, excl_off);
   if (rc) return rc;
   sdbg_ctx* c = segs[0]->ctx;
   const size_t kb = nq * size_t(k) * 8, nb = nq * 4, tb = nq * 8;
@@ -1221,18 +1304,39 @@ extern "C" int sdbg_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, in
   }
   return SDBG_OK;
 }
+}  // namespace
+
+extern "C" int sdbg_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
+                                    const uint32_t* term_off, size_t nq, float k1, float b, const sdbg_col_pred* filt,
+                                    uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
+                                    uint64_t* total_matches) {
+  return topk_batch_host(segs, n_segs, kind, terms, term_off, nq, nullptr, nullptr, k1, b, filt, k, threshold_in, out, n_out,
+                         total_matches);
+}
+
+extern "C" int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
+                                         const uint32_t* term_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
+                                         float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
+                                         uint32_t* n_out, uint64_t* total_matches) {
+  if (!excl_off) return SDBG_EINVAL;
+  return topk_batch_host(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, k1, b, filt, k, threshold_in, out, n_out,
+                         total_matches);
+}
 
 // Streaming mode (duckdb_search_full_scan.cpp RunStreamingScan :2370-2403; DocIterator::EmitScoredDocs,
 // iterators.hpp:202-204): every match of one query in docs [doc_min, doc_max) of one segment with its score, ascending
 // by doc. Same stream kernel as the top-k scan with pruning off; its sink writes through a global cursor and the
 // pairs are then radix-sorted by doc id on the device.
-extern "C" int sdbg_bm25_scan(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_terms, float k1, float b,
-                              const sdbg_col_pred* filt, uint32_t doc_min, uint32_t doc_max, uint32_t* out_docs, float* out_scores,
-                              uint64_t cap, uint64_t* n_out) {
+namespace {
+int scan_run(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_terms, const uint32_t* excl_terms, size_t n_excl,
+             float k1, float b, const sdbg_col_pred* filt, uint32_t doc_min, uint32_t doc_max, uint32_t* out_docs, float* out_scores,
+             uint64_t cap, uint64_t* n_out) {
   if (!s || !terms || !n_terms || !n_out || (cap && (!out_docs || !out_scores))) return SDBG_EINVAL;
   sdbg_ctx* c = s->ctx;
   CU(c, cudaSetDevice(c->device));
   if (!s->d_blocks) return fail(c, SDBG_EINVAL, "segment has no staged postings");
+  if (n_excl > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
+  if (n_excl && !excl_terms) return fail(c, SDBG_EINVAL, "excl_terms is NULL");
   const bool conj = kind == SDBG_QUERY_AND;
   if (n_terms > (conj ? size_t(kMaxQueryTerms) : size_t(kStreamMaxTerms)))
     return fail(c, SDBG_EUNSUPPORTED, "scored scan: disjunctions take 1..4 terms, conjunctions 1..16");
@@ -1246,10 +1350,12 @@ extern "C" int sdbg_bm25_scan(sdbg_segment* s, int kind, const sdbg_bm25_term* t
   const uint32_t scan_cap = 1024;                                    // candidate buffer of the kernel: unused here, kept minimal
   const uint32_t g = std::max(1u, std::min(uint32_t(c->sm_count) * 3u, range / 4096u));
   const uint32_t chunk = (range + g - 1) / g;
-  // descriptors: [QTermDev x T][term_off x 2][pad][work x g]
+  // descriptors: [QTermDev x T][term_off x 2][pad][work x g][excluded lists x n_excl][excl_off x 2]
   const size_t qt_bytes = size_t(T) * sizeof(QTermDev), off_bytes = 2 * sizeof(uint32_t);
   const size_t qt_pad = (qt_bytes + off_bytes + 15) & ~size_t(15), work_bytes = size_t(g) * sizeof(uint4);
-  int rc = ensure_pinned(c, qt_pad + work_bytes);
+  const size_t x_bytes = n_excl * sizeof(uint2);
+  const size_t desc_bytes = qt_pad + work_bytes + (n_excl ? x_bytes + off_bytes : 0);
+  int rc = ensure_pinned(c, desc_bytes);
   if (rc) return rc;
   auto* h_qt = static_cast<QTermDev*>(c->h_pinned);
   for (uint32_t i = 0; i < T; ++i) {
@@ -1265,6 +1371,10 @@ extern "C" int sdbg_bm25_scan(sdbg_segment* s, int kind, const sdbg_bm25_term* t
     h_work[j] = make_uint4(0u, lo, lo < doc_max ? std::min(chunk, doc_max - lo) : 0u, j);
     if (lo >= doc_max) h_work[j].y = s->n_docs + 1u;               // empty chain
   }
+  auto* h_x = reinterpret_cast<uint2*>(static_cast<char*>(c->h_pinned) + qt_pad + work_bytes);
+  for (size_t i = 0; i < n_excl; ++i) h_x[i] = excl_list(s, excl_terms[i]);
+  auto* h_xoff = reinterpret_cast<uint32_t*>(h_x + n_excl);
+  if (n_excl) { h_xoff[0] = 0; h_xoff[1] = uint32_t(n_excl); }
   DevBuf& b_qt = c->scratch[0]; DevBuf& b_theta = c->scratch[1]; DevBuf& b_cand = c->scratch[2]; DevBuf& b_candn = c->scratch[3];
   DevBuf& b_emit = c->scratch[12];
   const uint64_t room = std::max<uint64_t>(cap, 1);
@@ -1272,12 +1382,12 @@ extern "C" int sdbg_bm25_scan(sdbg_segment* s, int kind, const sdbg_bm25_term* t
   cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, static_cast<const uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr),
                                   static_cast<const float*>(nullptr), static_cast<float*>(nullptr), room, 0, 32, c->stream);
   const size_t pair_bytes = (size_t(room) * 4 + 255) & ~size_t(255);
-  if ((rc = ensure(c, b_qt, qt_pad + work_bytes))) return rc;
+  if ((rc = ensure(c, b_qt, desc_bytes))) return rc;
   if ((rc = ensure(c, b_theta, 32))) return rc;                      // theta | total | cursor
   if ((rc = ensure(c, b_cand, size_t(g) * scan_cap * 8))) return rc;
   if ((rc = ensure(c, b_candn, size_t(g) * 4))) return rc;
   if ((rc = ensure(c, b_emit, 4 * pair_bytes + sort_bytes))) return rc;
-  CU(c, cudaMemcpyAsync(b_qt.p, c->h_pinned, qt_pad + work_bytes, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(b_qt.p, c->h_pinned, desc_bytes, cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaMemsetAsync(b_theta.p, 0, 32, c->stream));
   TopkParams P;
   P.seg = postings_view(s, 0);
@@ -1292,13 +1402,17 @@ extern "C" int sdbg_bm25_scan(sdbg_segment* s, int kind, const sdbg_bm25_term* t
   P.cand_n = static_cast<uint32_t*>(b_candn.p);
   P.claim = nullptr;
   P.k = 1; P.cap = scan_cap; P.conjunction = conj ? 1 : 0; P.wand = 0;
+  if (n_excl) {
+    P.excl = reinterpret_cast<const uint2*>(static_cast<const char*>(b_qt.p) + qt_pad + work_bytes);
+    P.excl_off = reinterpret_cast<const uint32_t*>(P.excl + n_excl);
+  }
   char* e = static_cast<char*>(b_emit.p);
   P.emit_docs = reinterpret_cast<uint32_t*>(e);
   P.emit_scores = reinterpret_cast<float*>(e + pair_bytes);
   P.emit_cap = cap;
   auto* sorted_docs = reinterpret_cast<uint32_t*>(e + 2 * pair_bytes);
   auto* sorted_scores = reinterpret_cast<float*>(e + 3 * pair_bytes);
-  const bool lut = s->norm_width == 1 && env_int("SDBG_STREAM_LUT", 0) != 0;
+  const bool lut = n_excl == 0 && s->norm_width == 1 && env_int("SDBG_STREAM_LUT", 0) != 0;
   const uint32_t Tl = conj ? 1u : T;
   const size_t sm = size_t(scan_cap) * 8 + (lut ? size_t(Tl) * kLutFreqs * 1024 : 0) + size_t(kTopkWarps) * (Tl * kStreamTermBytes + (conj ? 1024 : 0));
   if (!c->scan_attr_set) {
@@ -1309,11 +1423,18 @@ extern "C" int sdbg_bm25_scan(sdbg_segment* s, int kind, const sdbg_bm25_term* t
 #undef SDBG_SCAN_ATTR
     CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeAnd>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, true, 3, kModeAnd>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CU(c, set_excl_attrs());
     c->scan_attr_set = true;
   }
   {
     ProfScope ps_(c, kProfTopk);
-    if (conj) {
+    if (n_excl) {                                                    // the kExcl instantiations, as in topk_run
+      if (conj) bm25_stream_kernel<1, false, 3, kModeAnd, true><<<g, kTopkThreads, sm, c->stream>>>(P);
+      else if (T == 1) bm25_stream_kernel<1, false, 3, kModeOr, true><<<g, kTopkThreads, sm, c->stream>>>(P);
+      else if (T == 2) bm25_stream_kernel<2, false, 3, kModeOr, true><<<g, kTopkThreads, sm, c->stream>>>(P);
+      else if (T == 3) bm25_stream_kernel<3, false, 3, kModeOr, true><<<g, kTopkThreads, sm, c->stream>>>(P);
+      else bm25_stream_kernel<4, false, 3, kModeOr, true><<<g, kTopkThreads, sm, c->stream>>>(P);
+    } else if (conj) {
       if (lut) bm25_stream_kernel<1, true, 3, kModeAnd><<<g, kTopkThreads, sm, c->stream>>>(P);
       else bm25_stream_kernel<1, false, 3, kModeAnd><<<g, kTopkThreads, sm, c->stream>>>(P);
     } else {
@@ -1345,6 +1466,19 @@ extern "C" int sdbg_bm25_scan(sdbg_segment* s, int kind, const sdbg_bm25_term* t
   CU(c, cudaMemcpyAsync(out_scores, sorted_scores, size_t(found) * 4, cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
   return SDBG_OK;
+}
+}  // namespace
+
+extern "C" int sdbg_bm25_scan(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_terms, float k1, float b,
+                              const sdbg_col_pred* filt, uint32_t doc_min, uint32_t doc_max, uint32_t* out_docs, float* out_scores,
+                              uint64_t cap, uint64_t* n_out) {
+  return scan_run(s, kind, terms, n_terms, nullptr, 0, k1, b, filt, doc_min, doc_max, out_docs, out_scores, cap, n_out);
+}
+
+extern "C" int sdbg_bm25_scan_excl(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_terms, const uint32_t* excl_terms,
+                                   size_t n_excl, float k1, float b, const sdbg_col_pred* filt, uint32_t doc_min, uint32_t doc_max,
+                                   uint32_t* out_docs, float* out_scores, uint64_t cap, uint64_t* n_out) {
+  return scan_run(s, kind, terms, n_terms, excl_terms, n_excl, k1, b, filt, doc_min, doc_max, out_docs, out_scores, cap, n_out);
 }
 
 extern "C" int sdbg_bm25_topk(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,

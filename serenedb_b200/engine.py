@@ -400,8 +400,23 @@ class IndexReader:
         return scorer.collect(self.docs_with_field, self.total_term_freq, int(self.docs_with_term[term]), term, boost)
 
 
-def ExecuteTopKBatch(reader, queries, kind, scorer, k, filt=None, threshold=FLT_MIN):
-    """Batch of ExecuteTopK calls (doc_collector.hpp:88-136). queries: list of term-id lists.
+def _exclusions(exclude, nq):
+    """Per-query excluded term ids -> (flat ids u32, offsets u32 [nq + 1]), or None when no query excludes anything."""
+    if exclude is None:
+        return None
+    if len(exclude) != nq:
+        raise ValueError("exclude needs one list (or None) per query")
+    lists = [list(x) if x is not None else [] for x in exclude]
+    if not any(lists):
+        return None
+    off = np.zeros(nq + 1, np.uint32)
+    off[1:] = np.cumsum([len(x) for x in lists])
+    return np.ascontiguousarray([t for x in lists for t in x], dtype=np.uint32), off
+
+
+def ExecuteTopKBatch(reader, queries, kind, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
+    """Batch of ExecuteTopK calls (doc_collector.hpp:88-136). queries: list of term-id lists. exclude: None, or one list of
+    excluded term ids (or None) per query -- `a & b & !c` (sdbg_bm25_topk_batch_excl).
     Returns (hits [Q, k] structured, n_out [Q], total_matches [Q])."""
     nq = len(queries)
     flat = [reader.stats(scorer, t) for q in queries for t in q]
@@ -415,9 +430,15 @@ def ExecuteTopKBatch(reader, queries, kind, scorer, k, filt=None, threshold=FLT_
     total = np.zeros(nq, np.uint64)
     ctx = reader.segments[0].ctx
     fp = C.byref(filt) if filt is not None else None
-    N.check(N.lib().sdbg_bm25_topk_batch(_seg_array(reader.segments), len(reader.segments), int(kind), terms,
-                                         _ptr(off), nq, scorer.k, scorer.b, fp, int(k), float(threshold), _ptr(hits),
-                                         _ptr(n_out), _ptr(total)), ctx._h)
+    x = _exclusions(exclude, nq)
+    if x is None:
+        N.check(N.lib().sdbg_bm25_topk_batch(_seg_array(reader.segments), len(reader.segments), int(kind), terms,
+                                             _ptr(off), nq, scorer.k, scorer.b, fp, int(k), float(threshold), _ptr(hits),
+                                             _ptr(n_out), _ptr(total)), ctx._h)
+    else:
+        N.check(N.lib().sdbg_bm25_topk_batch_excl(_seg_array(reader.segments), len(reader.segments), int(kind), terms,
+                                                  _ptr(off), nq, _ptr(x[0]), _ptr(x[1]), scorer.k, scorer.b, fp, int(k),
+                                                  float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)), ctx._h)
     return hits, n_out, total
 
 
@@ -437,11 +458,12 @@ def pack_for(values, out_words=None):
     return headers, words[:n.value], rows
 
 
-def StreamScoredDocs(reader, seg_idx, query, kind, scorer, filt=None, doc_min=1, doc_max=None):
+def StreamScoredDocs(reader, seg_idx, query, kind, scorer, filt=None, doc_min=1, doc_max=None, exclude=None):
     """The search scan's streaming mode (duckdb_search_full_scan.cpp:2370 RunStreamingScan over
     DocIterator::EmitScoredDocs): every match of `query` in docs [doc_min, doc_max) of segment `seg_idx` with its score,
-    ascending by doc id. Returns (docs u32, scores f32)."""
+    ascending by doc id; `exclude` = term ids whose docs are left out (sdbg_bm25_scan_excl). Returns (docs u32, scores f32)."""
     seg = reader.segments[seg_idx]
+    x = np.ascontiguousarray(list(exclude) if exclude else [], dtype=np.uint32)
     terms = (N.BM25Term * len(query))(*[reader.stats(scorer, t) for t in query])
     fp = C.byref(filt) if filt is not None else None
     hi = int(doc_max) if doc_max is not None else 0xFFFFFFFF
@@ -449,9 +471,13 @@ def StreamScoredDocs(reader, seg_idx, query, kind, scorer, filt=None, doc_min=1,
     cap = 0
     docs = scores = None
     for _ in range(2):   # count-only call first, then one with exactly the room needed
-        rc = N.lib().sdbg_bm25_scan(seg._h, int(kind), terms, len(query), scorer.k, scorer.b, fp, int(doc_min), hi,
-                                    _ptr(docs) if docs is not None else None, _ptr(scores) if scores is not None else None,
-                                    cap, C.byref(n))
+        dp, sp = _ptr(docs) if docs is not None else None, _ptr(scores) if scores is not None else None
+        if len(x):
+            rc = N.lib().sdbg_bm25_scan_excl(seg._h, int(kind), terms, len(query), _ptr(x), len(x), scorer.k, scorer.b, fp,
+                                             int(doc_min), hi, dp, sp, cap, C.byref(n))
+        else:
+            rc = N.lib().sdbg_bm25_scan(seg._h, int(kind), terms, len(query), scorer.k, scorer.b, fp, int(doc_min), hi,
+                                        dp, sp, cap, C.byref(n))
         if rc == -6 and n.value > cap:
             cap = n.value
             docs, scores = np.zeros(cap, np.uint32), np.zeros(cap, np.float32)
@@ -476,10 +502,11 @@ def _flatten_queries(reader, queries, scorer):
 class PreparedBatch:
     """Query descriptors marshalled once (terms + statistics), reusable across steps."""
 
-    def __init__(self, reader, queries, kind, scorer, k, filt=None, threshold=FLT_MIN):
+    def __init__(self, reader, queries, kind, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
         self.reader, self.kind, self.scorer, self.k, self.filt, self.threshold = reader, int(kind), scorer, int(k), filt, float(threshold)
         self.nq = len(queries)
         self.terms, self.off = _flatten_queries(reader, queries, scorer)
+        self.excl = _exclusions(exclude, self.nq)   # None: no query excludes anything
         self.hits = np.zeros((self.nq, self.k), HIT_DTYPE)
         self.n_out = np.zeros(self.nq, np.uint32)
         self.total = np.zeros(self.nq, np.uint64)
@@ -488,14 +515,25 @@ class PreparedBatch:
         """Full API call: host descriptors in, host hits out."""
         r = self.reader
         fp = C.byref(self.filt) if self.filt is not None else None
-        N.check(N.lib().sdbg_bm25_topk_batch(_seg_array(r.segments), len(r.segments), self.kind, self.terms,
-                                             _ptr(self.off), self.nq, self.scorer.k, self.scorer.b, fp, self.k, self.threshold,
-                                             _ptr(self.hits), _ptr(self.n_out), _ptr(self.total)), r.segments[0].ctx._h)
+        if self.excl is None:
+            N.check(N.lib().sdbg_bm25_topk_batch(_seg_array(r.segments), len(r.segments), self.kind, self.terms,
+                                                 _ptr(self.off), self.nq, self.scorer.k, self.scorer.b, fp, self.k, self.threshold,
+                                                 _ptr(self.hits), _ptr(self.n_out), _ptr(self.total)), r.segments[0].ctx._h)
+        else:
+            N.check(N.lib().sdbg_bm25_topk_batch_excl(_seg_array(r.segments), len(r.segments), self.kind, self.terms,
+                                                      _ptr(self.off), self.nq, _ptr(self.excl[0]), _ptr(self.excl[1]), self.scorer.k,
+                                                      self.scorer.b, fp, self.k, self.threshold, _ptr(self.hits), _ptr(self.n_out),
+                                                      _ptr(self.total)), r.segments[0].ctx._h)
         return self.hits, self.n_out, self.total
+
+    def _no_exclusions(self, what):
+        if self.excl is not None:
+            raise NotImplementedError(what + " has no exclusion form: use run_host")
 
     def run_dist(self, to_host=True):
         """Distributed top-k (sdbg_dist_bm25_topk_batch): local scan, one all-gather, local selection -- all enqueued by
         the library on its stream. to_host=False leaves the merged keys in HBM and returns without waiting."""
+        self._no_exclusions("run_dist")
         r = self.reader
         fp = C.byref(self.filt) if self.filt is not None else None
         if to_host:
@@ -511,6 +549,7 @@ class PreparedBatch:
 
     def run_device(self, rank, d_keys_ptr, d_totals_ptr=None):
         """Results stay in HBM as sortable keys (for the multi-GPU gather + merge)."""
+        self._no_exclusions("run_device")
         r = self.reader
         fp = C.byref(self.filt) if self.filt is not None else None
         N.check(N.lib().sdbg_bm25_topk_batch_device(_seg_array(r.segments), len(r.segments), self.kind, self.terms,
@@ -533,9 +572,11 @@ def merge_gathered(ctx, d_keys_all_ptr, n_ranks, nq, k, to_host=True):
     return hits, n_out
 
 
-def ExecuteTopK(reader, query_terms, kind, scorer, k, filt=None, threshold=FLT_MIN):
-    """irs::ExecuteTopK for one query: hits sorted by (score desc, seg asc, doc asc), total matches."""
-    hits, n_out, total = ExecuteTopKBatch(reader, [list(query_terms)], kind, scorer, k, filt, threshold)
+def ExecuteTopK(reader, query_terms, kind, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
+    """irs::ExecuteTopK for one query: hits sorted by (score desc, seg asc, doc asc), total matches. exclude: term ids whose
+    docs are left out (`a & b & !c`)."""
+    hits, n_out, total = ExecuteTopKBatch(reader, [list(query_terms)], kind, scorer, k, filt, threshold,
+                                          exclude=None if exclude is None else [list(exclude)])
     return hits[0, :n_out[0]].copy(), int(total[0])
 
 

@@ -1,8 +1,10 @@
 // adapter_selftest.cpp -- drives the two adapters the way the reference's callers would
 // (ExecuteTopK's collector loop, IResearchScanFunction's chunk loop) and prints results as JSON lines
-// for tests/test_gpu_adapters.py to compare with the oracle. Needs a GPU at run time.
+// for tests/test_gpu_adapters.py to compare with the oracle. Needs a GPU at run time. With a second argument "excl" it runs
+// only the exclusion case instead (an And with a Not child, tests/test_gpu_exclusion.py).
 #include <cstdio>
 #include <cstdlib>
+#include <string>
 #include <thread>
 #include <vector>
 
@@ -35,6 +37,33 @@ int main(int argc, char** argv) {
   const uint32_t ids[2] = {2, 5};
   for (int i = 0; i < 2; ++i) { sdbg_bm25_collect(n_docs, sum_dl, dc[ids[i]], 1.2f, 0.75f, &terms[size_t(i)]); terms[size_t(i)].term = ids[i]; }
   sdbg_col_pred filt{}; filt.field = 9; filt.op = SDBG_OP_BETWEEN; filt.lo_i = 250000; filt.hi_i = 749999;
+  if (argc > 2 && std::string(argv[2]) == "excl") {
+    // `t2 | t5` minus the docs of t3: Collect (top-100) and the streaming mode (k = 0), without and with the table filter
+    ListCollector col;
+    irs::ScoreFunction sf; irs::ColumnArgsFetcher fetcher;
+    for (int with_filter = 0; with_filter < 2; ++with_filter) {
+      sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_OR, terms, 1.2f, 0.75f, 100, with_filter ? &filt : nullptr, {3});
+      col.docs.clear();
+      it.Collect(sf, fetcher, col);
+      std::printf("{\"filter\": %d, \"topk\": [", with_filter);
+      for (size_t i = 0; i < col.docs.size(); ++i) std::printf("%s[%u, %.9g]", i ? ", " : "", col.docs[i].doc, double(col.docs[i].score));
+      std::printf("], \"total\": %llu, \"threshold\": %.9g", static_cast<unsigned long long>(it.total_matches()), double(it.threshold().value));
+      sdbg_host::GpuTopKIterator st(seg, SDBG_QUERY_OR, terms, 1.2f, 0.75f, 0, with_filter ? &filt : nullptr, {3});
+      std::vector<irs::doc_id_t> d(2048);
+      std::vector<irs::score_t> sc(2048);
+      uint64_t n = 0, doc_sum = 0; double score_sum = 0;
+      for (irs::doc_id_t lo = 1; lo <= n_docs; lo += 2048) {
+        const uint32_t got = st.EmitScoredDocs(d.data(), sc.data(), lo + 2048, sf, &fetcher, lo);
+        for (uint32_t i = 0; i < got; ++i) { doc_sum += d[i]; score_sum += sc[i]; }
+        n += got;
+      }
+      std::printf(", \"stream_n\": %llu, \"stream_doc_sum\": %llu, \"stream_score_sum\": %.12g}\n", static_cast<unsigned long long>(n),
+                  static_cast<unsigned long long>(doc_sum), score_sum);
+    }
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
   sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_OR, terms, 1.2f, 0.75f, 100, &filt);
   ListCollector col;
   irs::ScoreFunction sf; irs::ColumnArgsFetcher fetcher;

@@ -12,8 +12,9 @@ void check(int rc, const char* what) {
 }  // namespace
 
 GpuTopKIterator::GpuTopKIterator(sdbg_segment* segment, int kind, std::vector<sdbg_bm25_term> terms, float k1, float b,
-                                 uint32_t k, const sdbg_col_pred* table_filter)
-    : seg_(segment), kind_(kind), terms_(std::move(terms)), k1_(k1), b_(b), k_(k), has_filter_(table_filter != nullptr) {
+                                 uint32_t k, const sdbg_col_pred* table_filter, std::vector<uint32_t> excluded_terms)
+    : seg_(segment), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)), k1_(k1), b_(b), k_(k),
+      has_filter_(table_filter != nullptr) {
   if (table_filter) filter_ = *table_filter;
   threshold_.value = FLT_MIN;  // doc_collector.hpp:102
 }
@@ -25,10 +26,13 @@ void GpuTopKIterator::run() {
     std::vector<uint32_t> docs;
     std::vector<float> scores;
     for (;;) {
-      const int rc = sdbg_bm25_scan(seg_, kind_, terms_.data(), terms_.size(), k1_, b_, has_filter_ ? &filter_ : nullptr, 1, UINT32_MAX,
-                                    docs.data(), scores.data(), cap, &n);
+      const sdbg_col_pred* f = has_filter_ ? &filter_ : nullptr;
+      const int rc = excluded_.empty()
+                         ? sdbg_bm25_scan(seg_, kind_, terms_.data(), terms_.size(), k1_, b_, f, 1, UINT32_MAX, docs.data(), scores.data(), cap, &n)
+                         : sdbg_bm25_scan_excl(seg_, kind_, terms_.data(), terms_.size(), excluded_.data(), excluded_.size(), k1_, b_, f, 1,
+                                               UINT32_MAX, docs.data(), scores.data(), cap, &n);
       if (rc == SDBG_ECAPACITY && n > cap) { cap = n; docs.resize(n); scores.resize(n); continue; }   // count-only call, then one with room
-      check(rc, "sdbg_bm25_scan");
+      check(rc, excluded_.empty() ? "sdbg_bm25_scan" : "sdbg_bm25_scan_excl");
       break;
     }
     by_doc_.resize(n);
@@ -42,9 +46,17 @@ void GpuTopKIterator::run() {
   uint32_t n = 0;
   float thr_out = 0;
   sdbg_segment* segs[1] = {seg_};
-  check(sdbg_bm25_topk(segs, 1, kind_, terms_.data(), terms_.size(), k1_, b_, has_filter_ ? &filter_ : nullptr, k_,
-                       threshold_.value, hits_.data(), &n, &total_, &thr_out),
-        "sdbg_bm25_topk");
+  if (excluded_.empty()) {
+    check(sdbg_bm25_topk(segs, 1, kind_, terms_.data(), terms_.size(), k1_, b_, has_filter_ ? &filter_ : nullptr, k_,
+                         threshold_.value, hits_.data(), &n, &total_, &thr_out),
+          "sdbg_bm25_topk");
+  } else {
+    const uint32_t term_off[2] = {0, uint32_t(terms_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
+    check(sdbg_bm25_topk_batch_excl(segs, 1, kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off, k1_, b_,
+                                    has_filter_ ? &filter_ : nullptr, k_, threshold_.value, hits_.data(), &n, &total_),
+          "sdbg_bm25_topk_batch_excl");
+    thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;   // as sdbg_bm25_topk derives it
+  }
   hits_.resize(n);
   by_doc_ = hits_;
   std::sort(by_doc_.begin(), by_doc_.end(), [](const sdbg_hit& a, const sdbg_hit& b) { return a.doc < b.doc; });

@@ -37,7 +37,8 @@ class GpuTopKIterator final : public irs::DocIterator {
   GpuTopKIterator(sdbg_segment* segment, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */,
                   std::vector<sdbg_bm25_term> terms /* BM25Stats per term + boost */, float k1 /* BM25::k() */,
                   float b /* BM25::b() */, uint32_t k /* 0 = streaming mode: every match, see EmitScoredDocs */,
-                  const sdbg_col_pred* table_filter /* nullable: the ColFilter wrap */);
+                  const sdbg_col_pred* table_filter /* nullable: the ColFilter wrap */,
+                  std::vector<uint32_t> excluded_terms = {} /* term ids of the And's Not children (irs exclusion.hpp) */);
 
   // Scored top-k: the hot path.
   void Collect(const irs::ScoreFunction&, irs::ColumnArgsFetcher&, irs::ScoreCollector& collector) override;
@@ -69,6 +70,7 @@ class GpuTopKIterator final : public irs::DocIterator {
   sdbg_segment* seg_;
   int kind_;
   std::vector<sdbg_bm25_term> terms_;
+  std::vector<uint32_t> excluded_;
   float k1_, b_;
   uint32_t k_;
   bool has_filter_;
