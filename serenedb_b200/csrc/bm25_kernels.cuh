@@ -60,6 +60,7 @@ struct QTermDev {  // one term of one query over one segment, 40 bytes
 constexpr uint32_t kMaxQueryTerms = 16;
 constexpr uint32_t kTopkThreads = 256;
 constexpr uint32_t kTopkWarps = kTopkThreads / 32;
+constexpr uint32_t kTopkBudget = 32;   // bm25_topk_kernel: posting blocks per window, one planner lane each
 
 __device__ __forceinline__ uint32_t desc_doc_enc(uint32_t p) { return p & 63u; }
 __device__ __forceinline__ uint32_t desc_freq_enc(uint32_t p) { return (p >> 6) & 63u; }
@@ -276,8 +277,8 @@ decode_score_kernel(PostingsDev seg, uint32_t blk_begin, uint32_t nblk, float c0
 //
 // grid = (chains G, queries Q). CTA (g, q) owns the doc range [1 + g*chunk, min(N, (g+1)*chunk)] of
 // query q and walks it in WINDOWS DEFINED BY A BLOCK BUDGET, not by a doc count: every window holds
-// at most kBudget posting blocks in total (kBudget / T per term), so the fixed per-window costs are
-// amortised over up to kBudget*128 postings whether the lists are dense (p = 0.5: a window spans a
+// at most kTopkBudget posting blocks in total (kTopkBudget / T per term), so the fixed per-window costs are
+// amortised over up to kTopkBudget*128 postings whether the lists are dense (p = 0.5: a window spans a
 // few hundred docs) or sparse (p = 0.002: hundreds of thousands). The reference gets the same effect
 // from ComputeOuterWindow, which aligns windows with the essential lists' block boundaries
 // (search/max_score_iterator.hpp:510-539).
@@ -298,7 +299,7 @@ decode_score_kernel(PostingsDev seg, uint32_t blk_begin, uint32_t nblk, float c0
 //   3. emit: live in-window entries -> column filter -> threshold -> ballot-compacted append to the
 //      per-CTA candidate buffer (bitonic select when full = nth_element at 2k, iterators.hpp:216-228).
 //
-// Shared memory (dynamic): docs[E] u32 | score[E] f32 | cnt[E] u8 (AND only) | cand[cap] u64, E = kBudget*128.
+// Shared memory (dynamic): docs[E] u32 | score[E] f32 | cnt[E] u8 (AND only) | cand[cap] u64, E = kTopkBudget*128.
 // ------------------------------------------------------------------------------------------
 struct TopkParams {
   PostingsDev seg;
@@ -485,11 +486,11 @@ __device__ __noinline__ bool excluded_doc(const uint4* arena, const uint4* block
 
 // kDrive compiles the driver-mode code (pruning level 2) in; the default kernel stays free of its registers. kExcl: the
 // queries of the launch exclude terms (TopkParams::excl); likewise kept out of the other instantiations.
-template <uint32_t kBudget, bool kDrive, bool kExcl = false>
+template <bool kDrive, bool kExcl = false>
 __global__ void __launch_bounds__(kTopkThreads)
 bm25_topk_kernel(const TopkParams P) {
-  constexpr uint32_t kEntries = kBudget * 128u;
-  static_assert(kBudget <= 32, "one planner lane per block");
+  constexpr uint32_t kEntries = kTopkBudget * 128u;
+  static_assert(kTopkBudget <= 32, "one planner lane per block");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint32_t* e_doc = reinterpret_cast<uint32_t*>(smem_raw);
   float* e_score = reinterpret_cast<float*>(e_doc + kEntries);
@@ -522,7 +523,7 @@ bm25_topk_kernel(const TopkParams P) {
   const uint32_t T = min(P.qterm_off[q + 1] - t0, kMaxQueryTerms);
   const uint32_t x0 = kExcl ? P.excl_off[q] : 0u;
   const uint32_t n_ex = kExcl ? min(P.excl_off[q + 1] - x0, kMaxQueryTerms) : 0u;
-  const uint32_t m = max(1u, kBudget / T);                       // block budget per term
+  const uint32_t m = max(1u, kTopkBudget / T);                      // block budget per term
   const unsigned long long first64 = work.y;
   const bool chain_empty = first64 > P.seg.n_docs;
   const uint32_t chain_lo = chain_empty ? 1u : uint32_t(first64);
@@ -571,7 +572,7 @@ bm25_topk_kernel(const TopkParams P) {
     __syncwarp();
     const bool driver = kDrive && s_driver != 0u;
     const uint32_t Tp = driver ? T - 1u : T;             // lists that get planner lanes
-    const uint32_t mp = max(1u, kBudget / Tp);
+    const uint32_t mp = max(1u, kTopkBudget / Tp);
     for (uint32_t tries = 0;; ++tries) {
       if (lo > chain_hi || lo == 0u) {  // lo == 0: wrapped past 2^32-1
         if (lane == 0) s_valid[buf] = 0u;

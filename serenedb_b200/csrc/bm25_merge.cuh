@@ -79,19 +79,15 @@ __device__ __forceinline__ void merge_decode_block_smem(const uint4* pd, const u
 constexpr uint32_t kMergeWin = 16u;
 constexpr uint32_t kMergeTermBytes = 512u + 512u + 1024u + kMergeWin * 16u;
 
-#ifndef SDBG_MERGE_MIN_BLOCKS
-#define SDBG_MERGE_MIN_BLOCKS 3
-#endif
-// Dynamic shared memory: cand[cap] u64 | lut[T][kLutFreqs][256] f32 (kLut) | per warp: T x kMergeTermBytes.
+// Dynamic shared memory: cand[cap] u64 | per warp: T x kMergeTermBytes.
 // Terms are in ascending-cost order (the host sorts them); T-1 is the "top" term.
-template <uint32_t T, bool kLut>
-__global__ void __launch_bounds__(kTopkThreads, SDBG_MERGE_MIN_BLOCKS)
+template <uint32_t T>
+__global__ void __launch_bounds__(kTopkThreads, kStreamMinBlocks)
 bm25_merge_kernel(const TopkParams P) {
   static_assert(T >= 1 && T <= kStreamMaxTerms, "1..4 terms");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* cand = reinterpret_cast<unsigned long long*>(smem_raw);
-  float* lut = reinterpret_cast<float*>(cand + P.cap);
-  unsigned char* warp_area = reinterpret_cast<unsigned char*>(lut + (kLut ? T * kLutFreqs * 256u : 0u));
+  unsigned char* warp_area = reinterpret_cast<unsigned char*>(cand + P.cap);
 
   __shared__ __align__(16) StreamCtl ctl;
   __shared__ uint64_t s_bar[kTopkWarps][kStreamMaxTerms][2];
@@ -145,17 +141,8 @@ bm25_merge_kernel(const TopkParams P) {
     __syncthreads();
     if (ctl.full == 0xFFFFFFFFu) return;                 // the lead-mode kernel owns this item
   }
-  if constexpr (kLut) {
-    // thread = norm byte; same arithmetic as the per-posting evaluation, so a table hit is bit-identical
-#pragma unroll 1
-    for (uint32_t i = 0; i < T * kLutFreqs; ++i) {
-      const uint32_t t = i / kLutFreqs, f = i % kLutFreqs;
-      lut[i * 256u + tid] = bm25(f + 1u, tid, s_qt[t].c0, s_qt[t].norm_const, s_qt[t].norm_length);
-    }
-    __syncthreads();
-  }
   unsigned long long* const theta_global = P.theta + q;
-  const uint8_t* const norms_m1 = P.seg.norms ? P.seg.norms - 1 : nullptr;   // row = doc - 1 (1-byte norms: kLut)
+  const uint8_t* const norms_m1 = P.seg.norms ? P.seg.norms - 1 : nullptr;   // row = doc - 1 (full blocks, 1-byte norms)
 
   if (!warp_empty) {
     // ---- per-term stream state: registers (every loop over t is unrolled) ----
@@ -252,30 +239,13 @@ bm25_merge_kernel(const TopkParams P) {
         for (int j = 0; j < 4; ++j) {
           const bool valid = 4u * lane + j < len;
           if (!valid) { doc[j] = kNoDoc; f[j] = 1u; }
-          if constexpr (kLut) nrm[j] = (valid && norms_m1) ? __ldg(norms_m1 + doc[j]) : 1u;
-          else nrm[j] = valid ? load_norm(P.seg.norms, P.seg.norm_width, doc[j]) : 1u;
+          nrm[j] = valid ? load_norm(P.seg.norms, P.seg.norm_width, doc[j]) : 1u;
         }
       }
       float s[4];
-      if constexpr (kLut) {
-        bool slow = false;
-        const float* lt = lut + t * kLutFreqs * 256u;
+      const float c0 = s_qt[t].c0, nc = s_qt[t].norm_const, nl = s_qt[t].norm_length;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          slow |= f[j] > kLutFreqs;
-          s[j] = lt[min(f[j] - 1u, kLutFreqs - 1u) * 256u + nrm[j]];
-        }
-        if (__any_sync(kFull, slow)) {
-          const float c0 = s_qt[t].c0, nc = s_qt[t].norm_const, nl = s_qt[t].norm_length;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (f[j] > kLutFreqs) s[j] = bm25_plain(f[j], nrm[j], c0, nc, nl);
-        }
-      } else {
-        const float c0 = s_qt[t].c0, nc = s_qt[t].norm_const, nl = s_qt[t].norm_length;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) s[j] = bm25_plain(f[j], nrm[j], c0, nc, nl);
-      }
+      for (int j = 0; j < 4; ++j) s[j] = bm25_plain(f[j], nrm[j], c0, nc, nl);
       reinterpret_cast<uint4*>(ld)[lane] = make_uint4(doc[0], doc[1], doc[2], doc[3]);
       reinterpret_cast<float4*>(ls)[lane] = make_float4(s[0], s[1], s[2], s[3]);
       a0[t] = 0u;

@@ -70,8 +70,7 @@ struct sdbg_ctx {
   void* flush = nullptr;
   size_t flush_bytes = 0;
   cudaEvent_t ev_copy[16] = {};   // one per host conversion thread (sdbg_bm25_topk_batch)
-  bool scan_attr_set = false;
-  bool topk_attr_set = false;
+  bool topk_attr_set = false;   // topk_smem_attrs has run
   void* nccl_comm = nullptr;   // ncclComm_t once sdbg_dist_init ran
   unsigned long long* h_oor = nullptr;   // pinned: out-of-range key count of the last deferred GROUP BY partial
   void* h_result = nullptr;     // mapped pinned memory the point-query kernels write their result into (no D2H copy)
@@ -83,7 +82,6 @@ struct sdbg_ctx {
   uint64_t zone_blocks_total = 0;   // last GROUP BY scan: 2048-row blocks seen / proven dead by their zonemaps
   unsigned long long* d_zone_skipped = nullptr;
   int dist_rank = 0, dist_world = 1;
-  bool merge_attr_set = false;
   // optional per-kernel timing: CUDA events recorded on `stream` around the hot kernels
   int wand = 1;       // block-max pruning level: 0 off (exact total_matches), 1 planner-level block/window skips, 2 + exact-partial-score skips of the largest term
   bool profiling = false;
@@ -751,26 +749,60 @@ uint2 excl_list(const sdbg_segment* s, uint32_t term) {
   return make_uint2(s->term_blk_begin[term], s->term_blk_begin[term + 1] - s->term_blk_begin[term]);
 }
 
-// Dynamic shared memory limit of the kernels that serve queries with excluded terms (top-k and scored scan).
-cudaError_t set_excl_attrs() {
-  const cudaFuncAttribute a = cudaFuncAttributeMaxDynamicSharedMemorySize;
-  const int v = 200 * 1024;
-  cudaError_t e = cudaSuccess;
-  auto set = [&](cudaError_t r) { if (e == cudaSuccess) e = r; };
-  set(cudaFuncSetAttribute(bm25_topk_kernel<16, false, true>, a, v));
-  set(cudaFuncSetAttribute(bm25_topk_kernel<32, false, true>, a, v));
-  set(cudaFuncSetAttribute(bm25_topk_kernel<16, true, true>, a, v));
-  set(cudaFuncSetAttribute(bm25_topk_kernel<32, true, true>, a, v));
-  set(cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeOr, true>, a, v));
-  set(cudaFuncSetAttribute(bm25_stream_kernel<2, false, 3, kModeOr, true>, a, v));
-  set(cudaFuncSetAttribute(bm25_stream_kernel<3, false, 3, kModeOr, true>, a, v));
-  set(cudaFuncSetAttribute(bm25_stream_kernel<4, false, 3, kModeOr, true>, a, v));
-  set(cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeAnd, true>, a, v));
-  return e;
+// The instantiation of a top-k kernel family for a run-time term count T = 1..4. Conjunctions and lead mode stream one
+// list (T = 1) and probe the others.
+using TopkKernel = void (*)(TopkParams);
+TopkKernel merge_kernel(uint32_t T) {
+  switch (T) {
+    case 1: return bm25_merge_kernel<1>;
+    case 2: return bm25_merge_kernel<2>;
+    case 3: return bm25_merge_kernel<3>;
+    default: return bm25_merge_kernel<4>;
+  }
+}
+template <int kMode, bool kExcl = false>
+TopkKernel stream_kernel(uint32_t T) {
+  if constexpr (kMode != kModeOr) {
+    return bm25_stream_kernel<1, kMode, kExcl>;
+  } else {
+    switch (T) {
+      case 1: return bm25_stream_kernel<1, kModeOr, kExcl>;
+      case 2: return bm25_stream_kernel<2, kModeOr, kExcl>;
+      case 3: return bm25_stream_kernel<3, kModeOr, kExcl>;
+      default: return bm25_stream_kernel<4, kModeOr, kExcl>;
+    }
+  }
+}
+
+// Dynamic shared memory of bm25_stream_kernel: candidates | per warp T live blocks with their prefetch slots, plus the
+// probe ring when lists are probed (conjunctions, lead mode).
+size_t stream_smem(uint32_t cap, uint32_t T, bool probe_rest) {
+  return size_t(cap) * 8 + size_t(kTopkWarps) * (T * kStreamTermBytes + (probe_rest ? 1024 : 0));
+}
+
+// Lets every top-k kernel use 200 KB of dynamic shared memory; once per context.
+int topk_smem_attrs(sdbg_ctx* c) {
+  if (c->topk_attr_set) return SDBG_OK;
+  auto set = [](TopkKernel k) { return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); };
+  for (uint32_t T = 1; T <= kStreamMaxTerms; ++T) {
+    CU(c, set(merge_kernel(T)));
+    CU(c, set(stream_kernel<kModeOr>(T)));
+    CU(c, set(stream_kernel<kModeOr, true>(T)));
+  }
+  CU(c, set(stream_kernel<kModeAnd>(1)));
+  CU(c, set(stream_kernel<kModeAnd, true>(1)));
+  CU(c, set(stream_kernel<kModeLead>(1)));
+  CU(c, set(bm25_topk_kernel<false>));
+  CU(c, set(bm25_topk_kernel<true>));
+  CU(c, set(bm25_topk_kernel<false, true>));
+  CU(c, set(bm25_topk_kernel<true, true>));
+  CU(c, cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  c->topk_attr_set = true;
+  return SDBG_OK;
 }
 
 struct TopkPlan {
-  uint32_t G, cap, k, budget;
+  uint32_t G, cap, k;
   size_t smem;
 };
 
@@ -814,22 +846,20 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
 
   TopkPlan pl;
   pl.k = k;
-  pl.budget = uint32_t(env_int("SDBG_TOPK_BUDGET", 32));
-  if (pl.budget != 16 && pl.budget != 32) return fail(c, SDBG_EINVAL, "SDBG_TOPK_BUDGET must be 16 or 32");
-  const uint32_t entries = pl.budget * 128u;
-  pl.cap = std::max(next_pow2(k + 1024), uint32_t(env_int("SDBG_TOPK_CAP", 2048)));  // selection is O(n): buffer size trades shared memory (occupancy) against selection count
+  const uint32_t entries = kTopkBudget * 128u;
+  pl.cap = std::max(next_pow2(k + 1024), 2048u);  // selection is O(n): buffer size trades shared memory (occupancy) against selection count
   // Enough CTAs to fill the machine a few times over; a query is split into chains (contiguous doc
   // ranges) only when the batch alone cannot do that.
   const uint32_t target_ctas = uint32_t(c->sm_count) * 8u;
   pl.G = uint32_t(std::max<size_t>(1, (target_ctas + nq - 1) / nq));
-  const uint32_t max_chains = uint32_t(env_int("SDBG_TOPK_MAX_CHAINS", 2 * c->sm_count));
+  const uint32_t max_chains = 2u * uint32_t(c->sm_count);
   // Work list: (segment, query) pairs get max(G, postings / target) chains, so that a query over a 5 M-doc
   // list is not one CTA-long critical path next to thousands of short ones; largest chains are issued first.
   uint64_t batch_postings = 0;
   for (size_t si = 0; si < n_segs; ++si)
     for (uint32_t i = 0; i < total_terms; ++i)
       if (terms[i].term < segs[si]->term_docs.size()) batch_postings += segs[si]->term_docs[terms[i].term];
-  const uint64_t chain_target = std::max<uint64_t>(uint64_t(env_int("SDBG_TOPK_CHAIN_MIN", 65536)), batch_postings / (uint64_t(c->sm_count) * uint64_t(std::max(1, env_int("SDBG_TOPK_CHAIN_DIV", 4)))));
+  const uint64_t chain_target = std::max<uint64_t>(65536, batch_postings / (uint64_t(c->sm_count) * 4u));
   // Work classes (one launch each):
   //   0 / 1        legacy window kernel (driver mode / plain): > 4-term disjunctions, BM15 / BM1 forms
   //   2 + (T-1)    exhaustive warp-autonomous merge of T = 1..4 lists (bm25_merge.cuh): pruning off or not applicable
@@ -847,7 +877,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
                      kClsLead = kClsAnd + 2, kClasses = kClsAnd + 3, kAllClasses = 2 * kClasses;
   const bool level2 = c->wand >= 2 && kind != SDBG_QUERY_AND && k1 != 0.f && k1 != kTfidfK1 && b != 0.f;
   const bool stream_ok = env_int("SDBG_STREAM", 1) != 0 && k1 != 0.f && b != 0.f && k1 != kTfidfK1 &&
-                         size_t(pl.cap) * 8 + size_t(kStreamMaxTerms) * (kLutFreqs * 1024 + kTopkWarps * kStreamTermBytes) <= 200 * 1024;
+                         stream_smem(pl.cap, kStreamMaxTerms, false) <= 200 * 1024;
   const bool lead_ok = env_int("SDBG_STREAM_LEAD", 1) != 0;
   // The staged block-max pairs are maximisers for BM25 with the index-time b only (FreqNormProducer::CmpBm25,
   // wand_writer.hpp:142-175; the order of two pairs does not depend on k); the reference enables WAND only when
@@ -878,7 +908,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
       const bool excludes = total_excl && excl_off[q + 1] > excl_off[q];
       uint32_t cls = drive_q ? 0u : 1u;
       uint32_t slice_docs = 0;    // > 0: lead candidate
-      if (stream_ok && kind == SDBG_QUERY_AND && env_int("SDBG_STREAM_AND", 1) != 0) cls = kClsAnd;
+      if (stream_ok && kind == SDBG_QUERY_AND) cls = kClsAnd;
       else if (stream_ok && kind != SDBG_QUERY_AND && nt <= kStreamMaxTerms) {
         const bool plain = !filt && !s->d_deleted && !excludes;     // the merge kernel has no per-doc checks
         cls = (!plain || (wand && (nt != 2 || !lead_ok))) ? kClsStream + (nt - 1u) : kClsMerge + (nt - 1u);
@@ -917,7 +947,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
       if (excludes) cls += kClasses;
       uint32_t g = uint32_t(std::max<uint64_t>(pl.G, (rest_postings + chain_target - 1) / chain_target));
       // lead mode is latency-bound (dependent loads per probe), not throughput-bound: more, shorter chains
-      if (slice_docs) g = std::max(g, std::min<uint32_t>(uint32_t(env_int("SDBG_STREAM_LEAD_CHAINS", 16)), std::max(1u, smallest / 8192u)));
+      if (slice_docs) g = std::max(g, std::min(16u, std::max(1u, smallest / 8192u)));
       g = std::min(g, max_chains);
       g = std::min(g, std::max(1u, rest_docs / 4096u));
       const uint32_t chunk = (rest_docs + g - 1) / g;
@@ -993,32 +1023,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   ++c->launches;
   CU(c, cudaMemsetAsync(d_total, 0, nq * 8, c->stream));
 
-  // shared memory of the stream kernel: candidates | score table | per warp (live blocks + prefetch slots)
-  bool use_lut[n_segs ? n_segs : 1];
-  for (size_t si = 0; si < n_segs; ++si) use_lut[si] = segs[si]->norm_width == 1 && env_int("SDBG_STREAM_LUT", 0) != 0;
-  auto stream_smem = [&](uint32_t T, bool lut, bool conj) {
-    return size_t(pl.cap) * 8 + (lut ? size_t(T) * kLutFreqs * 1024 : 0) + size_t(kTopkWarps) * (T * kStreamTermBytes + (conj ? 1024 : 0));
-  };
-  if (!c->topk_attr_set) {
-    CU(c, cudaFuncSetAttribute(bm25_topk_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, cudaFuncSetAttribute(bm25_topk_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, cudaFuncSetAttribute(bm25_topk_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, cudaFuncSetAttribute(bm25_topk_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-#define SDBG_STREAM_ATTR(TT) \
-    CU(c, cudaFuncSetAttribute(bm25_merge_kernel<TT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
-    CU(c, cudaFuncSetAttribute(bm25_merge_kernel<TT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<TT, false, 3, kModeOr>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<TT, true, 3, kModeOr>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024))
-    SDBG_STREAM_ATTR(1); SDBG_STREAM_ATTR(2); SDBG_STREAM_ATTR(3); SDBG_STREAM_ATTR(4);
-#undef SDBG_STREAM_ATTR
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeAnd>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, true, 3, kModeAnd>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeLead>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, true, 3, kModeLead>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, set_excl_attrs());
-    c->topk_attr_set = true;
-  }
+  if ((rc = topk_smem_attrs(c))) return rc;
   // one claim word per work item of class kClsLead (zeroed per call)
   size_t n_lead_total = 0;
   for (size_t si = 0; si < n_segs; ++si) n_lead_total += n_cls[si][kClsLead];
@@ -1055,23 +1060,13 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
         P.excl_off = reinterpret_cast<const uint32_t*>(static_cast<const char*>(b_qt.p) + x_pos + x_lists);
       }
       const int wand = seg_wand(s);
-      const bool lut = use_lut[si];
       const uint4* const work0 = reinterpret_cast<const uint4*>(static_cast<const char*>(b_qt.p) + qt_pad) + work_done;
       work_done += seg_work[si].size();
       std::array<size_t, kAllClasses> cls_off{};
       { size_t o = 0; for (uint32_t cls = 0; cls < kAllClasses; ++cls) { cls_off[cls] = o; o += n_cls[si][cls]; } }
       auto launch_merge = [&](uint32_t T, size_t n, cudaStream_t st) {
-        const size_t sm = size_t(pl.cap) * 8 + (lut ? size_t(T) * kLutFreqs * 1024 : 0) + size_t(kTopkWarps) * T * kMergeTermBytes;
-#define SDBG_MERGE_LAUNCH(TT) \
-        if (lut) bm25_merge_kernel<TT, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); \
-        else bm25_merge_kernel<TT, false><<<unsigned(n), kTopkThreads, sm, st>>>(P)
-        switch (T) {
-          case 1: SDBG_MERGE_LAUNCH(1); break;
-          case 2: SDBG_MERGE_LAUNCH(2); break;
-          case 3: SDBG_MERGE_LAUNCH(3); break;
-          default: SDBG_MERGE_LAUNCH(4); break;
-        }
-#undef SDBG_MERGE_LAUNCH
+        const size_t sm = size_t(pl.cap) * 8 + size_t(kTopkWarps) * T * kMergeTermBytes;
+        merge_kernel(T)<<<unsigned(n), kTopkThreads, sm, st>>>(P);
         ++c->launches;
       };
       // first slices: before everything else of this segment, on the main stream
@@ -1089,79 +1084,45 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
         cudaStream_t st = (two_lanes && (lane_no++ & 1u)) ? c->stream2 : c->stream;
         P.work = work0 + cls_off[cls];
         P.claim = nullptr;
-        if (cls >= kClasses) {
-          // queries with excluded terms: the kExcl instantiations (without the opt-in score table, a speed variant only)
-          const uint32_t cb = cls - kClasses;
-          if (cb == 0) {
-            P.wand = wand;
-            if (pl.budget == 16) bm25_topk_kernel<16, true, true><<<unsigned(n), kTopkThreads, smem_drive, st>>>(P);
-            else bm25_topk_kernel<32, true, true><<<unsigned(n), kTopkThreads, smem_drive, st>>>(P);
-          } else if (cb == 1) {
-            P.wand = std::min(wand, 1);
-            if (pl.budget == 16) bm25_topk_kernel<16, false, true><<<unsigned(n), kTopkThreads, pl.smem, st>>>(P);
-            else bm25_topk_kernel<32, false, true><<<unsigned(n), kTopkThreads, pl.smem, st>>>(P);
-          } else if (cb == kClsAnd) {
-            P.wand = 0;
-            bm25_stream_kernel<1, false, 3, kModeAnd, true><<<unsigned(n), kTopkThreads, stream_smem(1, false, true), st>>>(P);
-          } else {
-            const uint32_t T = cb - kClsStream + 1u;
-            const size_t sm = stream_smem(T, false, false);
-            P.wand = wand ? (wand | (env_int("SDBG_STREAM_DBG", 0) & 0xF0)) : 0;
-            switch (T) {
-              case 1: bm25_stream_kernel<1, false, 3, kModeOr, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); break;
-              case 2: bm25_stream_kernel<2, false, 3, kModeOr, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); break;
-              case 3: bm25_stream_kernel<3, false, 3, kModeOr, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); break;
-              default: bm25_stream_kernel<4, false, 3, kModeOr, true><<<unsigned(n), kTopkThreads, sm, st>>>(P); break;
-            }
-          }
-          ++c->launches;
-        } else if (cls == 0) {
+        // queries with excluded terms: the kExcl instantiations of the same kernels
+        const bool excl = cls >= kClasses;
+        const uint32_t cb = excl ? cls - kClasses : cls;
+        TopkKernel kern;
+        size_t sm;
+        if (cb == 0) {
           P.wand = wand;
-          if (pl.budget == 16) bm25_topk_kernel<16, true><<<unsigned(n), kTopkThreads, smem_drive, st>>>(P);
-          else bm25_topk_kernel<32, true><<<unsigned(n), kTopkThreads, smem_drive, st>>>(P);
-          ++c->launches;
-        } else if (cls == 1) {
+          kern = excl ? bm25_topk_kernel<true, true> : bm25_topk_kernel<true>;
+          sm = smem_drive;
+        } else if (cb == 1) {
           P.wand = std::min(wand, 1);
-          if (pl.budget == 16) bm25_topk_kernel<16, false><<<unsigned(n), kTopkThreads, pl.smem, st>>>(P);
-          else bm25_topk_kernel<32, false><<<unsigned(n), kTopkThreads, pl.smem, st>>>(P);
-          ++c->launches;
-        } else if (cls == kClsAnd) {
-          const size_t sm = stream_smem(1, lut, true);
+          kern = excl ? bm25_topk_kernel<false, true> : bm25_topk_kernel<false>;
+          sm = pl.smem;
+        } else if (cb == kClsAnd) {
           P.wand = 0;                                  // conjunctions are exact: every candidate of the lead list is probed
-          if (lut) bm25_stream_kernel<1, true, 3, kModeAnd><<<unsigned(n), kTopkThreads, sm, st>>>(P);
-          else bm25_stream_kernel<1, false, 3, kModeAnd><<<unsigned(n), kTopkThreads, sm, st>>>(P);
-          ++c->launches;
-        } else if (cls == kClsLead) {
+          kern = excl ? stream_kernel<kModeAnd, true>(1) : stream_kernel<kModeAnd>(1);
+          sm = stream_smem(pl.cap, 1, true);
+        } else if (cb == kClsLead) {
           // both kernels over the same items; each item is run by exactly one of them (claim word)
           P.claim = static_cast<uint32_t*>(b_claim.p) + lead_done;
           lead_done += n;
           P.wand = 0;
           launch_merge(2, n, c->stream);
-          const size_t sm = stream_smem(1, lut, true);
-          P.wand = wand | (env_int("SDBG_STREAM_DBG", 0) & 0xF0);
-          cudaStream_t st2 = two_lanes ? c->stream2 : c->stream;
-          if (lut) bm25_stream_kernel<1, true, 3, kModeLead><<<unsigned(n), kTopkThreads, sm, st2>>>(P);
-          else bm25_stream_kernel<1, false, 3, kModeLead><<<unsigned(n), kTopkThreads, sm, st2>>>(P);
-          ++c->launches;
-        } else if (cls >= kClsStream) {
-          const uint32_t T = cls - kClsStream + 1u;
-          const size_t sm = stream_smem(T, lut, false);
-          P.wand = wand ? (wand | (env_int("SDBG_STREAM_DBG", 0) & 0xF0)) : 0;   // debug bits 16/32/64/128 switch parts of the pruning off
-#define SDBG_STREAM_LAUNCH(TT) \
-          if (lut) bm25_stream_kernel<TT, true, 3, kModeOr><<<unsigned(n), kTopkThreads, sm, st>>>(P); \
-          else bm25_stream_kernel<TT, false, 3, kModeOr><<<unsigned(n), kTopkThreads, sm, st>>>(P)
-          switch (T) {
-            case 1: SDBG_STREAM_LAUNCH(1); break;
-            case 2: SDBG_STREAM_LAUNCH(2); break;
-            case 3: SDBG_STREAM_LAUNCH(3); break;
-            default: SDBG_STREAM_LAUNCH(4); break;
-          }
-#undef SDBG_STREAM_LAUNCH
-          ++c->launches;
+          P.wand = wand;
+          kern = stream_kernel<kModeLead>(1);
+          sm = stream_smem(pl.cap, 1, true);
+          st = two_lanes ? c->stream2 : c->stream;
+        } else if (cb >= kClsStream) {
+          const uint32_t T = cb - kClsStream + 1u;
+          P.wand = wand;
+          kern = excl ? stream_kernel<kModeOr, true>(T) : stream_kernel<kModeOr>(T);
+          sm = stream_smem(pl.cap, T, false);
         } else {
           P.wand = 0;
-          launch_merge(cls - kClsMerge + 1u, n, st);
+          launch_merge(cb - kClsMerge + 1u, n, st);
+          continue;
         }
+        kern<<<unsigned(n), kTopkThreads, sm, st>>>(P);
+        ++c->launches;
       }
       CU(c, cudaGetLastError());
       base += s->n_docs;
@@ -1412,43 +1373,13 @@ int scan_run(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_te
   P.emit_cap = cap;
   auto* sorted_docs = reinterpret_cast<uint32_t*>(e + 2 * pair_bytes);
   auto* sorted_scores = reinterpret_cast<float*>(e + 3 * pair_bytes);
-  const bool lut = n_excl == 0 && s->norm_width == 1 && env_int("SDBG_STREAM_LUT", 0) != 0;
-  const uint32_t Tl = conj ? 1u : T;
-  const size_t sm = size_t(scan_cap) * 8 + (lut ? size_t(Tl) * kLutFreqs * 1024 : 0) + size_t(kTopkWarps) * (Tl * kStreamTermBytes + (conj ? 1024 : 0));
-  if (!c->scan_attr_set) {
-#define SDBG_SCAN_ATTR(TT) \
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<TT, false, 3, kModeOr>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<TT, true, 3, kModeOr>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024))
-    SDBG_SCAN_ATTR(1); SDBG_SCAN_ATTR(2); SDBG_SCAN_ATTR(3); SDBG_SCAN_ATTR(4);
-#undef SDBG_SCAN_ATTR
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, false, 3, kModeAnd>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, cudaFuncSetAttribute(bm25_stream_kernel<1, true, 3, kModeAnd>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU(c, set_excl_attrs());
-    c->scan_attr_set = true;
-  }
+  if ((rc = topk_smem_attrs(c))) return rc;
+  TopkKernel kern;
+  if (n_excl) kern = conj ? stream_kernel<kModeAnd, true>(1) : stream_kernel<kModeOr, true>(T);   // as in topk_run
+  else kern = conj ? stream_kernel<kModeAnd>(1) : stream_kernel<kModeOr>(T);
   {
     ProfScope ps_(c, kProfTopk);
-    if (n_excl) {                                                    // the kExcl instantiations, as in topk_run
-      if (conj) bm25_stream_kernel<1, false, 3, kModeAnd, true><<<g, kTopkThreads, sm, c->stream>>>(P);
-      else if (T == 1) bm25_stream_kernel<1, false, 3, kModeOr, true><<<g, kTopkThreads, sm, c->stream>>>(P);
-      else if (T == 2) bm25_stream_kernel<2, false, 3, kModeOr, true><<<g, kTopkThreads, sm, c->stream>>>(P);
-      else if (T == 3) bm25_stream_kernel<3, false, 3, kModeOr, true><<<g, kTopkThreads, sm, c->stream>>>(P);
-      else bm25_stream_kernel<4, false, 3, kModeOr, true><<<g, kTopkThreads, sm, c->stream>>>(P);
-    } else if (conj) {
-      if (lut) bm25_stream_kernel<1, true, 3, kModeAnd><<<g, kTopkThreads, sm, c->stream>>>(P);
-      else bm25_stream_kernel<1, false, 3, kModeAnd><<<g, kTopkThreads, sm, c->stream>>>(P);
-    } else {
-#define SDBG_SCAN_LAUNCH(TT) \
-      if (lut) bm25_stream_kernel<TT, true, 3, kModeOr><<<g, kTopkThreads, sm, c->stream>>>(P); \
-      else bm25_stream_kernel<TT, false, 3, kModeOr><<<g, kTopkThreads, sm, c->stream>>>(P)
-      switch (T) {
-        case 1: SDBG_SCAN_LAUNCH(1); break;
-        case 2: SDBG_SCAN_LAUNCH(2); break;
-        case 3: SDBG_SCAN_LAUNCH(3); break;
-        default: SDBG_SCAN_LAUNCH(4); break;
-      }
-#undef SDBG_SCAN_LAUNCH
-    }
+    kern<<<g, kTopkThreads, stream_smem(scan_cap, conj ? 1u : T, conj), c->stream>>>(P);
   }
   ++c->launches;
   CU(c, cudaGetLastError());
@@ -1553,10 +1484,7 @@ extern "C" int sdbg_topk_merge_gathered(sdbg_ctx* c, const void* d_keys_all, uin
                             static_cast<const char*>(d_keys_all) + size_t(r) * nq * k * 8, size_t(k) * 8, size_t(k) * 8, nq,
                             cudaMemcpyDeviceToDevice, c->stream));
   const uint32_t cap = std::max(next_pow2(k + 1024), 4096u);
-  if (!c->merge_attr_set) {
-    CU(c, cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    c->merge_attr_set = true;
-  }
+  if ((rc = topk_smem_attrs(c))) return rc;
   MergeParams M;
   M.cand = static_cast<const unsigned long long*>(b_in.p); M.cand_n = nullptr; M.list_off = nullptr;
   M.G = n_ranks; M.stride = k; M.k = k; M.cap = cap;

@@ -33,7 +33,7 @@ def shipped_pruning():
     ctx().set_wand(2)
     yield
     ctx().set_wand(0)
-    for k in ("SDBG_STREAM", "SDBG_STREAM_LEAD", "SDBG_STREAM_AND"):
+    for k in ("SDBG_STREAM", "SDBG_STREAM_LEAD"):
         os.environ.pop(k, None)
 
 
@@ -44,10 +44,12 @@ OR_QUERIES = [([81, 1], 100), ([5, 59], 1000), ([0, 1], 10), ([40, 41], 1000), (
 @pytest.mark.parametrize("tis,k", OR_QUERIES)
 def test_disjunctions_pruned_equal_exhaustive(corpus, tis, k):
     scorer = sdb.BM25()
-    hits, total = sdb.ExecuteTopK(corpus["reader"], tis, sdb.OR, scorer, k)
     oh, ototal, _ = orc.bm25_topk([corpus["oseg"]], "OR", oracle_terms(corpus["reader"], scorer, tis), k, mode=1)
-    assert_hits_equal(hits, oh)
-    assert total <= ototal
+    for wand in (2, 0):       # the shipped level, and pruning off (exact total)
+        ctx().set_wand(wand)
+        hits, total = sdb.ExecuteTopK(corpus["reader"], tis, sdb.OR, scorer, k)
+        assert_hits_equal(hits, oh)
+        assert total <= ototal if wand else total == ototal
 
 
 def test_lead_mode_engages_and_matches(corpus):
@@ -71,18 +73,21 @@ def test_lead_mode_engages_and_matches(corpus):
 
 
 @pytest.mark.parametrize("tis,k,with_filter", [([0, 1, 2, 3, 4], 1000, True), ([5, 59], 100, False), ([1, 36, 80], 100, True),
-                                               ([0, 95], 10, False), ([0, 1, 2, 3, 4, 5, 6, 7], 100, False)])
+                                               ([0, 95], 10, False), ([0, 1, 2, 3, 4, 5, 6, 7], 100, False),
+                                               ([0, 1, 2], 50, False)])
 def test_conjunctions_by_probe_exact(corpus, tis, k, with_filter):
     scorer = sdb.BM25()
     fg = sdb.pred(9, "BETWEEN", 250000, 749999) if with_filter else None
     fo = orc.make_pred(9, "BETWEEN", 250000, 749999) if with_filter else None
-    hits, total = sdb.ExecuteTopK(corpus["reader"], tis, sdb.AND, scorer, k, filt=fg)
     oh, ototal, _ = orc.bm25_topk([corpus["oseg"]], "AND", oracle_terms(corpus["reader"], scorer, tis), k, filt=fo, mode=1)
-    assert_hits_equal(hits, oh)
-    assert total == ototal
-    os.environ["SDBG_STREAM_AND"] = "0"       # the window kernel's conjunction must agree
+    for wand in (0, 2):       # exact at every pruning level
+        ctx().set_wand(wand)
+        hits, total = sdb.ExecuteTopK(corpus["reader"], tis, sdb.AND, scorer, k, filt=fg)
+        assert_hits_equal(hits, oh)
+        assert total == ototal
+    os.environ["SDBG_STREAM"] = "0"          # the window kernel's conjunction must agree
     hits2, total2 = sdb.ExecuteTopK(corpus["reader"], tis, sdb.AND, scorer, k, filt=fg)
-    os.environ.pop("SDBG_STREAM_AND")
+    os.environ.pop("SDBG_STREAM")
     assert_hits_equal(hits2, oh)
     assert total2 == ototal
 
@@ -157,28 +162,3 @@ def test_collectives_at_world_size_one(corpus):
     hl, nl, _ = batch.run_host()
     assert np.array_equal(nd, nl) and np.array_equal(hd["doc"], hl["doc"]) and np.array_equal(hd["score"].view(np.uint32), hl["score"].view(np.uint32))
     seg.close(); g.close(); c.close()
-
-
-@pytest.mark.parametrize("wand", [0, 2])
-def test_score_table_path_is_bit_identical(corpus, wand):
-    """SDBG_STREAM_LUT=1: scores come from the per-CTA table score[term][freq <= 8][norm byte] instead of being computed per
-    posting. The table is filled with the same arithmetic, so hits (docs, order, fp32 bits) must not change; measured 6 %
-    slower than computing on configs[2], hence opt-in -- this keeps the path covered."""
-    scorer = sdb.BM25()
-    ctx().set_wand(wand)
-    cases = [(sdb.OR, [81, 1], 100), (sdb.OR, [5, 59], 1000), (sdb.OR, [0, 1, 2], 100), (sdb.OR, [3, 40, 70, 90], 500),
-             (sdb.AND, [0, 1, 2], 50), (sdb.OR, [95], 1000)]
-    try:
-        for kind, tis, k in cases:
-            os.environ["SDBG_STREAM_LUT"] = "0"
-            a, ta = sdb.ExecuteTopK(corpus["reader"], tis, kind, scorer, k)
-            os.environ["SDBG_STREAM_LUT"] = "1"
-            b, tb = sdb.ExecuteTopK(corpus["reader"], tis, kind, scorer, k)
-            assert_hits_equal(a, b)
-            if wand == 0:
-                assert ta == tb
-            oh, _, _ = orc.bm25_topk([corpus["oseg"]], "AND" if kind == sdb.AND else "OR", oracle_terms(corpus["reader"], scorer, tis), k, mode=1)
-            assert_hits_equal(b, oh)
-    finally:
-        os.environ.pop("SDBG_STREAM_LUT", None)
-        ctx().set_wand(2)

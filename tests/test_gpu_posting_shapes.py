@@ -75,9 +75,9 @@ def test_topk_every_shape(seg, wand):
             assert total <= ototal
 
 
-@pytest.mark.parametrize("env", [{"SDBG_STREAM": "0"}, {"SDBG_STREAM_LUT": "1"}], ids=["legacy", "lut"])
+@pytest.mark.parametrize("env", [{"SDBG_STREAM": "0"}], ids=["legacy"])
 def test_topk_kernel_variants(seg, env, monkeypatch):
-    """The legacy window kernel, and the score table (used for 1-byte norms only, ignored for 2 and 4): same results."""
+    """The legacy window kernel: same results."""
     for k_, v_ in env.items():
         monkeypatch.setenv(k_, v_)
     scorer = sdb.BM25()
