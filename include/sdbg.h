@@ -207,6 +207,18 @@ int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_segs, int kind
 int sdbg_bm25_scan_excl(sdbg_segment*, int kind, const sdbg_bm25_term* terms, size_t n_terms,
                         const uint32_t* excl_terms, size_t n_excl, float k1, float b, const sdbg_col_pred* filt,
                         uint32_t doc_min, uint32_t doc_max, uint32_t* out_docs, float* out_scores, uint64_t cap, uint64_t* n_out);
+/* Count mode of the search scan (SELECT count(*) ... WHERE body @@ '...' [AND <pushed column filter>]): counts[q] = number
+ * of docs, summed over the segments, that match query q's positive part (OR / AND of terms[term_off[q] .. term_off[q+1]),
+ * 1..16 term ids), are not deleted, pass the hybrid filter (NULL never passes, as in the top-k), and occur in none of
+ * excl_terms[excl_off[q] .. excl_off[q+1]) (0..16 ids; excl_off NULL = no exclusions). Nothing is scored: no scorer
+ * parameters. Exact at every pruning level: equal to total_matches of sdbg_bm25_topk_batch(_excl) at pruning level 0, for
+ * any scorer (an excluded id a segment does not hold excludes nothing there). Errors and their codes are those of
+ * sdbg_bm25_topk_batch_excl; NULL counts: SDBG_EINVAL. Synchronous on the context's stream: counts is in host memory on
+ * return. A single-term query over a segment without filter, deleted docs or an excluded list holding blocks there is
+ * answered from the term's docs_count, without a launch. */
+int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
+                           const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms,
+                           const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

@@ -1,0 +1,243 @@
+// bm25_count.cuh -- sm_90a kernel for the Count mode of the search scan: the number of docs that match a full-text query
+// (OR / AND of 1..16 terms), minus deleted docs, minus docs that fail the pushed column predicate, minus the docs of up to
+// 16 excluded terms. Nothing is scored: the kernel reads block descriptors, doc payloads, the deleted bitmap, the filter
+// column and the excluded lists' doc payloads -- never frequencies, norms or block-max pairs.
+//
+// Mapping: one CTA per work item {query, first window, windows} of one segment. A window is kCountWindow docs aligned to
+// a multiple of kCountWindow, held as a bitmap `acc` in shared memory (bit i = doc ws + i). Because windows are aligned,
+// word i of `acc` is word ws / 32 + i of the deleted-docs bitmap.
+//   OR   warps decode every positive list's blocks that overlap the window and set their docs in `acc`.
+//   AND  the shortest list fills `acc`; each further list (ascending docs_count) decodes only the blocks whose doc range
+//        (prev_last, last_doc] holds a bit of `acc`, sets their docs in `tmp`, then acc &= tmp; the window ends early
+//        once `acc` is empty.
+//   NOT  the excluded lists' blocks whose range holds a bit of `acc` are decoded and their docs cleared.
+// Then acc &= ~deleted, the filter runs per remaining bit, and popcounts are summed: one 64-bit atomicAdd per CTA.
+// A window that no positive list reaches (OR) or that the shortest list does not reach (AND) is never touched: the CTA
+// jumps to the window of the next block's first possible doc, so a sparse query costs in proportion to its blocks.
+#pragma once
+
+#include "bm25_kernels.cuh"
+
+namespace sdbg {
+
+constexpr uint32_t kCountWindowLog = 16;
+constexpr uint32_t kCountWindow = 1u << kCountWindowLog;   // docs per window
+constexpr uint32_t kCountWords = kCountWindow / 32u;        // 2048 words: an 8 KB bitmap
+constexpr uint32_t kCountThreads = 256;
+constexpr uint32_t kCountWarps = kCountThreads / 32u;
+constexpr uint32_t kCountMaxLists = 2u * kMaxQueryTerms;   // positive + excluded lists of one query
+
+struct CountParams {
+  PostingsDev seg;              // arena, blocks, deleted, n_docs
+  FilterDev filt;
+  // Per query q of this segment: positive lists lists[term_off[q] .. term_off[q + 1]) as {first BlockDesc, blocks},
+  // ascending by docs_count; excluded lists lists[n_pos + excl_off[q] .. n_pos + excl_off[q + 1]) (0 blocks: a term the
+  // segment does not hold). excl_off null: no exclusions.
+  const uint2* lists;
+  const uint32_t* term_off;
+  const uint32_t* excl_off;
+  uint32_t n_pos;               // term_off[n_queries]
+  const uint4* work;            // {query, first window, windows, 0}
+  unsigned long long* counts;   // per query, summed over items and segments
+};
+
+__device__ __forceinline__ uint32_t warp_min(uint32_t v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_xor_sync(kFull, v, o));
+  return v;
+}
+
+// Sets (clear = false) or clears (clear = true) the bits of block `d`'s docs that fall in the window [ws, ws + W) of
+// `bm`. Whole warp. Bitset blocks are merged word by word without expanding them; the other encodings are decoded.
+// Returns the block's first doc past the window (0xFFFFFFFF: none), where the next window of a straddling block starts.
+__device__ __forceinline__ uint32_t block_to_bitmap(const uint4* arena, const uint4& d, uint32_t lane, uint32_t* stage,
+                                                    uint32_t ws, uint32_t* bm, bool clear) {
+  const long long wend = static_cast<long long>(ws) + kCountWindow;
+  uint32_t beyond = 0xFFFFFFFFu;
+  if (desc_doc_enc(d.w) == 4u) {   // de_for_bitset: bit j of the payload <=> doc prev + j
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(arena + d.x);
+    const uint32_t chunks = 2u * desc_words(d.w);
+    for (uint32_t c = lane; c < chunks; c += 32u) {
+      const uint32_t v = __ldg(w + c);
+      const long long r = static_cast<long long>(d.z) + 32ll * c - static_cast<long long>(ws);   // bit 0 of v, window-relative
+      if (v == 0u || r <= -32) continue;
+      if (r + 31 >= static_cast<long long>(kCountWindow)) {                                      // bits past the window
+        const uint32_t past = r >= static_cast<long long>(kCountWindow) ? v : v & (0xFFFFFFFFu << uint32_t(kCountWindow - r));
+        if (past) beyond = min(beyond, uint32_t(wend - static_cast<long long>(kCountWindow) + r) + uint32_t(__ffs(past) - 1));
+        if (r >= static_cast<long long>(kCountWindow)) continue;
+      }
+      const uint32_t sh = static_cast<uint32_t>(r & 31);
+      const long long wi = r >> 5;                                                               // floor
+      const uint32_t lo = v << sh, hi = sh ? v >> (32u - sh) : 0u;
+      if (wi >= 0 && lo) { if (clear) atomicAnd(&bm[wi], ~lo); else atomicOr(&bm[wi], lo); }
+      if (wi + 1 < static_cast<long long>(kCountWords) && hi) { if (clear) atomicAnd(&bm[wi + 1], ~hi); else atomicOr(&bm[wi + 1], hi); }
+    }
+    return warp_min(beyond);
+  }
+  uint32_t doc[4];
+  decode_docs(arena, d, lane, stage, doc);
+  const uint32_t len = desc_len(d.w);
+  uint32_t word = 0xFFFFFFFFu, bits = 0u;   // a lane's four docs ascend: one atomic per distinct word
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (4u * lane + j >= len) continue;
+    const uint32_t rel = doc[j] - ws;
+    if (rel >= kCountWindow) {
+      if (static_cast<long long>(doc[j]) >= wend) beyond = min(beyond, doc[j]);
+      continue;
+    }
+    if ((rel >> 5) != word) {
+      if (bits) { if (clear) atomicAnd(&bm[word], ~bits); else atomicOr(&bm[word], bits); }
+      word = rel >> 5; bits = 0u;
+    }
+    bits |= 1u << (rel & 31u);
+  }
+  if (bits) { if (clear) atomicAnd(&bm[word], ~bits); else atomicOr(&bm[word], bits); }
+  return warp_min(beyond);
+}
+
+// Does `bm` hold a bit for a doc in (prev_last, last_doc] within the window [ws, wlast]? Whole warp.
+__device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& d, uint32_t ws, uint32_t wlast, uint32_t lane) {
+  const uint32_t a = max(d.z + 1u, ws) - ws, b = min(d.y, wlast) - ws;   // d.z < wlast, d.y >= ws: a <= b
+  const uint32_t wa = a >> 5, wb = b >> 5;
+  uint32_t any = 0u;
+  for (uint32_t i = wa + lane; i <= wb; i += 32u) {
+    uint32_t v = bm[i];
+    if (i == wa) v &= 0xFFFFFFFFu << (a & 31u);
+    if (i == wb) v &= 0xFFFFFFFFu >> (31u - (b & 31u));
+    any |= v;
+  }
+  return __any_sync(kFull, any != 0u);
+}
+
+// kAnd: conjunction (else disjunction). The term loops are not unrolled: 1..16 terms share one instantiation.
+template <bool kAnd>
+__global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
+  __shared__ uint32_t acc[kCountWords];
+  __shared__ uint32_t tmp[kAnd ? kCountWords : 1];
+  __shared__ uint32_t stage[kCountWarps][128];
+  // per list: blocks [s_cur, s_end) overlap the current window; s_next = first block that reaches past it
+  __shared__ uint32_t s_cur[kCountMaxLists], s_end[kCountMaxLists], s_next[kCountMaxLists];
+  // per lead list: first doc of block s_next past the window, when that block straddled it and was decoded (else 0)
+  __shared__ uint32_t s_resume[kCountMaxLists];
+  __shared__ uint2 s_list[kCountMaxLists];
+  __shared__ uint32_t s_ws, s_done;
+  __shared__ unsigned long long s_sum[kCountWarps];
+
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  const uint4 item = P.work[blockIdx.x];
+  const uint32_t q = item.x, w_end = item.y + item.z;   // windows [item.y, w_end)
+  const uint32_t n_pos = P.term_off[q + 1] - P.term_off[q];
+  const uint32_t n_excl = P.excl_off ? P.excl_off[q + 1] - P.excl_off[q] : 0u;
+  const uint32_t n_lists = n_pos + n_excl;
+  const uint32_t n_lead = kAnd ? 1u : n_pos;            // lists that decide which windows hold matches
+  const uint4* const B = P.seg.blocks;
+  const uint32_t del_words = (P.seg.n_docs + 32u) / 32u + 1u;
+
+  if (tid < n_lists) {
+    const uint2 l = tid < n_pos ? P.lists[P.term_off[q] + tid] : P.lists[P.n_pos + P.excl_off[q] + (tid - n_pos)];
+    s_list[tid] = l;
+    s_resume[tid] = 0u;
+    // first block whose last doc reaches the item's first window
+    s_next[tid] = l.y ? find_block_from(B + l.x, 0u, l.y, 0u, item.y << kCountWindowLog) : 0u;
+  }
+  unsigned long long count = 0;
+  uint32_t ws = item.y << kCountWindowLog;              // start of the window being looked at
+  __syncthreads();
+  for (;;) {
+    // ---- next window: the first possible doc of the lead lists' current blocks ----
+    if (tid == 0) {
+      uint32_t nxt = 0xFFFFFFFFu;
+      bool any = false;
+      for (uint32_t i = 0; i < n_lead; ++i) {
+        const uint2 l = s_list[i];
+        if (s_next[i] >= l.y) continue;
+        const uint4 d = __ldg(B + l.x + s_next[i]);
+        nxt = min(nxt, max(max(d.z + 1u, ws), s_resume[i]));
+        any = true;
+      }
+      s_done = (!any || (nxt >> kCountWindowLog) >= w_end) ? 1u : 0u;
+      s_ws = (nxt >> kCountWindowLog) << kCountWindowLog;
+    }
+    __syncthreads();
+    if (s_done) break;
+    ws = s_ws;
+    const uint32_t wlast = ws + (kCountWindow - 1u);
+    if (tid < n_lists) {
+      const uint2 l = s_list[tid];
+      const uint4* LB = B + l.x;
+      uint32_t c = s_next[tid], e = l.y;
+      if (c < l.y) c = find_block_from(LB, c, l.y, c, ws);
+      if (c < l.y && wlast != 0xFFFFFFFFu) e = find_block_from(LB, c, l.y, c, wlast + 1u);
+      s_cur[tid] = c;
+      s_next[tid] = e;
+      s_resume[tid] = 0u;
+      s_end[tid] = (e < l.y && __ldg(&LB[e].z) < wlast) ? e + 1u : e;   // block e straddles the window's end
+    }
+    for (uint32_t i = tid; i < kCountWords; i += kCountThreads) acc[i] = 0u;
+    __syncthreads();
+
+    // Blocks [s_cur, s_end) of lists [lo, hi) spread over the warps; `filter`: only blocks whose range holds a bit of acc.
+    auto run_lists = [&](uint32_t lo, uint32_t hi, uint32_t* bm, bool clear, bool filter) {
+      const uint32_t li = lo + lane;
+      const uint32_t n = li < hi ? s_end[li] - s_cur[li] : 0u;
+      const uint32_t incl = warp_incl_scan(n, lane);
+      const uint32_t total = __shfl_sync(kFull, incl, 31);
+      for (uint32_t it = warp; it < total; it += kCountWarps) {
+        const uint32_t src = __ffs(__ballot_sync(kFull, incl > it)) - 1u;
+        const uint32_t before = __shfl_sync(kFull, incl - n, src);
+        const uint32_t li2 = lo + src, blk = s_cur[li2] + (it - before);
+        const uint4 d = __ldg(B + s_list[li2].x + blk);
+        if (filter && !range_has_bits(acc, d, ws, wlast, lane)) continue;
+        const uint32_t beyond = block_to_bitmap(P.seg.arena, d, lane, stage[warp], ws, bm, clear);
+        if (lane == 0 && blk == s_next[li2]) s_resume[li2] = beyond;   // the block that straddles the window's end
+      }
+    };
+
+    run_lists(0u, n_lead, acc, false, false);
+    __syncthreads();
+    bool live = true;
+    if constexpr (kAnd) {
+      for (uint32_t t = 1; t < n_pos; ++t) {
+        for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
+        __syncthreads();
+        run_lists(t, t + 1u, tmp, false, true);
+        __syncthreads();
+        uint32_t nz = 0u;
+        for (uint32_t i = tid; i < kCountWords; i += kCountThreads) { const uint32_t v = acc[i] & tmp[i]; acc[i] = v; nz |= v; }
+        if (!__syncthreads_or(nz != 0u)) { live = false; break; }
+      }
+    }
+    if (live && n_excl) {
+      run_lists(n_pos, n_lists, acc, true, true);
+      __syncthreads();
+    }
+    if (live) {
+      const uint32_t wbase = ws >> 5;
+      for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
+        uint32_t v = acc[i];
+        if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
+        if (v && P.filt.values) {
+          for (uint32_t r = v; r; r &= r - 1u) {
+            const uint32_t bit = __ffs(r) - 1u;
+            if (!filter_pass(P.filt, ws + 32u * i + bit)) v &= ~(1u << bit);
+          }
+        }
+        count += __popc(v);
+      }
+    }
+    __syncthreads();   // acc / tmp / cursors are rewritten by the next window
+    if (wlast == 0xFFFFFFFFu || (wlast >> kCountWindowLog) + 1u >= w_end) break;
+    ws = wlast + 1u;
+  }
+  count = warp_sum64(count);
+  if (lane == 0) s_sum[warp] = count;
+  __syncthreads();
+  if (tid == 0) {
+    unsigned long long s = 0;
+    for (uint32_t w = 0; w < kCountWarps; ++w) s += s_sum[w];
+    if (s) atomicAdd(P.counts + q, s);
+  }
+}
+
+}  // namespace sdbg

@@ -25,6 +25,7 @@
 #include "bm25_kernels.cuh"
 #include "bm25_stream.cuh"
 #include "bm25_merge.cuh"
+#include "bm25_count.cuh"
 #include "column_kernels.cuh"
 #include "posting_format.hpp"
 
@@ -809,6 +810,44 @@ struct TopkPlan {
 // Device-side result of a batch: keys_out[Q][k] (sorted desc, 0 = empty), n_out[Q], total[Q].
 struct TopkDevOut { unsigned long long* keys; uint32_t* n_out; unsigned long long* total; };
 
+uint32_t term_id(const sdbg_bm25_term& t) { return t.term; }
+uint32_t term_id(uint32_t t) { return t; }
+
+// Checks of a query batch shared by the top-k and count entries: 1..16 positive terms and at most 16 excluded ones per
+// query, a non-decreasing excl_off, segments of one context with staged postings, positive term ids every segment
+// holds, and a staged filter column. Sets *total_excl to excl_off[nq] when some query excludes terms, else 0.
+template <class Term>
+int check_query_batch(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* term_off, size_t nq,
+                      const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint32_t* total_excl) {
+  sdbg_ctx* c = segs[0]->ctx;
+  for (size_t q = 0; q < nq; ++q) {
+    const uint32_t nt = term_off[q + 1] - term_off[q];
+    if (nt == 0 || nt > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 terms");
+  }
+  *total_excl = 0;
+  if (excl_off) {
+    for (size_t q = 0; q < nq; ++q) {
+      if (excl_off[q + 1] < excl_off[q]) return fail(c, SDBG_EINVAL, "excl_off must be non-decreasing");
+      if (excl_off[q + 1] - excl_off[q] > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
+    }
+    if (excl_off[nq] > excl_off[0]) {
+      if (!excl_terms) return fail(c, SDBG_EINVAL, "excl_terms is NULL");
+      *total_excl = excl_off[nq];
+    }
+  }
+  for (size_t si = 0; si < n_segs; ++si) {
+    if (segs[si]->ctx != c) return fail(c, SDBG_EINVAL, "segments of one call must share a context");
+    if (!segs[si]->d_blocks) return fail(c, SDBG_EINVAL, "segment has no staged postings");
+  }
+  for (size_t si = 0; si < n_segs; ++si)
+    for (uint32_t i = term_off[0]; i < term_off[nq]; ++i)
+      if (size_t(term_id(terms[i])) + 1 >= segs[si]->term_blk_begin.size()) return fail(c, SDBG_EINVAL, "term id out of range");
+  FilterDev fv;
+  for (size_t si = 0; si < n_segs; ++si)
+    if (int rc = filter_view(segs[si], filt, &fv)) return rc;
+  return SDBG_OK;
+}
+
 // excl_terms / excl_off: query q excludes the term ids excl_terms[excl_off[q] .. excl_off[q + 1]) (NULL excl_off: none).
 int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
              size_t nq, float k1, const float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, TopkDevOut* dev,
@@ -819,26 +858,11 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   if (nq > 65535) return fail(c, SDBG_EUNSUPPORTED, "more than 65535 queries per batch");
   CU(c, cudaSetDevice(c->device));
   const uint32_t total_terms = term_off[nq];
-  for (size_t q = 0; q < nq; ++q) {
-    const uint32_t nt = term_off[q + 1] - term_off[q];
-    if (nt == 0 || nt > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 terms");
-  }
   uint32_t total_excl = 0;   // > 0: some query excludes terms
-  if (excl_off) {
-    for (size_t q = 0; q < nq; ++q) {
-      if (excl_off[q + 1] < excl_off[q]) return fail(c, SDBG_EINVAL, "excl_off must be non-decreasing");
-      if (excl_off[q + 1] - excl_off[q] > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
-    }
-    if (excl_off[nq] > excl_off[0]) {
-      if (!excl_terms) return fail(c, SDBG_EINVAL, "excl_terms is NULL");
-      total_excl = excl_off[nq];
-    }
-  }
+  if (int rc = check_query_batch(segs, n_segs, terms, term_off, nq, excl_terms, excl_off, filt, &total_excl)) return rc;
   uint64_t ord = 0;
   uint32_t max_docs = 0;
   for (size_t si = 0; si < n_segs; ++si) {
-    if (segs[si]->ctx != c) return fail(c, SDBG_EINVAL, "segments of one call must share a context");
-    if (!segs[si]->d_blocks) return fail(c, SDBG_EINVAL, "segment has no staged postings");
     ord += segs[si]->n_docs;
     max_docs = std::max(max_docs, segs[si]->n_docs);
   }
@@ -999,9 +1023,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
     for (size_t q = 0; q < nq; ++q) {
       const uint32_t t_begin = term_off[q], t_end = term_off[q + 1];
       for (uint32_t i = t_begin; i < t_end; ++i) {
-        const sdbg_bm25_term& t = terms[i];
-        if (t.term + 1 >= s->term_blk_begin.size()) return fail(c, SDBG_EINVAL, "term id out of range");
-        fill_qterm(s, t, k1, b, dst[i]);
+        fill_qterm(s, terms[i], k1, b, dst[i]);
       }
       std::stable_sort(dst + t_begin, dst + t_end, [](const QTermDev& x, const QTermDev& y) { return x.docs_count < y.docs_count; });
     }
@@ -1282,6 +1304,112 @@ extern "C" int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_seg
   if (!excl_off) return SDBG_EINVAL;
   return topk_batch_host(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, k1, b, filt, k, threshold_in, out, n_out,
                          total_matches);
+}
+
+// Count mode (duckdb_search_full_scan RunCountScan): bm25_count_kernel over work items {query, first window, windows} of
+// kCountWindow-doc windows, planned per segment from posting counts and issued largest first. A single-term query over a
+// segment without filter, deleted docs or an excluded list holding blocks there is answered from the term's docs_count.
+extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
+                                      const uint32_t* term_off, size_t nq, const uint32_t* excl_terms,
+                                      const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
+  if (!segs || !n_segs || !terms || !term_off || !nq || !counts) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  CU(c, cudaSetDevice(c->device));
+  uint32_t total_excl = 0;
+  if (int rc = check_query_batch(segs, n_segs, terms, term_off, nq, excl_terms, excl_off, filt, &total_excl)) return rc;
+  const bool conj = kind == SDBG_QUERY_AND;
+  const uint32_t n_pos = term_off[nq];
+  const size_t n_lists = size_t(n_pos) + total_excl;   // per segment: positive lists | excluded lists
+
+  std::vector<uint64_t> host(nq, 0);                    // shortcut counts
+  struct Item { uint32_t q, w0, nw; uint64_t weight; };
+  std::vector<std::vector<Item>> seg_work(n_segs);
+  std::vector<uint2> lists(n_lists * n_segs);
+  uint64_t batch_postings = 0;
+  for (size_t si = 0; si < n_segs; ++si)
+    for (uint32_t i = term_off[0]; i < n_pos; ++i) batch_postings += segs[si]->term_docs[terms[i]];
+  const uint64_t chain_target = std::max<uint64_t>(65536, batch_postings / (uint64_t(c->sm_count) * 4u));
+  const uint32_t G = uint32_t(std::max<size_t>(1, (size_t(c->sm_count) * 8u + nq - 1) / nq));
+  size_t total_items = 0;
+  for (size_t si = 0; si < n_segs; ++si) {
+    const sdbg_segment* s = segs[si];
+    uint2* L = lists.data() + si * n_lists;
+    for (uint32_t i = 0; i < total_excl; ++i) L[n_pos + i] = excl_list(s, excl_terms[i]);
+    const uint32_t n_win = (s->n_docs >> kCountWindowLog) + 1u;
+    for (size_t q = 0; q < nq; ++q) {
+      const uint32_t t0 = term_off[q], t1 = term_off[q + 1];
+      uint64_t sum = 0;
+      uint32_t smallest = UINT32_MAX;
+      std::array<std::pair<uint32_t, uint2>, kMaxQueryTerms> by_docs;
+      for (uint32_t i = t0; i < t1; ++i) {
+        const uint32_t dc = s->term_docs[terms[i]];
+        by_docs[i - t0] = {dc, excl_list(s, terms[i])};
+        sum += dc;
+        smallest = std::min(smallest, dc);
+      }
+      // ascending docs_count: the shortest list of a conjunction fills the window bitmap
+      std::stable_sort(by_docs.begin(), by_docs.begin() + (t1 - t0), [](const auto& a, const auto& b) { return a.first < b.first; });
+      for (uint32_t i = t0; i < t1; ++i) L[i] = by_docs[i - t0].second;
+      if (conj ? smallest == 0 : sum == 0) continue;
+      bool excl_blocks = false;
+      if (total_excl)
+        for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) excl_blocks |= L[n_pos + i].y != 0;
+      if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks) { host[q] += sum; continue; }
+      const uint64_t weight = conj ? uint64_t(smallest) * (t1 - t0) : sum;
+      uint32_t g = uint32_t(std::max<uint64_t>(G, (weight + chain_target - 1) / chain_target));
+      g = std::min({g, n_win, 2u * uint32_t(c->sm_count)});
+      const uint32_t per = (n_win + g - 1) / g;
+      for (uint32_t w0 = 0; w0 < n_win; w0 += per)
+        seg_work[si].push_back({uint32_t(q), w0, std::min(per, n_win - w0), weight / g});
+    }
+    std::stable_sort(seg_work[si].begin(), seg_work[si].end(), [](const Item& x, const Item& y) { return x.weight > y.weight; });
+    total_items += seg_work[si].size();
+  }
+  if (total_items) {
+    // [term_off | excl_off | lists per segment | work items]
+    const size_t off_bytes = (nq + 1) * 4;
+    const size_t lists_pos = (2 * off_bytes + 7) & ~size_t(7);
+    const size_t work_pos = (lists_pos + lists.size() * sizeof(uint2) + 15) & ~size_t(15);
+    const size_t bytes = work_pos + total_items * sizeof(uint4);
+    int rc = ensure_pinned(c, std::max(bytes, nq * 8));
+    if (rc) return rc;
+    char* h = static_cast<char*>(c->h_pinned);
+    std::memcpy(h, term_off, off_bytes);
+    if (total_excl) std::memcpy(h + off_bytes, excl_off, off_bytes);
+    std::memcpy(h + lists_pos, lists.data(), lists.size() * sizeof(uint2));
+    auto* hw = reinterpret_cast<uint4*>(h + work_pos);
+    for (auto& w : seg_work) for (const Item& it : w) *hw++ = make_uint4(it.q, it.w0, it.nw, 0u);
+    DevBuf& b_desc = c->scratch[0]; DevBuf& b_counts = c->scratch[1];
+    if ((rc = ensure(c, b_desc, bytes))) return rc;
+    if ((rc = ensure(c, b_counts, nq * 8))) return rc;
+    CU(c, cudaMemcpyAsync(b_desc.p, h, bytes, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemsetAsync(b_counts.p, 0, nq * 8, c->stream));
+    const char* d = static_cast<const char*>(b_desc.p);
+    size_t done = 0;
+    for (size_t si = 0; si < n_segs; ++si) {
+      if (seg_work[si].empty()) continue;
+      CountParams P;
+      P.seg = postings_view(segs[si], 0);
+      if ((rc = filter_view(segs[si], filt, &P.filt))) return rc;
+      P.lists = reinterpret_cast<const uint2*>(d + lists_pos) + si * n_lists;
+      P.term_off = reinterpret_cast<const uint32_t*>(d);
+      P.excl_off = total_excl ? reinterpret_cast<const uint32_t*>(d + off_bytes) : nullptr;
+      P.n_pos = n_pos;
+      P.work = reinterpret_cast<const uint4*>(d + work_pos) + done;
+      P.counts = static_cast<unsigned long long*>(b_counts.p);
+      done += seg_work[si].size();
+      if (conj) bm25_count_kernel<true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
+      else bm25_count_kernel<false><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
+      ++c->launches;
+    }
+    CU(c, cudaGetLastError());
+    CU(c, cudaMemcpyAsync(h, b_counts.p, nq * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    const auto* dc = reinterpret_cast<const unsigned long long*>(h);
+    for (size_t q = 0; q < nq; ++q) host[q] += dc[q];
+  }
+  std::memcpy(counts, host.data(), nq * 8);
+  return SDBG_OK;
 }
 
 // Streaming mode (duckdb_search_full_scan.cpp RunStreamingScan :2370-2403; DocIterator::EmitScoredDocs,

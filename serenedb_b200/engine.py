@@ -442,6 +442,30 @@ def ExecuteTopKBatch(reader, queries, kind, scorer, k, filt=None, threshold=FLT_
     return hits, n_out, total
 
 
+def ExecuteCountBatch(reader, queries, kind, filt=None, exclude=None):
+    """Count mode of the search scan (`SELECT count(*) ... WHERE body @@ '...'`, sdbg_match_count_batch): per query, the
+    number of docs over all segments that match its term ids (OR / AND), are not deleted, pass `filt` and hold none of its
+    `exclude` term ids. Nothing is scored, so no statistics are needed; exact at every pruning level. Returns uint64[Q]."""
+    nq = len(queries)
+    flat = np.ascontiguousarray([t for q in queries for t in q], dtype=np.uint32)
+    off = np.zeros(nq + 1, np.uint32)
+    off[1:] = np.cumsum([len(q) for q in queries])
+    counts = np.zeros(nq, np.uint64)
+    x = _exclusions(exclude, nq)
+    fp = C.byref(filt) if filt is not None else None
+    N.check(N.lib().sdbg_match_count_batch(_seg_array(reader.segments), len(reader.segments), int(kind),
+                                           _ptr(flat) if len(flat) else None, _ptr(off), nq,
+                                           _ptr(x[0]) if x is not None else None, _ptr(x[1]) if x is not None else None, fp,
+                                           _ptr(counts)), reader.segments[0].ctx._h)
+    return counts
+
+
+def ExecuteCount(reader, query_terms, kind, filt=None, exclude=None):
+    """ExecuteCountBatch for one query: its match count as an int."""
+    return int(ExecuteCountBatch(reader, [list(query_terms)], kind, filt,
+                                 exclude=None if exclude is None else [list(exclude)])[0])
+
+
 FOR_BLOCK_DTYPE = np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])
 
 

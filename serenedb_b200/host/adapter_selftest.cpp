@@ -1,7 +1,8 @@
 // adapter_selftest.cpp -- drives the two adapters the way the reference's callers would
 // (ExecuteTopK's collector loop, IResearchScanFunction's chunk loop) and prints results as JSON lines
 // for tests/test_gpu_adapters.py to compare with the oracle. Needs a GPU at run time. With a second argument "excl" it runs
-// only the exclusion case instead (an And with a Not child, tests/test_gpu_exclusion.py).
+// only the exclusion case instead (an And with a Not child, tests/test_gpu_exclusion.py); with "count", only the Count
+// scan mode (GpuCountScan, tests/test_gpu_count.py).
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -60,6 +61,25 @@ int main(int argc, char** argv) {
       std::printf(", \"stream_n\": %llu, \"stream_doc_sum\": %llu, \"stream_score_sum\": %.12g}\n", static_cast<unsigned long long>(n),
                   static_cast<unsigned long long>(doc_sum), score_sum);
     }
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
+  if (argc > 2 && std::string(argv[2]) == "count") {
+    // count(*) of `t2 | t5`, `t2 & t5` and `(t2 | t5) & !t3`, without and with the table filter: one row, then end of scan
+    for (int with_filter = 0; with_filter < 2; ++with_filter)
+      for (int kind : {int(SDBG_QUERY_OR), int(SDBG_QUERY_AND)})
+        for (int excl = 0; excl < 2; ++excl) {
+          sdbg_host::GpuCountScan scan({seg}, kind, {2, 5}, excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{},
+                                       with_filter ? &filt : nullptr);
+          duckdb::DataChunkMock chunk;
+          scan.Scan(chunk);
+          const uint64_t rows = chunk.size;
+          const long long count = rows ? chunk.count[0] : -1;
+          scan.Scan(chunk);
+          std::printf("{\"filter\": %d, \"kind\": %d, \"excl\": %d, \"rows\": %llu, \"count\": %lld, \"rows_after\": %llu}\n", with_filter,
+                      kind, excl, static_cast<unsigned long long>(rows), count, static_cast<unsigned long long>(chunk.size));
+        }
     sdbg_segment_destroy(seg);
     sdbg_destroy(ctx);
     return 0;

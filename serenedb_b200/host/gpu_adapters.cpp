@@ -172,6 +172,27 @@ void GpuAggScan::Scan(duckdb::DataChunkMock& output) {
   cursor_ += take;
 }
 
+GpuCountScan::GpuCountScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
+                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter)
+    : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
+      has_filter_(table_filter != nullptr) {
+  if (table_filter) filter_ = *table_filter;
+}
+
+void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
+  output.Reset();
+  if (done_) return;                                          // cardinality 0: the count has been emitted
+  const uint32_t term_off[2] = {0, uint32_t(terms_.size())};
+  const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
+  uint64_t n = 0;
+  const int rc = sdbg_match_count_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
+                                        has_filter_ ? &filter_ : nullptr, &n);
+  if (rc != SDBG_OK) throw GpuError(rc, std::string("sdbg_match_count_batch: ") + sdbg_last_error(sdbg_segment_context(segs_[0])));
+  output.count.push_back(int64_t(n));
+  output.size = 1;
+  done_ = true;
+}
+
 GpuAggGlobalState::GpuAggGlobalState(std::vector<sdbg_segment*> segments, std::vector<sdbg_col_pred> pushed_filters, uint64_t key_field,
                                      uint64_t sum_int_field, uint64_t avg_f64_field, uint32_t n_groups_hint)
     : segs(std::move(segments)), preds(std::move(pushed_filters)), key(key_field), sum_i(sum_int_field), avg_f(avg_f64_field),

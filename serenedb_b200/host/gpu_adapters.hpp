@@ -104,6 +104,25 @@ class GpuAggScan {
   uint64_t rows_scanned_ = 0;
 };
 
+// SELECT count(*) FROM t WHERE body @@ '<query>' [AND <pushed filter>] -- the body of ScanMode::Count
+// (duckdb_search_full_scan.cpp RunCountScan :2201-2239) for a text query: one row with the count, then cardinality 0.
+// Nothing is scored (sdbg_match_count_batch); the count is exact whatever the pruning level.
+class GpuCountScan {
+ public:
+  GpuCountScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
+               std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */);
+  // Fills `output` with one row, count[0] = the number of matches; the next call leaves it empty (end of scan).
+  void Scan(duckdb::DataChunkMock& output);
+
+ private:
+  std::vector<sdbg_segment*> segs_;
+  int kind_;
+  std::vector<uint32_t> terms_, excluded_;
+  bool has_filter_;
+  sdbg_col_pred filter_{};
+  bool done_ = false;
+};
+
 // The same scan mode under DuckDB's threading contract (duckdb_search_full_scan.hpp:85-255, .cpp:99-268): ONE global
 // state shared by all workers of the query -- touched through atomics only, like next_segment / next_unit there -- and
 // one local state per worker. The first worker to arrive runs the aggregation on the GPU (the others wait on the
