@@ -219,6 +219,33 @@ int sdbg_bm25_scan_excl(sdbg_segment*, int kind, const sdbg_bm25_term* terms, si
 int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
                            const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms,
                            const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts);
+/* Conjunctions of OR groups (`a & (b | c) & !d`: an And whose children are terms, Ors of terms and Nots of terms, as
+ * synonym expansion and query rewriting produce). Query q is the AND of the groups [query_group_off[q],
+ * query_group_off[q+1]) (1..16), group g the OR of terms[group_off[g] .. group_off[g+1]) (non-empty); its positive terms
+ * number 1..16 in all and are distinct. It excludes excl_terms[excl_off[q] .. excl_off[q+1]) as sdbg_bm25_topk_batch_excl
+ * does (excl_off NULL: none). A doc matches when every group has a term whose list holds it, no excluded list holds it,
+ * it is not deleted and it passes the hybrid filter (NULL never passes). A group whose lists are all empty in a segment
+ * matches nothing there.
+ * Scores: a hit's score is bit for bit the score the flat OR of the query's positive terms gives that doc (same scorer and
+ * statistics): the sum of its matching terms' scores in ascending docs_count order. BM25, BM15 (b = 0), BM1 (k1 = 0) and
+ * TFIDF (k1 = -1) as in the other batch entries; block-max pruning only for BM25 with the index-time b. total_matches is
+ * exact with pruning off and a lower bound with it; counts are exact at every pruning level and equal the level-0 totals.
+ * Degenerate queries take the existing paths and give exactly their results: a query of one group runs as
+ * sdbg_bm25_topk_batch_excl / sdbg_match_count_batch with kind OR, a query whose groups are all single terms as kind AND.
+ * Errors: an empty group, a decreasing offset array, a positive term id twice in a query, or NULL arrays with non-empty
+ * ranges: SDBG_EINVAL; more than 16 groups, positive terms or excluded terms in a query: SDBG_EUNSUPPORTED; otherwise the
+ * errors of sdbg_bm25_topk_batch_excl / sdbg_match_count_batch.
+ * Not supported yet: the streaming scan (sdbg_bm25_scan*), grouped forms of sdbg_bm25_topk_batch_device and
+ * sdbg_dist_bm25_topk_batch, deeper nesting (an OR of ANDs), more than 16 positive terms, phrases. */
+int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                const uint32_t* group_off, const uint32_t* query_group_off, size_t n_queries,
+                                const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in,
+                                sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches);
+int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                  const uint32_t* group_off, const uint32_t* query_group_off, size_t n_queries,
+                                  const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                  uint64_t* counts);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

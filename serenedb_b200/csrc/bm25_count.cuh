@@ -10,9 +10,13 @@
 //   AND  the shortest list fills `acc`; each further list (ascending docs_count) decodes only the blocks whose doc range
 //        (prev_last, last_doc] holds a bit of `acc`, sets their docs in `tmp`, then acc &= tmp; the window ends early
 //        once `acc` is empty.
+//   GROUPS  an AND of OR groups (kGroups): the lead group (smallest summed docs_count) fills `acc` like an OR; each further
+//        group ORs into `tmp` the docs of its lists' blocks whose range holds a bit of `acc`, then acc &= tmp, with the
+//        same early end.
 //   NOT  the excluded lists' blocks whose range holds a bit of `acc` are decoded and their docs cleared.
 // Then acc &= ~deleted, the filter runs per remaining bit, and popcounts are summed: one 64-bit atomicAdd per CTA.
-// A window that no positive list reaches (OR) or that the shortest list does not reach (AND) is never touched: the CTA
+// A window that no positive list reaches (OR), that the shortest list does not reach (AND) or that no list of the lead
+// group reaches (GROUPS) is never touched: the CTA
 // jumps to the window of the next block's first possible doc, so a sparse query costs in proportion to its blocks.
 #pragma once
 
@@ -36,6 +40,10 @@ struct CountParams {
   const uint2* lists;
   const uint32_t* term_off;
   const uint32_t* excl_off;
+  // kGroups: query q's positive lists form consecutive OR groups, lead group first; group g of q ends (exclusive, relative
+  // to term_off[q]) at grp_end[grp_off[q] + g]. Per segment, since the lead group and the list order depend on it.
+  const uint32_t* grp_end = nullptr;
+  const uint32_t* grp_off = nullptr;
   uint32_t n_pos;               // term_off[n_queries]
   const uint4* work;            // {query, first window, windows, 0}
   unsigned long long* counts;   // per query, summed over items and segments
@@ -110,17 +118,20 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
   return __any_sync(kFull, any != 0u);
 }
 
-// kAnd: conjunction (else disjunction). The term loops are not unrolled: 1..16 terms share one instantiation.
-template <bool kAnd>
+// kAnd: conjunction (else disjunction). kGroups: conjunction of OR groups (CountParams::grp_end). The term loops are not
+// unrolled: 1..16 terms share one instantiation.
+template <bool kAnd, bool kGroups = false>
 __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
+  static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
   __shared__ uint32_t acc[kCountWords];
-  __shared__ uint32_t tmp[kAnd ? kCountWords : 1];
+  __shared__ uint32_t tmp[kAnd || kGroups ? kCountWords : 1];
   __shared__ uint32_t stage[kCountWarps][128];
   // per list: blocks [s_cur, s_end) overlap the current window; s_next = first block that reaches past it
   __shared__ uint32_t s_cur[kCountMaxLists], s_end[kCountMaxLists], s_next[kCountMaxLists];
   // per lead list: first doc of block s_next past the window, when that block straddled it and was decoded (else 0)
   __shared__ uint32_t s_resume[kCountMaxLists];
   __shared__ uint2 s_list[kCountMaxLists];
+  __shared__ uint32_t s_gend[kGroups ? kMaxQueryTerms : 1];
   __shared__ uint32_t s_ws, s_done;
   __shared__ unsigned long long s_sum[kCountWarps];
 
@@ -130,7 +141,9 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   const uint32_t n_pos = P.term_off[q + 1] - P.term_off[q];
   const uint32_t n_excl = P.excl_off ? P.excl_off[q + 1] - P.excl_off[q] : 0u;
   const uint32_t n_lists = n_pos + n_excl;
-  const uint32_t n_lead = kAnd ? 1u : n_pos;            // lists that decide which windows hold matches
+  const uint32_t n_groups = kGroups ? P.grp_off[q + 1] - P.grp_off[q] : 0u;
+  if (kGroups && tid < n_groups) s_gend[tid] = P.grp_end[P.grp_off[q] + tid];
+  const uint32_t n_lead = kGroups ? P.grp_end[P.grp_off[q]] : kAnd ? 1u : n_pos;   // lists that decide which windows hold matches
   const uint4* const B = P.seg.blocks;
   const uint32_t del_words = (P.seg.n_docs + 32u) / 32u + 1u;
 
@@ -202,6 +215,17 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
         for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
         __syncthreads();
         run_lists(t, t + 1u, tmp, false, true);
+        __syncthreads();
+        uint32_t nz = 0u;
+        for (uint32_t i = tid; i < kCountWords; i += kCountThreads) { const uint32_t v = acc[i] & tmp[i]; acc[i] = v; nz |= v; }
+        if (!__syncthreads_or(nz != 0u)) { live = false; break; }
+      }
+    }
+    if constexpr (kGroups) {
+      for (uint32_t g = 1; g < n_groups; ++g) {
+        for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
+        __syncthreads();
+        run_lists(s_gend[g - 1], s_gend[g], tmp, false, true);
         __syncthreads();
         uint32_t nz = 0u;
         for (uint32_t i = tid; i < kCountWords; i += kCountThreads) { const uint32_t v = acc[i] & tmp[i]; acc[i] = v; nz |= v; }

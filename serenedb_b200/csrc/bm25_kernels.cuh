@@ -58,6 +58,9 @@ struct QTermDev {  // one term of one query over one segment, 40 bytes
 };
 
 constexpr uint32_t kMaxQueryTerms = 16;
+// Per-doc list checks of a query (TopkParams::excl): up to 16 excluded lists plus up to 16 lists of required OR groups.
+constexpr uint32_t kMaxCheckLists = 2u * kMaxQueryTerms;
+constexpr uint8_t kCheckExcl = 0xFF;   // tag of an excluded list; a group list carries its group index (0..15)
 constexpr uint32_t kTopkThreads = 256;
 constexpr uint32_t kTopkWarps = kTopkThreads / 32;
 constexpr uint32_t kTopkBudget = 32;   // bm25_topk_kernel: posting blocks per window, one planner lane each
@@ -329,8 +332,12 @@ struct TopkParams {
   // Excluded terms (the NOT children of an And, irs search/exclusion.hpp): query q rejects every doc that occurs in one
   // of the lists excl[excl_off[q] .. excl_off[q + 1]), each {first BlockDesc, blocks} in this segment (0 blocks: a term
   // the segment does not hold). Excluded terms never score. Null: no query of the call excludes anything.
+  // excl_grp, when set, tags each of those lists: kCheckExcl for an excluded list, else the index (0..15) of a required
+  // OR group of the query (`a & (b | c)`): a doc then also needs, for every group present, a tagged list that holds it.
+  // Set only for the kGroups instantiations, whose queries have at most kMaxCheckLists lists.
   const uint2* excl = nullptr;
   const uint32_t* excl_off = nullptr;
+  const uint8_t* excl_grp = nullptr;
   uint32_t k;
   uint32_t cap;                // candidate buffer capacity, power of two, > k
   int32_t conjunction;         // 0 OR, 1 AND
@@ -471,6 +478,13 @@ __device__ __forceinline__ bool probe_contains(const PostingsDev& S, uint2 list,
   return block_find_doc(S, desc, list.x + l, d, idx);
 }
 
+// Bit g set for every group tag g (< kCheckExcl) among the n list tags: the groups a doc has to satisfy.
+__device__ __forceinline__ uint32_t check_group_mask(const uint8_t* grp, uint32_t n) {
+  uint32_t need = 0u;
+  for (uint32_t x = 0; x < n; ++x) if (grp[x] != kCheckExcl) need |= 1u << grp[x];
+  return need;
+}
+
 // One thread: does any of the n excluded lists hold doc d (legacy window kernel's emit step)? Each list is searched from
 // its first block. Takes the views by value so that the kernel's parameter block is not copied to local memory.
 __device__ __noinline__ bool excluded_doc(const uint4* arena, const uint4* blocks, const uint4* anchors, const uint2* ex, uint32_t n,
@@ -484,9 +498,30 @@ __device__ __noinline__ bool excluded_doc(const uint4* arena, const uint4* block
   return false;
 }
 
+// The same with OR groups: is doc d rejected because an excluded list holds it, or because some group tagged in `grp`
+// has no list that holds it? A group's remaining lists are skipped once one of them holds d.
+__device__ __noinline__ bool excluded_doc(const uint4* arena, const uint4* blocks, const uint4* anchors, const uint2* ex,
+                                          const uint8_t* grp, uint32_t n, uint32_t d) {
+  const uint32_t need = check_group_mask(grp, n);
+  PostingsDev S{};
+  S.arena = arena; S.blocks = blocks; S.anchors = anchors;
+  uint32_t got = 0u;
+  for (uint32_t x = 0; x < n; ++x) {
+    const uint32_t g = grp[x];
+    if (g != kCheckExcl && ((got >> g) & 1u)) continue;
+    uint32_t blk = 0;
+    if (probe_contains(S, ex[x], d, 0u, blk)) {
+      if (g == kCheckExcl) return true;
+      got |= 1u << g;
+    }
+  }
+  return got != need;
+}
+
 // kDrive compiles the driver-mode code (pruning level 2) in; the default kernel stays free of its registers. kExcl: the
-// queries of the launch exclude terms (TopkParams::excl); likewise kept out of the other instantiations.
-template <bool kDrive, bool kExcl = false>
+// queries of the launch exclude terms (TopkParams::excl); with kGroups they also require OR groups (TopkParams::excl_grp).
+// Likewise kept out of the other instantiations.
+template <bool kDrive, bool kExcl = false, bool kGroups = false>
 __global__ void __launch_bounds__(kTopkThreads)
 bm25_topk_kernel(const TopkParams P) {
   constexpr uint32_t kEntries = kTopkBudget * 128u;
@@ -514,7 +549,8 @@ bm25_topk_kernel(const TopkParams P) {
   __shared__ uint32_t s_ncand, s_matched;
   __shared__ unsigned long long s_theta;
   __shared__ uint32_t s_hist[258];
-  __shared__ uint2 s_ex[kExcl ? kMaxQueryTerms : 1];   // excluded lists of the query (TopkParams::excl)
+  __shared__ uint2 s_ex[kGroups ? kMaxCheckLists : kExcl ? kMaxQueryTerms : 1];   // check lists of the query (TopkParams::excl)
+  __shared__ uint8_t s_exg[kGroups ? kMaxCheckLists : 1];                          // and their tags (kGroups)
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint4 work = P.work[blockIdx.x];
@@ -522,7 +558,7 @@ bm25_topk_kernel(const TopkParams P) {
   const uint32_t t0 = P.qterm_off[q];
   const uint32_t T = min(P.qterm_off[q + 1] - t0, kMaxQueryTerms);
   const uint32_t x0 = kExcl ? P.excl_off[q] : 0u;
-  const uint32_t n_ex = kExcl ? min(P.excl_off[q + 1] - x0, kMaxQueryTerms) : 0u;
+  const uint32_t n_ex = kExcl ? min(P.excl_off[q + 1] - x0, kGroups ? kMaxCheckLists : kMaxQueryTerms) : 0u;
   const uint32_t m = max(1u, kTopkBudget / T);                      // block budget per term
   const unsigned long long first64 = work.y;
   const bool chain_empty = first64 > P.seg.n_docs;
@@ -532,6 +568,7 @@ bm25_topk_kernel(const TopkParams P) {
   for (uint32_t i = tid; i < P.cap; i += blockDim.x) cand[i] = 0ull;
   if (tid < T) s_qt[tid] = P.qterms[t0 + tid];
   if (kExcl && tid < n_ex) s_ex[tid] = P.excl[x0 + tid];
+  if (kGroups && tid < n_ex) s_exg[tid] = P.excl_grp[x0 + tid];
   if (tid == 0) { s_ncand = 0u; s_matched = 0u; s_theta = 0ull; }
   __syncthreads();
 
@@ -919,7 +956,8 @@ bm25_topk_kernel(const TopkParams P) {
         if (live && P.conjunction) live = e_cnt[e] == T - 1u;
         if (live && P.seg.deleted != nullptr) live = ((__ldg(P.seg.deleted + (d >> 5)) >> (d & 31u)) & 1u) == 0u;   // MaskDocIterator: neither scored nor counted
         if (live && P.filt.values != nullptr) live = filter_pass(P.filt, d);
-        if (kExcl && live) live = !excluded_doc(P.seg.arena, P.seg.blocks, P.seg.anchors, s_ex, n_ex, d);   // neither collected nor counted
+        if (kGroups && live) live = !excluded_doc(P.seg.arena, P.seg.blocks, P.seg.anchors, s_ex, s_exg, n_ex, d);
+        else if (kExcl && live) live = !excluded_doc(P.seg.arena, P.seg.blocks, P.seg.anchors, s_ex, n_ex, d);   // neither collected nor counted
         // cheap pre-test on the score bits alone; the full 64-bit key only for the few that may qualify
         const uint32_t sbits = live ? __float_as_uint(e_score[e]) : 0u;
         matched += (live && first_pass) ? 1u : 0u;

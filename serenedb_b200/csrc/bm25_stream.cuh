@@ -300,6 +300,43 @@ __device__ __noinline__ bool stream_excl_pass(const PostingsDev* S, StreamExcl* 
   return alive;
 }
 
+// Check lists of a CTA's query with OR groups (TopkParams::excl / excl_grp: excluded lists and the groups' lists), in
+// shared memory.
+struct StreamGroups {
+  uint2 list[kMaxCheckLists];
+  uint8_t grp[kMaxCheckLists];                    // kCheckExcl or the list's group index
+  uint32_t n;
+  uint32_t need;                                  // bit g: group g must hold the doc
+  uint32_t hint[kTopkWarps][kMaxCheckLists];      // per warp and list: block where the warp's last probe ended
+};
+
+// The same with OR groups: false for lanes whose doc occurs in an excluded list, or whose doc no list of some required
+// group holds; else `alive`. A lane stops probing a group once one of its lists holds the doc.
+__device__ __noinline__ bool stream_excl_pass(const PostingsDev* S, StreamGroups* X, bool alive, uint32_t d) {
+  const uint32_t lane = threadIdx.x & 31u;
+  uint32_t* const hint = X->hint[threadIdx.x >> 5];
+  uint32_t got = 0u;
+  for (uint32_t x = 0; x < X->n; ++x) {
+    if (!__any_sync(kFull, alive)) break;
+    const uint32_t g = X->grp[x];
+    const bool excl = g == kCheckExcl;
+    const bool probe = alive && (excl || ((got >> g) & 1u) == 0u);
+    uint32_t fb = 0u;
+    bool hit = false;
+    if (probe) hit = probe_contains(*S, X->list[x], d, hint[x], fb);
+    const uint32_t who = __ballot_sync(kFull, probe);
+    if (who) {
+      fb = __shfl_sync(kFull, fb, __ffs(who) - 1);
+      __syncwarp();
+      if (lane == 0) hint[x] = fb;
+      __syncwarp();
+    }
+    if (excl) alive = alive && !hit;
+    else if (hit) got |= 1u << g;
+  }
+  return alive && (got & X->need) == X->need;
+}
+
 // Candidate buffer full: exact radix select keeps the best k and raises the thresholds. Called by every thread of the
 // CTA between two barriers of the rendezvous.
 __device__ __noinline__ void stream_compact(StreamCtl* ctl, unsigned long long* cand, uint32_t cap, uint32_t k,
@@ -338,10 +375,10 @@ __device__ __noinline__ bool stream_rendezvous(StreamCtl* ctl, unsigned long lon
 // kMode: 0 = disjunction, all T lists live at first; 1 = conjunction (kAnd); 2 = disjunction in LEAD mode: only the
 // shortest list is live from the start and every other list is probed -- valid once the query's threshold exceeds the
 // summed bounds of those lists, which the CTA checks when it claims its work item (TopkParams::claim).
-// kExcl: the queries of the launch exclude terms (TopkParams::excl); separate instantiations, so that the others carry
-// none of its code or registers.
+// kExcl: the queries of the launch exclude terms (TopkParams::excl); with kGroups they also require OR groups
+// (TopkParams::excl_grp). Separate instantiations, so that the others carry none of their code or registers.
 constexpr int kModeOr = 0, kModeAnd = 1, kModeLead = 2;
-template <uint32_t T, int kMode, bool kExcl = false>
+template <uint32_t T, int kMode, bool kExcl = false, bool kGroups = false>
 __global__ void __launch_bounds__(kTopkThreads, kStreamMinBlocks)
 bm25_stream_kernel(const __grid_constant__ TopkParams P) {
   constexpr bool kAnd = kMode == kModeAnd;
@@ -349,6 +386,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
   static_assert(T >= 1 && T <= kStreamMaxTerms, "1..4 live terms");
   static_assert(!kProbeRest || T == 1, "conjunctions and lead mode stream one list");
   static_assert(!kExcl || kMode != kModeLead, "lead mode has no per-doc checks");
+  static_assert(!kGroups || (kExcl && kMode == kModeOr), "OR groups run as the disjunction of their terms");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* cand = reinterpret_cast<unsigned long long*>(smem_raw);
   unsigned char* warp_area = reinterpret_cast<unsigned char*>(cand + P.cap);
@@ -358,7 +396,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
   __shared__ QTermDev s_qt[kMaxQueryTerms];
   __shared__ float s_sfx[kMaxQueryTerms + 1];          // s_sfx[e] = sum of the list-wide block-max bounds of terms e .. (inf when unknown)
   __shared__ uint32_t s_hint[kTopkWarps][kMaxQueryTerms];   // per warp and probed term: block where the last probe ended
-  __shared__ std::conditional_t<kExcl, StreamExcl, uint32_t> s_x;   // excluded lists (kExcl only)
+  __shared__ std::conditional_t<kExcl, std::conditional_t<kGroups, StreamGroups, StreamExcl>, uint32_t> s_x;   // kExcl only
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   constexpr uint32_t kWarpBytes = T * kStreamTermBytes + (kProbeRest ? 1024u : 0u);
@@ -384,7 +422,13 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
 
   for (uint32_t i = tid; i < P.cap; i += blockDim.x) cand[i] = 0ull;
   if (tid < n_terms) s_qt[tid] = P.qterms[t0 + tid];
-  if constexpr (kExcl) {
+  if constexpr (kGroups) {
+    const uint32_t x0 = P.excl_off[q];
+    const uint32_t n_ex = min(P.excl_off[q + 1] - x0, kMaxCheckLists);
+    if (tid < n_ex) { s_x.list[tid] = P.excl[x0 + tid]; s_x.grp[tid] = P.excl_grp[x0 + tid]; }
+    for (uint32_t i = tid; i < kTopkWarps * kMaxCheckLists; i += blockDim.x) (&s_x.hint[0][0])[i] = 0u;
+    if (tid == 0) { s_x.n = n_ex; s_x.need = check_group_mask(P.excl_grp + x0, n_ex); }
+  } else if constexpr (kExcl) {
     const uint32_t x0 = P.excl_off[q];
     const uint32_t n_ex = min(P.excl_off[q + 1] - x0, kMaxQueryTerms);
     if (tid < n_ex) s_x.list[tid] = P.excl[x0 + tid];
@@ -429,10 +473,10 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
   // accepted candidates, which is what block-max skipping lives on.
   const uint32_t lim = min(P.cap, (P.k + max(P.k, 256u) + kTopkThreads - 1u) / kTopkThreads * kTopkThreads);
   const bool doc_checks = P.filt.values != nullptr || P.seg.deleted != nullptr;   // hybrid filter / DocumentMask on final docs
-  // Excluded terms: a probe per doc costs a few dependent loads. With pruning and a top-k sink only docs whose final score
-  // passes the threshold pre-test are probed (late): an excluded doc then never enters the candidate buffer, so the
-  // threshold is raised by real results only and pruned == exhaustive, and `matched` counts only docs known to survive (a
-  // lower bound). Otherwise every match is probed before it is counted (early: exact count).
+  // Per-doc list checks (excluded terms, OR groups): a probe per doc costs a few dependent loads. With pruning and a top-k
+  // sink only docs whose final score passes the threshold pre-test are probed (late): a rejected doc then never enters the
+  // candidate buffer, so the threshold is raised by real results only and pruned == exhaustive, and `matched` counts only
+  // docs known to survive (a lower bound). Otherwise every match is probed before it is counted (early: exact count).
   const bool excl_late = kExcl && P.wand != 0 && P.emit_docs == nullptr;
   const bool excl_early = kExcl && !excl_late;
 

@@ -761,16 +761,16 @@ TopkKernel merge_kernel(uint32_t T) {
     default: return bm25_merge_kernel<4>;
   }
 }
-template <int kMode, bool kExcl = false>
+template <int kMode, bool kExcl = false, bool kGroups = false>
 TopkKernel stream_kernel(uint32_t T) {
   if constexpr (kMode != kModeOr) {
     return bm25_stream_kernel<1, kMode, kExcl>;
   } else {
     switch (T) {
-      case 1: return bm25_stream_kernel<1, kModeOr, kExcl>;
-      case 2: return bm25_stream_kernel<2, kModeOr, kExcl>;
-      case 3: return bm25_stream_kernel<3, kModeOr, kExcl>;
-      default: return bm25_stream_kernel<4, kModeOr, kExcl>;
+      case 1: return bm25_stream_kernel<1, kModeOr, kExcl, kGroups>;
+      case 2: return bm25_stream_kernel<2, kModeOr, kExcl, kGroups>;
+      case 3: return bm25_stream_kernel<3, kModeOr, kExcl, kGroups>;
+      default: return bm25_stream_kernel<4, kModeOr, kExcl, kGroups>;
     }
   }
 }
@@ -789,6 +789,7 @@ int topk_smem_attrs(sdbg_ctx* c) {
     CU(c, set(merge_kernel(T)));
     CU(c, set(stream_kernel<kModeOr>(T)));
     CU(c, set(stream_kernel<kModeOr, true>(T)));
+    CU(c, set(stream_kernel<kModeOr, true, true>(T)));
   }
   CU(c, set(stream_kernel<kModeAnd>(1)));
   CU(c, set(stream_kernel<kModeAnd, true>(1)));
@@ -797,6 +798,8 @@ int topk_smem_attrs(sdbg_ctx* c) {
   CU(c, set(bm25_topk_kernel<true>));
   CU(c, set(bm25_topk_kernel<false, true>));
   CU(c, set(bm25_topk_kernel<true, true>));
+  CU(c, set(bm25_topk_kernel<false, true, true>));
+  CU(c, set(bm25_topk_kernel<true, true, true>));
   CU(c, cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   c->topk_attr_set = true;
   return SDBG_OK;
@@ -849,9 +852,11 @@ int check_query_batch(sdbg_segment* const* segs, size_t n_segs, const Term* term
 }
 
 // excl_terms / excl_off: query q excludes the term ids excl_terms[excl_off[q] .. excl_off[q + 1]) (NULL excl_off: none).
+// term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] (0..15)
+// of its query. It runs as the OR of all its terms, and a doc must also occur in a list of every group.
 int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
              size_t nq, float k1, const float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, TopkDevOut* dev,
-             const uint32_t* excl_terms = nullptr, const uint32_t* excl_off = nullptr) {
+             const uint32_t* excl_terms = nullptr, const uint32_t* excl_off = nullptr, const uint8_t* term_grp = nullptr) {
   if (!segs || !n_segs || !terms || !term_off || !nq || !k) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   if (k > 8192) return fail(c, SDBG_EUNSUPPORTED, "k > 8192");
@@ -867,6 +872,21 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
     max_docs = std::max(max_docs, segs[si]->n_docs);
   }
   if (ord >= 0xFFFFFFFFull) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-1 docs per GPU");
+  // Per-doc check lists of each query: its excluded terms (tag kCheckExcl), then, for a query of OR groups, each positive
+  // term tagged with its group. chk_off[q] .. chk_off[q + 1] index chk_terms / chk_grp.
+  std::vector<uint32_t> chk_off, chk_terms;
+  std::vector<uint8_t> chk_grp;
+  if (total_excl || term_grp) {
+    chk_off.assign(nq + 1, 0u);
+    for (size_t q = 0; q < nq; ++q) {
+      if (total_excl)
+        for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) { chk_terms.push_back(excl_terms[i]); chk_grp.push_back(kCheckExcl); }
+      if (term_grp)
+        for (uint32_t i = term_off[q]; i < term_off[q + 1]; ++i) { chk_terms.push_back(terms[i].term); chk_grp.push_back(uint8_t(term_grp[i])); }
+      chk_off[q + 1] = uint32_t(chk_terms.size());
+    }
+  }
+  const uint32_t total_chk = uint32_t(chk_terms.size());   // > 0: some query has per-doc checks
 
   TopkPlan pl;
   pl.k = k;
@@ -896,9 +916,10 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   //                threshold which of the two runs the item (TopkParams::claim)
   //   kClasses + c class c (0 / 1, 6 .. 10 only) for queries that exclude terms: the kExcl instantiations of the same
   //                kernels. Never the merge kernel, slices or lead mode, which have no per-doc checks.
+  //   2 kClasses + c  the same for queries of OR groups (term_grp; classes 0 / 1, 6 .. 9): the kGroups instantiations.
   struct WorkItem { uint32_t q, lo, len, list; uint64_t weight; uint32_t cls; };
   constexpr uint32_t kClsMerge = 2, kClsStream = 2 + kStreamMaxTerms, kClsAnd = 2 + 2 * kStreamMaxTerms, kClsSlice = kClsAnd + 1,
-                     kClsLead = kClsAnd + 2, kClasses = kClsAnd + 3, kAllClasses = 2 * kClasses;
+                     kClsLead = kClsAnd + 2, kClasses = kClsAnd + 3, kAllClasses = 3 * kClasses;
   const bool level2 = c->wand >= 2 && kind != SDBG_QUERY_AND && k1 != 0.f && k1 != kTfidfK1 && b != 0.f;
   const bool stream_ok = env_int("SDBG_STREAM", 1) != 0 && k1 != 0.f && b != 0.f && k1 != kTfidfK1 &&
                          stream_smem(pl.cap, kStreamMaxTerms, false) <= 200 * 1024;
@@ -929,7 +950,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
       // Driver mode (pruning level 2) pays only when the largest list can be probed without decoding blocks; the
       // other queries run the plain kernel, which is lighter (fewer registers, no probe buffers, level-1 planner).
       const bool drive_q = level2 && wand && nt >= 2 && largest_term < s->term_probe.size() && s->term_probe[largest_term] != 0;
-      const bool excludes = total_excl && excl_off[q + 1] > excl_off[q];
+      const bool excludes = total_chk && chk_off[q + 1] > chk_off[q];
       uint32_t cls = drive_q ? 0u : 1u;
       uint32_t slice_docs = 0;    // > 0: lead candidate
       if (stream_ok && kind == SDBG_QUERY_AND) cls = kClsAnd;
@@ -968,7 +989,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
         ++lists;
         cls = kClsLead;
       }
-      if (excludes) cls += kClasses;
+      if (excludes) cls += term_grp ? 2 * kClasses : kClasses;
       uint32_t g = uint32_t(std::max<uint64_t>(pl.G, (rest_postings + chain_target - 1) / chain_target));
       // lead mode is latency-bound (dependent loads per probe), not throughput-bound: more, shorter chains
       if (slice_docs) g = std::max(g, std::min(16u, std::max(1u, smallest / 8192u)));
@@ -997,10 +1018,11 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   const size_t off_bytes = (nq + 1) * sizeof(uint32_t);
   const size_t work_bytes = total_work * sizeof(uint4);
   const size_t qt_pad = (qt_bytes + off_bytes + 15) & ~size_t(15);   // work items are 16-byte loads
-  // excluded lists, when there are any: [uint2 {first block, blocks} x total_excl per segment | excl_off]
+  // check lists, when there are any: [uint2 {first block, blocks} x total_chk per segment | chk_off | group tags when
+  // term_grp]
   const size_t x_pos = (qt_pad + work_bytes + off_bytes + 15) & ~size_t(15);
-  const size_t x_lists = size_t(total_excl) * n_segs * sizeof(uint2);
-  const size_t desc_bytes = total_excl ? x_pos + x_lists + off_bytes : qt_pad + work_bytes + off_bytes;
+  const size_t x_lists = size_t(total_chk) * n_segs * sizeof(uint2);
+  const size_t desc_bytes = total_chk ? x_pos + x_lists + off_bytes + (term_grp ? total_chk : 0) : qt_pad + work_bytes + off_bytes;
   int rc = ensure_pinned(c, desc_bytes);
   if (rc) return rc;
   auto* h_qt = static_cast<QTermDev*>(c->h_pinned);
@@ -1011,11 +1033,12 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
     for (auto& w : seg_work) for (const WorkItem& it : w) *h_work++ = make_uint4(it.q, it.lo, it.len, it.list);
     std::memcpy(static_cast<char*>(c->h_pinned) + qt_pad + work_bytes, list_off.data(), off_bytes);
   }
-  if (total_excl) {
+  if (total_chk) {
     auto* h_x = reinterpret_cast<uint2*>(static_cast<char*>(c->h_pinned) + x_pos);
     for (size_t si = 0; si < n_segs; ++si)
-      for (uint32_t i = 0; i < total_excl; ++i) h_x[si * total_excl + i] = excl_list(segs[si], excl_terms[i]);
-    std::memcpy(static_cast<char*>(c->h_pinned) + x_pos + x_lists, excl_off, off_bytes);
+      for (uint32_t i = 0; i < total_chk; ++i) h_x[si * total_chk + i] = excl_list(segs[si], chk_terms[i]);
+    std::memcpy(static_cast<char*>(c->h_pinned) + x_pos + x_lists, chk_off.data(), off_bytes);
+    if (term_grp) std::memcpy(static_cast<char*>(c->h_pinned) + x_pos + x_lists + off_bytes, chk_grp.data(), total_chk);
   }
   for (size_t si = 0; si < n_segs; ++si) {
     const sdbg_segment* s = segs[si];
@@ -1059,8 +1082,8 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
   // Work classes are separate launches; with more than one present they alternate between two streams (forked from
   // and joined back into the context's stream) so that no class waits for another's tail. First slices (class 11) go
   // first, and everything that depends on their thresholds is ordered behind them.
-  uint32_t classes_present = 0;
-  for (size_t si = 0; si < n_segs; ++si) for (uint32_t k2 = 0; k2 < kAllClasses; ++k2) if (n_cls[si][k2]) classes_present |= 1u << k2;
+  uint64_t classes_present = 0;
+  for (size_t si = 0; si < n_segs; ++si) for (uint32_t k2 = 0; k2 < kAllClasses; ++k2) if (n_cls[si][k2]) classes_present |= 1ull << k2;
   const bool two_lanes = (classes_present & (classes_present - 1u)) != 0u;
   {
     ProfScope ps_(c, kProfTopk);   // one span for all top-k launches of the call
@@ -1077,9 +1100,10 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
       P.cand_n = static_cast<uint32_t*>(b_candn.p);
       P.k = k; P.cap = pl.cap; P.conjunction = kind == SDBG_QUERY_AND ? 1 : 0;
       P.claim = nullptr;
-      if (total_excl) {
-        P.excl = reinterpret_cast<const uint2*>(static_cast<const char*>(b_qt.p) + x_pos) + si * total_excl;
+      if (total_chk) {
+        P.excl = reinterpret_cast<const uint2*>(static_cast<const char*>(b_qt.p) + x_pos) + si * total_chk;
         P.excl_off = reinterpret_cast<const uint32_t*>(static_cast<const char*>(b_qt.p) + x_pos + x_lists);
+        if (term_grp) P.excl_grp = reinterpret_cast<const uint8_t*>(static_cast<const char*>(b_qt.p) + x_pos + x_lists + off_bytes);
       }
       const int wand = seg_wand(s);
       const uint4* const work0 = reinterpret_cast<const uint4*>(static_cast<const char*>(b_qt.p) + qt_pad) + work_done;
@@ -1106,18 +1130,19 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
         cudaStream_t st = (two_lanes && (lane_no++ & 1u)) ? c->stream2 : c->stream;
         P.work = work0 + cls_off[cls];
         P.claim = nullptr;
-        // queries with excluded terms: the kExcl instantiations of the same kernels
-        const bool excl = cls >= kClasses;
-        const uint32_t cb = excl ? cls - kClasses : cls;
+        // queries with excluded terms / OR groups: the kExcl / kGroups instantiations of the same kernels
+        const bool grp = cls >= 2 * kClasses;
+        const bool excl = cls >= kClasses && !grp;
+        const uint32_t cb = cls % kClasses;
         TopkKernel kern;
         size_t sm;
         if (cb == 0) {
           P.wand = wand;
-          kern = excl ? bm25_topk_kernel<true, true> : bm25_topk_kernel<true>;
+          kern = grp ? bm25_topk_kernel<true, true, true> : excl ? bm25_topk_kernel<true, true> : bm25_topk_kernel<true>;
           sm = smem_drive;
         } else if (cb == 1) {
           P.wand = std::min(wand, 1);
-          kern = excl ? bm25_topk_kernel<false, true> : bm25_topk_kernel<false>;
+          kern = grp ? bm25_topk_kernel<false, true, true> : excl ? bm25_topk_kernel<false, true> : bm25_topk_kernel<false>;
           sm = pl.smem;
         } else if (cb == kClsAnd) {
           P.wand = 0;                                  // conjunctions are exact: every candidate of the lead list is probed
@@ -1136,7 +1161,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25
         } else if (cb >= kClsStream) {
           const uint32_t T = cb - kClsStream + 1u;
           P.wand = wand;
-          kern = excl ? stream_kernel<kModeOr, true>(T) : stream_kernel<kModeOr>(T);
+          kern = grp ? stream_kernel<kModeOr, true, true>(T) : excl ? stream_kernel<kModeOr, true>(T) : stream_kernel<kModeOr>(T);
           sm = stream_smem(pl.cap, T, false);
         } else {
           P.wand = 0;
@@ -1233,10 +1258,11 @@ extern "C" int sdbg_tfidf_topk_batch(sdbg_segment* const* segs, size_t n_segs, i
 namespace {
 int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
                     size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b, const sdbg_col_pred* filt,
-                    uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
+                    uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches,
+                    const uint8_t* term_grp = nullptr) {
   if (!out || !n_out) return SDBG_EINVAL;
   TopkDevOut dev{};
-  int rc = topk_run(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, &dev, excl_terms, excl_off);
+  int rc = topk_run(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, &dev, excl_terms, excl_off, term_grp);
   if (rc) return rc;
   sdbg_ctx* c = segs[0]->ctx;
   const size_t kb = nq * size_t(k) * 8, nb = nq * 4, tb = nq * 8;
@@ -1306,12 +1332,114 @@ extern "C" int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_seg
                          total_matches);
 }
 
+// ---- conjunctions of OR groups (`a & (b | c) & !d`) ----
+namespace {
+// A batch of group queries split by shape. Shape 0: one group, run as the flat OR of its terms; 1: every group one term,
+// run as the AND; 2: a true nested query, run with its groups (term_grp). Each shape becomes a batch of the existing
+// entry points' form: terms / term_off / excl_terms / excl_off over its queries, in batch order.
+template <class Term>
+struct GroupSplit {
+  std::vector<size_t> qs[3];
+  std::vector<Term> terms[3];
+  std::vector<uint32_t> term_off[3], excl_terms[3], excl_off[3];
+  std::vector<uint8_t> term_grp[3];
+};
+
+// Checks of sdbg_*_batch_groups beyond check_query_batch (which each sub-batch runs as well) and the split by shape:
+// non-decreasing query_group_off / group_off / excl_off, 1..16 groups, 1..16 positive terms and at most 16 excluded ones
+// per query, no empty group, no positive term id twice in a query.
+template <class Term>
+int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, const uint32_t* query_group_off, size_t nq,
+                 const uint32_t* excl_terms, const uint32_t* excl_off, GroupSplit<Term>& S) {
+  for (size_t q = 0; q < nq; ++q) {
+    if (query_group_off[q + 1] < query_group_off[q]) return fail(c, SDBG_EINVAL, "query_group_off must be non-decreasing");
+    for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g)
+      if (group_off[g + 1] < group_off[g]) return fail(c, SDBG_EINVAL, "group_off must be non-decreasing");
+    if (excl_off && excl_off[q + 1] < excl_off[q]) return fail(c, SDBG_EINVAL, "excl_off must be non-decreasing");
+  }
+  for (size_t q = 0; q < nq; ++q) {
+    const uint32_t ng = query_group_off[q + 1] - query_group_off[q];
+    if (ng == 0 || ng > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 groups");
+    const uint32_t t0 = group_off[query_group_off[q]], t1 = group_off[query_group_off[q + 1]];
+    if (t1 - t0 > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 terms");
+    if (excl_off && excl_off[q + 1] - excl_off[q] > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
+  }
+  for (size_t q = 0; q < nq; ++q) {
+    for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g)
+      if (group_off[g + 1] == group_off[g]) return fail(c, SDBG_EINVAL, "empty OR group");
+    const uint32_t t0 = group_off[query_group_off[q]], t1 = group_off[query_group_off[q + 1]];
+    if (!terms) return fail(c, SDBG_EINVAL, "terms is NULL");
+    if (excl_off && excl_off[q + 1] > excl_off[q] && !excl_terms) return fail(c, SDBG_EINVAL, "excl_terms is NULL");
+    std::array<uint32_t, kMaxQueryTerms> ids;
+    for (uint32_t i = t0; i < t1; ++i) ids[i - t0] = term_id(terms[i]);
+    std::sort(ids.begin(), ids.begin() + (t1 - t0));
+    if (std::adjacent_find(ids.begin(), ids.begin() + (t1 - t0)) != ids.begin() + (t1 - t0))
+      return fail(c, SDBG_EINVAL, "a positive term id occurs twice in a query");
+  }
+  for (int sh = 0; sh < 3; ++sh) { S.term_off[sh].assign(1, 0u); S.excl_off[sh].assign(1, 0u); }
+  for (size_t q = 0; q < nq; ++q) {
+    const uint32_t g0 = query_group_off[q], g1 = query_group_off[q + 1];
+    const uint32_t t0 = group_off[g0], t1 = group_off[g1];
+    const int sh = g1 - g0 == 1 ? 0 : (t1 - t0 == g1 - g0 ? 1 : 2);
+    S.qs[sh].push_back(q);
+    for (uint32_t g = g0; g < g1; ++g)
+      for (uint32_t i = group_off[g]; i < group_off[g + 1]; ++i) {
+        S.terms[sh].push_back(terms[i]);
+        if (sh == 2) S.term_grp[sh].push_back(uint8_t(g - g0));
+      }
+    S.term_off[sh].push_back(uint32_t(S.terms[sh].size()));
+    if (excl_off)
+      for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) S.excl_terms[sh].push_back(excl_terms[i]);
+    S.excl_off[sh].push_back(uint32_t(S.excl_terms[sh].size()));
+  }
+  return SDBG_OK;
+}
+}  // namespace
+
+// Top-k of group queries: each shape through topk_batch_host; a batch of one shape writes straight into the caller's arrays.
+extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                           const uint32_t* group_off, const uint32_t* query_group_off, size_t nq,
+                                           const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b,
+                                           const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
+                                           uint32_t* n_out, uint64_t* total_matches) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !out || !n_out) return SDBG_EINVAL;
+  GroupSplit<sdbg_bm25_term> S;
+  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, nq, excl_terms, excl_off, S)) return rc;
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    if (!n) continue;
+    const int kind = sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR;
+    const uint8_t* grp = sh == 2 ? S.term_grp[sh].data() : nullptr;
+    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
+    if (n == nq) {
+      return topk_batch_host(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), k1, b,
+                             filt, k, threshold_in, out, n_out, total_matches, grp);
+    }
+    std::vector<sdbg_hit> h(n * size_t(k));
+    std::vector<uint32_t> hn(n);
+    std::vector<uint64_t> ht(n);
+    if (int rc = topk_batch_host(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), k1, b,
+                                 filt, k, threshold_in, h.data(), hn.data(), ht.data(), grp))
+      return rc;
+    for (size_t j = 0; j < n; ++j) {
+      const size_t q = S.qs[sh][j];
+      std::copy(h.begin() + j * k, h.begin() + j * k + hn[j], out + q * k);
+      n_out[q] = hn[j];
+      if (total_matches) total_matches[q] = ht[j];
+    }
+  }
+  return SDBG_OK;
+}
+
 // Count mode (duckdb_search_full_scan RunCountScan): bm25_count_kernel over work items {query, first window, windows} of
 // kCountWindow-doc windows, planned per segment from posting counts and issued largest first. A single-term query over a
 // segment without filter, deleted docs or an excluded list holding blocks there is answered from the term's docs_count.
-extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
-                                      const uint32_t* term_off, size_t nq, const uint32_t* excl_terms,
-                                      const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
+// term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] of its
+// query (groups 0 .. n - 1 all present); those queries run bm25_count_kernel<false, true>.
+namespace {
+int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms, const uint32_t* term_off, size_t nq,
+              const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts,
+              const uint8_t* term_grp = nullptr) {
   if (!segs || !n_segs || !terms || !term_off || !nq || !counts) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   CU(c, cudaSetDevice(c->device));
@@ -1325,6 +1453,17 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
   struct Item { uint32_t q, w0, nw; uint64_t weight; };
   std::vector<std::vector<Item>> seg_work(n_segs);
   std::vector<uint2> lists(n_lists * n_segs);
+  // OR groups: grp_off[q] .. grp_off[q + 1] index each segment's group ends (relative to term_off[q]), lead group first
+  std::vector<uint32_t> grp_off, grp_end;
+  if (term_grp) {
+    grp_off.assign(nq + 1, 0u);
+    for (size_t q = 0; q < nq; ++q) {
+      uint32_t ng = 0;
+      for (uint32_t i = term_off[q]; i < term_off[q + 1]; ++i) ng = std::max(ng, uint32_t(term_grp[i]) + 1u);
+      grp_off[q + 1] = grp_off[q] + ng;
+    }
+    grp_end.assign(size_t(grp_off[nq]) * n_segs, 0u);
+  }
   uint64_t batch_postings = 0;
   for (size_t si = 0; si < n_segs; ++si)
     for (uint32_t i = term_off[0]; i < n_pos; ++i) batch_postings += segs[si]->term_docs[terms[i]];
@@ -1347,6 +1486,30 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
         sum += dc;
         smallest = std::min(smallest, dc);
       }
+      if (term_grp) {
+        // groups by ascending summed docs_count: the lead group (the cheapest) fills the window bitmap and the most
+        // selective groups narrow it first
+        const uint32_t ng = grp_off[q + 1] - grp_off[q];
+        std::array<uint64_t, kMaxQueryTerms> gsum{};
+        std::array<uint32_t, kMaxQueryTerms> order{}, gsize{};
+        for (uint32_t i = t0; i < t1; ++i) { gsum[term_grp[i]] += by_docs[i - t0].first; ++gsize[term_grp[i]]; }
+        for (uint32_t g = 0; g < ng; ++g) order[g] = g;
+        std::stable_sort(order.begin(), order.begin() + ng, [&](uint32_t a, uint32_t b) { return gsum[a] < gsum[b]; });
+        uint32_t* gend = grp_end.data() + si * grp_off[nq] + grp_off[q];
+        uint32_t o = 0;
+        for (uint32_t j = 0; j < ng; ++j) {
+          for (uint32_t i = t0; i < t1; ++i) if (term_grp[i] == order[j]) L[t0 + o++] = by_docs[i - t0].second;
+          gend[j] = o;
+        }
+        if (gsum[order[0]] == 0) continue;               // a group with no doc in this segment: no match here
+        const uint64_t weight = gsum[order[0]] * ng;
+        uint32_t g = uint32_t(std::max<uint64_t>(G, (weight + chain_target - 1) / chain_target));
+        g = std::min({g, n_win, 2u * uint32_t(c->sm_count)});
+        const uint32_t per = (n_win + g - 1) / g;
+        for (uint32_t w0 = 0; w0 < n_win; w0 += per)
+          seg_work[si].push_back({uint32_t(q), w0, std::min(per, n_win - w0), weight / g});
+        continue;
+      }
       // ascending docs_count: the shortest list of a conjunction fills the window bitmap
       std::stable_sort(by_docs.begin(), by_docs.begin() + (t1 - t0), [](const auto& a, const auto& b) { return a.first < b.first; });
       for (uint32_t i = t0; i < t1; ++i) L[i] = by_docs[i - t0].second;
@@ -1366,11 +1529,12 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
     total_items += seg_work[si].size();
   }
   if (total_items) {
-    // [term_off | excl_off | lists per segment | work items]
+    // [term_off | excl_off | lists per segment | work items | grp_off | group ends per segment]
     const size_t off_bytes = (nq + 1) * 4;
     const size_t lists_pos = (2 * off_bytes + 7) & ~size_t(7);
     const size_t work_pos = (lists_pos + lists.size() * sizeof(uint2) + 15) & ~size_t(15);
-    const size_t bytes = work_pos + total_items * sizeof(uint4);
+    const size_t grp_pos = work_pos + total_items * sizeof(uint4);
+    const size_t bytes = grp_pos + (term_grp ? off_bytes + grp_end.size() * 4 : 0);
     int rc = ensure_pinned(c, std::max(bytes, nq * 8));
     if (rc) return rc;
     char* h = static_cast<char*>(c->h_pinned);
@@ -1379,6 +1543,10 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
     std::memcpy(h + lists_pos, lists.data(), lists.size() * sizeof(uint2));
     auto* hw = reinterpret_cast<uint4*>(h + work_pos);
     for (auto& w : seg_work) for (const Item& it : w) *hw++ = make_uint4(it.q, it.w0, it.nw, 0u);
+    if (term_grp) {
+      std::memcpy(h + grp_pos, grp_off.data(), off_bytes);
+      std::memcpy(h + grp_pos + off_bytes, grp_end.data(), grp_end.size() * 4);
+    }
     DevBuf& b_desc = c->scratch[0]; DevBuf& b_counts = c->scratch[1];
     if ((rc = ensure(c, b_desc, bytes))) return rc;
     if ((rc = ensure(c, b_counts, nq * 8))) return rc;
@@ -1398,7 +1566,11 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
       P.work = reinterpret_cast<const uint4*>(d + work_pos) + done;
       P.counts = static_cast<unsigned long long*>(b_counts.p);
       done += seg_work[si].size();
-      if (conj) bm25_count_kernel<true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
+      if (term_grp) {
+        P.grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
+        P.grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[nq];
+        bm25_count_kernel<false, true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
+      } else if (conj) bm25_count_kernel<true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
       else bm25_count_kernel<false><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
       ++c->launches;
     }
@@ -1409,6 +1581,36 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
     for (size_t q = 0; q < nq; ++q) host[q] += dc[q];
   }
   std::memcpy(counts, host.data(), nq * 8);
+  return SDBG_OK;
+}
+}  // namespace
+
+extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
+                                      const uint32_t* term_off, size_t nq, const uint32_t* excl_terms,
+                                      const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
+  return count_run(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, filt, counts);
+}
+
+extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                             const uint32_t* group_off, const uint32_t* query_group_off, size_t nq,
+                                             const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                             uint64_t* counts) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts) return SDBG_EINVAL;
+  GroupSplit<uint32_t> S;
+  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, nq, excl_terms, excl_off, S)) return rc;
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    if (!n) continue;
+    const int kind = sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR;
+    const uint8_t* grp = sh == 2 ? S.term_grp[sh].data() : nullptr;
+    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
+    std::vector<uint64_t> cn(n);
+    if (int rc = count_run(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), filt,
+                           n == nq ? counts : cn.data(), grp))
+      return rc;
+    if (n != nq)
+      for (size_t j = 0; j < n; ++j) counts[S.qs[sh][j]] = cn[j];
+  }
   return SDBG_OK;
 }
 

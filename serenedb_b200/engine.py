@@ -466,7 +466,69 @@ def ExecuteCount(reader, query_terms, kind, filt=None, exclude=None):
                                  exclude=None if exclude is None else [list(exclude)])[0])
 
 
-FOR_BLOCK_DTYPE = np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])
+def _groups(queries):
+    """Queries as lists of OR groups -> (flat term ids, group_off u32, query_group_off u32)."""
+    groups = [list(g) for q in queries for g in q]
+    query_group_off = np.zeros(len(queries) + 1, np.uint32)
+    query_group_off[1:] = np.cumsum([len(q) for q in queries])
+    group_off = np.zeros(len(groups) + 1, np.uint32)
+    group_off[1:] = np.cumsum([len(g) for g in groups])
+    return [t for g in groups for t in g], group_off, query_group_off
+
+
+def ExecuteTopKGroupsBatch(reader, queries, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
+    """Top-k of conjunctions of OR groups (`a & (b | c) & !d`, sdbg_bm25_topk_batch_groups). queries: per query a list of
+    1..16 groups, each a non-empty list of term ids (1..16 distinct ids per query in all). A hit's score is the score the
+    flat OR of the query's terms gives that doc. exclude: as in ExecuteTopKBatch. Returns (hits [Q, k], n_out [Q],
+    total_matches [Q])."""
+    nq = len(queries)
+    ids, group_off, query_group_off = _groups(queries)
+    terms = (N.BM25Term * max(len(ids), 1))()
+    for i, t in enumerate(ids):
+        terms[i] = reader.stats(scorer, t)
+    hits = np.zeros((nq, k), HIT_DTYPE)
+    n_out = np.zeros(nq, np.uint32)
+    total = np.zeros(nq, np.uint64)
+    x = _exclusions(exclude, nq)
+    fp = C.byref(filt) if filt is not None else None
+    N.check(N.lib().sdbg_bm25_topk_batch_groups(_seg_array(reader.segments), len(reader.segments), terms, _ptr(group_off),
+                                                _ptr(query_group_off), nq, _ptr(x[0]) if x is not None else None,
+                                                _ptr(x[1]) if x is not None else None, scorer.k, scorer.b, fp, int(k),
+                                                float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
+    return hits, n_out, total
+
+
+def ExecuteTopKGroups(reader, groups, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
+    """ExecuteTopKGroupsBatch for one query (a list of OR groups): (hits, total_matches)."""
+    hits, n_out, total = ExecuteTopKGroupsBatch(reader, [[list(g) for g in groups]], scorer, k, filt, threshold,
+                                                exclude=None if exclude is None else [list(exclude)])
+    return hits[0, :n_out[0]].copy(), int(total[0])
+
+
+def ExecuteCountGroupsBatch(reader, queries, filt=None, exclude=None):
+    """Count mode for conjunctions of OR groups (sdbg_match_count_batch_groups): per query, the number of docs over all
+    segments in which every group has a term, that are not deleted, pass `filt` and hold none of its `exclude` term ids.
+    Exact at every pruning level. Returns uint64[Q]."""
+    nq = len(queries)
+    ids, group_off, query_group_off = _groups(queries)
+    flat = np.ascontiguousarray(ids, dtype=np.uint32)
+    counts = np.zeros(nq, np.uint64)
+    x = _exclusions(exclude, nq)
+    fp = C.byref(filt) if filt is not None else None
+    N.check(N.lib().sdbg_match_count_batch_groups(_seg_array(reader.segments), len(reader.segments),
+                                                  _ptr(flat) if len(flat) else None, _ptr(group_off), _ptr(query_group_off), nq,
+                                                  _ptr(x[0]) if x is not None else None, _ptr(x[1]) if x is not None else None,
+                                                  fp, _ptr(counts)), reader.segments[0].ctx._h)
+    return counts
+
+
+def ExecuteCountGroups(reader, groups, filt=None, exclude=None):
+    """ExecuteCountGroupsBatch for one query: its match count as an int."""
+    return int(ExecuteCountGroupsBatch(reader, [[list(g) for g in groups]], filt,
+                                       exclude=None if exclude is None else [list(exclude)])[0])
+
+
+FOR_BLOCK_DTYPE =np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])
 
 
 def pack_for(values, out_words=None):

@@ -2,7 +2,8 @@
 // (ExecuteTopK's collector loop, IResearchScanFunction's chunk loop) and prints results as JSON lines
 // for tests/test_gpu_adapters.py to compare with the oracle. Needs a GPU at run time. With a second argument "excl" it runs
 // only the exclusion case instead (an And with a Not child, tests/test_gpu_exclusion.py); with "count", only the Count
-// scan mode (GpuCountScan, tests/test_gpu_count.py).
+// scan mode (GpuCountScan, tests/test_gpu_count.py); with "groups", only an And of Or groups through both adapters
+// (tests/test_gpu_groups.py).
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -61,6 +62,37 @@ int main(int argc, char** argv) {
       std::printf(", \"stream_n\": %llu, \"stream_doc_sum\": %llu, \"stream_score_sum\": %.12g}\n", static_cast<unsigned long long>(n),
                   static_cast<unsigned long long>(doc_sum), score_sum);
     }
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
+  if (argc > 2 && std::string(argv[2]) == "groups") {
+    // `t2 & (t5 | t6)` and `t2 & (t5 | t6) & !t3`, without and with the table filter: Collect (top-100) and count(*)
+    std::vector<sdbg_bm25_term> g3(3);
+    const uint32_t gids[3] = {2, 5, 6};
+    for (int i = 0; i < 3; ++i) { sdbg_bm25_collect(n_docs, sum_dl, dc[gids[i]], 1.2f, 0.75f, &g3[size_t(i)]); g3[size_t(i)].term = gids[i]; }
+    ListCollector col;
+    irs::ScoreFunction sf; irs::ColumnArgsFetcher fetcher;
+    for (int with_filter = 0; with_filter < 2; ++with_filter)
+      for (int excl = 0; excl < 2; ++excl) {
+        const std::vector<uint32_t> ex = excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{};
+        sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_OR, g3, 1.2f, 0.75f, 100, with_filter ? &filt : nullptr, ex, {1, 2});
+        col.docs.clear();
+        it.Collect(sf, fetcher, col);
+        std::printf("{\"filter\": %d, \"excl\": %d, \"topk\": [", with_filter, excl);
+        for (size_t i = 0; i < col.docs.size(); ++i) std::printf("%s[%u, %.9g]", i ? ", " : "", col.docs[i].doc, double(col.docs[i].score));
+        sdbg_host::GpuCountScan scan({seg}, SDBG_QUERY_OR, {2, 5, 6}, ex, with_filter ? &filt : nullptr, {1, 2});
+        duckdb::DataChunkMock chunk;
+        scan.Scan(chunk);
+        const long long count = chunk.size ? chunk.count[0] : -1;
+        scan.Scan(chunk);
+        std::printf("], \"total\": %llu, \"threshold\": %.9g, \"count\": %lld, \"rows_after\": %llu}\n",
+                    static_cast<unsigned long long>(it.total_matches()), double(it.threshold().value), count,
+                    static_cast<unsigned long long>(chunk.size));
+      }
+    int code = 0;   // k = 0 (the streaming scan) has no grouped form
+    try { sdbg_host::GpuTopKIterator st(seg, SDBG_QUERY_OR, g3, 1.2f, 0.75f, 0, nullptr, {}, {1, 2}); } catch (const sdbg_host::GpuError& e) { code = e.code; }
+    std::printf("{\"stream_error\": %d}\n", code);
     sdbg_segment_destroy(seg);
     sdbg_destroy(ctx);
     return 0;

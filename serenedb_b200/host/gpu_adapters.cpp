@@ -9,14 +9,25 @@ namespace {
 void check(int rc, const char* what) {
   if (rc != SDBG_OK) throw GpuError(rc, std::string(what) + " failed with code " + std::to_string(rc));
 }
+
+// OR group sizes -> the group_off / query_group_off pair of one query (sdbg_*_batch_groups).
+std::vector<uint32_t> group_offsets(const std::vector<uint32_t>& sizes, size_t n_terms) {
+  std::vector<uint32_t> off(1, 0u);
+  for (uint32_t n : sizes) off.push_back(off.back() + n);
+  if (off.back() != n_terms) throw GpuError(SDBG_EINVAL, "OR group sizes must add up to the number of terms");
+  return off;
+}
 }  // namespace
 
 GpuTopKIterator::GpuTopKIterator(sdbg_segment* segment, int kind, std::vector<sdbg_bm25_term> terms, float k1, float b,
-                                 uint32_t k, const sdbg_col_pred* table_filter, std::vector<uint32_t> excluded_terms)
-    : seg_(segment), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)), k1_(k1), b_(b), k_(k),
-      has_filter_(table_filter != nullptr) {
+                                 uint32_t k, const sdbg_col_pred* table_filter, std::vector<uint32_t> excluded_terms,
+                                 std::vector<uint32_t> group_sizes)
+    : seg_(segment), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)), groups_(std::move(group_sizes)),
+      k1_(k1), b_(b), k_(k), has_filter_(table_filter != nullptr) {
   if (table_filter) filter_ = *table_filter;
   threshold_.value = FLT_MIN;  // doc_collector.hpp:102
+  // the streaming scan (sdbg_bm25_scan*) has no grouped form
+  if (!groups_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "OR groups need k > 0: the streaming scan has no grouped form");
 }
 
 void GpuTopKIterator::run() {
@@ -46,7 +57,14 @@ void GpuTopKIterator::run() {
   uint32_t n = 0;
   float thr_out = 0;
   sdbg_segment* segs[1] = {seg_};
-  if (excluded_.empty()) {
+  if (!groups_.empty()) {
+    const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
+    const uint32_t query_group_off[2] = {0, uint32_t(groups_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
+    check(sdbg_bm25_topk_batch_groups(segs, 1, terms_.data(), group_off.data(), query_group_off, 1, excluded_.data(), excl_off, k1_, b_,
+                                      has_filter_ ? &filter_ : nullptr, k_, threshold_.value, hits_.data(), &n, &total_),
+          "sdbg_bm25_topk_batch_groups");
+    thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;
+  } else if (excluded_.empty()) {
     check(sdbg_bm25_topk(segs, 1, kind_, terms_.data(), terms_.size(), k1_, b_, has_filter_ ? &filter_ : nullptr, k_,
                          threshold_.value, hits_.data(), &n, &total_, &thr_out),
           "sdbg_bm25_topk");
@@ -173,9 +191,9 @@ void GpuAggScan::Scan(duckdb::DataChunkMock& output) {
 }
 
 GpuCountScan::GpuCountScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
-                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter)
+                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, std::vector<uint32_t> group_sizes)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      has_filter_(table_filter != nullptr) {
+      groups_(std::move(group_sizes)), has_filter_(table_filter != nullptr) {
   if (table_filter) filter_ = *table_filter;
 }
 
@@ -185,9 +203,20 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
   const uint32_t term_off[2] = {0, uint32_t(terms_.size())};
   const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
   uint64_t n = 0;
-  const int rc = sdbg_match_count_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
-                                        has_filter_ ? &filter_ : nullptr, &n);
-  if (rc != SDBG_OK) throw GpuError(rc, std::string("sdbg_match_count_batch: ") + sdbg_last_error(sdbg_segment_context(segs_[0])));
+  int rc;
+  const char* what;
+  if (groups_.empty()) {
+    rc = sdbg_match_count_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
+                                has_filter_ ? &filter_ : nullptr, &n);
+    what = "sdbg_match_count_batch: ";
+  } else {                                                    // an And of Ors: kind_ is not used
+    const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
+    const uint32_t query_group_off[2] = {0, uint32_t(groups_.size())};
+    rc = sdbg_match_count_batch_groups(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off, 1,
+                                       excluded_.data(), excl_off, has_filter_ ? &filter_ : nullptr, &n);
+    what = "sdbg_match_count_batch_groups: ";
+  }
+  if (rc != SDBG_OK) throw GpuError(rc, std::string(what) + sdbg_last_error(sdbg_segment_context(segs_[0])));
   output.count.push_back(int64_t(n));
   output.size = 1;
   done_ = true;
