@@ -265,13 +265,19 @@ int sdbg_decode_score_term(sdbg_segment*, uint32_t term, float c0, float norm_co
  * group. This is the algorithm of DuckDB's `bitpacking` codec in FOR mode, which the reference's column blocks name in
  * ColumnBlockMeta::codec (irs/formats/column/column_reader.hpp:90-96); DuckDB is not vendored in the reference tree, so
  * the byte layout is this library's. sdbg_pack_for is the host-side writer (returns SDBG_ECAPACITY with *n_words = the
- * room needed); sdbg_stage_column_for copies the packed stream to the GPU and decodes it there into a staged SDBG_I64
- * column, so only the packed bytes cross PCIe. */
+ * room needed); sdbg_stage_column_for copies the packed stream to the GPU, so only the packed bytes cross PCIe.
+ * HBM keeps an owned NOT NULL SDBG_I64 column in this form whenever it is smaller than the raw values (sdbg_stage_column
+ * and sdbg_synth_column pack on the device; sdbg_stage_column_for keeps the caller's stream when every group starts at an
+ * even word offset, as sdbg_pack_for writes it, and decodes it otherwise). The GROUP BY scan reads the packed words;
+ * other readers see the raw values, decoded once on first use. sdbg_column_for_to_host copies a packed column's headers
+ * and words back (the same bytes sdbg_pack_for writes for the same values); *n_words = 0 when the column is held raw. */
 typedef struct { int64_t base; uint32_t bits; uint32_t off8; } sdbg_for_block;
 int sdbg_pack_for(const int64_t* values, uint64_t rows, sdbg_for_block* headers /* (rows + 2047) / 2048 */, uint64_t* words,
                   uint64_t cap_words, uint64_t* n_words);
 int sdbg_stage_column_for(sdbg_segment*, uint64_t field, const sdbg_for_block* headers, const uint64_t* words, uint64_t n_words,
                           uint64_t rows);
+int sdbg_column_for_to_host(sdbg_segment*, uint64_t field, sdbg_for_block* headers, uint64_t* words, uint64_t cap_words,
+                            uint64_t* n_words);
 
 /* Late materialisation (HitBatcher::MaterializeColumn, irs/index/hit_batcher.hpp:39; FinalizeBatch of the search scan):
  * out_values[i] = column[docs[i] - 1] for n hit docs of the segment (element width = the staged type's), out_valid[i]

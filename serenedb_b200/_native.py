@@ -67,6 +67,7 @@ SIGNATURES = {
     "sdbg_column_to_host": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint64]),
     "sdbg_pack_for": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint64, _u64p]),
     "sdbg_stage_column_for": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint64, C.c_uint64]),
+    "sdbg_column_for_to_host": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint64, _u64p]),
     "sdbg_gather_column": (C.c_int, [_vp, C.c_uint64, _vp, _sz, _vp, _vp]),
     "sdbg_segment_posting_stats": (C.c_int, [_vp, _u64p, _u64p, _u64p, _u64p]),
     "sdbg_segment_term_bytes": (C.c_int, [_vp, _vp, _sz]),

@@ -338,6 +338,14 @@ filter_groupby_kernel(const GroupByParams P) {
 // ------------------------------------------------------------------------------------------
 constexpr int kMaxStreams = 7;   // up to 4 predicate columns + key + sum_int + sum_f64 (deduplicated)
 
+// Frame-of-reference bit-packed int64 column (DuckDB's `bitpacking` codec in FOR mode): per 2048-row group a base and a
+// bit width; value i of the group sits at bit i * bits of the group's word run, little-endian; bits == 0 is a constant
+// group. Staged columns keep every group 16-byte aligned (off8 even), so a 512-row tile of a group is 64 * bits bytes at
+// byte offset (tile % 4) * 64 * bits of the group: one bulk copy.
+struct ForBlockDev { long long base; uint32_t bits; uint32_t off8; };
+constexpr uint32_t kForGroupRows = 2048;
+constexpr int kTypeFor = 3;      // stream / predicate / key / sum type: FOR bit-packed int64 (TMA GROUP BY only)
+
 // Everything the row loop needs is resolved on the host into plain scalars (direct constant-bank operands):
 // no stream indirection, no per-row type switch over parameter arrays.
 struct TmaGroupByParams {
@@ -381,6 +389,12 @@ struct TmaGroupByParams {
   // (per-block min / max against every predicate's range: ColFilterChain::FilterWindow / DeadUntil,
   // irs/index/table_filter_iterator.cpp:147-286). Such tiles are neither copied nor looked at.
   const uint8_t* skip;
+  // kFor kernels: hdr[s] != null marks stream s as FOR bit-packed (src[s] = its word stream, elem[s] = 8 keeps the raw
+  // stage size). The producer copies only the tile's packed bytes and puts the group header into the stage; the
+  // consumers decode from shared memory. *_stream: which stream feeds predicate i / the key / the integer sum.
+  const ForBlockDev* hdr[kMaxStreams];
+  int32_t pred_stream[kMaxPreds];
+  int32_t key_stream, sum_i_stream;
 };
 constexpr uint32_t kZoneRows = 2048;   // rows per zonemap block = the reference's filter window (STANDARD_VECTOR_SIZE)
 
@@ -437,16 +451,40 @@ __device__ __forceinline__ uint32_t range2(const unsigned char* col, uint32_t r,
   if (kType == 1) { v[0] = fkey(v[0]); v[1] = fkey(v[1]); }
   return (static_cast<unsigned long long>(v[0] - lo) <= span ? 1u : 0u) | (static_cast<unsigned long long>(v[1] - lo) <= span ? 2u : 0u);
 }
+// Rows r, r+1 (r even) of a FOR bit-packed tile in shared memory: `col` holds the tile's slice of its group's words, `h`
+// the group header {base lo, base hi, bits, off8}. bits is warp-uniform; any width 0..64 (0: the constant `base`).
+__device__ __forceinline__ void unpack2(const unsigned char* col, uint32_t r, const uint4 h, long long (&v)[2]) {
+  const unsigned long long* w = reinterpret_cast<const unsigned long long*>(col);
+  const uint32_t bits = h.z;
+  const long long base = static_cast<long long>((static_cast<unsigned long long>(h.y) << 32) | h.x);
+  const unsigned long long mask = bits >= 64u ? ~0ull : (1ull << bits) - 1ull;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const uint32_t bit = (r + uint32_t(j)) * bits, wi = bit >> 6, sh = bit & 63u;
+    unsigned long long x = w[wi] >> sh;
+    if (sh + bits > 64u) x |= w[wi + 1] << (64u - sh);    // the value straddles two words (never past the tile's data)
+    v[j] = base + static_cast<long long>(x & mask);        // two's complement wrap-around undoes the encoder's subtraction
+  }
+}
+__device__ __forceinline__ uint32_t range2_for(const unsigned char* col, uint32_t r, const uint4 h, long long lo, unsigned long long span) {
+  long long v[2];
+  unpack2(col, r, h, v);
+  return (static_cast<unsigned long long>(v[0] - lo) <= span ? 1u : 0u) | (static_cast<unsigned long long>(v[1] - lo) <= span ? 2u : 0u);
+}
 
 // kQuad (opt-in, SDBG_GROUPBY_QUAD=1): every accumulator of the slot is an integer (fixed-point SUM(double) or
 // no double sum), and the four words of a row's slot are updated by four adjacent lanes of ONE RED
 // instruction: one L2 request per passing row, sums independent of update order (bit-reproducible), at the
 // cost of a compaction through shared memory and limb arithmetic in the consumer warps. Off by default.
-template <int kStages, int kTileRows, int kConsumerWarps, bool kPacked, bool kQuad>
+// kFor: some streams are FOR bit-packed (TmaGroupByParams::hdr); needs kTileRows to divide kForGroupRows with 16-byte
+// aligned tile slices, i.e. the default 512-row shape. The group headers of the stages live behind the ring (and behind
+// the quad area): kStages * kMaxStreams * 16 bytes.
+template <int kStages, int kTileRows, int kConsumerWarps, bool kPacked, bool kQuad, bool kFor = false>
 __global__ void __launch_bounds__((kConsumerWarps + 1) * 32)
 filter_groupby_tma_kernel(const TmaGroupByParams P) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages];
+  static_assert(!kFor || (kForGroupRows % kTileRows == 0 && kTileRows % 128 == 0), "a tile's packed slice must be 16-byte aligned");
 
   const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
   if (tid == 0) {
@@ -456,8 +494,54 @@ filter_groupby_tma_kernel(const TmaGroupByParams P) {
   __syncthreads();
   const uint32_t stage_bytes = P.off[P.n_streams];
   const uint64_t n_tiles = (P.rows + kTileRows - 1) / kTileRows;
+  uint4* const pk_hdr = reinterpret_cast<uint4*>(smem + size_t(kStages) * stage_bytes + (kQuad ? size_t(kConsumerWarps) * (2048u + 256u) : 0u));
 
   if (warp == kConsumerWarps) {
+    if (kFor) {
+      // ===== producer over packed streams: lane s moves stream s =====
+      // Each lane loads the group header of its stream for the NEXT tile while this one waits for its stage, so no copy
+      // address waits on a dependent global load; lane 0 puts the headers into the stage before its arrive (release).
+      const bool mine = lane < uint32_t(P.n_streams);
+      const ForBlockDev* hp = mine ? P.hdr[lane] : nullptr;
+      const char* src = mine ? static_cast<const char*>(P.src[lane]) : nullptr;
+      const uint32_t elem = mine ? uint32_t(P.elem[lane]) : 0u, soff = mine ? P.off[lane] : 0u;
+      auto header = [&](uint64_t t) { return __ldg(reinterpret_cast<const uint4*>(hp + (t * kTileRows) / kForGroupRows)); };
+      uint4 nh = make_uint4(0u, 0u, 0u, 0u);
+      uint64_t nh_tile = ~0ull;                              // the tile `nh` belongs to
+      uint32_t it = 0;
+      for (uint64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        if (P.skip != nullptr && P.skip[(tile * kTileRows) / kZoneRows]) continue;   // zonemap verdict (warp-uniform): no header
+        uint4 h = make_uint4(0u, 0u, 0u, 0u);
+        if (hp != nullptr) h = nh_tile == tile ? nh : header(tile);   // not prefetched only after a skipped tile
+        const uint64_t next = tile + gridDim.x;
+        if (hp != nullptr && next < n_tiles && (P.skip == nullptr || !P.skip[(next * kTileRows) / kZoneRows])) { nh = header(next); nh_tile = next; }
+        const uint32_t st = it % kStages, use = it / kStages;
+        ++it;
+        const uint64_t row0 = tile * kTileRows;
+        const uint32_t nrows = uint32_t(min(static_cast<unsigned long long>(kTileRows), static_cast<unsigned long long>(P.rows - row0)));
+        uint32_t bytes = 0u;
+        const char* g = nullptr;
+        if (hp != nullptr) {
+          // the tile's slice of its group's words, rounded up to 16 bytes (covered by the column's slack); none when bits == 0
+          bytes = (nrows * h.z + 127u) / 128u * 16u;
+          g = src + uint64_t(h.w) * 8u + (row0 % kForGroupRows) * h.z / 8u;
+        } else if (mine) {
+          bytes = (nrows * elem + 15u) & ~15u;
+          g = src + row0 * elem;
+        }
+        const uint32_t total = __reduce_add_sync(kFull, bytes);
+        if (lane == 0) mbar_wait(&empty_bar[st], (use & 1u) ^ 1u);   // consumers released the previous use of this stage
+        for (int s = 0; s < P.n_streams; ++s) {                // every lane shuffles, lane 0 writes
+          uint4 x;
+          x.x = __shfl_sync(kFull, h.x, s); x.y = __shfl_sync(kFull, h.y, s); x.z = __shfl_sync(kFull, h.z, s); x.w = __shfl_sync(kFull, h.w, s);
+          if (lane == 0) pk_hdr[st * kMaxStreams + s] = x;
+        }
+        if (lane == 0) mbar_arrive_expect_tx(&full_bar[st], total);   // counts only the bytes issued below
+        __syncwarp();
+        if (bytes != 0u) bulk_g2s(smem + size_t(st) * stage_bytes + soff, g, bytes, &full_bar[st]);
+      }
+      return;
+    }
     // ===== producer: one thread keeps the ring full =====
     if (lane == 0) {
       uint32_t it = 0;
@@ -498,6 +582,7 @@ filter_groupby_tma_kernel(const TmaGroupByParams P) {
     const uint64_t row0 = tile * kTileRows;
     const uint32_t nrows = uint32_t(min(static_cast<unsigned long long>(kTileRows), static_cast<unsigned long long>(P.rows - row0)));
     const uint32_t pack_word = kPacked ? uint32_t(tile % uint64_t(P.pack_tables)) : 0u;   // words 0..2 of a slot: count / sum_lo / sum_hi
+    const uint4* const hst = pk_hdr + st * kMaxStreams;       // kFor: this stage's group headers, one per stream
     for (uint32_t rb = warp * 64u; rb < nrows; rb += kConsumerWarps * 64u) {   // warp-uniform trip count
       const uint32_t r = rb + 2u * lane;
       uint32_t m = r + 1u < nrows ? 3u : r < nrows ? 1u : 0u;   // bit j: row r + j exists and still passes
@@ -506,7 +591,8 @@ filter_groupby_tma_kernel(const TmaGroupByParams P) {
         if (i < P.n_preds) {
           const unsigned char* col = base + P.pred_off[i];
           uint32_t in;
-          switch (P.pred_type[i]) {
+          if (kFor && P.pred_type[i] == kTypeFor) in = range2_for(col, r, hst[P.pred_stream[i]], P.pred_lo[i], P.pred_span[i]);
+          else switch (P.pred_type[i]) {
             case 0: in = range2<0>(col, r, P.pred_lo[i], P.pred_span[i]); break;
             case 1: in = range2<1>(col, r, P.pred_lo[i], P.pred_span[i]); break;
             default: in = range2<2>(col, r, P.pred_lo[i], P.pred_span[i]); break;
@@ -517,9 +603,11 @@ filter_groupby_tma_kernel(const TmaGroupByParams P) {
       if (!kQuad && m == 0u) continue;          // quad mode: every lane takes part in the warp-wide compaction
       long long key[2], v[2] = {0, 0};
       double w[2] = {0.0, 0.0};
-      if (P.key_type == 2) load2<2>(base + P.key_off, r, key); else load2<0>(base + P.key_off, r, key);
+      if (kFor && P.key_type == kTypeFor) unpack2(base + P.key_off, r, hst[P.key_stream], key);
+      else if (P.key_type == 2) load2<2>(base + P.key_off, r, key); else load2<0>(base + P.key_off, r, key);
       if (kPacked || P.has_sum_i) {
-        if (P.sum_i_type == 2) load2<2>(base + P.sum_i_off, r, v); else load2<0>(base + P.sum_i_off, r, v);
+        if (kFor && P.sum_i_type == kTypeFor) unpack2(base + P.sum_i_off, r, hst[P.sum_i_stream], v);
+        else if (P.sum_i_type == 2) load2<2>(base + P.sum_i_off, r, v); else load2<0>(base + P.sum_i_off, r, v);
       }
       if (P.has_sum_f) {
         const double2 x = *reinterpret_cast<const double2*>(base + P.sum_f_off + size_t(r) * 8u);
@@ -848,10 +936,20 @@ gather_rows_kernel(const T* __restrict__ values, const unsigned long long* __res
   }
 }
 
-// Frame-of-reference bit-packed int64 column -> raw values (staging-time decode). One warp per 2048-row group:
-// value i of the group sits at bit i * bits of the group's word run, little-endian; bits == 0 is a constant group.
-struct ForBlockDev { long long base; uint32_t bits; uint32_t off8; };
-constexpr uint32_t kForGroupRows = 2048;
+// Frame-of-reference bit-packed int64 column (ForBlockDev above) -> raw values: the raw view of a packed column, and the
+// decode of a caller's stream whose groups are not 16-byte aligned. One warp per 2048-row group.
+__device__ __forceinline__ long long for_value(const ForBlockDev& h, const unsigned long long* w, uint32_t i) {
+  unsigned long long v = 0ull;
+  if (h.bits != 0u) {
+    const unsigned long long mask = h.bits >= 64u ? ~0ull : ((1ull << h.bits) - 1ull);
+    const uint64_t bit = uint64_t(i) * h.bits;
+    const uint32_t sh = uint32_t(bit & 63ull);
+    const unsigned long long lo = w[bit >> 6] >> sh;
+    const unsigned long long hi = (sh != 0u && sh + h.bits > 64u) ? (w[(bit >> 6) + 1ull] << (64u - sh)) : 0ull;
+    v = (lo | hi) & mask;
+  }
+  return h.base + static_cast<long long>(v);   // two's complement wrap-around = the encoder's subtraction undone
+}
 
 __global__ void __launch_bounds__(256)
 for_unpack_kernel(const ForBlockDev* __restrict__ headers, const unsigned long long* __restrict__ words, uint64_t rows,
@@ -860,21 +958,73 @@ for_unpack_kernel(const ForBlockDev* __restrict__ headers, const unsigned long l
   const uint32_t lane = threadIdx.x & 31u;
   for (uint64_t g = (uint64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; g < n_groups; g += (uint64_t(gridDim.x) * blockDim.x) >> 5) {
     const ForBlockDev h = headers[g];
-    const unsigned long long* w = words + h.off8;
     const uint64_t row0 = g * kForGroupRows;
     const uint32_t n = (rows - row0 < kForGroupRows) ? uint32_t(rows - row0) : kForGroupRows;
-    const unsigned long long mask = h.bits >= 64u ? ~0ull : ((1ull << h.bits) - 1ull);
-    for (uint32_t i = lane; i < n; i += 32u) {             // consecutive lanes -> consecutive values: coalesced stores
-      unsigned long long v = 0ull;
-      if (h.bits != 0u) {
-        const uint64_t bit = uint64_t(i) * h.bits;
-        const uint32_t sh = uint32_t(bit & 63ull);
-        const unsigned long long lo = w[bit >> 6] >> sh;
-        const unsigned long long hi = (sh != 0u && sh + h.bits > 64u) ? (w[(bit >> 6) + 1ull] << (64u - sh)) : 0ull;
-        v = (lo | hi) & mask;
-      }
-      out[row0 + i] = h.base + static_cast<long long>(v);   // two's complement wrap-around = the encoder's subtraction undone
+    for (uint32_t i = lane; i < n; i += 32u) out[row0 + i] = for_value(h, words + h.off8, i);   // coalesced stores
+  }
+}
+
+// Device packer, pass 1: per 2048-row group min / max of raw int64 values (or of an already packed stream when
+// `words` is given: only the zonemap is written then). Writes the zonemap {min, max} per group (the predicate key space
+// of an integer column is the value itself), and for raw input the header {base = min, bits = width of max - min} and
+// the group's word count. One warp per group.
+__global__ void __launch_bounds__(256)
+for_stats_kernel(const long long* __restrict__ values, const ForBlockDev* __restrict__ packed_hdr,
+                 const unsigned long long* __restrict__ words, uint64_t rows, long long* __restrict__ zone,
+                 ForBlockDev* __restrict__ hdr, unsigned long long* __restrict__ n_words) {
+  const uint64_t n_groups = (rows + kForGroupRows - 1) / kForGroupRows;
+  const uint32_t lane = threadIdx.x & 31u;
+  for (uint64_t g = (uint64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; g < n_groups; g += (uint64_t(gridDim.x) * blockDim.x) >> 5) {
+    const uint64_t row0 = g * kForGroupRows;
+    const uint32_t n = (rows - row0 < kForGroupRows) ? uint32_t(rows - row0) : kForGroupRows;
+    long long mn = 0x7FFFFFFFFFFFFFFFll, mx = -0x7FFFFFFFFFFFFFFFll - 1;
+    for (uint32_t i = lane; i < n; i += 32u) {
+      const long long v = words ? for_value(packed_hdr[g], words + packed_hdr[g].off8, i) : values[row0 + i];
+      mn = min(mn, v); mx = max(mx, v);
     }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { mn = min(mn, __shfl_xor_sync(kFull, mn, o)); mx = max(mx, __shfl_xor_sync(kFull, mx, o)); }
+    if (lane == 0) {
+      zone[2 * g] = mn; zone[2 * g + 1] = mx;
+      if (!words) {
+        const unsigned long long span = static_cast<unsigned long long>(mx) - static_cast<unsigned long long>(mn);
+        const uint32_t bits = span == 0ull ? 0u : uint32_t(64 - __clzll(static_cast<long long>(span)));
+        ForBlockDev h; h.base = mn; h.bits = bits; h.off8 = 0u;
+        hdr[g] = h;
+        n_words[g] = (uint64_t(n) * bits + 63u) / 64u;
+      }
+    }
+  }
+}
+
+// Device packer, pass 2: the word stream in sdbg_pack_for's layout (same bytes for the same values). Each lane builds
+// whole 64-bit words from the values that overlap them, so no atomics are needed; off8 is the exclusive scan of the word
+// counts. One warp per group; the last word of the stream (offsets[n_groups]) is the writer's zero slack word.
+__global__ void __launch_bounds__(256)
+for_pack_kernel(const long long* __restrict__ values, const ForBlockDev* __restrict__ stats_hdr,
+                const unsigned long long* __restrict__ offsets, uint64_t rows, ForBlockDev* __restrict__ hdr,
+                unsigned long long* __restrict__ words) {
+  const uint64_t n_groups = (rows + kForGroupRows - 1) / kForGroupRows;
+  const uint32_t lane = threadIdx.x & 31u;
+  for (uint64_t g = (uint64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; g < n_groups; g += (uint64_t(gridDim.x) * blockDim.x) >> 5) {
+    ForBlockDev h = stats_hdr[g];
+    h.off8 = uint32_t(offsets[g]);
+    const uint64_t row0 = g * kForGroupRows;
+    const uint32_t n = (rows - row0 < kForGroupRows) ? uint32_t(rows - row0) : kForGroupRows;
+    if (lane == 0) hdr[g] = h;
+    const uint32_t nw = uint32_t(offsets[g + 1] - offsets[g]);
+    for (uint32_t wi = lane; wi < nw; wi += 32u) {
+      const uint64_t b0 = uint64_t(wi) * 64u;
+      const uint32_t i0 = uint32_t(b0 / h.bits), i1 = min(n - 1u, uint32_t((b0 + 63u) / h.bits));
+      unsigned long long word = 0ull;
+      for (uint32_t i = i0; i <= i1; ++i) {
+        const unsigned long long d = static_cast<unsigned long long>(values[row0 + i]) - static_cast<unsigned long long>(h.base);
+        const uint64_t p = uint64_t(i) * h.bits;
+        word |= p >= b0 ? d << (p - b0) : d >> (b0 - p);
+      }
+      words[h.off8 + wi] = word;
+    }
+    if (g + 1 == n_groups && lane == 0) words[offsets[n_groups]] = 0ull;
   }
 }
 

@@ -3,6 +3,7 @@
 // in bm25_kernels.cuh and column_kernels.cuh. There is no CPU fallback anywhere in this file.
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <dlfcn.h>
 #include <nccl.h>   // types only: the library is resolved at run time (sdbg_dist_init)
 
@@ -42,7 +43,14 @@ struct DevBuf {  // grow-only device scratch
 };
 
 struct ColumnObj {
+  // Raw values. For a packed column this is the raw view, decoded on first use by raw_values() and kept until the column
+  // is restaged or freed.
   void* d_values = nullptr;
+  // Owned NOT NULL int64 columns whose frame-of-reference bit-packed form is smaller than the raw one stay packed:
+  // ForBlockDev headers (packed_hdr_bytes, 256-aligned) | word stream (every group 16-byte aligned) | 64 B of slack.
+  // The default-shape TMA GROUP BY reads this directly; every other reader goes through raw_values().
+  void* d_packed = nullptr;
+  size_t packed_bytes = 0;
   uint64_t* d_validity = nullptr;
   int type = 0;
   uint64_t rows = 0;
@@ -50,6 +58,7 @@ struct ColumnObj {
   bool has_minmax = false;
   int64_t mn = 0, mx = 0;
   long long* d_zone = nullptr;  // zonemap: {min, max} per 2048-row block in predicate key space (NOT NULL columns, built on first use)
+  bool zone_ok = false;         // d_zone holds the current values' zonemap (a restage of the same shape keeps the allocation)
   bool has_absmax = false;      // double columns: bits of the largest |value| (>= 0x7FF0... when NaN / inf occur)
   uint64_t absmax_bits = 0;
 };
@@ -66,6 +75,7 @@ struct sdbg_ctx {
   std::string err;
   uint64_t launches = 0;
   DevBuf scratch[16];
+  DevBuf stage_raw;          // raw int64 values of a column being packed at staging (reused: restaging allocates nothing)
   void* h_pinned = nullptr;  // pinned host staging for small transfers
   size_t h_pinned_cap = 0;
   void* flush = nullptr;
@@ -222,6 +232,7 @@ extern "C" void sdbg_destroy(sdbg_ctx* c) {
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
   for (auto& b : c->scratch) if (b.p) cudaFree(b.p);
+  if (c->stage_raw.p) cudaFree(c->stage_raw.p);
   if (c->h_pinned) cudaFreeHost(c->h_pinned);
   if (c->h_oor) cudaFreeHost(c->h_oor);
   if (c->d_zone_skipped) cudaFree(c->d_zone_skipped);
@@ -312,8 +323,9 @@ void free_postings(sdbg_segment* s) {
 void free_column(ColumnObj& c) {
   if (c.d_zone) { cudaFree(c.d_zone); c.d_zone = nullptr; }
   if (c.owned && c.d_values) cudaFree(c.d_values);
+  if (c.d_packed) cudaFree(c.d_packed);
   if (c.d_validity) cudaFree(c.d_validity);
-  c.d_values = nullptr; c.d_validity = nullptr;
+  c.d_values = nullptr; c.d_validity = nullptr; c.d_packed = nullptr;
 }
 }  // namespace
 
@@ -472,7 +484,102 @@ extern "C" int sdbg_stage_norms(sdbg_segment* s, const uint8_t* bytes, size_t n,
 
 namespace {
 size_t type_width(int t) { return t == SDBG_I32 ? 4 : 8; }
+
+// ---- bit-packed storage of int64 columns (ColumnObj::d_packed) ----
+uint64_t for_groups(uint64_t rows) { return (rows + kForGroupRows - 1) / kForGroupRows; }
+size_t for_hdr_bytes(uint64_t rows) { return (for_groups(rows) * sizeof(ForBlockDev) + 255) & ~size_t(255); }
+const ForBlockDev* for_headers(const ColumnObj& col) { return static_cast<const ForBlockDev*>(col.d_packed); }
+const unsigned long long* for_words(const ColumnObj& col) {
+  return reinterpret_cast<const unsigned long long*>(static_cast<const char*>(col.d_packed) + for_hdr_bytes(col.rows));
 }
+unsigned grid_per_group_warp(sdbg_ctx* c, uint64_t n_groups) {
+  return unsigned(std::max<uint64_t>(1, std::min<uint64_t>((n_groups * 32 + 255) / 256, uint64_t(c->sm_count) * 16)));
+}
+int ensure_zone(sdbg_ctx* c, ColumnObj& col) {
+  if (!col.d_zone) CU(c, cudaMalloc(reinterpret_cast<void**>(&col.d_zone), for_groups(col.rows) * 16));
+  return SDBG_OK;
+}
+
+// Raw values of a column for every reader that does not decode the packed form: a packed column is decoded once and the
+// raw view kept until the column is restaged or freed.
+int raw_values(sdbg_ctx* c, ColumnObj& col, void** out) {
+  if (!col.d_values && col.d_packed) {
+    CU(c, cudaMalloc(&col.d_values, col.rows * 8 + 64));
+    CU(c, cudaMemsetAsync(static_cast<char*>(col.d_values) + col.rows * 8, 0, 64, c->stream));
+    for_unpack_kernel<<<grid_per_group_warp(c, for_groups(col.rows)), 256, 0, c->stream>>>(for_headers(col), for_words(col), col.rows,
+                                                                                           static_cast<long long*>(col.d_values));
+    ++c->launches;
+    CU(c, cudaGetLastError());
+  }
+  *out = col.d_values;
+  return SDBG_OK;
+}
+
+// Staging of an owned NOT NULL int64 column: its raw values are in c->stage_raw (rows * 8 bytes + 64 zeroed). Fills the
+// zonemap (one pass over the values), then bit-packs the column on the device when that is smaller, else copies the raw
+// values into the column. Synchronises the stream once (the packed size decides the layout). A column restaged with the
+// same packed size keeps its allocation.
+int pack_column(sdbg_ctx* c, ColumnObj& col) {
+  const uint64_t rows = col.rows, n_groups = for_groups(rows);
+  int rc;
+  auto keep_raw = [&]() -> int {
+    if (col.d_packed) { cudaFree(col.d_packed); col.d_packed = nullptr; col.packed_bytes = 0; }
+    CU(c, cudaMalloc(&col.d_values, rows * 8 + 64));
+    CU(c, cudaMemcpyAsync(col.d_values, c->stage_raw.p, rows * 8 + 64, cudaMemcpyDeviceToDevice, c->stream));
+    return SDBG_OK;
+  };
+  if (rows >= (1ull << 32)) return keep_raw();                   // 32-bit word offsets: such a column stays raw
+  if ((rc = ensure_zone(c, col))) return rc;
+  // scratch: stats headers | word counts [n_groups + 1] | offsets [n_groups + 1] | scan temp
+  const size_t h_bytes = (n_groups * sizeof(ForBlockDev) + 255) & ~size_t(255), n_bytes = ((n_groups + 1) * 8 + 255) & ~size_t(255);
+  size_t scan_bytes = 0;
+  CU(c, cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, static_cast<const unsigned long long*>(nullptr),
+                                      static_cast<unsigned long long*>(nullptr), int(n_groups + 1), c->stream));
+  if ((rc = ensure(c, c->scratch[12], h_bytes + 2 * n_bytes + scan_bytes))) return rc;
+  char* base = static_cast<char*>(c->scratch[12].p);
+  auto* s_hdr = reinterpret_cast<ForBlockDev*>(base);
+  auto* s_nw = reinterpret_cast<unsigned long long*>(base + h_bytes);
+  auto* s_off = reinterpret_cast<unsigned long long*>(base + h_bytes + n_bytes);
+  CU(c, cudaMemsetAsync(s_nw + n_groups, 0, 8, c->stream));
+  const auto* raw = static_cast<const long long*>(c->stage_raw.p);
+  const unsigned grid = grid_per_group_warp(c, n_groups);
+  for_stats_kernel<<<grid, 256, 0, c->stream>>>(raw, nullptr, nullptr, rows, col.d_zone, s_hdr, s_nw);
+  col.zone_ok = true;
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  CU(c, cub::DeviceScan::ExclusiveSum(base + h_bytes + 2 * n_bytes, scan_bytes, s_nw, s_off, int(n_groups + 1), c->stream));
+  unsigned long long total = 0;
+  CU(c, cudaMemcpyAsync(&total, s_off + n_groups, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  const size_t packed_bytes = for_hdr_bytes(rows) + (total + 1) * 8 + 64;   // + the writer's slack word + 64 B of slack
+  if (packed_bytes >= rows * 8) return keep_raw();               // not smaller (e.g. full 64-bit hashes): stays raw
+  if (col.d_packed && col.packed_bytes != packed_bytes) { cudaFree(col.d_packed); col.d_packed = nullptr; }
+  if (!col.d_packed) CU(c, cudaMalloc(&col.d_packed, packed_bytes));
+  col.packed_bytes = packed_bytes;
+  CU(c, cudaMemsetAsync(static_cast<char*>(col.d_packed) + packed_bytes - 64, 0, 64, c->stream));
+  for_pack_kernel<<<grid, 256, 0, c->stream>>>(raw, s_hdr, s_off, rows, static_cast<ForBlockDev*>(col.d_packed),
+                                               const_cast<unsigned long long*>(for_words(col)));
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  return SDBG_OK;
+}
+
+// Resets `col` for a restaged owned int64 column of `rows` rows. A column of the same length keeps its packed and zonemap
+// allocations for pack_column to reuse, so restaging allocates and frees nothing (a cudaFree would wait for the device).
+void reset_for_packing(ColumnObj& col, uint64_t rows) {
+  void* keep = nullptr;
+  long long* zone = nullptr;
+  size_t keep_bytes = 0;
+  if (col.owned && col.rows == rows) {
+    keep = col.d_packed; keep_bytes = col.packed_bytes; zone = col.d_zone;
+    col.d_packed = nullptr; col.d_zone = nullptr;
+  }
+  free_column(col);
+  col = ColumnObj{};
+  col.type = SDBG_I64; col.rows = rows; col.owned = true;
+  col.d_packed = keep; col.packed_bytes = keep_bytes; col.d_zone = zone;
+}
+}  // namespace
 
 extern "C" int sdbg_stage_column(sdbg_segment* s, uint64_t field, sdbg_type t, const void* values,
                                  const uint64_t* validity, uint64_t rows) {
@@ -481,12 +588,21 @@ extern "C" int sdbg_stage_column(sdbg_segment* s, uint64_t field, sdbg_type t, c
   CU(c, cudaSetDevice(c->device));
   ColumnObj& col = s->cols[field];
   const size_t bytes = rows * type_width(t);
-  if (!(col.owned && col.d_values && col.rows == rows && col.type == t)) {
+  if (t == SDBG_I64 && !validity && rows) {   // NOT NULL int64: packed on the device when that is smaller
+    int rc;
+    if ((rc = ensure(c, c->stage_raw, bytes + 64))) return rc;
+    reset_for_packing(col, rows);
+    CU(c, cudaMemsetAsync(static_cast<char*>(c->stage_raw.p) + bytes, 0, 64, c->stream));
+    CU(c, cudaMemcpyAsync(c->stage_raw.p, values, bytes, cudaMemcpyHostToDevice, c->stream));
+    return pack_column(c, col);
+  }
+  if (col.d_packed || !(col.owned && col.d_values && col.rows == rows && col.type == t)) {
     free_column(col);
     col = ColumnObj{};
     CU(c, cudaMalloc(&col.d_values, bytes + 64));  // slack: row pairs are loaded as one 16-byte vector
     CU(c, cudaMemsetAsync(static_cast<char*>(col.d_values) + bytes, 0, 64, c->stream));
   }
+  col.zone_ok = false;   // new values: the zonemap is built again on first use (into the same allocation)
   col.type = t; col.rows = rows; col.owned = true; col.has_minmax = false; col.has_absmax = false;
   CU(c, cudaMemcpyAsync(col.d_values, values, bytes, cudaMemcpyHostToDevice, c->stream));
   if (validity) {
@@ -572,7 +688,31 @@ extern "C" int sdbg_stage_column_for(sdbg_segment* s, uint64_t field, const sdbg
   }
   ColumnObj& col = s->cols[field];
   const size_t bytes = rows * 8;
-  if (!(col.owned && col.d_values && col.rows == rows && col.type == SDBG_I64)) {
+  // The caller's stream is kept as the column's storage when every group starts 16-byte aligned (what sdbg_pack_for
+  // writes) and it is smaller than the raw column; otherwise it is decoded to raw values.
+  bool aligned = rows < (1ull << 32);
+  for (uint64_t g = 0; g < n_groups && aligned; ++g) aligned = (headers[g].off8 & 1u) == 0u;
+  const size_t packed_bytes = for_hdr_bytes(rows) + n_words * 8 + 64;
+  if (aligned && packed_bytes < bytes) {
+    if (!(col.d_packed && col.packed_bytes == packed_bytes && col.rows == rows && !col.d_values && col.d_zone)) {   // else: same shape, reused
+      free_column(col);
+      col = ColumnObj{};
+      col.rows = rows; col.packed_bytes = packed_bytes;
+      CU(c, cudaMalloc(&col.d_packed, packed_bytes));
+    }
+    col.type = SDBG_I64; col.rows = rows; col.owned = true; col.has_minmax = false; col.has_absmax = false;
+    CU(c, cudaMemcpyAsync(col.d_packed, headers, n_groups * sizeof(ForBlockDev), cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(const_cast<unsigned long long*>(for_words(col)), words, n_words * 8, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemsetAsync(static_cast<char*>(col.d_packed) + packed_bytes - 64, 0, 64, c->stream));
+    { int rc = ensure_zone(c, col); if (rc) return rc; }
+    col.zone_ok = true;
+    for_stats_kernel<<<grid_per_group_warp(c, n_groups), 256, 0, c->stream>>>(nullptr, for_headers(col), for_words(col), rows, col.d_zone,
+                                                                              nullptr, nullptr);
+    ++c->launches;
+    CU(c, cudaGetLastError());
+    return SDBG_OK;   // asynchronous on the context stream, like sdbg_stage_column
+  }
+  if (col.d_packed || !(col.owned && col.d_values && col.rows == rows && col.type == SDBG_I64)) {
     free_column(col);
     col = ColumnObj{};
     CU(c, cudaMalloc(&col.d_values, bytes + 64));
@@ -580,7 +720,7 @@ extern "C" int sdbg_stage_column_for(sdbg_segment* s, uint64_t field, const sdbg
   }
   if (col.d_validity) { cudaFree(col.d_validity); col.d_validity = nullptr; }
   col.type = SDBG_I64; col.rows = rows; col.owned = true; col.has_minmax = false; col.has_absmax = false;
-  if (col.d_zone) { cudaFree(col.d_zone); col.d_zone = nullptr; }
+  col.zone_ok = false;
   DevBuf& buf = c->scratch[12];
   const size_t hdr_bytes = (n_groups * sizeof(ForBlockDev) + 255) & ~size_t(255);
   int rc = ensure(c, buf, hdr_bytes + n_words * 8);
@@ -611,8 +751,31 @@ extern "C" int sdbg_column_device_ptr(sdbg_segment* s, uint64_t field, void** d_
   if (!s) return SDBG_EINVAL;
   auto it = s->cols.find(field);
   if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "unknown column");
-  if (d_values) *d_values = it->second.d_values;
+  CU(s->ctx, cudaSetDevice(s->ctx->device));
+  void* p = nullptr;
+  const int rc = raw_values(s->ctx, it->second, &p);
+  if (rc) return rc;
+  if (d_values) *d_values = p;
   if (rows) *rows = it->second.rows;
+  return SDBG_OK;
+}
+
+extern "C" int sdbg_column_for_to_host(sdbg_segment* s, uint64_t field, sdbg_for_block* headers, uint64_t* words, uint64_t cap_words,
+                                       uint64_t* n_words) {
+  if (!s || !n_words) return SDBG_EINVAL;
+  auto it = s->cols.find(field);
+  if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "unknown column");
+  const ColumnObj& col = it->second;
+  *n_words = 0;
+  if (!col.d_packed) return SDBG_OK;                             // held raw
+  const uint64_t n = (col.packed_bytes - for_hdr_bytes(col.rows) - 64) / 8;
+  *n_words = n;
+  if (n > cap_words || !headers || !words) return SDBG_ECAPACITY;
+  sdbg_ctx* c = s->ctx;
+  CU(c, cudaSetDevice(c->device));
+  CU(c, cudaMemcpyAsync(headers, col.d_packed, for_groups(col.rows) * sizeof(ForBlockDev), cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaMemcpyAsync(words, for_words(col), n * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
   return SDBG_OK;
 }
 
@@ -623,7 +786,10 @@ extern "C" int sdbg_column_to_host(sdbg_segment* s, uint64_t field, void* host_d
   if (rows > it->second.rows) return fail(s->ctx, SDBG_EINVAL, "more rows requested than staged");
   sdbg_ctx* c = s->ctx;
   CU(c, cudaSetDevice(c->device));
-  CU(c, cudaMemcpyAsync(host_dst, it->second.d_values, rows * type_width(it->second.type), cudaMemcpyDeviceToHost, c->stream));
+  void* src = nullptr;
+  const int rc = raw_values(c, it->second, &src);
+  if (rc) return rc;
+  CU(c, cudaMemcpyAsync(host_dst, src, rows * type_width(it->second.type), cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
   return SDBG_OK;
 }
@@ -637,12 +803,14 @@ extern "C" int sdbg_gather_column(sdbg_segment* s, uint64_t field, const uint32_
   if (it == s->cols.end()) return fail(c, SDBG_ENOTFOUND, "unknown column");
   if (!n) return SDBG_OK;
   CU(c, cudaSetDevice(c->device));
-  const ColumnObj& co = it->second;
+  ColumnObj& co = it->second;
+  void* raw = nullptr;
+  int rc = raw_values(c, co, &raw);
+  if (rc) return rc;
   const size_t w = type_width(co.type);
   const size_t docs_bytes = (n * 4 + 255) & ~size_t(255), val_bytes = (n * w + 255) & ~size_t(255);
   DevBuf& buf = c->scratch[12];
-  int rc = ensure(c, buf, docs_bytes + val_bytes + n);
-  if (rc) return rc;
+  if ((rc = ensure(c, buf, docs_bytes + val_bytes + n))) return rc;
   char* base = static_cast<char*>(buf.p);
   auto* d_docs = reinterpret_cast<uint32_t*>(base);
   void* d_out = base + docs_bytes;
@@ -650,8 +818,8 @@ extern "C" int sdbg_gather_column(sdbg_segment* s, uint64_t field, const uint32_
   CU(c, cudaMemcpyAsync(d_docs, docs, n * 4, cudaMemcpyHostToDevice, c->stream));
   const unsigned grid = unsigned(std::min<size_t>((n + 255) / 256, size_t(c->sm_count) * 8));
   const auto* valid = reinterpret_cast<const unsigned long long*>(co.d_validity);
-  if (w == 4) gather_rows_kernel<uint32_t><<<grid, 256, 0, c->stream>>>(static_cast<const uint32_t*>(co.d_values), valid, d_docs, n, co.rows, static_cast<uint32_t*>(d_out), out_valid ? d_valid : nullptr);
-  else gather_rows_kernel<unsigned long long><<<grid, 256, 0, c->stream>>>(static_cast<const unsigned long long*>(co.d_values), valid, d_docs, n, co.rows, static_cast<unsigned long long*>(d_out), out_valid ? d_valid : nullptr);
+  if (w == 4) gather_rows_kernel<uint32_t><<<grid, 256, 0, c->stream>>>(static_cast<const uint32_t*>(raw), valid, d_docs, n, co.rows, static_cast<uint32_t*>(d_out), out_valid ? d_valid : nullptr);
+  else gather_rows_kernel<unsigned long long><<<grid, 256, 0, c->stream>>>(static_cast<const unsigned long long*>(raw), valid, d_docs, n, co.rows, static_cast<unsigned long long*>(d_out), out_valid ? d_valid : nullptr);
   ++c->launches;
   CU(c, cudaGetLastError());
   CU(c, cudaMemcpyAsync(out_values, d_out, n * w, cudaMemcpyDeviceToHost, c->stream));
@@ -701,7 +869,10 @@ int filter_view(sdbg_segment* s, const sdbg_col_pred* f, FilterDev* out) {
   auto it = s->cols.find(f->field);
   if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "filter column not staged");
   if (it->second.rows < s->n_docs) return fail(s->ctx, SDBG_EINVAL, "filter column shorter than segment");
-  out->values = it->second.d_values; out->validity = it->second.d_validity; out->type = it->second.type;
+  void* raw = nullptr;
+  const int rc = raw_values(s->ctx, it->second, &raw);
+  if (rc) return rc;
+  out->values = raw; out->validity = it->second.d_validity; out->type = it->second.type;
   out->op = f->op; out->lo_i = f->lo_i; out->hi_i = f->hi_i; out->lo_f = f->lo_f; out->hi_f = f->hi_f;
   return SDBG_OK;
 }
@@ -1888,21 +2059,26 @@ extern "C" int sdbg_decode_score_term(sdbg_segment* s, uint32_t term, float c0, 
 // ------------------------------------------------------------------------------------------
 namespace {
 
-int col_view(sdbg_segment* s, uint64_t field, ColDev* out, uint64_t* rows) {
+// packed_ok: a packed column is described as {values = its d_packed block, type = kTypeFor} (for the TMA GROUP BY);
+// otherwise every column is described by its raw values.
+int col_view(sdbg_segment* s, uint64_t field, ColDev* out, uint64_t* rows, bool packed_ok = false) {
   auto it = s->cols.find(field);
   if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "column " + std::to_string(field) + " not staged");
-  out->values = it->second.d_values; out->validity = it->second.d_validity; out->type = it->second.type; out->pad = 0;
-  if (rows) *rows = it->second.rows;
+  ColumnObj& col = it->second;
+  out->validity = col.d_validity; out->type = col.type; out->pad = 0;
+  if (packed_ok && col.d_packed) { out->values = col.d_packed; out->type = kTypeFor; }
+  else { const int rc = raw_values(s->ctx, col, const_cast<void**>(&out->values)); if (rc) return rc; }
+  if (rows) *rows = col.rows;
   return SDBG_OK;
 }
 
-int pred_set(sdbg_segment* s, const sdbg_col_pred* preds, size_t n, PredSet* ps, uint64_t* rows) {
+int pred_set(sdbg_segment* s, const sdbg_col_pred* preds, size_t n, PredSet* ps, uint64_t* rows, bool packed_ok = false) {
   if (n > size_t(kMaxPreds)) return fail(s->ctx, SDBG_EUNSUPPORTED, "more than 4 pushed predicates");
   std::memset(ps, 0, sizeof *ps);
   ps->n = int(n);
   for (size_t i = 0; i < n; ++i) {
     uint64_t r = 0;
-    const int rc = col_view(s, preds[i].field, &ps->p[i].col, &r);
+    const int rc = col_view(s, preds[i].field, &ps->p[i].col, &r, packed_ok);
     if (rc) return rc;
     if (*rows == 0) *rows = r;
     if (r != *rows) return fail(s->ctx, SDBG_EINVAL, "columns of one segment differ in length");
@@ -1925,8 +2101,12 @@ int column_minmax(sdbg_segment* s, uint64_t field, int64_t* mn, int64_t* mx) {
     if ((rc = ensure(c, c->scratch[10], 16))) return rc;
     const long long init[2] = {INT64_MAX, INT64_MIN};
     CU(c, cudaMemcpyAsync(c->scratch[10].p, init, 16, cudaMemcpyHostToDevice, c->stream));
-    ColDev cd; cd.values = col.d_values; cd.validity = col.d_validity; cd.type = col.type; cd.pad = 0;
-    minmax_i64_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(cd, col.rows, static_cast<long long*>(c->scratch[10].p));
+    // a packed column's min / max are those of its zonemap entries (filled at staging): no raw view needed
+    ColDev cd; cd.validity = col.d_validity; cd.type = col.type; cd.pad = 0;
+    uint64_t n = col.rows;
+    if (col.d_packed) { cd.values = col.d_zone; n = 2 * for_groups(col.rows); }
+    else cd.values = col.d_values;
+    minmax_i64_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(cd, n, static_cast<long long*>(c->scratch[10].p));
     ++c->launches;
     CU(c, cudaGetLastError());
     long long res[2];
@@ -2154,18 +2334,25 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
   // All accumulators integer => the four words of a slot go out as one RED request per passing row.
   plan.quad = all_tma && (avg_f64_field == UINT64_MAX || plan.fix_limb) && env_int("SDBG_GROUPBY_QUAD", 0);
   if (!plan.quad) plan.fix_limb = 0, plan.fix_eunit = 0;            // separate REDs: one f64 RED beats two integer ones
+  const int shape = env_int("SDBG_GROUPBY_TMA_SHAPE", 0);
   for (size_t si = 0; si < n_segs; ++si) {
     sdbg_segment* s = segs[si];
+    // Packed columns are read packed by the default-shape TMA kernel, which takes segments without nullable columns;
+    // every other path reads their raw view.
+    auto nullable = [&](uint64_t f) { auto it = s->cols.find(f); return it != s->cols.end() && it->second.d_validity != nullptr; };
+    bool packed_ok = env_int("SDBG_GROUPBY_TMA", 1) != 0 && shape == 0 && !nullable(key_field) &&
+                     (sum_int_field == UINT64_MAX || !nullable(sum_int_field)) && (avg_f64_field == UINT64_MAX || !nullable(avg_f64_field));
+    for (size_t i = 0; i < n_preds; ++i) packed_ok = packed_ok && preds[i].op < 7 && !nullable(preds[i].field);
     GroupByParams P;
     std::memset(&P, 0, sizeof P);
     uint64_t rows = 0;
-    if ((rc = pred_set(s, preds, n_preds, &P.ps, &rows))) return rc;
+    if ((rc = pred_set(s, preds, n_preds, &P.ps, &rows, packed_ok))) return rc;
     uint64_t r = 0;
-    if ((rc = col_view(s, key_field, &P.key, &r))) return rc;
+    if ((rc = col_view(s, key_field, &P.key, &r, packed_ok))) return rc;
     if (!rows) rows = r;
     if (r != rows) return fail(c, SDBG_EINVAL, "key column length differs");
     if (sum_int_field != UINT64_MAX) {
-      if ((rc = col_view(s, sum_int_field, &P.sum_i, &r))) return rc;
+      if ((rc = col_view(s, sum_int_field, &P.sum_i, &r, packed_ok))) return rc;
       if (r != rows) return fail(c, SDBG_EINVAL, "sum_int column length differs");
       if (P.sum_i.type == SDBG_F64) return fail(c, SDBG_EINVAL, "sum_int_field is a float column");
       P.has_sum_i = 1;
@@ -2187,10 +2374,24 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
     if (!any_nullable && env_int("SDBG_GROUPBY_TMA", 1)) {
       TmaGroupByParams T;
       std::memset(&T, 0, sizeof T);
+      // the column a stream comes from: its raw values or, for kTypeFor, its packed block
+      auto column_of = [&](const void* id) -> ColumnObj* {
+        for (auto& kv : s->cols) if (kv.second.d_values == id || (id && kv.second.d_packed == id)) return &kv.second;
+        return nullptr;
+      };
+      const void* stream_id[kMaxStreams] = {};
       auto stream_of = [&](const ColDev& col) {
-        for (int i = 0; i < T.n_streams; ++i) if (T.src[i] == col.values) return i;
-        T.src[T.n_streams] = col.values; T.elem[T.n_streams] = col.type == SDBG_I32 ? 4 : 8;
-        return T.n_streams++;
+        for (int i = 0; i < T.n_streams; ++i) if (stream_id[i] == col.values) return i;
+        const int n = T.n_streams++;
+        stream_id[n] = col.values;
+        T.elem[n] = col.type == SDBG_I32 ? 4 : 8;
+        if (col.type == kTypeFor) {
+          T.hdr[n] = static_cast<const ForBlockDev*>(col.values);
+          T.src[n] = static_cast<const char*>(col.values) + for_hdr_bytes(rows);
+        } else {
+          T.src[n] = col.values;
+        }
+        return n;
       };
       // Every comparison becomes a closed range [lo, lo + span] in an int64 key space (integers as they
       // are, doubles through fkey()): exact, because integers step by 1 and doubles by one ulp. Predicates
@@ -2254,11 +2455,11 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
         bool any_zone = false;
         for (int k2 = 0; k2 < T.n_preds; ++k2) {
           Z.lo[k2] = T.pred_lo[k2]; Z.span[k2] = T.pred_span[k2]; Z.negate[k2] = T.pred_negate[k2];
-          ColumnObj* co = nullptr;
-          for (auto& kv : s->cols) if (kv.second.d_values == T.src[stream_idx[k2]]) { co = &kv.second; break; }
+          ColumnObj* co = column_of(stream_id[stream_idx[k2]]);
           if (!co || co->d_validity) continue;
-          if (!co->d_zone) {
-            CU(c, cudaMalloc(reinterpret_cast<void**>(&co->d_zone), Z.n_blocks * 16));
+          if (!co->zone_ok) {
+            if (!co->d_zone) CU(c, cudaMalloc(reinterpret_cast<void**>(&co->d_zone), Z.n_blocks * 16));
+            co->zone_ok = true;
             const unsigned zg = unsigned(std::min<uint64_t>((Z.n_blocks + 7) / 8, uint64_t(c->sm_count) * 8));
             const auto* vals = static_cast<const unsigned char*>(co->d_values);
             if (co->type == SDBG_F64) zonemap_kernel<1><<<zg, 256, 0, c->stream>>>(vals, rows, co->d_zone);
@@ -2290,7 +2491,13 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
       T.wide_int = plan.wide_int; T.key_min = key_min; T.key_span = span; T.rows = rows; T.table = table; T.out_of_range = oor;
       T.pack_shift = plan.pack_shift; T.pack_tables = plan.pack_tables; T.pack_bias = plan.pack_bias;
       T.fix_limb = plan.fix_limb; T.fix_eunit = plan.fix_eunit;
-      auto set_offsets = [&](int tile_rows) {   // stream offsets inside a stage depend on the tile shape
+      for (int i = 0; i < T.n_preds; ++i) T.pred_stream[i] = stream_idx[i];
+      T.key_stream = key_s; T.sum_i_stream = sum_i_s >= 0 ? sum_i_s : 0;
+      bool any_for = false;
+      for (int i = 0; i < T.n_streams; ++i) any_for |= T.hdr[i] != nullptr;
+      // Stream offsets inside a stage depend on the tile shape. A packed stream keeps its raw slot size, so the
+      // shared-memory footprint, ring depth and CTAs per SM are those of the raw scan.
+      auto set_offsets = [&](int tile_rows) {
         uint32_t o = 0;
         for (int i = 0; i < T.n_streams; ++i) { T.off[i] = o; o += uint32_t(T.elem[i]) * uint32_t(tile_rows); }
         T.off[T.n_streams] = o;
@@ -2299,15 +2506,17 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
         T.sum_i_off = sum_i_s >= 0 ? T.off[sum_i_s] : 0;
         T.sum_f_off = sum_f_s >= 0 ? T.off[sum_f_s] : 0;
       };
-      const int shape = env_int("SDBG_GROUPBY_TMA_SHAPE", 0);
       const bool quad = plan.quad != 0;
       auto launch = [&](auto kern, int stages, int tile_rows, int consumer_warps) -> int {
         set_offsets(tile_rows);
-        const size_t smem = size_t(stages) * size_t(T.off[T.n_streams]) + (quad ? size_t(consumer_warps) * (2048 + 256) : 0);
+        const size_t smem = size_t(stages) * size_t(T.off[T.n_streams]) + (quad ? size_t(consumer_warps) * (2048 + 256) : 0) +
+                            (any_for ? size_t(stages) * kMaxStreams * 16 : 0);
         CU(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
         const size_t fit = std::max<size_t>(1, (220 * 1024) / (smem + 2048));
         const size_t by_threads = std::max<size_t>(1, 2048 / (size_t(consumer_warps + 1) * 32));
-        const unsigned per_sm = unsigned(std::min<size_t>(std::min(fit, by_threads), size_t(env_int("SDBG_GROUPBY_TMA_CTAS", 8))));
+        int resident = 0;   // persistent CTAs: never more per SM than can be resident at once (registers included)
+        CU(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, (consumer_warps + 1) * 32, smem));
+        const unsigned per_sm = unsigned(std::max<size_t>(1, std::min<size_t>({fit, by_threads, size_t(env_int("SDBG_GROUPBY_TMA_CTAS", 8)), size_t(resident)})));
         const unsigned grid = unsigned(c->sm_count) * per_sm;
         ProfScope ps_(c, kProfGroupBy);
         kern<<<grid, (consumer_warps + 1) * 32, smem, c->stream>>>(T);
@@ -2322,13 +2531,14 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
         default: {
           // default shape: 512-row tiles, 8 consumer warps; ring depth by SDBG_GROUPBY_TMA_STAGES (the CTAs per
           // SM follow from the shared-memory footprint, so fewer stages = more resident consumer warps)
+#define SDBG_GB_LAUNCH(ST, FOR) \
+          (plan.pack_tables ? (quad ? launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, true, true, FOR>, ST, kGroupByTileRows, 8) \
+                                    : launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, true, false, FOR>, ST, kGroupByTileRows, 8)) \
+                            : (quad ? launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, false, true, FOR>, ST, kGroupByTileRows, 8) \
+                                    : launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, false, false, FOR>, ST, kGroupByTileRows, 8)))
           const int stages = env_int("SDBG_GROUPBY_TMA_STAGES", kGroupByDefaultStages);
-#define SDBG_GB_LAUNCH(ST) \
-          (plan.pack_tables ? (quad ? launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, true, true>, ST, kGroupByTileRows, 8) \
-                                    : launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, true, false>, ST, kGroupByTileRows, 8)) \
-                            : (quad ? launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, false, true>, ST, kGroupByTileRows, 8) \
-                                    : launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, false, false>, ST, kGroupByTileRows, 8)))
-          lrc = stages == 2 ? SDBG_GB_LAUNCH(2) : stages == 3 ? SDBG_GB_LAUNCH(3) : SDBG_GB_LAUNCH(4);
+          if (any_for) lrc = stages == 2 ? SDBG_GB_LAUNCH(2, true) : stages == 3 ? SDBG_GB_LAUNCH(3, true) : SDBG_GB_LAUNCH(4, true);
+          else lrc = stages == 2 ? SDBG_GB_LAUNCH(2, false) : stages == 3 ? SDBG_GB_LAUNCH(3, false) : SDBG_GB_LAUNCH(4, false);
 #undef SDBG_GB_LAUNCH
           break;
         }
@@ -2792,9 +3002,19 @@ extern "C" int sdbg_synth_column(sdbg_segment* seg, uint64_t field, uint64_t str
   CU(c, cudaSetDevice(c->device));
   const int type = (kind == 2 || kind == 4) ? SDBG_F64 : (kind == 6 ? SDBG_I32 : SDBG_I64);
   ColumnObj& col = seg->cols[field];
+  const size_t bytes = rows * type_width(type);
+  if (type == SDBG_I64) {   // generated into the staging buffer, then packed when that is smaller
+    int rc;
+    if ((rc = ensure(c, c->stage_raw, bytes + 64))) return rc;
+    reset_for_packing(col, rows);
+    CU(c, cudaMemsetAsync(static_cast<char*>(c->stage_raw.p) + bytes, 0, 64, c->stream));
+    synth_column_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(stream, kind, row0, rows, c->stage_raw.p);
+    ++c->launches;
+    CU(c, cudaGetLastError());
+    return pack_column(c, col);
+  }
   free_column(col);
   col = ColumnObj{};
-  const size_t bytes = rows * type_width(type);
   CU(c, cudaMalloc(&col.d_values, bytes + 64));
   CU(c, cudaMemsetAsync(static_cast<char*>(col.d_values) + bytes, 0, 64, c->stream));
   col.type = type; col.rows = rows; col.owned = true;

@@ -294,6 +294,19 @@ class Segment:
     def column_to_host(self, field, host_ptr, rows):
         N.check(N.lib().sdbg_column_to_host(self._h, int(field), C.c_void_p(int(host_ptr)), int(rows)), self.ctx._h)
 
+    def column_packed(self, field, rows):
+        """The staged column's bit-packed storage as (headers, words) in pack_for's format, or None when it is held raw."""
+        n = C.c_uint64(0)
+        rc = N.lib().sdbg_column_for_to_host(self._h, int(field), None, None, 0, C.byref(n))
+        if rc != -6 and rc != 0:   # -6: SDBG_ECAPACITY, *n = the words needed
+            N.check(rc, self.ctx._h)
+        if n.value == 0:
+            return None
+        headers = np.zeros((int(rows) + 2047) // 2048, FOR_BLOCK_DTYPE)
+        words = np.zeros(n.value, np.uint64)
+        N.check(N.lib().sdbg_column_for_to_host(self._h, int(field), _ptr(headers), _ptr(words), n.value, C.byref(n)), self.ctx._h)
+        return headers, words
+
     def synth_corpus(self, doc0, t0, nt, threads=8, p_floor=0.0):
         """SURVEY §8d corpus shard: returns (docs_count per term, sum of doc lengths). p_floor > 0 gives every term at
         least that inclusion probability (a flat tail: an index far larger than L2)."""
