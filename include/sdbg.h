@@ -110,7 +110,9 @@ int sdbg_segment_set_wand_b(sdbg_segment*, float wand_b);
    that used another average needs this; call it after sdbg_stage_norms. 0 = no norms. Queries score the entries as upper
    bounds under their own (corpus-wide) average length, so pruning stays exact when the two averages differ. */
 int sdbg_segment_set_wand_avg_dl(sdbg_segment*, float avg_dl);
-/* Zonemap effect of the last GROUP BY scan: 2048-row blocks judged / proven dead from their min-max (never read). */
+/* Zonemap effect of the last GROUP BY or sorted scan. GROUP BY: 2048-row blocks judged / proven dead from their min-max
+ * (never read). Sorted scan (sdbg_match_topk_by_column_batch): 65 536-doc windows judged / skipped before any list was
+ * decoded. */
 int sdbg_scan_stats(sdbg_ctx*, uint64_t* blocks_total, uint64_t* blocks_skipped);
 /* The context a segment was created in (for sdbg_last_error after a failed call that only has segments at hand). */
 sdbg_ctx* sdbg_segment_context(const sdbg_segment*);
@@ -219,6 +221,28 @@ int sdbg_bm25_scan_excl(sdbg_segment*, int kind, const sdbg_bm25_term* terms, si
 int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
                            const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms,
                            const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts);
+/* Sorted scan (SELECT ... WHERE body @@ '...' [AND <pushed filter>] ORDER BY col [DESC] [NULLS FIRST|LAST] LIMIT k): per
+ * query, the k first of the docs sdbg_match_count_batch counts for it, ordered by column `sort_field` (staged in every
+ * segment with one type: int64 raw or bit-packed, int32 or float64; NOT NULL or nullable; row = doc - 1, and a doc past
+ * the column's rows is NULL). Values ascend (descending = 0) or descend; NULLs all come first (nulls_first = 1) or last;
+ * ties, NULLs included, go by (segment index asc, doc asc). float64: -0.0 equals +0.0, every NaN equals every NaN and
+ * sorts above +inf. out[q * k .. q * k + n_out[q]) holds n_out[q] = min(k, matches) hits in that order: the stored value
+ * bit for bit (int32 sign-extended, float64 as its bits; 0 for NULL), doc, segment index and a NULL flag. Identical at
+ * every pruning level; levels 1 and 2 skip matches, and (NOT NULL sort columns) whole 65 536-doc windows, that the
+ * zonemap shows cannot beat the k-th value found so far (sdbg_scan_stats: windows judged / skipped).
+ * Errors: those of sdbg_match_count_batch; k == 0, NULL out or n_out, or a sort column whose type differs between
+ * segments: SDBG_EINVAL; a segment without the sort column: SDBG_ENOTFOUND; k > 4096: SDBG_EUNSUPPORTED (each CTA keeps
+ * 2 * next_pow2(k) 16-byte candidate keys in shared memory). Synchronous on the context's stream.
+ * Device scratch: k keys of 16 B per work item before the per-query merge, where a work item is a range of 65 536-doc
+ * windows of one query in one segment (at least one per query and segment holding a match, at most 2 x SMs), plus
+ * n_queries * k * 24 B of hits: 4096 queries x 1 segment x 1 item at k = 1000 take 66 MB; k = 4096 over 20 segments
+ * with one item each takes 5.4 GB. Split larger batches. */
+typedef struct { int64_t value; uint32_t doc; uint32_t seg; uint8_t is_null; } sdbg_sort_hit;
+int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
+                                    const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms,
+                                    const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                                    uint64_t sort_field, int descending, int nulls_first, uint32_t k,
+                                    sdbg_sort_hit* out /* n_queries * k */, uint32_t* n_out);
 /* Conjunctions of OR groups (`a & (b | c) & !d`: an And whose children are terms, Ors of terms and Nots of terms, as
  * synonym expansion and query rewriting produce). Query q is the AND of the groups [query_group_off[q],
  * query_group_off[q+1]) (1..16), group g the OR of terms[group_off[g] .. group_off[g+1]) (non-empty); its positive terms

@@ -21,6 +21,7 @@
 #pragma once
 
 #include "bm25_kernels.cuh"
+#include "bm25_sort.cuh"
 
 namespace sdbg {
 
@@ -47,6 +48,7 @@ struct CountParams {
   uint32_t n_pos;               // term_off[n_queries]
   const uint4* work;            // {query, first window, windows, 0}
   unsigned long long* counts;   // per query, summed over items and segments
+  SortSink sort;                // kSort: the sorted scan's sink (work item .w = its output slot)
 };
 
 __device__ __forceinline__ uint32_t warp_min(uint32_t v) {
@@ -120,9 +122,16 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
 
 // kAnd: conjunction (else disjunction). kGroups: conjunction of OR groups (CountParams::grp_end). The term loops are not
 // unrolled: 1..16 terms share one instantiation.
-template <bool kAnd, bool kGroups = false>
+// kSort: the sorted scan (bm25_sort.cuh). Instead of popcounting, every surviving doc's sort key enters a buffer of
+// P.sort.cap keys in dynamic shared memory; a full buffer is sorted and cut to the k best, whose k-th hi raises the
+// query's threshold word. With a threshold word (pruning level >= 1), a key whose hi is below the threshold never enters,
+// and with a zonemap each window is judged before any list is decoded: a window none of whose zones can reach the
+// threshold is skipped, and in a kept window the docs of such zones are cleared before the column is read. The item's
+// k best go to output slot item.w.
+template <bool kAnd, bool kGroups = false, bool kSort = false>
 __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
   static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
+  static_assert(!(kSort && kGroups), "the sorted scan takes OR / AND queries");
   __shared__ uint32_t acc[kCountWords];
   __shared__ uint32_t tmp[kAnd || kGroups ? kCountWords : 1];
   __shared__ uint32_t stage[kCountWarps][128];
@@ -134,6 +143,9 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   __shared__ uint32_t s_gend[kGroups ? kMaxQueryTerms : 1];
   __shared__ uint32_t s_ws, s_done;
   __shared__ unsigned long long s_sum[kCountWarps];
+  __shared__ unsigned long long s_thr[1];   // kSort: this item's best known k-th hi
+  __shared__ uint32_t s_fill[1], s_zmask[2];  // kSort: keys in the buffer; the window's zones that can reach s_thr
+  extern __shared__ unsigned long long sort_buf[];   // kSort: hi[cap] | lo[cap]
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint4 item = P.work[blockIdx.x];
@@ -156,6 +168,11 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   }
   unsigned long long count = 0;
   uint32_t ws = item.y << kCountWindowLog;              // start of the window being looked at
+  uint32_t judged = 0, skipped = 0;                     // kSort: windows judged / skipped by the zonemap
+  if constexpr (kSort) {
+    for (uint32_t i = tid; i < 2u * P.sort.cap; i += kCountThreads) sort_buf[i] = 0ull;
+    if (tid == 0) { s_thr[0] = 0ull; s_fill[0] = 0u; }
+  }
   __syncthreads();
   for (;;) {
     // ---- next window: the first possible doc of the lead lists' current blocks ----
@@ -171,6 +188,9 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       }
       s_done = (!any || (nxt >> kCountWindowLog) >= w_end) ? 1u : 0u;
       s_ws = (nxt >> kCountWindowLog) << kCountWindowLog;
+      if constexpr (kSort) {
+        if (P.sort.thr) s_thr[0] = max(s_thr[0], *reinterpret_cast<volatile unsigned long long*>(P.sort.thr + q));
+      }
     }
     __syncthreads();
     if (s_done) break;
@@ -187,8 +207,27 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       s_resume[tid] = 0u;
       s_end[tid] = (e < l.y && __ldg(&LB[e].z) < wlast) ? e + 1u : e;   // block e straddles the window's end
     }
+    // kSort with a zonemap: zones zb .. zb + 32 hold the window's rows ws - 1 .. ws + 65534 (32 zones for ws = 0)
+    const uint32_t zb = ws == 0u ? 0u : (ws >> 11) - 1u;
+    if constexpr (kSort) {
+      if (P.sort.zone && tid < 64u) {
+        const uint32_t nz = ws == 0u ? 32u : 33u;
+        const bool comp = tid < nz && sort_zone_bound(P.sort, zb + tid) >= s_thr[0];
+        const uint32_t m = __ballot_sync(kFull, comp);
+        if (lane == 0) s_zmask[warp] = m;
+      }
+    }
     for (uint32_t i = tid; i < kCountWords; i += kCountThreads) acc[i] = 0u;
     __syncthreads();
+    bool skip = false;
+    if constexpr (kSort) {
+      if (P.sort.zone) {
+        ++judged;
+        skip = (s_zmask[0] | s_zmask[1]) == 0u;
+        skipped += skip;
+      }
+    }
+    if (!skip) {
 
     // Blocks [s_cur, s_end) of lists [lo, hi) spread over the warps; `filter`: only blocks whose range holds a bit of acc.
     auto run_lists = [&](uint32_t lo, uint32_t hi, uint32_t* bm, bool clear, bool filter) {
@@ -236,7 +275,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       run_lists(n_pos, n_lists, acc, true, true);
       __syncthreads();
     }
-    if (live) {
+    if (live && !kSort) {
       const uint32_t wbase = ws >> 5;
       for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
         uint32_t v = acc[i];
@@ -250,9 +289,63 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
         count += __popc(v);
       }
     }
+    if constexpr (kSort) {
+      if (live) {
+        const uint32_t wbase = ws >> 5, cap = P.sort.cap;
+        unsigned long long* hi = sort_buf;
+        unsigned long long* lo = sort_buf + cap;
+        auto zone_ok = [&](uint32_t zr) { return (s_zmask[zr >> 5] >> (zr & 31u)) & 1u; };
+        for (uint32_t base = 0; base < kCountWords; base += kCountThreads) {   // uniform trip count
+          const uint32_t i = base + tid;
+          uint32_t v = acc[i];
+          if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
+          if (v && P.sort.zone) {   // bit 0 is row ws + 32i - 1, which starts a zone when ws + 32i does
+            const uint32_t d0 = ws + 32u * i;
+            uint32_t keep = zone_ok((d0 >> 11) - zb) ? 0xFFFFFFFEu : 0u;
+            if (d0 != 0u && zone_ok(((d0 - 1u) >> 11) - zb)) keep |= 1u;
+            v &= keep;
+          }
+          if (v && P.filt.values) {
+            for (uint32_t r = v; r; r &= r - 1u) {
+              const uint32_t bit = __ffs(r) - 1u;
+              if (!filter_pass(P.filt, ws + 32u * i + bit)) v &= ~(1u << bit);
+            }
+          }
+          for (;;) {   // a full buffer is cut to the k best and the remaining bits go on
+            const unsigned long long thr = s_thr[0];
+            for (; v; v &= v - 1u) {
+              const ulonglong2 key = sort_key(P.sort, ws + 32u * i + (__ffs(v) - 1u));
+              if (key.x < thr) continue;
+              const uint32_t slot = atomicAdd(&s_fill[0], 1u);
+              if (slot >= cap) break;
+              hi[slot] = key.x; lo[slot] = key.y;
+            }
+            if (!__syncthreads_or(v != 0u)) break;
+            const unsigned long long kth = sort_select(hi, lo, cap, P.sort.k, &s_fill[0]);
+            if (P.sort.thr && tid == 0 && kth > s_thr[0]) { s_thr[0] = kth; atomicMax(P.sort.thr + q, kth); }
+            __syncthreads();
+          }
+        }
+      }
+    }
+    }   // !skip
     __syncthreads();   // acc / tmp / cursors are rewritten by the next window
     if (wlast == 0xFFFFFFFFu || (wlast >> kCountWindowLog) + 1u >= w_end) break;
     ws = wlast + 1u;
+  }
+  if constexpr (kSort) {
+    unsigned long long* hi = sort_buf;
+    unsigned long long* lo = sort_buf + P.sort.cap;
+    const unsigned long long kth = sort_select(hi, lo, P.sort.cap, P.sort.k, &s_fill[0]);
+    const uint32_t n = s_fill[0];
+    ulonglong2* out = P.sort.out + size_t(item.w) * P.sort.k;
+    for (uint32_t i = tid; i < n; i += kCountThreads) out[i] = make_ulonglong2(hi[i], lo[i]);
+    if (tid == 0) {
+      P.sort.out_n[item.w] = n;
+      if (P.sort.thr && kth) atomicMax(P.sort.thr + q, kth);
+      if (judged) { atomicAdd(P.sort.stats, judged); if (skipped) atomicAdd(P.sort.stats + 1, skipped); }
+    }
+    return;
   }
   count = warp_sum64(count);
   if (lane == 0) s_sum[warp] = count;

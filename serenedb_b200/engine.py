@@ -213,6 +213,7 @@ class Segment:
         N.check(N.lib().sdbg_segment_create(ctx._h, self.n_docs, C.byref(self._h)), ctx._h)
         self.term_docs = None  # docs_count per term (filled by staging)
         self._keep = []        # host buffers that must outlive async copies
+        self.col_types = {}    # field -> sdbg_type of the staged column
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -260,6 +261,7 @@ class Segment:
             self._keep.append(validity)
             vv = _ptr(validity)
         N.check(N.lib().sdbg_stage_column(self._h, int(field), t, vp, vv, int(rows)), self.ctx._h)
+        self.col_types[int(field)] = t
 
     def stage_column_for(self, field, packed):
         """Stage an int64 column from its frame-of-reference bit-packed form (pack_for): only the packed bytes cross PCIe,
@@ -267,6 +269,7 @@ class Segment:
         headers, words, rows = packed
         self._keep.append(packed)
         N.check(N.lib().sdbg_stage_column_for(self._h, int(field), _ptr(headers), _ptr(words), len(words), int(rows)), self.ctx._h)
+        self.col_types[int(field)] = 0
 
     def stage_docs_mask(self, deleted_docs):
         """DocumentMask of the segment: doc ids that queries must neither score nor count (None / empty clears)."""
@@ -276,6 +279,7 @@ class Segment:
     def stage_column_device(self, field, device_ptr, dtype, rows):
         N.check(N.lib().sdbg_stage_column_device(self._h, int(field), TYPES[np.dtype(dtype)],
                                                  C.c_void_p(int(device_ptr)), int(rows)), self.ctx._h)
+        self.col_types[int(field)] = TYPES[np.dtype(dtype)]
 
     def column_device_ptr(self, field):
         p, r = C.c_void_p(), C.c_uint64()
@@ -320,6 +324,7 @@ class Segment:
     def synth_column(self, field, stream, kind, row0, rows):
         N.check(N.lib().sdbg_synth_column(self._h, int(field), int(stream), int(kind), int(row0), int(rows)),
                 self.ctx._h)
+        self.col_types[int(field)] = 1 if kind in (2, 4) else 2 if kind == 6 else 0
 
     def posting_stats(self):
         a, b, c, d = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_uint64()
@@ -477,6 +482,53 @@ def ExecuteCount(reader, query_terms, kind, filt=None, exclude=None):
     """ExecuteCountBatch for one query: its match count as an int."""
     return int(ExecuteCountBatch(reader, [list(query_terms)], kind, filt,
                                  exclude=None if exclude is None else [list(exclude)])[0])
+
+
+SORT_HIT_DTYPE = np.dtype([("value", "<i8"), ("doc", "<u4"), ("seg", "<u4"), ("is_null", "u1"), ("pad", "V7")])
+_SORT_VALUE_DTYPE = {0: np.int64, 1: np.float64, 2: np.int32}
+
+
+def ExecuteTopKByColumnBatch(reader, queries, kind, sort_field, k, descending=False, nulls_first=False, filt=None,
+                             exclude=None):
+    """Sorted scan (`WHERE body @@ '...' ORDER BY col [DESC] [NULLS FIRST] LIMIT k`, sdbg_match_topk_by_column_batch): per
+    query, the first k of the docs ExecuteCountBatch counts, ordered by column `sort_field` (int64 / int32 / float64,
+    staged in every segment); ties, NULLs included, by (segment, doc). Returns a dict of per-query arrays: docs, segs,
+    values (typed by the column; 0 for NULL), nulls (bool) and n_out (uint32[Q])."""
+    col_type = reader.segments[0].col_types.get(int(sort_field))
+    if col_type is None:   # the values come back as raw bits: their type must be known, not guessed
+        raise ValueError("sort column %d was not staged through this Segment" % int(sort_field))
+    nq = len(queries)
+    flat = np.ascontiguousarray([t for q in queries for t in q], dtype=np.uint32)
+    off = np.zeros(nq + 1, np.uint32)
+    off[1:] = np.cumsum([len(q) for q in queries])
+    hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
+    n_out = np.zeros(max(nq, 1), np.uint32)
+    x = _exclusions(exclude, nq)
+    fp = C.byref(filt) if filt is not None else None
+    N.check(N.lib().sdbg_match_topk_by_column_batch(_seg_array(reader.segments), len(reader.segments), int(kind),
+                                                    _ptr(flat) if len(flat) else None, _ptr(off), nq,
+                                                    _ptr(x[0]) if x is not None else None,
+                                                    _ptr(x[1]) if x is not None else None, fp, int(sort_field),
+                                                    int(bool(descending)), int(bool(nulls_first)), int(k), _ptr(hits),
+                                                    _ptr(n_out)), reader.segments[0].ctx._h)
+    vt = _SORT_VALUE_DTYPE[col_type]
+    out = dict(docs=[], segs=[], values=[], nulls=[], n_out=n_out[:nq])
+    for q in range(nq):
+        h = hits[q * k:q * k + int(n_out[q])]
+        raw = h["value"].copy()
+        out["values"].append(raw.view(np.float64) if vt is np.float64 else raw.astype(vt))
+        out["docs"].append(h["doc"].copy())
+        out["segs"].append(h["seg"].copy())
+        out["nulls"].append(h["is_null"].astype(bool))
+    return out
+
+
+def ExecuteTopKByColumn(reader, query_terms, kind, sort_field, k, descending=False, nulls_first=False, filt=None,
+                        exclude=None):
+    """ExecuteTopKByColumnBatch for one query: dict of docs, segs, values, nulls (arrays of n_out entries)."""
+    r = ExecuteTopKByColumnBatch(reader, [list(query_terms)], kind, sort_field, k, descending, nulls_first, filt,
+                                 exclude=None if exclude is None else [list(exclude)])
+    return dict(docs=r["docs"][0], segs=r["segs"][0], values=r["values"][0], nulls=r["nulls"][0])
 
 
 def _groups(queries):

@@ -3,7 +3,8 @@
 // for tests/test_gpu_adapters.py to compare with the oracle. Needs a GPU at run time. With a second argument "excl" it runs
 // only the exclusion case instead (an And with a Not child, tests/test_gpu_exclusion.py); with "count", only the Count
 // scan mode (GpuCountScan, tests/test_gpu_count.py); with "groups", only an And of Or groups through both adapters
-// (tests/test_gpu_groups.py).
+// (tests/test_gpu_groups.py); with "sorted", only the sorted scan (GpuSortedScan, tests/test_gpu_sort_by_column.py).
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -93,6 +94,47 @@ int main(int argc, char** argv) {
     int code = 0;   // k = 0 (the streaming scan) has no grouped form
     try { sdbg_host::GpuTopKIterator st(seg, SDBG_QUERY_OR, g3, 1.2f, 0.75f, 0, nullptr, {}, {1, 2}); } catch (const sdbg_host::GpuError& e) { code = e.code; }
     std::printf("{\"stream_error\": %d}\n", code);
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
+  if (argc > 2 && std::string(argv[2]) == "sorted") {
+    // `t2 | t5` and `(t2 | t5) & !t3` ORDER BY the int32 column 9, LIMIT 4096 (two chunks), every direction and NULL
+    // placement, without and with the table filter: every row in order, then end of scan
+    for (int with_filter = 0; with_filter < 2; ++with_filter)
+      for (int excl = 0; excl < 2; ++excl)
+        for (int desc = 0; desc < 2; ++desc)
+          for (int nf = 0; nf < 2; ++nf) {
+            sdbg_host::GpuSortedScan scan({seg}, SDBG_QUERY_OR, {2, 5}, excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{},
+                                          with_filter ? &filt : nullptr, 9, desc != 0, nf != 0, 4096);
+            duckdb::DataChunkMock chunk;
+            std::vector<uint32_t> docs, segs;
+            std::vector<int64_t> vals;
+            std::vector<uint8_t> valid;
+            uint64_t chunks = 0, max_chunk = 0;
+            for (;;) {
+              scan.Scan(chunk);
+              if (chunk.size == 0) break;
+              ++chunks;
+              max_chunk = std::max<uint64_t>(max_chunk, chunk.size);
+              docs.insert(docs.end(), chunk.doc.begin(), chunk.doc.end());
+              segs.insert(segs.end(), chunk.segment.begin(), chunk.segment.end());
+              vals.insert(vals.end(), chunk.value.begin(), chunk.value.end());
+              valid.insert(valid.end(), chunk.valid.begin(), chunk.valid.end());
+            }
+            scan.Scan(chunk);
+            std::printf("{\"filter\": %d, \"excl\": %d, \"desc\": %d, \"nulls_first\": %d, \"chunks\": %llu, \"max_chunk\": %llu, "
+                        "\"rows_after\": %llu, \"docs\": [", with_filter, excl, desc, nf, static_cast<unsigned long long>(chunks),
+                        static_cast<unsigned long long>(max_chunk), static_cast<unsigned long long>(chunk.size));
+            for (size_t i = 0; i < docs.size(); ++i) std::printf("%s%u", i ? ", " : "", docs[i]);
+            std::printf("], \"segs\": [");
+            for (size_t i = 0; i < segs.size(); ++i) std::printf("%s%u", i ? ", " : "", segs[i]);
+            std::printf("], \"values\": [");
+            for (size_t i = 0; i < vals.size(); ++i) std::printf("%s%lld", i ? ", " : "", static_cast<long long>(vals[i]));
+            std::printf("], \"valid\": [");
+            for (size_t i = 0; i < valid.size(); ++i) std::printf("%s%u", i ? ", " : "", unsigned(valid[i]));
+            std::printf("]}\n");
+          }
     sdbg_segment_destroy(seg);
     sdbg_destroy(ctx);
     return 0;

@@ -222,6 +222,41 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
   done_ = true;
 }
 
+GpuSortedScan::GpuSortedScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
+                             std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t sort_field,
+                             bool descending, bool nulls_first, uint32_t k)
+    : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
+      has_filter_(table_filter != nullptr), field_(sort_field), desc_(descending), nulls_first_(nulls_first), k_(k) {
+  if (table_filter) filter_ = *table_filter;
+}
+
+void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
+  output.Reset();
+  if (!ran_) {
+    const uint32_t term_off[2] = {0, uint32_t(terms_.size())};
+    const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
+    hits_.resize(k_);
+    uint32_t n = 0;
+    const int rc = sdbg_match_topk_by_column_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(),
+                                                   excl_off, has_filter_ ? &filter_ : nullptr, field_, desc_ ? 1 : 0,
+                                                   nulls_first_ ? 1 : 0, k_, hits_.data(), &n);
+    if (rc != SDBG_OK)
+      throw GpuError(rc, std::string("sdbg_match_topk_by_column_batch: ") + sdbg_last_error(sdbg_segment_context(segs_[0])));
+    hits_.resize(n);
+    ran_ = true;
+  }
+  const size_t take = std::min<size_t>(duckdb::STANDARD_VECTOR_SIZE, hits_.size() - cursor_);   // 0: end of scan
+  for (size_t i = 0; i < take; ++i) {
+    const sdbg_sort_hit& h = hits_[cursor_ + i];
+    output.doc.push_back(h.doc);
+    output.segment.push_back(h.seg);
+    output.value.push_back(h.value);
+    output.valid.push_back(h.is_null ? 0 : 1);
+  }
+  output.size = take;
+  cursor_ += take;
+}
+
 GpuAggGlobalState::GpuAggGlobalState(std::vector<sdbg_segment*> segments, std::vector<sdbg_col_pred> pushed_filters, uint64_t key_field,
                                      uint64_t sum_int_field, uint64_t avg_f64_field, uint32_t n_groups_hint)
     : segs(std::move(segments)), preds(std::move(pushed_filters)), key(key_field), sum_i(sum_int_field), avg_f(avg_f64_field),

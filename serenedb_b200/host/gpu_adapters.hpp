@@ -126,6 +126,33 @@ class GpuCountScan {
   bool done_ = false;
 };
 
+// SELECT ... FROM t WHERE body @@ '<query>' [AND <pushed filter>] ORDER BY col [DESC] [NULLS FIRST|LAST] LIMIT k -- the body
+// of the TOP_N(col) <- IRESEARCH_SCAN(Stream) plan shape (duckdb_search_full_scan.cpp IResearchSetScanOrder :1711-1762 pushes
+// only score orders; RunStreamingScan :2370-2403 serves the rest under TOP_N). One sdbg_match_topk_by_column_batch call
+// on the first Scan; then rows (doc, segment, value, valid) in TOP_N's order, <= STANDARD_VECTOR_SIZE per call,
+// cardinality 0 at the end.
+class GpuSortedScan {
+ public:
+  GpuSortedScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
+                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
+                uint64_t sort_field, bool descending, bool nulls_first /* the plan's resolved OrderByNullType */,
+                uint32_t k /* LIMIT (+ OFFSET), 1..4096 */);
+  void Scan(duckdb::DataChunkMock& output);
+
+ private:
+  std::vector<sdbg_segment*> segs_;
+  int kind_;
+  std::vector<uint32_t> terms_, excluded_;
+  bool has_filter_;
+  sdbg_col_pred filter_{};
+  uint64_t field_;
+  bool desc_, nulls_first_;
+  uint32_t k_;
+  std::vector<sdbg_sort_hit> hits_;
+  size_t cursor_ = 0;
+  bool ran_ = false;
+};
+
 // The same scan mode under DuckDB's threading contract (duckdb_search_full_scan.hpp:85-255, .cpp:99-268): ONE global
 // state shared by all workers of the query -- touched through atomics only, like next_segment / next_unit there -- and
 // one local state per worker. The first worker to arrive runs the aggregation on the GPU (the others wait on the

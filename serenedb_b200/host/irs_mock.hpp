@@ -228,7 +228,15 @@ struct DataChunkMock {          // stands in for duckdb::DataChunk with flat vec
   std::vector<int64_t> sum_lo;  // SUM(v) as HUGEINT: lower / upper
   std::vector<int64_t> sum_hi;
   std::vector<double> avg;      // AVG(w)
+  std::vector<uint32_t> doc;    // sorted scan: the hit's doc id, segment index, sort value (int64, sign-extended int32 or
+  std::vector<uint32_t> segment;//   the double's bits) and validity (0 = NULL)
+  std::vector<int64_t> value;
+  std::vector<uint8_t> valid;
   uint64_t size = 0;
-  void Reset() { key.clear(); count.clear(); sum_lo.clear(); sum_hi.clear(); avg.clear(); size = 0; }
+  void Reset() {
+    key.clear(); count.clear(); sum_lo.clear(); sum_hi.clear(); avg.clear();
+    doc.clear(); segment.clear(); value.clear(); valid.clear();
+    size = 0;
+  }
 };
 }  // namespace duckdb
