@@ -243,6 +243,25 @@ int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, in
                                     const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
                                     uint64_t sort_field, int descending, int nulls_first, uint32_t k,
                                     sdbg_sort_hit* out /* n_queries * k */, uint32_t* n_out);
+/* Facet counts (SELECT col, count(*) ... WHERE body @@ '...' [AND <pushed filter>] GROUP BY col): per query, how the docs
+ * sdbg_match_count_batch counts for it split over the values of column `key_field` (staged in every segment with one
+ * type: int64 raw or bit-packed, or int32; NOT NULL or nullable; may be the filter's column; row = doc - 1, and a doc past
+ * the column's rows has a NULL key). counts[q * key_span + (v - key_min)] = query q's matches whose key is v, summed over
+ * the segments; null_counts[q] = its matches whose key is NULL (one group, as in SQL). So sum(counts[q, :]) +
+ * null_counts[q] equals sdbg_match_count_batch's count. Identical at every pruning level: nothing is pruned.
+ * The caller gives the key range, so the dense layout can be all-reduced across GPUs as it is and a fixed domain (enum ids)
+ * needs no statistics pass; sdbg_column_minmax_i64 gives a column's range (NULLs skipped).
+ * Errors, all found before anything is queued: those of sdbg_match_count_batch; NULL counts or null_counts, key_span == 0,
+ * key_min + key_span - 1 past INT64_MAX, or a key type that differs between segments: SDBG_EINVAL; a segment without the
+ * key column: SDBG_ENOTFOUND; a float64 key column, or key_span > 32768 (each CTA keeps key_span u32 bins in shared
+ * memory): SDBG_EUNSUPPORTED. Found after the scan: a counted doc whose key lies outside [key_min, key_min + key_span):
+ * SDBG_EINVAL, and the outputs are unspecified. Synchronous on the context's stream.
+ * Device scratch: n_queries * key_span * 8 B + n_queries * 8 B (4096 queries x 2001 keys: 66 MB). Split larger batches. */
+int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
+                                  const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms,
+                                  const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                                  uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                  uint64_t* counts /* n_queries * key_span */, uint64_t* null_counts /* n_queries */);
 /* Conjunctions of OR groups (`a & (b | c) & !d`: an And whose children are terms, Ors of terms and Nots of terms, as
  * synonym expansion and query rewriting produce). Query q is the AND of the groups [query_group_off[q],
  * query_group_off[q+1]) (1..16), group g the OR of terms[group_off[g] .. group_off[g+1]) (non-empty); its positive terms

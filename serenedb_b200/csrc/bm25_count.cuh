@@ -15,12 +15,14 @@
 //        same early end.
 //   NOT  the excluded lists' blocks whose range holds a bit of `acc` are decoded and their docs cleared.
 // Then acc &= ~deleted, the filter runs per remaining bit, and popcounts are summed: one 64-bit atomicAdd per CTA.
+// The facet pass (kFacet, bm25_facet.cuh) also counts each remaining bit in its key's shared-memory bin.
 // A window that no positive list reaches (OR), that the shortest list does not reach (AND) or that no list of the lead
 // group reaches (GROUPS) is never touched: the CTA
 // jumps to the window of the next block's first possible doc, so a sparse query costs in proportion to its blocks.
 #pragma once
 
 #include "bm25_kernels.cuh"
+#include "bm25_facet.cuh"
 #include "bm25_sort.cuh"
 
 namespace sdbg {
@@ -49,6 +51,7 @@ struct CountParams {
   const uint4* work;            // {query, first window, windows, 0}
   unsigned long long* counts;   // per query, summed over items and segments
   SortSink sort;                // kSort: the sorted scan's sink (work item .w = its output slot)
+  FacetSink facet;              // kFacet: the facet pass's sink
 };
 
 __device__ __forceinline__ uint32_t warp_min(uint32_t v) {
@@ -128,10 +131,13 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
 // and with a zonemap each window is judged before any list is decoded: a window none of whose zones can reach the
 // threshold is skipped, and in a kept window the docs of such zones are cleared before the column is read. The item's
 // k best go to output slot item.w.
-template <bool kAnd, bool kGroups = false, bool kSort = false>
+// kFacet: the facet pass (bm25_facet.cuh). Besides the popcount, every surviving doc's key is counted in the item's
+// histogram of P.facet.span u32 bins in dynamic shared memory, flushed to the query's row of P.facet.counts at the end.
+template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false>
 __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
   static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
   static_assert(!(kSort && kGroups), "the sorted scan takes OR / AND queries");
+  static_assert(!(kFacet && (kSort || kGroups)), "the facet pass takes OR / AND queries and has its own sink");
   __shared__ uint32_t acc[kCountWords];
   __shared__ uint32_t tmp[kAnd || kGroups ? kCountWords : 1];
   __shared__ uint32_t stage[kCountWarps][128];
@@ -144,8 +150,9 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   __shared__ uint32_t s_ws, s_done;
   __shared__ unsigned long long s_sum[kCountWarps];
   __shared__ unsigned long long s_thr[1];   // kSort: this item's best known k-th hi
-  __shared__ uint32_t s_fill[1], s_zmask[2];  // kSort: keys in the buffer; the window's zones that can reach s_thr
-  extern __shared__ unsigned long long sort_buf[];   // kSort: hi[cap] | lo[cap]
+  __shared__ uint32_t s_fill[1], s_zmask[2];  // kSort: keys in the buffer (kFacet: NULL keys); the window's zones that can reach s_thr
+  extern __shared__ unsigned long long sort_buf[];   // kSort: hi[cap] | lo[cap]; kFacet: the u32 bins
+  uint32_t* const bins = reinterpret_cast<uint32_t*>(sort_buf);
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint4 item = P.work[blockIdx.x];
@@ -167,11 +174,16 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
     s_next[tid] = l.y ? find_block_from(B + l.x, 0u, l.y, 0u, item.y << kCountWindowLog) : 0u;
   }
   unsigned long long count = 0;
+  bool oor = false;                                     // kFacet: this thread counted a key outside the bins
   uint32_t ws = item.y << kCountWindowLog;              // start of the window being looked at
   uint32_t judged = 0, skipped = 0;                     // kSort: windows judged / skipped by the zonemap
   if constexpr (kSort) {
     for (uint32_t i = tid; i < 2u * P.sort.cap; i += kCountThreads) sort_buf[i] = 0ull;
     if (tid == 0) { s_thr[0] = 0ull; s_fill[0] = 0u; }
+  }
+  if constexpr (kFacet) {
+    for (uint32_t i = tid; i < P.facet.span; i += kCountThreads) bins[i] = 0u;
+    if (tid == 0) s_fill[0] = 0u;
   }
   __syncthreads();
   for (;;) {
@@ -286,6 +298,9 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
             if (!filter_pass(P.filt, ws + 32u * i + bit)) v &= ~(1u << bit);
           }
         }
+        if constexpr (kFacet) {
+          for (uint32_t r = v; r; r &= r - 1u) oor |= facet_add(P.facet, ws + 32u * i + (__ffs(r) - 1u), bins, &s_fill[0]);
+        }
         count += __popc(v);
       }
     }
@@ -346,6 +361,14 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       if (judged) { atomicAdd(P.sort.stats, judged); if (skipped) atomicAdd(P.sort.stats + 1, skipped); }
     }
     return;
+  }
+  if constexpr (kFacet) {
+    // A work item covers docs of one segment, fewer than 2^32, so no u32 bin can wrap before this flush.
+    unsigned long long* out = P.facet.counts + size_t(q) * P.facet.span;
+    for (uint32_t i = tid; i < P.facet.span; i += kCountThreads)
+      if (bins[i]) atomicAdd(out + i, static_cast<unsigned long long>(bins[i]));
+    if (oor) *P.facet.out_of_range = 1u;
+    if (tid == 0 && s_fill[0]) atomicAdd(P.facet.nulls + q, static_cast<unsigned long long>(s_fill[0]));
   }
   count = warp_sum64(count);
   if (lane == 0) s_sum[warp] = count;

@@ -1610,7 +1610,44 @@ extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_s
 // query (groups 0 .. n - 1 all present); those queries run bm25_count_kernel<false, true>.
 // sort (NULL: count): the sorted scan of sdbg_match_topk_by_column_batch on the same plan, without the single-term
 // shortcut; see sort_prepare / sort_finish.
+// facet (NULL: count): the facet pass of sdbg_match_facet_counts_batch on the same plan and launches, without the
+// single-term shortcut; see facet_prepare.
 namespace {
+
+// The facet pass's part of a count_run call.
+struct FacetJob {
+  uint64_t field;
+  int64_t key_min;
+  uint32_t span;
+  uint64_t* counts;        // host: [query][span]
+  uint64_t* null_counts;   // host: [query]
+  std::vector<FacetSink> sink;   // per segment, filled by facet_prepare (output pointers set at launch)
+};
+
+// Checks the key range and the key column of every segment, then fills the per-segment sinks. Every check runs before
+// anything is queued (a packed column's raw view is decoded on first use).
+int facet_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, FacetJob& J) {
+  if (J.span == 0) return fail(c, SDBG_EINVAL, "key_span is 0");
+  if (J.key_min > INT64_MAX - int64_t(J.span - 1)) return fail(c, SDBG_EINVAL, "key_min + key_span - 1 overflows int64");
+  if (J.span > kFacetMaxSpan) return fail(c, SDBG_EUNSUPPORTED, "key_span > 32768 (the bins are shared memory)");
+  for (size_t si = 0; si < n_segs; ++si) {
+    auto it = segs[si]->cols.find(J.field);
+    if (it == segs[si]->cols.end()) return fail(c, SDBG_ENOTFOUND, "key column not staged in every segment");
+    if (it->second.type != segs[0]->cols.find(J.field)->second.type)
+      return fail(c, SDBG_EINVAL, "key column type differs between segments");
+  }
+  if (segs[0]->cols.find(J.field)->second.type == SDBG_F64) return fail(c, SDBG_EUNSUPPORTED, "float64 key column");
+  J.sink.assign(n_segs, FacetSink{});
+  for (size_t si = 0; si < n_segs; ++si) {
+    ColumnObj& col = segs[si]->cols.find(J.field)->second;
+    FacetSink& F = J.sink[si];
+    void* raw = nullptr;
+    if (int rc = raw_values(c, col, &raw)) return rc;
+    F.values = raw; F.validity = reinterpret_cast<const unsigned long long*>(col.d_validity); F.rows = col.rows;
+    F.type = uint32_t(col.type); F.span = J.span; F.key_min = J.key_min;
+  }
+  return SDBG_OK;
+}
 
 // The sorted scan's part of a count_run call.
 struct SortJob {
@@ -1812,14 +1849,16 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const uin
 
 int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms, const uint32_t* term_off, size_t nq,
               const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts,
-              const uint8_t* term_grp = nullptr, SortJob* sort = nullptr) {
-  if (!segs || !n_segs || !terms || !term_off || !nq || (!counts && !sort)) return SDBG_EINVAL;
+              const uint8_t* term_grp = nullptr, SortJob* sort = nullptr, FacetJob* facet = nullptr) {
+  if (!segs || !n_segs || !terms || !term_off || !nq || (!counts && !sort && !facet)) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   CU(c, cudaSetDevice(c->device));
   uint32_t total_excl = 0;
   if (int rc = check_query_batch(segs, n_segs, terms, term_off, nq, excl_terms, excl_off, filt, &total_excl)) return rc;
   if (sort)
     if (int rc = sort_prepare(c, segs, n_segs, *sort)) return rc;
+  if (facet)
+    if (int rc = facet_prepare(c, segs, n_segs, *facet)) return rc;
   const bool conj = kind == SDBG_QUERY_AND;
   const uint32_t n_pos = term_off[nq];
   const size_t n_lists = size_t(n_pos) + total_excl;   // per segment: positive lists | excluded lists
@@ -1911,7 +1950,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
       bool excl_blocks = false;
       if (total_excl)
         for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) excl_blocks |= L[n_pos + i].y != 0;
-      if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks && !sort) { host[q] += sum; continue; }
+      if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks && !sort && !facet) { host[q] += sum; continue; }
       const uint64_t weight = conj ? uint64_t(smallest) * (t1 - t0) : sum;
       uint32_t g = uint32_t(std::max<uint64_t>(G, (weight + chain_target - 1) / chain_target));
       g = std::min({g, n_win, 2u * uint32_t(c->sm_count)});
@@ -1959,10 +1998,19 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
       std::memcpy(h + grp_pos + off_bytes, grp_end.data(), grp_end.size() * 4);
     }
     DevBuf& b_desc = c->scratch[0]; DevBuf& b_counts = c->scratch[1];
+    // facet pass: b_counts holds [counts | facet counts [nq][span] | NULL counts [nq] | out-of-range word]
+    const size_t fc_pos = nq * 8, fn_pos = fc_pos + (facet ? nq * size_t(facet->span) * 8 : 0), oor_pos = fn_pos + nq * 8;
+    const size_t out_bytes = facet ? oor_pos + 8 : nq * 8;
     if ((rc = ensure(c, b_desc, bytes))) return rc;
-    if ((rc = ensure(c, b_counts, nq * 8))) return rc;
+    if ((rc = ensure(c, b_counts, out_bytes))) return rc;
     CU(c, cudaMemcpyAsync(b_desc.p, h, bytes, cudaMemcpyHostToDevice, c->stream));
-    CU(c, cudaMemsetAsync(b_counts.p, 0, nq * 8, c->stream));
+    CU(c, cudaMemsetAsync(b_counts.p, 0, out_bytes, c->stream));
+    char* fo = static_cast<char*>(b_counts.p);
+    const size_t facet_smem = facet ? (size_t(facet->span) * 4 + 15) & ~size_t(15) : 0;
+    if (facet && facet_smem > 48 * 1024) {
+      CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(facet_smem)));
+      CU(c, cudaFuncSetAttribute(bm25_count_kernel<true, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(facet_smem)));
+    }
     const char* d = static_cast<const char*>(b_desc.p);
     size_t done = 0;
     for (size_t si = 0; si < n_segs; ++si) {
@@ -1977,7 +2025,14 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
       P.work = reinterpret_cast<const uint4*>(d + work_pos) + done;
       P.counts = static_cast<unsigned long long*>(b_counts.p);
       done += seg_work[si].size();
-      if (term_grp) {
+      if (facet) {
+        P.facet = facet->sink[si];
+        P.facet.counts = reinterpret_cast<unsigned long long*>(fo + fc_pos);
+        P.facet.nulls = reinterpret_cast<unsigned long long*>(fo + fn_pos);
+        P.facet.out_of_range = reinterpret_cast<unsigned int*>(fo + oor_pos);
+        if (conj) bm25_count_kernel<true, false, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem, c->stream>>>(P);
+        else bm25_count_kernel<false, false, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem, c->stream>>>(P);
+      } else if (term_grp) {
         P.grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
         P.grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[nq];
         bm25_count_kernel<false, true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
@@ -1986,10 +2041,24 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
       ++c->launches;
     }
     CU(c, cudaGetLastError());
+    if (facet) {
+      unsigned int oor = 0;
+      CU(c, cudaMemcpyAsync(facet->counts, fo + fc_pos, nq * size_t(facet->span) * 8, cudaMemcpyDeviceToHost, c->stream));
+      CU(c, cudaMemcpyAsync(facet->null_counts, fo + fn_pos, nq * 8, cudaMemcpyDeviceToHost, c->stream));
+      CU(c, cudaMemcpyAsync(&oor, fo + oor_pos, 4, cudaMemcpyDeviceToHost, c->stream));
+      CU(c, cudaStreamSynchronize(c->stream));
+      if (oor) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
+      return SDBG_OK;
+    }
     CU(c, cudaMemcpyAsync(h, b_counts.p, nq * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     const auto* dc = reinterpret_cast<const unsigned long long*>(h);
     for (size_t q = 0; q < nq; ++q) host[q] += dc[q];
+  }
+  if (facet) {   // no query matches anywhere
+    std::memset(facet->counts, 0, nq * size_t(facet->span) * 8);
+    std::memset(facet->null_counts, 0, nq * 8);
+    return SDBG_OK;
   }
   std::memcpy(counts, host.data(), nq * 8);
   return SDBG_OK;
@@ -2010,6 +2079,15 @@ extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t
   if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
   SortJob J{sort_field, descending, nulls_first, k, out, n_out, false, {}, {}};
   return count_run(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, filt, nullptr, nullptr, &J);
+}
+
+extern "C" int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
+                                             const uint32_t* term_off, size_t nq, const uint32_t* excl_terms,
+                                             const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                             int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
+  if (!counts || !null_counts) return SDBG_EINVAL;
+  FacetJob J{key_field, key_min, key_span, counts, null_counts, {}};
+  return count_run(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, filt, nullptr, nullptr, nullptr, &J);
 }
 
 extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,

@@ -531,6 +531,52 @@ def ExecuteTopKByColumn(reader, query_terms, kind, sort_field, k, descending=Fal
     return dict(docs=r["docs"][0], segs=r["segs"][0], values=r["values"][0], nulls=r["nulls"][0])
 
 
+def ExecuteFacetCountsBatch(reader, queries, kind, key_field, key_min=None, key_span=None, filt=None, exclude=None):
+    """Facet counts (`SELECT col, count(*) ... WHERE body @@ '...' GROUP BY col`, sdbg_match_facet_counts_batch): per
+    query, how the docs ExecuteCountBatch counts split over the values of column `key_field` (int64 / int32, staged in
+    every segment). The key range [key_min, key_min + key_span) defaults to the segments' column_minmax (an all-NULL column
+    gives one bin). Returns dict(key_min, counts uint64[Q, key_span], nulls uint64[Q]): counts[q, v - key_min] = matches
+    whose key is v, nulls[q] = matches whose key is NULL."""
+    col_type = reader.segments[0].col_types.get(int(key_field))
+    if col_type is None:   # the kernel reads raw values: their type must be known, not guessed
+        raise ValueError("key column %d was not staged through this Segment" % int(key_field))
+    if col_type not in (0, 2):
+        raise ValueError("facet counts need an int64 or int32 key column")
+    if key_min is None or key_span is None:
+        mm = [s.column_minmax(key_field) for s in reader.segments]
+        lo, hi = min(m[0] for m in mm), max(m[1] for m in mm)
+        if lo > hi:   # every key NULL
+            lo = hi = 0
+        key_min = lo if key_min is None else key_min
+        key_span = hi - key_min + 1 if key_span is None else key_span
+    nq = len(queries)
+    flat = np.ascontiguousarray([t for q in queries for t in q], dtype=np.uint32)
+    off = np.zeros(nq + 1, np.uint32)
+    off[1:] = np.cumsum([len(q) for q in queries])
+    counts = np.zeros((max(nq, 1), max(int(key_span), 1)), np.uint64)
+    nulls = np.zeros(max(nq, 1), np.uint64)
+    x = _exclusions(exclude, nq)
+    fp = C.byref(filt) if filt is not None else None
+    N.check(N.lib().sdbg_match_facet_counts_batch(_seg_array(reader.segments), len(reader.segments), int(kind),
+                                                  _ptr(flat) if len(flat) else None, _ptr(off), nq,
+                                                  _ptr(x[0]) if x is not None else None,
+                                                  _ptr(x[1]) if x is not None else None, fp, int(key_field), int(key_min),
+                                                  int(key_span), _ptr(counts), _ptr(nulls)), reader.segments[0].ctx._h)
+    return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
+
+
+def ExecuteFacetCounts(reader, query_terms, kind, key_field, key_min=None, key_span=None, filt=None, exclude=None):
+    """ExecuteFacetCountsBatch for one query: {key: count} for the keys with matches, plus {None: n} when n > 0 matches
+    have a NULL key."""
+    r = ExecuteFacetCountsBatch(reader, [list(query_terms)], kind, key_field, key_min, key_span, filt,
+                                exclude=None if exclude is None else [list(exclude)])
+    row = r["counts"][0]
+    out = {r["key_min"] + int(i): int(row[i]) for i in np.nonzero(row)[0]}
+    if r["nulls"][0]:
+        out[None] = int(r["nulls"][0])
+    return out
+
+
 def _groups(queries):
     """Queries as lists of OR groups -> (flat term ids, group_off u32, query_group_off u32)."""
     groups = [list(g) for q in queries for g in q]

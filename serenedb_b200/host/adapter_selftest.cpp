@@ -3,7 +3,8 @@
 // for tests/test_gpu_adapters.py to compare with the oracle. Needs a GPU at run time. With a second argument "excl" it runs
 // only the exclusion case instead (an And with a Not child, tests/test_gpu_exclusion.py); with "count", only the Count
 // scan mode (GpuCountScan, tests/test_gpu_count.py); with "groups", only an And of Or groups through both adapters
-// (tests/test_gpu_groups.py); with "sorted", only the sorted scan (GpuSortedScan, tests/test_gpu_sort_by_column.py).
+// (tests/test_gpu_groups.py); with "sorted", only the sorted scan (GpuSortedScan, tests/test_gpu_sort_by_column.py); with
+// "facet", only the facet counts (GpuFacetScan, tests/test_gpu_facets.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -135,6 +136,50 @@ int main(int argc, char** argv) {
             for (size_t i = 0; i < valid.size(); ++i) std::printf("%s%u", i ? ", " : "", unsigned(valid[i]));
             std::printf("]}\n");
           }
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
+  if (argc > 2 && std::string(argv[2]) == "facet") {
+    // `t2 | t5`, `t2 & t5` and `(t2 | t5) & !t3` GROUP BY the 2001-key int64 column 15 (count(*)), without and with the
+    // table filter: every group in key order, then end of scan. Then the int32 column 9, whose range is too wide.
+    sdbg_synth_column(seg, 15, 15, 3, 1, n_docs);
+    for (int with_filter = 0; with_filter < 2; ++with_filter)
+      for (int kind : {int(SDBG_QUERY_OR), int(SDBG_QUERY_AND)})
+        for (int excl = 0; excl < 2; ++excl) {
+          sdbg_host::GpuFacetScan scan({seg}, kind, {2, 5}, excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{},
+                                       with_filter ? &filt : nullptr, 15);
+          duckdb::DataChunkMock chunk;
+          std::vector<int64_t> keys, counts;
+          std::vector<uint8_t> valid;
+          uint64_t chunks = 0, max_chunk = 0;
+          for (;;) {
+            scan.Scan(chunk);
+            if (chunk.size == 0) break;
+            ++chunks;
+            max_chunk = std::max<uint64_t>(max_chunk, chunk.size);
+            keys.insert(keys.end(), chunk.key.begin(), chunk.key.end());
+            counts.insert(counts.end(), chunk.count.begin(), chunk.count.end());
+            valid.insert(valid.end(), chunk.valid.begin(), chunk.valid.end());
+          }
+          scan.Scan(chunk);
+          std::printf("{\"filter\": %d, \"kind\": %d, \"excl\": %d, \"chunks\": %llu, \"max_chunk\": %llu, \"rows_after\": %llu, "
+                      "\"keys\": [", with_filter, kind, excl, static_cast<unsigned long long>(chunks),
+                      static_cast<unsigned long long>(max_chunk), static_cast<unsigned long long>(chunk.size));
+          for (size_t i = 0; i < keys.size(); ++i) std::printf("%s%lld", i ? ", " : "", static_cast<long long>(keys[i]));
+          std::printf("], \"counts\": [");
+          for (size_t i = 0; i < counts.size(); ++i) std::printf("%s%lld", i ? ", " : "", static_cast<long long>(counts[i]));
+          std::printf("], \"valid\": [");
+          for (size_t i = 0; i < valid.size(); ++i) std::printf("%s%u", i ? ", " : "", unsigned(valid[i]));
+          std::printf("]}\n");
+        }
+    int code = 0;
+    try {
+      sdbg_host::GpuFacetScan wide({seg}, SDBG_QUERY_OR, {2, 5}, {}, nullptr, 9);
+      duckdb::DataChunkMock chunk;
+      wide.Scan(chunk);
+    } catch (const sdbg_host::GpuError& e) { code = e.code; }
+    std::printf("{\"wide_error\": %d}\n", code);
     sdbg_segment_destroy(seg);
     sdbg_destroy(ctx);
     return 0;

@@ -257,6 +257,51 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
   cursor_ += take;
 }
 
+GpuFacetScan::GpuFacetScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
+                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field)
+    : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
+      has_filter_(table_filter != nullptr), field_(key_field) {
+  if (table_filter) filter_ = *table_filter;
+}
+
+void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
+  output.Reset();
+  if (!ran_) {
+    sdbg_ctx* ctx = sdbg_segment_context(segs_[0]);
+    int64_t lo = INT64_MAX, hi = INT64_MIN;
+    for (sdbg_segment* s : segs_) {
+      int64_t mn = 0, mx = 0;
+      const int rc = sdbg_column_minmax_i64(s, field_, &mn, &mx);
+      if (rc != SDBG_OK) throw GpuError(rc, std::string("sdbg_column_minmax_i64: ") + sdbg_last_error(ctx));
+      lo = std::min(lo, mn);
+      hi = std::max(hi, mx);
+    }
+    if (lo > hi) lo = hi = 0;   // every key NULL: one (empty) bin, every match in the NULL group
+    const uint64_t span = uint64_t(hi) - uint64_t(lo) + 1;
+    if (span == 0 || span > 32768) throw GpuError(SDBG_EUNSUPPORTED, "GpuFacetScan: the key range spans more than 32768 values");
+    const uint32_t term_off[2] = {0, uint32_t(terms_.size())};
+    const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
+    std::vector<uint64_t> counts(span);
+    const int rc = sdbg_match_facet_counts_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(),
+                                                 excl_off, has_filter_ ? &filter_ : nullptr, field_, lo, uint32_t(span),
+                                                 counts.data(), &nulls_);
+    if (rc != SDBG_OK) throw GpuError(rc, std::string("sdbg_match_facet_counts_batch: ") + sdbg_last_error(ctx));
+    for (uint64_t i = 0; i < span; ++i)
+      if (counts[i]) groups_.emplace_back(int64_t(uint64_t(lo) + i), counts[i]);
+    ran_ = true;
+  }
+  const size_t rows = groups_.size() + (nulls_ ? 1 : 0);
+  const size_t take = std::min<size_t>(duckdb::STANDARD_VECTOR_SIZE, rows - cursor_);   // 0: end of scan
+  for (size_t i = cursor_; i < cursor_ + take; ++i) {
+    const bool null_group = i == groups_.size();
+    output.key.push_back(null_group ? 0 : groups_[i].first);
+    output.count.push_back(int64_t(null_group ? nulls_ : groups_[i].second));
+    output.valid.push_back(null_group ? 0 : 1);
+  }
+  output.size = take;
+  cursor_ += take;
+}
+
 GpuAggGlobalState::GpuAggGlobalState(std::vector<sdbg_segment*> segments, std::vector<sdbg_col_pred> pushed_filters, uint64_t key_field,
                                      uint64_t sum_int_field, uint64_t avg_f64_field, uint32_t n_groups_hint)
     : segs(std::move(segments)), preds(std::move(pushed_filters)), key(key_field), sum_i(sum_int_field), avg_f(avg_f64_field),

@@ -153,6 +153,31 @@ class GpuSortedScan {
   bool ran_ = false;
 };
 
+// SELECT col, count(*) FROM t WHERE body @@ '<query>' [AND <pushed filter>] GROUP BY col -- the body of the
+// HASH_GROUP_BY(col; count_star()) <- IRESEARCH_SCAN(text query) plan shape (facet counts). The first Scan takes the key
+// range from sdbg_column_minmax_i64 over the segments and runs one sdbg_match_facet_counts_batch call; then the non-empty
+// groups as rows (key, count, valid) in ascending key order, the NULL group (valid = 0) last, <= STANDARD_VECTOR_SIZE per
+// call, cardinality 0 at the end. A key range wider than 32768 throws GpuError(SDBG_EUNSUPPORTED): the plan stays on the CPU.
+class GpuFacetScan {
+ public:
+  GpuFacetScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
+               std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
+               uint64_t key_field /* int64 or int32 */);
+  void Scan(duckdb::DataChunkMock& output);
+
+ private:
+  std::vector<sdbg_segment*> segs_;
+  int kind_;
+  std::vector<uint32_t> terms_, excluded_;
+  bool has_filter_;
+  sdbg_col_pred filter_{};
+  uint64_t field_;
+  std::vector<std::pair<int64_t, uint64_t>> groups_;   // (key, count) of the non-empty groups
+  uint64_t nulls_ = 0;                                 // the NULL group's count
+  size_t cursor_ = 0;                                  // rows emitted; the NULL group is row groups_.size()
+  bool ran_ = false;
+};
+
 // The same scan mode under DuckDB's threading contract (duckdb_search_full_scan.hpp:85-255, .cpp:99-268): ONE global
 // state shared by all workers of the query -- touched through atomics only, like next_segment / next_unit there -- and
 // one local state per worker. The first worker to arrive runs the aggregation on the GPU (the others wait on the
