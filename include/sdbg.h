@@ -289,6 +289,26 @@ int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n_segs, cons
                                   const uint32_t* group_off, const uint32_t* query_group_off, size_t n_queries,
                                   const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
                                   uint64_t* counts);
+/* OR groups with a minimum match count (`2 of (a | b | c) & d`: an Or with min_match_count, as minimum_should_match and
+ * relaxed natural-language queries produce). The groups entries' parameters plus group_min: group g (indexed like
+ * group_off) needs group_min[g] of its s_g terms, 1 <= group_min[g] <= s_g; a doc satisfies the group when at least
+ * group_min[g] of its posting lists hold it. group_min NULL: every group needs 1, exactly sdbg_*_batch_groups.
+ * A term a segment does not hold is an empty list there and still counts in s_g, so a group with fewer than group_min[g]
+ * non-empty lists in a segment matches nothing there. Scores, totals and counts as for the groups entries.
+ * Normalisation: a group with group_min[g] == s_g is its terms as single-term groups; a query whose groups then all need
+ * 1 term is an ordinary groups query and gives exactly its results.
+ * Errors: group_min[g] == 0 or > s_g: SDBG_EINVAL; otherwise those of the groups entries. */
+int sdbg_bm25_topk_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                    const uint32_t* group_off, const uint32_t* query_group_off,
+                                    const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                    const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                    float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in,
+                                    sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches);
+int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                      const uint32_t* group_off, const uint32_t* query_group_off,
+                                      const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                      const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                      uint64_t* counts);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

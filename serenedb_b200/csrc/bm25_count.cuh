@@ -12,7 +12,8 @@
 //        once `acc` is empty.
 //   GROUPS  an AND of OR groups (kGroups): the lead group (smallest summed docs_count) fills `acc` like an OR; each further
 //        group ORs into `tmp` the docs of its lists' blocks whose range holds a bit of `acc`, then acc &= tmp, with the
-//        same early end.
+//        same early end. A group that needs m >= 2 of its s lists (`2 of (a | b | c)`) leads with its s - m + 1 shortest
+//        lists; it decodes each list into `tmp` the same way, adds it into a bit-sliced counter, then acc &= counter >= m.
 //   NOT  the excluded lists' blocks whose range holds a bit of `acc` are decoded and their docs cleared.
 // Then acc &= ~deleted, the filter runs per remaining bit, and popcounts are summed: one 64-bit atomicAdd per CTA.
 // The facet pass (kFacet, bm25_facet.cuh) also counts each remaining bit in its key's shared-memory bin.
@@ -43,8 +44,11 @@ struct CountParams {
   const uint2* lists;
   const uint32_t* term_off;
   const uint32_t* excl_off;
-  // kGroups: query q's positive lists form consecutive OR groups, lead group first; group g of q ends (exclusive, relative
-  // to term_off[q]) at grp_end[grp_off[q] + g]. Per segment, since the lead group and the list order depend on it.
+  // kGroups: query q's positive lists form consecutive OR groups, lead group first, each group's lists by ascending
+  // docs_count; group g of q ends (exclusive, relative to term_off[q]) at grp_end[grp_off[q] + g] & 0xFF, and needs
+  // m_g = (grp_end[grp_off[q] + g] >> 8) + 1 of its lists to hold a doc. Per segment, since the lead group and the list
+  // order depend on it. A group with m_g >= 2 counts in a bit-sliced counter of bits(m_g) planes of kCountWords words in
+  // dynamic shared memory; the launch provides the batch's largest.
   const uint32_t* grp_end = nullptr;
   const uint32_t* grp_off = nullptr;
   uint32_t n_pos;               // term_off[n_queries]
@@ -162,7 +166,10 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   const uint32_t n_lists = n_pos + n_excl;
   const uint32_t n_groups = kGroups ? P.grp_off[q + 1] - P.grp_off[q] : 0u;
   if (kGroups && tid < n_groups) s_gend[tid] = P.grp_end[P.grp_off[q] + tid];
-  const uint32_t n_lead = kGroups ? P.grp_end[P.grp_off[q]] : kAnd ? 1u : n_pos;   // lists that decide which windows hold matches
+  // lists that decide which windows hold matches; for groups the lead group's s - m + 1 shortest (a doc that m of its s
+  // lists hold is in one of them)
+  const uint32_t gend0 = kGroups ? P.grp_end[P.grp_off[q]] : 0u;
+  const uint32_t n_lead = kGroups ? (gend0 & 0xFFu) - (gend0 >> 8) : kAnd ? 1u : n_pos;
   const uint4* const B = P.seg.blocks;
   const uint32_t del_words = (P.seg.n_docs + 32u) / 32u + 1u;
 
@@ -273,13 +280,45 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       }
     }
     if constexpr (kGroups) {
-      for (uint32_t g = 1; g < n_groups; ++g) {
-        for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
-        __syncthreads();
-        run_lists(s_gend[g - 1], s_gend[g], tmp, false, true);
-        __syncthreads();
+      // the lead group is already in acc unless it needs m >= 2 of its lists
+      for (uint32_t g = (gend0 >> 8) ? 0u : 1u; g < n_groups; ++g) {
+        const uint32_t lo = g ? s_gend[g - 1] & 0xFFu : 0u, hi = s_gend[g] & 0xFFu, m = (s_gend[g] >> 8) + 1u;
         uint32_t nz = 0u;
-        for (uint32_t i = tid; i < kCountWords; i += kCountThreads) { const uint32_t v = acc[i] & tmp[i]; acc[i] = v; nz |= v; }
+        if (m == 1u) {
+          for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
+          __syncthreads();
+          run_lists(lo, hi, tmp, false, true);
+          __syncthreads();
+          for (uint32_t i = tid; i < kCountWords; i += kCountThreads) { const uint32_t v = acc[i] & tmp[i]; acc[i] = v; nz |= v; }
+        } else {
+          // at least m of the lists: each list's bitmap is added into a saturating bit-sliced counter (plane p = bit p)
+          const uint32_t np = 32u - __clz(m);
+          uint32_t* const plane = bins;
+          for (uint32_t i = tid; i < np * kCountWords; i += kCountThreads) plane[i] = 0u;
+          for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
+          for (uint32_t li = lo; li < hi; ++li) {
+            __syncthreads();
+            run_lists(li, li + 1u, tmp, false, true);
+            __syncthreads();
+            for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
+              uint32_t c = tmp[i];
+              tmp[i] = 0u;
+              for (uint32_t p = 0; p < np && c; ++p) { const uint32_t t = plane[p * kCountWords + i] & c; plane[p * kCountWords + i] ^= c; c = t; }
+              if (c) for (uint32_t p = 0; p < np; ++p) plane[p * kCountWords + i] |= c;   // 2^np - 1 >= m: saturate
+            }
+          }
+          __syncthreads();
+          for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
+            uint32_t gt = 0u, eq = 0xFFFFFFFFu;   // counter > m / == m on the bits above p
+            for (uint32_t p = np; p-- > 0;) {
+              const uint32_t v = plane[p * kCountWords + i];
+              if ((m >> p) & 1u) eq &= v;
+              else { gt |= eq & v; eq &= ~v; }
+            }
+            const uint32_t v = acc[i] & (gt | eq);
+            acc[i] = v; nz |= v;
+          }
+        }
         if (!__syncthreads_or(nz != 0u)) { live = false; break; }
       }
     }

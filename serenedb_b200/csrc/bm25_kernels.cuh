@@ -60,7 +60,9 @@ struct QTermDev {  // one term of one query over one segment, 40 bytes
 constexpr uint32_t kMaxQueryTerms = 16;
 // Per-doc list checks of a query (TopkParams::excl): up to 16 excluded lists plus up to 16 lists of required OR groups.
 constexpr uint32_t kMaxCheckLists = 2u * kMaxQueryTerms;
-constexpr uint8_t kCheckExcl = 0xFF;   // tag of an excluded list; a group list carries its group index (0..15)
+// Tag of an excluded list. A group list's tag holds its group index g (0..15) in the low nibble and the group's minimum
+// match count m_g - 1 in the high nibble (0 for a plain OR group; m_g <= 15, so no group tag equals kCheckExcl).
+constexpr uint8_t kCheckExcl = 0xFF;
 constexpr uint32_t kTopkThreads = 256;
 constexpr uint32_t kTopkWarps = kTopkThreads / 32;
 constexpr uint32_t kTopkBudget = 32;   // bm25_topk_kernel: posting blocks per window, one planner lane each
@@ -332,8 +334,9 @@ struct TopkParams {
   // Excluded terms (the NOT children of an And, irs search/exclusion.hpp): query q rejects every doc that occurs in one
   // of the lists excl[excl_off[q] .. excl_off[q + 1]), each {first BlockDesc, blocks} in this segment (0 blocks: a term
   // the segment does not hold). Excluded terms never score. Null: no query of the call excludes anything.
-  // excl_grp, when set, tags each of those lists: kCheckExcl for an excluded list, else the index (0..15) of a required
-  // OR group of the query (`a & (b | c)`): a doc then also needs, for every group present, a tagged list that holds it.
+  // excl_grp, when set, tags each of those lists: kCheckExcl for an excluded list, else a required OR group of the query
+  // (`a & (b | c)`, `2 of (a | b | c)`; kCheckExcl's comment gives the layout): a doc then also needs, for every group
+  // present, at least m_g of the group's tagged lists that hold it.
   // Set only for the kGroups instantiations, whose queries have at most kMaxCheckLists lists.
   const uint2* excl = nullptr;
   const uint32_t* excl_off = nullptr;
@@ -478,11 +481,28 @@ __device__ __forceinline__ bool probe_contains(const PostingsDev& S, uint2 list,
   return block_find_doc(S, desc, list.x + l, d, idx);
 }
 
-// Bit g set for every group tag g (< kCheckExcl) among the n list tags: the groups a doc has to satisfy.
-__device__ __forceinline__ uint32_t check_group_mask(const uint8_t* grp, uint32_t n) {
-  uint32_t need = 0u;
-  for (uint32_t x = 0; x < n; ++x) if (grp[x] != kCheckExcl) need |= 1u << grp[x];
-  return need;
+// Per-doc state of the OR-group check, one 4-bit counter per group g at bits 4g .. 4g + 3: `need` = lists that must still
+// hold the doc (m_g at first), `slack` = lists that may still miss it (s_g - m_g at first, s_g = the group's lists).
+// A group is satisfied once its need is 0 and fails once a list misses with its slack at 0.
+struct GroupNeed { unsigned long long need, slack; };
+__device__ __forceinline__ GroupNeed check_group_need(const uint8_t* grp, uint32_t n) {
+  unsigned long long need = 0ull, lists = 0ull;
+  for (uint32_t x = 0; x < n; ++x) {
+    if (grp[x] == kCheckExcl) continue;
+    const uint32_t g4 = 4u * (grp[x] & 15u);
+    need |= static_cast<unsigned long long>((grp[x] >> 4) + 1u) << g4;
+    lists += 1ull << g4;   // s_g = 16 carries into the next nibble; lists - need is still exact per nibble
+  }
+  return {need, lists - need};
+}
+
+// One group list's verdict for one doc: counts a hit towards the group's minimum, a miss against its slack. False when
+// the group can no longer reach its minimum.
+__device__ __forceinline__ bool group_step(GroupNeed& st, uint32_t g4, bool hit) {
+  if (hit) { st.need -= 1ull << g4; return true; }
+  if (((st.slack >> g4) & 15ull) == 0ull) return false;
+  st.slack -= 1ull << g4;
+  return true;
 }
 
 // One thread: does any of the n excluded lists hold doc d (legacy window kernel's emit step)? Each list is searched from
@@ -499,23 +519,26 @@ __device__ __noinline__ bool excluded_doc(const uint4* arena, const uint4* block
 }
 
 // The same with OR groups: is doc d rejected because an excluded list holds it, or because some group tagged in `grp`
-// has no list that holds it? A group's remaining lists are skipped once one of them holds d.
+// has fewer than m_g lists that hold it? A group's remaining lists are skipped once m_g of them hold d, and d is rejected
+// as soon as a group's remaining lists cannot reach m_g.
 __device__ __noinline__ bool excluded_doc(const uint4* arena, const uint4* blocks, const uint4* anchors, const uint2* ex,
                                           const uint8_t* grp, uint32_t n, uint32_t d) {
-  const uint32_t need = check_group_mask(grp, n);
+  GroupNeed st = check_group_need(grp, n);
   PostingsDev S{};
   S.arena = arena; S.blocks = blocks; S.anchors = anchors;
-  uint32_t got = 0u;
   for (uint32_t x = 0; x < n; ++x) {
     const uint32_t g = grp[x];
-    if (g != kCheckExcl && ((got >> g) & 1u)) continue;
+    const uint32_t g4 = 4u * (g & 15u);
+    if (g != kCheckExcl && ((st.need >> g4) & 15ull) == 0ull) continue;
     uint32_t blk = 0;
-    if (probe_contains(S, ex[x], d, 0u, blk)) {
-      if (g == kCheckExcl) return true;
-      got |= 1u << g;
+    const bool hit = probe_contains(S, ex[x], d, 0u, blk);
+    if (g == kCheckExcl) {
+      if (hit) return true;
+    } else if (!group_step(st, g4, hit)) {
+      return true;
     }
   }
-  return got != need;
+  return st.need != 0ull;
 }
 
 // kDrive compiles the driver-mode code (pruning level 2) in; the default kernel stays free of its registers. kExcl: the

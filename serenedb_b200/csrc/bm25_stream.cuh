@@ -304,23 +304,26 @@ __device__ __noinline__ bool stream_excl_pass(const PostingsDev* S, StreamExcl* 
 // shared memory.
 struct StreamGroups {
   uint2 list[kMaxCheckLists];
-  uint8_t grp[kMaxCheckLists];                    // kCheckExcl or the list's group index
+  uint8_t grp[kMaxCheckLists];                    // kCheckExcl or the list's group tag
   uint32_t n;
-  uint32_t need;                                  // bit g: group g must hold the doc
+  uint32_t e0;                                    // live terms at the start of the scan (pigeonhole lead; else T)
+  GroupNeed need;                                 // per-group counters at the start of a doc's check
   uint32_t hint[kTopkWarps][kMaxCheckLists];      // per warp and list: block where the warp's last probe ended
 };
 
-// The same with OR groups: false for lanes whose doc occurs in an excluded list, or whose doc no list of some required
-// group holds; else `alive`. A lane stops probing a group once one of its lists holds the doc.
+// The same with OR groups: false for lanes whose doc occurs in an excluded list, or whose doc fewer than m_g lists of
+// some required group hold; else `alive`. A lane stops probing a group once m_g of its lists hold the doc, and rejects
+// the doc once the group's remaining lists cannot reach m_g.
 __device__ __noinline__ bool stream_excl_pass(const PostingsDev* S, StreamGroups* X, bool alive, uint32_t d) {
   const uint32_t lane = threadIdx.x & 31u;
   uint32_t* const hint = X->hint[threadIdx.x >> 5];
-  uint32_t got = 0u;
+  GroupNeed st = X->need;
   for (uint32_t x = 0; x < X->n; ++x) {
     if (!__any_sync(kFull, alive)) break;
     const uint32_t g = X->grp[x];
+    const uint32_t g4 = 4u * (g & 15u);
     const bool excl = g == kCheckExcl;
-    const bool probe = alive && (excl || ((got >> g) & 1u) == 0u);
+    const bool probe = alive && (excl || ((st.need >> g4) & 15ull) != 0ull);
     uint32_t fb = 0u;
     bool hit = false;
     if (probe) hit = probe_contains(*S, X->list[x], d, hint[x], fb);
@@ -332,9 +335,9 @@ __device__ __noinline__ bool stream_excl_pass(const PostingsDev* S, StreamGroups
       __syncwarp();
     }
     if (excl) alive = alive && !hit;
-    else if (hit) got |= 1u << g;
+    else if (probe) alive = group_step(st, g4, hit);
   }
-  return alive && (got & X->need) == X->need;
+  return alive && st.need == 0ull;
 }
 
 // Candidate buffer full: exact radix select keeps the best k and raises the thresholds. Called by every thread of the
@@ -427,7 +430,14 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
     const uint32_t n_ex = min(P.excl_off[q + 1] - x0, kMaxCheckLists);
     if (tid < n_ex) { s_x.list[tid] = P.excl[x0 + tid]; s_x.grp[tid] = P.excl_grp[x0 + tid]; }
     for (uint32_t i = tid; i < kTopkWarps * kMaxCheckLists; i += blockDim.x) (&s_x.hint[0][0])[i] = 0u;
-    if (tid == 0) { s_x.n = n_ex; s_x.need = check_group_mask(P.excl_grp + x0, n_ex); }
+    if (tid == 0) {
+      s_x.n = n_ex;
+      s_x.need = check_group_need(P.excl_grp + x0, n_ex);
+      // Pigeonhole lead: a query of one group with m >= 2 ("m of n") matches only docs that one of its n - m + 1
+      // shortest lists holds. Only those are streamed; its m - 1 longest lists are probed per candidate from the start.
+      const unsigned long long nd = s_x.need.need;
+      s_x.e0 = (nd >> 4) == 0ull && nd >= 2ull ? T + 1u - uint32_t(nd) : T;
+    }
   } else if constexpr (kExcl) {
     const uint32_t x0 = P.excl_off[q];
     const uint32_t n_ex = min(P.excl_off[q + 1] - x0, kMaxQueryTerms);
@@ -514,6 +524,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
     // ---- candidates that still have lists to visit (probed terms) wait in a per-warp ring of 128 (doc, partial score);
     // a round looks 32 of them up at once, one per lane ----
     uint32_t E = T;                      // live terms 0 .. E-1 are streamed; terms E .. n_terms-1 are probed
+    if constexpr (kGroups) E = s_x.e0;
     uint32_t qhead = 0u, qcount = 0u;
     uint32_t* const qd = kProbeRest ? reinterpret_cast<uint32_t*>(mine + T * kStreamTermBytes) : live_docs(T - 1u);   // plain OR: the ring
     float* const qs = kProbeRest ? reinterpret_cast<float*>(mine + T * kStreamTermBytes + 512u) : live_scores(T - 1u);  // reuses the dropped top list's arrays
@@ -738,6 +749,13 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
 #pragma unroll
     for (uint32_t t = 0; t < T; ++t) {
       const uint32_t st = warp_first_block(P.seg.blocks + s_qt[t].blk_begin, s_qt[t].nblk, lo_w, lane);
+      if (kGroups && t >= E) {
+        // probed from the start (pigeonhole lead): never loaded, so nothing to drain; the top list's arrays hold the ring
+        if (lane == 0) s_hint[warp][t] = st;
+        cur[t] = s_qt[t].nblk; widx[t] = 0u; rr[t] = 0u;
+        fr[t] = kNoDoc; nxt[t] = kNoDoc; a0[t] = 128u;
+        continue;
+      }
       cur[t] = st; widx[t] = 0u; rr[t] = 0u;
       load_window(t, st);
       if (st < s_qt[t].nblk) prefetch(t, 0u, 0u);

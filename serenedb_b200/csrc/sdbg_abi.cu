@@ -1024,8 +1024,9 @@ int check_query_batch(sdbg_segment* const* segs, size_t n_segs, const Term* term
 }
 
 // excl_terms / excl_off: query q excludes the term ids excl_terms[excl_off[q] .. excl_off[q + 1]) (NULL excl_off: none).
-// term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] (0..15)
-// of its query. It runs as the OR of all its terms, and a doc must also occur in a list of every group.
+// term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] & 15
+// of its query, which needs (term_grp[i] >> 4) + 1 of its lists. It runs as the OR of all its terms, and a doc must also
+// occur in that many lists of every group.
 int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
              size_t nq, float k1, const float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, TopkDevOut* dev,
              const uint32_t* excl_terms = nullptr, const uint32_t* excl_off = nullptr, const uint8_t* term_grp = nullptr) {
@@ -1517,12 +1518,16 @@ struct GroupSplit {
   std::vector<uint8_t> term_grp[3];
 };
 
-// Checks of sdbg_*_batch_groups beyond check_query_batch (which each sub-batch runs as well) and the split by shape:
+// Checks of sdbg_*_batch_groups(_min) beyond check_query_batch (which each sub-batch runs as well) and the split by shape:
 // non-decreasing query_group_off / group_off / excl_off, 1..16 groups, 1..16 positive terms and at most 16 excluded ones
-// per query, no empty group, no positive term id twice in a query.
+// per query, no empty group, no positive term id twice in a query, 1 <= group_min[g] <= the group's size.
+// group_min (NULL: every group 1) is normalised first: a group that needs all its s terms is s single-term groups, so
+// that a query whose groups then all need 1 term takes the shapes above with exactly their results. The remaining queries
+// (some group needs 2 <= m < s terms, so m <= 15) run with their groups, and each term's tag carries m - 1 in its high
+// nibble (kCheckExcl's comment).
 template <class Term>
-int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, const uint32_t* query_group_off, size_t nq,
-                 const uint32_t* excl_terms, const uint32_t* excl_off, GroupSplit<Term>& S) {
+int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, const uint32_t* query_group_off,
+                 const uint32_t* group_min, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, GroupSplit<Term>& S) {
   for (size_t q = 0; q < nq; ++q) {
     if (query_group_off[q + 1] < query_group_off[q]) return fail(c, SDBG_EINVAL, "query_group_off must be non-decreasing");
     for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g)
@@ -1537,8 +1542,11 @@ int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, cons
     if (excl_off && excl_off[q + 1] - excl_off[q] > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
   }
   for (size_t q = 0; q < nq; ++q) {
-    for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g)
+    for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g) {
       if (group_off[g + 1] == group_off[g]) return fail(c, SDBG_EINVAL, "empty OR group");
+      if (group_min && (group_min[g] == 0 || group_min[g] > group_off[g + 1] - group_off[g]))
+        return fail(c, SDBG_EINVAL, "a group's minimum match count must be 1..its number of terms");
+    }
     const uint32_t t0 = group_off[query_group_off[q]], t1 = group_off[query_group_off[q + 1]];
     if (!terms) return fail(c, SDBG_EINVAL, "terms is NULL");
     if (excl_off && excl_off[q + 1] > excl_off[q] && !excl_terms) return fail(c, SDBG_EINVAL, "excl_terms is NULL");
@@ -1552,13 +1560,25 @@ int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, cons
   for (size_t q = 0; q < nq; ++q) {
     const uint32_t g0 = query_group_off[q], g1 = query_group_off[q + 1];
     const uint32_t t0 = group_off[g0], t1 = group_off[g1];
-    const int sh = g1 - g0 == 1 ? 0 : (t1 - t0 == g1 - g0 ? 1 : 2);
+    // normalised groups: m == s becomes s single-term groups; a group of 2 <= m < s keeps its m
+    uint32_t n_groups = 0;
+    bool min_group = false;
+    for (uint32_t g = g0; g < g1; ++g) {
+      const uint32_t s = group_off[g + 1] - group_off[g], m = group_min ? group_min[g] : 1u;
+      if (m == s) n_groups += s;
+      else { ++n_groups; min_group |= m > 1u; }
+    }
+    const int sh = min_group ? 2 : n_groups == 1 ? 0 : (t1 - t0 == n_groups ? 1 : 2);
     S.qs[sh].push_back(q);
-    for (uint32_t g = g0; g < g1; ++g)
+    uint32_t gi = 0;
+    for (uint32_t g = g0; g < g1; ++g) {
+      const uint32_t s = group_off[g + 1] - group_off[g], m = group_min ? group_min[g] : 1u;
       for (uint32_t i = group_off[g]; i < group_off[g + 1]; ++i) {
         S.terms[sh].push_back(terms[i]);
-        if (sh == 2) S.term_grp[sh].push_back(uint8_t(g - g0));
+        if (sh == 2) S.term_grp[sh].push_back(m == s ? uint8_t(gi++) : uint8_t(gi | ((m - 1u) << 4)));
       }
+      if (m != s) ++gi;
+    }
     S.term_off[sh].push_back(uint32_t(S.terms[sh].size()));
     if (excl_off)
       for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) S.excl_terms[sh].push_back(excl_terms[i]);
@@ -1569,14 +1589,14 @@ int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, cons
 }  // namespace
 
 // Top-k of group queries: each shape through topk_batch_host; a batch of one shape writes straight into the caller's arrays.
-extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
-                                           const uint32_t* group_off, const uint32_t* query_group_off, size_t nq,
-                                           const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b,
-                                           const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
-                                           uint32_t* n_out, uint64_t* total_matches) {
+extern "C" int sdbg_bm25_topk_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                               const uint32_t* group_off, const uint32_t* query_group_off, const uint32_t* group_min,
+                                               size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b,
+                                               const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
+                                               uint32_t* n_out, uint64_t* total_matches) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !out || !n_out) return SDBG_EINVAL;
   GroupSplit<sdbg_bm25_term> S;
-  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, nq, excl_terms, excl_off, S)) return rc;
+  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
   for (int sh = 0; sh < 3; ++sh) {
     const size_t n = S.qs[sh].size();
     if (!n) continue;
@@ -1603,11 +1623,21 @@ extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_s
   return SDBG_OK;
 }
 
+extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                           const uint32_t* group_off, const uint32_t* query_group_off, size_t nq,
+                                           const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b,
+                                           const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
+                                           uint32_t* n_out, uint64_t* total_matches) {
+  return sdbg_bm25_topk_batch_groups_min(segs, n_segs, terms, group_off, query_group_off, nullptr, nq, excl_terms, excl_off, k1, b,
+                                         filt, k, threshold_in, out, n_out, total_matches);
+}
+
 // Count mode (duckdb_search_full_scan RunCountScan): bm25_count_kernel over work items {query, first window, windows} of
 // kCountWindow-doc windows, planned per segment from posting counts and issued largest first. A single-term query over a
 // segment without filter, deleted docs or an excluded list holding blocks there is answered from the term's docs_count.
-// term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] of its
-// query (groups 0 .. n - 1 all present); those queries run bm25_count_kernel<false, true>.
+// term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] & 15 of
+// its query (groups 0 .. n - 1 all present), which needs (term_grp[i] >> 4) + 1 of its lists; those queries run
+// bm25_count_kernel<false, true>.
 // sort (NULL: count): the sorted scan of sdbg_match_topk_by_column_batch on the same plan, without the single-term
 // shortcut; see sort_prepare / sort_finish.
 // facet (NULL: count): the facet pass of sdbg_match_facet_counts_batch on the same plan and launches, without the
@@ -1888,11 +1918,15 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
   std::vector<uint2> lists(n_lists * n_segs);
   // OR groups: grp_off[q] .. grp_off[q + 1] index each segment's group ends (relative to term_off[q]), lead group first
   std::vector<uint32_t> grp_off, grp_end;
+  uint32_t max_min = 1;   // largest group minimum of the batch: sizes the count kernel's bit-sliced counter
   if (term_grp) {
     grp_off.assign(nq + 1, 0u);
     for (size_t q = 0; q < nq; ++q) {
       uint32_t ng = 0;
-      for (uint32_t i = term_off[q]; i < term_off[q + 1]; ++i) ng = std::max(ng, uint32_t(term_grp[i]) + 1u);
+      for (uint32_t i = term_off[q]; i < term_off[q + 1]; ++i) {
+        ng = std::max(ng, uint32_t(term_grp[i] & 15u) + 1u);
+        max_min = std::max(max_min, uint32_t(term_grp[i] >> 4) + 1u);
+      }
       grp_off[q + 1] = grp_off[q] + ng;
     }
     grp_end.assign(size_t(grp_off[nq]) * n_segs, 0u);
@@ -1920,21 +1954,37 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
         smallest = std::min(smallest, dc);
       }
       if (term_grp) {
-        // groups by ascending summed docs_count: the lead group (the cheapest) fills the window bitmap and the most
-        // selective groups narrow it first
+        // Each group's lists by ascending docs_count; a group of s lists that needs m of them costs its s - m + 1
+        // shortest lists (all of them for m = 1), which is what it leads with. Groups by ascending cost: the lead group
+        // (the cheapest) fills the window bitmap and the most selective groups narrow it first.
         const uint32_t ng = grp_off[q + 1] - grp_off[q];
         std::array<uint64_t, kMaxQueryTerms> gsum{};
-        std::array<uint32_t, kMaxQueryTerms> order{}, gsize{};
-        for (uint32_t i = t0; i < t1; ++i) { gsum[term_grp[i]] += by_docs[i - t0].first; ++gsize[term_grp[i]]; }
+        std::array<uint32_t, kMaxQueryTerms> order{}, gsize{}, gmin{}, gnz{}, seen{};
+        std::array<uint32_t, kMaxQueryTerms> by_cost{};   // positions i - t0, ascending docs_count
+        for (uint32_t i = t0; i < t1; ++i) {
+          const uint32_t g = term_grp[i] & 15u;
+          by_cost[i - t0] = i - t0;
+          gmin[g] = (term_grp[i] >> 4) + 1u;
+          ++gsize[g];
+          gnz[g] += by_docs[i - t0].first != 0u;
+        }
+        std::stable_sort(by_cost.begin(), by_cost.begin() + (t1 - t0), [&](uint32_t a, uint32_t b) { return by_docs[a].first < by_docs[b].first; });
+        for (uint32_t j = 0; j < t1 - t0; ++j) {
+          const uint32_t g = term_grp[t0 + by_cost[j]] & 15u;
+          if (seen[g]++ < gsize[g] - gmin[g] + 1u) gsum[g] += by_docs[by_cost[j]].first;
+        }
+        bool short_group = false;
+        for (uint32_t g = 0; g < ng; ++g) short_group |= gnz[g] < gmin[g];
         for (uint32_t g = 0; g < ng; ++g) order[g] = g;
         std::stable_sort(order.begin(), order.begin() + ng, [&](uint32_t a, uint32_t b) { return gsum[a] < gsum[b]; });
         uint32_t* gend = grp_end.data() + si * grp_off[nq] + grp_off[q];
         uint32_t o = 0;
         for (uint32_t j = 0; j < ng; ++j) {
-          for (uint32_t i = t0; i < t1; ++i) if (term_grp[i] == order[j]) L[t0 + o++] = by_docs[i - t0].second;
-          gend[j] = o;
+          for (uint32_t x = 0; x < t1 - t0; ++x)
+            if ((term_grp[t0 + by_cost[x]] & 15u) == order[j]) L[t0 + o++] = by_docs[by_cost[x]].second;
+          gend[j] = o | ((gmin[order[j]] - 1u) << 8);
         }
-        if (gsum[order[0]] == 0) continue;               // a group with no doc in this segment: no match here
+        if (short_group) continue;                       // a group with fewer than m non-empty lists here: no match
         const uint64_t weight = gsum[order[0]] * ng;
         uint32_t g = uint32_t(std::max<uint64_t>(G, (weight + chain_target - 1) / chain_target));
         g = std::min({g, n_win, 2u * uint32_t(c->sm_count)});
@@ -2011,6 +2061,14 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
       CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(facet_smem)));
       CU(c, cudaFuncSetAttribute(bm25_count_kernel<true, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(facet_smem)));
     }
+    // groups that need m >= 2 of their lists: a bit-sliced counter of bits(m) planes for the batch's largest m
+    size_t count_smem = 0;
+    if (max_min > 1u) {
+      uint32_t planes = 0;
+      while ((max_min >> planes) != 0u) ++planes;
+      count_smem = size_t(planes) * kCountWords * 4u;
+      CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(count_smem)));
+    }
     const char* d = static_cast<const char*>(b_desc.p);
     size_t done = 0;
     for (size_t si = 0; si < n_segs; ++si) {
@@ -2035,7 +2093,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
       } else if (term_grp) {
         P.grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
         P.grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[nq];
-        bm25_count_kernel<false, true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
+        bm25_count_kernel<false, true><<<unsigned(seg_work[si].size()), kCountThreads, count_smem, c->stream>>>(P);
       } else if (conj) bm25_count_kernel<true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
       else bm25_count_kernel<false><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
       ++c->launches;
@@ -2090,13 +2148,13 @@ extern "C" int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n
   return count_run(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, filt, nullptr, nullptr, nullptr, &J);
 }
 
-extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
-                                             const uint32_t* group_off, const uint32_t* query_group_off, size_t nq,
-                                             const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
-                                             uint64_t* counts) {
+extern "C" int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                 const uint32_t* group_off, const uint32_t* query_group_off,
+                                                 const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                 const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts) return SDBG_EINVAL;
   GroupSplit<uint32_t> S;
-  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, nq, excl_terms, excl_off, S)) return rc;
+  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
   for (int sh = 0; sh < 3; ++sh) {
     const size_t n = S.qs[sh].size();
     if (!n) continue;
@@ -2111,6 +2169,14 @@ extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n
       for (size_t j = 0; j < n; ++j) counts[S.qs[sh][j]] = cn[j];
   }
   return SDBG_OK;
+}
+
+extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                             const uint32_t* group_off, const uint32_t* query_group_off, size_t nq,
+                                             const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                             uint64_t* counts) {
+  return sdbg_match_count_batch_groups_min(segs, n_segs, terms, group_off, query_group_off, nullptr, nq, excl_terms, excl_off,
+                                           filt, counts);
 }
 
 // Streaming mode (duckdb_search_full_scan.cpp RunStreamingScan :2370-2403; DocIterator::EmitScoredDocs,

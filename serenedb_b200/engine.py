@@ -587,13 +587,24 @@ def _groups(queries):
     return [t for g in groups for t in g], group_off, query_group_off
 
 
-def ExecuteTopKGroupsBatch(reader, queries, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
-    """Top-k of conjunctions of OR groups (`a & (b | c) & !d`, sdbg_bm25_topk_batch_groups). queries: per query a list of
+def _group_min(min_match, queries):
+    """Per query one minimum per group -> group_min u32 indexed like group_off (None: every group needs 1 term)."""
+    if min_match is None:
+        return None
+    if len(min_match) != len(queries) or any(len(m) != len(q) for m, q in zip(min_match, queries)):
+        raise ValueError("min_match needs one value per group of each query")
+    return np.ascontiguousarray([int(v) for m in min_match for v in m], dtype=np.uint32)
+
+
+def ExecuteTopKGroupsBatch(reader, queries, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, min_match=None):
+    """Top-k of conjunctions of OR groups (`a & (b | c) & !d`, sdbg_bm25_topk_batch_groups_min). queries: per query a list of
     1..16 groups, each a non-empty list of term ids (1..16 distinct ids per query in all). A hit's score is the score the
-    flat OR of the query's terms gives that doc. exclude: as in ExecuteTopKBatch. Returns (hits [Q, k], n_out [Q],
-    total_matches [Q])."""
+    flat OR of the query's terms gives that doc. exclude: as in ExecuteTopKBatch. min_match: per query one minimum per
+    group (`2 of (a | b | c)`: a doc needs that many of the group's terms), 1..the group's size; None: 1 everywhere.
+    Returns (hits [Q, k], n_out [Q], total_matches [Q])."""
     nq = len(queries)
     ids, group_off, query_group_off = _groups(queries)
+    gmin = _group_min(min_match, queries)
     terms = (N.BM25Term * max(len(ids), 1))()
     for i, t in enumerate(ids):
         terms[i] = reader.stats(scorer, t)
@@ -602,41 +613,47 @@ def ExecuteTopKGroupsBatch(reader, queries, scorer, k, filt=None, threshold=FLT_
     total = np.zeros(nq, np.uint64)
     x = _exclusions(exclude, nq)
     fp = C.byref(filt) if filt is not None else None
-    N.check(N.lib().sdbg_bm25_topk_batch_groups(_seg_array(reader.segments), len(reader.segments), terms, _ptr(group_off),
-                                                _ptr(query_group_off), nq, _ptr(x[0]) if x is not None else None,
-                                                _ptr(x[1]) if x is not None else None, scorer.k, scorer.b, fp, int(k),
-                                                float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
+    N.check(N.lib().sdbg_bm25_topk_batch_groups_min(_seg_array(reader.segments), len(reader.segments), terms, _ptr(group_off),
+                                                    _ptr(query_group_off), _ptr(gmin) if gmin is not None else None, nq,
+                                                    _ptr(x[0]) if x is not None else None,
+                                                    _ptr(x[1]) if x is not None else None, scorer.k, scorer.b, fp, int(k),
+                                                    float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
     return hits, n_out, total
 
 
-def ExecuteTopKGroups(reader, groups, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
-    """ExecuteTopKGroupsBatch for one query (a list of OR groups): (hits, total_matches)."""
+def ExecuteTopKGroups(reader, groups, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, min_match=None):
+    """ExecuteTopKGroupsBatch for one query (a list of OR groups; min_match: one minimum per group): (hits, total_matches)."""
     hits, n_out, total = ExecuteTopKGroupsBatch(reader, [[list(g) for g in groups]], scorer, k, filt, threshold,
-                                                exclude=None if exclude is None else [list(exclude)])
+                                                exclude=None if exclude is None else [list(exclude)],
+                                                min_match=None if min_match is None else [list(min_match)])
     return hits[0, :n_out[0]].copy(), int(total[0])
 
 
-def ExecuteCountGroupsBatch(reader, queries, filt=None, exclude=None):
-    """Count mode for conjunctions of OR groups (sdbg_match_count_batch_groups): per query, the number of docs over all
-    segments in which every group has a term, that are not deleted, pass `filt` and hold none of its `exclude` term ids.
-    Exact at every pruning level. Returns uint64[Q]."""
+def ExecuteCountGroupsBatch(reader, queries, filt=None, exclude=None, min_match=None):
+    """Count mode for conjunctions of OR groups (sdbg_match_count_batch_groups_min): per query, the number of docs over all
+    segments in which every group has a term (min_match: per query one minimum per group, as in ExecuteTopKGroupsBatch),
+    that are not deleted, pass `filt` and hold none of its `exclude` term ids. Exact at every pruning level. Returns
+    uint64[Q]."""
     nq = len(queries)
     ids, group_off, query_group_off = _groups(queries)
+    gmin = _group_min(min_match, queries)
     flat = np.ascontiguousarray(ids, dtype=np.uint32)
     counts = np.zeros(nq, np.uint64)
     x = _exclusions(exclude, nq)
     fp = C.byref(filt) if filt is not None else None
-    N.check(N.lib().sdbg_match_count_batch_groups(_seg_array(reader.segments), len(reader.segments),
-                                                  _ptr(flat) if len(flat) else None, _ptr(group_off), _ptr(query_group_off), nq,
-                                                  _ptr(x[0]) if x is not None else None, _ptr(x[1]) if x is not None else None,
-                                                  fp, _ptr(counts)), reader.segments[0].ctx._h)
+    N.check(N.lib().sdbg_match_count_batch_groups_min(_seg_array(reader.segments), len(reader.segments),
+                                                      _ptr(flat) if len(flat) else None, _ptr(group_off), _ptr(query_group_off),
+                                                      _ptr(gmin) if gmin is not None else None, nq,
+                                                      _ptr(x[0]) if x is not None else None, _ptr(x[1]) if x is not None else None,
+                                                      fp, _ptr(counts)), reader.segments[0].ctx._h)
     return counts
 
 
-def ExecuteCountGroups(reader, groups, filt=None, exclude=None):
+def ExecuteCountGroups(reader, groups, filt=None, exclude=None, min_match=None):
     """ExecuteCountGroupsBatch for one query: its match count as an int."""
     return int(ExecuteCountGroupsBatch(reader, [[list(g) for g in groups]], filt,
-                                       exclude=None if exclude is None else [list(exclude)])[0])
+                                       exclude=None if exclude is None else [list(exclude)],
+                                       min_match=None if min_match is None else [list(min_match)])[0])
 
 
 FOR_BLOCK_DTYPE =np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])

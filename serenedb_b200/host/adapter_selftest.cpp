@@ -3,7 +3,8 @@
 // for tests/test_gpu_adapters.py to compare with the oracle. Needs a GPU at run time. With a second argument "excl" it runs
 // only the exclusion case instead (an And with a Not child, tests/test_gpu_exclusion.py); with "count", only the Count
 // scan mode (GpuCountScan, tests/test_gpu_count.py); with "groups", only an And of Or groups through both adapters
-// (tests/test_gpu_groups.py); with "sorted", only the sorted scan (GpuSortedScan, tests/test_gpu_sort_by_column.py); with
+// (tests/test_gpu_groups.py); with "minmatch", only an Or with min_match_count through both adapters
+// (tests/test_gpu_min_match.py); with "sorted", only the sorted scan (GpuSortedScan, tests/test_gpu_sort_by_column.py); with
 // "facet", only the facet counts (GpuFacetScan, tests/test_gpu_facets.py).
 #include <algorithm>
 #include <cstdio>
@@ -95,6 +96,45 @@ int main(int argc, char** argv) {
     int code = 0;   // k = 0 (the streaming scan) has no grouped form
     try { sdbg_host::GpuTopKIterator st(seg, SDBG_QUERY_OR, g3, 1.2f, 0.75f, 0, nullptr, {}, {1, 2}); } catch (const sdbg_host::GpuError& e) { code = e.code; }
     std::printf("{\"stream_error\": %d}\n", code);
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
+  if (argc > 2 && std::string(argv[2]) == "minmatch") {
+    // Or with min_match_count 2 over t2, t5, t6: alone (a root Or) and as the child of an And with t1, without and with the
+    // table filter: Collect (top-100) and count(*)
+    std::vector<sdbg_bm25_term> g4(4);
+    const uint32_t gids[4] = {1, 2, 5, 6};
+    for (int i = 0; i < 4; ++i) { sdbg_bm25_collect(n_docs, sum_dl, dc[gids[i]], 1.2f, 0.75f, &g4[size_t(i)]); g4[size_t(i)].term = gids[i]; }
+    ListCollector col;
+    irs::ScoreFunction sf; irs::ColumnArgsFetcher fetcher;
+    for (int nested = 0; nested < 2; ++nested)
+      for (int with_filter = 0; with_filter < 2; ++with_filter) {
+        const std::vector<sdbg_bm25_term> t = nested ? g4 : std::vector<sdbg_bm25_term>(g4.begin() + 1, g4.end());
+        const std::vector<uint32_t> ids = nested ? std::vector<uint32_t>{1, 2, 5, 6} : std::vector<uint32_t>{2, 5, 6};
+        const std::vector<uint32_t> sizes = nested ? std::vector<uint32_t>{1, 3} : std::vector<uint32_t>{3};
+        const std::vector<uint32_t> mins = nested ? std::vector<uint32_t>{1, 2} : std::vector<uint32_t>{2};
+        sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_OR, t, 1.2f, 0.75f, 100, with_filter ? &filt : nullptr, {}, sizes, mins);
+        col.docs.clear();
+        it.Collect(sf, fetcher, col);
+        std::printf("{\"nested\": %d, \"filter\": %d, \"topk\": [", nested, with_filter);
+        for (size_t i = 0; i < col.docs.size(); ++i) std::printf("%s[%u, %.9g]", i ? ", " : "", col.docs[i].doc, double(col.docs[i].score));
+        sdbg_host::GpuCountScan scan({seg}, SDBG_QUERY_OR, ids, {}, with_filter ? &filt : nullptr, sizes, mins);
+        duckdb::DataChunkMock chunk;
+        scan.Scan(chunk);
+        const long long count = chunk.size ? chunk.count[0] : -1;
+        scan.Scan(chunk);
+        std::printf("], \"total\": %llu, \"threshold\": %.9g, \"count\": %lld, \"rows_after\": %llu}\n",
+                    static_cast<unsigned long long>(it.total_matches()), double(it.threshold().value), count,
+                    static_cast<unsigned long long>(chunk.size));
+      }
+    int code = 0;   // a minimum above the group's size
+    try {
+      sdbg_host::GpuCountScan scan({seg}, SDBG_QUERY_OR, {2, 5, 6}, {}, nullptr, {3}, {4});
+      duckdb::DataChunkMock chunk;
+      scan.Scan(chunk);
+    } catch (const sdbg_host::GpuError& e) { code = e.code; }
+    std::printf("{\"min_error\": %d}\n", code);
     sdbg_segment_destroy(seg);
     sdbg_destroy(ctx);
     return 0;

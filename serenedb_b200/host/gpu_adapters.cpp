@@ -17,13 +17,20 @@ std::vector<uint32_t> group_offsets(const std::vector<uint32_t>& sizes, size_t n
   if (off.back() != n_terms) throw GpuError(SDBG_EINVAL, "OR group sizes must add up to the number of terms");
   return off;
 }
+
+// Per-group minimum match counts: one per group, or none (every group 1).
+const uint32_t* group_minimums(const std::vector<uint32_t>& mins, size_t n_groups) {
+  if (mins.empty()) return nullptr;
+  if (mins.size() != n_groups) throw GpuError(SDBG_EINVAL, "one minimum match count per OR group");
+  return mins.data();
+}
 }  // namespace
 
 GpuTopKIterator::GpuTopKIterator(sdbg_segment* segment, int kind, std::vector<sdbg_bm25_term> terms, float k1, float b,
                                  uint32_t k, const sdbg_col_pred* table_filter, std::vector<uint32_t> excluded_terms,
-                                 std::vector<uint32_t> group_sizes)
+                                 std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)
     : seg_(segment), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)), groups_(std::move(group_sizes)),
-      k1_(k1), b_(b), k_(k), has_filter_(table_filter != nullptr) {
+      group_min_(std::move(group_min_match)), k1_(k1), b_(b), k_(k), has_filter_(table_filter != nullptr) {
   if (table_filter) filter_ = *table_filter;
   threshold_.value = FLT_MIN;  // doc_collector.hpp:102
   // the streaming scan (sdbg_bm25_scan*) has no grouped form
@@ -60,9 +67,10 @@ void GpuTopKIterator::run() {
   if (!groups_.empty()) {
     const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
     const uint32_t query_group_off[2] = {0, uint32_t(groups_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
-    check(sdbg_bm25_topk_batch_groups(segs, 1, terms_.data(), group_off.data(), query_group_off, 1, excluded_.data(), excl_off, k1_, b_,
-                                      has_filter_ ? &filter_ : nullptr, k_, threshold_.value, hits_.data(), &n, &total_),
-          "sdbg_bm25_topk_batch_groups");
+    check(sdbg_bm25_topk_batch_groups_min(segs, 1, terms_.data(), group_off.data(), query_group_off,
+                                          group_minimums(group_min_, groups_.size()), 1, excluded_.data(), excl_off, k1_, b_,
+                                          has_filter_ ? &filter_ : nullptr, k_, threshold_.value, hits_.data(), &n, &total_),
+          "sdbg_bm25_topk_batch_groups_min");
     thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;
   } else if (excluded_.empty()) {
     check(sdbg_bm25_topk(segs, 1, kind_, terms_.data(), terms_.size(), k1_, b_, has_filter_ ? &filter_ : nullptr, k_,
@@ -191,9 +199,10 @@ void GpuAggScan::Scan(duckdb::DataChunkMock& output) {
 }
 
 GpuCountScan::GpuCountScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
-                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, std::vector<uint32_t> group_sizes)
+                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, std::vector<uint32_t> group_sizes,
+                           std::vector<uint32_t> group_min_match)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      groups_(std::move(group_sizes)), has_filter_(table_filter != nullptr) {
+      groups_(std::move(group_sizes)), group_min_(std::move(group_min_match)), has_filter_(table_filter != nullptr) {
   if (table_filter) filter_ = *table_filter;
 }
 
@@ -212,9 +221,10 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
   } else {                                                    // an And of Ors: kind_ is not used
     const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
     const uint32_t query_group_off[2] = {0, uint32_t(groups_.size())};
-    rc = sdbg_match_count_batch_groups(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off, 1,
-                                       excluded_.data(), excl_off, has_filter_ ? &filter_ : nullptr, &n);
-    what = "sdbg_match_count_batch_groups: ";
+    rc = sdbg_match_count_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
+                                           group_minimums(group_min_, groups_.size()), 1, excluded_.data(), excl_off,
+                                           has_filter_ ? &filter_ : nullptr, &n);
+    what = "sdbg_match_count_batch_groups_min: ";
   }
   if (rc != SDBG_OK) throw GpuError(rc, std::string(what) + sdbg_last_error(sdbg_segment_context(segs_[0])));
   output.count.push_back(int64_t(n));

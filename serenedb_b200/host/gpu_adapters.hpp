@@ -39,7 +39,8 @@ class GpuTopKIterator final : public irs::DocIterator {
                   float b /* BM25::b() */, uint32_t k /* 0 = streaming mode: every match, see EmitScoredDocs */,
                   const sdbg_col_pred* table_filter /* nullable: the ColFilter wrap */,
                   std::vector<uint32_t> excluded_terms = {} /* term ids of the And's Not children (irs exclusion.hpp) */,
-                  std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */);
+                  std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */,
+                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
 
   // Scored top-k: the hot path.
   void Collect(const irs::ScoreFunction&, irs::ColumnArgsFetcher&, irs::ScoreCollector& collector) override;
@@ -73,6 +74,7 @@ class GpuTopKIterator final : public irs::DocIterator {
   std::vector<sdbg_bm25_term> terms_;
   std::vector<uint32_t> excluded_;
   std::vector<uint32_t> groups_;   // sizes of the OR groups over terms_ (empty: the flat `kind_` query)
+  std::vector<uint32_t> group_min_;   // their minimum match counts (empty: all 1)
   float k1_, b_;
   uint32_t k_;
   bool has_filter_;
@@ -113,14 +115,15 @@ class GpuCountScan {
  public:
   GpuCountScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
-               std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */);
+               std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */,
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
   // Fills `output` with one row, count[0] = the number of matches; the next call leaves it empty (end of scan).
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, groups_;
+  std::vector<uint32_t> terms_, excluded_, groups_, group_min_;
   bool has_filter_;
   sdbg_col_pred filter_{};
   bool done_ = false;
