@@ -111,8 +111,8 @@ int sdbg_segment_set_wand_b(sdbg_segment*, float wand_b);
    bounds under their own (corpus-wide) average length, so pruning stays exact when the two averages differ. */
 int sdbg_segment_set_wand_avg_dl(sdbg_segment*, float avg_dl);
 /* Zonemap effect of the last GROUP BY or sorted scan. GROUP BY: 2048-row blocks judged / proven dead from their min-max
- * (never read). Sorted scan (sdbg_match_topk_by_column_batch): 65 536-doc windows judged / skipped before any list was
- * decoded. */
+ * (never read). Sorted scan (sdbg_match_topk_by_column_batch(_groups_min)): 65 536-doc windows judged / skipped before
+ * any list was decoded, over the whole call. */
 int sdbg_scan_stats(sdbg_ctx*, uint64_t* blocks_total, uint64_t* blocks_skipped);
 /* The context a segment was created in (for sdbg_last_error after a failed call that only has segments at hand). */
 sdbg_ctx* sdbg_segment_context(const sdbg_segment*);
@@ -278,6 +278,8 @@ int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int 
  * Errors: an empty group, a decreasing offset array, a positive term id twice in a query, or NULL arrays with non-empty
  * ranges: SDBG_EINVAL; more than 16 groups, positive terms or excluded terms in a query: SDBG_EUNSUPPORTED; otherwise the
  * errors of sdbg_bm25_topk_batch_excl / sdbg_match_count_batch.
+ * The sorted scan and facet counts of group queries: sdbg_match_topk_by_column_batch_groups_min /
+ * sdbg_match_facet_counts_batch_groups_min below.
  * Not supported yet: the streaming scan (sdbg_bm25_scan*), grouped forms of sdbg_bm25_topk_batch_device and
  * sdbg_dist_bm25_topk_batch, deeper nesting (an OR of ANDs), more than 16 positive terms, phrases. */
 int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
@@ -309,6 +311,26 @@ int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, 
                                       const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
                                       const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
                                       uint64_t* counts);
+/* Sorted scan and facet counts of group queries (`WHERE body @@ 'a & (b | c)' ORDER BY col LIMIT k`, `... GROUP BY col`):
+ * the query parameters of sdbg_match_count_batch_groups_min, then the output parameters of
+ * sdbg_match_topk_by_column_batch / sdbg_match_facet_counts_batch. Per query, the docs sdbg_match_count_batch_groups_min
+ * counts, sorted or counted per key under exactly the rules of those entries (column types, NULLs, ties, n_out =
+ * min(k, matches), the dense counts layout, sum(counts[q, :]) + null_counts[q] == the count); identical at every pruning
+ * level. Degenerate queries normalise as in the groups entries and give exactly the flat entries' results. After a sorted
+ * call, sdbg_scan_stats reports the windows of the whole call. Errors: those of sdbg_match_count_batch_groups_min and of
+ * the flat entry, all found before anything is queued, except the facet pass's out-of-range key, found after the scan. */
+int sdbg_match_topk_by_column_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                               const uint32_t* group_off, const uint32_t* query_group_off,
+                                               const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                               const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                               const sdbg_col_pred* filt, uint64_t sort_field, int descending, int nulls_first,
+                                               uint32_t k, sdbg_sort_hit* out /* n_queries * k */, uint32_t* n_out);
+int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                             const uint32_t* group_off, const uint32_t* query_group_off,
+                                             const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                             const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                             const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                             uint64_t* counts /* n_queries * key_span */, uint64_t* null_counts /* n_queries */);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

@@ -109,6 +109,10 @@ SIGNATURES = {
     "sdbg_bm25_topk_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, C.c_float, C.c_float, _vp,
                                                   C.c_uint32, C.c_float, _vp, _vp, _vp]),
     "sdbg_match_count_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "sdbg_match_topk_by_column_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
+                                                             C.c_int, C.c_int, C.c_uint32, _vp, _vp]),
+    "sdbg_match_facet_counts_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
+                                                           C.c_int64, C.c_uint32, _vp, _vp]),
     "sdbg_topk_merge_gathered": (C.c_int, [_vp, _vp, C.c_uint32, _sz, C.c_uint32, _vp, _vp]),
     "sdbg_decode_score_term": (C.c_int, [_vp, C.c_uint32, C.c_float, C.c_float, C.c_float, _vp, _vp, _vp]),
     "sdbg_filter_bitmap": (C.c_int, [_vp, _vp, _sz, _vp]),

@@ -137,11 +137,12 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
 // k best go to output slot item.w.
 // kFacet: the facet pass (bm25_facet.cuh). Besides the popcount, every surviving doc's key is counted in the item's
 // histogram of P.facet.span u32 bins in dynamic shared memory, flushed to the query's row of P.facet.counts at the end.
+// Both sinks take kGroups queries: the groups narrow `acc` before the sink reads the column, and the bit-sliced counter
+// planes follow the sink's region of dynamic shared memory (16 * cap B, or 4 * span B rounded up to 16 B).
 template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false>
 __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
   static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
-  static_assert(!(kSort && kGroups), "the sorted scan takes OR / AND queries");
-  static_assert(!(kFacet && (kSort || kGroups)), "the facet pass takes OR / AND queries and has its own sink");
+  static_assert(!(kFacet && kSort), "the facet pass has its own sink");
   __shared__ uint32_t acc[kCountWords];
   __shared__ uint32_t tmp[kAnd || kGroups ? kCountWords : 1];
   __shared__ uint32_t stage[kCountWarps][128];
@@ -155,7 +156,8 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   __shared__ unsigned long long s_sum[kCountWarps];
   __shared__ unsigned long long s_thr[1];   // kSort: this item's best known k-th hi
   __shared__ uint32_t s_fill[1], s_zmask[2];  // kSort: keys in the buffer (kFacet: NULL keys); the window's zones that can reach s_thr
-  extern __shared__ unsigned long long sort_buf[];   // kSort: hi[cap] | lo[cap]; kFacet: the u32 bins
+  // kSort: hi[cap] | lo[cap]; kFacet: the u32 bins, padded to 16 B; then (kGroups) the bit-sliced counter planes
+  extern __shared__ unsigned long long sort_buf[];
   uint32_t* const bins = reinterpret_cast<uint32_t*>(sort_buf);
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
@@ -293,7 +295,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
         } else {
           // at least m of the lists: each list's bitmap is added into a saturating bit-sliced counter (plane p = bit p)
           const uint32_t np = 32u - __clz(m);
-          uint32_t* const plane = bins;
+          uint32_t* const plane = bins + (kSort ? 4u * P.sort.cap : kFacet ? (P.facet.span + 3u) & ~3u : 0u);
           for (uint32_t i = tid; i < np * kCountWords; i += kCountThreads) plane[i] = 0u;
           for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
           for (uint32_t li = lo; li < hi; ++li) {

@@ -1637,7 +1637,7 @@ extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_s
 // segment without filter, deleted docs or an excluded list holding blocks there is answered from the term's docs_count.
 // term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] & 15 of
 // its query (groups 0 .. n - 1 all present), which needs (term_grp[i] >> 4) + 1 of its lists; those queries run
-// bm25_count_kernel<false, true>.
+// bm25_count_kernel<false, true> (with sort / facet: <false, true, true> / <false, true, false, true>).
 // sort (NULL: count): the sorted scan of sdbg_match_topk_by_column_batch on the same plan, without the single-term
 // shortcut; see sort_prepare / sort_finish.
 // facet (NULL: count): the facet pass of sdbg_match_facet_counts_batch on the same plan and launches, without the
@@ -1654,12 +1654,17 @@ struct FacetJob {
   std::vector<FacetSink> sink;   // per segment, filled by facet_prepare (output pointers set at launch)
 };
 
+int facet_check_range(sdbg_ctx* c, int64_t key_min, uint32_t span) {
+  if (span == 0) return fail(c, SDBG_EINVAL, "key_span is 0");
+  if (key_min > INT64_MAX - int64_t(span - 1)) return fail(c, SDBG_EINVAL, "key_min + key_span - 1 overflows int64");
+  if (span > kFacetMaxSpan) return fail(c, SDBG_EUNSUPPORTED, "key_span > 32768 (the bins are shared memory)");
+  return SDBG_OK;
+}
+
 // Checks the key range and the key column of every segment, then fills the per-segment sinks. Every check runs before
 // anything is queued (a packed column's raw view is decoded on first use).
 int facet_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, FacetJob& J) {
-  if (J.span == 0) return fail(c, SDBG_EINVAL, "key_span is 0");
-  if (J.key_min > INT64_MAX - int64_t(J.span - 1)) return fail(c, SDBG_EINVAL, "key_min + key_span - 1 overflows int64");
-  if (J.span > kFacetMaxSpan) return fail(c, SDBG_EUNSUPPORTED, "key_span > 32768 (the bins are shared memory)");
+  if (int rc = facet_check_range(c, J.key_min, J.span)) return rc;
   for (size_t si = 0; si < n_segs; ++si) {
     auto it = segs[si]->cols.find(J.field);
     if (it == segs[si]->cols.end()) return fail(c, SDBG_ENOTFOUND, "key column not staged in every segment");
@@ -1762,30 +1767,58 @@ unsigned long long sort_window_bound(const SortJob& J, size_t si, uint32_t w) {
 
 struct CountItem { uint32_t q, w0, nw; uint64_t weight; bool seed = false; };
 
+// Raises `kernel`'s dynamic shared memory limit to `bytes` when a launch with them needs it: by default a launch may
+// take 48 KB minus the kernel's static shared memory (9.1 / 17.4 KB for the count kernels).
+template <class Kernel>
+cudaError_t fit_dynamic_smem(Kernel* kernel, size_t bytes) {
+  cudaFuncAttributes a;
+  cudaError_t e = cudaFuncGetAttributes(&a, kernel);
+  if (e == cudaSuccess && bytes + a.sharedSizeBytes > 48 * 1024)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes));
+  return e;
+}
+
+// Planes of the bit-sliced counter for groups that need up to max_min of their lists: bits(max_min), none for 1.
+uint32_t count_planes(uint32_t max_min) {
+  uint32_t planes = 0;
+  if (max_min > 1u)
+    while ((max_min >> planes) != 0u) ++planes;
+  return planes;
+}
+
 // Launches of the sorted scan over the planned items: per segment its seed items first (all segments), then the rest,
 // each item writing its k best to its own slot (its index in the work array); then sort_merge_kernel per query.
+// grp_off / grp_end (empty: no groups): count_run's OR groups, run by the grouped sorted scan with `planes` counter planes.
 int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const uint32_t* term_off, const uint32_t* excl_off,
                 size_t nq, uint32_t n_pos, uint32_t total_excl, const std::vector<uint2>& lists,
-                const std::vector<std::vector<CountItem>>& seg_work, const sdbg_col_pred* filt, SortJob& J) {
+                const std::vector<std::vector<CountItem>>& seg_work, const sdbg_col_pred* filt,
+                const std::vector<uint32_t>& grp_off, const std::vector<uint32_t>& grp_end, uint32_t planes, SortJob& J) {
   const size_t n_lists = size_t(n_pos) + total_excl;
   const uint32_t k = J.k, cap = J.sink[0].cap;
+  const bool groups = !grp_off.empty();
   size_t total = 0;
   bool any_zone = false;
   for (size_t si = 0; si < n_segs; ++si) { total += seg_work[si].size(); any_zone |= J.sink[si].zone != nullptr; }
-  // host staging: [term_off | excl_off | lists per segment | work items | slot_off | slots | segments]
+  // host staging: [term_off | excl_off | lists per segment | work items | slot_off | slots | segments | grp_off |
+  // group ends per segment]
   const size_t off_bytes = (nq + 1) * 4;
   const size_t lists_pos = (2 * off_bytes + 7) & ~size_t(7);
   const size_t work_pos = (lists_pos + lists.size() * sizeof(uint2) + 15) & ~size_t(15);
   const size_t slot_off_pos = work_pos + total * sizeof(uint4);
   const size_t slots_pos = slot_off_pos + off_bytes;
   const size_t segs_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
-  const size_t bytes = segs_pos + n_segs * sizeof(SortSegDev);
+  const size_t grp_pos = segs_pos + n_segs * sizeof(SortSegDev);
+  const size_t bytes = grp_pos + (groups ? off_bytes + grp_end.size() * 4 : 0);
   int rc = ensure_pinned(c, bytes);
   if (rc) return rc;
   char* h = static_cast<char*>(c->h_pinned);
   std::memcpy(h, term_off, off_bytes);
   if (total_excl) std::memcpy(h + off_bytes, excl_off, off_bytes);
   std::memcpy(h + lists_pos, lists.data(), lists.size() * sizeof(uint2));
+  if (groups) {
+    std::memcpy(h + grp_pos, grp_off.data(), off_bytes);
+    std::memcpy(h + grp_pos + off_bytes, grp_end.data(), grp_end.size() * 4);
+  }
   auto* hw = reinterpret_cast<uint4*>(h + work_pos);
   auto* h_slot_off = reinterpret_cast<uint32_t*>(h + slot_off_pos);
   auto* h_slots = reinterpret_cast<uint32_t*>(h + slots_pos);
@@ -1821,6 +1854,10 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const uin
   CU(c, cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaMemsetAsync(thr, 0, nq * 8 + 16, c->stream));   // thresholds and stats
   const size_t smem = size_t(cap) * 16;
+  // groups: the counter planes follow the keys (k = 4096 with 4 planes: 128 + 32 KB)
+  const size_t grp_smem = smem + size_t(planes) * kCountWords * 4u;
+  if (groups)
+    CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(grp_smem)));
   CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   CU(c, cudaFuncSetAttribute(bm25_count_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   CU(c, cudaFuncSetAttribute(sort_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
@@ -1847,7 +1884,11 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const uin
         P.sort.out = reinterpret_cast<ulonglong2*>(o);
         P.sort.out_n = reinterpret_cast<uint32_t*>(o + keys_n_pos);
         P.sort.stats = stats;
-        if (J.kind_and) bm25_count_kernel<true, false, true><<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
+        if (groups) {
+          P.grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
+          P.grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[nq];
+          bm25_count_kernel<false, true, true><<<unsigned(n), kCountThreads, grp_smem, c->stream>>>(P);
+        } else if (J.kind_and) bm25_count_kernel<true, false, true><<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
         else bm25_count_kernel<false, false, true><<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
         ++c->launches;
       }
@@ -1953,6 +1994,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
         sum += dc;
         smallest = std::min(smallest, dc);
       }
+      uint64_t weight;
       if (term_grp) {
         // Each group's lists by ascending docs_count; a group of s lists that needs m of them costs its s - m + 1
         // shortest lists (all of them for m = 1), which is what it leads with. Groups by ascending cost: the lead group
@@ -1985,23 +2027,18 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
           gend[j] = o | ((gmin[order[j]] - 1u) << 8);
         }
         if (short_group) continue;                       // a group with fewer than m non-empty lists here: no match
-        const uint64_t weight = gsum[order[0]] * ng;
-        uint32_t g = uint32_t(std::max<uint64_t>(G, (weight + chain_target - 1) / chain_target));
-        g = std::min({g, n_win, 2u * uint32_t(c->sm_count)});
-        const uint32_t per = (n_win + g - 1) / g;
-        for (uint32_t w0 = 0; w0 < n_win; w0 += per)
-          seg_work[si].push_back({uint32_t(q), w0, std::min(per, n_win - w0), weight / g});
-        continue;
+        weight = gsum[order[0]] * ng;
+      } else {
+        // ascending docs_count: the shortest list of a conjunction fills the window bitmap
+        std::stable_sort(by_docs.begin(), by_docs.begin() + (t1 - t0), [](const auto& a, const auto& b) { return a.first < b.first; });
+        for (uint32_t i = t0; i < t1; ++i) L[i] = by_docs[i - t0].second;
+        if (conj ? smallest == 0 : sum == 0) continue;
+        bool excl_blocks = false;
+        if (total_excl)
+          for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) excl_blocks |= L[n_pos + i].y != 0;
+        if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks && !sort && !facet) { host[q] += sum; continue; }
+        weight = conj ? uint64_t(smallest) * (t1 - t0) : sum;
       }
-      // ascending docs_count: the shortest list of a conjunction fills the window bitmap
-      std::stable_sort(by_docs.begin(), by_docs.begin() + (t1 - t0), [](const auto& a, const auto& b) { return a.first < b.first; });
-      for (uint32_t i = t0; i < t1; ++i) L[i] = by_docs[i - t0].second;
-      if (conj ? smallest == 0 : sum == 0) continue;
-      bool excl_blocks = false;
-      if (total_excl)
-        for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) excl_blocks |= L[n_pos + i].y != 0;
-      if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks && !sort && !facet) { host[q] += sum; continue; }
-      const uint64_t weight = conj ? uint64_t(smallest) * (t1 - t0) : sum;
       uint32_t g = uint32_t(std::max<uint64_t>(G, (weight + chain_target - 1) / chain_target));
       g = std::min({g, n_win, 2u * uint32_t(c->sm_count)});
       const uint32_t per = (n_win + g - 1) / g;
@@ -2026,7 +2063,8 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
   }
   if (sort) {
     sort->kind_and = conj;
-    return sort_finish(c, segs, n_segs, term_off, excl_off, nq, n_pos, total_excl, lists, seg_work, filt, *sort);
+    return sort_finish(c, segs, n_segs, term_off, excl_off, nq, n_pos, total_excl, lists, seg_work, filt, grp_off, grp_end,
+                       count_planes(max_min), *sort);
   }
   if (total_items) {
     // [term_off | excl_off | lists per segment | work items | grp_off | group ends per segment]
@@ -2057,18 +2095,17 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
     CU(c, cudaMemsetAsync(b_counts.p, 0, out_bytes, c->stream));
     char* fo = static_cast<char*>(b_counts.p);
     const size_t facet_smem = facet ? (size_t(facet->span) * 4 + 15) & ~size_t(15) : 0;
-    if (facet && facet_smem > 48 * 1024) {
-      CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(facet_smem)));
-      CU(c, cudaFuncSetAttribute(bm25_count_kernel<true, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(facet_smem)));
+    if (facet && !term_grp) {
+      CU(c, fit_dynamic_smem(bm25_count_kernel<false, false, false, true>, facet_smem));
+      CU(c, fit_dynamic_smem(bm25_count_kernel<true, false, false, true>, facet_smem));
     }
-    // groups that need m >= 2 of their lists: a bit-sliced counter of bits(m) planes for the batch's largest m
-    size_t count_smem = 0;
-    if (max_min > 1u) {
-      uint32_t planes = 0;
-      while ((max_min >> planes) != 0u) ++planes;
-      count_smem = size_t(planes) * kCountWords * 4u;
+    // groups that need m >= 2 of their lists: a bit-sliced counter of bits(m) planes for the batch's largest m, after the
+    // facet bins (at most 128 + 32 KB)
+    const size_t count_smem = size_t(count_planes(max_min)) * kCountWords * 4u;
+    if (term_grp && facet)
+      CU(c, fit_dynamic_smem(bm25_count_kernel<false, true, false, true>, facet_smem + count_smem));
+    else if (term_grp && count_smem)
       CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(count_smem)));
-    }
     const char* d = static_cast<const char*>(b_desc.p);
     size_t done = 0;
     for (size_t si = 0; si < n_segs; ++si) {
@@ -2083,16 +2120,20 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
       P.work = reinterpret_cast<const uint4*>(d + work_pos) + done;
       P.counts = static_cast<unsigned long long*>(b_counts.p);
       done += seg_work[si].size();
+      if (term_grp) {
+        P.grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
+        P.grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[nq];
+      }
       if (facet) {
         P.facet = facet->sink[si];
         P.facet.counts = reinterpret_cast<unsigned long long*>(fo + fc_pos);
         P.facet.nulls = reinterpret_cast<unsigned long long*>(fo + fn_pos);
         P.facet.out_of_range = reinterpret_cast<unsigned int*>(fo + oor_pos);
-        if (conj) bm25_count_kernel<true, false, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem, c->stream>>>(P);
+        if (term_grp)
+          bm25_count_kernel<false, true, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem + count_smem, c->stream>>>(P);
+        else if (conj) bm25_count_kernel<true, false, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem, c->stream>>>(P);
         else bm25_count_kernel<false, false, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem, c->stream>>>(P);
       } else if (term_grp) {
-        P.grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
-        P.grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[nq];
         bm25_count_kernel<false, true><<<unsigned(seg_work[si].size()), kCountThreads, count_smem, c->stream>>>(P);
       } else if (conj) bm25_count_kernel<true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
       else bm25_count_kernel<false><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
@@ -2177,6 +2218,101 @@ extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n
                                              uint64_t* counts) {
   return sdbg_match_count_batch_groups_min(segs, n_segs, terms, group_off, query_group_off, nullptr, nq, excl_terms, excl_off,
                                            filt, counts);
+}
+
+namespace {
+// The query checks of every shape of a split batch, so that a batch whose later shape is malformed queues nothing. The
+// column checks are the same for every shape: the first shape's count_run makes them before it queues anything.
+int check_shapes(sdbg_segment* const* segs, size_t n_segs, const GroupSplit<uint32_t>& S, const sdbg_col_pred* filt) {
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    if (!n) continue;
+    uint32_t total_excl = 0;
+    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
+    if (int rc = check_query_batch(segs, n_segs, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), filt,
+                                   &total_excl))
+      return rc;
+  }
+  return SDBG_OK;
+}
+}  // namespace
+
+// Sorted scan of group queries: each shape through count_run's sorted scan (shape 2 with its groups), results scattered
+// back to the caller's query positions; sdbg_scan_stats then reports the sum over the shapes.
+extern "C" int sdbg_match_topk_by_column_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                          const uint32_t* group_off, const uint32_t* query_group_off,
+                                                          const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                          const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
+                                                          int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out,
+                                                          uint32_t* n_out) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !out || !n_out) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
+  GroupSplit<uint32_t> S;
+  if (int rc = split_groups(c, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
+  if (int rc = check_shapes(segs, n_segs, S, filt)) return rc;
+  uint64_t judged = 0, skipped = 0;
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    if (!n) continue;
+    const int kind = sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR;
+    const uint8_t* grp = sh == 2 ? S.term_grp[sh].data() : nullptr;
+    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
+    std::vector<sdbg_sort_hit> h(n == nq ? 0 : n * size_t(k));
+    std::vector<uint32_t> hn(n == nq ? 0 : n);
+    SortJob J{sort_field, descending, nulls_first, k, n == nq ? out : h.data(), n == nq ? n_out : hn.data(), false, {}, {}};
+    if (int rc = count_run(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), filt,
+                           nullptr, grp, &J))
+      return rc;
+    if (n == nq) return SDBG_OK;
+    for (size_t j = 0; j < n; ++j) {
+      const size_t q = S.qs[sh][j];
+      std::copy(h.begin() + j * k, h.begin() + j * k + hn[j], out + q * k);
+      n_out[q] = hn[j];
+    }
+    uint64_t t = 0, s = 0;
+    if (int rc = sdbg_scan_stats(c, &t, &s)) return rc;
+    judged += t; skipped += s;
+  }
+  // the windows of the whole call, not of its last shape
+  c->zone_blocks_total = judged;
+  CU(c, cudaMemcpyAsync(c->d_zone_skipped, &skipped, 8, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  return SDBG_OK;
+}
+
+// Facet counts of group queries: each shape through count_run's facet pass (shape 2 with its groups), rows scattered back
+// to the caller's query positions.
+extern "C" int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                        const uint32_t* group_off, const uint32_t* query_group_off,
+                                                        const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                        const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                                        int64_t key_min, uint32_t key_span, uint64_t* counts,
+                                                        uint64_t* null_counts) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts || !null_counts) return SDBG_EINVAL;
+  GroupSplit<uint32_t> S;
+  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
+  if (int rc = check_shapes(segs, n_segs, S, filt)) return rc;
+  if (int rc = facet_check_range(segs[0]->ctx, key_min, key_span)) return rc;   // before the staging rows are sized
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    if (!n) continue;
+    const int kind = sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR;
+    const uint8_t* grp = sh == 2 ? S.term_grp[sh].data() : nullptr;
+    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
+    std::vector<uint64_t> fc(n == nq ? 0 : n * size_t(key_span)), fn(n == nq ? 0 : n);
+    FacetJob J{key_field, key_min, key_span, n == nq ? counts : fc.data(), n == nq ? null_counts : fn.data(), {}};
+    if (int rc = count_run(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), filt,
+                           nullptr, grp, nullptr, &J))
+      return rc;
+    if (n == nq) return SDBG_OK;
+    for (size_t j = 0; j < n; ++j) {
+      const size_t q = S.qs[sh][j];
+      std::copy(fc.begin() + j * key_span, fc.begin() + (j + 1) * key_span, counts + q * key_span);
+      null_counts[q] = fn[j];
+    }
+  }
+  return SDBG_OK;
 }
 
 // Streaming mode (duckdb_search_full_scan.cpp RunStreamingScan :2370-2403; DocIterator::EmitScoredDocs,

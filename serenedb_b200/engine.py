@@ -494,9 +494,7 @@ def ExecuteTopKByColumnBatch(reader, queries, kind, sort_field, k, descending=Fa
     query, the first k of the docs ExecuteCountBatch counts, ordered by column `sort_field` (int64 / int32 / float64,
     staged in every segment); ties, NULLs included, by (segment, doc). Returns a dict of per-query arrays: docs, segs,
     values (typed by the column; 0 for NULL), nulls (bool) and n_out (uint32[Q])."""
-    col_type = reader.segments[0].col_types.get(int(sort_field))
-    if col_type is None:   # the values come back as raw bits: their type must be known, not guessed
-        raise ValueError("sort column %d was not staged through this Segment" % int(sort_field))
+    vt = _sort_value_type(reader, sort_field)
     nq = len(queries)
     flat = np.ascontiguousarray([t for q in queries for t in q], dtype=np.uint32)
     off = np.zeros(nq + 1, np.uint32)
@@ -511,7 +509,18 @@ def ExecuteTopKByColumnBatch(reader, queries, kind, sort_field, k, descending=Fa
                                                     _ptr(x[1]) if x is not None else None, fp, int(sort_field),
                                                     int(bool(descending)), int(bool(nulls_first)), int(k), _ptr(hits),
                                                     _ptr(n_out)), reader.segments[0].ctx._h)
-    vt = _SORT_VALUE_DTYPE[col_type]
+    return _sort_result(hits, n_out, nq, k, vt)
+
+
+def _sort_value_type(reader, sort_field):
+    col_type = reader.segments[0].col_types.get(int(sort_field))
+    if col_type is None:   # the values come back as raw bits: their type must be known, not guessed
+        raise ValueError("sort column %d was not staged through this Segment" % int(sort_field))
+    return _SORT_VALUE_DTYPE[col_type]
+
+
+def _sort_result(hits, n_out, nq, k, vt):
+    """Sorted-scan hits [nq * k] -> the per-query dict the sorted-scan functions return."""
     out = dict(docs=[], segs=[], values=[], nulls=[], n_out=n_out[:nq])
     for q in range(nq):
         h = hits[q * k:q * k + int(n_out[q])]
@@ -537,18 +546,7 @@ def ExecuteFacetCountsBatch(reader, queries, kind, key_field, key_min=None, key_
     every segment). The key range [key_min, key_min + key_span) defaults to the segments' column_minmax (an all-NULL column
     gives one bin). Returns dict(key_min, counts uint64[Q, key_span], nulls uint64[Q]): counts[q, v - key_min] = matches
     whose key is v, nulls[q] = matches whose key is NULL."""
-    col_type = reader.segments[0].col_types.get(int(key_field))
-    if col_type is None:   # the kernel reads raw values: their type must be known, not guessed
-        raise ValueError("key column %d was not staged through this Segment" % int(key_field))
-    if col_type not in (0, 2):
-        raise ValueError("facet counts need an int64 or int32 key column")
-    if key_min is None or key_span is None:
-        mm = [s.column_minmax(key_field) for s in reader.segments]
-        lo, hi = min(m[0] for m in mm), max(m[1] for m in mm)
-        if lo > hi:   # every key NULL
-            lo = hi = 0
-        key_min = lo if key_min is None else key_min
-        key_span = hi - key_min + 1 if key_span is None else key_span
+    key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
     nq = len(queries)
     flat = np.ascontiguousarray([t for q in queries for t in q], dtype=np.uint32)
     off = np.zeros(nq + 1, np.uint32)
@@ -563,6 +561,23 @@ def ExecuteFacetCountsBatch(reader, queries, kind, key_field, key_min=None, key_
                                                   _ptr(x[1]) if x is not None else None, fp, int(key_field), int(key_min),
                                                   int(key_span), _ptr(counts), _ptr(nulls)), reader.segments[0].ctx._h)
     return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
+
+
+def _facet_key_range(reader, key_field, key_min, key_span):
+    """(key_min, key_span), each defaulting to the segments' column_minmax (an all-NULL column gives one bin)."""
+    col_type = reader.segments[0].col_types.get(int(key_field))
+    if col_type is None:   # the kernel reads raw values: their type must be known, not guessed
+        raise ValueError("key column %d was not staged through this Segment" % int(key_field))
+    if col_type not in (0, 2):
+        raise ValueError("facet counts need an int64 or int32 key column")
+    if key_min is None or key_span is None:
+        mm = [s.column_minmax(key_field) for s in reader.segments]
+        lo, hi = min(m[0] for m in mm), max(m[1] for m in mm)
+        if lo > hi:   # every key NULL
+            lo = hi = 0
+        key_min = lo if key_min is None else key_min
+        key_span = hi - key_min + 1 if key_span is None else key_span
+    return key_min, key_span
 
 
 def ExecuteFacetCounts(reader, query_terms, kind, key_field, key_min=None, key_span=None, filt=None, exclude=None):
@@ -654,6 +669,74 @@ def ExecuteCountGroups(reader, groups, filt=None, exclude=None, min_match=None):
     return int(ExecuteCountGroupsBatch(reader, [[list(g) for g in groups]], filt,
                                        exclude=None if exclude is None else [list(exclude)],
                                        min_match=None if min_match is None else [list(min_match)])[0])
+
+
+def ExecuteTopKByColumnGroupsBatch(reader, queries, sort_field, k, descending=False, nulls_first=False, filt=None,
+                                   exclude=None, min_match=None):
+    """Sorted scan of conjunctions of OR groups (`WHERE body @@ 'a & (b | c)' ORDER BY col LIMIT k`,
+    sdbg_match_topk_by_column_batch_groups_min): per query, the first k of the docs ExecuteCountGroupsBatch counts, in the
+    order of ExecuteTopKByColumnBatch. queries / exclude / min_match as in ExecuteCountGroupsBatch. Returns the dict
+    ExecuteTopKByColumnBatch returns."""
+    vt = _sort_value_type(reader, sort_field)
+    nq = len(queries)
+    ids, group_off, query_group_off = _groups(queries)
+    gmin = _group_min(min_match, queries)
+    flat = np.ascontiguousarray(ids, dtype=np.uint32)
+    hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
+    n_out = np.zeros(max(nq, 1), np.uint32)
+    x = _exclusions(exclude, nq)
+    fp = C.byref(filt) if filt is not None else None
+    N.check(N.lib().sdbg_match_topk_by_column_batch_groups_min(
+        _seg_array(reader.segments), len(reader.segments), _ptr(flat) if len(flat) else None, _ptr(group_off),
+        _ptr(query_group_off), _ptr(gmin) if gmin is not None else None, nq, _ptr(x[0]) if x is not None else None,
+        _ptr(x[1]) if x is not None else None, fp, int(sort_field), int(bool(descending)), int(bool(nulls_first)), int(k),
+        _ptr(hits), _ptr(n_out)), reader.segments[0].ctx._h)
+    return _sort_result(hits, n_out, nq, k, vt)
+
+
+def ExecuteTopKByColumnGroups(reader, groups, sort_field, k, descending=False, nulls_first=False, filt=None, exclude=None,
+                              min_match=None):
+    """ExecuteTopKByColumnGroupsBatch for one query (a list of OR groups): dict of docs, segs, values, nulls."""
+    r = ExecuteTopKByColumnGroupsBatch(reader, [[list(g) for g in groups]], sort_field, k, descending, nulls_first, filt,
+                                       exclude=None if exclude is None else [list(exclude)],
+                                       min_match=None if min_match is None else [list(min_match)])
+    return dict(docs=r["docs"][0], segs=r["segs"][0], values=r["values"][0], nulls=r["nulls"][0])
+
+
+def ExecuteFacetCountsGroupsBatch(reader, queries, key_field, key_min=None, key_span=None, filt=None, exclude=None,
+                                  min_match=None):
+    """Facet counts of conjunctions of OR groups (`WHERE body @@ 'a & (b | c)' GROUP BY col`,
+    sdbg_match_facet_counts_batch_groups_min): per query, how the docs ExecuteCountGroupsBatch counts split over the values
+    of column `key_field`. queries / exclude / min_match as in ExecuteCountGroupsBatch; the key range as in
+    ExecuteFacetCountsBatch. Returns the dict ExecuteFacetCountsBatch returns."""
+    key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
+    nq = len(queries)
+    ids, group_off, query_group_off = _groups(queries)
+    gmin = _group_min(min_match, queries)
+    flat = np.ascontiguousarray(ids, dtype=np.uint32)
+    counts = np.zeros((max(nq, 1), max(int(key_span), 1)), np.uint64)
+    nulls = np.zeros(max(nq, 1), np.uint64)
+    x = _exclusions(exclude, nq)
+    fp = C.byref(filt) if filt is not None else None
+    N.check(N.lib().sdbg_match_facet_counts_batch_groups_min(
+        _seg_array(reader.segments), len(reader.segments), _ptr(flat) if len(flat) else None, _ptr(group_off),
+        _ptr(query_group_off), _ptr(gmin) if gmin is not None else None, nq, _ptr(x[0]) if x is not None else None,
+        _ptr(x[1]) if x is not None else None, fp, int(key_field), int(key_min), int(key_span), _ptr(counts), _ptr(nulls)),
+        reader.segments[0].ctx._h)
+    return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
+
+
+def ExecuteFacetCountsGroups(reader, groups, key_field, key_min=None, key_span=None, filt=None, exclude=None,
+                             min_match=None):
+    """ExecuteFacetCountsGroupsBatch for one query: {key: count} plus {None: n} for NULL keys, as ExecuteFacetCounts."""
+    r = ExecuteFacetCountsGroupsBatch(reader, [[list(g) for g in groups]], key_field, key_min, key_span, filt,
+                                      exclude=None if exclude is None else [list(exclude)],
+                                      min_match=None if min_match is None else [list(min_match)])
+    row = r["counts"][0]
+    out = {r["key_min"] + int(i): int(row[i]) for i in np.nonzero(row)[0]}
+    if r["nulls"][0]:
+        out[None] = int(r["nulls"][0])
+    return out
 
 
 FOR_BLOCK_DTYPE =np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])

@@ -5,7 +5,8 @@
 // scan mode (GpuCountScan, tests/test_gpu_count.py); with "groups", only an And of Or groups through both adapters
 // (tests/test_gpu_groups.py); with "minmatch", only an Or with min_match_count through both adapters
 // (tests/test_gpu_min_match.py); with "sorted", only the sorted scan (GpuSortedScan, tests/test_gpu_sort_by_column.py); with
-// "facet", only the facet counts (GpuFacetScan, tests/test_gpu_facets.py).
+// "facet", only the facet counts (GpuFacetScan, tests/test_gpu_facets.py). "sorted groups" / "facet groups" run those two
+// with group queries (tests/test_gpu_groups_column.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -139,15 +140,23 @@ int main(int argc, char** argv) {
     sdbg_destroy(ctx);
     return 0;
   }
+  // With a third argument "groups", the sorted and facet modes run group queries instead of `t2 | t5` (and `t2 & t5`):
+  // query 0 is `t2 & (t5 | t6)`, query 1 `2 of (t2 | t5 | t6)`.
+  const bool grouped = argc > 3 && std::string(argv[3]) == "groups";
+  const std::vector<uint32_t> flat_ids{2, 5}, group_ids{2, 5, 6};
+  auto group_sizes = [&](int q) { return !grouped ? std::vector<uint32_t>{} : q ? std::vector<uint32_t>{3} : std::vector<uint32_t>{1, 2}; };
+  auto group_mins = [&](int q) { return grouped && q ? std::vector<uint32_t>{2} : std::vector<uint32_t>{}; };
   if (argc > 2 && std::string(argv[2]) == "sorted") {
     // `t2 | t5` and `(t2 | t5) & !t3` ORDER BY the int32 column 9, LIMIT 4096 (two chunks), every direction and NULL
     // placement, without and with the table filter: every row in order, then end of scan
+    for (int query = 0; query < (grouped ? 2 : 1); ++query)
     for (int with_filter = 0; with_filter < 2; ++with_filter)
       for (int excl = 0; excl < 2; ++excl)
         for (int desc = 0; desc < 2; ++desc)
           for (int nf = 0; nf < 2; ++nf) {
-            sdbg_host::GpuSortedScan scan({seg}, SDBG_QUERY_OR, {2, 5}, excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{},
-                                          with_filter ? &filt : nullptr, 9, desc != 0, nf != 0, 4096);
+            sdbg_host::GpuSortedScan scan({seg}, SDBG_QUERY_OR, grouped ? group_ids : flat_ids,
+                                          excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{}, with_filter ? &filt : nullptr, 9,
+                                          desc != 0, nf != 0, 4096, group_sizes(query), group_mins(query));
             duckdb::DataChunkMock chunk;
             std::vector<uint32_t> docs, segs;
             std::vector<int64_t> vals;
@@ -164,8 +173,9 @@ int main(int argc, char** argv) {
               valid.insert(valid.end(), chunk.valid.begin(), chunk.valid.end());
             }
             scan.Scan(chunk);
-            std::printf("{\"filter\": %d, \"excl\": %d, \"desc\": %d, \"nulls_first\": %d, \"chunks\": %llu, \"max_chunk\": %llu, "
-                        "\"rows_after\": %llu, \"docs\": [", with_filter, excl, desc, nf, static_cast<unsigned long long>(chunks),
+            if (grouped) std::printf("{\"query\": %d, ", query);
+            std::printf("%s\"filter\": %d, \"excl\": %d, \"desc\": %d, \"nulls_first\": %d, \"chunks\": %llu, \"max_chunk\": %llu, "
+                        "\"rows_after\": %llu, \"docs\": [", grouped ? "" : "{", with_filter, excl, desc, nf, static_cast<unsigned long long>(chunks),
                         static_cast<unsigned long long>(max_chunk), static_cast<unsigned long long>(chunk.size));
             for (size_t i = 0; i < docs.size(); ++i) std::printf("%s%u", i ? ", " : "", docs[i]);
             std::printf("], \"segs\": [");
@@ -183,12 +193,14 @@ int main(int argc, char** argv) {
   if (argc > 2 && std::string(argv[2]) == "facet") {
     // `t2 | t5`, `t2 & t5` and `(t2 | t5) & !t3` GROUP BY the 2001-key int64 column 15 (count(*)), without and with the
     // table filter: every group in key order, then end of scan. Then the int32 column 9, whose range is too wide.
+    // (grouped: "kind" 0 / 1 is query 0 / 1)
     sdbg_synth_column(seg, 15, 15, 3, 1, n_docs);
     for (int with_filter = 0; with_filter < 2; ++with_filter)
       for (int kind : {int(SDBG_QUERY_OR), int(SDBG_QUERY_AND)})
         for (int excl = 0; excl < 2; ++excl) {
-          sdbg_host::GpuFacetScan scan({seg}, kind, {2, 5}, excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{},
-                                       with_filter ? &filt : nullptr, 15);
+          sdbg_host::GpuFacetScan scan({seg}, kind, grouped ? group_ids : flat_ids,
+                                       excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{}, with_filter ? &filt : nullptr, 15,
+                                       group_sizes(kind), group_mins(kind));
           duckdb::DataChunkMock chunk;
           std::vector<int64_t> keys, counts;
           std::vector<uint8_t> valid;

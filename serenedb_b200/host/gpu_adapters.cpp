@@ -234,9 +234,11 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
 
 GpuSortedScan::GpuSortedScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                              std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t sort_field,
-                             bool descending, bool nulls_first, uint32_t k)
+                             bool descending, bool nulls_first, uint32_t k, std::vector<uint32_t> group_sizes,
+                             std::vector<uint32_t> group_min_match)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      has_filter_(table_filter != nullptr), field_(sort_field), desc_(descending), nulls_first_(nulls_first), k_(k) {
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), has_filter_(table_filter != nullptr),
+      field_(sort_field), desc_(descending), nulls_first_(nulls_first), k_(k) {
   if (table_filter) filter_ = *table_filter;
 }
 
@@ -247,11 +249,23 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
     const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
     hits_.resize(k_);
     uint32_t n = 0;
-    const int rc = sdbg_match_topk_by_column_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(),
-                                                   excl_off, has_filter_ ? &filter_ : nullptr, field_, desc_ ? 1 : 0,
-                                                   nulls_first_ ? 1 : 0, k_, hits_.data(), &n);
-    if (rc != SDBG_OK)
-      throw GpuError(rc, std::string("sdbg_match_topk_by_column_batch: ") + sdbg_last_error(sdbg_segment_context(segs_[0])));
+    int rc;
+    const char* what;
+    if (group_sizes_.empty()) {
+      rc = sdbg_match_topk_by_column_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
+                                           has_filter_ ? &filter_ : nullptr, field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
+                                           hits_.data(), &n);
+      what = "sdbg_match_topk_by_column_batch: ";
+    } else {                                                  // an And of Ors: kind_ is not used
+      const std::vector<uint32_t> group_off = group_offsets(group_sizes_, terms_.size());
+      const uint32_t query_group_off[2] = {0, uint32_t(group_sizes_.size())};
+      rc = sdbg_match_topk_by_column_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
+                                                      group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(),
+                                                      excl_off, has_filter_ ? &filter_ : nullptr, field_, desc_ ? 1 : 0,
+                                                      nulls_first_ ? 1 : 0, k_, hits_.data(), &n);
+      what = "sdbg_match_topk_by_column_batch_groups_min: ";
+    }
+    if (rc != SDBG_OK) throw GpuError(rc, std::string(what) + sdbg_last_error(sdbg_segment_context(segs_[0])));
     hits_.resize(n);
     ran_ = true;
   }
@@ -268,9 +282,11 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
 }
 
 GpuFacetScan::GpuFacetScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
-                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field)
+                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
+                           std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      has_filter_(table_filter != nullptr), field_(key_field) {
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), has_filter_(table_filter != nullptr),
+      field_(key_field) {
   if (table_filter) filter_ = *table_filter;
 }
 
@@ -292,10 +308,22 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
     const uint32_t term_off[2] = {0, uint32_t(terms_.size())};
     const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
     std::vector<uint64_t> counts(span);
-    const int rc = sdbg_match_facet_counts_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(),
-                                                 excl_off, has_filter_ ? &filter_ : nullptr, field_, lo, uint32_t(span),
-                                                 counts.data(), &nulls_);
-    if (rc != SDBG_OK) throw GpuError(rc, std::string("sdbg_match_facet_counts_batch: ") + sdbg_last_error(ctx));
+    int rc;
+    const char* what;
+    if (group_sizes_.empty()) {
+      rc = sdbg_match_facet_counts_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
+                                         has_filter_ ? &filter_ : nullptr, field_, lo, uint32_t(span), counts.data(), &nulls_);
+      what = "sdbg_match_facet_counts_batch: ";
+    } else {                                                  // an And of Ors: kind_ is not used
+      const std::vector<uint32_t> group_off = group_offsets(group_sizes_, terms_.size());
+      const uint32_t query_group_off[2] = {0, uint32_t(group_sizes_.size())};
+      rc = sdbg_match_facet_counts_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
+                                                    group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(),
+                                                    excl_off, has_filter_ ? &filter_ : nullptr, field_, lo, uint32_t(span),
+                                                    counts.data(), &nulls_);
+      what = "sdbg_match_facet_counts_batch_groups_min: ";
+    }
+    if (rc != SDBG_OK) throw GpuError(rc, std::string(what) + sdbg_last_error(ctx));
     for (uint64_t i = 0; i < span; ++i)
       if (counts[i]) groups_.emplace_back(int64_t(uint64_t(lo) + i), counts[i]);
     ran_ = true;

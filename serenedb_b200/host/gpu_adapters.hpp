@@ -132,20 +132,22 @@ class GpuCountScan {
 // SELECT ... FROM t WHERE body @@ '<query>' [AND <pushed filter>] ORDER BY col [DESC] [NULLS FIRST|LAST] LIMIT k -- the body
 // of the TOP_N(col) <- IRESEARCH_SCAN(Stream) plan shape (duckdb_search_full_scan.cpp IResearchSetScanOrder :1711-1762 pushes
 // only score orders; RunStreamingScan :2370-2403 serves the rest under TOP_N). One sdbg_match_topk_by_column_batch call
-// on the first Scan; then rows (doc, segment, value, valid) in TOP_N's order, <= STANDARD_VECTOR_SIZE per call,
+// (sdbg_match_topk_by_column_batch_groups_min with group_sizes) on the first Scan; then rows (doc, segment, value, valid) in TOP_N's order, <= STANDARD_VECTOR_SIZE per call,
 // cardinality 0 at the end.
 class GpuSortedScan {
  public:
   GpuSortedScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
                 std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
                 uint64_t sort_field, bool descending, bool nulls_first /* the plan's resolved OrderByNullType */,
-                uint32_t k /* LIMIT (+ OFFSET), 1..4096 */);
+                uint32_t k /* LIMIT (+ OFFSET), 1..4096 */,
+                std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
+                std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
   bool has_filter_;
   sdbg_col_pred filter_{};
   uint64_t field_;
@@ -158,20 +160,23 @@ class GpuSortedScan {
 
 // SELECT col, count(*) FROM t WHERE body @@ '<query>' [AND <pushed filter>] GROUP BY col -- the body of the
 // HASH_GROUP_BY(col; count_star()) <- IRESEARCH_SCAN(text query) plan shape (facet counts). The first Scan takes the key
-// range from sdbg_column_minmax_i64 over the segments and runs one sdbg_match_facet_counts_batch call; then the non-empty
+// range from sdbg_column_minmax_i64 over the segments and runs one sdbg_match_facet_counts_batch call
+// (sdbg_match_facet_counts_batch_groups_min with group_sizes); then the non-empty
 // groups as rows (key, count, valid) in ascending key order, the NULL group (valid = 0) last, <= STANDARD_VECTOR_SIZE per
 // call, cardinality 0 at the end. A key range wider than 32768 throws GpuError(SDBG_EUNSUPPORTED): the plan stays on the CPU.
 class GpuFacetScan {
  public:
   GpuFacetScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
-               uint64_t key_field /* int64 or int32 */);
+               uint64_t key_field /* int64 or int32 */,
+               std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
   bool has_filter_;
   sdbg_col_pred filter_{};
   uint64_t field_;

@@ -33,6 +33,21 @@ def gpu_info():
     return out.stdout.strip().splitlines()[0] if out.returncode == 0 and out.stdout.strip() else "unknown"
 
 
+def make_group_queries(n):
+    """bench.make_queries' pairs (a, b) with a third term c: `a & (b | c)`, the flat `a | b | c` and `a & b`."""
+    rng = np.random.default_rng(20261015)
+    grouped, flat_or, flat_and = [], [], []
+    for q in bench.make_queries(n):
+        a, b = int(q[0]), int(q[1])
+        c = int(rng.integers(0, bench.N_TERMS))
+        while c in (a, b):
+            c = int(rng.integers(0, bench.N_TERMS))
+        grouped.append([[a], [b, c]])
+        flat_or.append([a, b, c])
+        flat_and.append([a, b])
+    return grouped, flat_or, flat_and
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
@@ -45,17 +60,7 @@ def main():
     seg = sdb.Segment(ctx, args.docs)
     dc, sum_dl = seg.synth_corpus(0, 0, bench.N_TERMS, threads=min(os.cpu_count() or 1, 64))
     reader = sdb.IndexReader([seg], args.docs, sum_dl, dc)
-    pairs = bench.make_queries(args.queries)
-    rng = np.random.default_rng(20261015)
-    grouped, flat_or, flat_and = [], [], []
-    for q in pairs:
-        a, b = int(q[0]), int(q[1])
-        c = int(rng.integers(0, bench.N_TERMS))
-        while c in (a, b):
-            c = int(rng.integers(0, bench.N_TERMS))
-        grouped.append([[a], [b, c]])
-        flat_or.append([a, b, c])
-        flat_and.append([a, b])
+    grouped, flat_or, flat_and = make_group_queries(args.queries)
     scorer = sdb.BM25(1.2, 0.75)
     k = bench.TOPK
 

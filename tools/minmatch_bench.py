@@ -34,6 +34,23 @@ def gpu_info():
     return out.stdout.strip().splitlines()[0] if out.returncode == 0 and out.stdout.strip() else "unknown"
 
 
+def make_min_queries(n):
+    """bench.make_queries' pairs extended to six distinct terms: the `2 of (a | b | c)` groups, the `3 of 6` groups and
+    the flat `a | b | c`."""
+    rng = np.random.default_rng(20261016)
+    three, six, flat_or = [], [], []
+    for q in bench.make_queries(n):
+        ids = [int(q[0]), int(q[1])]
+        while len(ids) < 6:
+            t = int(rng.integers(0, bench.N_TERMS))
+            if t not in ids:
+                ids.append(t)
+        three.append([ids[:3]])
+        six.append([ids])
+        flat_or.append(ids[:3])
+    return three, six, flat_or
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
@@ -47,18 +64,7 @@ def main():
     seg = sdb.Segment(ctx, args.docs)
     dc, sum_dl = seg.synth_corpus(0, 0, bench.N_TERMS, threads=min(os.cpu_count() or 1, 64))
     reader = sdb.IndexReader([seg], args.docs, sum_dl, dc)
-    pairs = bench.make_queries(args.queries)
-    rng = np.random.default_rng(20261016)
-    three, six, flat_or = [], [], []
-    for q in pairs:
-        ids = [int(q[0]), int(q[1])]
-        while len(ids) < 6:
-            t = int(rng.integers(0, bench.N_TERMS))
-            if t not in ids:
-                ids.append(t)
-        three.append([ids[:3]])
-        six.append([ids])
-        flat_or.append(ids[:3])
+    three, six, flat_or = make_min_queries(args.queries)
     scorer = sdb.BM25(1.2, 0.75)
     k = bench.TOPK
 
