@@ -136,7 +136,17 @@ int sdbg_segment_posting_stats(const sdbg_segment*, uint64_t* payload_bytes, uin
 /* Encoded bytes (block headers + payloads, as in the .doc stream) of the first n_terms terms. */
 int sdbg_segment_term_bytes(const sdbg_segment*, uint64_t* bytes_out, size_t n_terms);
 
-/* ---- predicates (pushed TableFilterSet entries; NULL never passes) ---- */
+/* ---- predicates (pushed TableFilterSet entries; NULL never passes) ----
+ * `column op lo` (BETWEEN: lo <= column AND column <= hi, so lo > hi selects nothing). is_float selects which pair holds
+ * the constants: lo_f / hi_f when is_float != 0, lo_i / hi_i otherwise; the other pair is ignored. Every entry point
+ * resolves the constants against the filtered column's type (sdbg_col_pred_resolve) before any kernel sees them:
+ *   - double column: IEEE comparison with the constant as a double (an integer constant is rounded to the nearest
+ *     double, as a SQL cast of the constant to the column type does). NaN compares false, so `<> NaN` holds for every
+ *     non-NULL row; -0.0 equals +0.0.
+ *   - integer column (int64 raw or bit-packed, int32): the exact comparison of the integer with the constant. A double
+ *     constant becomes the tightest integer bounds (v < 2.5 is v <= 2, v >= 2.5 is v >= 3); bounds beyond int64 hold
+ *     for every row or none (v < 1e300, v > -inf: every row; v = 1e30: none); NaN holds for none, except `<> NaN`,
+ *     which holds for every non-NULL row; `= 2.5` holds for none and `<> 2.5` for every non-NULL row. */
 enum { SDBG_OP_LT = 0, SDBG_OP_LE, SDBG_OP_GT, SDBG_OP_GE, SDBG_OP_EQ, SDBG_OP_NE, SDBG_OP_BETWEEN,
        SDBG_OP_IS_NULL, SDBG_OP_IS_NOT_NULL };
 typedef struct {
@@ -146,6 +156,11 @@ typedef struct {
   int64_t lo_i, hi_i;
   double lo_f, hi_f;
 } sdbg_col_pred;
+/* The predicate the kernels evaluate for `in` on a column of type `type` (sdbg_type), under the rules above: on a double
+ * column is_float = 1 with lo_f / hi_f; on an integer column is_float = 0 with lo_i / hi_i, a double constant turned into
+ * BETWEEN [lo_i, hi_i] (lo_i > hi_i: no row) or, for `<>` an integral constant inside int64, `<>` that integer. Host-only
+ * (no device needed). Errors: NULL pointers, an op outside SDBG_OP_*, an unknown type: SDBG_EINVAL. */
+int sdbg_col_pred_resolve(const sdbg_col_pred* in, int type, sdbg_col_pred* out);
 
 /* ---- BM25 top-k (boundary B2, irs::DocIterator::Collect) ---- */
 enum { SDBG_QUERY_OR = 0, SDBG_QUERY_AND = 1 };

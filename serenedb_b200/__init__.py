@@ -10,7 +10,7 @@ from .engine import (AND, OR, BM25, TFIDF, FLT_MIN, Context, ExecuteCount, Execu
                      ExecuteCountGroupsBatch, ExecuteFacetCounts, ExecuteFacetCountsBatch, ExecuteFacetCountsGroups,
                      ExecuteFacetCountsGroupsBatch, ExecuteTopK, ExecuteTopKBatch, ExecuteTopKByColumn, ExecuteTopKByColumnBatch,
                      ExecuteTopKByColumnGroups, ExecuteTopKByColumnGroupsBatch, ExecuteTopKGroups, ExecuteTopKGroupsBatch, IndexReader, IResearchScan, PostingsWriter, PreparedBatch, Segment, merge_gathered, pred,
-                     stage_parse_host, sum_i128, StreamScoredDocs, pack_for)
+                     resolve_pred, stage_parse_host, sum_i128, StreamScoredDocs, pack_for)
 
 _native.lib()  # fail loudly at import time when the CUDA extension is missing
 
@@ -18,4 +18,4 @@ __all__ = ["AND", "OR", "BM25", "TFIDF", "FLT_MIN", "Context", "ExecuteCount", "
            "ExecuteCountGroupsBatch", "ExecuteFacetCounts", "ExecuteFacetCountsBatch", "ExecuteFacetCountsGroups",
            "ExecuteFacetCountsGroupsBatch", "ExecuteTopK", "ExecuteTopKBatch", "ExecuteTopKByColumn", "ExecuteTopKByColumnBatch",
            "ExecuteTopKByColumnGroups", "ExecuteTopKByColumnGroupsBatch", "ExecuteTopKGroups", "ExecuteTopKGroupsBatch", "IndexReader", "IResearchScan", "PostingsWriter", "PreparedBatch", "Segment", "merge_gathered",
-           "pred", "stage_parse_host", "sum_i128", "StreamScoredDocs", "pack_for"]
+           "pred", "resolve_pred", "stage_parse_host", "sum_i128", "StreamScoredDocs", "pack_for"]

@@ -115,6 +115,7 @@ SIGNATURES = {
                                                            C.c_int64, C.c_uint32, _vp, _vp]),
     "sdbg_topk_merge_gathered": (C.c_int, [_vp, _vp, C.c_uint32, _sz, C.c_uint32, _vp, _vp]),
     "sdbg_decode_score_term": (C.c_int, [_vp, C.c_uint32, C.c_float, C.c_float, C.c_float, _vp, _vp, _vp]),
+    "sdbg_col_pred_resolve": (C.c_int, [C.POINTER(ColPred), C.c_int, C.POINTER(ColPred)]),
     "sdbg_filter_bitmap": (C.c_int, [_vp, _vp, _sz, _vp]),
     "sdbg_filter_count_sum": (C.c_int, [_vp, _sz, _vp, _sz, C.c_uint64, _u64p, _vp, C.POINTER(C.c_double)]),
     "sdbg_filter_groupby": (C.c_int, [_vp, _sz, _vp, _sz, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, _vp,

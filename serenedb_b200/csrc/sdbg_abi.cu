@@ -846,6 +846,67 @@ extern "C" int sdbg_segment_term_bytes(const sdbg_segment* s, uint64_t* bytes_ou
 }
 
 // ------------------------------------------------------------------------------------------
+// Pushed predicates: the constant resolved against the column's type before any kernel sees it
+// ------------------------------------------------------------------------------------------
+namespace {
+
+constexpr double kTwo63 = 9223372036854775808.0;   // 2^63, the first double above INT64_MAX
+
+// Smallest int64 v with v >= x (strict: v > x); false when no int64 qualifies (x NaN or beyond INT64_MAX).
+bool int_lower_bound(double x, bool strict, int64_t* v) {
+  if (std::isnan(x)) return false;
+  const double c = strict ? std::floor(x) : std::ceil(x);
+  if (c >= kTwo63) return false;
+  if (c < -kTwo63) { *v = INT64_MIN; return true; }
+  *v = static_cast<int64_t>(c) + (strict ? 1 : 0);   // c <= 2^63 - 1024 here (doubles below 2^63 step by 1024): no overflow
+  return true;
+}
+// Largest int64 v with v <= x (strict: v < x); false when no int64 qualifies (x NaN or below INT64_MIN).
+bool int_upper_bound(double x, bool strict, int64_t* v) {
+  if (std::isnan(x)) return false;
+  const double c = strict ? std::ceil(x) : std::floor(x);
+  if (strict ? c <= -kTwo63 : c < -kTwo63) return false;
+  if (c >= kTwo63) { *v = INT64_MAX; return true; }
+  *v = static_cast<int64_t>(c) - (strict ? 1 : 0);
+  return true;
+}
+
+}  // namespace
+
+extern "C" int sdbg_col_pred_resolve(const sdbg_col_pred* in, int type, sdbg_col_pred* out) {
+  if (!in || !out || in->op < SDBG_OP_LT || in->op > SDBG_OP_IS_NOT_NULL || type < SDBG_I64 || type > SDBG_I32) return SDBG_EINVAL;
+  sdbg_col_pred p = *in;
+  const bool compares = p.op < SDBG_OP_IS_NULL;
+  if (compares && type == SDBG_F64 && !p.is_float) {
+    p.lo_f = static_cast<double>(p.lo_i); p.hi_f = static_cast<double>(p.hi_i); p.is_float = 1;   // rounded to nearest
+  } else if (compares && type != SDBG_F64 && p.is_float) {
+    int64_t lo = INT64_MIN, hi = INT64_MAX;
+    bool some = true;
+    const double x = p.lo_f;
+    switch (p.op) {
+      case SDBG_OP_LT: some = int_upper_bound(x, true, &hi); break;
+      case SDBG_OP_LE: some = int_upper_bound(x, false, &hi); break;
+      case SDBG_OP_GT: some = int_lower_bound(x, true, &lo); break;
+      case SDBG_OP_GE: some = int_lower_bound(x, false, &lo); break;
+      case SDBG_OP_EQ: some = int_lower_bound(x, false, &lo) && int_upper_bound(x, false, &hi); break;
+      case SDBG_OP_NE:
+        if (int_lower_bound(x, false, &lo) && int_upper_bound(x, false, &hi) && lo == hi) {   // an int64 value: stays <>
+          p.lo_i = lo; p.is_float = 0;
+          *out = p;
+          return SDBG_OK;
+        }
+        lo = INT64_MIN; hi = INT64_MAX;   // NaN, fractional or outside int64: every non-NULL row
+        break;
+      default: some = int_lower_bound(x, false, &lo) && int_upper_bound(p.hi_f, false, &hi); break;
+    }
+    if (!some) { lo = INT64_MAX; hi = INT64_MIN; }
+    p.op = SDBG_OP_BETWEEN; p.is_float = 0; p.lo_i = lo; p.hi_i = hi;
+  }
+  *out = p;
+  return SDBG_OK;
+}
+
+// ------------------------------------------------------------------------------------------
 // BM25 top-k
 // ------------------------------------------------------------------------------------------
 namespace {
@@ -870,11 +931,13 @@ int filter_view(sdbg_segment* s, const sdbg_col_pred* f, FilterDev* out) {
   auto it = s->cols.find(f->field);
   if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "filter column not staged");
   if (it->second.rows < s->n_docs) return fail(s->ctx, SDBG_EINVAL, "filter column shorter than segment");
+  sdbg_col_pred p;
+  if (sdbg_col_pred_resolve(f, it->second.type, &p)) return fail(s->ctx, SDBG_EINVAL, "bad predicate op");
   void* raw = nullptr;
   const int rc = raw_values(s->ctx, it->second, &raw);
   if (rc) return rc;
   out->values = raw; out->validity = it->second.d_validity; out->type = it->second.type;
-  out->op = f->op; out->lo_i = f->lo_i; out->hi_i = f->hi_i; out->lo_f = f->lo_f; out->hi_f = f->hi_f;
+  out->op = p.op; out->lo_i = p.lo_i; out->hi_i = p.hi_i; out->lo_f = p.lo_f; out->hi_f = p.hi_f;
   return SDBG_OK;
 }
 
@@ -2612,10 +2675,12 @@ int pred_set(sdbg_segment* s, const sdbg_col_pred* preds, size_t n, PredSet* ps,
     if (rc) return rc;
     if (*rows == 0) *rows = r;
     if (r != *rows) return fail(s->ctx, SDBG_EINVAL, "columns of one segment differ in length");
-    if (preds[i].op < 0 || preds[i].op > 8) return fail(s->ctx, SDBG_EINVAL, "bad predicate op");
-    ps->p[i].op = preds[i].op;
-    ps->p[i].lo_i = preds[i].lo_i; ps->p[i].hi_i = preds[i].hi_i;
-    ps->p[i].lo_f = preds[i].lo_f; ps->p[i].hi_f = preds[i].hi_f;
+    sdbg_col_pred p;
+    const int type = ps->p[i].col.type == kTypeFor ? SDBG_I64 : ps->p[i].col.type;   // a packed column holds int64
+    if (sdbg_col_pred_resolve(&preds[i], type, &p)) return fail(s->ctx, SDBG_EINVAL, "bad predicate op");
+    ps->p[i].op = p.op;
+    ps->p[i].lo_i = p.lo_i; ps->p[i].hi_i = p.hi_i;
+    ps->p[i].lo_f = p.lo_f; ps->p[i].hi_f = p.hi_f;
   }
   return SDBG_OK;
 }

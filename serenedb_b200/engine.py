@@ -7,6 +7,7 @@ Names follow the reference: `BM25` (irs/search/bm25.hpp:58), `ExecuteTopK`
 in libsdbg.so on the GPU; this module only marshals arguments.
 """
 import ctypes as C
+import operator
 
 import numpy as np
 
@@ -28,40 +29,68 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+_INT64_MIN, _INT64_MAX = -(1 << 63), (1 << 63) - 1
+
+
+def _as_double(v):
+    """An integer as the nearest double (+-inf beyond the double range)."""
+    try:
+        return float(v)
+    except OverflowError:
+        return float("inf") if v > 0 else float("-inf")
+
+
 def pred(field, op, lo=0, hi=0):
-    """One pushed column predicate (duckdb TableFilter). Float bounds select a double comparison on a double column;
-    on an integer column the kernels compare integers, so the integer bounds are the tightest integers with the same
-    truth set (v < 2.5 <=> v < 3, v >= 2.5 <=> v >= 3, v <= 2.5 <=> v <= 2, v > 2.5 <=> v > 2)."""
-    import math
+    """One pushed column predicate (duckdb TableFilter), `column op lo` (BETWEEN: lo <= column <= hi), with SQL's meaning
+    whatever the constants' types; NULL never passes. A float constant (Python float or any NumPy floating scalar) goes to
+    libsdbg as a double, an integer constant (int, NumPy integer) inside int64 as an integer, and the library resolves
+    both against the column's type (sdbg.h, sdbg_col_pred_resolve):
+    - double column: IEEE comparison with the constant as a double (an integer is rounded to the nearest double). NaN
+      compares false, so `<> NaN` holds for every non-NULL row; -0.0 == +0.0.
+    - integer column: the exact comparison of the integer with the constant. v < 2.5 is v <= 2, v >= 2.5 is v >= 3;
+      v < 1e300 and v > -inf hold for every row; NaN holds for no row, except `<> NaN`, which holds for every non-NULL
+      row. `= 2.5` is resolved as no row and `<> 2.5` as every non-NULL row.
+    An integer constant outside int64 goes as the nearest double (+-inf beyond the double range): on an integer column
+    that keeps the exact answer (every row or none), on a double column it is the rounding above. The exception is an
+    integer within 1024 below INT64_MIN, whose nearest double is -2^63 = INT64_MIN itself (ValueError: pass it as a
+    float). BETWEEN with one float and one integer bound sends both as doubles, so such an integer bound must be a double
+    exactly (ValueError)."""
     p = N.ColPred()
     p.field = int(field)
     p.op = OPS[op] if isinstance(op, str) else int(op)
-    is_float = isinstance(lo, float) or isinstance(hi, float)
-    p.is_float = 1 if is_float else 0
-    p.lo_f, p.hi_f = float(lo), float(hi)
-    if not is_float:
-        p.lo_i, p.hi_i = int(lo), int(hi)
+    bounds = (lo, hi) if p.op == OPS["BETWEEN"] else (lo, 0)
+    ints = [None if isinstance(x, (float, np.floating)) else operator.index(x) for x in bounds]
+    if all(v is not None and _INT64_MIN <= v <= _INT64_MAX for v in ints):
+        p.is_float = 0
+        p.lo_i, p.hi_i = ints
         return p
-    name = {v: k for k, v in OPS.items()}.get(p.op, "")
-    big = (1 << 62)
-    clamp = lambda x: int(max(-big, min(big, x)))
-    lo_f, hi_f = float(lo), float(hi)
-    if math.isnan(lo_f) or math.isinf(lo_f) or math.isnan(hi_f) or math.isinf(hi_f):
-        p.lo_i, p.hi_i = clamp(-big if lo_f < 0 else big) if not math.isnan(lo_f) else 0, 0
-        return p
-    if name in ("LT", "GE"):
-        p.lo_i = clamp(math.ceil(lo_f))
-    elif name in ("LE", "GT"):
-        p.lo_i = clamp(math.floor(lo_f))
-    elif name == "BETWEEN":
-        p.lo_i, p.hi_i = clamp(math.ceil(lo_f)), clamp(math.floor(hi_f))
-    elif name in ("EQ", "NE"):
-        # = / <> with a fractional constant on an integer column is a constant predicate the planner folds away
-        # (DuckDB does); it is not representable here, so reject it instead of comparing with a rounded value
-        if lo_f != math.floor(lo_f):
-            raise ValueError("fold '= / <> fractional constant' on an integer column before pushing it down")
-        p.lo_i = clamp(lo_f)
+    doubles = []
+    for x, v in zip(bounds, ints):
+        if v is None:
+            doubles.append(float(x))
+        elif _INT64_MIN <= v <= _INT64_MAX:
+            if int(float(v)) != v:
+                raise ValueError("integer bound %d next to a float bound is not a double: pass both bounds as integers or "
+                                 "as floats" % v)
+            doubles.append(float(v))
+        else:
+            d = _as_double(v)
+            if v < _INT64_MIN and d == float(_INT64_MIN):
+                raise ValueError("integer constant %d below INT64_MIN rounds to the double -2^63, which is INT64_MIN: "
+                                 "no double stands for it on both column types" % v)
+            doubles.append(d)
+    p.is_float = 1
+    p.lo_f, p.hi_f = doubles
     return p
+
+
+def resolve_pred(p, dtype):
+    """The predicate the kernels evaluate for pred() `p` on a column of `dtype` (int64 / float64 / int32):
+    sdbg_col_pred_resolve, a host-only call. On an integer column lo_i / hi_i hold the integer form, on a double column
+    lo_f / hi_f the double form."""
+    out = N.ColPred()
+    N.check(N.lib().sdbg_col_pred_resolve(C.byref(p), TYPES[np.dtype(dtype)], C.byref(out)))
+    return out
 
 
 def _pred_array(preds):
