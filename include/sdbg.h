@@ -290,9 +290,10 @@ int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int 
  * exact with pruning off and a lower bound with it; counts are exact at every pruning level and equal the level-0 totals.
  * Degenerate queries take the existing paths and give exactly their results: a query of one group runs as
  * sdbg_bm25_topk_batch_excl / sdbg_match_count_batch with kind OR, a query whose groups are all single terms as kind AND.
- * Errors: an empty group, a decreasing offset array, a positive term id twice in a query, or NULL arrays with non-empty
- * ranges: SDBG_EINVAL; more than 16 groups, positive terms or excluded terms in a query: SDBG_EUNSUPPORTED; otherwise the
- * errors of sdbg_bm25_topk_batch_excl / sdbg_match_count_batch.
+ * Errors, all found before anything is queued (whatever the shapes of a batch's queries): an empty group, a decreasing
+ * offset array, a positive term id twice in a query, or NULL arrays with non-empty ranges: SDBG_EINVAL; more than 16
+ * groups, positive terms or excluded terms in a query: SDBG_EUNSUPPORTED; otherwise the errors of
+ * sdbg_bm25_topk_batch_excl / sdbg_match_count_batch.
  * The sorted scan and facet counts of group queries: sdbg_match_topk_by_column_batch_groups_min /
  * sdbg_match_facet_counts_batch_groups_min below.
  * Not supported yet: the streaming scan (sdbg_bm25_scan*), grouped forms of sdbg_bm25_topk_batch_device and

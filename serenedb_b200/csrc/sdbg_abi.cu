@@ -1051,12 +1051,29 @@ struct TopkDevOut { unsigned long long* keys; uint32_t* n_out; unsigned long lon
 uint32_t term_id(const sdbg_bm25_term& t) { return t.term; }
 uint32_t term_id(uint32_t t) { return t; }
 
+// A batch of queries as the flat entries take it (the caller's arrays, not copied). Query q has the positive terms
+// terms[term_off[q] .. term_off[q + 1]) and excludes the term ids excl_terms[excl_off[q] .. excl_off[q + 1]) (NULL
+// excl_off: none). term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group
+// term_grp[i] & 15 of its query, which needs (term_grp[i] >> 4) + 1 of its lists. Term: sdbg_bm25_term for top-k, the
+// bare term id for the unscored passes.
+template <class Term>
+struct QueryBatch {
+  int kind;
+  const Term* terms;
+  const uint32_t* term_off;
+  size_t nq;
+  const uint32_t* excl_terms;
+  const uint32_t* excl_off;
+  const uint8_t* term_grp;
+};
+
 // Checks of a query batch shared by the top-k and count entries: 1..16 positive terms and at most 16 excluded ones per
 // query, a non-decreasing excl_off, segments of one context with staged postings, positive term ids every segment
 // holds, and a staged filter column. Sets *total_excl to excl_off[nq] when some query excludes terms, else 0.
 template <class Term>
-int check_query_batch(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* term_off, size_t nq,
-                      const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint32_t* total_excl) {
+int check_query_batch(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<Term>& Q, const sdbg_col_pred* filt,
+                      uint32_t* total_excl) {
+  const auto& [kind, terms, term_off, nq, excl_terms, excl_off, term_grp] = Q;
   sdbg_ctx* c = segs[0]->ctx;
   for (size_t q = 0; q < nq; ++q) {
     const uint32_t nt = term_off[q + 1] - term_off[q];
@@ -1086,21 +1103,24 @@ int check_query_batch(sdbg_segment* const* segs, size_t n_segs, const Term* term
   return SDBG_OK;
 }
 
-// excl_terms / excl_off: query q excludes the term ids excl_terms[excl_off[q] .. excl_off[q + 1]) (NULL excl_off: none).
-// term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] & 15
-// of its query, which needs (term_grp[i] >> 4) + 1 of its lists. It runs as the OR of all its terms, and a doc must also
-// occur in that many lists of every group.
-int topk_run(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
-             size_t nq, float k1, const float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, TopkDevOut* dev,
-             const uint32_t* excl_terms = nullptr, const uint32_t* excl_off = nullptr, const uint8_t* term_grp = nullptr) {
-  if (!segs || !n_segs || !terms || !term_off || !nq || !k) return SDBG_EINVAL;
-  sdbg_ctx* c = segs[0]->ctx;
+int topk_limits(sdbg_ctx* c, size_t nq, uint32_t k) {
   if (k > 8192) return fail(c, SDBG_EUNSUPPORTED, "k > 8192");
   if (nq > 65535) return fail(c, SDBG_EUNSUPPORTED, "more than 65535 queries per batch");
+  return SDBG_OK;
+}
+
+// A query of OR groups (Q.term_grp) runs as the OR of all its terms, and a doc must also occur in as many lists of every
+// group as the group needs.
+int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm25_term>& Q, float k1, const float b,
+             const sdbg_col_pred* filt, uint32_t k, float threshold_in, TopkDevOut* dev) {
+  const auto& [kind, terms, term_off, nq, excl_terms, excl_off, term_grp] = Q;
+  if (!segs || !n_segs || !terms || !term_off || !nq || !k) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (int rc = topk_limits(c, nq, k)) return rc;
   CU(c, cudaSetDevice(c->device));
   const uint32_t total_terms = term_off[nq];
   uint32_t total_excl = 0;   // > 0: some query excludes terms
-  if (int rc = check_query_batch(segs, n_segs, terms, term_off, nq, excl_terms, excl_off, filt, &total_excl)) return rc;
+  if (int rc = check_query_batch(segs, n_segs, Q, filt, &total_excl)) return rc;
   uint64_t ord = 0;
   uint32_t max_docs = 0;
   for (size_t si = 0; si < n_segs; ++si) {
@@ -1492,15 +1512,15 @@ extern "C" int sdbg_tfidf_topk_batch(sdbg_segment* const* segs, size_t n_segs, i
 }
 
 namespace {
-int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
-                    size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b, const sdbg_col_pred* filt,
-                    uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches,
-                    const uint8_t* term_grp = nullptr) {
+int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm25_term>& Q, float k1, float b,
+                    const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
+                    uint64_t* total_matches) {
   if (!out || !n_out) return SDBG_EINVAL;
   TopkDevOut dev{};
-  int rc = topk_run(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, &dev, excl_terms, excl_off, term_grp);
+  int rc = topk_run(segs, n_segs, Q, k1, b, filt, k, threshold_in, &dev);
   if (rc) return rc;
   sdbg_ctx* c = segs[0]->ctx;
+  const size_t nq = Q.nq;
   const size_t kb = nq * size_t(k) * 8, nb = nq * 4, tb = nq * 8;
   // results come back through a dedicated pinned block (the query descriptors are done with by now)
   if ((rc = ensure_pinned(c, kb + nb + tb + 64))) return rc;
@@ -1555,8 +1575,8 @@ extern "C" int sdbg_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, in
                                     const uint32_t* term_off, size_t nq, float k1, float b, const sdbg_col_pred* filt,
                                     uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
                                     uint64_t* total_matches) {
-  return topk_batch_host(segs, n_segs, kind, terms, term_off, nq, nullptr, nullptr, k1, b, filt, k, threshold_in, out, n_out,
-                         total_matches);
+  return topk_batch_host(segs, n_segs, {kind, terms, term_off, nq, nullptr, nullptr, nullptr}, k1, b, filt, k, threshold_in, out,
+                         n_out, total_matches);
 }
 
 extern "C" int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
@@ -1564,8 +1584,8 @@ extern "C" int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_seg
                                          float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
                                          uint32_t* n_out, uint64_t* total_matches) {
   if (!excl_off) return SDBG_EINVAL;
-  return topk_batch_host(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, k1, b, filt, k, threshold_in, out, n_out,
-                         total_matches);
+  return topk_batch_host(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, k1, b, filt, k, threshold_in,
+                         out, n_out, total_matches);
 }
 
 // ---- conjunctions of OR groups (`a & (b | c) & !d`) ----
@@ -1579,6 +1599,12 @@ struct GroupSplit {
   std::vector<Term> terms[3];
   std::vector<uint32_t> term_off[3], excl_terms[3], excl_off[3];
   std::vector<uint8_t> term_grp[3];
+
+  QueryBatch<Term> view(int sh) const {
+    return {sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR, terms[sh].data(), term_off[sh].data(), qs[sh].size(),
+            excl_terms[sh].empty() ? nullptr : excl_terms[sh].data(), excl_off[sh].data(),
+            sh == 2 ? term_grp[sh].data() : nullptr};
+  }
 };
 
 // Checks of sdbg_*_batch_groups(_min) beyond check_query_batch (which each sub-batch runs as well) and the split by shape:
@@ -1649,41 +1675,61 @@ int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, cons
   }
   return SDBG_OK;
 }
+
+// One per-query output array of a group entry: query q's row is the `bytes` bytes at p + q * bytes (p NULL: not wanted).
+struct OutRows {
+  void* p;
+  size_t bytes;
+};
+
+// Runs a batch of group queries: splits it by shape, checks every shape before anything is queued, then runs each shape
+// as a batch of the flat form, run(view, rows). A batch of one shape writes straight into the caller's rows; otherwise each
+// shape writes temporary rows, which go to the caller's query positions. Checks of the result that every shape would
+// make alike (k, the key range) are the caller's, before this call.
+template <class Term, size_t N, class Run>
+int run_groups(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* group_off,
+               const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+               const uint32_t* excl_off, const sdbg_col_pred* filt, const OutRows (&rows)[N], Run run) {
+  GroupSplit<Term> S;
+  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
+  for (int sh = 0; sh < 3; ++sh) {
+    uint32_t total_excl = 0;
+    if (!S.qs[sh].empty())
+      if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &total_excl)) return rc;
+  }
+  for (int sh = 0; sh < 3; ++sh) {
+    const std::vector<size_t>& qs = S.qs[sh];
+    if (qs.empty()) continue;
+    if (qs.size() == nq) return run(S.view(sh), rows);
+    std::vector<char> tmp[N];
+    OutRows part[N];
+    for (size_t i = 0; i < N; ++i) {
+      if (rows[i].p) tmp[i].resize(qs.size() * rows[i].bytes);
+      part[i] = {rows[i].p ? tmp[i].data() : nullptr, rows[i].bytes};
+    }
+    if (int rc = run(S.view(sh), part)) return rc;
+    for (size_t i = 0; i < N; ++i)
+      if (rows[i].p)
+        for (size_t j = 0; j < qs.size(); ++j)
+          std::memcpy(static_cast<char*>(rows[i].p) + qs[j] * rows[i].bytes, tmp[i].data() + j * rows[i].bytes, rows[i].bytes);
+  }
+  return SDBG_OK;
+}
 }  // namespace
 
-// Top-k of group queries: each shape through topk_batch_host; a batch of one shape writes straight into the caller's arrays.
 extern "C" int sdbg_bm25_topk_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
                                                const uint32_t* group_off, const uint32_t* query_group_off, const uint32_t* group_min,
                                                size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b,
                                                const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
                                                uint32_t* n_out, uint64_t* total_matches) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !out || !n_out) return SDBG_EINVAL;
-  GroupSplit<sdbg_bm25_term> S;
-  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
-  for (int sh = 0; sh < 3; ++sh) {
-    const size_t n = S.qs[sh].size();
-    if (!n) continue;
-    const int kind = sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR;
-    const uint8_t* grp = sh == 2 ? S.term_grp[sh].data() : nullptr;
-    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
-    if (n == nq) {
-      return topk_batch_host(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), k1, b,
-                             filt, k, threshold_in, out, n_out, total_matches, grp);
-    }
-    std::vector<sdbg_hit> h(n * size_t(k));
-    std::vector<uint32_t> hn(n);
-    std::vector<uint64_t> ht(n);
-    if (int rc = topk_batch_host(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), k1, b,
-                                 filt, k, threshold_in, h.data(), hn.data(), ht.data(), grp))
-      return rc;
-    for (size_t j = 0; j < n; ++j) {
-      const size_t q = S.qs[sh][j];
-      std::copy(h.begin() + j * k, h.begin() + j * k + hn[j], out + q * k);
-      n_out[q] = hn[j];
-      if (total_matches) total_matches[q] = ht[j];
-    }
-  }
-  return SDBG_OK;
+  if (int rc = topk_limits(segs[0]->ctx, nq, k)) return rc;
+  return run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                    {{out, k * sizeof(sdbg_hit)}, {n_out, 4}, {total_matches, 8}},
+                    [&](const QueryBatch<sdbg_bm25_term>& Q, const OutRows* r) {
+                      return topk_batch_host(segs, n_segs, Q, k1, b, filt, k, threshold_in, static_cast<sdbg_hit*>(r[0].p),
+                                             static_cast<uint32_t*>(r[1].p), static_cast<uint64_t*>(r[2].p));
+                    });
 }
 
 extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
@@ -1698,9 +1744,8 @@ extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_s
 // Count mode (duckdb_search_full_scan RunCountScan): bm25_count_kernel over work items {query, first window, windows} of
 // kCountWindow-doc windows, planned per segment from posting counts and issued largest first. A single-term query over a
 // segment without filter, deleted docs or an excluded list holding blocks there is answered from the term's docs_count.
-// term_grp (kind OR only; NULL: none): query q is an AND of OR groups, positive term i belongs to group term_grp[i] & 15 of
-// its query (groups 0 .. n - 1 all present), which needs (term_grp[i] >> 4) + 1 of its lists; those queries run
-// bm25_count_kernel<false, true> (with sort / facet: <false, true, true> / <false, true, false, true>).
+// Queries of OR groups (Q.term_grp; groups 0 .. n - 1 of a query all present) run the kGroups instantiations
+// (CountPlan::kernel).
 // sort (NULL: count): the sorted scan of sdbg_match_topk_by_column_batch on the same plan, without the single-term
 // shortcut; see sort_prepare / sort_finish.
 // facet (NULL: count): the facet pass of sdbg_match_facet_counts_batch on the same plan and launches, without the
@@ -1754,7 +1799,6 @@ struct SortJob {
   uint32_t k;
   sdbg_sort_hit* out;
   uint32_t* n_out;
-  bool kind_and;
   // filled by sort_prepare
   std::vector<SortSink> sink;                 // per segment (pointers to outputs set at launch)
   std::vector<std::vector<long long>> zone;   // per segment: host copy of the zonemap (empty: no zone pruning there)
@@ -1849,50 +1893,100 @@ uint32_t count_planes(uint32_t max_min) {
   return planes;
 }
 
+using CountKernel = void (*)(CountParams);
+enum class CountMode { count, sort, facet };
+
+// A count_run plan: per segment each query's lists and the work items; with OR groups (Q.term_grp), each segment's group
+// ends. Its host staging, which every mode shares: [term_off | excl_off | lists per segment | work items {query, first
+// window, windows, 0} | grp_off | group ends per segment]; the sorted scan appends its own arrays.
+struct CountPlan {
+  QueryBatch<uint32_t> Q;
+  uint32_t n_pos, total_excl;
+  uint32_t planes;                               // of the bit-sliced counter, for the batch's largest group minimum
+  std::vector<uint2> lists;                      // per segment: positive lists | excluded lists
+  std::vector<std::vector<CountItem>> seg_work;  // per segment
+  std::vector<uint32_t> grp_off, grp_end;        // grp_off[q] .. grp_off[q + 1] index each segment's group ends
+  size_t off_bytes = 0, lists_pos = 0, work_pos = 0, grp_pos = 0, staged = 0;   // the staging's layout; staged: its bytes
+
+  size_t n_lists() const { return size_t(n_pos) + total_excl; }
+
+  void layout() {
+    size_t items = 0;
+    for (const auto& w : seg_work) items += w.size();
+    off_bytes = (Q.nq + 1) * 4;
+    lists_pos = (2 * off_bytes + 7) & ~size_t(7);
+    work_pos = (lists_pos + lists.size() * sizeof(uint2) + 15) & ~size_t(15);
+    grp_pos = work_pos + items * sizeof(uint4);
+    staged = grp_pos + (Q.term_grp ? off_bytes + grp_end.size() * 4 : 0);
+  }
+
+  void write(char* h) const {
+    std::memcpy(h, Q.term_off, off_bytes);
+    if (total_excl) std::memcpy(h + off_bytes, Q.excl_off, off_bytes);
+    std::memcpy(h + lists_pos, lists.data(), lists.size() * sizeof(uint2));
+    auto* hw = reinterpret_cast<uint4*>(h + work_pos);
+    for (const auto& w : seg_work) for (const CountItem& it : w) *hw++ = make_uint4(it.q, it.w0, it.nw, 0u);
+    if (Q.term_grp) {
+      std::memcpy(h + grp_pos, grp_off.data(), off_bytes);
+      std::memcpy(h + grp_pos + off_bytes, grp_end.data(), grp_end.size() * 4);
+    }
+  }
+
+  // The parameters of segment si's launch over its work items from `first` on, d the device copy of the staging.
+  int params(const char* d, sdbg_segment* s, size_t si, size_t first, const sdbg_col_pred* filt, CountParams* P) const {
+    P->seg = postings_view(s, 0);
+    if (int rc = filter_view(s, filt, &P->filt)) return rc;
+    P->lists = reinterpret_cast<const uint2*>(d + lists_pos) + si * n_lists();
+    P->term_off = reinterpret_cast<const uint32_t*>(d);
+    P->excl_off = total_excl ? reinterpret_cast<const uint32_t*>(d + off_bytes) : nullptr;
+    P->n_pos = n_pos;
+    P->work = reinterpret_cast<const uint4*>(d + work_pos) + first;
+    if (Q.term_grp) {
+      P->grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
+      P->grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[Q.nq];
+    }
+    return SDBG_OK;
+  }
+
+  // The bm25_count_kernel instantiation of this plan's launches in `mode`, with its dynamic shared memory: the mode's
+  // own bytes (facet bins, sorted keys; none for a count), then the counter planes.
+  std::pair<CountKernel, size_t> kernel(CountMode mode, size_t mode_bytes) const {
+    static const CountKernel kernels[3][3] = {   // [OR | AND | OR groups][count | sort | facet]
+        {bm25_count_kernel<false>, bm25_count_kernel<false, false, true>, bm25_count_kernel<false, false, false, true>},
+        {bm25_count_kernel<true>, bm25_count_kernel<true, false, true>, bm25_count_kernel<true, false, false, true>},
+        {bm25_count_kernel<false, true>, bm25_count_kernel<false, true, true>, bm25_count_kernel<false, true, false, true>}};
+    const int shape = Q.term_grp ? 2 : Q.kind == SDBG_QUERY_AND ? 1 : 0;
+    return {kernels[shape][int(mode)], mode_bytes + size_t(planes) * kCountWords * 4u};
+  }
+};
+
 // Launches of the sorted scan over the planned items: per segment its seed items first (all segments), then the rest,
 // each item writing its k best to its own slot (its index in the work array); then sort_merge_kernel per query.
-// grp_off / grp_end (empty: no groups): count_run's OR groups, run by the grouped sorted scan with `planes` counter planes.
-int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const uint32_t* term_off, const uint32_t* excl_off,
-                size_t nq, uint32_t n_pos, uint32_t total_excl, const std::vector<uint2>& lists,
-                const std::vector<std::vector<CountItem>>& seg_work, const sdbg_col_pred* filt,
-                const std::vector<uint32_t>& grp_off, const std::vector<uint32_t>& grp_end, uint32_t planes, SortJob& J) {
-  const size_t n_lists = size_t(n_pos) + total_excl;
+int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt,
+                SortJob& J) {
+  const size_t nq = pl.Q.nq;
   const uint32_t k = J.k, cap = J.sink[0].cap;
-  const bool groups = !grp_off.empty();
   size_t total = 0;
   bool any_zone = false;
-  for (size_t si = 0; si < n_segs; ++si) { total += seg_work[si].size(); any_zone |= J.sink[si].zone != nullptr; }
-  // host staging: [term_off | excl_off | lists per segment | work items | slot_off | slots | segments | grp_off |
-  // group ends per segment]
-  const size_t off_bytes = (nq + 1) * 4;
-  const size_t lists_pos = (2 * off_bytes + 7) & ~size_t(7);
-  const size_t work_pos = (lists_pos + lists.size() * sizeof(uint2) + 15) & ~size_t(15);
-  const size_t slot_off_pos = work_pos + total * sizeof(uint4);
-  const size_t slots_pos = slot_off_pos + off_bytes;
+  for (size_t si = 0; si < n_segs; ++si) { total += pl.seg_work[si].size(); any_zone |= J.sink[si].zone != nullptr; }
+  // host staging: the plan's, then [slot_off | slots | segments]
+  const size_t slot_off_pos = pl.staged;
+  const size_t slots_pos = slot_off_pos + pl.off_bytes;
   const size_t segs_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
-  const size_t grp_pos = segs_pos + n_segs * sizeof(SortSegDev);
-  const size_t bytes = grp_pos + (groups ? off_bytes + grp_end.size() * 4 : 0);
+  const size_t bytes = segs_pos + n_segs * sizeof(SortSegDev);
   int rc = ensure_pinned(c, bytes);
   if (rc) return rc;
   char* h = static_cast<char*>(c->h_pinned);
-  std::memcpy(h, term_off, off_bytes);
-  if (total_excl) std::memcpy(h + off_bytes, excl_off, off_bytes);
-  std::memcpy(h + lists_pos, lists.data(), lists.size() * sizeof(uint2));
-  if (groups) {
-    std::memcpy(h + grp_pos, grp_off.data(), off_bytes);
-    std::memcpy(h + grp_pos + off_bytes, grp_end.data(), grp_end.size() * 4);
-  }
-  auto* hw = reinterpret_cast<uint4*>(h + work_pos);
+  pl.write(h);
+  auto* hw = reinterpret_cast<uint4*>(h + pl.work_pos);
   auto* h_slot_off = reinterpret_cast<uint32_t*>(h + slot_off_pos);
   auto* h_slots = reinterpret_cast<uint32_t*>(h + slots_pos);
   std::fill(h_slot_off, h_slot_off + nq + 1, 0u);
-  uint32_t slot = 0;
-  for (const auto& w : seg_work)
-    for (const CountItem& it : w) { hw[slot] = make_uint4(it.q, it.w0, it.nw, slot); ++h_slot_off[it.q + 1]; ++slot; }
+  for (uint32_t i = 0; i < total; ++i) { hw[i].w = i; ++h_slot_off[hw[i].x + 1]; }
   for (size_t q = 0; q < nq; ++q) h_slot_off[q + 1] += h_slot_off[q];
   {
     std::vector<uint32_t> fillq(h_slot_off, h_slot_off + nq);
-    for (uint32_t i = 0; i < slot; ++i) h_slots[fillq[hw[i].x]++] = i;
+    for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
   }
   auto* h_segs = reinterpret_cast<SortSegDev*>(h + segs_pos);
   for (size_t si = 0; si < n_segs; ++si) {
@@ -1918,41 +2012,27 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const uin
   CU(c, cudaMemsetAsync(thr, 0, nq * 8 + 16, c->stream));   // thresholds and stats
   const size_t smem = size_t(cap) * 16;
   // groups: the counter planes follow the keys (k = 4096 with 4 planes: 128 + 32 KB)
-  const size_t grp_smem = smem + size_t(planes) * kCountWords * 4u;
-  if (groups)
-    CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(grp_smem)));
-  CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-  CU(c, cudaFuncSetAttribute(bm25_count_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-  CU(c, cudaFuncSetAttribute(sort_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  const auto [kernel, kernel_smem] = pl.kernel(CountMode::sort, smem);
+  CU(c, fit_dynamic_smem(kernel, kernel_smem));
+  CU(c, fit_dynamic_smem(sort_merge_kernel, smem));
   if (total) {
     for (int phase = 0; phase < 2; ++phase) {   // seeds, then the rest
       size_t begin = 0;
       for (size_t si = 0; si < n_segs; ++si) {
-        const auto& w = seg_work[si];
+        const auto& w = pl.seg_work[si];
         const size_t n_seed = size_t(std::count_if(w.begin(), w.end(), [](const CountItem& x) { return x.seed; }));
         const size_t first = begin + (phase ? n_seed : 0), n = phase ? w.size() - n_seed : n_seed;
         begin += w.size();
         if (!n) continue;
         CountParams P;
-        P.seg = postings_view(segs[si], 0);
-        if ((rc = filter_view(segs[si], filt, &P.filt))) return rc;
-        P.lists = reinterpret_cast<const uint2*>(d + lists_pos) + si * n_lists;
-        P.term_off = reinterpret_cast<const uint32_t*>(d);
-        P.excl_off = total_excl ? reinterpret_cast<const uint32_t*>(d + off_bytes) : nullptr;
-        P.n_pos = n_pos;
-        P.work = reinterpret_cast<const uint4*>(d + work_pos) + first;
+        if ((rc = pl.params(d, segs[si], si, first, filt, &P))) return rc;
         P.counts = nullptr;
         P.sort = J.sink[si];
         P.sort.thr = c->wand ? thr : nullptr;
         P.sort.out = reinterpret_cast<ulonglong2*>(o);
         P.sort.out_n = reinterpret_cast<uint32_t*>(o + keys_n_pos);
         P.sort.stats = stats;
-        if (groups) {
-          P.grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
-          P.grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[nq];
-          bm25_count_kernel<false, true, true><<<unsigned(n), kCountThreads, grp_smem, c->stream>>>(P);
-        } else if (J.kind_and) bm25_count_kernel<true, false, true><<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
-        else bm25_count_kernel<false, false, true><<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
+        kernel<<<unsigned(n), kCountThreads, kernel_smem, c->stream>>>(P);
         ++c->launches;
       }
     }
@@ -1981,14 +2061,14 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const uin
   return SDBG_OK;
 }
 
-int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms, const uint32_t* term_off, size_t nq,
-              const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts,
-              const uint8_t* term_grp = nullptr, SortJob* sort = nullptr, FacetJob* facet = nullptr) {
+int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_t>& Q, const sdbg_col_pred* filt,
+              uint64_t* counts, SortJob* sort = nullptr, FacetJob* facet = nullptr) {
+  const auto& [kind, terms, term_off, nq, excl_terms, excl_off, term_grp] = Q;
   if (!segs || !n_segs || !terms || !term_off || !nq || (!counts && !sort && !facet)) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   CU(c, cudaSetDevice(c->device));
   uint32_t total_excl = 0;
-  if (int rc = check_query_batch(segs, n_segs, terms, term_off, nq, excl_terms, excl_off, filt, &total_excl)) return rc;
+  if (int rc = check_query_batch(segs, n_segs, Q, filt, &total_excl)) return rc;
   if (sort)
     if (int rc = sort_prepare(c, segs, n_segs, *sort)) return rc;
   if (facet)
@@ -2124,30 +2204,16 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
     std::stable_partition(seg_work[si].begin(), seg_work[si].end(), [](const Item& x) { return x.seed; });
     total_items += seg_work[si].size();
   }
-  if (sort) {
-    sort->kind_and = conj;
-    return sort_finish(c, segs, n_segs, term_off, excl_off, nq, n_pos, total_excl, lists, seg_work, filt, grp_off, grp_end,
-                       count_planes(max_min), *sort);
-  }
+  CountPlan pl{Q, n_pos, total_excl, count_planes(max_min), std::move(lists), std::move(seg_work), std::move(grp_off),
+               std::move(grp_end)};
+  pl.layout();
+  if (sort) return sort_finish(c, segs, n_segs, pl, filt, *sort);
   if (total_items) {
-    // [term_off | excl_off | lists per segment | work items | grp_off | group ends per segment]
-    const size_t off_bytes = (nq + 1) * 4;
-    const size_t lists_pos = (2 * off_bytes + 7) & ~size_t(7);
-    const size_t work_pos = (lists_pos + lists.size() * sizeof(uint2) + 15) & ~size_t(15);
-    const size_t grp_pos = work_pos + total_items * sizeof(uint4);
-    const size_t bytes = grp_pos + (term_grp ? off_bytes + grp_end.size() * 4 : 0);
+    const size_t bytes = pl.staged;
     int rc = ensure_pinned(c, std::max(bytes, nq * 8));
     if (rc) return rc;
     char* h = static_cast<char*>(c->h_pinned);
-    std::memcpy(h, term_off, off_bytes);
-    if (total_excl) std::memcpy(h + off_bytes, excl_off, off_bytes);
-    std::memcpy(h + lists_pos, lists.data(), lists.size() * sizeof(uint2));
-    auto* hw = reinterpret_cast<uint4*>(h + work_pos);
-    for (auto& w : seg_work) for (const Item& it : w) *hw++ = make_uint4(it.q, it.w0, it.nw, 0u);
-    if (term_grp) {
-      std::memcpy(h + grp_pos, grp_off.data(), off_bytes);
-      std::memcpy(h + grp_pos + off_bytes, grp_end.data(), grp_end.size() * 4);
-    }
+    pl.write(h);
     DevBuf& b_desc = c->scratch[0]; DevBuf& b_counts = c->scratch[1];
     // facet pass: b_counts holds [counts | facet counts [nq][span] | NULL counts [nq] | out-of-range word]
     const size_t fc_pos = nq * 8, fn_pos = fc_pos + (facet ? nq * size_t(facet->span) * 8 : 0), oor_pos = fn_pos + nq * 8;
@@ -2157,49 +2223,27 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
     CU(c, cudaMemcpyAsync(b_desc.p, h, bytes, cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaMemsetAsync(b_counts.p, 0, out_bytes, c->stream));
     char* fo = static_cast<char*>(b_counts.p);
-    const size_t facet_smem = facet ? (size_t(facet->span) * 4 + 15) & ~size_t(15) : 0;
-    if (facet && !term_grp) {
-      CU(c, fit_dynamic_smem(bm25_count_kernel<false, false, false, true>, facet_smem));
-      CU(c, fit_dynamic_smem(bm25_count_kernel<true, false, false, true>, facet_smem));
-    }
-    // groups that need m >= 2 of their lists: a bit-sliced counter of bits(m) planes for the batch's largest m, after the
-    // facet bins (at most 128 + 32 KB)
-    const size_t count_smem = size_t(count_planes(max_min)) * kCountWords * 4u;
-    if (term_grp && facet)
-      CU(c, fit_dynamic_smem(bm25_count_kernel<false, true, false, true>, facet_smem + count_smem));
-    else if (term_grp && count_smem)
-      CU(c, cudaFuncSetAttribute(bm25_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(count_smem)));
+    // the facet bins, then for groups that need m >= 2 of their lists a bit-sliced counter of bits(m) planes for the
+    // batch's largest m (at most 128 + 32 KB)
+    const auto [kernel, smem] = facet ? pl.kernel(CountMode::facet, (size_t(facet->span) * 4 + 15) & ~size_t(15))
+                                      : pl.kernel(CountMode::count, 0);
+    CU(c, fit_dynamic_smem(kernel, smem));
     const char* d = static_cast<const char*>(b_desc.p);
     size_t done = 0;
     for (size_t si = 0; si < n_segs; ++si) {
-      if (seg_work[si].empty()) continue;
+      const size_t n = pl.seg_work[si].size();
+      if (!n) continue;
       CountParams P;
-      P.seg = postings_view(segs[si], 0);
-      if ((rc = filter_view(segs[si], filt, &P.filt))) return rc;
-      P.lists = reinterpret_cast<const uint2*>(d + lists_pos) + si * n_lists;
-      P.term_off = reinterpret_cast<const uint32_t*>(d);
-      P.excl_off = total_excl ? reinterpret_cast<const uint32_t*>(d + off_bytes) : nullptr;
-      P.n_pos = n_pos;
-      P.work = reinterpret_cast<const uint4*>(d + work_pos) + done;
+      if ((rc = pl.params(d, segs[si], si, done, filt, &P))) return rc;
       P.counts = static_cast<unsigned long long*>(b_counts.p);
-      done += seg_work[si].size();
-      if (term_grp) {
-        P.grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
-        P.grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[nq];
-      }
+      done += n;
       if (facet) {
         P.facet = facet->sink[si];
         P.facet.counts = reinterpret_cast<unsigned long long*>(fo + fc_pos);
         P.facet.nulls = reinterpret_cast<unsigned long long*>(fo + fn_pos);
         P.facet.out_of_range = reinterpret_cast<unsigned int*>(fo + oor_pos);
-        if (term_grp)
-          bm25_count_kernel<false, true, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem + count_smem, c->stream>>>(P);
-        else if (conj) bm25_count_kernel<true, false, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem, c->stream>>>(P);
-        else bm25_count_kernel<false, false, false, true><<<unsigned(seg_work[si].size()), kCountThreads, facet_smem, c->stream>>>(P);
-      } else if (term_grp) {
-        bm25_count_kernel<false, true><<<unsigned(seg_work[si].size()), kCountThreads, count_smem, c->stream>>>(P);
-      } else if (conj) bm25_count_kernel<true><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
-      else bm25_count_kernel<false><<<unsigned(seg_work[si].size()), kCountThreads, 0, c->stream>>>(P);
+      }
+      kernel<<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
       ++c->launches;
     }
     CU(c, cudaGetLastError());
@@ -2230,7 +2274,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t
 extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
                                       const uint32_t* term_off, size_t nq, const uint32_t* excl_terms,
                                       const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
-  return count_run(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, filt, counts);
+  return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, counts);
 }
 
 extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -2239,8 +2283,8 @@ extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t
                                                int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
   if (!segs || !n_segs || !segs[0] || !k || !out || !n_out) return SDBG_EINVAL;
   if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
-  SortJob J{sort_field, descending, nulls_first, k, out, n_out, false, {}, {}};
-  return count_run(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, filt, nullptr, nullptr, &J);
+  SortJob J{sort_field, descending, nulls_first, k, out, n_out, {}, {}};
+  return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, nullptr, &J);
 }
 
 extern "C" int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -2249,7 +2293,7 @@ extern "C" int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n
                                              int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
   if (!counts || !null_counts) return SDBG_EINVAL;
   FacetJob J{key_field, key_min, key_span, counts, null_counts, {}};
-  return count_run(segs, n_segs, kind, terms, term_off, nq, excl_terms, excl_off, filt, nullptr, nullptr, nullptr, &J);
+  return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, nullptr, nullptr, &J);
 }
 
 extern "C" int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2257,22 +2301,10 @@ extern "C" int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size
                                                  const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
                                                  const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts) return SDBG_EINVAL;
-  GroupSplit<uint32_t> S;
-  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
-  for (int sh = 0; sh < 3; ++sh) {
-    const size_t n = S.qs[sh].size();
-    if (!n) continue;
-    const int kind = sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR;
-    const uint8_t* grp = sh == 2 ? S.term_grp[sh].data() : nullptr;
-    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
-    std::vector<uint64_t> cn(n);
-    if (int rc = count_run(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), filt,
-                           n == nq ? counts : cn.data(), grp))
-      return rc;
-    if (n != nq)
-      for (size_t j = 0; j < n; ++j) counts[S.qs[sh][j]] = cn[j];
-  }
-  return SDBG_OK;
+  return run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, {{counts, 8}},
+                    [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
+                      return count_run(segs, n_segs, Q, filt, static_cast<uint64_t*>(r[0].p));
+                    });
 }
 
 extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2283,25 +2315,6 @@ extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n
                                            filt, counts);
 }
 
-namespace {
-// The query checks of every shape of a split batch, so that a batch whose later shape is malformed queues nothing. The
-// column checks are the same for every shape: the first shape's count_run makes them before it queues anything.
-int check_shapes(sdbg_segment* const* segs, size_t n_segs, const GroupSplit<uint32_t>& S, const sdbg_col_pred* filt) {
-  for (int sh = 0; sh < 3; ++sh) {
-    const size_t n = S.qs[sh].size();
-    if (!n) continue;
-    uint32_t total_excl = 0;
-    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
-    if (int rc = check_query_batch(segs, n_segs, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), filt,
-                                   &total_excl))
-      return rc;
-  }
-  return SDBG_OK;
-}
-}  // namespace
-
-// Sorted scan of group queries: each shape through count_run's sorted scan (shape 2 with its groups), results scattered
-// back to the caller's query positions; sdbg_scan_stats then reports the sum over the shapes.
 extern "C" int sdbg_match_topk_by_column_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
                                                           const uint32_t* group_off, const uint32_t* query_group_off,
                                                           const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
@@ -2311,32 +2324,20 @@ extern "C" int sdbg_match_topk_by_column_batch_groups_min(sdbg_segment* const* s
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !out || !n_out) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
-  GroupSplit<uint32_t> S;
-  if (int rc = split_groups(c, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
-  if (int rc = check_shapes(segs, n_segs, S, filt)) return rc;
   uint64_t judged = 0, skipped = 0;
-  for (int sh = 0; sh < 3; ++sh) {
-    const size_t n = S.qs[sh].size();
-    if (!n) continue;
-    const int kind = sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR;
-    const uint8_t* grp = sh == 2 ? S.term_grp[sh].data() : nullptr;
-    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
-    std::vector<sdbg_sort_hit> h(n == nq ? 0 : n * size_t(k));
-    std::vector<uint32_t> hn(n == nq ? 0 : n);
-    SortJob J{sort_field, descending, nulls_first, k, n == nq ? out : h.data(), n == nq ? n_out : hn.data(), false, {}, {}};
-    if (int rc = count_run(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), filt,
-                           nullptr, grp, &J))
-      return rc;
-    if (n == nq) return SDBG_OK;
-    for (size_t j = 0; j < n; ++j) {
-      const size_t q = S.qs[sh][j];
-      std::copy(h.begin() + j * k, h.begin() + j * k + hn[j], out + q * k);
-      n_out[q] = hn[j];
-    }
-    uint64_t t = 0, s = 0;
-    if (int rc = sdbg_scan_stats(c, &t, &s)) return rc;
-    judged += t; skipped += s;
-  }
+  bool whole = false;   // the batch is one shape: the scan statistics are already the call's
+  const int rc = run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                            {{out, k * sizeof(sdbg_sort_hit)}, {n_out, 4}}, [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
+                              SortJob J{sort_field, descending, nulls_first, k, static_cast<sdbg_sort_hit*>(r[0].p),
+                                        static_cast<uint32_t*>(r[1].p), {}, {}};
+                              if (int rc = count_run(segs, n_segs, Q, filt, nullptr, &J)) return rc;
+                              whole = Q.nq == nq;
+                              uint64_t t = 0, s = 0;
+                              if (int rc = whole ? SDBG_OK : sdbg_scan_stats(c, &t, &s)) return rc;
+                              judged += t; skipped += s;
+                              return SDBG_OK;
+                            });
+  if (rc || whole) return rc;
   // the windows of the whole call, not of its last shape
   c->zone_blocks_total = judged;
   CU(c, cudaMemcpyAsync(c->d_zone_skipped, &skipped, 8, cudaMemcpyHostToDevice, c->stream));
@@ -2344,8 +2345,6 @@ extern "C" int sdbg_match_topk_by_column_batch_groups_min(sdbg_segment* const* s
   return SDBG_OK;
 }
 
-// Facet counts of group queries: each shape through count_run's facet pass (shape 2 with its groups), rows scattered back
-// to the caller's query positions.
 extern "C" int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
                                                         const uint32_t* group_off, const uint32_t* query_group_off,
                                                         const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
@@ -2353,29 +2352,12 @@ extern "C" int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* seg
                                                         int64_t key_min, uint32_t key_span, uint64_t* counts,
                                                         uint64_t* null_counts) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts || !null_counts) return SDBG_EINVAL;
-  GroupSplit<uint32_t> S;
-  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
-  if (int rc = check_shapes(segs, n_segs, S, filt)) return rc;
-  if (int rc = facet_check_range(segs[0]->ctx, key_min, key_span)) return rc;   // before the staging rows are sized
-  for (int sh = 0; sh < 3; ++sh) {
-    const size_t n = S.qs[sh].size();
-    if (!n) continue;
-    const int kind = sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR;
-    const uint8_t* grp = sh == 2 ? S.term_grp[sh].data() : nullptr;
-    const uint32_t* xt = S.excl_terms[sh].empty() ? nullptr : S.excl_terms[sh].data();
-    std::vector<uint64_t> fc(n == nq ? 0 : n * size_t(key_span)), fn(n == nq ? 0 : n);
-    FacetJob J{key_field, key_min, key_span, n == nq ? counts : fc.data(), n == nq ? null_counts : fn.data(), {}};
-    if (int rc = count_run(segs, n_segs, kind, S.terms[sh].data(), S.term_off[sh].data(), n, xt, S.excl_off[sh].data(), filt,
-                           nullptr, grp, nullptr, &J))
-      return rc;
-    if (n == nq) return SDBG_OK;
-    for (size_t j = 0; j < n; ++j) {
-      const size_t q = S.qs[sh][j];
-      std::copy(fc.begin() + j * key_span, fc.begin() + (j + 1) * key_span, counts + q * key_span);
-      null_counts[q] = fn[j];
-    }
-  }
-  return SDBG_OK;
+  if (int rc = facet_check_range(segs[0]->ctx, key_min, key_span)) return rc;   // before the rows are sized
+  return run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                    {{counts, size_t(key_span) * 8}, {null_counts, 8}}, [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
+                      FacetJob J{key_field, key_min, key_span, static_cast<uint64_t*>(r[0].p), static_cast<uint64_t*>(r[1].p), {}};
+                      return count_run(segs, n_segs, Q, filt, nullptr, nullptr, &J);
+                    });
 }
 
 // Streaming mode (duckdb_search_full_scan.cpp RunStreamingScan :2370-2403; DocIterator::EmitScoredDocs,
@@ -2545,7 +2527,7 @@ int topk_batch_device_impl(sdbg_segment* const* segs, size_t n_segs, int kind, c
                            void* d_keys, void* d_totals, bool sync) {
   if (!d_keys) return SDBG_EINVAL;
   TopkDevOut dev{};
-  int rc = topk_run(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, &dev);
+  int rc = topk_run(segs, n_segs, {kind, terms, term_off, nq, nullptr, nullptr, nullptr}, k1, b, filt, k, threshold_in, &dev);
   if (rc) return rc;
   sdbg_ctx* c = segs[0]->ctx;
   // Each rank owns a 2^28-ordinal slot in the merged key space: rank r's docs sort after rank r-1's on ties.

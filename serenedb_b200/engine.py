@@ -461,31 +461,53 @@ def _exclusions(exclude, nq):
     return np.ascontiguousarray([t for x in lists for t in x], dtype=np.uint32), off
 
 
+def _query_args(queries, exclude, min_match=None, groups=False, stats=None):
+    """The query arguments of a batch entry: (terms, term_off, nq, excl_terms, excl_off) of a flat entry or, with `groups`,
+    (terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off) of a group entry. terms: the term ids as u32
+    (NULL when there are none), or with `stats` (term id -> sdbg_bm25_term) the scored entries' array. excl_terms and
+    excl_off are NULL when no query excludes anything."""
+    nq = len(queries)
+    if groups:
+        ids, group_off, query_group_off = _groups(queries)
+        offsets = (_ptr(group_off), _ptr(query_group_off), _ptr(_group_min(min_match, queries)))
+    else:
+        ids = [t for q in queries for t in q]
+        off = np.zeros(nq + 1, np.uint32)
+        off[1:] = np.cumsum([len(q) for q in queries])
+        offsets = (_ptr(off),)
+    if stats is None:
+        flat = np.ascontiguousarray(ids, dtype=np.uint32)
+        terms = _ptr(flat) if len(flat) else None
+    else:
+        terms = (N.BM25Term * max(len(ids), 1))(*[stats(t) for t in ids])
+    x = _exclusions(exclude, nq) or (None, None)
+    return (terms,) + offsets + (nq, _ptr(x[0]), _ptr(x[1]))
+
+
+def _one(x):
+    """A single query's per-query argument (its terms, groups, exclusions or group minimums) as a batch of one."""
+    return None if x is None else [list(x)]
+
+
+def _ref(filt):
+    return C.byref(filt) if filt is not None else None
+
+
 def ExecuteTopKBatch(reader, queries, kind, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
     """Batch of ExecuteTopK calls (doc_collector.hpp:88-136). queries: list of term-id lists. exclude: None, or one list of
     excluded term ids (or None) per query -- `a & b & !c` (sdbg_bm25_topk_batch_excl).
     Returns (hits [Q, k] structured, n_out [Q], total_matches [Q])."""
-    nq = len(queries)
-    flat = [reader.stats(scorer, t) for q in queries for t in q]
-    terms = (N.BM25Term * max(len(flat), 1))()
-    for i, t in enumerate(flat):
-        terms[i] = t
-    off = np.zeros(nq + 1, np.uint32)
-    off[1:] = np.cumsum([len(q) for q in queries])
+    terms, off, nq, excl_terms, excl_off = _query_args(queries, exclude, stats=lambda t: reader.stats(scorer, t))
     hits = np.zeros((nq, k), HIT_DTYPE)
     n_out = np.zeros(nq, np.uint32)
     total = np.zeros(nq, np.uint64)
-    ctx = reader.segments[0].ctx
-    fp = C.byref(filt) if filt is not None else None
-    x = _exclusions(exclude, nq)
-    if x is None:
-        N.check(N.lib().sdbg_bm25_topk_batch(_seg_array(reader.segments), len(reader.segments), int(kind), terms,
-                                             _ptr(off), nq, scorer.k, scorer.b, fp, int(k), float(threshold), _ptr(hits),
-                                             _ptr(n_out), _ptr(total)), ctx._h)
+    head = (_seg_array(reader.segments), len(reader.segments), int(kind), terms, off, nq)
+    tail = (scorer.k, scorer.b, _ref(filt), int(k), float(threshold), _ptr(hits), _ptr(n_out), _ptr(total))
+    if excl_off is None:
+        rc = N.lib().sdbg_bm25_topk_batch(*head, *tail)
     else:
-        N.check(N.lib().sdbg_bm25_topk_batch_excl(_seg_array(reader.segments), len(reader.segments), int(kind), terms,
-                                                  _ptr(off), nq, _ptr(x[0]), _ptr(x[1]), scorer.k, scorer.b, fp, int(k),
-                                                  float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)), ctx._h)
+        rc = N.lib().sdbg_bm25_topk_batch_excl(*head, excl_terms, excl_off, *tail)
+    N.check(rc, reader.segments[0].ctx._h)
     return hits, n_out, total
 
 
@@ -493,24 +515,16 @@ def ExecuteCountBatch(reader, queries, kind, filt=None, exclude=None):
     """Count mode of the search scan (`SELECT count(*) ... WHERE body @@ '...'`, sdbg_match_count_batch): per query, the
     number of docs over all segments that match its term ids (OR / AND), are not deleted, pass `filt` and hold none of its
     `exclude` term ids. Nothing is scored, so no statistics are needed; exact at every pruning level. Returns uint64[Q]."""
-    nq = len(queries)
-    flat = np.ascontiguousarray([t for q in queries for t in q], dtype=np.uint32)
-    off = np.zeros(nq + 1, np.uint32)
-    off[1:] = np.cumsum([len(q) for q in queries])
-    counts = np.zeros(nq, np.uint64)
-    x = _exclusions(exclude, nq)
-    fp = C.byref(filt) if filt is not None else None
+    counts = np.zeros(len(queries), np.uint64)
     N.check(N.lib().sdbg_match_count_batch(_seg_array(reader.segments), len(reader.segments), int(kind),
-                                           _ptr(flat) if len(flat) else None, _ptr(off), nq,
-                                           _ptr(x[0]) if x is not None else None, _ptr(x[1]) if x is not None else None, fp,
-                                           _ptr(counts)), reader.segments[0].ctx._h)
+                                           *_query_args(queries, exclude), _ref(filt), _ptr(counts)),
+            reader.segments[0].ctx._h)
     return counts
 
 
 def ExecuteCount(reader, query_terms, kind, filt=None, exclude=None):
     """ExecuteCountBatch for one query: its match count as an int."""
-    return int(ExecuteCountBatch(reader, [list(query_terms)], kind, filt,
-                                 exclude=None if exclude is None else [list(exclude)])[0])
+    return int(ExecuteCountBatch(reader, _one(query_terms), kind, filt, exclude=_one(exclude))[0])
 
 
 SORT_HIT_DTYPE = np.dtype([("value", "<i8"), ("doc", "<u4"), ("seg", "<u4"), ("is_null", "u1"), ("pad", "V7")])
@@ -525,17 +539,10 @@ def ExecuteTopKByColumnBatch(reader, queries, kind, sort_field, k, descending=Fa
     values (typed by the column; 0 for NULL), nulls (bool) and n_out (uint32[Q])."""
     vt = _sort_value_type(reader, sort_field)
     nq = len(queries)
-    flat = np.ascontiguousarray([t for q in queries for t in q], dtype=np.uint32)
-    off = np.zeros(nq + 1, np.uint32)
-    off[1:] = np.cumsum([len(q) for q in queries])
     hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
     n_out = np.zeros(max(nq, 1), np.uint32)
-    x = _exclusions(exclude, nq)
-    fp = C.byref(filt) if filt is not None else None
     N.check(N.lib().sdbg_match_topk_by_column_batch(_seg_array(reader.segments), len(reader.segments), int(kind),
-                                                    _ptr(flat) if len(flat) else None, _ptr(off), nq,
-                                                    _ptr(x[0]) if x is not None else None,
-                                                    _ptr(x[1]) if x is not None else None, fp, int(sort_field),
+                                                    *_query_args(queries, exclude), _ref(filt), int(sort_field),
                                                     int(bool(descending)), int(bool(nulls_first)), int(k), _ptr(hits),
                                                     _ptr(n_out)), reader.segments[0].ctx._h)
     return _sort_result(hits, n_out, nq, k, vt)
@@ -561,12 +568,16 @@ def _sort_result(hits, n_out, nq, k, vt):
     return out
 
 
+def _sort_row(r):
+    """The first query of a sorted-scan result: dict of docs, segs, values, nulls."""
+    return {key: r[key][0] for key in ("docs", "segs", "values", "nulls")}
+
+
 def ExecuteTopKByColumn(reader, query_terms, kind, sort_field, k, descending=False, nulls_first=False, filt=None,
                         exclude=None):
     """ExecuteTopKByColumnBatch for one query: dict of docs, segs, values, nulls (arrays of n_out entries)."""
-    r = ExecuteTopKByColumnBatch(reader, [list(query_terms)], kind, sort_field, k, descending, nulls_first, filt,
-                                 exclude=None if exclude is None else [list(exclude)])
-    return dict(docs=r["docs"][0], segs=r["segs"][0], values=r["values"][0], nulls=r["nulls"][0])
+    return _sort_row(ExecuteTopKByColumnBatch(reader, _one(query_terms), kind, sort_field, k, descending, nulls_first, filt,
+                                              exclude=_one(exclude)))
 
 
 def ExecuteFacetCountsBatch(reader, queries, kind, key_field, key_min=None, key_span=None, filt=None, exclude=None):
@@ -577,17 +588,10 @@ def ExecuteFacetCountsBatch(reader, queries, kind, key_field, key_min=None, key_
     whose key is v, nulls[q] = matches whose key is NULL."""
     key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
     nq = len(queries)
-    flat = np.ascontiguousarray([t for q in queries for t in q], dtype=np.uint32)
-    off = np.zeros(nq + 1, np.uint32)
-    off[1:] = np.cumsum([len(q) for q in queries])
     counts = np.zeros((max(nq, 1), max(int(key_span), 1)), np.uint64)
     nulls = np.zeros(max(nq, 1), np.uint64)
-    x = _exclusions(exclude, nq)
-    fp = C.byref(filt) if filt is not None else None
     N.check(N.lib().sdbg_match_facet_counts_batch(_seg_array(reader.segments), len(reader.segments), int(kind),
-                                                  _ptr(flat) if len(flat) else None, _ptr(off), nq,
-                                                  _ptr(x[0]) if x is not None else None,
-                                                  _ptr(x[1]) if x is not None else None, fp, int(key_field), int(key_min),
+                                                  *_query_args(queries, exclude), _ref(filt), int(key_field), int(key_min),
                                                   int(key_span), _ptr(counts), _ptr(nulls)), reader.segments[0].ctx._h)
     return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
 
@@ -609,16 +613,21 @@ def _facet_key_range(reader, key_field, key_min, key_span):
     return key_min, key_span
 
 
-def ExecuteFacetCounts(reader, query_terms, kind, key_field, key_min=None, key_span=None, filt=None, exclude=None):
-    """ExecuteFacetCountsBatch for one query: {key: count} for the keys with matches, plus {None: n} when n > 0 matches
+def _facet_row(r):
+    """The first query of a facet-counts result: {key: count} for the keys with matches, plus {None: n} when n > 0 matches
     have a NULL key."""
-    r = ExecuteFacetCountsBatch(reader, [list(query_terms)], kind, key_field, key_min, key_span, filt,
-                                exclude=None if exclude is None else [list(exclude)])
     row = r["counts"][0]
     out = {r["key_min"] + int(i): int(row[i]) for i in np.nonzero(row)[0]}
     if r["nulls"][0]:
         out[None] = int(r["nulls"][0])
     return out
+
+
+def ExecuteFacetCounts(reader, query_terms, kind, key_field, key_min=None, key_span=None, filt=None, exclude=None):
+    """ExecuteFacetCountsBatch for one query: {key: count} for the keys with matches, plus {None: n} when n > 0 matches
+    have a NULL key."""
+    return _facet_row(ExecuteFacetCountsBatch(reader, _one(query_terms), kind, key_field, key_min, key_span, filt,
+                                              exclude=_one(exclude)))
 
 
 def _groups(queries):
@@ -640,36 +649,32 @@ def _group_min(min_match, queries):
     return np.ascontiguousarray([int(v) for m in min_match for v in m], dtype=np.uint32)
 
 
+def _one_groups(groups):
+    """A single query of OR groups as a batch of one."""
+    return [[list(g) for g in groups]]
+
+
 def ExecuteTopKGroupsBatch(reader, queries, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, min_match=None):
     """Top-k of conjunctions of OR groups (`a & (b | c) & !d`, sdbg_bm25_topk_batch_groups_min). queries: per query a list of
     1..16 groups, each a non-empty list of term ids (1..16 distinct ids per query in all). A hit's score is the score the
     flat OR of the query's terms gives that doc. exclude: as in ExecuteTopKBatch. min_match: per query one minimum per
     group (`2 of (a | b | c)`: a doc needs that many of the group's terms), 1..the group's size; None: 1 everywhere.
     Returns (hits [Q, k], n_out [Q], total_matches [Q])."""
+    args = _query_args(queries, exclude, min_match, groups=True, stats=lambda t: reader.stats(scorer, t))
     nq = len(queries)
-    ids, group_off, query_group_off = _groups(queries)
-    gmin = _group_min(min_match, queries)
-    terms = (N.BM25Term * max(len(ids), 1))()
-    for i, t in enumerate(ids):
-        terms[i] = reader.stats(scorer, t)
     hits = np.zeros((nq, k), HIT_DTYPE)
     n_out = np.zeros(nq, np.uint32)
     total = np.zeros(nq, np.uint64)
-    x = _exclusions(exclude, nq)
-    fp = C.byref(filt) if filt is not None else None
-    N.check(N.lib().sdbg_bm25_topk_batch_groups_min(_seg_array(reader.segments), len(reader.segments), terms, _ptr(group_off),
-                                                    _ptr(query_group_off), _ptr(gmin) if gmin is not None else None, nq,
-                                                    _ptr(x[0]) if x is not None else None,
-                                                    _ptr(x[1]) if x is not None else None, scorer.k, scorer.b, fp, int(k),
-                                                    float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
+    N.check(N.lib().sdbg_bm25_topk_batch_groups_min(_seg_array(reader.segments), len(reader.segments), *args, scorer.k,
+                                                    scorer.b, _ref(filt), int(k), float(threshold), _ptr(hits), _ptr(n_out),
+                                                    _ptr(total)), reader.segments[0].ctx._h)
     return hits, n_out, total
 
 
 def ExecuteTopKGroups(reader, groups, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, min_match=None):
     """ExecuteTopKGroupsBatch for one query (a list of OR groups; min_match: one minimum per group): (hits, total_matches)."""
-    hits, n_out, total = ExecuteTopKGroupsBatch(reader, [[list(g) for g in groups]], scorer, k, filt, threshold,
-                                                exclude=None if exclude is None else [list(exclude)],
-                                                min_match=None if min_match is None else [list(min_match)])
+    hits, n_out, total = ExecuteTopKGroupsBatch(reader, _one_groups(groups), scorer, k, filt, threshold, exclude=_one(exclude),
+                                                min_match=_one(min_match))
     return hits[0, :n_out[0]].copy(), int(total[0])
 
 
@@ -678,26 +683,16 @@ def ExecuteCountGroupsBatch(reader, queries, filt=None, exclude=None, min_match=
     segments in which every group has a term (min_match: per query one minimum per group, as in ExecuteTopKGroupsBatch),
     that are not deleted, pass `filt` and hold none of its `exclude` term ids. Exact at every pruning level. Returns
     uint64[Q]."""
-    nq = len(queries)
-    ids, group_off, query_group_off = _groups(queries)
-    gmin = _group_min(min_match, queries)
-    flat = np.ascontiguousarray(ids, dtype=np.uint32)
-    counts = np.zeros(nq, np.uint64)
-    x = _exclusions(exclude, nq)
-    fp = C.byref(filt) if filt is not None else None
+    counts = np.zeros(len(queries), np.uint64)
     N.check(N.lib().sdbg_match_count_batch_groups_min(_seg_array(reader.segments), len(reader.segments),
-                                                      _ptr(flat) if len(flat) else None, _ptr(group_off), _ptr(query_group_off),
-                                                      _ptr(gmin) if gmin is not None else None, nq,
-                                                      _ptr(x[0]) if x is not None else None, _ptr(x[1]) if x is not None else None,
-                                                      fp, _ptr(counts)), reader.segments[0].ctx._h)
+                                                      *_query_args(queries, exclude, min_match, groups=True), _ref(filt),
+                                                      _ptr(counts)), reader.segments[0].ctx._h)
     return counts
 
 
 def ExecuteCountGroups(reader, groups, filt=None, exclude=None, min_match=None):
     """ExecuteCountGroupsBatch for one query: its match count as an int."""
-    return int(ExecuteCountGroupsBatch(reader, [[list(g) for g in groups]], filt,
-                                       exclude=None if exclude is None else [list(exclude)],
-                                       min_match=None if min_match is None else [list(min_match)])[0])
+    return int(ExecuteCountGroupsBatch(reader, _one_groups(groups), filt, exclude=_one(exclude), min_match=_one(min_match))[0])
 
 
 def ExecuteTopKByColumnGroupsBatch(reader, queries, sort_field, k, descending=False, nulls_first=False, filt=None,
@@ -708,28 +703,20 @@ def ExecuteTopKByColumnGroupsBatch(reader, queries, sort_field, k, descending=Fa
     ExecuteTopKByColumnBatch returns."""
     vt = _sort_value_type(reader, sort_field)
     nq = len(queries)
-    ids, group_off, query_group_off = _groups(queries)
-    gmin = _group_min(min_match, queries)
-    flat = np.ascontiguousarray(ids, dtype=np.uint32)
     hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
     n_out = np.zeros(max(nq, 1), np.uint32)
-    x = _exclusions(exclude, nq)
-    fp = C.byref(filt) if filt is not None else None
     N.check(N.lib().sdbg_match_topk_by_column_batch_groups_min(
-        _seg_array(reader.segments), len(reader.segments), _ptr(flat) if len(flat) else None, _ptr(group_off),
-        _ptr(query_group_off), _ptr(gmin) if gmin is not None else None, nq, _ptr(x[0]) if x is not None else None,
-        _ptr(x[1]) if x is not None else None, fp, int(sort_field), int(bool(descending)), int(bool(nulls_first)), int(k),
-        _ptr(hits), _ptr(n_out)), reader.segments[0].ctx._h)
+        _seg_array(reader.segments), len(reader.segments), *_query_args(queries, exclude, min_match, groups=True),
+        _ref(filt), int(sort_field), int(bool(descending)), int(bool(nulls_first)), int(k), _ptr(hits), _ptr(n_out)),
+        reader.segments[0].ctx._h)
     return _sort_result(hits, n_out, nq, k, vt)
 
 
 def ExecuteTopKByColumnGroups(reader, groups, sort_field, k, descending=False, nulls_first=False, filt=None, exclude=None,
                               min_match=None):
     """ExecuteTopKByColumnGroupsBatch for one query (a list of OR groups): dict of docs, segs, values, nulls."""
-    r = ExecuteTopKByColumnGroupsBatch(reader, [[list(g) for g in groups]], sort_field, k, descending, nulls_first, filt,
-                                       exclude=None if exclude is None else [list(exclude)],
-                                       min_match=None if min_match is None else [list(min_match)])
-    return dict(docs=r["docs"][0], segs=r["segs"][0], values=r["values"][0], nulls=r["nulls"][0])
+    return _sort_row(ExecuteTopKByColumnGroupsBatch(reader, _one_groups(groups), sort_field, k, descending, nulls_first, filt,
+                                                    exclude=_one(exclude), min_match=_one(min_match)))
 
 
 def ExecuteFacetCountsGroupsBatch(reader, queries, key_field, key_min=None, key_span=None, filt=None, exclude=None,
@@ -740,32 +727,19 @@ def ExecuteFacetCountsGroupsBatch(reader, queries, key_field, key_min=None, key_
     ExecuteFacetCountsBatch. Returns the dict ExecuteFacetCountsBatch returns."""
     key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
     nq = len(queries)
-    ids, group_off, query_group_off = _groups(queries)
-    gmin = _group_min(min_match, queries)
-    flat = np.ascontiguousarray(ids, dtype=np.uint32)
     counts = np.zeros((max(nq, 1), max(int(key_span), 1)), np.uint64)
     nulls = np.zeros(max(nq, 1), np.uint64)
-    x = _exclusions(exclude, nq)
-    fp = C.byref(filt) if filt is not None else None
     N.check(N.lib().sdbg_match_facet_counts_batch_groups_min(
-        _seg_array(reader.segments), len(reader.segments), _ptr(flat) if len(flat) else None, _ptr(group_off),
-        _ptr(query_group_off), _ptr(gmin) if gmin is not None else None, nq, _ptr(x[0]) if x is not None else None,
-        _ptr(x[1]) if x is not None else None, fp, int(key_field), int(key_min), int(key_span), _ptr(counts), _ptr(nulls)),
-        reader.segments[0].ctx._h)
+        _seg_array(reader.segments), len(reader.segments), *_query_args(queries, exclude, min_match, groups=True),
+        _ref(filt), int(key_field), int(key_min), int(key_span), _ptr(counts), _ptr(nulls)), reader.segments[0].ctx._h)
     return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
 
 
 def ExecuteFacetCountsGroups(reader, groups, key_field, key_min=None, key_span=None, filt=None, exclude=None,
                              min_match=None):
     """ExecuteFacetCountsGroupsBatch for one query: {key: count} plus {None: n} for NULL keys, as ExecuteFacetCounts."""
-    r = ExecuteFacetCountsGroupsBatch(reader, [[list(g) for g in groups]], key_field, key_min, key_span, filt,
-                                      exclude=None if exclude is None else [list(exclude)],
-                                      min_match=None if min_match is None else [list(min_match)])
-    row = r["counts"][0]
-    out = {r["key_min"] + int(i): int(row[i]) for i in np.nonzero(row)[0]}
-    if r["nulls"][0]:
-        out[None] = int(r["nulls"][0])
-    return out
+    return _facet_row(ExecuteFacetCountsGroupsBatch(reader, _one_groups(groups), key_field, key_min, key_span, filt,
+                                                    exclude=_one(exclude), min_match=_one(min_match)))
 
 
 FOR_BLOCK_DTYPE =np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])
@@ -901,8 +875,7 @@ def merge_gathered(ctx, d_keys_all_ptr, n_ranks, nq, k, to_host=True):
 def ExecuteTopK(reader, query_terms, kind, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
     """irs::ExecuteTopK for one query: hits sorted by (score desc, seg asc, doc asc), total matches. exclude: term ids whose
     docs are left out (`a & b & !c`)."""
-    hits, n_out, total = ExecuteTopKBatch(reader, [list(query_terms)], kind, scorer, k, filt, threshold,
-                                          exclude=None if exclude is None else [list(exclude)])
+    hits, n_out, total = ExecuteTopKBatch(reader, _one(query_terms), kind, scorer, k, filt, threshold, exclude=_one(exclude))
     return hits[0, :n_out[0]].copy(), int(total[0])
 
 

@@ -265,6 +265,10 @@ def test_errors(synth):
         assert _raw(reader, fn, ids, u(0, 1, 1, 3), u(0, 3), u(1, 1, 1), 1) == -1          # empty group, as before
         assert _raw(reader, fn, u(0, 1, 0), u(0, 3), u(0, 1), u(2), 1) == -1               # a term twice in a query
         assert _raw(reader, fn, np.arange(17, dtype=np.uint32), u(0, 17), u(0, 1), u(2), 1) == -7   # 17 positive terms
+        # a mixed batch whose shape-2 query has an out-of-range term: the valid shape-0 query is not run either
+        before = ctx().launches
+        assert _raw(reader, fn, u(0, 1, 2, 3, 10_000), u(0, 2, 3, 5), u(0, 1, 3), u(1, 1, 1), 2) == -1
+        assert ctx().launches == before, fn
     with pytest.raises(N.SdbgError, match="EINVAL"):
         sdb.ExecuteTopKGroups(reader, [[0, 1, 2]], sdb.BM25(), 10, min_match=[4])
     with pytest.raises(N.SdbgError, match="EINVAL"):
