@@ -354,7 +354,12 @@ int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int ki
                                 float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in,
                                 uint32_t rank, void* d_keys /* n_queries*k u64 */,
                                 void* d_totals /* n_queries u64 */);
-/* out may be NULL: the merged keys then stay in HBM (device-resident pipelines / timing). */
+/* sdbg_bm25_topk_batch_device: rank < 15 and fewer than 2^28 docs over the rank's segments (each rank owns 2^28
+ * ordinals of the merged key space), else SDBG_EUNSUPPORTED before anything is queued. Each query's k slots hold its
+ * keys sorted descending, then zeros.
+ * sdbg_topk_merge_gathered: the k best keys per query over all ranks' lists (a list's keys are its non-zero prefix).
+ * k <= 8192 and n_queries <= 65535 as for the top-k entries, else SDBG_EUNSUPPORTED; a zero count: SDBG_EINVAL.
+ * out may be NULL: the merged keys then stay in HBM (device-resident pipelines / timing). */
 int sdbg_topk_merge_gathered(sdbg_ctx*, const void* d_keys_all /* n_ranks*n_queries*k u64 */,
                              uint32_t n_ranks, size_t n_queries, uint32_t k, sdbg_hit* out, uint32_t* n_out);
 /* Test probe: decode+score one whole posting list (exhaustive, no top-k). Buffers sized docs_count. */
@@ -444,8 +449,14 @@ int sdbg_dist_destroy(sdbg_ctx*);
 int sdbg_dist_allreduce_i64(sdbg_ctx*, void* d_buf, size_t n);                          /* in place, SUM */
 int sdbg_dist_allgather(sdbg_ctx*, const void* d_send, void* d_recv, size_t bytes_per_rank);
 /* Dense GROUP BY partials (sdbg_filter_groupby_partial) of every rank -> global partials on every rank with ONE
-   ncclAllReduce: counts, SUM(int) limbs and SUM(double) as 120-bit fixed point share one int64 buffer (exact and
-   independent of the rank order). abs_bound >= |SUM(double column)| over all ranks, identical on every rank. */
+   ncclAllReduce: counts, SUM(int) limbs (exact) and SUM(double) as 120-bit fixed point share one int64 buffer
+   (independent of the rank order). abs_bound: finite, identical on every rank, and at least every rank's |partial
+   SUM(double)| of every key -- not only the |total|: partials of opposite sign can be far larger than their sum.
+   Σ|w| over all passing rows of all ranks is a safe choice. With abs_bound < 2^e, each partial is truncated toward zero
+   to a multiple of 2^(e - 116) before the sum (a zero comes back as +0.0). NaN and +-inf partials are carried as counts:
+   the merged value is NaN if any partial is NaN or both infinities occur, else the infinity that occurs. A finite partial
+   above abs_bound on any rank makes the next sdbg_groupby_finalize / sdbg_sync return SDBG_EINVAL on every rank.
+   A non-finite or negative abs_bound: SDBG_EINVAL. */
 int sdbg_dist_groupby_merge(sdbg_ctx*, void* d_i64, void* d_f64, uint64_t span, double abs_bound);
 /* BM25 top-k over the segments of ALL ranks: local scan -> one all-gather of the k best keys per query -> local
    selection, back to back on the context's stream. hit.seg = rank, hit.doc = ordinal within the rank. out == NULL:

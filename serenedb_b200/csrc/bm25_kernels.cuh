@@ -1032,7 +1032,7 @@ bm25_topk_kernel(const TopkParams P) {
 // ------------------------------------------------------------------------------------------
 struct MergeParams {
   const unsigned long long* cand;  // [lists][stride]; query q owns lists [list_off[q], list_off[q+1]), or [q*G, (q+1)*G) when list_off is null
-  const uint32_t* cand_n;          // [lists] (null => every list holds `stride` entries, zeros = empty)
+  const uint32_t* cand_n;          // [lists] (null => every list holds `stride` slots: its keys, then zeros)
   const uint32_t* list_off;        // [Q+1] or null
   uint32_t G, stride, k, cap;      // cap = power of two > k, multiple of the CTA size
   unsigned long long* keys_out;    // [Q][k]
@@ -1061,7 +1061,19 @@ topk_merge_kernel(const MergeParams P) {
   }
   for (uint32_t g = l_begin; g < l_end; ++g) {
     const unsigned long long* src = P.cand + size_t(g) * P.stride;
-    const uint32_t n = P.cand_n ? min(P.cand_n[g], P.stride) : P.stride;
+    uint32_t n;
+    if (P.cand_n) {
+      n = min(P.cand_n[g], P.stride);
+    } else {
+      // zero-padded list: only its non-zero prefix counts (sorted descending, so the zeros are the tail). A zero taken
+      // into the buffer would count as a key and could stop the select below from compacting.
+      uint32_t lo = 0, hi = P.stride;
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (src[mid] != 0ull) lo = mid + 1; else hi = mid;
+      }
+      n = lo;
+    }
     uint32_t base = 0;
     while (base < n) {
       const uint32_t have = s_n;

@@ -84,13 +84,16 @@ struct sdbg_ctx {
   cudaEvent_t ev_copy[16] = {};   // one per host conversion thread (sdbg_bm25_topk_batch)
   bool topk_attr_set = false;   // topk_smem_attrs has run
   void* nccl_comm = nullptr;   // ncclComm_t once sdbg_dist_init ran
-  unsigned long long* h_oor = nullptr;   // pinned: out-of-range key count of the last deferred GROUP BY partial
+  // pinned [2]: out-of-range key count of the last deferred GROUP BY partial, and the number of SUM(double) partials
+  // beyond abs_bound of the last sdbg_dist_groupby_merge (over all ranks)
+  unsigned long long* h_oor = nullptr;
   void* h_result = nullptr;     // mapped pinned memory the point-query kernels write their result into (no D2H copy)
   void* d_result = nullptr;     // its device address
   unsigned long long result_seq = 0;   // completion word value of the last point query
   size_t h_result_cap = 0;
   bool counter_zeroed = false;  // scratch[10] starts at zero; every kernel that uses it leaves it at zero
   bool oor_pending = false;
+  bool fix_over_pending = false;
   uint64_t zone_blocks_total = 0;   // last GROUP BY scan: 2048-row blocks seen / proven dead by their zonemaps
   unsigned long long* d_zone_skipped = nullptr;
   int dist_rank = 0, dist_world = 1;
@@ -196,6 +199,15 @@ int env_int(const char* name, int dflt) {
   return s && *s ? std::atoi(s) : dflt;
 }
 
+// The GROUP BY errors found on the device after an asynchronous call returned (h_oor); the stream has been synchronised.
+int deferred_groupby_errors(sdbg_ctx* c) {
+  const bool oor = c->oor_pending && c->h_oor[0], over = c->fix_over_pending && c->h_oor[1];
+  c->oor_pending = c->fix_over_pending = false;
+  if (oor) return fail(c, SDBG_EINVAL, "GROUP BY key outside [key_min, key_min + span)");
+  if (over) return fail(c, SDBG_EINVAL, "a SUM(double) partial exceeds the abs_bound of sdbg_dist_groupby_merge");
+  return SDBG_OK;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------
@@ -258,11 +270,7 @@ extern "C" int sdbg_timer_stop(sdbg_ctx* c, float* ms) {
 }
 extern "C" int sdbg_sync(sdbg_ctx* c) {
   CU(c, cudaStreamSynchronize(c->stream));
-  if (c->oor_pending) {
-    c->oor_pending = false;
-    if (*c->h_oor) return fail(c, SDBG_EINVAL, "GROUP BY key outside [key_min, key_min + span)");
-  }
-  return SDBG_OK;
+  return deferred_groupby_errors(c);
 }
 extern "C" uint64_t sdbg_launch_count(const sdbg_ctx* c) { return c ? c->launches : 0; }
 extern "C" int sdbg_flush_l2(sdbg_ctx* c) {
@@ -2525,15 +2533,18 @@ namespace {
 int topk_batch_device_impl(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
                            size_t nq, float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, uint32_t rank,
                            void* d_keys, void* d_totals, bool sync) {
-  if (!d_keys) return SDBG_EINVAL;
+  if (!d_keys || !segs || !n_segs) return SDBG_EINVAL;
+  for (size_t si = 0; si < n_segs; ++si) if (!segs[si]) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  // Each rank owns a 2^28-ordinal slot in the merged key space: rank r's docs sort after rank r-1's on ties. Checked
+  // before the scan is queued, so a rejected call does no work.
+  uint64_t docs = 0;
+  for (size_t si = 0; si < n_segs; ++si) docs += segs[si]->n_docs;
+  if (rank >= 15) return fail(c, SDBG_EUNSUPPORTED, "rank slot overflow (rank >= 15)");
+  if (docs >= (1ull << 28)) return fail(c, SDBG_EUNSUPPORTED, "rank slot overflow (>= 2^28 docs per rank)");
   TopkDevOut dev{};
   int rc = topk_run(segs, n_segs, {kind, terms, term_off, nq, nullptr, nullptr, nullptr}, k1, b, filt, k, threshold_in, &dev);
   if (rc) return rc;
-  sdbg_ctx* c = segs[0]->ctx;
-  // Each rank owns a 2^28-ordinal slot in the merged key space: rank r's docs sort after rank r-1's on ties.
-  uint64_t docs = 0;
-  for (size_t si = 0; si < n_segs; ++si) docs += segs[si]->n_docs;
-  if (docs >= (1ull << 28) || rank >= 15) return fail(c, SDBG_EUNSUPPORTED, "rank slot overflow (>= 2^28 docs per rank)");
   shift_keys_kernel<<<256, 256, 0, c->stream>>>(dev.keys, static_cast<unsigned long long*>(d_keys), nq * size_t(k), rank << 28);
   ++c->launches;
   CU(c, cudaGetLastError());
@@ -2546,6 +2557,7 @@ int topk_batch_device_impl(sdbg_segment* const* segs, size_t n_segs, int kind, c
 extern "C" int sdbg_topk_merge_gathered(sdbg_ctx* c, const void* d_keys_all, uint32_t n_ranks, size_t nq, uint32_t k,
                                         sdbg_hit* out, uint32_t* n_out) {
   if (!c || !d_keys_all || !n_ranks || !nq || !k || (out && !n_out)) return SDBG_EINVAL;   // out == NULL: n_out != NULL asks for a sync
+  if (int rc = topk_limits(c, nq, k)) return rc;   // the keys come from top-k entries, which produce no larger lists
   CU(c, cudaSetDevice(c->device));
   // gathered layout [rank][query][k]; the merge kernel wants [query][list][stride] -> stride trick:
   // treat each rank's block as a list with a rank-major base pointer. Re-pack with a tiny kernel-free
@@ -3137,7 +3149,7 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
   if (defer_check) {
     // the partial path stays asynchronous (a collective usually follows on the same stream): the out-of-range count
     // lands in pinned memory and is looked at by the next call that synchronises (finalize / sdbg_sync)
-    if (!c->h_oor) CU(c, cudaHostAlloc(reinterpret_cast<void**>(&c->h_oor), 8, cudaHostAllocDefault));
+    if (!c->h_oor) CU(c, cudaHostAlloc(reinterpret_cast<void**>(&c->h_oor), 16, cudaHostAllocDefault));
     CU(c, cudaMemcpyAsync(c->h_oor, oor, 8, cudaMemcpyDeviceToHost, c->stream));
     c->oor_pending = true;
   } else {
@@ -3253,10 +3265,7 @@ extern "C" int sdbg_groupby_finalize(sdbg_ctx* c, int64_t key_min, uint64_t span
   CU(c, cudaMemcpyAsync(h_i, d_i64, span * 32, cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaMemcpyAsync(h_f, d_f64, span * 8, cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
-  if (c->oor_pending) {
-    c->oor_pending = false;
-    if (*c->h_oor) return fail(c, SDBG_EINVAL, "GROUP BY key outside [key_min, key_min + span)");
-  }
+  if ((rc = deferred_groupby_errors(c))) return rc;
   uint64_t n = 0;
   for (uint64_t i = 0; i < span; ++i) {
     if (h_i[i] == 0) continue;
@@ -3351,12 +3360,17 @@ NcclApi& nccl_api() {
     if (r_ != ncclSuccess) return fail((c), SDBG_ECUDA, std::string("NCCL: ") + nccl_api().GetErrorString(r_)); \
   } while (0)
 
-// SUM(double) partials as fixed point: x / 2^eunit rounded to a 120-bit integer, two signed 60-bit limbs in int64 --
+// SUM(double) partials as fixed point: x / 2^eunit truncated to a 120-bit integer, two signed 60-bit limbs in int64 --
 // sums of up to 8 ranks cannot overflow a limb, the integer all-reduce is exact and independent of the rank order,
-// and the only rounding left is the final conversion back to double.
+// and the only roundings left are the truncation below 2^eunit and the final conversion back to double.
+// A NaN or infinite partial has no fixed-point form: it adds one to its key's count of NaN, +inf or -inf partials
+// (one 16-bit field each of one more word per key, summed by the same all-reduce) and the unpack rebuilds the IEEE sum
+// from the counts. A finite partial beyond abs_bound adds one to the last word of the wire instead; the next
+// synchronising call reports it.
+constexpr long long kWireNan = 1ll, kWirePosInf = 1ll << 16, kWireNegInf = 1ll << 32;
 __global__ void __launch_bounds__(256)
 dist_pack_kernel(const long long* __restrict__ part_i64, const double* __restrict__ part_f64, uint64_t span, int eunit,
-                 long long* __restrict__ wire /* [6 * span] */) {
+                 double abs_bound, long long* __restrict__ wire /* [7 * span + 1], the last word zeroed */) {
   for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < span; i += uint64_t(gridDim.x) * blockDim.x) {
     wire[i] = part_i64[i];
     // SUM(int) limbs normalised so that lo is in [0, 2^32): the all-reduce of up to 2^31 ranks' lo limbs cannot wrap
@@ -3365,10 +3379,15 @@ dist_pack_kernel(const long long* __restrict__ part_i64, const double* __restric
     wire[span + i] = lo - (carry << 32);
     wire[2 * span + i] = hi + carry;
     wire[3 * span + i] = part_i64[3 * span + i];
-    long long l0, l1;
-    fix_limbs(part_f64[i], 60, eunit, l0, l1);
+    const double w = part_f64[i];
+    long long l0 = 0, l1 = 0, special = 0;
+    if (isnan(w)) special = kWireNan;
+    else if (isinf(w)) special = w > 0.0 ? kWirePosInf : kWireNegInf;
+    else if (fabs(w) <= abs_bound) fix_limbs(w, 60, eunit, l0, l1);
+    else atomicAdd(reinterpret_cast<unsigned long long*>(wire + 7 * span), 1ull);
     wire[4 * span + i] = l0;
     wire[5 * span + i] = l1;
+    wire[6 * span + i] = special;
   }
 }
 __global__ void __launch_bounds__(256)
@@ -3379,7 +3398,13 @@ dist_unpack_kernel(const long long* __restrict__ wire, uint64_t span, int eunit,
     part_i64[span + i] = wire[span + i];
     part_i64[2 * span + i] = wire[2 * span + i];
     part_i64[3 * span + i] = wire[3 * span + i];
-    part_f64[i] = fix_total(wire[4 * span + i], wire[5 * span + i], 60, eunit);
+    // IEEE sum semantics: NaN if any partial is NaN or both infinities occur, else the infinity that occurs
+    const long long special = wire[6 * span + i];
+    const bool nan = (special & 0xFFFF) != 0, pinf = ((special >> 16) & 0xFFFF) != 0, ninf = ((special >> 32) & 0xFFFF) != 0;
+    part_f64[i] = nan || (pinf && ninf) ? __longlong_as_double(0x7FF8000000000000ll)
+                : pinf                  ? __longlong_as_double(0x7FF0000000000000ll)
+                : ninf                  ? __longlong_as_double(static_cast<long long>(0xFFF0000000000000ull))
+                                        : fix_total(wire[4 * span + i], wire[5 * span + i], 60, eunit);
   }
 }
 }  // namespace
@@ -3432,9 +3457,9 @@ extern "C" int sdbg_dist_allgather(sdbg_ctx* c, const void* d_send, void* d_recv
 }
 
 // Dense GROUP BY partials of every rank -> the global partials on every rank, in ONE all-reduce: counts, the SUM(int)
-// limbs and SUM(double) as fixed-point limbs travel in one int64 buffer. abs_bound >= |sum of the double column over
-// all ranks' passing rows| fixes the fixed-point unit (identical on every rank: derive it from the column statistics
-// and the total row count, which are known when the shards are built).
+// limbs and SUM(double) as fixed-point limbs travel in one int64 buffer. abs_bound >= every rank's |partial| fixes the
+// fixed-point unit (identical on every rank: derive it from the column statistics and the total row count, which are
+// known when the shards are built; the sum of |w| over all passing rows bounds every partial).
 // Distributed top-k in one call: local scan of this rank's segments, ONE all-gather of every rank's k best keys per query
 // over NVLink, local selection of the global top-k -- enqueued back to back on the context's stream, one host
 // synchronisation at the very end (none when out == NULL: the keys stay in HBM, see sdbg_topk_merge_gathered).
@@ -3458,7 +3483,7 @@ extern "C" int sdbg_dist_bm25_topk_batch(sdbg_segment* const* segs, size_t n_seg
 }
 
 extern "C" int sdbg_dist_groupby_merge(sdbg_ctx* c, void* d_i64, void* d_f64, uint64_t span, double abs_bound) {
-  if (!c || !d_i64 || !d_f64 || !span || !(abs_bound >= 0.0)) return SDBG_EINVAL;
+  if (!c || !d_i64 || !d_f64 || !span || !(abs_bound >= 0.0) || std::isinf(abs_bound)) return SDBG_EINVAL;
   if (!c->nccl_comm) return c->dist_world == 1 ? SDBG_OK : fail(c, SDBG_EINVAL, "sdbg_dist_init has not run");
   if (c->dist_world > 8) return fail(c, SDBG_EUNSUPPORTED, "fixed-point limbs are sized for up to 8 ranks");
   CU(c, cudaSetDevice(c->device));
@@ -3467,16 +3492,22 @@ extern "C" int sdbg_dist_groupby_merge(sdbg_ctx* c, void* d_i64, void* d_f64, ui
   const int eunit = ex + 1 - 117;                              // 120-bit fixed point with 3 bits of headroom for 8 ranks
   DevBuf& wire = c->scratch[14];
   int rc;
-  if ((rc = ensure(c, wire, span * 6 * sizeof(long long)))) return rc;
+  if ((rc = ensure(c, wire, (span * 7 + 1) * sizeof(long long)))) return rc;
+  if (!c->h_oor) CU(c, cudaHostAlloc(reinterpret_cast<void**>(&c->h_oor), 16, cudaHostAllocDefault));
+  long long* over = static_cast<long long*>(wire.p) + span * 7;
+  CU(c, cudaMemsetAsync(over, 0, sizeof(long long), c->stream));
   const unsigned grid = unsigned(std::min<uint64_t>((span + 255) / 256, uint64_t(c->sm_count) * 8));
   dist_pack_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const long long*>(d_i64), static_cast<const double*>(d_f64), span, eunit,
-                                               static_cast<long long*>(wire.p));
+                                               abs_bound, static_cast<long long*>(wire.p));
   ++c->launches;
-  NC(c, nccl_api().AllReduce(wire.p, wire.p, span * 6, ncclInt64, ncclSum, static_cast<ncclComm_t>(c->nccl_comm), c->stream));
+  // the overflow word travels with the partials, so every rank sees a bound broken on any rank
+  NC(c, nccl_api().AllReduce(wire.p, wire.p, span * 7 + 1, ncclInt64, ncclSum, static_cast<ncclComm_t>(c->nccl_comm), c->stream));
   dist_unpack_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const long long*>(wire.p), span, eunit, static_cast<long long*>(d_i64),
                                                  static_cast<double*>(d_f64));
   ++c->launches;
   CU(c, cudaGetLastError());
+  CU(c, cudaMemcpyAsync(c->h_oor + 1, over, 8, cudaMemcpyDeviceToHost, c->stream));
+  c->fix_over_pending = true;
   return SDBG_OK;
 }
 
