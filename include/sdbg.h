@@ -86,6 +86,9 @@ typedef struct {
   uint64_t e_skip_start; /* e_single_doc when docs_count == 1 (same union as reader.hpp:213-217) */
 } sdbg_term_meta;
 
+/* Doc ids are 1 .. 2^32 - 2: doc_limits::eof() = 2^32 - 1 is never a doc. docs_count > 2^32 - 2: SDBG_EINVAL.
+ * The top-k and sorted entries take at most 2^32 - 2 docs summed over a call's segments (more:
+ * SDBG_EUNSUPPORTED, nothing queued); the count and facet entries have no per-call limit. */
 int sdbg_segment_create(sdbg_ctx*, uint32_t docs_count, sdbg_segment** out);
 void sdbg_segment_destroy(sdbg_segment*);
 /* doc_file: the ".doc" stream (posting blocks + skip data, format "1_5simd"); has_wand != 0 when
@@ -414,7 +417,8 @@ int sdbg_groupby_finalize(sdbg_ctx*, int64_t key_min, uint64_t key_span, const v
 int sdbg_column_minmax_i64(sdbg_segment*, uint64_t field, int64_t* mn, int64_t* mx);
 
 /* ---- host-side writer mirror + deterministic synthetic inputs (index-build side; not timed) ---- */
-/* PostingsWriter mirror (irs/formats/posting/writer.hpp): builds a ".doc" stream on the host. */
+/* PostingsWriter mirror (irs/formats/posting/writer.hpp): builds a ".doc" stream on the host. segment_docs > 2^32 - 2:
+ * SDBG_EINVAL. */
 typedef struct sdbg_writer sdbg_writer;
 int sdbg_writer_create(uint32_t segment_docs, int has_wand, float wand_b, const uint32_t* norms /* per doc, may be NULL */,
                        sdbg_writer** out);

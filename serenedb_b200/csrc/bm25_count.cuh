@@ -173,7 +173,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   const uint32_t gend0 = kGroups ? P.grp_end[P.grp_off[q]] : 0u;
   const uint32_t n_lead = kGroups ? (gend0 & 0xFFu) - (gend0 >> 8) : kAnd ? 1u : n_pos;
   const uint4* const B = P.seg.blocks;
-  const uint32_t del_words = (P.seg.n_docs + 32u) / 32u + 1u;
+  const uint32_t del_words = (P.seg.n_docs >> 5) + 2u;   // (n_docs + 32) / 32 + 1, the host bitmap's words, without wrapping
 
   if (tid < n_lists) {
     const uint2 l = tid < n_pos ? P.lists[P.term_off[q] + tid] : P.lists[P.n_pos + P.excl_off[q] + (tid - n_pos)];

@@ -348,6 +348,9 @@ struct TopkParams {
 };
 
 constexpr uint32_t kPadDoc = 0xFFFFFFFFu;
+// Doc ids are 1 .. 2^32 - 2 (doc_limits::eof() = 2^32 - 1 is never a doc): the largest segment, and the most docs one
+// top-k or sorted call takes summed over its segments (ordinal_base + doc stays a valid id).
+constexpr uint32_t kMaxDocId = 0xFFFFFFFEu;
 
 // First index in sorted a[0..n) with a[i] >= d (n > 0 is a multiple of 128).
 __device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* a, uint32_t n, uint32_t d) {

@@ -108,10 +108,11 @@ bm25_merge_kernel(const TopkParams P) {
   const uint32_t chain_lo = chain_empty ? 1u : uint32_t(first64);
   const uint32_t chain_hi = chain_empty ? 0u : uint32_t(min(static_cast<unsigned long long>(P.seg.n_docs), first64 + chunk - 1ull));
   const uint32_t clen = chain_empty ? 0u : chain_hi - chain_lo + 1u;
-  const uint32_t sub = (clen + kTopkWarps - 1u) / kTopkWarps;
+  const uint32_t sub = uint32_t((clen + (kTopkWarps - 1ull)) / kTopkWarps);   // 64-bit: clen reaches 2^32 - 2
   const bool warp_empty = clen == 0u || warp * sub >= clen;
   const uint32_t lo_w = warp_empty ? 1u : chain_lo + warp * sub;
-  const uint32_t hi_w = warp_empty ? 0u : min(chain_hi, lo_w + sub - 1u);
+  // 64-bit: the last warp's sub-range may end past 2^32 - 1 before it is cut to the chain
+  const uint32_t hi_w = warp_empty ? 0u : uint32_t(min(static_cast<unsigned long long>(chain_hi), lo_w + (sub - 1ull)));
 
   for (uint32_t i = tid; i < P.cap; i += blockDim.x) cand[i] = 0ull;
   if (tid < T) s_qt[tid] = P.qterms[t0 + tid];

@@ -314,6 +314,7 @@ extern "C" int sdbg_profile_read(sdbg_ctx* c, int kernel_id, double* total_ms, u
 // ------------------------------------------------------------------------------------------
 extern "C" int sdbg_segment_create(sdbg_ctx* c, uint32_t docs_count, sdbg_segment** out) {
   if (!c || !out) return SDBG_EINVAL;
+  if (docs_count > kMaxDocId) return fail(c, SDBG_EINVAL, "docs_count > 2^32-2 (2^32-1 is doc_limits::eof)");
   auto* s = new sdbg_segment;
   s->ctx = c; s->n_docs = docs_count;
   *out = s;
@@ -1135,7 +1136,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm2
     ord += segs[si]->n_docs;
     max_docs = std::max(max_docs, segs[si]->n_docs);
   }
-  if (ord >= 0xFFFFFFFFull) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-1 docs per GPU");
+  if (ord > kMaxDocId) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-2 docs per call");
   // Per-doc check lists of each query: its excluded terms (tag kCheckExcl), then, for a query of OR groups, each positive
   // term tagged with its group. chk_off[q] .. chk_off[q + 1] index chk_terms / chk_grp.
   std::vector<uint32_t> chk_off, chk_terms;
@@ -1259,7 +1260,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm2
       if (slice_docs) g = std::max(g, std::min(16u, std::max(1u, smallest / 8192u)));
       g = std::min(g, max_chains);
       g = std::min(g, std::max(1u, rest_docs / 4096u));
-      const uint32_t chunk = (rest_docs + g - 1) / g;
+      const uint32_t chunk = uint32_t((uint64_t(rest_docs) + g - 1) / g);   // 64-bit: rest_docs reaches 2^32 - 2
       for (uint32_t j = 0; j < g; ++j)
         seg_work[si].push_back({uint32_t(q), first + j * chunk, chunk, list_off[q] + lists + j, rest_postings / g, cls});
       n_cls[si][cls] += g;
@@ -1827,7 +1828,8 @@ int sort_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, SortJob&
       return fail(c, SDBG_EINVAL, "sort column type differs between segments");
     total_docs += segs[si]->n_docs;
   }
-  if (total_docs + 1 >= 0xFFFFFFFFull) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-2 docs per call");
+  // ordinals reach total_docs - 1 <= 2^32 - 3, so ~ordinal (the key's lo) stays non-zero
+  if (total_docs > kMaxDocId) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-2 docs per call");
   uint32_t base = 0;   // ordinals of the earlier segments (the total fits in 32 bits)
   for (size_t si = 0; si < n_segs; ++si) {
     ColumnObj& col = segs[si]->cols.find(J.field)->second;
@@ -2394,7 +2396,7 @@ int scan_run(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_te
   const uint32_t T = uint32_t(n_terms);
   const uint32_t scan_cap = 1024;                                    // candidate buffer of the kernel: unused here, kept minimal
   const uint32_t g = std::max(1u, std::min(uint32_t(c->sm_count) * 3u, range / 4096u));
-  const uint32_t chunk = (range + g - 1) / g;
+  const uint32_t chunk = uint32_t((uint64_t(range) + g - 1) / g);   // 64-bit: range reaches 2^32 - 2
   // descriptors: [QTermDev x T][term_off x 2][pad][work x g][excluded lists x n_excl][excl_off x 2]
   const size_t qt_bytes = size_t(T) * sizeof(QTermDev), off_bytes = 2 * sizeof(uint32_t);
   const size_t qt_pad = (qt_bytes + off_bytes + 15) & ~size_t(15), work_bytes = size_t(g) * sizeof(uint4);
@@ -3515,7 +3517,7 @@ extern "C" int sdbg_dist_groupby_merge(sdbg_ctx* c, void* d_i64, void* d_f64, ui
 // host-side writer mirror + synthetic inputs
 // ------------------------------------------------------------------------------------------
 extern "C" int sdbg_writer_create(uint32_t segment_docs, int has_wand, float wand_b, const uint32_t* norms, sdbg_writer** out) {
-  if (!out) return SDBG_EINVAL;
+  if (!out || segment_docs > kMaxDocId) return SDBG_EINVAL;
   auto* w = new sdbg_writer;
   w->w.reset(new PostingWriter(segment_docs, has_wand != 0, wand_b, norms));
   *out = w;

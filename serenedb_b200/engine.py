@@ -30,6 +30,15 @@ def _ptr(a):
 
 
 _INT64_MIN, _INT64_MAX = -(1 << 63), (1 << 63) - 1
+MAX_DOC_ID = (1 << 32) - 2   # doc ids are 1 .. 2^32 - 2; 2^32 - 1 is doc_limits::eof()
+
+
+def _check_docs_count(n):
+    """A segment's doc count as an int in 1 .. MAX_DOC_ID; ctypes would silently truncate a larger one to 32 bits."""
+    n = int(n)
+    if not 1 <= n <= MAX_DOC_ID:
+        raise ValueError(f"a segment holds 1 .. 2^32 - 2 docs, not {n}")
+    return n
 
 
 def _as_double(v):
@@ -184,6 +193,7 @@ class PostingsWriter:
 
     def __init__(self, segment_docs, norms=None, has_wand=True, wand_b=0.75):
         self._h = C.c_void_p()
+        _check_docs_count(segment_docs)
         self._norms = None if norms is None else np.ascontiguousarray(norms, dtype=np.uint32)
         N.check(N.lib().sdbg_writer_create(int(segment_docs), 1 if has_wand else 0, float(wand_b),
                                            _ptr(self._norms), C.byref(self._h)))
@@ -237,7 +247,7 @@ class Segment:
 
     def __init__(self, ctx, n_docs):
         self.ctx = ctx
-        self.n_docs = int(n_docs)
+        self.n_docs = _check_docs_count(n_docs)
         self._h = C.c_void_p()
         N.check(N.lib().sdbg_segment_create(ctx._h, self.n_docs, C.byref(self._h)), ctx._h)
         self.term_docs = None  # docs_count per term (filled by staging)
