@@ -350,6 +350,53 @@ int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n
                                              const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
                                              const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
                                              uint64_t* counts /* n_queries * key_span */, uint64_t* null_counts /* n_queries */);
+/* Aggregates over the matches (SELECT col, count(*), count(v), sum(v), avg(v), min(v), max(v) ... WHERE body @@ '...'
+ * [AND <pushed filter>] GROUP BY col, or the same without GROUP BY): per query and group, COUNT(*), COUNT(value), SUM, MIN
+ * and MAX of column `value_field` over the docs sdbg_match_count_batch (sdbg_match_count_batch_groups_min) counts for it.
+ * Deleted docs, the pushed filter, exclusions, groups and min-match apply exactly as there; identical at every pruning level.
+ * Grouping: by `key_field` exactly as the facet entries group (int64 raw or bit-packed, or int32; the key_min / key_span
+ * layout): out[q * key_span + (v - key_min)] is query q's group of key v, null_out[q] the group of the NULL key (docs past
+ * the key column's rows included). key_field == UINT64_MAX: no GROUP BY, one group out[q]; key_min must be 0 and key_span
+ * 1, and null_out[q] comes back zeroed.
+ * The value column: int64 (raw or bit-packed), int32 or float64, NOT NULL or nullable, with one type in every segment; it
+ * may be the key column or the filter's column. A doc past its rows has a NULL value.
+ * count equals the facet entry's counts[q * key_span + b] (null_out[q].count its null_counts[q]) exactly; count_value
+ * counts the non-NULL values. When count_value == 0, sum_i128, sum_f64, min and max are 0 and the caller emits SQL NULL
+ * for them; AVG is the caller's SUM / count_value, as with sdbg_group_row.
+ * Integer columns: sum_i128 is the exact two's-complement 128-bit sum ({low, high} words as in sdbg_group_row) for any
+ * values and any number of matches; min / max the int64 (int32 sign-extended). sum_f64 is 0.
+ * float64 columns: sum_f64 follows IEEE rules (NaN if any value is NaN or both infinities occur, else the infinity that
+ * occurs); the order of the finite additions is unspecified. min / max are the float64 bits of the extremes under the
+ * sorted scan's order: -0.0 equals +0.0, every NaN equals every NaN and sorts above +inf; a zero extreme comes back as
+ * +0.0 and a NaN one as 0x7FF8000000000000. sum_i128 is 0.
+ * Errors, all found before anything is queued: those of the facet entries for the key column and range; NULL out or
+ * null_out, a value column whose type differs between segments, or key_field == UINT64_MAX with (key_min, key_span) !=
+ * (0, 1): SDBG_EINVAL; a segment without the value column: SDBG_ENOTFOUND; key_span > 4096 (each CTA keeps key_span + 1
+ * cells of 40 B in shared memory): SDBG_EUNSUPPORTED. Found after the scan: a matching doc whose key lies outside
+ * [key_min, key_min + key_span): SDBG_EINVAL, and the outputs are unspecified. Synchronous on the context's stream.
+ * Device scratch: (n_queries * (key_span + 1)) * 48 B + n_queries * 8 B (4096 queries x 2001 keys: 394 MB), and as
+ * much pinned host memory for the copy back. Split larger batches.
+ * Not supported: several value columns in one call (call once per column), key spans above 4096, float64 keys, HAVING,
+ * COUNT(DISTINCT), a multi-GPU merge of the cells, the top-k and streaming entries. */
+typedef struct {
+  uint64_t count;         /* COUNT(*) of the group's matches */
+  uint64_t count_value;   /* COUNT(value): those whose value is not NULL */
+  int64_t sum_i128[2];    /* integer value column: SUM(value), exact; {low, high} words as in sdbg_group_row */
+  double sum_f64;         /* float64 value column: SUM(value) */
+  int64_t min, max;       /* MIN / MAX(value): the integer (int32 sign-extended), or the float64's bits */
+} sdbg_match_agg;
+int sdbg_match_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
+                               const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms,
+                               const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt, uint64_t key_field,
+                               int64_t key_min, uint32_t key_span, uint64_t value_field,
+                               sdbg_match_agg* out /* n_queries * key_span */, sdbg_match_agg* null_out /* n_queries */);
+int sdbg_match_aggregate_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                          const uint32_t* group_off, const uint32_t* query_group_off,
+                                          const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                          const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                          const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                          uint64_t value_field, sdbg_match_agg* out /* n_queries * key_span */,
+                                          sdbg_match_agg* null_out /* n_queries */);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

@@ -8,7 +8,8 @@ import raises -- there is no Python or CPU fallback for any operation.
 from . import _native
 from .engine import (AND, OR, BM25, TFIDF, FLT_MIN, Context, ExecuteCount, ExecuteCountBatch, ExecuteCountGroups,
                      ExecuteCountGroupsBatch, ExecuteFacetCounts, ExecuteFacetCountsBatch, ExecuteFacetCountsGroups,
-                     ExecuteFacetCountsGroupsBatch, ExecuteTopK, ExecuteTopKBatch, ExecuteTopKByColumn, ExecuteTopKByColumnBatch,
+                     ExecuteFacetCountsGroupsBatch, ExecuteMatchAggregates, ExecuteMatchAggregatesBatch,
+                     ExecuteMatchAggregatesGroups, ExecuteMatchAggregatesGroupsBatch, ExecuteTopK, ExecuteTopKBatch, ExecuteTopKByColumn, ExecuteTopKByColumnBatch,
                      ExecuteTopKByColumnGroups, ExecuteTopKByColumnGroupsBatch, ExecuteTopKGroups, ExecuteTopKGroupsBatch, IndexReader, IResearchScan, PostingsWriter, PreparedBatch, Segment, merge_gathered, pred,
                      resolve_pred, stage_parse_host, sum_i128, StreamScoredDocs, pack_for)
 
@@ -16,6 +17,7 @@ _native.lib()  # fail loudly at import time when the CUDA extension is missing
 
 __all__ = ["AND", "OR", "BM25", "TFIDF", "FLT_MIN", "Context", "ExecuteCount", "ExecuteCountBatch", "ExecuteCountGroups",
            "ExecuteCountGroupsBatch", "ExecuteFacetCounts", "ExecuteFacetCountsBatch", "ExecuteFacetCountsGroups",
-           "ExecuteFacetCountsGroupsBatch", "ExecuteTopK", "ExecuteTopKBatch", "ExecuteTopKByColumn", "ExecuteTopKByColumnBatch",
+           "ExecuteFacetCountsGroupsBatch", "ExecuteMatchAggregates", "ExecuteMatchAggregatesBatch",
+           "ExecuteMatchAggregatesGroups", "ExecuteMatchAggregatesGroupsBatch", "ExecuteTopK", "ExecuteTopKBatch", "ExecuteTopKByColumn", "ExecuteTopKByColumnBatch",
            "ExecuteTopKByColumnGroups", "ExecuteTopKByColumnGroupsBatch", "ExecuteTopKGroups", "ExecuteTopKGroupsBatch", "IndexReader", "IResearchScan", "PostingsWriter", "PreparedBatch", "Segment", "merge_gathered",
            "pred", "resolve_pred", "stage_parse_host", "sum_i128", "StreamScoredDocs", "pack_for"]

@@ -41,6 +41,11 @@ class GroupRow(C.Structure):
                 ("sum_f64", C.c_double), ("cnt_f64", C.c_uint64)]
 
 
+class MatchAgg(C.Structure):
+    _fields_ = [("count", C.c_uint64), ("count_value", C.c_uint64), ("sum_i128", C.c_int64 * 2), ("sum_f64", C.c_double),
+                ("min", C.c_int64), ("max", C.c_int64)]
+
+
 # every symbol include/sdbg.h declares: name -> (restype, argtypes)
 _vp, _sz = C.c_void_p, C.c_size_t
 _u32p, _u64p, _f32p = C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_float)
@@ -113,6 +118,10 @@ SIGNATURES = {
                                                              C.c_int, C.c_int, C.c_uint32, _vp, _vp]),
     "sdbg_match_facet_counts_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
                                                            C.c_int64, C.c_uint32, _vp, _vp]),
+    "sdbg_match_aggregate_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,
+                                             C.c_uint32, C.c_uint64, _vp, _vp]),
+    "sdbg_match_aggregate_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
+                                                        C.c_int64, C.c_uint32, C.c_uint64, _vp, _vp]),
     "sdbg_topk_merge_gathered": (C.c_int, [_vp, _vp, C.c_uint32, _sz, C.c_uint32, _vp, _vp]),
     "sdbg_decode_score_term": (C.c_int, [_vp, C.c_uint32, C.c_float, C.c_float, C.c_float, _vp, _vp, _vp]),
     "sdbg_col_pred_resolve": (C.c_int, [C.POINTER(ColPred), C.c_int, C.POINTER(ColPred)]),

@@ -16,13 +16,15 @@
 //        lists; it decodes each list into `tmp` the same way, adds it into a bit-sliced counter, then acc &= counter >= m.
 //   NOT  the excluded lists' blocks whose range holds a bit of `acc` are decoded and their docs cleared.
 // Then acc &= ~deleted, the filter runs per remaining bit, and popcounts are summed: one 64-bit atomicAdd per CTA.
-// The facet pass (kFacet, bm25_facet.cuh) also counts each remaining bit in its key's shared-memory bin.
+// The facet pass (kFacet, bm25_facet.cuh) also counts each remaining bit in its key's shared-memory bin; the aggregate pass
+// (kAgg, bm25_agg.cuh) also adds its value to its key's shared-memory cell.
 // A window that no positive list reaches (OR), that the shortest list does not reach (AND) or that no list of the lead
 // group reaches (GROUPS) is never touched: the CTA
 // jumps to the window of the next block's first possible doc, so a sparse query costs in proportion to its blocks.
 #pragma once
 
 #include "bm25_kernels.cuh"
+#include "bm25_agg.cuh"
 #include "bm25_facet.cuh"
 #include "bm25_sort.cuh"
 
@@ -56,6 +58,7 @@ struct CountParams {
   unsigned long long* counts;   // per query, summed over items and segments
   SortSink sort;                // kSort: the sorted scan's sink (work item .w = its output slot)
   FacetSink facet;              // kFacet: the facet pass's sink
+  AggSink agg;                  // kAgg: the aggregate pass's sink
 };
 
 __device__ __forceinline__ uint32_t warp_min(uint32_t v) {
@@ -137,12 +140,17 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
 // k best go to output slot item.w.
 // kFacet: the facet pass (bm25_facet.cuh). Besides the popcount, every surviving doc's key is counted in the item's
 // histogram of P.facet.span u32 bins in dynamic shared memory, flushed to the query's row of P.facet.counts at the end.
-// Both sinks take kGroups queries: the groups narrow `acc` before the sink reads the column, and the bit-sliced counter
-// planes follow the sink's region of dynamic shared memory (16 * cap B, or 4 * span B rounded up to 16 B).
-template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false>
+// kAgg: the aggregate pass (bm25_agg.cuh). Besides the popcount, every surviving doc's value is added to its key's cell
+// among the item's P.agg.key.span + 1 cells in dynamic shared memory (ungrouped: to the thread's register cell), flushed
+// to the query's output cells at the end.
+// The sinks take kGroups queries: the groups narrow `acc` before the sink reads the column, and the bit-sliced counter
+// planes follow the sink's region of dynamic shared memory (16 * cap B, 4 * span B or agg_cells_bytes(span), rounded up
+// to 16 B).
+template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false, bool kAgg = false>
 __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
   static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
   static_assert(!(kFacet && kSort), "the facet pass has its own sink");
+  static_assert(!(kAgg && (kSort || kFacet)), "the aggregate pass has its own sink");
   __shared__ uint32_t acc[kCountWords];
   __shared__ uint32_t tmp[kAnd || kGroups ? kCountWords : 1];
   __shared__ uint32_t stage[kCountWarps][128];
@@ -156,9 +164,11 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   __shared__ unsigned long long s_sum[kCountWarps];
   __shared__ unsigned long long s_thr[1];   // kSort: this item's best known k-th hi
   __shared__ uint32_t s_fill[1], s_zmask[2];  // kSort: keys in the buffer (kFacet: NULL keys); the window's zones that can reach s_thr
-  // kSort: hi[cap] | lo[cap]; kFacet: the u32 bins, padded to 16 B; then (kGroups) the bit-sliced counter planes
+  // kSort: hi[cap] | lo[cap]; kFacet: the u32 bins, padded to 16 B; kAgg: the cells; then (kGroups) the bit-sliced
+  // counter planes
   extern __shared__ unsigned long long sort_buf[];
   uint32_t* const bins = reinterpret_cast<uint32_t*>(sort_buf);
+  AggSmemCell* const cells = reinterpret_cast<AggSmemCell*>(sort_buf);
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint4 item = P.work[blockIdx.x];
@@ -183,7 +193,8 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
     s_next[tid] = l.y ? find_block_from(B + l.x, 0u, l.y, 0u, item.y << kCountWindowLog) : 0u;
   }
   unsigned long long count = 0;
-  bool oor = false;                                     // kFacet: this thread counted a key outside the bins
+  bool oor = false;                                     // kFacet, kAgg: this thread met a key outside the bins
+  AggSmemCell mine{};                                   // kAgg without a key column: this thread's group
   uint32_t ws = item.y << kCountWindowLog;              // start of the window being looked at
   uint32_t judged = 0, skipped = 0;                     // kSort: windows judged / skipped by the zonemap
   if constexpr (kSort) {
@@ -193,6 +204,9 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   if constexpr (kFacet) {
     for (uint32_t i = tid; i < P.facet.span; i += kCountThreads) bins[i] = 0u;
     if (tid == 0) s_fill[0] = 0u;
+  }
+  if constexpr (kAgg) {
+    for (uint32_t i = tid; i < agg_cells_bytes(P.agg.key.span) / 4u; i += kCountThreads) bins[i] = 0u;
   }
   __syncthreads();
   for (;;) {
@@ -295,7 +309,8 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
         } else {
           // at least m of the lists: each list's bitmap is added into a saturating bit-sliced counter (plane p = bit p)
           const uint32_t np = 32u - __clz(m);
-          uint32_t* const plane = bins + (kSort ? 4u * P.sort.cap : kFacet ? (P.facet.span + 3u) & ~3u : 0u);
+          uint32_t* const plane = bins + (kSort ? 4u * P.sort.cap : kFacet ? (P.facet.span + 3u) & ~3u
+                                                                  : kAgg ? agg_cells_bytes(P.agg.key.span) / 4u : 0u);
           for (uint32_t i = tid; i < np * kCountWords; i += kCountThreads) plane[i] = 0u;
           for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
           for (uint32_t li = lo; li < hi; ++li) {
@@ -341,6 +356,9 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
         }
         if constexpr (kFacet) {
           for (uint32_t r = v; r; r &= r - 1u) oor |= facet_add(P.facet, ws + 32u * i + (__ffs(r) - 1u), bins, &s_fill[0]);
+        }
+        if constexpr (kAgg) {
+          for (uint32_t r = v; r; r &= r - 1u) oor |= agg_add(P.agg, ws + 32u * i + (__ffs(r) - 1u), cells, mine);
         }
         count += __popc(v);
       }
@@ -410,6 +428,20 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       if (bins[i]) atomicAdd(out + i, static_cast<unsigned long long>(bins[i]));
     if (oor) *P.facet.out_of_range = 1u;
     if (tid == 0 && s_fill[0]) atomicAdd(P.facet.nulls + q, static_cast<unsigned long long>(s_fill[0]));
+  }
+  if constexpr (kAgg) {
+    // A work item covers docs of one segment, fewer than 2^32, so no u32 count or 64-bit limb can wrap before this flush.
+    const uint32_t span = P.agg.key.span;
+    if (!P.agg.key.values) {
+      agg_merge(&cells[0], mine, P.agg.type);
+      __syncthreads();
+    }
+    AggCell* out = P.agg.cells + size_t(q) * span;
+    for (uint32_t i = tid; i <= span; i += kCountThreads) {
+      const AggSmemCell c = cells[i];
+      if (c.n) agg_flush(i < span ? out + i : P.agg.nulls + q, c, P.agg.type);
+    }
+    if (oor) *P.agg.out_of_range = 1u;
   }
   count = warp_sum64(count);
   if (lane == 0) s_sum[warp] = count;

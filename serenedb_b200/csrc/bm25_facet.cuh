@@ -22,11 +22,14 @@ struct FacetSink {
   unsigned int* out_of_range = nullptr;          // set to 1 when a counted doc's key lies outside the bins
 };
 
-// Counts doc `doc` (row doc - 1) in its key's bin or the NULL counter. Returns true when its key lies outside the bins.
-__device__ __forceinline__ bool facet_add(const FacetSink& F, uint32_t doc, uint32_t* bins, uint32_t* nulls) {
+// Groups doc `doc` (row doc - 1) by its key: calls on_null() for a NULL key, else on_bin(bin) with bin = key - key_min
+// when the key lies in the bins. Returns true when it does not. The facet pass and the aggregate sink (bm25_agg.cuh)
+// both group through it.
+template <class OnNull, class OnBin>
+__device__ __forceinline__ bool facet_key(const FacetSink& F, uint32_t doc, OnNull on_null, OnBin on_bin) {
   const uint64_t r = uint64_t(doc) - 1ull;
   if (r >= F.rows || (F.validity && !((__ldg(F.validity + (r >> 6)) >> (r & 63ull)) & 1ull))) {
-    atomicAdd(nulls, 1u);
+    on_null();
     return false;
   }
   const long long v = F.type == 2u ? static_cast<long long>(__ldg(static_cast<const int*>(F.values) + r))
@@ -35,8 +38,13 @@ __device__ __forceinline__ bool facet_add(const FacetSink& F, uint32_t doc, uint
   // keys in range
   const unsigned long long bin = static_cast<unsigned long long>(v) - static_cast<unsigned long long>(F.key_min);
   if (bin >= F.span) return true;
-  atomicAdd(&bins[bin], 1u);
+  on_bin(static_cast<uint32_t>(bin));
   return false;
+}
+
+// Counts doc `doc` in its key's bin or the NULL counter. Returns true when its key lies outside the bins.
+__device__ __forceinline__ bool facet_add(const FacetSink& F, uint32_t doc, uint32_t* bins, uint32_t* nulls) {
+  return facet_key(F, doc, [&] { atomicAdd(nulls, 1u); }, [&](uint32_t bin) { atomicAdd(&bins[bin], 1u); });
 }
 
 }  // namespace sdbg

@@ -1759,6 +1759,7 @@ extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_s
 // shortcut; see sort_prepare / sort_finish.
 // facet (NULL: count): the facet pass of sdbg_match_facet_counts_batch on the same plan and launches, without the
 // single-term shortcut; see facet_prepare.
+// agg (NULL: count): the aggregate pass of sdbg_match_aggregate_batch, the same way; see agg_prepare.
 namespace {
 
 // The facet pass's part of a count_run call.
@@ -1771,10 +1772,11 @@ struct FacetJob {
   std::vector<FacetSink> sink;   // per segment, filled by facet_prepare (output pointers set at launch)
 };
 
-int facet_check_range(sdbg_ctx* c, int64_t key_min, uint32_t span) {
+int facet_check_range(sdbg_ctx* c, int64_t key_min, uint32_t span, uint32_t max_span = kFacetMaxSpan) {
   if (span == 0) return fail(c, SDBG_EINVAL, "key_span is 0");
   if (key_min > INT64_MAX - int64_t(span - 1)) return fail(c, SDBG_EINVAL, "key_min + key_span - 1 overflows int64");
-  if (span > kFacetMaxSpan) return fail(c, SDBG_EUNSUPPORTED, "key_span > 32768 (the bins are shared memory)");
+  if (span > max_span)
+    return fail(c, SDBG_EUNSUPPORTED, "key_span > " + std::to_string(max_span) + " (the bins are shared memory)");
   return SDBG_OK;
 }
 
@@ -1799,6 +1801,62 @@ int facet_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, FacetJo
     F.type = uint32_t(col.type); F.span = J.span; F.key_min = J.key_min;
   }
   return SDBG_OK;
+}
+
+// The aggregate pass's part of a count_run call.
+struct AggJob {
+  FacetJob key;               // key column and range (key.field UINT64_MAX: one group); its host outputs are unused
+  uint64_t field;             // value column
+  sdbg_match_agg* out;        // host: [query][span]
+  sdbg_match_agg* null_out;   // host: [query]
+  std::vector<AggSink> sink;  // per segment, filled by agg_prepare (output pointers set at launch)
+};
+
+// The key range of an aggregate call: a key column's range as for the facet pass (at most kAggMaxSpan keys); no key
+// column: exactly (0, 1).
+int agg_check_range(sdbg_ctx* c, uint64_t key_field, int64_t key_min, uint32_t span) {
+  if (key_field == UINT64_MAX)
+    return key_min == 0 && span == 1 ? SDBG_OK : fail(c, SDBG_EINVAL, "an ungrouped aggregate needs key_min 0 and key_span 1");
+  return facet_check_range(c, key_min, span, kAggMaxSpan);
+}
+
+// Checks the key range, the key column (facet_prepare) and the value column of every segment, then fills the
+// per-segment sinks. Every check runs before anything is queued.
+int agg_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, AggJob& J) {
+  if (int rc = agg_check_range(c, J.key.field, J.key.key_min, J.key.span)) return rc;
+  for (size_t si = 0; si < n_segs; ++si) {
+    auto it = segs[si]->cols.find(J.field);
+    if (it == segs[si]->cols.end()) return fail(c, SDBG_ENOTFOUND, "value column not staged in every segment");
+    if (it->second.type != segs[0]->cols.find(J.field)->second.type)
+      return fail(c, SDBG_EINVAL, "value column type differs between segments");
+  }
+  if (J.key.field != UINT64_MAX)
+    if (int rc = facet_prepare(c, segs, n_segs, J.key)) return rc;
+  J.sink.assign(n_segs, AggSink{});
+  for (size_t si = 0; si < n_segs; ++si) {
+    ColumnObj& col = segs[si]->cols.find(J.field)->second;
+    AggSink& A = J.sink[si];
+    if (J.key.field != UINT64_MAX) A.key = J.key.sink[si];
+    else A.key.span = 1;
+    void* raw = nullptr;
+    if (int rc = raw_values(c, col, &raw)) return rc;
+    A.values = raw; A.validity = reinterpret_cast<const unsigned long long*>(col.d_validity); A.rows = col.rows;
+    A.type = uint32_t(col.type);
+  }
+  return SDBG_OK;
+}
+
+// One output cell as the caller sees it: the limbs and order keys of AggCell turned into values; zeros when no value.
+sdbg_match_agg agg_result(const AggCell& g, uint32_t type) {
+  sdbg_match_agg a{};
+  a.count = g.count;
+  a.count_value = g.count_value;
+  if (!g.count_value) return a;
+  if (type == SDBG_F64) std::memcpy(&a.sum_f64, &g.sum_lo, 8);
+  else { a.sum_i128[0] = int64_t(g.sum_lo); a.sum_i128[1] = int64_t(g.sum_hi); }
+  a.min = int64_t(sort_order_value(~g.nmin, type));
+  a.max = int64_t(sort_order_value(g.max, type));
+  return a;
 }
 
 // The sorted scan's part of a count_run call.
@@ -1904,7 +1962,7 @@ uint32_t count_planes(uint32_t max_min) {
 }
 
 using CountKernel = void (*)(CountParams);
-enum class CountMode { count, sort, facet };
+enum class CountMode { count, sort, facet, agg };
 
 // A count_run plan: per segment each query's lists and the work items; with OR groups (Q.term_grp), each segment's group
 // ends. Its host staging, which every mode shares: [term_off | excl_off | lists per segment | work items {query, first
@@ -1959,12 +2017,15 @@ struct CountPlan {
   }
 
   // The bm25_count_kernel instantiation of this plan's launches in `mode`, with its dynamic shared memory: the mode's
-  // own bytes (facet bins, sorted keys; none for a count), then the counter planes.
+  // own bytes (facet bins, sorted keys, aggregate cells; none for a count), then the counter planes.
   std::pair<CountKernel, size_t> kernel(CountMode mode, size_t mode_bytes) const {
-    static const CountKernel kernels[3][3] = {   // [OR | AND | OR groups][count | sort | facet]
-        {bm25_count_kernel<false>, bm25_count_kernel<false, false, true>, bm25_count_kernel<false, false, false, true>},
-        {bm25_count_kernel<true>, bm25_count_kernel<true, false, true>, bm25_count_kernel<true, false, false, true>},
-        {bm25_count_kernel<false, true>, bm25_count_kernel<false, true, true>, bm25_count_kernel<false, true, false, true>}};
+    static const CountKernel kernels[3][4] = {   // [OR | AND | OR groups][count | sort | facet | agg]
+        {bm25_count_kernel<false>, bm25_count_kernel<false, false, true>, bm25_count_kernel<false, false, false, true>,
+         bm25_count_kernel<false, false, false, false, true>},
+        {bm25_count_kernel<true>, bm25_count_kernel<true, false, true>, bm25_count_kernel<true, false, false, true>,
+         bm25_count_kernel<true, false, false, false, true>},
+        {bm25_count_kernel<false, true>, bm25_count_kernel<false, true, true>, bm25_count_kernel<false, true, false, true>,
+         bm25_count_kernel<false, true, false, false, true>}};
     const int shape = Q.term_grp ? 2 : Q.kind == SDBG_QUERY_AND ? 1 : 0;
     return {kernels[shape][int(mode)], mode_bytes + size_t(planes) * kCountWords * 4u};
   }
@@ -2072,9 +2133,9 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const Cou
 }
 
 int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_t>& Q, const sdbg_col_pred* filt,
-              uint64_t* counts, SortJob* sort = nullptr, FacetJob* facet = nullptr) {
+              uint64_t* counts, SortJob* sort = nullptr, FacetJob* facet = nullptr, AggJob* agg = nullptr) {
   const auto& [kind, terms, term_off, nq, excl_terms, excl_off, term_grp] = Q;
-  if (!segs || !n_segs || !terms || !term_off || !nq || (!counts && !sort && !facet)) return SDBG_EINVAL;
+  if (!segs || !n_segs || !terms || !term_off || !nq || (!counts && !sort && !facet && !agg)) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   CU(c, cudaSetDevice(c->device));
   uint32_t total_excl = 0;
@@ -2083,6 +2144,8 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
     if (int rc = sort_prepare(c, segs, n_segs, *sort)) return rc;
   if (facet)
     if (int rc = facet_prepare(c, segs, n_segs, *facet)) return rc;
+  if (agg)
+    if (int rc = agg_prepare(c, segs, n_segs, *agg)) return rc;
   const bool conj = kind == SDBG_QUERY_AND;
   const uint32_t n_pos = term_off[nq];
   const size_t n_lists = size_t(n_pos) + total_excl;   // per segment: positive lists | excluded lists
@@ -2189,7 +2252,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
         bool excl_blocks = false;
         if (total_excl)
           for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) excl_blocks |= L[n_pos + i].y != 0;
-        if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks && !sort && !facet) { host[q] += sum; continue; }
+        if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks && !sort && !facet && !agg) { host[q] += sum; continue; }
         weight = conj ? uint64_t(smallest) * (t1 - t0) : sum;
       }
       uint32_t g = uint32_t(std::max<uint64_t>(G, (weight + chain_target - 1) / chain_target));
@@ -2225,9 +2288,11 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
     char* h = static_cast<char*>(c->h_pinned);
     pl.write(h);
     DevBuf& b_desc = c->scratch[0]; DevBuf& b_counts = c->scratch[1];
-    // facet pass: b_counts holds [counts | facet counts [nq][span] | NULL counts [nq] | out-of-range word]
-    const size_t fc_pos = nq * 8, fn_pos = fc_pos + (facet ? nq * size_t(facet->span) * 8 : 0), oor_pos = fn_pos + nq * 8;
-    const size_t out_bytes = facet ? oor_pos + 8 : nq * 8;
+    // facet pass: b_counts holds [counts | facet counts [nq][span] | NULL counts [nq] | out-of-range word]; aggregate
+    // pass: the same with cells of sizeof(AggCell) for the counts
+    const size_t cell = agg ? sizeof(AggCell) : 8, span = facet ? facet->span : agg ? agg->key.span : 0;
+    const size_t fc_pos = nq * 8, fn_pos = fc_pos + nq * span * cell, oor_pos = fn_pos + nq * cell;
+    const size_t out_bytes = facet || agg ? oor_pos + 8 : nq * 8;
     if ((rc = ensure(c, b_desc, bytes))) return rc;
     if ((rc = ensure(c, b_counts, out_bytes))) return rc;
     CU(c, cudaMemcpyAsync(b_desc.p, h, bytes, cudaMemcpyHostToDevice, c->stream));
@@ -2236,6 +2301,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
     // the facet bins, then for groups that need m >= 2 of their lists a bit-sliced counter of bits(m) planes for the
     // batch's largest m (at most 128 + 32 KB)
     const auto [kernel, smem] = facet ? pl.kernel(CountMode::facet, (size_t(facet->span) * 4 + 15) & ~size_t(15))
+                                : agg ? pl.kernel(CountMode::agg, agg_cells_bytes(agg->key.span))
                                       : pl.kernel(CountMode::count, 0);
     CU(c, fit_dynamic_smem(kernel, smem));
     const char* d = static_cast<const char*>(b_desc.p);
@@ -2253,6 +2319,12 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
         P.facet.nulls = reinterpret_cast<unsigned long long*>(fo + fn_pos);
         P.facet.out_of_range = reinterpret_cast<unsigned int*>(fo + oor_pos);
       }
+      if (agg) {
+        P.agg = agg->sink[si];
+        P.agg.cells = reinterpret_cast<AggCell*>(fo + fc_pos);
+        P.agg.nulls = reinterpret_cast<AggCell*>(fo + fn_pos);
+        P.agg.out_of_range = reinterpret_cast<unsigned int*>(fo + oor_pos);
+      }
       kernel<<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
       ++c->launches;
     }
@@ -2266,6 +2338,19 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
       if (oor) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
       return SDBG_OK;
     }
+    if (agg) {   // cells, NULL cells and the out-of-range word in one copy, into the pinned staging (the plan is on the device)
+      if ((rc = ensure_pinned(c, out_bytes - fc_pos))) return rc;
+      const auto* g = static_cast<const AggCell*>(c->h_pinned);
+      CU(c, cudaMemcpyAsync(c->h_pinned, fo + fc_pos, out_bytes - fc_pos, cudaMemcpyDeviceToHost, c->stream));
+      CU(c, cudaStreamSynchronize(c->stream));
+      unsigned int oor = 0;
+      std::memcpy(&oor, static_cast<const char*>(c->h_pinned) + (oor_pos - fc_pos), 4);
+      if (oor) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
+      const uint32_t type = agg->sink[0].type;
+      for (size_t i = 0; i < nq * span; ++i) agg->out[i] = agg_result(g[i], type);
+      for (size_t q = 0; q < nq; ++q) agg->null_out[q] = agg_result(g[nq * span + q], type);
+      return SDBG_OK;
+    }
     CU(c, cudaMemcpyAsync(h, b_counts.p, nq * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     const auto* dc = reinterpret_cast<const unsigned long long*>(h);
@@ -2274,6 +2359,11 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
   if (facet) {   // no query matches anywhere
     std::memset(facet->counts, 0, nq * size_t(facet->span) * 8);
     std::memset(facet->null_counts, 0, nq * 8);
+    return SDBG_OK;
+  }
+  if (agg) {
+    std::memset(agg->out, 0, nq * size_t(agg->key.span) * sizeof(sdbg_match_agg));
+    std::memset(agg->null_out, 0, nq * sizeof(sdbg_match_agg));
     return SDBG_OK;
   }
   std::memcpy(counts, host.data(), nq * 8);
@@ -2304,6 +2394,17 @@ extern "C" int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n
   if (!counts || !null_counts) return SDBG_EINVAL;
   FacetJob J{key_field, key_min, key_span, counts, null_counts, {}};
   return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, nullptr, nullptr, &J);
+}
+
+extern "C" int sdbg_match_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
+                                          const uint32_t* term_off, size_t nq, const uint32_t* excl_terms,
+                                          const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                          int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
+                                          sdbg_match_agg* null_out) {
+  if (!out || !null_out) return SDBG_EINVAL;
+  AggJob J{{key_field, key_min, key_span, nullptr, nullptr, {}}, value_field, out, null_out, {}};
+  return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, nullptr, nullptr, nullptr,
+                   &J);
 }
 
 extern "C" int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2367,6 +2468,23 @@ extern "C" int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* seg
                     {{counts, size_t(key_span) * 8}, {null_counts, 8}}, [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
                       FacetJob J{key_field, key_min, key_span, static_cast<uint64_t*>(r[0].p), static_cast<uint64_t*>(r[1].p), {}};
                       return count_run(segs, n_segs, Q, filt, nullptr, nullptr, &J);
+                    });
+}
+
+extern "C" int sdbg_match_aggregate_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                     const uint32_t* group_off, const uint32_t* query_group_off,
+                                                     const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                     const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                                     int64_t key_min, uint32_t key_span, uint64_t value_field,
+                                                     sdbg_match_agg* out, sdbg_match_agg* null_out) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !out || !null_out) return SDBG_EINVAL;
+  if (int rc = agg_check_range(segs[0]->ctx, key_field, key_min, key_span)) return rc;   // before the rows are sized
+  return run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                    {{out, size_t(key_span) * sizeof(sdbg_match_agg)}, {null_out, sizeof(sdbg_match_agg)}},
+                    [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
+                      AggJob J{{key_field, key_min, key_span, nullptr, nullptr, {}}, value_field,
+                               static_cast<sdbg_match_agg*>(r[0].p), static_cast<sdbg_match_agg*>(r[1].p), {}};
+                      return count_run(segs, n_segs, Q, filt, nullptr, nullptr, nullptr, &J);
                     });
 }
 

@@ -640,6 +640,86 @@ def ExecuteFacetCounts(reader, query_terms, kind, key_field, key_min=None, key_s
                                               exclude=_one(exclude)))
 
 
+MATCH_AGG_DTYPE = np.dtype([("count", "<u8"), ("count_value", "<u8"), ("sum_lo", "<i8"), ("sum_hi", "<i8"),
+                            ("sum_f64", "<f8"), ("min", "<i8"), ("max", "<i8")])
+
+
+def _agg_args(reader, value_field, key_field, key_min, key_span):
+    """(value type code, key field, key_min, key_span) of an aggregate call; key_field None: one group, (0, 1)."""
+    vt = reader.segments[0].col_types.get(int(value_field))
+    if vt is None:   # the values come back as raw bits: their type must be known, not guessed
+        raise ValueError("value column %d was not staged through this Segment" % int(value_field))
+    if key_field is None:
+        return vt, N.UINT64_MAX, 0, 1
+    key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
+    return vt, int(key_field), key_min, key_span
+
+
+def _agg_fields(a, vt):
+    """Structured sdbg_match_agg cells -> dict of count, count_value, sum (Python ints in an object array for integer
+    columns, float64 for float64 ones), avg (float64, NaN without values), min and max (typed by the column; 0 without
+    values)."""
+    cv = a["count_value"]
+    if vt == 1:
+        s = a["sum_f64"].copy()
+        mn, mx = a["min"].view(np.float64).copy(), a["max"].view(np.float64).copy()
+    else:
+        s = np.empty(a.shape, dtype=object)
+        for i in np.ndindex(a.shape):
+            s[i] = (int(a["sum_hi"][i]) << 64) | (int(a["sum_lo"][i]) & 0xFFFFFFFFFFFFFFFF)
+        mn, mx = a["min"].copy(), a["max"].copy()
+    avg = np.full(a.shape, np.nan)
+    for i in zip(*np.nonzero(cv)):
+        avg[i] = s[i] / int(cv[i])
+    return dict(count=a["count"].copy(), count_value=cv.copy(), sum=s, avg=avg, min=mn, max=mx)
+
+
+def _agg_result(out, null_out, nq, key_min, vt):
+    """The dict the aggregate functions return: key_min, the per-key fields [Q, key_span] and the NULL key's [Q]."""
+    r = _agg_fields(out[:nq], vt)
+    r["key_min"] = int(key_min)
+    r["null"] = _agg_fields(null_out[:nq], vt)
+    return r
+
+
+def ExecuteMatchAggregatesBatch(reader, queries, kind, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                                exclude=None):
+    """Aggregates over a full-text query's matches (`SELECT col, count(*), count(v), sum(v), avg(v), min(v), max(v) ...
+    WHERE body @@ '...' GROUP BY col`, sdbg_match_aggregate_batch): per query, over the docs ExecuteCountBatch counts,
+    grouped by `key_field` as ExecuteFacetCountsBatch groups them (key range defaults likewise), or ungrouped (key_field
+    None: one group, key_span 1). `value_field` is an int64 / int32 / float64 column. Returns dict(key_min, count,
+    count_value, sum, avg, min, max, each [Q, key_span], null: the same fields [Q] for the NULL key). sum is exact (Python
+    ints) for integer columns; avg is NaN and sum / min / max are 0 where a group has no non-NULL value."""
+    vt, kf, key_min, key_span = _agg_args(reader, value_field, key_field, key_min, key_span)
+    nq = len(queries)
+    out = np.zeros((max(nq, 1), max(int(key_span), 1)), MATCH_AGG_DTYPE)
+    null_out = np.zeros(max(nq, 1), MATCH_AGG_DTYPE)
+    N.check(N.lib().sdbg_match_aggregate_batch(_seg_array(reader.segments), len(reader.segments), int(kind),
+                                               *_query_args(queries, exclude), _ref(filt), kf, int(key_min), int(key_span),
+                                               int(value_field), _ptr(out), _ptr(null_out)), reader.segments[0].ctx._h)
+    return _agg_result(out, null_out, nq, key_min, vt)
+
+
+def _agg_row(r, grouped):
+    """The first query of an aggregate result: ungrouped its fields as a dict; grouped {key: fields} for the keys with
+    matches, plus {None: fields} when matches have a NULL key."""
+    names = ("count", "count_value", "sum", "avg", "min", "max")
+    if not grouped:
+        return {f: r[f][0][0] for f in names}
+    out = {r["key_min"] + int(i): {f: r[f][0][i] for f in names} for i in np.nonzero(r["count"][0])[0]}
+    if r["null"]["count"][0]:
+        out[None] = {f: r["null"][f][0] for f in names}
+    return out
+
+
+def ExecuteMatchAggregates(reader, query_terms, kind, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                           exclude=None):
+    """ExecuteMatchAggregatesBatch for one query: ungrouped a dict of count, count_value, sum, avg, min, max; grouped
+    {key: that dict} for the keys with matches, plus {None: ...} for the NULL key's matches."""
+    return _agg_row(ExecuteMatchAggregatesBatch(reader, _one(query_terms), kind, value_field, key_field, key_min, key_span,
+                                                filt, exclude=_one(exclude)), key_field is not None)
+
+
 def _groups(queries):
     """Queries as lists of OR groups -> (flat term ids, group_off u32, query_group_off u32)."""
     groups = [list(g) for q in queries for g in q]
@@ -750,6 +830,29 @@ def ExecuteFacetCountsGroups(reader, groups, key_field, key_min=None, key_span=N
     """ExecuteFacetCountsGroupsBatch for one query: {key: count} plus {None: n} for NULL keys, as ExecuteFacetCounts."""
     return _facet_row(ExecuteFacetCountsGroupsBatch(reader, _one_groups(groups), key_field, key_min, key_span, filt,
                                                     exclude=_one(exclude), min_match=_one(min_match)))
+
+
+def ExecuteMatchAggregatesGroupsBatch(reader, queries, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                                      exclude=None, min_match=None):
+    """Aggregates over the matches of conjunctions of OR groups (sdbg_match_aggregate_batch_groups_min): per query, over
+    the docs ExecuteCountGroupsBatch counts. queries / exclude / min_match as in ExecuteCountGroupsBatch; the grouping and
+    the result as in ExecuteMatchAggregatesBatch."""
+    vt, kf, key_min, key_span = _agg_args(reader, value_field, key_field, key_min, key_span)
+    nq = len(queries)
+    out = np.zeros((max(nq, 1), max(int(key_span), 1)), MATCH_AGG_DTYPE)
+    null_out = np.zeros(max(nq, 1), MATCH_AGG_DTYPE)
+    N.check(N.lib().sdbg_match_aggregate_batch_groups_min(
+        _seg_array(reader.segments), len(reader.segments), *_query_args(queries, exclude, min_match, groups=True),
+        _ref(filt), kf, int(key_min), int(key_span), int(value_field), _ptr(out), _ptr(null_out)), reader.segments[0].ctx._h)
+    return _agg_result(out, null_out, nq, key_min, vt)
+
+
+def ExecuteMatchAggregatesGroups(reader, groups, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                                 exclude=None, min_match=None):
+    """ExecuteMatchAggregatesGroupsBatch for one query (a list of OR groups), in the form ExecuteMatchAggregates returns."""
+    return _agg_row(ExecuteMatchAggregatesGroupsBatch(reader, _one_groups(groups), value_field, key_field, key_min, key_span,
+                                                      filt, exclude=_one(exclude), min_match=_one(min_match)),
+                    key_field is not None)
 
 
 FOR_BLOCK_DTYPE =np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])

@@ -6,7 +6,8 @@
 // (tests/test_gpu_groups.py); with "minmatch", only an Or with min_match_count through both adapters
 // (tests/test_gpu_min_match.py); with "sorted", only the sorted scan (GpuSortedScan, tests/test_gpu_sort_by_column.py); with
 // "facet", only the facet counts (GpuFacetScan, tests/test_gpu_facets.py). "sorted groups" / "facet groups" run those two
-// with group queries (tests/test_gpu_groups_column.py).
+// with group queries (tests/test_gpu_groups_column.py). "aggregate" / "aggregate groups" run the aggregates over the matches
+// (GpuMatchAggScan, tests/test_gpu_match_aggregates.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -228,6 +229,74 @@ int main(int argc, char** argv) {
     int code = 0;
     try {
       sdbg_host::GpuFacetScan wide({seg}, SDBG_QUERY_OR, {2, 5}, {}, nullptr, 9);
+      duckdb::DataChunkMock chunk;
+      wide.Scan(chunk);
+    } catch (const sdbg_host::GpuError& e) { code = e.code; }
+    std::printf("{\"wide_error\": %d}\n", code);
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
+  if (argc > 2 && std::string(argv[2]) == "aggregate") {
+    // `t2 | t5`, `t2 & t5` and `(t2 | t5) & !t3` (grouped: "kind" 0 / 1 is query 0 / 1), without and with the table filter:
+    // count, count(v), sum, avg, min, max of the int32 column 9 GROUP BY the 2001-key int64 column 15 (every group in key
+    // order, then end of scan), and of the float64 column 16 without GROUP BY (one row). Then column 9 as the key, whose
+    // range is too wide.
+    sdbg_synth_column(seg, 15, 15, 3, 1, n_docs);
+    sdbg_synth_column(seg, 16, 16, 4, 1, n_docs);
+    auto run = [&](sdbg_host::GpuMatchAggScan& scan, const char* name) {
+      duckdb::DataChunkMock chunk;
+      std::vector<long long> keys, cnt, cntv, lo, hi, mn, mx;
+      std::vector<double> sf, avg;
+      std::vector<unsigned> valid;
+      uint64_t chunks = 0, max_chunk = 0;
+      for (;;) {
+        scan.Scan(chunk);
+        if (chunk.size == 0) break;
+        ++chunks;
+        max_chunk = std::max<uint64_t>(max_chunk, chunk.size);
+        for (size_t i = 0; i < chunk.size; ++i) {
+          keys.push_back(chunk.key[i]); cnt.push_back(chunk.count[i]); cntv.push_back(chunk.count_value[i]);
+          lo.push_back(chunk.sum_lo[i]); hi.push_back(chunk.sum_hi[i]); sf.push_back(chunk.sum_f64[i]); avg.push_back(chunk.avg[i]);
+          mn.push_back(chunk.min[i]); mx.push_back(chunk.max[i]); valid.push_back(chunk.valid[i]);
+        }
+      }
+      scan.Scan(chunk);
+      std::printf("\"%s\": {\"chunks\": %llu, \"max_chunk\": %llu, \"rows_after\": %llu", name, static_cast<unsigned long long>(chunks),
+                  static_cast<unsigned long long>(max_chunk), static_cast<unsigned long long>(chunk.size));
+      auto ints = [](const char* f, const std::vector<long long>& v) {
+        std::printf(", \"%s\": [", f);
+        for (size_t i = 0; i < v.size(); ++i) std::printf("%s%lld", i ? ", " : "", v[i]);
+        std::printf("]");
+      };
+      auto dbls = [](const char* f, const std::vector<double>& v) {
+        std::printf(", \"%s\": [", f);
+        for (size_t i = 0; i < v.size(); ++i) std::printf("%s%.17g", i ? ", " : "", v[i]);
+        std::printf("]");
+      };
+      ints("keys", keys); ints("count", cnt); ints("count_value", cntv); ints("sum_lo", lo); ints("sum_hi", hi);
+      dbls("sum_f64", sf); dbls("avg", avg); ints("min", mn); ints("max", mx);
+      std::printf(", \"valid\": [");
+      for (size_t i = 0; i < valid.size(); ++i) std::printf("%s%u", i ? ", " : "", valid[i]);
+      std::printf("]}");
+    };
+    for (int with_filter = 0; with_filter < 2; ++with_filter)
+      for (int kind : {int(SDBG_QUERY_OR), int(SDBG_QUERY_AND)})
+        for (int excl = 0; excl < 2; ++excl) {
+          const std::vector<uint32_t> ex = excl ? std::vector<uint32_t>{3} : std::vector<uint32_t>{};
+          sdbg_host::GpuMatchAggScan by_key({seg}, kind, grouped ? group_ids : flat_ids, ex, with_filter ? &filt : nullptr, 15, 9,
+                                            SDBG_I32, group_sizes(kind), group_mins(kind));
+          sdbg_host::GpuMatchAggScan whole({seg}, kind, grouped ? group_ids : flat_ids, ex, with_filter ? &filt : nullptr, UINT64_MAX,
+                                           16, SDBG_F64, group_sizes(kind), group_mins(kind));
+          std::printf("{\"filter\": %d, \"kind\": %d, \"excl\": %d, ", with_filter, kind, excl);
+          run(by_key, "grouped");
+          std::printf(", ");
+          run(whole, "ungrouped");
+          std::printf("}\n");
+        }
+    int code = 0;
+    try {
+      sdbg_host::GpuMatchAggScan wide({seg}, SDBG_QUERY_OR, {2, 5}, {}, nullptr, 9, 16, SDBG_F64);
       duckdb::DataChunkMock chunk;
       wide.Scan(chunk);
     } catch (const sdbg_host::GpuError& e) { code = e.code; }

@@ -340,6 +340,83 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
   cursor_ += take;
 }
 
+GpuMatchAggScan::GpuMatchAggScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
+                                 std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
+                                 uint64_t value_field, sdbg_type value_type, std::vector<uint32_t> group_sizes,
+                                 std::vector<uint32_t> group_min_match)
+    : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), has_filter_(table_filter != nullptr),
+      key_field_(key_field), value_field_(value_field), value_type_(value_type) {
+  if (table_filter) filter_ = *table_filter;
+}
+
+void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
+  output.Reset();
+  if (!ran_) {
+    sdbg_ctx* ctx = sdbg_segment_context(segs_[0]);
+    const bool grouped = key_field_ != UINT64_MAX;
+    int64_t lo = 0;
+    uint64_t span = 1;
+    if (grouped) {
+      int64_t mn_all = INT64_MAX, mx_all = INT64_MIN;
+      for (sdbg_segment* s : segs_) {
+        int64_t mn = 0, mx = 0;
+        const int rc = sdbg_column_minmax_i64(s, key_field_, &mn, &mx);
+        if (rc != SDBG_OK) throw GpuError(rc, std::string("sdbg_column_minmax_i64: ") + sdbg_last_error(ctx));
+        mn_all = std::min(mn_all, mn);
+        mx_all = std::max(mx_all, mx);
+      }
+      if (mn_all > mx_all) mn_all = mx_all = 0;   // every key NULL: one (empty) group, every match in the NULL group
+      lo = mn_all;
+      span = uint64_t(mx_all) - uint64_t(mn_all) + 1;
+      if (span == 0 || span > 4096) throw GpuError(SDBG_EUNSUPPORTED, "GpuMatchAggScan: the key range spans more than 4096 values");
+    }
+    const uint32_t term_off[2] = {0, uint32_t(terms_.size())};
+    const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
+    std::vector<sdbg_match_agg> cells(span);
+    sdbg_match_agg null_cell{};
+    int rc;
+    const char* what;
+    if (group_sizes_.empty()) {
+      rc = sdbg_match_aggregate_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
+                                      has_filter_ ? &filter_ : nullptr, key_field_, lo, uint32_t(span), value_field_, cells.data(),
+                                      &null_cell);
+      what = "sdbg_match_aggregate_batch: ";
+    } else {                                                  // an And of Ors: kind_ is not used
+      const std::vector<uint32_t> group_off = group_offsets(group_sizes_, terms_.size());
+      const uint32_t query_group_off[2] = {0, uint32_t(group_sizes_.size())};
+      rc = sdbg_match_aggregate_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
+                                                 group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(), excl_off,
+                                                 has_filter_ ? &filter_ : nullptr, key_field_, lo, uint32_t(span), value_field_,
+                                                 cells.data(), &null_cell);
+      what = "sdbg_match_aggregate_batch_groups_min: ";
+    }
+    if (rc != SDBG_OK) throw GpuError(rc, std::string(what) + sdbg_last_error(ctx));
+    for (uint64_t i = 0; i < span; ++i)
+      if (cells[i].count || !grouped) groups_.emplace_back(int64_t(uint64_t(lo) + i), cells[i]);   // ungrouped: always one row
+    if (grouped && null_cell.count) { groups_.emplace_back(0, null_cell); null_row_ = true; }
+    ran_ = true;
+  }
+  const size_t take = std::min<size_t>(duckdb::STANDARD_VECTOR_SIZE, groups_.size() - cursor_);   // 0: end of scan
+  for (size_t i = cursor_; i < cursor_ + take; ++i) {
+    const sdbg_match_agg& a = groups_[i].second;
+    const bool null_group = null_row_ && i + 1 == groups_.size();
+    const __int128 sum = (static_cast<__int128>(a.sum_i128[1]) << 64) | static_cast<unsigned long long>(a.sum_i128[0]);
+    output.key.push_back(null_group || key_field_ == UINT64_MAX ? 0 : groups_[i].first);
+    output.valid.push_back(null_group ? 0 : 1);
+    output.count.push_back(int64_t(a.count));
+    output.count_value.push_back(int64_t(a.count_value));
+    output.sum_lo.push_back(a.sum_i128[0]);
+    output.sum_hi.push_back(a.sum_i128[1]);
+    output.sum_f64.push_back(a.sum_f64);
+    output.avg.push_back(!a.count_value ? 0.0 : (value_type_ == SDBG_F64 ? a.sum_f64 : double(sum)) / double(a.count_value));
+    output.min.push_back(a.min);
+    output.max.push_back(a.max);
+  }
+  output.size = take;
+  cursor_ += take;
+}
+
 GpuAggGlobalState::GpuAggGlobalState(std::vector<sdbg_segment*> segments, std::vector<sdbg_col_pred> pushed_filters, uint64_t key_field,
                                      uint64_t sum_int_field, uint64_t avg_f64_field, uint32_t n_groups_hint)
     : segs(std::move(segments)), preds(std::move(pushed_filters)), key(key_field), sum_i(sum_int_field), avg_f(avg_f64_field),

@@ -186,6 +186,39 @@ class GpuFacetScan {
   bool ran_ = false;
 };
 
+// SELECT [col,] count(*), count(v), sum(v), avg(v), min(v), max(v) FROM t WHERE body @@ '<query>' [AND <pushed filter>]
+// [GROUP BY col] -- the body of the HASH_GROUP_BY(col; count_star(), count(v), sum(v), avg(v), min(v), max(v)) and
+// UNGROUPED_AGGREGATE(...) <- IRESEARCH_SCAN(text query) plan shapes, for one value column (two columns: two scans). The
+// first Scan takes the key range as GpuFacetScan does and runs one sdbg_match_aggregate_batch call
+// (sdbg_match_aggregate_batch_groups_min with group_sizes). Grouped, it then emits the non-empty groups as rows (key, count,
+// count_value, sum_lo / sum_hi or sum_f64, avg, min, max, valid) in ascending key order, the NULL group (valid = 0) last;
+// ungrouped (key_field UINT64_MAX), one row. <= STANDARD_VECTOR_SIZE rows per call, cardinality 0 at the end. A row with
+// count_value 0 has NULL sum, avg, min and max (emitted as 0). A key range wider than 4096 values throws
+// GpuError(SDBG_EUNSUPPORTED): the plan stays on the CPU.
+class GpuMatchAggScan {
+ public:
+  GpuMatchAggScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
+                  std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
+                  uint64_t key_field /* int64 or int32; UINT64_MAX: no GROUP BY */, uint64_t value_field,
+                  sdbg_type value_type /* as staged: picks sum_f64 or the 128-bit sum for avg */,
+                  std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
+                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
+  void Scan(duckdb::DataChunkMock& output);
+
+ private:
+  std::vector<sdbg_segment*> segs_;
+  int kind_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
+  bool has_filter_;
+  sdbg_col_pred filter_{};
+  uint64_t key_field_, value_field_;
+  sdbg_type value_type_;
+  std::vector<std::pair<int64_t, sdbg_match_agg>> groups_;   // (key, cell) of the rows to emit
+  bool null_row_ = false;                                    // the last row of groups_ is the NULL group
+  size_t cursor_ = 0;
+  bool ran_ = false;
+};
+
 // The same scan mode under DuckDB's threading contract (duckdb_search_full_scan.hpp:85-255, .cpp:99-268): ONE global
 // state shared by all workers of the query -- touched through atomics only, like next_segment / next_unit there -- and
 // one local state per worker. The first worker to arrive runs the aggregation on the GPU (the others wait on the

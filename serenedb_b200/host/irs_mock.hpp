@@ -228,6 +228,9 @@ struct DataChunkMock {          // stands in for duckdb::DataChunk with flat vec
   std::vector<int64_t> sum_lo;  // SUM(v) as HUGEINT: lower / upper
   std::vector<int64_t> sum_hi;
   std::vector<double> avg;      // AVG(w)
+  std::vector<int64_t> count_value;   // aggregates over a text query's matches: COUNT(v), SUM(v) of a float64 column,
+  std::vector<double> sum_f64;        //   MIN / MAX(v) (int64, sign-extended int32 or the double's bits)
+  std::vector<int64_t> min, max;
   std::vector<uint32_t> doc;    // sorted scan: the hit's doc id, segment index, sort value (int64, sign-extended int32 or
   std::vector<uint32_t> segment;//   the double's bits) and validity (0 = NULL)
   std::vector<int64_t> value;
@@ -235,6 +238,7 @@ struct DataChunkMock {          // stands in for duckdb::DataChunk with flat vec
   uint64_t size = 0;
   void Reset() {
     key.clear(); count.clear(); sum_lo.clear(); sum_hi.clear(); avg.clear();
+    count_value.clear(); sum_f64.clear(); min.clear(); max.clear();
     doc.clear(); segment.clear(); value.clear(); valid.clear();
     size = 0;
   }
