@@ -377,7 +377,7 @@ int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n
  * Device scratch: (n_queries * (key_span + 1)) * 48 B + n_queries * 8 B (4096 queries x 2001 keys: 394 MB), and as
  * much pinned host memory for the copy back. Split larger batches.
  * Not supported: several value columns in one call (call once per column), key spans above 4096, float64 keys, HAVING,
- * COUNT(DISTINCT), a multi-GPU merge of the cells, the top-k and streaming entries. */
+ * COUNT(DISTINCT), the top-k and streaming entries. The multi-GPU merge: sdbg_dist_match_aggregate_batch_groups_min. */
 typedef struct {
   uint64_t count;         /* COUNT(*) of the group's matches */
   uint64_t count_value;   /* COUNT(value): those whose value is not NULL */
@@ -515,6 +515,111 @@ int sdbg_dist_groupby_merge(sdbg_ctx*, void* d_i64, void* d_f64, uint64_t span, 
 int sdbg_dist_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
                               const uint32_t* term_off, size_t n_queries, float k1, float b, const sdbg_col_pred* filt,
                               uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out);
+/* Count, facet counts, aggregates and the sorted scan over the segments of ALL ranks (a corpus sharded by segment, one
+   context per GPU): each rank runs the local pass over its own segments with the results left in HBM, then one collective
+   and, for the aggregates and the sorted scan, a merge kernel, back to back on the context's stream; the one wait is the
+   copy back at the end (the sorted scan's zonemap planning also waits for its own small copies, before its launches).
+   The query parameters are those of the *_batch_groups_min entries. A flat query is a degenerate groups query (OR: one
+   group, AND: single-term groups), which the groups entries run as the flat entries and with exactly their results
+   (§ "Conjunctions of OR groups" above), so there are no flat-form dist entries. Results are those of the local entry
+   over the union of all ranks' segments, the same on every rank.
+   Caller's contract, as for any collective: every rank makes the same call with the same queries, key_field, key_min,
+   key_span, value_field, sort_field, order and k (the collective's size follows from n_queries, key_span and k); every
+   rank holds at least one segment (a rank without segments passes a segment with no docs); and every rank has the HBM
+   for the scratch below (a failed allocation returns SDBG_ECUDA before the collective, like any CUDA failure).
+   Errors: checks of the call's scalar arguments (NULL outputs or offsets, n_queries == 0, the key range as in the local
+   entries, world > 1 without sdbg_dist_init) fail alike on every rank before anything is queued. Failures of a rank's
+   own pass (a bad term id, a missing or mistyped column, a key outside the range, a value column whose type differs from
+   other ranks') still join the collective with a failure flag in the exchanged buffer: the failing rank returns its own
+   code, every other rank SDBG_EINVAL, and the outputs are unspecified.
+   Without sdbg_dist_init the world is one rank: the all-reduce is a no-op, the all-gather a copy and the merge of one
+   rank's buffer the identity on its cells and rows, so each entry gives its local entry's result: exactly for counts,
+   facet counts, the integer aggregates, MIN / MAX and the sorted hits; for float64 sums the local pass's own sum, whose
+   last bits vary from run to run (its atomics add in no fixed order).
+   sdbg_dist_match_count_batch_groups_min / sdbg_dist_match_facet_counts_batch_groups_min: one ncclAllReduce(int64, sum)
+   over [counts | NULL counts | out-of-range word | failure flag]; a key outside the range on any rank fails the call on
+   every rank. Device scratch: the local entry's, plus (n_queries * (key_span + 2) + 2) * 8 B, plus for a batch
+   of several query shapes (flat OR, flat AND, nested) one more set of per-query rows before they are scattered to query
+   order.
+   sdbg_match_aggregate_batch_groups_min_device: this rank's cells of sdbg_match_aggregate_batch_groups_min left in
+   d_cells, with no wait: a 64-byte header {value type, key_span, n_queries, failure word, out-of-range word, 3 zero words}
+   then n_queries * (key_span + 1) cells of 48 B (the per-key cells, then the NULL key's). A failure of the local pass
+   returns its code and sets the header's failure word, so that a merge of the buffer fails on every rank.
+   sdbg_match_aggregate_merge_gathered: the aggregates of n_ranks such buffers back to back (rank order). One thread per
+   (query, key) cell: counts add, integer sums add in 128-bit two's complement with an exact carry, float64 sums are the
+   ranks' partials added in rank order (bit-identical on every rank; IEEE NaN / inf rules hold), MIN / MAX are the largest
+   order keys; then the local entry's conversion. The float64 sum therefore differs from the local entry's over the
+   unsharded corpus only by the order of the additions. Headers that disagree (value type, key_span, n_queries) or any
+   rank's failure or out-of-range word: SDBG_EINVAL. key_span > 4096: SDBG_EUNSUPPORTED.
+   sdbg_dist_match_aggregate_batch_groups_min: the device form, one sdbg_dist_allgather, the merge. Device scratch:
+   (1 + world) buffers of the device form plus one of merged cells: 4096 queries x 2002 keys x 48 B = 394 MB per buffer,
+   3.9 GB at 8 ranks, a batch of several query shapes one more buffer of rows, and 394 MB of pinned host memory for the
+   copy back. Split larger batches.
+   sdbg_match_topk_by_column_batch_groups_min_device: this rank's min(k, matches) best rows per query of
+   sdbg_match_topk_by_column_batch_groups_min, best first, left in d_rows with no wait: a 64-byte header {sort type, desc,
+   nulls_first, k, n_queries, failure word, 2 zero words}, the row count of each query (u64 [n_queries]), then rows
+   [n_queries][k] of 24 B: the 16-byte key of the sorted scan (bm25_sort.cuh) with ~rank in bits 32..62 of its low word, so
+   that ties go to the lower rank, and the stored value's 8 bytes (the key canonicalises -0.0 and NaN). Each rank keeps up
+   to 2^32 - 2 docs per call, as the local entry. rank >= 2^31: SDBG_EUNSUPPORTED; a failure of the local pass returns its
+   code and sets the failure word.
+   sdbg_match_topk_by_column_merge_gathered: per query (one CTA) the k best of n_ranks such buffers, in order, as
+   sdbg_sort_hit: the value bits, doc = the hit's ordinal within its rank + 1 (the rank's earlier segments' docs plus the
+   doc id), seg = the rank, is_null. Ties go to (rank asc, segment asc, doc asc): with ranks holding consecutive segments
+   in corpus order, the order of the local entry over the unsharded corpus. Headers that disagree (sort type, desc,
+   nulls_first, k, n_queries) or any rank's failure word: SDBG_EINVAL. k == 0: SDBG_EINVAL; k > 4096: SDBG_EUNSUPPORTED.
+   sdbg_dist_match_topk_by_column_batch_groups_min: the device form, one sdbg_dist_allgather, the merge; hit.seg = rank.
+   Device scratch: the local entry's, (1 + world) device-form buffers of 64 + n_queries * (8 + 24 k) B (8 ranks, 4096
+   queries, k = 1000: 787 MB gathered), n_queries * k * 24 B of merged hits, and as much pinned host memory.
+   Not supported: exclusion / group forms of sdbg_bm25_topk_batch_device and sdbg_dist_bm25_topk_batch (they run on the
+   top-k path with 2^28-ordinal rank slots), the streaming scan across ranks, a sort threshold exchanged between ranks
+   during the scan. */
+int sdbg_dist_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                           const uint32_t* group_off, const uint32_t* query_group_off,
+                                           const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                           const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                           const sdbg_col_pred* filt, uint64_t* counts /* n_queries */);
+int sdbg_dist_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                  const uint32_t* group_off, const uint32_t* query_group_off,
+                                                  const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                                  const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                                  const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min,
+                                                  uint32_t key_span, uint64_t* counts /* n_queries * key_span */,
+                                                  uint64_t* null_counts /* n_queries */);
+int sdbg_match_aggregate_batch_groups_min_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                 const uint32_t* group_off, const uint32_t* query_group_off,
+                                                 const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                                 const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                                 const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min,
+                                                 uint32_t key_span, uint64_t value_field,
+                                                 void* d_cells /* 64 + n_queries * (key_span + 1) * 48 B */);
+int sdbg_match_aggregate_merge_gathered(sdbg_ctx*, const void* d_all /* n_ranks device-form buffers */, uint32_t n_ranks,
+                                        size_t n_queries, uint32_t key_span, sdbg_match_agg* out /* n_queries * key_span */,
+                                        sdbg_match_agg* null_out /* n_queries */);
+int sdbg_match_topk_by_column_batch_groups_min_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                      const uint32_t* group_off, const uint32_t* query_group_off,
+                                                      const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                                      const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                                      const sdbg_col_pred* filt, uint64_t sort_field, int descending,
+                                                      int nulls_first, uint32_t k, uint32_t rank,
+                                                      void* d_rows /* 64 + n_queries * (8 + 24 * k) B */);
+int sdbg_match_topk_by_column_merge_gathered(sdbg_ctx*, const void* d_all /* n_ranks device-form buffers */, uint32_t n_ranks,
+                                             size_t n_queries, uint32_t k, sdbg_sort_hit* out /* n_queries * k */,
+                                             uint32_t* n_out /* n_queries */);
+int sdbg_dist_match_topk_by_column_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                    const uint32_t* group_off, const uint32_t* query_group_off,
+                                                    const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                                    const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                                    const sdbg_col_pred* filt, uint64_t sort_field, int descending,
+                                                    int nulls_first, uint32_t k, sdbg_sort_hit* out /* n_queries * k */,
+                                                    uint32_t* n_out /* n_queries */);
+int sdbg_dist_match_aggregate_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                               const uint32_t* group_off, const uint32_t* query_group_off,
+                                               const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                               const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                               const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min,
+                                               uint32_t key_span, uint64_t value_field,
+                                               sdbg_match_agg* out /* n_queries * key_span */,
+                                               sdbg_match_agg* null_out /* n_queries */);
 
 #ifdef __cplusplus
 }

@@ -6,6 +6,9 @@ include/sdbg.h). Importing it loads the native library; if the library cannot be
 import raises -- there is no Python or CPU fallback for any operation.
 """
 from . import _native
+from .engine import (ExecuteDistCountGroupsBatch, ExecuteDistFacetCountsGroupsBatch, ExecuteDistMatchAggregatesGroupsBatch,
+                     ExecuteDistTopKByColumnGroupsBatch, MatchAggregatesDevice, TopKByColumnDevice, match_aggregate_device_bytes,
+                     merge_aggregates_gathered, merge_topk_by_column_gathered, topk_by_column_device_bytes)
 from .engine import (AND, OR, BM25, TFIDF, FLT_MIN, Context, ExecuteCount, ExecuteCountBatch, ExecuteCountGroups,
                      ExecuteCountGroupsBatch, ExecuteFacetCounts, ExecuteFacetCountsBatch, ExecuteFacetCountsGroups,
                      ExecuteFacetCountsGroupsBatch, ExecuteMatchAggregates, ExecuteMatchAggregatesBatch,
@@ -20,4 +23,8 @@ __all__ = ["AND", "OR", "BM25", "TFIDF", "FLT_MIN", "Context", "ExecuteCount", "
            "ExecuteFacetCountsGroupsBatch", "ExecuteMatchAggregates", "ExecuteMatchAggregatesBatch",
            "ExecuteMatchAggregatesGroups", "ExecuteMatchAggregatesGroupsBatch", "ExecuteTopK", "ExecuteTopKBatch", "ExecuteTopKByColumn", "ExecuteTopKByColumnBatch",
            "ExecuteTopKByColumnGroups", "ExecuteTopKByColumnGroupsBatch", "ExecuteTopKGroups", "ExecuteTopKGroupsBatch", "IndexReader", "IResearchScan", "PostingsWriter", "PreparedBatch", "Segment", "merge_gathered",
-           "pred", "resolve_pred", "stage_parse_host", "sum_i128", "StreamScoredDocs", "pack_for"]
+           "pred", "resolve_pred", "stage_parse_host", "sum_i128", "StreamScoredDocs", "pack_for",
+           "ExecuteDistCountGroupsBatch", "ExecuteDistFacetCountsGroupsBatch", "ExecuteDistMatchAggregatesGroupsBatch",
+           "MatchAggregatesDevice", "match_aggregate_device_bytes", "merge_aggregates_gathered",
+           "ExecuteDistTopKByColumnGroupsBatch", "TopKByColumnDevice", "topk_by_column_device_bytes",
+           "merge_topk_by_column_gathered"]

@@ -191,4 +191,110 @@ __global__ void __launch_bounds__(256) sort_merge_kernel(SortMergeParams P) {
   if (threadIdx.x == 0) P.n_out[q] = n;
 }
 
+// ---- the sorted scan across ranks ----
+// A rank's buffer: SortDistHeader, then its per-query row counts (u64 [nq]), then rows [nq][k], best first. A row is the
+// key above with the rank folded into lo bits 32..62 as ~rank (ties go to the lower rank, then the lower ordinal), and
+// the stored value: the key canonicalises -0.0 and NaN, so the value cannot be rebuilt from it.
+struct SortDistHeader {
+  unsigned long long type, desc, nulls_first, k, nq;   // the sort column's sdbg_type (UINT64_MAX: not found), the call's order
+  unsigned long long failed;                           // non-zero: this rank's local pass failed
+  unsigned long long pad[2];
+};
+static_assert(sizeof(SortDistHeader) == 64, "the rows stay 16-byte aligned");
+
+struct SortDistRow { unsigned long long hi, lo, value; };
+
+__host__ __device__ __forceinline__ unsigned long long sort_rank_bits(uint32_t rank) {
+  return static_cast<unsigned long long>(~rank & 0x7FFFFFFFu) << 32;
+}
+
+// One CTA per query: the local result's hits (sort_merge_kernel's output) -> this rank's rows.
+__global__ void __launch_bounds__(256) sort_dist_rows_kernel(const SortHitDev* __restrict__ hits, const uint32_t* __restrict__ n_out,
+                                                             const SortSegDev* __restrict__ segs, uint32_t k, uint32_t type,
+                                                             uint32_t desc, uint32_t nulls_first, uint32_t rank,
+                                                             unsigned long long* __restrict__ rows_n, SortDistRow* __restrict__ rows) {
+  const uint32_t q = blockIdx.x, n = n_out[q];
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const SortHitDev h = hits[size_t(q) * k + i];
+    const uint32_t ord = segs[h.seg].ordinal_base + h.doc - 1u;
+    const unsigned long long rlo = sort_rank_bits(rank) | (~static_cast<unsigned long long>(ord) & 0xFFFFFFFFull);
+    SortDistRow w;
+    if (h.is_null) {
+      w = {static_cast<unsigned long long>(nulls_first) << 63, rlo, 0ull};
+    } else {
+      const unsigned long long o = sort_order(static_cast<unsigned long long>(h.value), type), vkey = desc ? o : ~o;
+      w = {(static_cast<unsigned long long>(nulls_first ^ 1u) << 63) | (vkey >> 1), ((vkey & 1ull) << 63) | rlo,
+           static_cast<unsigned long long>(h.value)};
+    }
+    rows[size_t(q) * k + i] = w;
+  }
+  if (threadIdx.x == 0) rows_n[q] = n;
+}
+
+// One CTA per query: the k best of n_ranks ranks' rows (buffers of rank_bytes back to back), in order, as sdbg_sort_hit
+// (doc = ordinal within the rank + 1, seg = rank). Each selected key's value is found by a binary search of its rank's
+// list, which is sorted best first with unique keys. Block 0 also checks the headers: status = {headers disagree, some
+// rank failed}.
+__global__ void __launch_bounds__(256) sort_merge_gathered_kernel(const char* __restrict__ all, size_t rank_bytes, uint32_t n_ranks,
+                                                                  uint32_t nq, uint32_t k, uint32_t cap,
+                                                                  unsigned long long* __restrict__ status, SortHitDev* __restrict__ out,
+                                                                  uint32_t* __restrict__ n_out) {
+  extern __shared__ unsigned long long sm_keys[];
+  __shared__ uint32_t s_fill;
+  unsigned long long* hi = sm_keys;
+  unsigned long long* lo = sm_keys + cap;
+  const uint32_t q = blockIdx.x;
+  const auto* h0 = reinterpret_cast<const SortDistHeader*>(all);
+  if (q == 0 && threadIdx.x == 0) {
+    unsigned long long bad = 0, failed = 0;
+    for (uint32_t r = 0; r < n_ranks; ++r) {
+      const auto* h = reinterpret_cast<const SortDistHeader*>(all + r * rank_bytes);
+      bad |= h->type != h0->type || h->desc != h0->desc || h->nulls_first != h0->nulls_first || h->k != k || h->nq != nq;
+      failed |= h->failed;
+    }
+    status[0] = bad; status[1] = failed;
+  }
+  const size_t rows_pos = sizeof(SortDistHeader) + size_t(nq) * 8;
+  for (uint32_t i = threadIdx.x; i < cap; i += blockDim.x) { hi[i] = 0ull; lo[i] = 0ull; }
+  if (threadIdx.x == 0) s_fill = 0u;
+  __syncthreads();
+  for (uint32_t r = 0; r < n_ranks; ++r) {
+    const char* b = all + r * rank_bytes;
+    const uint32_t n = static_cast<uint32_t>(min(reinterpret_cast<const unsigned long long*>(b + sizeof(SortDistHeader))[q],
+                                                 static_cast<unsigned long long>(k)));
+    if (s_fill + n > cap) sort_select(hi, lo, cap, k, &s_fill);   // n <= k and cap >= 2k: room after a select
+    const uint32_t f = s_fill;
+    const auto* rows = reinterpret_cast<const SortDistRow*>(b + rows_pos) + size_t(q) * k;
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) { hi[f + i] = rows[i].hi; lo[f + i] = rows[i].lo; }
+    __syncthreads();
+    if (threadIdx.x == 0) s_fill = f + n;
+    __syncthreads();
+  }
+  sort_select(hi, lo, cap, k, &s_fill);
+  const uint32_t n = s_fill;
+  const uint32_t nulls_first = static_cast<uint32_t>(h0->nulls_first);
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const unsigned long long kh = hi[i], kl = lo[i];
+    const uint32_t r = ~static_cast<uint32_t>(kl >> 32) & 0x7FFFFFFFu;
+    SortHitDev h{};
+    h.doc = ~static_cast<uint32_t>(kl) + 1u;
+    h.seg = r;
+    h.is_null = static_cast<uint8_t>((kh >> 63) == nulls_first);
+    if (!h.is_null && r < n_ranks) {
+      const char* b = all + r * rank_bytes;
+      const auto* rows = reinterpret_cast<const SortDistRow*>(b + rows_pos) + size_t(q) * k;
+      const uint32_t cnt = static_cast<uint32_t>(min(reinterpret_cast<const unsigned long long*>(b + sizeof(SortDistHeader))[q],
+                                                     static_cast<unsigned long long>(k)));
+      uint32_t a = 0, e = cnt;
+      while (a < e) {   // first row not better than the key: the key itself
+        const uint32_t m = (a + e) >> 1;
+        if (key_less(kh, kl, rows[m].hi, rows[m].lo)) a = m + 1u; else e = m;
+      }
+      if (a < cnt) h.value = static_cast<long long>(rows[a].value);
+    }
+    out[size_t(q) * k + i] = h;
+  }
+  if (threadIdx.x == 0) n_out[q] = n;
+}
+
 }  // namespace sdbg

@@ -76,6 +76,9 @@ struct sdbg_ctx {
   std::string err;
   uint64_t launches = 0;
   DevBuf scratch[16];
+  // the full-text dist entries: [0] this rank's buffer, [1] the gathered buffers, [2] per-shape rows of a mixed-shape
+  // batch, [3] the device passes' count scratch and the merged cells
+  DevBuf dist[4];
   DevBuf stage_raw;          // raw int64 values of a column being packed at staging (reused: restaging allocates nothing)
   void* h_pinned = nullptr;  // pinned host staging for small transfers
   size_t h_pinned_cap = 0;
@@ -245,6 +248,7 @@ extern "C" void sdbg_destroy(sdbg_ctx* c) {
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
   for (auto& b : c->scratch) if (b.p) cudaFree(b.p);
+  for (auto& b : c->dist) if (b.p) cudaFree(b.p);
   if (c->stage_raw.p) cudaFree(c->stage_raw.p);
   if (c->h_pinned) cudaFreeHost(c->h_pinned);
   if (c->h_oor) cudaFreeHost(c->h_oor);
@@ -2031,10 +2035,23 @@ struct CountPlan {
   }
 };
 
+// Device-output mode of count_run: the results stay in these device arrays, nothing is copied back and nothing waits
+// (the sorted scan's zonemap planning excepted), so a collective can follow on the stream. The plan is staged from
+// pageable memory, which the copy has consumed when it returns, so calls can follow one another without a wait.
+struct CountDevOut {
+  unsigned long long* counts;   // [nq]: the counts (set to the single-term shortcut's, the kernels add theirs); scratch
+                                // for the facet and aggregate passes
+  void* bins;                   // zeroed by the caller: facet u64 [nq][span], aggregate AggCell [nq][span]
+  void* nulls;                  // zeroed by the caller: facet u64 [nq], aggregate AggCell [nq]
+  unsigned int* oor;            // zeroed by the caller: set to 1 when a matching doc's key lies outside the range
+  // the sorted scan: counts holds each query's row count (u64), bins its rows [nq][k] (SortDistRow) for rank `rank`
+  uint32_t rank;
+};
+
 // Launches of the sorted scan over the planned items: per segment its seed items first (all segments), then the rest,
 // each item writing its k best to its own slot (its index in the work array); then sort_merge_kernel per query.
 int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt,
-                SortJob& J) {
+                SortJob& J, const CountDevOut* dev) {
   const size_t nq = pl.Q.nq;
   const uint32_t k = J.k, cap = J.sink[0].cap;
   size_t total = 0;
@@ -2045,9 +2062,11 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const Cou
   const size_t slots_pos = slot_off_pos + pl.off_bytes;
   const size_t segs_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
   const size_t bytes = segs_pos + n_segs * sizeof(SortSegDev);
-  int rc = ensure_pinned(c, bytes);
+  std::vector<char> staging;   // device mode's pageable staging
+  int rc = dev ? SDBG_OK : ensure_pinned(c, bytes);
   if (rc) return rc;
-  char* h = static_cast<char*>(c->h_pinned);
+  if (dev) staging.resize(bytes);
+  char* h = dev ? staging.data() : static_cast<char*>(c->h_pinned);
   pl.write(h);
   auto* hw = reinterpret_cast<uint4*>(h + pl.work_pos);
   auto* h_slot_off = reinterpret_cast<uint32_t*>(h + slot_off_pos);
@@ -2120,6 +2139,13 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const Cou
   sort_merge_kernel<<<unsigned(nq), 256, smem, c->stream>>>(M);
   ++c->launches;
   CU(c, cudaGetLastError());
+  if (dev) {
+    sort_dist_rows_kernel<<<unsigned(nq), 256, 0, c->stream>>>(M.out, M.n_out, M.segs, k, M.type, J.sink[0].desc, M.nulls_first,
+                                                               dev->rank, dev->counts, static_cast<SortDistRow*>(dev->bins));
+    ++c->launches;
+    CU(c, cudaGetLastError());
+    return SDBG_OK;
+  }
   // scan statistics of the last sorted scan: windows judged (host) / skipped (device word, as GROUP BY leaves it)
   if (!c->d_zone_skipped) CU(c, cudaMalloc(reinterpret_cast<void**>(&c->d_zone_skipped), 8));
   CU(c, cudaMemcpyAsync(c->d_zone_skipped, stats + 1, 8, cudaMemcpyDeviceToDevice, c->stream));
@@ -2133,9 +2159,10 @@ int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const Cou
 }
 
 int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_t>& Q, const sdbg_col_pred* filt,
-              uint64_t* counts, SortJob* sort = nullptr, FacetJob* facet = nullptr, AggJob* agg = nullptr) {
+              uint64_t* counts, SortJob* sort = nullptr, FacetJob* facet = nullptr, AggJob* agg = nullptr,
+              const CountDevOut* dev = nullptr) {
   const auto& [kind, terms, term_off, nq, excl_terms, excl_off, term_grp] = Q;
-  if (!segs || !n_segs || !terms || !term_off || !nq || (!counts && !sort && !facet && !agg)) return SDBG_EINVAL;
+  if (!segs || !n_segs || !terms || !term_off || !nq || (!counts && !dev && !sort && !facet && !agg)) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   CU(c, cudaSetDevice(c->device));
   uint32_t total_excl = 0;
@@ -2280,12 +2307,15 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
   CountPlan pl{Q, n_pos, total_excl, count_planes(max_min), std::move(lists), std::move(seg_work), std::move(grp_off),
                std::move(grp_end)};
   pl.layout();
-  if (sort) return sort_finish(c, segs, n_segs, pl, filt, *sort);
+  if (sort) return sort_finish(c, segs, n_segs, pl, filt, *sort, dev);
+  if (dev) CU(c, cudaMemcpyAsync(dev->counts, host.data(), nq * 8, cudaMemcpyHostToDevice, c->stream));
   if (total_items) {
     const size_t bytes = pl.staged;
-    int rc = ensure_pinned(c, std::max(bytes, nq * 8));
+    std::vector<char> staging;   // device mode's pageable staging
+    int rc = dev ? SDBG_OK : ensure_pinned(c, std::max(bytes, nq * 8));
     if (rc) return rc;
-    char* h = static_cast<char*>(c->h_pinned);
+    if (dev) staging.resize(bytes);
+    char* h = dev ? staging.data() : static_cast<char*>(c->h_pinned);
     pl.write(h);
     DevBuf& b_desc = c->scratch[0]; DevBuf& b_counts = c->scratch[1];
     // facet pass: b_counts holds [counts | facet counts [nq][span] | NULL counts [nq] | out-of-range word]; aggregate
@@ -2294,10 +2324,14 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
     const size_t fc_pos = nq * 8, fn_pos = fc_pos + nq * span * cell, oor_pos = fn_pos + nq * cell;
     const size_t out_bytes = facet || agg ? oor_pos + 8 : nq * 8;
     if ((rc = ensure(c, b_desc, bytes))) return rc;
-    if ((rc = ensure(c, b_counts, out_bytes))) return rc;
+    if (!dev && (rc = ensure(c, b_counts, out_bytes))) return rc;
     CU(c, cudaMemcpyAsync(b_desc.p, h, bytes, cudaMemcpyHostToDevice, c->stream));
-    CU(c, cudaMemsetAsync(b_counts.p, 0, out_bytes, c->stream));
+    if (!dev) CU(c, cudaMemsetAsync(b_counts.p, 0, out_bytes, c->stream));
     char* fo = static_cast<char*>(b_counts.p);
+    auto* d_counts = dev ? dev->counts : static_cast<unsigned long long*>(b_counts.p);
+    char* d_bins = dev ? static_cast<char*>(dev->bins) : fo + fc_pos;
+    char* d_nulls = dev ? static_cast<char*>(dev->nulls) : fo + fn_pos;
+    auto* d_oor = dev ? dev->oor : reinterpret_cast<unsigned int*>(fo + oor_pos);
     // the facet bins, then for groups that need m >= 2 of their lists a bit-sliced counter of bits(m) planes for the
     // batch's largest m (at most 128 + 32 KB)
     const auto [kernel, smem] = facet ? pl.kernel(CountMode::facet, (size_t(facet->span) * 4 + 15) & ~size_t(15))
@@ -2311,24 +2345,25 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
       if (!n) continue;
       CountParams P;
       if ((rc = pl.params(d, segs[si], si, done, filt, &P))) return rc;
-      P.counts = static_cast<unsigned long long*>(b_counts.p);
+      P.counts = d_counts;
       done += n;
       if (facet) {
         P.facet = facet->sink[si];
-        P.facet.counts = reinterpret_cast<unsigned long long*>(fo + fc_pos);
-        P.facet.nulls = reinterpret_cast<unsigned long long*>(fo + fn_pos);
-        P.facet.out_of_range = reinterpret_cast<unsigned int*>(fo + oor_pos);
+        P.facet.counts = reinterpret_cast<unsigned long long*>(d_bins);
+        P.facet.nulls = reinterpret_cast<unsigned long long*>(d_nulls);
+        P.facet.out_of_range = d_oor;
       }
       if (agg) {
         P.agg = agg->sink[si];
-        P.agg.cells = reinterpret_cast<AggCell*>(fo + fc_pos);
-        P.agg.nulls = reinterpret_cast<AggCell*>(fo + fn_pos);
-        P.agg.out_of_range = reinterpret_cast<unsigned int*>(fo + oor_pos);
+        P.agg.cells = reinterpret_cast<AggCell*>(d_bins);
+        P.agg.nulls = reinterpret_cast<AggCell*>(d_nulls);
+        P.agg.out_of_range = d_oor;
       }
       kernel<<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
       ++c->launches;
     }
     CU(c, cudaGetLastError());
+    if (dev) return SDBG_OK;
     if (facet) {
       unsigned int oor = 0;
       CU(c, cudaMemcpyAsync(facet->counts, fo + fc_pos, nq * size_t(facet->span) * 8, cudaMemcpyDeviceToHost, c->stream));
@@ -2356,6 +2391,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
     const auto* dc = reinterpret_cast<const unsigned long long*>(h);
     for (size_t q = 0; q < nq; ++q) host[q] += dc[q];
   }
+  if (dev) return SDBG_OK;
   if (facet) {   // no query matches anywhere
     std::memset(facet->counts, 0, nq * size_t(facet->span) * 8);
     std::memset(facet->null_counts, 0, nq * 8);
@@ -2486,6 +2522,385 @@ extern "C" int sdbg_match_aggregate_batch_groups_min(sdbg_segment* const* segs, 
                                static_cast<sdbg_match_agg*>(r[0].p), static_cast<sdbg_match_agg*>(r[1].p), {}};
                       return count_run(segs, n_segs, Q, filt, nullptr, nullptr, nullptr, &J);
                     });
+}
+
+// ---- the count, facet and aggregate passes across GPUs ----
+namespace {
+// dst row to[j] = src row j, rows of row_words words.
+__global__ void __launch_bounds__(256) scatter_rows_kernel(const unsigned long long* __restrict__ src,
+                                                           unsigned long long* __restrict__ dst, const uint32_t* __restrict__ to,
+                                                           size_t n_rows, size_t row_words) {
+  const size_t n = n_rows * row_words;
+  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
+    const size_t j = i / row_words;
+    dst[size_t(to[j]) * row_words + (i - j * row_words)] = src[i];
+  }
+}
+
+// run_groups for count_run's device mode: rows[i] are device arrays (bytes a multiple of 8). A batch of one shape writes
+// straight into them; otherwise each shape writes zeroed rows of its own (c->dist[2]), which scatter_rows_kernel moves
+// to the caller's query positions on the stream. Nothing waits.
+template <size_t N, class Run>
+int run_groups_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* group_off,
+                      const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                      const uint32_t* excl_off, const sdbg_col_pred* filt, const OutRows (&rows)[N], Run run) {
+  sdbg_ctx* c = segs[0]->ctx;
+  GroupSplit<uint32_t> S;
+  if (int rc = split_groups(c, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
+  for (int sh = 0; sh < 3; ++sh) {
+    uint32_t total_excl = 0;
+    if (!S.qs[sh].empty())
+      if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &total_excl)) return rc;
+  }
+  for (int sh = 0; sh < 3; ++sh)
+    if (S.qs[sh].size() == nq) return run(S.view(sh), rows);
+  // per shape: its query positions (u32, padded to 8 B), then its rows
+  size_t pos[3] = {}, bytes = 0;
+  for (int sh = 0; sh < 3; ++sh) {
+    pos[sh] = bytes;
+    bytes += (S.qs[sh].size() * 4 + 7) & ~size_t(7);
+    for (size_t i = 0; i < N; ++i) bytes += S.qs[sh].size() * rows[i].bytes;
+  }
+  if (int rc = ensure(c, c->dist[2], bytes)) return rc;
+  char* d = static_cast<char*>(c->dist[2].p);
+  CU(c, cudaMemsetAsync(d, 0, bytes, c->stream));
+  for (int sh = 0; sh < 3; ++sh) {
+    std::vector<uint32_t> at(S.qs[sh].begin(), S.qs[sh].end());
+    if (!at.empty())   // pageable: consumed on return
+      CU(c, cudaMemcpyAsync(d + pos[sh], at.data(), at.size() * 4, cudaMemcpyHostToDevice, c->stream));
+  }
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    if (!n) continue;
+    OutRows part[N];
+    char* p = d + pos[sh] + ((n * 4 + 7) & ~size_t(7));
+    for (size_t i = 0; i < N; ++i) { part[i] = {p, rows[i].bytes}; p += n * rows[i].bytes; }
+    if (int rc = run(S.view(sh), part)) return rc;
+    for (size_t i = 0; i < N; ++i) {
+      const size_t words = rows[i].bytes / 8;
+      const unsigned grid = unsigned(std::min<size_t>((n * words + 255) / 256, size_t(c->sm_count) * 8));
+      scatter_rows_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const unsigned long long*>(part[i].p),
+                                                       static_cast<unsigned long long*>(rows[i].p),
+                                                       reinterpret_cast<const uint32_t*>(d + pos[sh]), n, words);
+      ++c->launches;
+    }
+    CU(c, cudaGetLastError());
+  }
+  return SDBG_OK;
+}
+
+// The dist entries' checks of the call's scalar arguments, which fail alike on every rank: before anything is queued.
+int dist_check(sdbg_segment* const* segs, size_t n_segs, const uint32_t* group_off, const uint32_t* query_group_off, size_t nq) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (c->dist_world > 1 && !c->nccl_comm) return fail(c, SDBG_EINVAL, "sdbg_dist_init has not run");
+  return SDBG_OK;
+}
+
+// All-reduces `words` int64 words of this rank's buffer, whose last word is its failure flag, and copies them to the
+// pinned staging: the call's one wait. rc_local: this rank's local pass. A flag set on any rank fails the call on every
+// rank: the failing rank returns its own code, the others SDBG_EINVAL.
+int dist_reduce_to_host(sdbg_ctx* c, int rc_local, unsigned long long* d, size_t words) {
+  if (rc_local) CU(c, cudaMemsetAsync(d + words - 1, 1, 1, c->stream));
+  if (int rc = sdbg_dist_allreduce_i64(c, d, words)) return rc_local ? rc_local : rc;
+  if (int rc = ensure_pinned(c, words * 8)) return rc;
+  CU(c, cudaMemcpyAsync(c->h_pinned, d, words * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  if (rc_local) return rc_local;
+  if (static_cast<const unsigned long long*>(c->h_pinned)[words - 1]) return fail(c, SDBG_EINVAL, "the call failed on another rank");
+  return SDBG_OK;
+}
+
+// The aggregate device form's buffer: this header, then AggCell [nq][span], then AggCell [nq] for the NULL key.
+struct AggDistHeader {
+  unsigned long long type;           // the value column's sdbg_type (UINT64_MAX: not found)
+  unsigned long long span, nq;
+  unsigned long long failed;         // non-zero: this rank's local pass failed
+  unsigned long long out_of_range;   // non-zero: a matching doc's key lay outside the range
+  unsigned long long pad[3];
+};
+static_assert(sizeof(AggDistHeader) == 64, "the cells stay 16-byte aligned");
+
+size_t agg_dist_bytes(size_t nq, uint32_t span) { return sizeof(AggDistHeader) + nq * (size_t(span) + 1) * sizeof(AggCell); }
+
+// One thread per (query, key) cell: the cells of ranks 0 .. n_ranks - 1 in rank order. Counts are u64 sums, the integer
+// sum a 128-bit add with its carry, the float64 sum the ranks' partials added in rank order (so every rank computes the
+// same bits), MIN / MAX the maxima of the order keys. Block 0 also checks the headers: status = {headers disagree, some
+// rank failed, some key out of range, the value type}.
+__global__ void __launch_bounds__(256) agg_merge_gathered_kernel(const char* __restrict__ all, size_t rank_bytes, uint32_t n_ranks,
+                                                                 unsigned long long nq, unsigned long long span,
+                                                                 unsigned long long* __restrict__ status, AggCell* __restrict__ out) {
+  const auto* h0 = reinterpret_cast<const AggDistHeader*>(all);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    unsigned long long bad = 0, failed = 0, oor = 0;
+    for (uint32_t r = 0; r < n_ranks; ++r) {
+      const auto* h = reinterpret_cast<const AggDistHeader*>(all + r * rank_bytes);
+      bad |= h->type != h0->type || h->span != span || h->nq != nq;
+      failed |= h->failed;
+      oor |= h->out_of_range;
+    }
+    status[0] = bad; status[1] = failed; status[2] = oor; status[3] = h0->type;
+  }
+  const bool is_f64 = h0->type == SDBG_F64;
+  const unsigned long long n = nq * (span + 1);
+  for (unsigned long long i = blockIdx.x * 256ull + threadIdx.x; i < n; i += gridDim.x * 256ull) {
+    AggCell a = reinterpret_cast<const AggCell*>(all + sizeof(AggDistHeader))[i];
+    for (uint32_t r = 1; r < n_ranks; ++r) {
+      const AggCell b = reinterpret_cast<const AggCell*>(all + r * rank_bytes + sizeof(AggDistHeader))[i];
+      a.count += b.count;
+      if (!b.count_value) continue;
+      a.count_value += b.count_value;
+      if (is_f64) {
+        a.sum_lo = __double_as_longlong(__longlong_as_double(a.sum_lo) + __longlong_as_double(b.sum_lo));
+      } else {
+        const unsigned long long lo = a.sum_lo + b.sum_lo;
+        a.sum_hi += b.sum_hi + (lo < a.sum_lo ? 1ull : 0ull);
+        a.sum_lo = lo;
+      }
+      a.nmin = a.nmin > b.nmin ? a.nmin : b.nmin;
+      a.max = a.max > b.max ? a.max : b.max;
+    }
+    out[i] = a;
+  }
+}
+
+// The aggregate device form after the scalar checks: zeroes the buffer, writes the header, runs the pass into it and, when
+// the pass fails, sets the header's failure word.
+int agg_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* group_off,
+               const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+               const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
+               uint64_t value_field, void* d_buf) {
+  sdbg_ctx* c = segs[0]->ctx;
+  CU(c, cudaSetDevice(c->device));
+  auto* hdr = static_cast<AggDistHeader*>(d_buf);
+  auto* cells = reinterpret_cast<AggCell*>(hdr + 1);
+  AggDistHeader h{};
+  const auto it = segs[0]->cols.find(value_field);
+  h.type = it == segs[0]->cols.end() ? UINT64_MAX : uint64_t(it->second.type);
+  h.span = key_span; h.nq = nq;
+  CU(c, cudaMemsetAsync(d_buf, 0, agg_dist_bytes(nq, key_span), c->stream));
+  CU(c, cudaMemcpyAsync(hdr, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
+  int rc = ensure(c, c->dist[3], nq * 8);
+  if (!rc) rc = run_groups_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                                   {{c->dist[3].p, 8}, {cells, size_t(key_span) * sizeof(AggCell)}, {cells + nq * key_span, sizeof(AggCell)}},
+                                   [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
+                                     AggJob J{{key_field, key_min, key_span, nullptr, nullptr, {}}, value_field, nullptr, nullptr, {}};
+                                     const CountDevOut D{static_cast<unsigned long long*>(r[0].p), r[1].p, r[2].p,
+                                                         reinterpret_cast<unsigned int*>(&hdr->out_of_range)};
+                                     return count_run(segs, n_segs, Q, filt, nullptr, nullptr, nullptr, &J, &D);
+                                   });
+  if (rc) CU(c, cudaMemsetAsync(&hdr->failed, 1, 1, c->stream));
+  return rc;
+}
+}  // namespace
+
+extern "C" int sdbg_dist_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                      const uint32_t* group_off, const uint32_t* query_group_off,
+                                                      const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                      const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
+  if (int rc = dist_check(segs, n_segs, group_off, query_group_off, nq)) return rc;
+  if (!counts) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  CU(c, cudaSetDevice(c->device));
+  // [counts [nq] | failure flag]
+  if (int rc = ensure(c, c->dist[0], (nq + 1) * 8)) return rc;
+  auto* d = static_cast<unsigned long long*>(c->dist[0].p);
+  CU(c, cudaMemsetAsync(d, 0, (nq + 1) * 8, c->stream));
+  const int rc_local = run_groups_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off,
+                                         filt, {{d, 8}}, [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
+                                           const CountDevOut D{static_cast<unsigned long long*>(r[0].p), nullptr, nullptr, nullptr};
+                                           return count_run(segs, n_segs, Q, filt, nullptr, nullptr, nullptr, nullptr, &D);
+                                         });
+  if (int rc = dist_reduce_to_host(c, rc_local, d, nq + 1)) return rc;
+  std::memcpy(counts, c->h_pinned, nq * 8);
+  return SDBG_OK;
+}
+
+extern "C" int sdbg_dist_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                             const uint32_t* group_off, const uint32_t* query_group_off,
+                                                             const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                             const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                                             uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                                             uint64_t* counts, uint64_t* null_counts) {
+  if (int rc = dist_check(segs, n_segs, group_off, query_group_off, nq)) return rc;
+  if (!counts || !null_counts) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (int rc = facet_check_range(c, key_min, key_span)) return rc;
+  CU(c, cudaSetDevice(c->device));
+  // [counts [nq][span] | NULL counts [nq] | out-of-range word | failure flag]
+  const size_t bins = nq * size_t(key_span), words = bins + nq + 2;
+  if (int rc = ensure(c, c->dist[0], words * 8)) return rc;
+  if (int rc = ensure(c, c->dist[3], nq * 8)) return rc;
+  auto* d = static_cast<unsigned long long*>(c->dist[0].p);
+  CU(c, cudaMemsetAsync(d, 0, words * 8, c->stream));
+  const int rc_local = run_groups_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                                         {{c->dist[3].p, 8}, {d, size_t(key_span) * 8}, {d + bins, 8}},
+                                         [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
+                                           FacetJob J{key_field, key_min, key_span, nullptr, nullptr, {}};
+                                           const CountDevOut D{static_cast<unsigned long long*>(r[0].p), r[1].p, r[2].p,
+                                                               reinterpret_cast<unsigned int*>(d + bins + nq)};
+                                           return count_run(segs, n_segs, Q, filt, nullptr, nullptr, &J, nullptr, &D);
+                                         });
+  if (int rc = dist_reduce_to_host(c, rc_local, d, words)) return rc;
+  const auto* h = static_cast<const unsigned long long*>(c->h_pinned);
+  if (h[bins + nq]) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
+  std::memcpy(counts, h, bins * 8);
+  std::memcpy(null_counts, h + bins, nq * 8);
+  return SDBG_OK;
+}
+
+extern "C" int sdbg_match_aggregate_batch_groups_min_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                            const uint32_t* group_off, const uint32_t* query_group_off,
+                                                            const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                            const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                                            uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                                            uint64_t value_field, void* d_cells) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !d_cells) return SDBG_EINVAL;
+  if (int rc = agg_check_range(segs[0]->ctx, key_field, key_min, key_span)) return rc;
+  return agg_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, key_field,
+                    key_min, key_span, value_field, d_cells);
+}
+
+extern "C" int sdbg_match_aggregate_merge_gathered(sdbg_ctx* c, const void* d_all, uint32_t n_ranks, size_t nq, uint32_t key_span,
+                                                   sdbg_match_agg* out, sdbg_match_agg* null_out) {
+  if (!c || !d_all || !n_ranks || !nq || !key_span || !out || !null_out) return SDBG_EINVAL;
+  if (key_span > kAggMaxSpan) return fail(c, SDBG_EUNSUPPORTED, "key_span > 4096");
+  CU(c, cudaSetDevice(c->device));
+  const size_t n = nq * (size_t(key_span) + 1), bytes = 64 + n * sizeof(AggCell);
+  if (int rc = ensure(c, c->dist[3], bytes)) return rc;
+  char* m = static_cast<char*>(c->dist[3].p);
+  const unsigned grid = unsigned(std::max<size_t>(1, std::min<size_t>((n + 255) / 256, size_t(c->sm_count) * 16)));
+  agg_merge_gathered_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const char*>(d_all), agg_dist_bytes(nq, key_span), n_ranks, nq,
+                                                        key_span, reinterpret_cast<unsigned long long*>(m),
+                                                        reinterpret_cast<AggCell*>(m + 64));
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  if (int rc = ensure_pinned(c, bytes)) return rc;
+  CU(c, cudaMemcpyAsync(c->h_pinned, m, bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  const auto* st = static_cast<const unsigned long long*>(c->h_pinned);
+  if (st[0]) return fail(c, SDBG_EINVAL, "the ranks' aggregate headers disagree (value type, key_span or n_queries)");
+  if (st[1]) return fail(c, SDBG_EINVAL, "the aggregate pass failed on a rank");
+  if (st[2]) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
+  const auto* g = reinterpret_cast<const AggCell*>(static_cast<const char*>(c->h_pinned) + 64);
+  const uint32_t type = uint32_t(st[3]);
+  for (size_t i = 0; i < nq * key_span; ++i) out[i] = agg_result(g[i], type);
+  for (size_t q = 0; q < nq; ++q) null_out[q] = agg_result(g[nq * key_span + q], type);
+  return SDBG_OK;
+}
+
+extern "C" int sdbg_dist_match_aggregate_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                          const uint32_t* group_off, const uint32_t* query_group_off,
+                                                          const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                          const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                                          int64_t key_min, uint32_t key_span, uint64_t value_field,
+                                                          sdbg_match_agg* out, sdbg_match_agg* null_out) {
+  if (int rc = dist_check(segs, n_segs, group_off, query_group_off, nq)) return rc;
+  if (!out || !null_out) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (int rc = agg_check_range(c, key_field, key_min, key_span)) return rc;
+  const uint32_t world = uint32_t(c->dist_world);
+  const size_t bytes = agg_dist_bytes(nq, key_span);
+  if (int rc = ensure(c, c->dist[0], bytes)) return rc;
+  if (int rc = ensure(c, c->dist[1], bytes * world)) return rc;
+  const int rc_local = agg_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                                  key_field, key_min, key_span, value_field, c->dist[0].p);
+  if (int rc = sdbg_dist_allgather(c, c->dist[0].p, c->dist[1].p, bytes)) return rc_local ? rc_local : rc;
+  const int rc = sdbg_match_aggregate_merge_gathered(c, c->dist[1].p, world, nq, key_span, out, null_out);
+  return rc_local ? rc_local : rc;
+}
+
+namespace {
+size_t sort_dist_bytes(size_t nq, uint32_t k) { return sizeof(SortDistHeader) + nq * 8 + nq * size_t(k) * sizeof(SortDistRow); }
+
+// The sorted device form after the scalar checks: zeroes the buffer, writes the header, runs the sorted scan into it and,
+// when the scan fails, sets the header's failure word.
+int sort_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* group_off,
+                const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field, int descending, int nulls_first,
+                uint32_t k, uint32_t rank, void* d_buf) {
+  sdbg_ctx* c = segs[0]->ctx;
+  CU(c, cudaSetDevice(c->device));
+  auto* hdr = static_cast<SortDistHeader*>(d_buf);
+  auto* counts = reinterpret_cast<unsigned long long*>(hdr + 1);
+  auto* rows = reinterpret_cast<SortDistRow*>(counts + nq);
+  SortDistHeader h{};
+  const auto it = segs[0]->cols.find(sort_field);
+  h.type = it == segs[0]->cols.end() ? UINT64_MAX : uint64_t(it->second.type);
+  h.desc = descending ? 1u : 0u; h.nulls_first = nulls_first ? 1u : 0u; h.k = k; h.nq = nq;
+  CU(c, cudaMemsetAsync(d_buf, 0, sort_dist_bytes(nq, k), c->stream));
+  CU(c, cudaMemcpyAsync(hdr, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
+  const int rc = run_groups_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                                   {{counts, 8}, {rows, size_t(k) * sizeof(SortDistRow)}},
+                                   [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
+                                     SortJob J{sort_field, descending, nulls_first, k, nullptr, nullptr, {}, {}};
+                                     const CountDevOut D{static_cast<unsigned long long*>(r[0].p), r[1].p, nullptr, nullptr, rank};
+                                     return count_run(segs, n_segs, Q, filt, nullptr, &J, nullptr, nullptr, &D);
+                                   });
+  if (rc) CU(c, cudaMemsetAsync(&hdr->failed, 1, 1, c->stream));
+  return rc;
+}
+}  // namespace
+
+extern "C" int sdbg_match_topk_by_column_batch_groups_min_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                                 const uint32_t* group_off, const uint32_t* query_group_off,
+                                                                 const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                                 const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                                                 uint64_t sort_field, int descending, int nulls_first, uint32_t k,
+                                                                 uint32_t rank, void* d_rows) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !d_rows) return SDBG_EINVAL;
+  if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
+  if (rank > 0x7FFFFFFFu) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "rank >= 2^31");
+  return sort_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, sort_field,
+                     descending, nulls_first, k, rank, d_rows);
+}
+
+extern "C" int sdbg_match_topk_by_column_merge_gathered(sdbg_ctx* c, const void* d_all, uint32_t n_ranks, size_t nq, uint32_t k,
+                                                        sdbg_sort_hit* out, uint32_t* n_out) {
+  if (!c || !d_all || !n_ranks || !nq || !k || !out || !n_out) return SDBG_EINVAL;
+  if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
+  if (nq > 0x7FFFFFFFu) return fail(c, SDBG_EUNSUPPORTED, "more than 2^31 queries");
+  CU(c, cudaSetDevice(c->device));
+  const size_t hits_bytes = nq * size_t(k) * sizeof(SortHitDev), bytes = 64 + hits_bytes + nq * 4;
+  if (int rc = ensure(c, c->dist[3], bytes)) return rc;
+  char* m = static_cast<char*>(c->dist[3].p);
+  const uint32_t cap = std::max(256u, 2u * next_pow2(k));
+  CU(c, fit_dynamic_smem(sort_merge_gathered_kernel, size_t(cap) * 16));
+  sort_merge_gathered_kernel<<<unsigned(nq), 256, size_t(cap) * 16, c->stream>>>(
+      static_cast<const char*>(d_all), sort_dist_bytes(nq, k), n_ranks, uint32_t(nq), k, cap,
+      reinterpret_cast<unsigned long long*>(m), reinterpret_cast<SortHitDev*>(m + 64), reinterpret_cast<uint32_t*>(m + 64 + hits_bytes));
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  if (int rc = ensure_pinned(c, bytes)) return rc;
+  CU(c, cudaMemcpyAsync(c->h_pinned, m, bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  const auto* st = static_cast<const unsigned long long*>(c->h_pinned);
+  if (st[0]) return fail(c, SDBG_EINVAL, "the ranks' sorted-scan headers disagree (sort type, order, k or n_queries)");
+  if (st[1]) return fail(c, SDBG_EINVAL, "the sorted scan failed on a rank");
+  std::memcpy(out, static_cast<const char*>(c->h_pinned) + 64, hits_bytes);
+  std::memcpy(n_out, static_cast<const char*>(c->h_pinned) + 64 + hits_bytes, nq * 4);
+  return SDBG_OK;
+}
+
+extern "C" int sdbg_dist_match_topk_by_column_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                               const uint32_t* group_off, const uint32_t* query_group_off,
+                                                               const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                               const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                                               uint64_t sort_field, int descending, int nulls_first, uint32_t k,
+                                                               sdbg_sort_hit* out, uint32_t* n_out) {
+  if (int rc = dist_check(segs, n_segs, group_off, query_group_off, nq)) return rc;
+  if (!k || !out || !n_out) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
+  const uint32_t world = uint32_t(c->dist_world);
+  const size_t bytes = sort_dist_bytes(nq, k);
+  if (int rc = ensure(c, c->dist[0], bytes)) return rc;
+  if (int rc = ensure(c, c->dist[1], bytes * world)) return rc;
+  const int rc_local = sort_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
+                                   sort_field, descending, nulls_first, k, uint32_t(c->dist_rank), c->dist[0].p);
+  if (int rc = sdbg_dist_allgather(c, c->dist[0].p, c->dist[1].p, bytes)) return rc_local ? rc_local : rc;
+  const int rc = sdbg_match_topk_by_column_merge_gathered(c, c->dist[1].p, world, nq, k, out, n_out);
+  return rc_local ? rc_local : rc;
 }
 
 // Streaming mode (duckdb_search_full_scan.cpp RunStreamingScan :2370-2403; DocIterator::EmitScoredDocs,

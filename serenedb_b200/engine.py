@@ -855,6 +855,136 @@ def ExecuteMatchAggregatesGroups(reader, groups, value_field, key_field=None, ke
                     key_field is not None)
 
 
+def ExecuteDistCountGroupsBatch(reader, queries, filt=None, exclude=None, min_match=None):
+    """ExecuteCountGroupsBatch over the segments of every rank (sdbg_dist_match_count_batch_groups_min): this rank's counts
+    are all-reduced on the device. Every rank makes the call with the same queries; a flat OR is one group per query, a
+    flat AND single-term groups. Returns uint64[Q], the same on every rank."""
+    counts = np.zeros(len(queries), np.uint64)
+    N.check(N.lib().sdbg_dist_match_count_batch_groups_min(_seg_array(reader.segments), len(reader.segments),
+                                                           *_query_args(queries, exclude, min_match, groups=True), _ref(filt),
+                                                           _ptr(counts)), reader.segments[0].ctx._h)
+    return counts
+
+
+def _dist_key_range(key_min, key_span):
+    if key_min is None or key_span is None:   # a per-rank column range would differ between ranks
+        raise ValueError("the dist entries need key_min and key_span: the same range on every rank")
+    return int(key_min), int(key_span)
+
+
+# The dist wrappers check nothing that depends on this rank's segments before the library call: a missing or mistyped
+# column is reported by the call after the collective, on every rank. The column type the results are decoded with is
+# read after the call has succeeded, when every rank's segments are known to hold the column with one type.
+def _value_type(reader, field):
+    vt = reader.segments[0].col_types.get(int(field))
+    if vt is None:   # the values come back as raw bits: their type must be known, not guessed
+        raise ValueError("column %d was not staged through this Segment" % int(field))
+    return vt
+
+
+def ExecuteDistFacetCountsGroupsBatch(reader, queries, key_field, key_min, key_span, filt=None, exclude=None, min_match=None):
+    """ExecuteFacetCountsGroupsBatch over the segments of every rank (sdbg_dist_match_facet_counts_batch_groups_min): the
+    counts are all-reduced on the device. key_min / key_span are required and must be the same on every rank. Returns the
+    dict ExecuteFacetCountsBatch returns."""
+    key_min, key_span = _dist_key_range(key_min, key_span)
+    nq = len(queries)
+    counts = np.zeros((max(nq, 1), max(key_span, 1)), np.uint64)
+    nulls = np.zeros(max(nq, 1), np.uint64)
+    N.check(N.lib().sdbg_dist_match_facet_counts_batch_groups_min(
+        _seg_array(reader.segments), len(reader.segments), *_query_args(queries, exclude, min_match, groups=True),
+        _ref(filt), int(key_field), key_min, key_span, _ptr(counts), _ptr(nulls)), reader.segments[0].ctx._h)
+    return dict(key_min=key_min, counts=counts[:nq], nulls=nulls[:nq])
+
+
+def _dist_agg_key(key_field, key_min, key_span):
+    """(key field, key_min, key_span) of a dist aggregate call; key_field None: one group, (0, 1)."""
+    if key_field is None:
+        return N.UINT64_MAX, 0, 1
+    return (int(key_field),) + _dist_key_range(key_min, key_span)
+
+
+def ExecuteDistMatchAggregatesGroupsBatch(reader, queries, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                                          exclude=None, min_match=None):
+    """ExecuteMatchAggregatesGroupsBatch over the segments of every rank (sdbg_dist_match_aggregate_batch_groups_min): each
+    rank's cells are all-gathered and merged on the device. Grouped, key_min / key_span are required and must be the same
+    on every rank. Returns the dict ExecuteMatchAggregatesBatch returns, the same on every rank."""
+    kf, key_min, key_span = _dist_agg_key(key_field, key_min, key_span)
+    nq = len(queries)
+    out = np.zeros((max(nq, 1), max(key_span, 1)), MATCH_AGG_DTYPE)
+    null_out = np.zeros(max(nq, 1), MATCH_AGG_DTYPE)
+    N.check(N.lib().sdbg_dist_match_aggregate_batch_groups_min(
+        _seg_array(reader.segments), len(reader.segments), *_query_args(queries, exclude, min_match, groups=True),
+        _ref(filt), kf, key_min, key_span, int(value_field), _ptr(out), _ptr(null_out)), reader.segments[0].ctx._h)
+    return _agg_result(out, null_out, nq, key_min, _value_type(reader, value_field))
+
+
+def match_aggregate_device_bytes(nq, key_span=1):
+    """Bytes of one rank's buffer of MatchAggregatesDevice: a 64-byte header and nq * (key_span + 1) cells of 48 bytes."""
+    return 64 + int(nq) * (int(key_span) + 1) * 48
+
+
+def MatchAggregatesDevice(reader, queries, value_field, d_cells_ptr, key_field=None, key_min=None, key_span=None, filt=None,
+                          exclude=None, min_match=None):
+    """This rank's aggregate cells left in HBM at d_cells_ptr (match_aggregate_device_bytes), for an all-gather and
+    merge_aggregates_gathered (sdbg_match_aggregate_batch_groups_min_device). Nothing waits."""
+    kf, key_min, key_span = _dist_agg_key(key_field, key_min, key_span)
+    N.check(N.lib().sdbg_match_aggregate_batch_groups_min_device(
+        _seg_array(reader.segments), len(reader.segments), *_query_args(queries, exclude, min_match, groups=True),
+        _ref(filt), kf, key_min, key_span, int(value_field), C.c_void_p(int(d_cells_ptr))), reader.segments[0].ctx._h)
+
+
+def merge_aggregates_gathered(ctx, d_all_ptr, n_ranks, nq, value_type, key_min=0, key_span=1):
+    """The aggregates of n_ranks ranks' MatchAggregatesDevice buffers, back to back in HBM
+    (sdbg_match_aggregate_merge_gathered). value_type: the value column's type code. Returns the dict
+    ExecuteMatchAggregatesBatch returns."""
+    out = np.zeros((max(int(nq), 1), max(int(key_span), 1)), MATCH_AGG_DTYPE)
+    null_out = np.zeros(max(int(nq), 1), MATCH_AGG_DTYPE)
+    N.check(N.lib().sdbg_match_aggregate_merge_gathered(ctx._h, C.c_void_p(int(d_all_ptr)), int(n_ranks), int(nq), int(key_span),
+                                                        _ptr(out), _ptr(null_out)), ctx._h)
+    return _agg_result(out, null_out, int(nq), key_min, value_type)
+
+
+def ExecuteDistTopKByColumnGroupsBatch(reader, queries, sort_field, k, descending=False, nulls_first=False, filt=None,
+                                       exclude=None, min_match=None):
+    """ExecuteTopKByColumnGroupsBatch over the segments of every rank (sdbg_dist_match_topk_by_column_batch_groups_min):
+    each rank's k best rows are all-gathered and merged on the device. Returns the dict ExecuteTopKByColumnBatch returns,
+    with segs = the rank and docs = the ordinal within the rank + 1; the same on every rank."""
+    nq = len(queries)
+    hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
+    n_out = np.zeros(max(nq, 1), np.uint32)
+    N.check(N.lib().sdbg_dist_match_topk_by_column_batch_groups_min(
+        _seg_array(reader.segments), len(reader.segments), *_query_args(queries, exclude, min_match, groups=True),
+        _ref(filt), int(sort_field), int(bool(descending)), int(bool(nulls_first)), int(k), _ptr(hits), _ptr(n_out)),
+        reader.segments[0].ctx._h)
+    return _sort_result(hits, n_out, nq, k, _SORT_VALUE_DTYPE[_value_type(reader, sort_field)])
+
+
+def topk_by_column_device_bytes(nq, k):
+    """Bytes of one rank's buffer of TopKByColumnDevice: a 64-byte header, nq row counts and nq * k rows of 24 bytes."""
+    return 64 + int(nq) * (8 + 24 * int(k))
+
+
+def TopKByColumnDevice(reader, queries, sort_field, k, rank, d_rows_ptr, descending=False, nulls_first=False, filt=None,
+                       exclude=None, min_match=None):
+    """This rank's k best rows per query left in HBM at d_rows_ptr (topk_by_column_device_bytes), for an all-gather and
+    merge_topk_by_column_gathered (sdbg_match_topk_by_column_batch_groups_min_device)."""
+    N.check(N.lib().sdbg_match_topk_by_column_batch_groups_min_device(
+        _seg_array(reader.segments), len(reader.segments), *_query_args(queries, exclude, min_match, groups=True),
+        _ref(filt), int(sort_field), int(bool(descending)), int(bool(nulls_first)), int(k), int(rank),
+        C.c_void_p(int(d_rows_ptr))), reader.segments[0].ctx._h)
+
+
+def merge_topk_by_column_gathered(ctx, d_all_ptr, n_ranks, nq, k, value_type):
+    """The sorted hits of n_ranks ranks' TopKByColumnDevice buffers, back to back in HBM
+    (sdbg_match_topk_by_column_merge_gathered). value_type: the sort column's type code. Returns the dict
+    ExecuteTopKByColumnBatch returns, with segs = the rank and docs = the ordinal within the rank + 1."""
+    hits = np.zeros(max(int(nq), 1) * max(int(k), 1), SORT_HIT_DTYPE)
+    n_out = np.zeros(max(int(nq), 1), np.uint32)
+    N.check(N.lib().sdbg_match_topk_by_column_merge_gathered(ctx._h, C.c_void_p(int(d_all_ptr)), int(n_ranks), int(nq), int(k),
+                                                             _ptr(hits), _ptr(n_out)), ctx._h)
+    return _sort_result(hits, n_out, int(nq), int(k), _SORT_VALUE_DTYPE[value_type])
+
+
 FOR_BLOCK_DTYPE =np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])
 
 
