@@ -254,7 +254,9 @@ int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, c
  * Device scratch: k keys of 16 B per work item before the per-query merge, where a work item is a range of 65 536-doc
  * windows of one query in one segment (at least one per query and segment holding a match, at most 2 x SMs), plus
  * n_queries * k * 24 B of hits: 4096 queries x 1 segment x 1 item at k = 1000 take 66 MB; k = 4096 over 20 segments
- * with one item each takes 5.4 GB. Split larger batches. */
+ * with one item each takes 5.4 GB. The hits come back through as much pinned host memory. A mixed-shape batch of the
+ * groups entry below holds its per-shape rows in HBM (the same bytes again) before they go to query order. Split larger
+ * batches. */
 typedef struct { int64_t value; uint32_t doc; uint32_t seg; uint8_t is_null; } sdbg_sort_hit;
 int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
                                     const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms,
@@ -274,7 +276,9 @@ int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, in
  * key column: SDBG_ENOTFOUND; a float64 key column, or key_span > 32768 (each CTA keeps key_span u32 bins in shared
  * memory): SDBG_EUNSUPPORTED. Found after the scan: a counted doc whose key lies outside [key_min, key_min + key_span):
  * SDBG_EINVAL, and the outputs are unspecified. Synchronous on the context's stream.
- * Device scratch: n_queries * key_span * 8 B + n_queries * 8 B (4096 queries x 2001 keys: 66 MB). Split larger batches. */
+ * Device scratch: n_queries * key_span * 8 B + n_queries * 8 B (4096 queries x 2001 keys: 66 MB), and as much pinned
+ * host memory for the copy back; a mixed-shape batch of the groups entry below holds its per-shape rows in HBM (the same
+ * bytes again) before they go to query order. Split larger batches. */
 int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
                                   const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms,
                                   const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
@@ -375,7 +379,8 @@ int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n
  * cells of 40 B in shared memory): SDBG_EUNSUPPORTED. Found after the scan: a matching doc whose key lies outside
  * [key_min, key_min + key_span): SDBG_EINVAL, and the outputs are unspecified. Synchronous on the context's stream.
  * Device scratch: (n_queries * (key_span + 1)) * 48 B + n_queries * 8 B (4096 queries x 2001 keys: 394 MB), and as
- * much pinned host memory for the copy back. Split larger batches.
+ * much pinned host memory for the copy back; a mixed-shape batch of the groups entry holds its per-shape rows in HBM (the
+ * same bytes again) before they go to query order. Split larger batches.
  * Not supported: several value columns in one call (call once per column), key spans above 4096, float64 keys, HAVING,
  * COUNT(DISTINCT), the top-k and streaming entries. The multi-GPU merge: sdbg_dist_match_aggregate_batch_groups_min. */
 typedef struct {

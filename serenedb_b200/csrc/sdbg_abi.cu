@@ -76,9 +76,9 @@ struct sdbg_ctx {
   std::string err;
   uint64_t launches = 0;
   DevBuf scratch[16];
-  // the full-text dist entries: [0] this rank's buffer, [1] the gathered buffers, [2] per-shape rows of a mixed-shape
-  // batch, [3] the device passes' count scratch and the merged cells
-  DevBuf dist[4];
+  // the full-text count, facet, aggregate and sorted passes: [0] the call's region (a dist rank's buffer), [1] the
+  // gathered buffers, [2] per-shape rows of a mixed-shape batch, [3] count scratch and the merged cells
+  DevBuf pass[4];
   DevBuf stage_raw;          // raw int64 values of a column being packed at staging (reused: restaging allocates nothing)
   void* h_pinned = nullptr;  // pinned host staging for small transfers
   size_t h_pinned_cap = 0;
@@ -248,7 +248,7 @@ extern "C" void sdbg_destroy(sdbg_ctx* c) {
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
   for (auto& b : c->scratch) if (b.p) cudaFree(b.p);
-  for (auto& b : c->dist) if (b.p) cudaFree(b.p);
+  for (auto& b : c->pass) if (b.p) cudaFree(b.p);
   if (c->stage_raw.p) cudaFree(c->stage_raw.p);
   if (c->h_pinned) cudaFreeHost(c->h_pinned);
   if (c->h_oor) cudaFreeHost(c->h_oor);
@@ -1608,10 +1608,12 @@ namespace {
 // entry points' form: terms / term_off / excl_terms / excl_off over its queries, in batch order.
 template <class Term>
 struct GroupSplit {
-  std::vector<size_t> qs[3];
+  std::vector<uint32_t> qs[3];   // the batch positions of each shape's queries
   std::vector<Term> terms[3];
   std::vector<uint32_t> term_off[3], excl_terms[3], excl_off[3];
   std::vector<uint8_t> term_grp[3];
+  uint32_t total_excl[3] = {};   // per shape, as check_query_batch sets it
+  int whole = -1;                 // the shape of a batch of one shape; -1: several
 
   QueryBatch<Term> view(int sh) const {
     return {sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR, terms[sh].data(), term_off[sh].data(), qs[sh].size(),
@@ -1620,16 +1622,19 @@ struct GroupSplit {
   }
 };
 
-// Checks of sdbg_*_batch_groups(_min) beyond check_query_batch (which each sub-batch runs as well) and the split by shape:
+// Splits a batch of sdbg_*_batch_groups(_min) by shape and checks it, every shape included, before anything is queued:
 // non-decreasing query_group_off / group_off / excl_off, 1..16 groups, 1..16 positive terms and at most 16 excluded ones
-// per query, no empty group, no positive term id twice in a query, 1 <= group_min[g] <= the group's size.
+// per query, no empty group, no positive term id twice in a query, 1 <= group_min[g] <= the group's size; then
+// check_query_batch on every shape.
 // group_min (NULL: every group 1) is normalised first: a group that needs all its s terms is s single-term groups, so
 // that a query whose groups then all need 1 term takes the shapes above with exactly their results. The remaining queries
 // (some group needs 2 <= m < s terms, so m <= 15) run with their groups, and each term's tag carries m - 1 in its high
 // nibble (kCheckExcl's comment).
 template <class Term>
-int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, const uint32_t* query_group_off,
-                 const uint32_t* group_min, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, GroupSplit<Term>& S) {
+int split_groups(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* group_off,
+                 const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                 const uint32_t* excl_off, const sdbg_col_pred* filt, GroupSplit<Term>& S) {
+  sdbg_ctx* c = segs[0]->ctx;
   for (size_t q = 0; q < nq; ++q) {
     if (query_group_off[q + 1] < query_group_off[q]) return fail(c, SDBG_EINVAL, "query_group_off must be non-decreasing");
     for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g)
@@ -1671,7 +1676,7 @@ int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, cons
       else { ++n_groups; min_group |= m > 1u; }
     }
     const int sh = min_group ? 2 : n_groups == 1 ? 0 : (t1 - t0 == n_groups ? 1 : 2);
-    S.qs[sh].push_back(q);
+    S.qs[sh].push_back(uint32_t(q));
     uint32_t gi = 0;
     for (uint32_t g = g0; g < g1; ++g) {
       const uint32_t s = group_off[g + 1] - group_off[g], m = group_min ? group_min[g] : 1u;
@@ -1686,6 +1691,11 @@ int split_groups(sdbg_ctx* c, const Term* terms, const uint32_t* group_off, cons
       for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) S.excl_terms[sh].push_back(excl_terms[i]);
     S.excl_off[sh].push_back(uint32_t(S.excl_terms[sh].size()));
   }
+  for (int sh = 0; sh < 3; ++sh) {
+    if (S.qs[sh].empty()) continue;
+    if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &S.total_excl[sh])) return rc;
+    if (S.qs[sh].size() == nq) S.whole = sh;
+  }
   return SDBG_OK;
 }
 
@@ -1695,25 +1705,20 @@ struct OutRows {
   size_t bytes;
 };
 
-// Runs a batch of group queries: splits it by shape, checks every shape before anything is queued, then runs each shape
-// as a batch of the flat form, run(view, rows). A batch of one shape writes straight into the caller's rows; otherwise each
-// shape writes temporary rows, which go to the caller's query positions. Checks of the result that every shape would
-// make alike (k, the key range) are the caller's, before this call.
+// Runs a batch of group top-k queries: splits and checks it (split_groups), then runs each shape as a batch of the flat
+// form, run(view, rows). A batch of one shape writes straight into the caller's rows; otherwise each shape writes
+// temporary rows, which go to the caller's query positions. Checks of the result that every shape would make alike (k)
+// are the caller's, before this call.
 template <class Term, size_t N, class Run>
 int run_groups(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* group_off,
                const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
                const uint32_t* excl_off, const sdbg_col_pred* filt, const OutRows (&rows)[N], Run run) {
   GroupSplit<Term> S;
-  if (int rc = split_groups(segs[0]->ctx, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
+  if (int rc = split_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, S)) return rc;
+  if (S.whole >= 0) return run(S.view(S.whole), rows);
   for (int sh = 0; sh < 3; ++sh) {
-    uint32_t total_excl = 0;
-    if (!S.qs[sh].empty())
-      if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &total_excl)) return rc;
-  }
-  for (int sh = 0; sh < 3; ++sh) {
-    const std::vector<size_t>& qs = S.qs[sh];
+    const std::vector<uint32_t>& qs = S.qs[sh];
     if (qs.empty()) continue;
-    if (qs.size() == nq) return run(S.view(sh), rows);
     std::vector<char> tmp[N];
     OutRows part[N];
     for (size_t i = 0; i < N; ++i) {
@@ -1759,11 +1764,9 @@ extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_s
 // segment without filter, deleted docs or an excluded list holding blocks there is answered from the term's docs_count.
 // Queries of OR groups (Q.term_grp; groups 0 .. n - 1 of a query all present) run the kGroups instantiations
 // (CountPlan::kernel).
-// sort (NULL: count): the sorted scan of sdbg_match_topk_by_column_batch on the same plan, without the single-term
-// shortcut; see sort_prepare / sort_finish.
-// facet (NULL: count): the facet pass of sdbg_match_facet_counts_batch on the same plan and launches, without the
-// single-term shortcut; see facet_prepare.
-// agg (NULL: count): the aggregate pass of sdbg_match_aggregate_batch, the same way; see agg_prepare.
+// The same plan serves three more passes (CountJob), without the single-term shortcut: the sorted scan of
+// sdbg_match_topk_by_column_batch (sort_prepare), the facet pass of sdbg_match_facet_counts_batch
+// (facet_prepare) and the aggregate pass of sdbg_match_aggregate_batch (agg_prepare).
 namespace {
 
 // The facet pass's part of a count_run call.
@@ -1771,8 +1774,6 @@ struct FacetJob {
   uint64_t field;
   int64_t key_min;
   uint32_t span;
-  uint64_t* counts;        // host: [query][span]
-  uint64_t* null_counts;   // host: [query]
   std::vector<FacetSink> sink;   // per segment, filled by facet_prepare (output pointers set at launch)
 };
 
@@ -1809,10 +1810,8 @@ int facet_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, FacetJo
 
 // The aggregate pass's part of a count_run call.
 struct AggJob {
-  FacetJob key;               // key column and range (key.field UINT64_MAX: one group); its host outputs are unused
+  FacetJob key;               // key column and range (key.field UINT64_MAX: one group)
   uint64_t field;             // value column
-  sdbg_match_agg* out;        // host: [query][span]
-  sdbg_match_agg* null_out;   // host: [query]
   std::vector<AggSink> sink;  // per segment, filled by agg_prepare (output pointers set at launch)
 };
 
@@ -1863,13 +1862,17 @@ sdbg_match_agg agg_result(const AggCell& g, uint32_t type) {
   return a;
 }
 
+// The caller's cells from the device's: out [nq][span] from g [nq][span], null_out [nq] from the NULL cells after them.
+void agg_results(const AggCell* g, size_t nq, uint32_t span, uint32_t type, sdbg_match_agg* out, sdbg_match_agg* null_out) {
+  for (size_t i = 0; i < nq * span; ++i) out[i] = agg_result(g[i], type);
+  for (size_t q = 0; q < nq; ++q) null_out[q] = agg_result(g[nq * span + q], type);
+}
+
 // The sorted scan's part of a count_run call.
 struct SortJob {
   uint64_t field;
   int desc, nulls_first;
   uint32_t k;
-  sdbg_sort_hit* out;
-  uint32_t* n_out;
   // filled by sort_prepare
   std::vector<SortSink> sink;                 // per segment (pointers to outputs set at launch)
   std::vector<std::vector<long long>> zone;   // per segment: host copy of the zonemap (empty: no zone pruning there)
@@ -1968,6 +1971,46 @@ uint32_t count_planes(uint32_t max_min) {
 using CountKernel = void (*)(CountParams);
 enum class CountMode { count, sort, facet, agg };
 
+// One pass of count_run: its mode and that mode's parameters. job_prepare checks them and fills the sinks, once per call.
+struct CountJob {
+  CountMode mode;
+  SortJob sort;     // CountMode::sort
+  FacetJob facet;   // CountMode::facet
+  AggJob agg;       // CountMode::agg
+
+  // Bytes per query of count_run's per-query arrays {counts, bins, nulls} (CountOut); rank: the sorted scan's rank form.
+  std::array<size_t, 3> rows(bool rank) const {
+    switch (mode) {
+      case CountMode::sort: return {rank ? 8u : 4u, size_t(sort.k) * (rank ? sizeof(SortDistRow) : sizeof(SortHitDev)), 0};
+      case CountMode::facet: return {8, size_t(facet.span) * 8, 8};
+      case CountMode::agg: return {8, size_t(agg.key.span) * sizeof(AggCell), sizeof(AggCell)};
+      default: return {8, 0, 0};
+    }
+  }
+};
+
+int job_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, CountJob& job) {
+  switch (job.mode) {
+    case CountMode::sort: return sort_prepare(c, segs, n_segs, job.sort);
+    case CountMode::facet: return facet_prepare(c, segs, n_segs, job.facet);
+    case CountMode::agg: return agg_prepare(c, segs, n_segs, job.agg);
+    default: return SDBG_OK;
+  }
+}
+
+// Where count_run leaves a pass's results: device arrays the caller has zeroed, which the pass adds to. Nothing is copied
+// back and nothing waits (the sorted scan's zonemap planning in sort_prepare excepted), so a collective can follow.
+struct CountOut {
+  void* counts;                // [nq]: count u64 counts; facet / aggregate u64 scratch; sorted scan u32 n_out (rank < 0) or
+                               // u64 row counts
+  void* bins;                  // facet u64 [nq][span], aggregate AggCell [nq][span]; sorted scan SortHitDev [nq][k] (rank < 0)
+                               // or SortDistRow [nq][k]
+  void* nulls;                 // facet u64 [nq], aggregate AggCell [nq]
+  unsigned int* oor;           // facet / aggregate: set to 1 when a matching doc's key lies outside the range
+  unsigned long long* stats;   // sorted scan: windows judged / skipped by the zonemaps
+  int64_t rank;                // sorted scan: < 0 hits, else this rank's rows (sort_dist_rows_kernel)
+};
+
 // A count_run plan: per segment each query's lists and the work items; with OR groups (Q.term_grp), each segment's group
 // ends. Its host staging, which every mode shares: [term_off | excl_off | lists per segment | work items {query, first
 // window, windows, 0} | grp_off | group ends per segment]; the sorted scan appends its own arrays.
@@ -1978,6 +2021,8 @@ struct CountPlan {
   std::vector<uint2> lists;                      // per segment: positive lists | excluded lists
   std::vector<std::vector<CountItem>> seg_work;  // per segment
   std::vector<uint32_t> grp_off, grp_end;        // grp_off[q] .. grp_off[q + 1] index each segment's group ends
+  std::vector<uint64_t> host;                    // per query: the counts of the single-term shortcut
+  size_t items = 0;                              // work items over all segments
   size_t off_bytes = 0, lists_pos = 0, work_pos = 0, grp_pos = 0, staged = 0;   // the staging's layout; staged: its bytes
 
   size_t n_lists() const { return size_t(n_pos) + total_excl; }
@@ -2035,144 +2080,13 @@ struct CountPlan {
   }
 };
 
-// Device-output mode of count_run: the results stay in these device arrays, nothing is copied back and nothing waits
-// (the sorted scan's zonemap planning excepted), so a collective can follow on the stream. The plan is staged from
-// pageable memory, which the copy has consumed when it returns, so calls can follow one another without a wait.
-struct CountDevOut {
-  unsigned long long* counts;   // [nq]: the counts (set to the single-term shortcut's, the kernels add theirs); scratch
-                                // for the facet and aggregate passes
-  void* bins;                   // zeroed by the caller: facet u64 [nq][span], aggregate AggCell [nq][span]
-  void* nulls;                  // zeroed by the caller: facet u64 [nq], aggregate AggCell [nq]
-  unsigned int* oor;            // zeroed by the caller: set to 1 when a matching doc's key lies outside the range
-  // the sorted scan: counts holds each query's row count (u64), bins its rows [nq][k] (SortDistRow) for rank `rank`
-  uint32_t rank;
-};
-
-// Launches of the sorted scan over the planned items: per segment its seed items first (all segments), then the rest,
-// each item writing its k best to its own slot (its index in the work array); then sort_merge_kernel per query.
-int sort_finish(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt,
-                SortJob& J, const CountDevOut* dev) {
-  const size_t nq = pl.Q.nq;
-  const uint32_t k = J.k, cap = J.sink[0].cap;
-  size_t total = 0;
-  bool any_zone = false;
-  for (size_t si = 0; si < n_segs; ++si) { total += pl.seg_work[si].size(); any_zone |= J.sink[si].zone != nullptr; }
-  // host staging: the plan's, then [slot_off | slots | segments]
-  const size_t slot_off_pos = pl.staged;
-  const size_t slots_pos = slot_off_pos + pl.off_bytes;
-  const size_t segs_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
-  const size_t bytes = segs_pos + n_segs * sizeof(SortSegDev);
-  std::vector<char> staging;   // device mode's pageable staging
-  int rc = dev ? SDBG_OK : ensure_pinned(c, bytes);
-  if (rc) return rc;
-  if (dev) staging.resize(bytes);
-  char* h = dev ? staging.data() : static_cast<char*>(c->h_pinned);
-  pl.write(h);
-  auto* hw = reinterpret_cast<uint4*>(h + pl.work_pos);
-  auto* h_slot_off = reinterpret_cast<uint32_t*>(h + slot_off_pos);
-  auto* h_slots = reinterpret_cast<uint32_t*>(h + slots_pos);
-  std::fill(h_slot_off, h_slot_off + nq + 1, 0u);
-  for (uint32_t i = 0; i < total; ++i) { hw[i].w = i; ++h_slot_off[hw[i].x + 1]; }
-  for (size_t q = 0; q < nq; ++q) h_slot_off[q + 1] += h_slot_off[q];
-  {
-    std::vector<uint32_t> fillq(h_slot_off, h_slot_off + nq);
-    for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
-  }
-  auto* h_segs = reinterpret_cast<SortSegDev*>(h + segs_pos);
-  for (size_t si = 0; si < n_segs; ++si) {
-    const SortSink& S = J.sink[si];
-    h_segs[si] = SortSegDev{S.values, S.validity, S.rows, S.ordinal_base, 0u};
-  }
-  // device outputs: [item keys | item key counts | thresholds | stats | hits | n_out]
-  const size_t keys_bytes = std::max<size_t>(total, 1) * k * sizeof(ulonglong2);
-  const size_t keys_n_pos = keys_bytes;
-  const size_t thr_pos = (keys_n_pos + std::max<size_t>(total, 1) * 4 + 15) & ~size_t(15);
-  const size_t stats_pos = thr_pos + nq * 8;
-  const size_t hits_pos = (stats_pos + 16 + 15) & ~size_t(15);
-  const size_t n_out_pos = hits_pos + nq * k * sizeof(SortHitDev);
-  const size_t out_bytes = n_out_pos + nq * 4;
-  DevBuf& b_desc = c->scratch[0]; DevBuf& b_out = c->scratch[1];
-  if ((rc = ensure(c, b_desc, bytes))) return rc;
-  if ((rc = ensure(c, b_out, out_bytes))) return rc;
-  char* d = static_cast<char*>(b_desc.p);
-  char* o = static_cast<char*>(b_out.p);
-  auto* thr = reinterpret_cast<unsigned long long*>(o + thr_pos);
-  auto* stats = reinterpret_cast<unsigned long long*>(o + stats_pos);
-  CU(c, cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaMemsetAsync(thr, 0, nq * 8 + 16, c->stream));   // thresholds and stats
-  const size_t smem = size_t(cap) * 16;
-  // groups: the counter planes follow the keys (k = 4096 with 4 planes: 128 + 32 KB)
-  const auto [kernel, kernel_smem] = pl.kernel(CountMode::sort, smem);
-  CU(c, fit_dynamic_smem(kernel, kernel_smem));
-  CU(c, fit_dynamic_smem(sort_merge_kernel, smem));
-  if (total) {
-    for (int phase = 0; phase < 2; ++phase) {   // seeds, then the rest
-      size_t begin = 0;
-      for (size_t si = 0; si < n_segs; ++si) {
-        const auto& w = pl.seg_work[si];
-        const size_t n_seed = size_t(std::count_if(w.begin(), w.end(), [](const CountItem& x) { return x.seed; }));
-        const size_t first = begin + (phase ? n_seed : 0), n = phase ? w.size() - n_seed : n_seed;
-        begin += w.size();
-        if (!n) continue;
-        CountParams P;
-        if ((rc = pl.params(d, segs[si], si, first, filt, &P))) return rc;
-        P.counts = nullptr;
-        P.sort = J.sink[si];
-        P.sort.thr = c->wand ? thr : nullptr;
-        P.sort.out = reinterpret_cast<ulonglong2*>(o);
-        P.sort.out_n = reinterpret_cast<uint32_t*>(o + keys_n_pos);
-        P.sort.stats = stats;
-        kernel<<<unsigned(n), kCountThreads, kernel_smem, c->stream>>>(P);
-        ++c->launches;
-      }
-    }
-  }
-  SortMergeParams M;
-  M.keys = reinterpret_cast<const ulonglong2*>(o);
-  M.keys_n = reinterpret_cast<const uint32_t*>(o + keys_n_pos);
-  M.slot_off = reinterpret_cast<const uint32_t*>(d + slot_off_pos);
-  M.slots = reinterpret_cast<const uint32_t*>(d + slots_pos);
-  M.segs = reinterpret_cast<const SortSegDev*>(d + segs_pos);
-  M.n_segs = uint32_t(n_segs); M.type = J.sink[0].type; M.nulls_first = J.sink[0].nulls_first; M.k = k; M.cap = cap;
-  M.out = reinterpret_cast<SortHitDev*>(o + hits_pos);
-  M.n_out = reinterpret_cast<uint32_t*>(o + n_out_pos);
-  sort_merge_kernel<<<unsigned(nq), 256, smem, c->stream>>>(M);
-  ++c->launches;
-  CU(c, cudaGetLastError());
-  if (dev) {
-    sort_dist_rows_kernel<<<unsigned(nq), 256, 0, c->stream>>>(M.out, M.n_out, M.segs, k, M.type, J.sink[0].desc, M.nulls_first,
-                                                               dev->rank, dev->counts, static_cast<SortDistRow*>(dev->bins));
-    ++c->launches;
-    CU(c, cudaGetLastError());
-    return SDBG_OK;
-  }
-  // scan statistics of the last sorted scan: windows judged (host) / skipped (device word, as GROUP BY leaves it)
-  if (!c->d_zone_skipped) CU(c, cudaMalloc(reinterpret_cast<void**>(&c->d_zone_skipped), 8));
-  CU(c, cudaMemcpyAsync(c->d_zone_skipped, stats + 1, 8, cudaMemcpyDeviceToDevice, c->stream));
-  unsigned long long judged = 0;
-  CU(c, cudaMemcpyAsync(&judged, stats, 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaMemcpyAsync(J.out, o + hits_pos, nq * k * sizeof(SortHitDev), cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaMemcpyAsync(J.n_out, o + n_out_pos, nq * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  c->zone_blocks_total = any_zone ? judged : 0;
-  return SDBG_OK;
-}
-
-int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_t>& Q, const sdbg_col_pred* filt,
-              uint64_t* counts, SortJob* sort = nullptr, FacetJob* facet = nullptr, AggJob* agg = nullptr,
-              const CountDevOut* dev = nullptr) {
+// The plan of a batch checked by check_query_batch (total_excl: what it set) for a prepared job (job_prepare), on the
+// host: queues nothing.
+CountPlan count_plan(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_t>& Q, uint32_t total_excl,
+                     const sdbg_col_pred* filt, const CountJob& job) {
   const auto& [kind, terms, term_off, nq, excl_terms, excl_off, term_grp] = Q;
-  if (!segs || !n_segs || !terms || !term_off || !nq || (!counts && !dev && !sort && !facet && !agg)) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
-  CU(c, cudaSetDevice(c->device));
-  uint32_t total_excl = 0;
-  if (int rc = check_query_batch(segs, n_segs, Q, filt, &total_excl)) return rc;
-  if (sort)
-    if (int rc = sort_prepare(c, segs, n_segs, *sort)) return rc;
-  if (facet)
-    if (int rc = facet_prepare(c, segs, n_segs, *facet)) return rc;
-  if (agg)
-    if (int rc = agg_prepare(c, segs, n_segs, *agg)) return rc;
+  const SortJob* sort = job.mode == CountMode::sort ? &job.sort : nullptr;
   const bool conj = kind == SDBG_QUERY_AND;
   const uint32_t n_pos = term_off[nq];
   const size_t n_lists = size_t(n_pos) + total_excl;   // per segment: positive lists | excluded lists
@@ -2279,7 +2193,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
         bool excl_blocks = false;
         if (total_excl)
           for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) excl_blocks |= L[n_pos + i].y != 0;
-        if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks && !sort && !facet && !agg) { host[q] += sum; continue; }
+        if (t1 - t0 == 1 && !filt && !s->d_deleted && !excl_blocks && job.mode == CountMode::count) { host[q] += sum; continue; }
         weight = conj ? uint64_t(smallest) * (t1 - t0) : sum;
       }
       uint32_t g = uint32_t(std::max<uint64_t>(G, (weight + chain_target - 1) / chain_target));
@@ -2305,112 +2219,339 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_
     total_items += seg_work[si].size();
   }
   CountPlan pl{Q, n_pos, total_excl, count_planes(max_min), std::move(lists), std::move(seg_work), std::move(grp_off),
-               std::move(grp_end)};
+               std::move(grp_end), std::move(host), total_items};
   pl.layout();
-  if (sort) return sort_finish(c, segs, n_segs, pl, filt, *sort, dev);
-  if (dev) CU(c, cudaMemcpyAsync(dev->counts, host.data(), nq * 8, cudaMemcpyHostToDevice, c->stream));
-  if (total_items) {
-    const size_t bytes = pl.staged;
-    std::vector<char> staging;   // device mode's pageable staging
-    int rc = dev ? SDBG_OK : ensure_pinned(c, std::max(bytes, nq * 8));
-    if (rc) return rc;
-    if (dev) staging.resize(bytes);
-    char* h = dev ? staging.data() : static_cast<char*>(c->h_pinned);
-    pl.write(h);
-    DevBuf& b_desc = c->scratch[0]; DevBuf& b_counts = c->scratch[1];
-    // facet pass: b_counts holds [counts | facet counts [nq][span] | NULL counts [nq] | out-of-range word]; aggregate
-    // pass: the same with cells of sizeof(AggCell) for the counts
-    const size_t cell = agg ? sizeof(AggCell) : 8, span = facet ? facet->span : agg ? agg->key.span : 0;
-    const size_t fc_pos = nq * 8, fn_pos = fc_pos + nq * span * cell, oor_pos = fn_pos + nq * cell;
-    const size_t out_bytes = facet || agg ? oor_pos + 8 : nq * 8;
-    if ((rc = ensure(c, b_desc, bytes))) return rc;
-    if (!dev && (rc = ensure(c, b_counts, out_bytes))) return rc;
-    CU(c, cudaMemcpyAsync(b_desc.p, h, bytes, cudaMemcpyHostToDevice, c->stream));
-    if (!dev) CU(c, cudaMemsetAsync(b_counts.p, 0, out_bytes, c->stream));
-    char* fo = static_cast<char*>(b_counts.p);
-    auto* d_counts = dev ? dev->counts : static_cast<unsigned long long*>(b_counts.p);
-    char* d_bins = dev ? static_cast<char*>(dev->bins) : fo + fc_pos;
-    char* d_nulls = dev ? static_cast<char*>(dev->nulls) : fo + fn_pos;
-    auto* d_oor = dev ? dev->oor : reinterpret_cast<unsigned int*>(fo + oor_pos);
-    // the facet bins, then for groups that need m >= 2 of their lists a bit-sliced counter of bits(m) planes for the
-    // batch's largest m (at most 128 + 32 KB)
-    const auto [kernel, smem] = facet ? pl.kernel(CountMode::facet, (size_t(facet->span) * 4 + 15) & ~size_t(15))
-                                : agg ? pl.kernel(CountMode::agg, agg_cells_bytes(agg->key.span))
-                                      : pl.kernel(CountMode::count, 0);
-    CU(c, fit_dynamic_smem(kernel, smem));
-    const char* d = static_cast<const char*>(b_desc.p);
-    size_t done = 0;
+  return pl;
+}
+
+// Queues a pass over its plan into out. A count pass first sets out.counts to the single-term shortcut's counts. The
+// sorted scan launches per segment its seed items first (all segments), then the rest, each item writing its k best to
+// its own slot (its index in the work array); then sort_merge_kernel per query, and for a rank sort_dist_rows_kernel.
+// The plan is staged from pageable memory, which the copy has consumed when it returns, so calls can follow one another
+// without a wait (a host group entry queues its shapes back to back).
+int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt, const CountJob& job,
+              const CountOut& out) {
+  sdbg_ctx* c = segs[0]->ctx;
+  const size_t nq = pl.Q.nq, total = pl.items;
+  const bool sort = job.mode == CountMode::sort;
+  if (std::any_of(pl.host.begin(), pl.host.end(), [](uint64_t v) { return v != 0; }))   // else out.counts is zero already
+    CU(c, cudaMemcpyAsync(out.counts, pl.host.data(), nq * 8, cudaMemcpyHostToDevice, c->stream));
+  if (!total && !sort) return SDBG_OK;
+  const SortJob& J = job.sort;
+  const uint32_t k = J.k, cap = sort ? J.sink[0].cap : 0u;
+  // host staging: the plan's, then for the sorted scan [slot_off | slots | segments]
+  const size_t slot_off_pos = pl.staged;
+  const size_t slots_pos = slot_off_pos + pl.off_bytes;
+  const size_t segs_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
+  const size_t bytes = sort ? segs_pos + n_segs * sizeof(SortSegDev) : pl.staged;
+  std::vector<char> staging(bytes);
+  char* h = staging.data();
+  pl.write(h);
+  if (sort) {
+    auto* hw = reinterpret_cast<uint4*>(h + pl.work_pos);
+    auto* h_slot_off = reinterpret_cast<uint32_t*>(h + slot_off_pos);
+    auto* h_slots = reinterpret_cast<uint32_t*>(h + slots_pos);
+    std::fill(h_slot_off, h_slot_off + nq + 1, 0u);
+    for (uint32_t i = 0; i < total; ++i) { hw[i].w = i; ++h_slot_off[hw[i].x + 1]; }
+    for (size_t q = 0; q < nq; ++q) h_slot_off[q + 1] += h_slot_off[q];
+    std::vector<uint32_t> fillq(h_slot_off, h_slot_off + nq);
+    for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
+    auto* h_segs = reinterpret_cast<SortSegDev*>(h + segs_pos);
     for (size_t si = 0; si < n_segs; ++si) {
-      const size_t n = pl.seg_work[si].size();
+      const SortSink& S = J.sink[si];
+      h_segs[si] = SortSegDev{S.values, S.validity, S.rows, S.ordinal_base, 0u};
+    }
+  }
+  // the sorted scan's device scratch: [item keys | item key counts | thresholds | a rank's hits | its n_out]
+  const size_t keys_n_pos = std::max<size_t>(total, 1) * k * sizeof(ulonglong2);
+  const size_t thr_pos = (keys_n_pos + std::max<size_t>(total, 1) * 4 + 15) & ~size_t(15);
+  const size_t hits_pos = (thr_pos + nq * 8 + 15) & ~size_t(15);
+  const size_t n_out_pos = hits_pos + nq * k * sizeof(SortHitDev);
+  DevBuf& b_desc = c->scratch[0]; DevBuf& b_out = c->scratch[1];
+  if (int rc = ensure(c, b_desc, bytes)) return rc;
+  if (int rc = sort ? ensure(c, b_out, out.rank < 0 ? hits_pos : n_out_pos + nq * 4) : SDBG_OK) return rc;
+  char* d = static_cast<char*>(b_desc.p);
+  char* o = static_cast<char*>(b_out.p);
+  auto* thr = reinterpret_cast<unsigned long long*>(o + thr_pos);
+  CU(c, cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, c->stream));
+  if (sort) CU(c, cudaMemsetAsync(thr, 0, nq * 8, c->stream));
+  // the sorted keys, facet bins or aggregate cells, then for groups that need m >= 2 of their lists a bit-sliced counter
+  // of bits(m) planes for the batch's largest m (at most 128 + 32 KB)
+  const size_t mode_bytes = sort ? size_t(cap) * 16
+                            : job.mode == CountMode::facet ? (size_t(job.facet.span) * 4 + 15) & ~size_t(15)
+                            : job.mode == CountMode::agg   ? agg_cells_bytes(job.agg.key.span)
+                                                           : 0;
+  const auto [kernel, smem] = pl.kernel(job.mode, mode_bytes);
+  CU(c, fit_dynamic_smem(kernel, smem));
+  for (int phase = 0; phase < 2; ++phase) {   // seeds (sorted scan only), then the rest
+    size_t begin = 0;
+    for (size_t si = 0; si < n_segs; ++si) {
+      const auto& w = pl.seg_work[si];
+      const size_t n_seed = size_t(std::count_if(w.begin(), w.end(), [](const CountItem& x) { return x.seed; }));
+      const size_t first = begin + (phase ? n_seed : 0), n = phase ? w.size() - n_seed : n_seed;
+      begin += w.size();
       if (!n) continue;
       CountParams P;
-      if ((rc = pl.params(d, segs[si], si, done, filt, &P))) return rc;
-      P.counts = d_counts;
-      done += n;
-      if (facet) {
-        P.facet = facet->sink[si];
-        P.facet.counts = reinterpret_cast<unsigned long long*>(d_bins);
-        P.facet.nulls = reinterpret_cast<unsigned long long*>(d_nulls);
-        P.facet.out_of_range = d_oor;
+      if (int rc = pl.params(d, segs[si], si, first, filt, &P)) return rc;
+      P.counts = static_cast<unsigned long long*>(out.counts);
+      if (sort) {
+        P.counts = nullptr;
+        P.sort = J.sink[si];
+        P.sort.thr = c->wand ? thr : nullptr;
+        P.sort.out = reinterpret_cast<ulonglong2*>(o);
+        P.sort.out_n = reinterpret_cast<uint32_t*>(o + keys_n_pos);
+        P.sort.stats = out.stats;
       }
-      if (agg) {
-        P.agg = agg->sink[si];
-        P.agg.cells = reinterpret_cast<AggCell*>(d_bins);
-        P.agg.nulls = reinterpret_cast<AggCell*>(d_nulls);
-        P.agg.out_of_range = d_oor;
+      if (job.mode == CountMode::facet) {
+        P.facet = job.facet.sink[si];
+        P.facet.counts = static_cast<unsigned long long*>(out.bins);
+        P.facet.nulls = static_cast<unsigned long long*>(out.nulls);
+        P.facet.out_of_range = out.oor;
+      }
+      if (job.mode == CountMode::agg) {
+        P.agg = job.agg.sink[si];
+        P.agg.cells = static_cast<AggCell*>(out.bins);
+        P.agg.nulls = static_cast<AggCell*>(out.nulls);
+        P.agg.out_of_range = out.oor;
       }
       kernel<<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
       ++c->launches;
     }
-    CU(c, cudaGetLastError());
-    if (dev) return SDBG_OK;
-    if (facet) {
-      unsigned int oor = 0;
-      CU(c, cudaMemcpyAsync(facet->counts, fo + fc_pos, nq * size_t(facet->span) * 8, cudaMemcpyDeviceToHost, c->stream));
-      CU(c, cudaMemcpyAsync(facet->null_counts, fo + fn_pos, nq * 8, cudaMemcpyDeviceToHost, c->stream));
-      CU(c, cudaMemcpyAsync(&oor, fo + oor_pos, 4, cudaMemcpyDeviceToHost, c->stream));
-      CU(c, cudaStreamSynchronize(c->stream));
-      if (oor) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
-      return SDBG_OK;
-    }
-    if (agg) {   // cells, NULL cells and the out-of-range word in one copy, into the pinned staging (the plan is on the device)
-      if ((rc = ensure_pinned(c, out_bytes - fc_pos))) return rc;
-      const auto* g = static_cast<const AggCell*>(c->h_pinned);
-      CU(c, cudaMemcpyAsync(c->h_pinned, fo + fc_pos, out_bytes - fc_pos, cudaMemcpyDeviceToHost, c->stream));
-      CU(c, cudaStreamSynchronize(c->stream));
-      unsigned int oor = 0;
-      std::memcpy(&oor, static_cast<const char*>(c->h_pinned) + (oor_pos - fc_pos), 4);
-      if (oor) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
-      const uint32_t type = agg->sink[0].type;
-      for (size_t i = 0; i < nq * span; ++i) agg->out[i] = agg_result(g[i], type);
-      for (size_t q = 0; q < nq; ++q) agg->null_out[q] = agg_result(g[nq * span + q], type);
-      return SDBG_OK;
-    }
-    CU(c, cudaMemcpyAsync(h, b_counts.p, nq * 8, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    const auto* dc = reinterpret_cast<const unsigned long long*>(h);
-    for (size_t q = 0; q < nq; ++q) host[q] += dc[q];
   }
-  if (dev) return SDBG_OK;
-  if (facet) {   // no query matches anywhere
-    std::memset(facet->counts, 0, nq * size_t(facet->span) * 8);
-    std::memset(facet->null_counts, 0, nq * 8);
-    return SDBG_OK;
-  }
-  if (agg) {
-    std::memset(agg->out, 0, nq * size_t(agg->key.span) * sizeof(sdbg_match_agg));
-    std::memset(agg->null_out, 0, nq * sizeof(sdbg_match_agg));
-    return SDBG_OK;
-  }
-  std::memcpy(counts, host.data(), nq * 8);
+  CU(c, cudaGetLastError());
+  if (!sort) return SDBG_OK;
+  SortMergeParams M;
+  M.keys = reinterpret_cast<const ulonglong2*>(o);
+  M.keys_n = reinterpret_cast<const uint32_t*>(o + keys_n_pos);
+  M.slot_off = reinterpret_cast<const uint32_t*>(d + slot_off_pos);
+  M.slots = reinterpret_cast<const uint32_t*>(d + slots_pos);
+  M.segs = reinterpret_cast<const SortSegDev*>(d + segs_pos);
+  M.n_segs = uint32_t(n_segs); M.type = J.sink[0].type; M.nulls_first = J.sink[0].nulls_first; M.k = k; M.cap = cap;
+  const bool rank = out.rank >= 0;   // a rank's hits stay in the scratch and become its rows below
+  M.out = rank ? reinterpret_cast<SortHitDev*>(o + hits_pos) : static_cast<SortHitDev*>(out.bins);
+  M.n_out = rank ? reinterpret_cast<uint32_t*>(o + n_out_pos) : static_cast<uint32_t*>(out.counts);
+  CU(c, fit_dynamic_smem(sort_merge_kernel, size_t(cap) * 16));
+  sort_merge_kernel<<<unsigned(nq), 256, size_t(cap) * 16, c->stream>>>(M);
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  if (!rank) return SDBG_OK;
+  sort_dist_rows_kernel<<<unsigned(nq), 256, 0, c->stream>>>(M.out, M.n_out, M.segs, k, M.type, J.sink[0].desc, M.nulls_first,
+                                                             uint32_t(out.rank), static_cast<unsigned long long*>(out.counts),
+                                                             static_cast<SortDistRow*>(out.bins));
+  ++c->launches;
+  CU(c, cudaGetLastError());
   return SDBG_OK;
+}
+
+// dst row to[j] = src row j, rows of row_words words.
+template <class Word>
+__global__ void __launch_bounds__(256) scatter_rows_kernel(const Word* __restrict__ src, Word* __restrict__ dst,
+                                                           const uint32_t* __restrict__ to, size_t n_rows, size_t row_words) {
+  const size_t n = n_rows * row_words;
+  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
+    const size_t j = i / row_words;
+    dst[size_t(to[j]) * row_words + (i - j * row_words)] = src[i];
+  }
+}
+
+// The queries of one pass, checked before anything is queued (rc: the checks' result): a batch count_run takes whole (a
+// flat batch, or a group batch of one shape), or a group batch of several shapes (S; whole.nq == 0).
+struct PassBatch {
+  int rc;
+  size_t nq;
+  QueryBatch<uint32_t> whole{};
+  uint32_t total_excl = 0;   // whole's, as check_query_batch sets it
+  GroupSplit<uint32_t> S;
+
+  PassBatch(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_t>& Q, const sdbg_col_pred* filt) : nq(Q.nq), whole(Q) {
+    rc = !segs || !n_segs || !Q.terms || !Q.term_off || !Q.nq ? SDBG_EINVAL : check_query_batch(segs, n_segs, Q, filt, &total_excl);
+  }
+  PassBatch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* group_off, const uint32_t* query_group_off,
+            const uint32_t* group_min, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt)
+      : nq(nq) {
+    rc = split_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, S);
+    if (S.whole >= 0) { whole = S.view(S.whole); total_excl = S.total_excl[S.whole]; }
+  }
+  PassBatch(const PassBatch&) = delete;   // whole may point into S
+};
+
+// Runs a prepared pass over B into out: count_run for a whole batch; otherwise each shape into zeroed rows of its own
+// (c->pass[2]), which scatter_rows_kernel moves to the caller's query positions on the stream. Nothing waits.
+int pass_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, const CountJob& job,
+             const CountOut& out) {
+  if (B.whole.nq) return count_run(segs, n_segs, count_plan(segs, n_segs, B.whole, B.total_excl, filt, job), filt, job, out);
+  sdbg_ctx* c = segs[0]->ctx;
+  const GroupSplit<uint32_t>& S = B.S;
+  const std::array<size_t, 3> row = job.rows(out.rank >= 0);
+  void* const dst[3] = {out.counts, out.bins, out.nulls};
+  const auto pad = [](size_t b) { return (b + 7) & ~size_t(7); };
+  // per shape: its query positions (u32), then its rows of each array, every part 8-byte aligned
+  size_t pos[3] = {}, bytes = 0;
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    pos[sh] = bytes;
+    bytes += pad(n * 4);
+    for (size_t r : row) bytes += pad(n * r);
+  }
+  if (int rc = ensure(c, c->pass[2], bytes)) return rc;
+  char* d = static_cast<char*>(c->pass[2].p);
+  CU(c, cudaMemsetAsync(d, 0, bytes, c->stream));
+  for (int sh = 0; sh < 3; ++sh)   // pageable: consumed on return
+    if (!S.qs[sh].empty()) CU(c, cudaMemcpyAsync(d + pos[sh], S.qs[sh].data(), S.qs[sh].size() * 4, cudaMemcpyHostToDevice, c->stream));
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    if (!n) continue;
+    const auto* to = reinterpret_cast<const uint32_t*>(d + pos[sh]);
+    void* part[3];
+    char* p = d + pos[sh] + pad(n * 4);
+    for (int i = 0; i < 3; ++i) { part[i] = p; p += pad(n * row[i]); }
+    const CountOut o{part[0], part[1], part[2], out.oor, out.stats, out.rank};
+    if (int rc = count_run(segs, n_segs, count_plan(segs, n_segs, S.view(sh), S.total_excl[sh], filt, job), filt, job, o)) return rc;
+    for (int i = 0; i < 3; ++i) {
+      if (!row[i]) continue;
+      const size_t words = row[i] % 8 ? row[i] / 4 : row[i] / 8;
+      const unsigned grid = unsigned(std::min<size_t>((n * words + 255) / 256, size_t(c->sm_count) * 8));
+      if (row[i] % 8)   // the sorted scan's u32 n_out
+        scatter_rows_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const uint32_t*>(part[i]), static_cast<uint32_t*>(dst[i]),
+                                                         to, n, words);
+      else
+        scatter_rows_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const unsigned long long*>(part[i]),
+                                                         static_cast<unsigned long long*>(dst[i]), to, n, words);
+      ++c->launches;
+    }
+    CU(c, cudaGetLastError());
+  }
+  return SDBG_OK;
+}
+
+// The aggregate device form's buffer: this header, then AggCell [nq][span], then AggCell [nq] for the NULL key.
+struct AggDistHeader {
+  unsigned long long type;           // the value column's sdbg_type (UINT64_MAX: not found)
+  unsigned long long span, nq;
+  unsigned long long failed;         // non-zero: this rank's local pass failed
+  unsigned long long out_of_range;   // non-zero: a matching doc's key lay outside the range
+  unsigned long long pad[3];
+};
+static_assert(sizeof(AggDistHeader) == 64, "the cells stay 16-byte aligned");
+
+size_t agg_dist_bytes(size_t nq, uint32_t span) { return sizeof(AggDistHeader) + nq * (size_t(span) + 1) * sizeof(AggCell); }
+size_t sort_dist_bytes(size_t nq, uint32_t k) { return sizeof(SortDistHeader) + nq * 8 + nq * size_t(k) * sizeof(SortDistRow); }
+
+// Where count_run's arrays lie in one device buffer, the region of a call: byte offsets (kNone: not in the region) and
+// its size. One layout per pass, the same for the host entries and a rank's buffer.
+constexpr size_t kNone = SIZE_MAX;
+struct PassRegion {
+  size_t counts, bins, nulls, oor, stats, bytes;
+
+  CountOut at(void* base, int64_t rank = -1) const {
+    const auto in = [&](size_t o) -> void* { return o == kNone ? nullptr : static_cast<char*>(base) + o; };
+    return {in(counts), in(bins), in(nulls), static_cast<unsigned int*>(in(oor)), static_cast<unsigned long long*>(in(stats)), rank};
+  }
+};
+
+// The count and facet passes: u64 words [counts [nq] | facet: counts [nq][span], NULL counts [nq] | out-of-range |
+// failed], which one all-reduce of int64 merges across ranks (dist_reduce_to_host: the failure word last).
+PassRegion words_region(size_t nq, uint32_t span /* 0: the count pass */) {
+  const size_t w = nq + (span ? nq * (size_t(span) + 1) : 0);
+  return {0, span ? nq * 8 : kNone, span ? (w - nq) * 8 : kNone, w * 8, kNone, (w + 2) * 8};
+}
+
+// The aggregate pass: its device form's buffer (AggDistHeader, cells, NULL cells); the counts are scratch.
+PassRegion agg_region(size_t nq, uint32_t span) {
+  return {kNone, sizeof(AggDistHeader), sizeof(AggDistHeader) + nq * span * sizeof(AggCell), offsetof(AggDistHeader, out_of_range),
+          kNone, agg_dist_bytes(nq, span)};
+}
+
+// The sorted scan of the local entries: [n_out u32 [nq] | windows judged, skipped | hits SortHitDev [nq][k]].
+PassRegion sort_region(size_t nq, uint32_t k) {
+  const size_t stats = (nq * 4 + 15) & ~size_t(15);
+  return {0, stats + 16, kNone, kNone, stats, stats + 16 + nq * k * sizeof(SortHitDev)};
+}
+
+// A rank's sorted scan: its device form's buffer (SortDistHeader, row counts, rows); the windows are scratch.
+PassRegion sort_rank_region(size_t nq, uint32_t k) {
+  return {sizeof(SortDistHeader), sizeof(SortDistHeader) + nq * 8, kNone, kNone, kNone, sort_dist_bytes(nq, k)};
+}
+
+// The host copy h of a call's region: fails on its out-of-range word, else fills the caller's arrays (fill(h)).
+template <class Fill>
+int pass_finish(sdbg_ctx* c, const PassRegion& L, const char* h, Fill fill) {
+  unsigned int oor = 0;
+  if (L.oor != kNone) std::memcpy(&oor, h + L.oor, 4);
+  if (oor) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
+  fill(h);
+  return SDBG_OK;
+}
+
+void facet_fill(const char* h, size_t nq, uint32_t span, uint64_t* counts, uint64_t* null_counts) {
+  const PassRegion L = words_region(nq, span);
+  std::memcpy(counts, h + L.bins, nq * size_t(span) * 8);
+  std::memcpy(null_counts, h + L.nulls, nq * 8);
+}
+
+// The host entries' one path, after their checks (B): prepares the job, then lays out its region L in c->pass[0], zeroes
+// it, runs the pass into it, copies it back through the pinned staging with one copy and one wait, and finishes
+// (pass_finish). The sorted scan's windows go to sdbg_scan_stats. A count batch that the plan answers entirely from
+// docs_count queues nothing: fill gets the plan's counts, which is where the count region starts.
+template <class Fill>
+int pass_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, CountJob& job,
+                 const PassRegion& L, Fill fill) {
+  if (B.rc) return B.rc;
+  sdbg_ctx* c = segs[0]->ctx;
+  CU(c, cudaSetDevice(c->device));
+  if (int rc = job_prepare(c, segs, n_segs, job)) return rc;
+  CountPlan pl;
+  if (B.whole.nq) {
+    pl = count_plan(segs, n_segs, B.whole, B.total_excl, filt, job);
+    if (job.mode == CountMode::count && !pl.items) {
+      fill(reinterpret_cast<const char*>(pl.host.data()));
+      return SDBG_OK;
+    }
+  }
+  if (int rc = ensure(c, c->pass[0], L.bytes + B.nq * 8)) return rc;   // then the aggregate pass's count scratch
+  if (int rc = ensure_pinned(c, L.bytes)) return rc;
+  CountOut out = L.at(c->pass[0].p);
+  if (!out.counts) out.counts = static_cast<char*>(c->pass[0].p) + L.bytes;
+  CU(c, cudaMemsetAsync(c->pass[0].p, 0, L.bytes + B.nq * 8, c->stream));
+  if (int rc = B.whole.nq ? count_run(segs, n_segs, pl, filt, job, out) : pass_run(segs, n_segs, B, filt, job, out)) return rc;
+  if (out.stats) {   // windows skipped: a device word, as the GROUP BY scan leaves it
+    if (!c->d_zone_skipped) CU(c, cudaMalloc(reinterpret_cast<void**>(&c->d_zone_skipped), 8));
+    CU(c, cudaMemcpyAsync(c->d_zone_skipped, out.stats + 1, 8, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  CU(c, cudaMemcpyAsync(c->h_pinned, c->pass[0].p, L.bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  const char* h = static_cast<const char*>(c->h_pinned);
+  if (out.stats) std::memcpy(&c->zone_blocks_total, h + L.stats, 8);   // windows judged (only where a zonemap is)
+  return pass_finish(c, L, h, fill);
+}
+
+int sort_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, uint64_t field,
+                 int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
+  CountJob job{CountMode::sort, {field, descending, nulls_first, k, {}, {}}, {}, {}};
+  const PassRegion L = sort_region(B.nq, k);
+  return pass_to_host(segs, n_segs, B, filt, job, L, [&](const char* h) {
+    std::memcpy(n_out, h + L.counts, B.nq * 4);
+    std::memcpy(out, h + L.bins, B.nq * k * sizeof(SortHitDev));
+  });
+}
+
+int agg_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, uint64_t key_field,
+                int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out, sdbg_match_agg* null_out) {
+  CountJob job{CountMode::agg, {}, {}, {{key_field, key_min, key_span, {}}, value_field, {}}};
+  const PassRegion L = agg_region(B.nq, key_span);
+  return pass_to_host(segs, n_segs, B, filt, job, L, [&](const char* h) {
+    agg_results(reinterpret_cast<const AggCell*>(h + L.bins), B.nq, key_span, job.agg.sink[0].type, out, null_out);
+  });
 }
 }  // namespace
 
 extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
                                       const uint32_t* term_off, size_t nq, const uint32_t* excl_terms,
                                       const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
-  return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, counts);
+  if (!counts) return SDBG_EINVAL;
+  const PassBatch B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  CountJob job{CountMode::count, {}, {}, {}};
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
 }
 
 extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -2419,8 +2560,8 @@ extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t
                                                int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
   if (!segs || !n_segs || !segs[0] || !k || !out || !n_out) return SDBG_EINVAL;
   if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
-  SortJob J{sort_field, descending, nulls_first, k, out, n_out, {}, {}};
-  return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, nullptr, &J);
+  const PassBatch B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  return sort_to_host(segs, n_segs, B, filt, sort_field, descending, nulls_first, k, out, n_out);
 }
 
 extern "C" int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -2428,8 +2569,10 @@ extern "C" int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n
                                              const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
                                              int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
   if (!counts || !null_counts) return SDBG_EINVAL;
-  FacetJob J{key_field, key_min, key_span, counts, null_counts, {}};
-  return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, nullptr, nullptr, &J);
+  const PassBatch B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, key_span),
+                      [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
 }
 
 extern "C" int sdbg_match_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -2438,9 +2581,8 @@ extern "C" int sdbg_match_aggregate_batch(sdbg_segment* const* segs, size_t n_se
                                           int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
                                           sdbg_match_agg* null_out) {
   if (!out || !null_out) return SDBG_EINVAL;
-  AggJob J{{key_field, key_min, key_span, nullptr, nullptr, {}}, value_field, out, null_out, {}};
-  return count_run(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt, nullptr, nullptr, nullptr,
-                   &J);
+  const PassBatch B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out);
 }
 
 extern "C" int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2448,10 +2590,9 @@ extern "C" int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size
                                                  const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
                                                  const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts) return SDBG_EINVAL;
-  return run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, {{counts, 8}},
-                    [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
-                      return count_run(segs, n_segs, Q, filt, static_cast<uint64_t*>(r[0].p));
-                    });
+  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  CountJob job{CountMode::count, {}, {}, {}};
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
 }
 
 extern "C" int sdbg_match_count_batch_groups(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2469,27 +2610,9 @@ extern "C" int sdbg_match_topk_by_column_batch_groups_min(sdbg_segment* const* s
                                                           int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out,
                                                           uint32_t* n_out) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !out || !n_out) return SDBG_EINVAL;
-  sdbg_ctx* c = segs[0]->ctx;
-  if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
-  uint64_t judged = 0, skipped = 0;
-  bool whole = false;   // the batch is one shape: the scan statistics are already the call's
-  const int rc = run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                            {{out, k * sizeof(sdbg_sort_hit)}, {n_out, 4}}, [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
-                              SortJob J{sort_field, descending, nulls_first, k, static_cast<sdbg_sort_hit*>(r[0].p),
-                                        static_cast<uint32_t*>(r[1].p), {}, {}};
-                              if (int rc = count_run(segs, n_segs, Q, filt, nullptr, &J)) return rc;
-                              whole = Q.nq == nq;
-                              uint64_t t = 0, s = 0;
-                              if (int rc = whole ? SDBG_OK : sdbg_scan_stats(c, &t, &s)) return rc;
-                              judged += t; skipped += s;
-                              return SDBG_OK;
-                            });
-  if (rc || whole) return rc;
-  // the windows of the whole call, not of its last shape
-  c->zone_blocks_total = judged;
-  CU(c, cudaMemcpyAsync(c->d_zone_skipped, &skipped, 8, cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  return SDBG_OK;
+  if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
+  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  return sort_to_host(segs, n_segs, B, filt, sort_field, descending, nulls_first, k, out, n_out);
 }
 
 extern "C" int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2500,11 +2623,10 @@ extern "C" int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* seg
                                                         uint64_t* null_counts) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts || !null_counts) return SDBG_EINVAL;
   if (int rc = facet_check_range(segs[0]->ctx, key_min, key_span)) return rc;   // before the rows are sized
-  return run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                    {{counts, size_t(key_span) * 8}, {null_counts, 8}}, [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
-                      FacetJob J{key_field, key_min, key_span, static_cast<uint64_t*>(r[0].p), static_cast<uint64_t*>(r[1].p), {}};
-                      return count_run(segs, n_segs, Q, filt, nullptr, nullptr, &J);
-                    });
+  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, key_span),
+                      [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
 }
 
 extern "C" int sdbg_match_aggregate_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2515,80 +2637,12 @@ extern "C" int sdbg_match_aggregate_batch_groups_min(sdbg_segment* const* segs, 
                                                      sdbg_match_agg* out, sdbg_match_agg* null_out) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !out || !null_out) return SDBG_EINVAL;
   if (int rc = agg_check_range(segs[0]->ctx, key_field, key_min, key_span)) return rc;   // before the rows are sized
-  return run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                    {{out, size_t(key_span) * sizeof(sdbg_match_agg)}, {null_out, sizeof(sdbg_match_agg)}},
-                    [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
-                      AggJob J{{key_field, key_min, key_span, nullptr, nullptr, {}}, value_field,
-                               static_cast<sdbg_match_agg*>(r[0].p), static_cast<sdbg_match_agg*>(r[1].p), {}};
-                      return count_run(segs, n_segs, Q, filt, nullptr, nullptr, nullptr, &J);
-                    });
+  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out);
 }
 
-// ---- the count, facet and aggregate passes across GPUs ----
+// ---- the count, facet, aggregate and sorted passes across GPUs ----
 namespace {
-// dst row to[j] = src row j, rows of row_words words.
-__global__ void __launch_bounds__(256) scatter_rows_kernel(const unsigned long long* __restrict__ src,
-                                                           unsigned long long* __restrict__ dst, const uint32_t* __restrict__ to,
-                                                           size_t n_rows, size_t row_words) {
-  const size_t n = n_rows * row_words;
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
-    const size_t j = i / row_words;
-    dst[size_t(to[j]) * row_words + (i - j * row_words)] = src[i];
-  }
-}
-
-// run_groups for count_run's device mode: rows[i] are device arrays (bytes a multiple of 8). A batch of one shape writes
-// straight into them; otherwise each shape writes zeroed rows of its own (c->dist[2]), which scatter_rows_kernel moves
-// to the caller's query positions on the stream. Nothing waits.
-template <size_t N, class Run>
-int run_groups_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* group_off,
-                      const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
-                      const uint32_t* excl_off, const sdbg_col_pred* filt, const OutRows (&rows)[N], Run run) {
-  sdbg_ctx* c = segs[0]->ctx;
-  GroupSplit<uint32_t> S;
-  if (int rc = split_groups(c, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, S)) return rc;
-  for (int sh = 0; sh < 3; ++sh) {
-    uint32_t total_excl = 0;
-    if (!S.qs[sh].empty())
-      if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &total_excl)) return rc;
-  }
-  for (int sh = 0; sh < 3; ++sh)
-    if (S.qs[sh].size() == nq) return run(S.view(sh), rows);
-  // per shape: its query positions (u32, padded to 8 B), then its rows
-  size_t pos[3] = {}, bytes = 0;
-  for (int sh = 0; sh < 3; ++sh) {
-    pos[sh] = bytes;
-    bytes += (S.qs[sh].size() * 4 + 7) & ~size_t(7);
-    for (size_t i = 0; i < N; ++i) bytes += S.qs[sh].size() * rows[i].bytes;
-  }
-  if (int rc = ensure(c, c->dist[2], bytes)) return rc;
-  char* d = static_cast<char*>(c->dist[2].p);
-  CU(c, cudaMemsetAsync(d, 0, bytes, c->stream));
-  for (int sh = 0; sh < 3; ++sh) {
-    std::vector<uint32_t> at(S.qs[sh].begin(), S.qs[sh].end());
-    if (!at.empty())   // pageable: consumed on return
-      CU(c, cudaMemcpyAsync(d + pos[sh], at.data(), at.size() * 4, cudaMemcpyHostToDevice, c->stream));
-  }
-  for (int sh = 0; sh < 3; ++sh) {
-    const size_t n = S.qs[sh].size();
-    if (!n) continue;
-    OutRows part[N];
-    char* p = d + pos[sh] + ((n * 4 + 7) & ~size_t(7));
-    for (size_t i = 0; i < N; ++i) { part[i] = {p, rows[i].bytes}; p += n * rows[i].bytes; }
-    if (int rc = run(S.view(sh), part)) return rc;
-    for (size_t i = 0; i < N; ++i) {
-      const size_t words = rows[i].bytes / 8;
-      const unsigned grid = unsigned(std::min<size_t>((n * words + 255) / 256, size_t(c->sm_count) * 8));
-      scatter_rows_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const unsigned long long*>(part[i].p),
-                                                       static_cast<unsigned long long*>(rows[i].p),
-                                                       reinterpret_cast<const uint32_t*>(d + pos[sh]), n, words);
-      ++c->launches;
-    }
-    CU(c, cudaGetLastError());
-  }
-  return SDBG_OK;
-}
-
 // The dist entries' checks of the call's scalar arguments, which fail alike on every rank: before anything is queued.
 int dist_check(sdbg_segment* const* segs, size_t n_segs, const uint32_t* group_off, const uint32_t* query_group_off, size_t nq) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq) return SDBG_EINVAL;
@@ -2610,18 +2664,6 @@ int dist_reduce_to_host(sdbg_ctx* c, int rc_local, unsigned long long* d, size_t
   if (static_cast<const unsigned long long*>(c->h_pinned)[words - 1]) return fail(c, SDBG_EINVAL, "the call failed on another rank");
   return SDBG_OK;
 }
-
-// The aggregate device form's buffer: this header, then AggCell [nq][span], then AggCell [nq] for the NULL key.
-struct AggDistHeader {
-  unsigned long long type;           // the value column's sdbg_type (UINT64_MAX: not found)
-  unsigned long long span, nq;
-  unsigned long long failed;         // non-zero: this rank's local pass failed
-  unsigned long long out_of_range;   // non-zero: a matching doc's key lay outside the range
-  unsigned long long pad[3];
-};
-static_assert(sizeof(AggDistHeader) == 64, "the cells stay 16-byte aligned");
-
-size_t agg_dist_bytes(size_t nq, uint32_t span) { return sizeof(AggDistHeader) + nq * (size_t(span) + 1) * sizeof(AggCell); }
 
 // One thread per (query, key) cell: the cells of ranks 0 .. n_ranks - 1 in rank order. Counts are u64 sums, the integer
 // sum a 128-bit add with its carry, the float64 sum the ranks' partials added in rank order (so every rank computes the
@@ -2664,32 +2706,43 @@ __global__ void __launch_bounds__(256) agg_merge_gathered_kernel(const char* __r
   }
 }
 
-// The aggregate device form after the scalar checks: zeroes the buffer, writes the header, runs the pass into it and, when
-// the pass fails, sets the header's failure word.
-int agg_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* group_off,
-               const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
-               const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
-               uint64_t value_field, void* d_buf) {
+// The dist count and facet entries after their checks (B): this rank's region (words_region) in c->pass[0], zeroed, the
+// pass run into it, one all-reduce of int64 over it, then the host entries' finish (pass_finish). A rank whose checks or
+// pass fail still joins the collective, with its failure word set.
+template <class Fill>
+int dist_words(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, CountJob& job, Fill fill) {
   sdbg_ctx* c = segs[0]->ctx;
   CU(c, cudaSetDevice(c->device));
-  auto* hdr = static_cast<AggDistHeader*>(d_buf);
-  auto* cells = reinterpret_cast<AggCell*>(hdr + 1);
-  AggDistHeader h{};
-  const auto it = segs[0]->cols.find(value_field);
-  h.type = it == segs[0]->cols.end() ? UINT64_MAX : uint64_t(it->second.type);
-  h.span = key_span; h.nq = nq;
-  CU(c, cudaMemsetAsync(d_buf, 0, agg_dist_bytes(nq, key_span), c->stream));
-  CU(c, cudaMemcpyAsync(hdr, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
-  int rc = ensure(c, c->dist[3], nq * 8);
-  if (!rc) rc = run_groups_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                                   {{c->dist[3].p, 8}, {cells, size_t(key_span) * sizeof(AggCell)}, {cells + nq * key_span, sizeof(AggCell)}},
-                                   [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
-                                     AggJob J{{key_field, key_min, key_span, nullptr, nullptr, {}}, value_field, nullptr, nullptr, {}};
-                                     const CountDevOut D{static_cast<unsigned long long*>(r[0].p), r[1].p, r[2].p,
-                                                         reinterpret_cast<unsigned int*>(&hdr->out_of_range)};
-                                     return count_run(segs, n_segs, Q, filt, nullptr, nullptr, nullptr, &J, &D);
-                                   });
-  if (rc) CU(c, cudaMemsetAsync(&hdr->failed, 1, 1, c->stream));
+  const PassRegion L = words_region(B.nq, job.mode == CountMode::facet ? job.facet.span : 0);
+  if (int rc = ensure(c, c->pass[0], L.bytes)) return rc;
+  int rc_local = B.rc ? B.rc : job_prepare(c, segs, n_segs, job);
+  CU(c, cudaMemsetAsync(c->pass[0].p, 0, L.bytes, c->stream));
+  if (!rc_local) rc_local = pass_run(segs, n_segs, B, filt, job, L.at(c->pass[0].p));
+  if (int rc = dist_reduce_to_host(c, rc_local, static_cast<unsigned long long*>(c->pass[0].p), L.bytes / 8)) return rc;
+  return pass_finish(c, L, static_cast<const char*>(c->h_pinned), fill);
+}
+
+// The aggregate and sorted device forms after their checks (B): zeroes the buffer (region L), writes its 64-byte header
+// hdr, prepares the job and runs the pass into the buffer, with c->pass[3] zeroed for what the device forms do not
+// report (the aggregate pass's counts, the sorted scan's windows). When the checks or the pass fail, sets the header's
+// failure word (at byte `failed`), so that the rank still joins the collective and the merge fails.
+int rank_device(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, CountJob& job,
+                const void* hdr, size_t failed, const PassRegion& L, int64_t rank, void* d_buf) {
+  sdbg_ctx* c = segs[0]->ctx;
+  CU(c, cudaSetDevice(c->device));
+  int rc = B.rc ? B.rc : job_prepare(c, segs, n_segs, job);
+  CU(c, cudaMemsetAsync(d_buf, 0, L.bytes, c->stream));
+  CU(c, cudaMemcpyAsync(d_buf, hdr, 64, cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
+  CountOut out = L.at(d_buf, rank);
+  if (!rc) rc = ensure(c, c->pass[3], B.nq * 8 + 16);
+  if (!rc) {
+    auto* scratch = static_cast<unsigned long long*>(c->pass[3].p);
+    CU(c, cudaMemsetAsync(scratch, 0, B.nq * 8 + 16, c->stream));
+    if (!out.counts) out.counts = scratch + 2;
+    if (!out.stats) out.stats = scratch;
+    rc = pass_run(segs, n_segs, B, filt, job, out);
+  }
+  if (rc) CU(c, cudaMemsetAsync(static_cast<char*>(d_buf) + failed, 1, 1, c->stream));
   return rc;
 }
 }  // namespace
@@ -2700,20 +2753,9 @@ extern "C" int sdbg_dist_match_count_batch_groups_min(sdbg_segment* const* segs,
                                                       const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
   if (int rc = dist_check(segs, n_segs, group_off, query_group_off, nq)) return rc;
   if (!counts) return SDBG_EINVAL;
-  sdbg_ctx* c = segs[0]->ctx;
-  CU(c, cudaSetDevice(c->device));
-  // [counts [nq] | failure flag]
-  if (int rc = ensure(c, c->dist[0], (nq + 1) * 8)) return rc;
-  auto* d = static_cast<unsigned long long*>(c->dist[0].p);
-  CU(c, cudaMemsetAsync(d, 0, (nq + 1) * 8, c->stream));
-  const int rc_local = run_groups_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off,
-                                         filt, {{d, 8}}, [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
-                                           const CountDevOut D{static_cast<unsigned long long*>(r[0].p), nullptr, nullptr, nullptr};
-                                           return count_run(segs, n_segs, Q, filt, nullptr, nullptr, nullptr, nullptr, &D);
-                                         });
-  if (int rc = dist_reduce_to_host(c, rc_local, d, nq + 1)) return rc;
-  std::memcpy(counts, c->h_pinned, nq * 8);
-  return SDBG_OK;
+  CountJob job{CountMode::count, {}, {}, {}};
+  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  return dist_words(segs, n_segs, B, filt, job, [&](const char* h) { std::memcpy(counts, h, nq * 8); });
 }
 
 extern "C" int sdbg_dist_match_facet_counts_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2724,29 +2766,10 @@ extern "C" int sdbg_dist_match_facet_counts_batch_groups_min(sdbg_segment* const
                                                              uint64_t* counts, uint64_t* null_counts) {
   if (int rc = dist_check(segs, n_segs, group_off, query_group_off, nq)) return rc;
   if (!counts || !null_counts) return SDBG_EINVAL;
-  sdbg_ctx* c = segs[0]->ctx;
-  if (int rc = facet_check_range(c, key_min, key_span)) return rc;
-  CU(c, cudaSetDevice(c->device));
-  // [counts [nq][span] | NULL counts [nq] | out-of-range word | failure flag]
-  const size_t bins = nq * size_t(key_span), words = bins + nq + 2;
-  if (int rc = ensure(c, c->dist[0], words * 8)) return rc;
-  if (int rc = ensure(c, c->dist[3], nq * 8)) return rc;
-  auto* d = static_cast<unsigned long long*>(c->dist[0].p);
-  CU(c, cudaMemsetAsync(d, 0, words * 8, c->stream));
-  const int rc_local = run_groups_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                                         {{c->dist[3].p, 8}, {d, size_t(key_span) * 8}, {d + bins, 8}},
-                                         [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
-                                           FacetJob J{key_field, key_min, key_span, nullptr, nullptr, {}};
-                                           const CountDevOut D{static_cast<unsigned long long*>(r[0].p), r[1].p, r[2].p,
-                                                               reinterpret_cast<unsigned int*>(d + bins + nq)};
-                                           return count_run(segs, n_segs, Q, filt, nullptr, nullptr, &J, nullptr, &D);
-                                         });
-  if (int rc = dist_reduce_to_host(c, rc_local, d, words)) return rc;
-  const auto* h = static_cast<const unsigned long long*>(c->h_pinned);
-  if (h[bins + nq]) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
-  std::memcpy(counts, h, bins * 8);
-  std::memcpy(null_counts, h + bins, nq * 8);
-  return SDBG_OK;
+  if (int rc = facet_check_range(segs[0]->ctx, key_min, key_span)) return rc;
+  CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
+  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  return dist_words(segs, n_segs, B, filt, job, [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
 }
 
 extern "C" int sdbg_match_aggregate_batch_groups_min_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
@@ -2757,8 +2780,11 @@ extern "C" int sdbg_match_aggregate_batch_groups_min_device(sdbg_segment* const*
                                                             uint64_t value_field, void* d_cells) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !d_cells) return SDBG_EINVAL;
   if (int rc = agg_check_range(segs[0]->ctx, key_field, key_min, key_span)) return rc;
-  return agg_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, key_field,
-                    key_min, key_span, value_field, d_cells);
+  CountJob job{CountMode::agg, {}, {}, {{key_field, key_min, key_span, {}}, value_field, {}}};
+  const auto it = segs[0]->cols.find(value_field);   // the header's type: UINT64_MAX when not staged
+  const AggDistHeader h{it == segs[0]->cols.end() ? UINT64_MAX : uint64_t(it->second.type), key_span, nq, 0, 0, {}};
+  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  return rank_device(segs, n_segs, B, filt, job, &h, offsetof(AggDistHeader, failed), agg_region(nq, key_span), -1, d_cells);
 }
 
 extern "C" int sdbg_match_aggregate_merge_gathered(sdbg_ctx* c, const void* d_all, uint32_t n_ranks, size_t nq, uint32_t key_span,
@@ -2767,8 +2793,8 @@ extern "C" int sdbg_match_aggregate_merge_gathered(sdbg_ctx* c, const void* d_al
   if (key_span > kAggMaxSpan) return fail(c, SDBG_EUNSUPPORTED, "key_span > 4096");
   CU(c, cudaSetDevice(c->device));
   const size_t n = nq * (size_t(key_span) + 1), bytes = 64 + n * sizeof(AggCell);
-  if (int rc = ensure(c, c->dist[3], bytes)) return rc;
-  char* m = static_cast<char*>(c->dist[3].p);
+  if (int rc = ensure(c, c->pass[3], bytes)) return rc;
+  char* m = static_cast<char*>(c->pass[3].p);
   const unsigned grid = unsigned(std::max<size_t>(1, std::min<size_t>((n + 255) / 256, size_t(c->sm_count) * 16)));
   agg_merge_gathered_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const char*>(d_all), agg_dist_bytes(nq, key_span), n_ranks, nq,
                                                         key_span, reinterpret_cast<unsigned long long*>(m),
@@ -2782,10 +2808,8 @@ extern "C" int sdbg_match_aggregate_merge_gathered(sdbg_ctx* c, const void* d_al
   if (st[0]) return fail(c, SDBG_EINVAL, "the ranks' aggregate headers disagree (value type, key_span or n_queries)");
   if (st[1]) return fail(c, SDBG_EINVAL, "the aggregate pass failed on a rank");
   if (st[2]) return fail(c, SDBG_EINVAL, "a matching doc's key lies outside [key_min, key_min + key_span)");
-  const auto* g = reinterpret_cast<const AggCell*>(static_cast<const char*>(c->h_pinned) + 64);
-  const uint32_t type = uint32_t(st[3]);
-  for (size_t i = 0; i < nq * key_span; ++i) out[i] = agg_result(g[i], type);
-  for (size_t q = 0; q < nq; ++q) null_out[q] = agg_result(g[nq * key_span + q], type);
+  agg_results(reinterpret_cast<const AggCell*>(static_cast<const char*>(c->h_pinned) + 64), nq, key_span, uint32_t(st[3]), out,
+              null_out);
   return SDBG_OK;
 }
 
@@ -2801,46 +2825,15 @@ extern "C" int sdbg_dist_match_aggregate_batch_groups_min(sdbg_segment* const* s
   if (int rc = agg_check_range(c, key_field, key_min, key_span)) return rc;
   const uint32_t world = uint32_t(c->dist_world);
   const size_t bytes = agg_dist_bytes(nq, key_span);
-  if (int rc = ensure(c, c->dist[0], bytes)) return rc;
-  if (int rc = ensure(c, c->dist[1], bytes * world)) return rc;
-  const int rc_local = agg_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                                  key_field, key_min, key_span, value_field, c->dist[0].p);
-  if (int rc = sdbg_dist_allgather(c, c->dist[0].p, c->dist[1].p, bytes)) return rc_local ? rc_local : rc;
-  const int rc = sdbg_match_aggregate_merge_gathered(c, c->dist[1].p, world, nq, key_span, out, null_out);
+  if (int rc = ensure(c, c->pass[0], bytes)) return rc;
+  if (int rc = ensure(c, c->pass[1], bytes * world)) return rc;
+  const int rc_local = sdbg_match_aggregate_batch_groups_min_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq,
+                                                                    excl_terms, excl_off, filt, key_field, key_min, key_span,
+                                                                    value_field, c->pass[0].p);
+  if (int rc = sdbg_dist_allgather(c, c->pass[0].p, c->pass[1].p, bytes)) return rc_local ? rc_local : rc;
+  const int rc = sdbg_match_aggregate_merge_gathered(c, c->pass[1].p, world, nq, key_span, out, null_out);
   return rc_local ? rc_local : rc;
 }
-
-namespace {
-size_t sort_dist_bytes(size_t nq, uint32_t k) { return sizeof(SortDistHeader) + nq * 8 + nq * size_t(k) * sizeof(SortDistRow); }
-
-// The sorted device form after the scalar checks: zeroes the buffer, writes the header, runs the sorted scan into it and,
-// when the scan fails, sets the header's failure word.
-int sort_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* group_off,
-                const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
-                const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field, int descending, int nulls_first,
-                uint32_t k, uint32_t rank, void* d_buf) {
-  sdbg_ctx* c = segs[0]->ctx;
-  CU(c, cudaSetDevice(c->device));
-  auto* hdr = static_cast<SortDistHeader*>(d_buf);
-  auto* counts = reinterpret_cast<unsigned long long*>(hdr + 1);
-  auto* rows = reinterpret_cast<SortDistRow*>(counts + nq);
-  SortDistHeader h{};
-  const auto it = segs[0]->cols.find(sort_field);
-  h.type = it == segs[0]->cols.end() ? UINT64_MAX : uint64_t(it->second.type);
-  h.desc = descending ? 1u : 0u; h.nulls_first = nulls_first ? 1u : 0u; h.k = k; h.nq = nq;
-  CU(c, cudaMemsetAsync(d_buf, 0, sort_dist_bytes(nq, k), c->stream));
-  CU(c, cudaMemcpyAsync(hdr, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
-  const int rc = run_groups_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                                   {{counts, 8}, {rows, size_t(k) * sizeof(SortDistRow)}},
-                                   [&](const QueryBatch<uint32_t>& Q, const OutRows* r) {
-                                     SortJob J{sort_field, descending, nulls_first, k, nullptr, nullptr, {}, {}};
-                                     const CountDevOut D{static_cast<unsigned long long*>(r[0].p), r[1].p, nullptr, nullptr, rank};
-                                     return count_run(segs, n_segs, Q, filt, nullptr, &J, nullptr, nullptr, &D);
-                                   });
-  if (rc) CU(c, cudaMemsetAsync(&hdr->failed, 1, 1, c->stream));
-  return rc;
-}
-}  // namespace
 
 extern "C" int sdbg_match_topk_by_column_batch_groups_min_device(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
                                                                  const uint32_t* group_off, const uint32_t* query_group_off,
@@ -2851,8 +2844,12 @@ extern "C" int sdbg_match_topk_by_column_batch_groups_min_device(sdbg_segment* c
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !d_rows) return SDBG_EINVAL;
   if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
   if (rank > 0x7FFFFFFFu) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "rank >= 2^31");
-  return sort_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, sort_field,
-                     descending, nulls_first, k, rank, d_rows);
+  CountJob job{CountMode::sort, {sort_field, descending, nulls_first, k, {}, {}}, {}, {}};
+  const auto it = segs[0]->cols.find(sort_field);   // the header's type: UINT64_MAX when not staged
+  const SortDistHeader h{it == segs[0]->cols.end() ? UINT64_MAX : uint64_t(it->second.type), descending ? 1u : 0u,
+                         nulls_first ? 1u : 0u, k, nq, 0, {}};
+  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  return rank_device(segs, n_segs, B, filt, job, &h, offsetof(SortDistHeader, failed), sort_rank_region(nq, k), rank, d_rows);
 }
 
 extern "C" int sdbg_match_topk_by_column_merge_gathered(sdbg_ctx* c, const void* d_all, uint32_t n_ranks, size_t nq, uint32_t k,
@@ -2862,8 +2859,8 @@ extern "C" int sdbg_match_topk_by_column_merge_gathered(sdbg_ctx* c, const void*
   if (nq > 0x7FFFFFFFu) return fail(c, SDBG_EUNSUPPORTED, "more than 2^31 queries");
   CU(c, cudaSetDevice(c->device));
   const size_t hits_bytes = nq * size_t(k) * sizeof(SortHitDev), bytes = 64 + hits_bytes + nq * 4;
-  if (int rc = ensure(c, c->dist[3], bytes)) return rc;
-  char* m = static_cast<char*>(c->dist[3].p);
+  if (int rc = ensure(c, c->pass[3], bytes)) return rc;
+  char* m = static_cast<char*>(c->pass[3].p);
   const uint32_t cap = std::max(256u, 2u * next_pow2(k));
   CU(c, fit_dynamic_smem(sort_merge_gathered_kernel, size_t(cap) * 16));
   sort_merge_gathered_kernel<<<unsigned(nq), 256, size_t(cap) * 16, c->stream>>>(
@@ -2894,12 +2891,13 @@ extern "C" int sdbg_dist_match_topk_by_column_batch_groups_min(sdbg_segment* con
   if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
   const uint32_t world = uint32_t(c->dist_world);
   const size_t bytes = sort_dist_bytes(nq, k);
-  if (int rc = ensure(c, c->dist[0], bytes)) return rc;
-  if (int rc = ensure(c, c->dist[1], bytes * world)) return rc;
-  const int rc_local = sort_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                                   sort_field, descending, nulls_first, k, uint32_t(c->dist_rank), c->dist[0].p);
-  if (int rc = sdbg_dist_allgather(c, c->dist[0].p, c->dist[1].p, bytes)) return rc_local ? rc_local : rc;
-  const int rc = sdbg_match_topk_by_column_merge_gathered(c, c->dist[1].p, world, nq, k, out, n_out);
+  if (int rc = ensure(c, c->pass[0], bytes)) return rc;
+  if (int rc = ensure(c, c->pass[1], bytes * world)) return rc;
+  const int rc_local = sdbg_match_topk_by_column_batch_groups_min_device(segs, n_segs, terms, group_off, query_group_off, group_min,
+                                                                         nq, excl_terms, excl_off, filt, sort_field, descending,
+                                                                         nulls_first, k, uint32_t(c->dist_rank), c->pass[0].p);
+  if (int rc = sdbg_dist_allgather(c, c->pass[0].p, c->pass[1].p, bytes)) return rc_local ? rc_local : rc;
+  const int rc = sdbg_match_topk_by_column_merge_gathered(c, c->pass[1].p, world, nq, k, out, n_out);
   return rc_local ? rc_local : rc;
 }
 
