@@ -766,9 +766,18 @@ extern "C" int sdbg_column_device_ptr(sdbg_segment* s, uint64_t field, void** d_
   auto it = s->cols.find(field);
   if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "unknown column");
   CU(s->ctx, cudaSetDevice(s->ctx->device));
+  ColumnObj& col = it->second;
   void* p = nullptr;
-  const int rc = raw_values(s->ctx, it->second, &p);
+  const int rc = raw_values(s->ctx, col, &p);
   if (rc) return rc;
+  // The caller is about to write the values: every statistic of the old ones is dropped, and a packed column becomes
+  // its raw view (the packed words would keep the old values) until it is restaged.
+  if (col.d_packed) {
+    CU(s->ctx, cudaStreamSynchronize(s->ctx->stream));   // queued readers of the packed words finish first
+    cudaFree(col.d_packed);
+    col.d_packed = nullptr; col.packed_bytes = 0;
+  }
+  col.has_minmax = false; col.has_absmax = false; col.zone_ok = false;
   if (d_values) *d_values = p;
   if (rows) *rows = it->second.rows;
   return SDBG_OK;
@@ -3451,7 +3460,9 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
     double mx; std::memcpy(&mx, &absmax_bits, 8);
     int e = 0;
     if (mx > 0) std::frexp(mx, &e);                                  // mx < 2^e
-    plan.fix_eunit = e - 2 * plan.fix_limb;                          // |w| / 2^eunit < 2^(2*limb)
+    // |w| / 2^eunit < 2^(2*limb); never below 2^-1074, the unit of every double: a finer unit would shift a subnormal's
+    // mantissa 64 bits or more (fix_limbs) and gains nothing, since every value is already an integer multiple of it
+    plan.fix_eunit = std::max(e - 2 * plan.fix_limb, -1074);
   }
   // All accumulators integer => the four words of a slot go out as one RED request per passing row.
   plan.quad = all_tma && (avg_f64_field == UINT64_MAX || plan.fix_limb) && env_int("SDBG_GROUPBY_QUAD", 0);
@@ -3703,6 +3714,13 @@ int groupby_hash(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred* 
                  uint32_t n_groups_hint, uint64_t sum_int_field, uint64_t avg_f64_field, sdbg_group_row* out, uint64_t cap,
                  uint64_t* n_out) {
   sdbg_ctx* c = segs[0]->ctx;
+  // the SUM(int) lo limb adds up to 2^32 - 1 per row as a signed 64-bit value: the dense path's row limit holds here too
+  uint64_t total_rows = 0;
+  for (size_t si = 0; si < n_segs; ++si) {
+    auto it = segs[si]->cols.find(key_field);
+    if (it != segs[si]->cols.end()) total_rows += it->second.rows;
+  }
+  if (total_rows >= (1ull << 31)) return fail(c, SDBG_EUNSUPPORTED, ">= 2^31 rows per GPU in one GROUP BY (limb overflow guard)");
   uint64_t capacity = 1 << 16;
   while (capacity < 2ull * std::max<uint64_t>(n_groups_hint, cap)) capacity <<= 1;
   int rc;
