@@ -192,7 +192,9 @@ int sdbg_bm25_topk(sdbg_segment* const* segs, size_t n_segs, int kind, const sdb
                    size_t n_terms, float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in,
                    sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches, float* threshold_out);
 /* A batch of independent queries in one launch set (the benchmark-game / many-workers shape).
- * Query q uses terms[term_off[q] .. term_off[q+1]); out holds n_queries*k hits, n_out/total per query. */
+ * Query q uses terms[term_off[q] .. term_off[q+1]); out holds n_queries*k hits, n_out/total per query.
+ * Memory: the results take n_queries * (8k + 12) B of HBM and as much pinned host memory for the copy back; the
+ * query descriptors are staged from pageable memory. Synchronous on the context's stream. */
 /* k1 = -1 is reserved: it selects the TFIDF scorer (b != 0: normalised) -- sdbg_tfidf_topk_batch is the named entry. */
 int sdbg_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
                          const uint32_t* term_off, size_t n_queries, float k1, float b, const sdbg_col_pred* filt,
@@ -309,6 +311,8 @@ int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int 
  * sdbg_bm25_topk_batch_excl / sdbg_match_count_batch.
  * The sorted scan and facet counts of group queries: sdbg_match_topk_by_column_batch_groups_min /
  * sdbg_match_facet_counts_batch_groups_min below.
+ * Memory: as sdbg_bm25_topk_batch; a batch whose queries take several of the shapes above also holds its per-shape rows
+ * in HBM (n_queries * (8k + 12) B) before they go to query order on the device.
  * Not supported yet: the streaming scan (sdbg_bm25_scan*), grouped forms of sdbg_bm25_topk_batch_device and
  * sdbg_dist_bm25_topk_batch, deeper nesting (an OR of ANDs), more than 16 positive terms, phrases. */
 int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,

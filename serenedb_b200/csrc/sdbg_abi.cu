@@ -76,7 +76,7 @@ struct sdbg_ctx {
   std::string err;
   uint64_t launches = 0;
   DevBuf scratch[16];
-  // the full-text count, facet, aggregate and sorted passes: [0] the call's region (a dist rank's buffer), [1] the
+  // the full-text top-k, count, facet, aggregate and sorted passes: [0] the call's region (a dist rank's buffer), [1] the
   // gathered buffers, [2] per-shape rows of a mixed-shape batch, [3] count scratch and the merged cells
   DevBuf pass[4];
   DevBuf stage_raw;          // raw int64 values of a column being packed at staging (reused: restaging allocates nothing)
@@ -84,7 +84,7 @@ struct sdbg_ctx {
   size_t h_pinned_cap = 0;
   void* flush = nullptr;
   size_t flush_bytes = 0;
-  cudaEvent_t ev_copy[16] = {};   // one per host conversion thread (sdbg_bm25_topk_batch)
+  cudaEvent_t ev_copy[16] = {};   // one per host conversion thread of a top-k copy back (topk_to_host)
   bool topk_attr_set = false;   // topk_smem_attrs has run
   void* nccl_comm = nullptr;   // ncclComm_t once sdbg_dist_init ran
   // pinned [2]: out-of-range key count of the last deferred GROUP BY partial, and the number of SUM(double) partials
@@ -1131,25 +1131,267 @@ int topk_limits(sdbg_ctx* c, size_t nq, uint32_t k) {
   return SDBG_OK;
 }
 
-// A query of OR groups (Q.term_grp) runs as the OR of all its terms, and a doc must also occur in as many lists of every
-// group as the group needs.
-int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm25_term>& Q, float k1, const float b,
-             const sdbg_col_pred* filt, uint32_t k, float threshold_in, TopkDevOut* dev) {
-  const auto& [kind, terms, term_off, nq, excl_terms, excl_off, term_grp] = Q;
-  if (!segs || !n_segs || !terms || !term_off || !nq || !k) return SDBG_EINVAL;
+// A batch of group queries split by shape. Shape 0: one group, run as the flat OR of its terms; 1: every group one term,
+// run as the AND; 2: a true nested query, run with its groups (term_grp). Each shape becomes a batch of the existing
+// entry points' form: terms / term_off / excl_terms / excl_off over its queries, in batch order.
+template <class Term>
+struct GroupSplit {
+  std::vector<uint32_t> qs[3];   // the batch positions of each shape's queries
+  std::vector<Term> terms[3];
+  std::vector<uint32_t> term_off[3], excl_terms[3], excl_off[3];
+  std::vector<uint8_t> term_grp[3];
+  uint32_t total_excl[3] = {};   // per shape, as check_query_batch sets it
+  int whole = -1;                 // the shape of a batch of one shape; -1: several
+
+  QueryBatch<Term> view(int sh) const {
+    return {sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR, terms[sh].data(), term_off[sh].data(), qs[sh].size(),
+            excl_terms[sh].empty() ? nullptr : excl_terms[sh].data(), excl_off[sh].data(),
+            sh == 2 ? term_grp[sh].data() : nullptr};
+  }
+};
+
+// Splits a batch of sdbg_*_batch_groups(_min) by shape and checks it, every shape included, before anything is queued:
+// non-decreasing query_group_off / group_off / excl_off, 1..16 groups, 1..16 positive terms and at most 16 excluded ones
+// per query, no empty group, no positive term id twice in a query, 1 <= group_min[g] <= the group's size; then
+// check_query_batch on every shape.
+// group_min (NULL: every group 1) is normalised first: a group that needs all its s terms is s single-term groups, so
+// that a query whose groups then all need 1 term takes the shapes above with exactly their results. The remaining queries
+// (some group needs 2 <= m < s terms, so m <= 15) run with their groups, and each term's tag carries m - 1 in its high
+// nibble (kCheckExcl's comment).
+template <class Term>
+int split_groups(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* group_off,
+                 const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                 const uint32_t* excl_off, const sdbg_col_pred* filt, GroupSplit<Term>& S) {
+  sdbg_ctx* c = segs[0]->ctx;
+  for (size_t q = 0; q < nq; ++q) {
+    if (query_group_off[q + 1] < query_group_off[q]) return fail(c, SDBG_EINVAL, "query_group_off must be non-decreasing");
+    for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g)
+      if (group_off[g + 1] < group_off[g]) return fail(c, SDBG_EINVAL, "group_off must be non-decreasing");
+    if (excl_off && excl_off[q + 1] < excl_off[q]) return fail(c, SDBG_EINVAL, "excl_off must be non-decreasing");
+  }
+  for (size_t q = 0; q < nq; ++q) {
+    const uint32_t ng = query_group_off[q + 1] - query_group_off[q];
+    if (ng == 0 || ng > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 groups");
+    const uint32_t t0 = group_off[query_group_off[q]], t1 = group_off[query_group_off[q + 1]];
+    if (t1 - t0 > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 terms");
+    if (excl_off && excl_off[q + 1] - excl_off[q] > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
+  }
+  for (size_t q = 0; q < nq; ++q) {
+    for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g) {
+      if (group_off[g + 1] == group_off[g]) return fail(c, SDBG_EINVAL, "empty OR group");
+      if (group_min && (group_min[g] == 0 || group_min[g] > group_off[g + 1] - group_off[g]))
+        return fail(c, SDBG_EINVAL, "a group's minimum match count must be 1..its number of terms");
+    }
+    const uint32_t t0 = group_off[query_group_off[q]], t1 = group_off[query_group_off[q + 1]];
+    if (!terms) return fail(c, SDBG_EINVAL, "terms is NULL");
+    if (excl_off && excl_off[q + 1] > excl_off[q] && !excl_terms) return fail(c, SDBG_EINVAL, "excl_terms is NULL");
+    std::array<uint32_t, kMaxQueryTerms> ids;
+    for (uint32_t i = t0; i < t1; ++i) ids[i - t0] = term_id(terms[i]);
+    std::sort(ids.begin(), ids.begin() + (t1 - t0));
+    if (std::adjacent_find(ids.begin(), ids.begin() + (t1 - t0)) != ids.begin() + (t1 - t0))
+      return fail(c, SDBG_EINVAL, "a positive term id occurs twice in a query");
+  }
+  for (int sh = 0; sh < 3; ++sh) { S.term_off[sh].assign(1, 0u); S.excl_off[sh].assign(1, 0u); }
+  for (size_t q = 0; q < nq; ++q) {
+    const uint32_t g0 = query_group_off[q], g1 = query_group_off[q + 1];
+    const uint32_t t0 = group_off[g0], t1 = group_off[g1];
+    // normalised groups: m == s becomes s single-term groups; a group of 2 <= m < s keeps its m
+    uint32_t n_groups = 0;
+    bool min_group = false;
+    for (uint32_t g = g0; g < g1; ++g) {
+      const uint32_t s = group_off[g + 1] - group_off[g], m = group_min ? group_min[g] : 1u;
+      if (m == s) n_groups += s;
+      else { ++n_groups; min_group |= m > 1u; }
+    }
+    const int sh = min_group ? 2 : n_groups == 1 ? 0 : (t1 - t0 == n_groups ? 1 : 2);
+    S.qs[sh].push_back(uint32_t(q));
+    uint32_t gi = 0;
+    for (uint32_t g = g0; g < g1; ++g) {
+      const uint32_t s = group_off[g + 1] - group_off[g], m = group_min ? group_min[g] : 1u;
+      for (uint32_t i = group_off[g]; i < group_off[g + 1]; ++i) {
+        S.terms[sh].push_back(terms[i]);
+        if (sh == 2) S.term_grp[sh].push_back(m == s ? uint8_t(gi++) : uint8_t(gi | ((m - 1u) << 4)));
+      }
+      if (m != s) ++gi;
+    }
+    S.term_off[sh].push_back(uint32_t(S.terms[sh].size()));
+    if (excl_off)
+      for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) S.excl_terms[sh].push_back(excl_terms[i]);
+    S.excl_off[sh].push_back(uint32_t(S.excl_terms[sh].size()));
+  }
+  for (int sh = 0; sh < 3; ++sh) {
+    if (S.qs[sh].empty()) continue;
+    if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &S.total_excl[sh])) return rc;
+    if (S.qs[sh].size() == nq) S.whole = sh;
+  }
+  return SDBG_OK;
+}
+
+// The queries of one call, checked before anything is queued (rc: the checks' result): a batch that runs whole (a flat
+// batch, or a group batch of one shape), or a group batch of several shapes (S; whole.nq == 0). Term: sdbg_bm25_term for
+// the top-k, the bare term id for the count, facet, aggregate and sorted passes.
+template <class Term>
+struct PassBatch {
+  int rc;
+  size_t nq;
+  QueryBatch<Term> whole{};
+  uint32_t total_excl = 0;   // whole's, as check_query_batch sets it
+  GroupSplit<Term> S;
+
+  PassBatch(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<Term>& Q, const sdbg_col_pred* filt) : nq(Q.nq), whole(Q) {
+    rc = !segs || !n_segs || !Q.terms || !Q.term_off || !Q.nq ? SDBG_EINVAL : check_query_batch(segs, n_segs, Q, filt, &total_excl);
+  }
+  PassBatch(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* group_off, const uint32_t* query_group_off,
+            const uint32_t* group_min, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt)
+      : nq(nq) {
+    rc = split_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, S);
+    if (S.whole >= 0) { whole = S.view(S.whole); total_excl = S.total_excl[S.whole]; }
+  }
+  PassBatch(const PassBatch&) = delete;   // whole may point into S
+};
+
+// dst row to[j] = src row j, rows of row_words words.
+template <class Word>
+__global__ void __launch_bounds__(256) scatter_rows_kernel(const Word* __restrict__ src, Word* __restrict__ dst,
+                                                           const uint32_t* __restrict__ to, size_t n_rows, size_t row_words) {
+  const size_t n = n_rows * row_words;
+  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
+    const size_t j = i / row_words;
+    dst[size_t(to[j]) * row_words + (i - j * row_words)] = src[i];
+  }
+}
+
+// Runs the shapes of a mixed-shape batch S one after another, each into zeroed rows of its own (c->pass[2]):
+// run(sh, part) fills shape sh's rows part[i], row[i] bytes per query (0: no such array), and scatter_rows_kernel moves
+// them to the caller's query positions in dst[i] on the stream (rows of u32 words when row[i] is not a multiple of 8,
+// else of u64 words). Nothing waits.
+template <class Term, class Run>
+int shapes_run(sdbg_ctx* c, const GroupSplit<Term>& S, const std::array<size_t, 3>& row, void* const (&dst)[3], Run run) {
+  const auto pad = [](size_t b) { return (b + 7) & ~size_t(7); };
+  // per shape: its query positions (u32), then its rows of each array, every part 8-byte aligned
+  size_t pos[3] = {}, bytes = 0;
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    pos[sh] = bytes;
+    bytes += pad(n * 4);
+    for (size_t r : row) bytes += pad(n * r);
+  }
+  if (int rc = ensure(c, c->pass[2], bytes)) return rc;
+  char* d = static_cast<char*>(c->pass[2].p);
+  CU(c, cudaMemsetAsync(d, 0, bytes, c->stream));
+  for (int sh = 0; sh < 3; ++sh)   // pageable: consumed on return
+    if (!S.qs[sh].empty()) CU(c, cudaMemcpyAsync(d + pos[sh], S.qs[sh].data(), S.qs[sh].size() * 4, cudaMemcpyHostToDevice, c->stream));
+  for (int sh = 0; sh < 3; ++sh) {
+    const size_t n = S.qs[sh].size();
+    if (!n) continue;
+    const auto* to = reinterpret_cast<const uint32_t*>(d + pos[sh]);
+    void* part[3];
+    char* p = d + pos[sh] + pad(n * 4);
+    for (int i = 0; i < 3; ++i) { part[i] = p; p += pad(n * row[i]); }
+    if (int rc = run(sh, part)) return rc;
+    for (int i = 0; i < 3; ++i) {
+      if (!row[i]) continue;
+      const size_t words = row[i] % 8 ? row[i] / 4 : row[i] / 8;
+      const unsigned grid = unsigned(std::min<size_t>((n * words + 255) / 256, size_t(c->sm_count) * 8));
+      if (row[i] % 8)
+        scatter_rows_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const uint32_t*>(part[i]), static_cast<uint32_t*>(dst[i]),
+                                                         to, n, words);
+      else
+        scatter_rows_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const unsigned long long*>(part[i]),
+                                                         static_cast<unsigned long long*>(dst[i]), to, n, words);
+      ++c->launches;
+    }
+    CU(c, cudaGetLastError());
+  }
+  return SDBG_OK;
+}
+
+// The top-k entries' checks of their scalar arguments, before their batch's (PassBatch).
+int topk_args(sdbg_segment* const* segs, size_t n_segs, size_t nq, uint32_t k) {
+  if (!segs || !n_segs || !segs[0] || !nq || !k) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
   if (int rc = topk_limits(c, nq, k)) return rc;
   CU(c, cudaSetDevice(c->device));
-  const uint32_t total_terms = term_off[nq];
-  uint32_t total_excl = 0;   // > 0: some query excludes terms
-  if (int rc = check_query_batch(segs, n_segs, Q, filt, &total_excl)) return rc;
+  return SDBG_OK;
+}
+
+// The top-k entries' checks after topk_args and their batch's: at most 2^32 - 2 docs per call (the kernels' ordinals).
+int topk_checked(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_bm25_term>& B) {
+  if (B.rc) return B.rc;
   uint64_t ord = 0;
-  uint32_t max_docs = 0;
-  for (size_t si = 0; si < n_segs; ++si) {
-    ord += segs[si]->n_docs;
-    max_docs = std::max(max_docs, segs[si]->n_docs);
+  for (size_t si = 0; si < n_segs; ++si) ord += segs[si]->n_docs;
+  if (ord > kMaxDocId) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "more than 2^32-2 docs per call");
+  return SDBG_OK;
+}
+
+// The descriptor block of the top-k kernels (TopkParams, MergeParams::list_off), staged in pageable memory for one copy:
+// [QTermDev [segment][term_off[nq]], each query's terms by ascending docs_count (conjunction.hpp:520-523) | term_off
+// [nq + 1] | from 16 B on, the work items {query, first doc, docs, candidate list} | list_off [nq + 1] | when some query
+// has per-doc checks, from 16 B on: {first block, blocks} [segment][check] | chk_off [nq + 1] | with Q.term_grp, each
+// check's group tag].
+struct TopkDesc {
+  std::vector<char> h;
+  size_t n_segs, n_terms, n_chk, off_pos, work_pos, list_pos, x_pos, chk_off_pos, grp_pos;
+  bool grp;
+
+  // Points segment si's launch parameters at the block's device copy d, its work items from `first` on.
+  void params(const char* d, size_t si, size_t first, TopkParams& P) const {
+    P.qterms = reinterpret_cast<const QTermDev*>(d) + si * n_terms;
+    P.qterm_off = reinterpret_cast<const uint32_t*>(d + off_pos);
+    P.work = reinterpret_cast<const uint4*>(d + work_pos) + first;
+    if (!n_chk) return;
+    P.excl = reinterpret_cast<const uint2*>(d + x_pos) + si * n_chk;
+    P.excl_off = reinterpret_cast<const uint32_t*>(d + chk_off_pos);
+    if (grp) P.excl_grp = reinterpret_cast<const uint8_t*>(d + grp_pos);
   }
-  if (ord > kMaxDocId) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-2 docs per call");
+};
+
+// Writes the descriptor block of queries Q over segs (term ids checked): work items `work`, list_off, and the per-doc
+// check lists chk_terms[chk_off[q] .. chk_off[q + 1]) of query q with their group tags chk_grp (Q.term_grp).
+TopkDesc topk_desc(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm25_term>& Q, float k1, float b,
+                   const std::vector<uint4>& work, const std::vector<uint32_t>& list_off, const std::vector<uint32_t>& chk_terms,
+                   const std::vector<uint32_t>& chk_off, const std::vector<uint8_t>& chk_grp) {
+  const size_t nq = Q.nq, n_terms = Q.term_off[nq], n_chk = chk_terms.size(), off_bytes = (nq + 1) * sizeof(uint32_t);
+  TopkDesc D{{}, n_segs, n_terms, n_chk, 0, 0, 0, 0, 0, 0, Q.term_grp != nullptr};
+  D.off_pos = n_terms * sizeof(QTermDev) * n_segs;
+  D.work_pos = (D.off_pos + off_bytes + 15) & ~size_t(15);   // work items are 16-byte loads
+  D.list_pos = D.work_pos + work.size() * sizeof(uint4);
+  D.x_pos = (D.list_pos + off_bytes + 15) & ~size_t(15);
+  D.chk_off_pos = D.x_pos + n_chk * n_segs * sizeof(uint2);
+  D.grp_pos = D.chk_off_pos + off_bytes;
+  D.h.resize(n_chk ? D.grp_pos + (D.grp ? n_chk : 0) : D.list_pos + off_bytes);
+  char* h = D.h.data();
+  for (size_t si = 0; si < n_segs; ++si) {
+    QTermDev* dst = reinterpret_cast<QTermDev*>(h) + si * n_terms;
+    for (size_t q = 0; q < nq; ++q) {
+      const uint32_t t_begin = Q.term_off[q], t_end = Q.term_off[q + 1];
+      for (uint32_t i = t_begin; i < t_end; ++i) fill_qterm(segs[si], Q.terms[i], k1, b, dst[i]);
+      std::stable_sort(dst + t_begin, dst + t_end, [](const QTermDev& x, const QTermDev& y) { return x.docs_count < y.docs_count; });
+    }
+  }
+  std::memcpy(h + D.off_pos, Q.term_off, off_bytes);
+  std::memcpy(h + D.work_pos, work.data(), work.size() * sizeof(uint4));
+  std::memcpy(h + D.list_pos, list_off.data(), off_bytes);
+  if (n_chk) {
+    auto* x = reinterpret_cast<uint2*>(h + D.x_pos);
+    for (size_t si = 0; si < n_segs; ++si)
+      for (size_t i = 0; i < n_chk; ++i) x[si * n_chk + i] = excl_list(segs[si], chk_terms[i]);
+    std::memcpy(h + D.chk_off_pos, chk_off.data(), off_bytes);
+    if (D.grp) std::memcpy(h + D.grp_pos, chk_grp.data(), n_chk);
+  }
+  return D;
+}
+
+// Queues a batch that passed topk_args and topk_checked (total_excl: as check_query_batch set it) into the device arrays
+// out: keys [nq][k] (sorted descending, then zeros), n_out [nq] and total [nq] (NULL: not wanted). The descriptors are
+// staged from pageable memory, which the copy has consumed when it returns, so the shapes of a mixed batch follow one
+// another without a wait. A query of OR groups (Q.term_grp) runs as the OR of all its terms, and a doc must also occur in
+// as many lists of every group as the group needs.
+int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm25_term>& Q, uint32_t total_excl, float k1,
+             const float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, const TopkDevOut& out) {
+  const auto& [kind, terms, term_off, nq, excl_terms, excl_off, term_grp] = Q;
+  sdbg_ctx* c = segs[0]->ctx;
+  const uint32_t total_terms = term_off[nq];
   // Per-doc check lists of each query: its excluded terms (tag kCheckExcl), then, for a query of OR groups, each positive
   // term tagged with its group. chk_off[q] .. chk_off[q + 1] index chk_terms / chk_grp.
   std::vector<uint32_t> chk_off, chk_terms;
@@ -1291,55 +1533,20 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm2
   const size_t smem_drive = pl.smem + size_t(entries) * 4;   // probe list | decode-fallback list
   if (smem_drive > 200 * 1024) return fail(c, SDBG_EUNSUPPORTED, "hash window + candidate buffer exceed shared memory");
 
-  // host-side query descriptors, per segment, sorted by ascending docs_count (conjunction.hpp:520-523)
-  const size_t qt_bytes = size_t(total_terms) * sizeof(QTermDev) * n_segs;
-  const size_t off_bytes = (nq + 1) * sizeof(uint32_t);
-  const size_t work_bytes = total_work * sizeof(uint4);
-  const size_t qt_pad = (qt_bytes + off_bytes + 15) & ~size_t(15);   // work items are 16-byte loads
-  // check lists, when there are any: [uint2 {first block, blocks} x total_chk per segment | chk_off | group tags when
-  // term_grp]
-  const size_t x_pos = (qt_pad + work_bytes + off_bytes + 15) & ~size_t(15);
-  const size_t x_lists = size_t(total_chk) * n_segs * sizeof(uint2);
-  const size_t desc_bytes = total_chk ? x_pos + x_lists + off_bytes + (term_grp ? total_chk : 0) : qt_pad + work_bytes + off_bytes;
-  int rc = ensure_pinned(c, desc_bytes);
-  if (rc) return rc;
-  auto* h_qt = static_cast<QTermDev*>(c->h_pinned);
-  auto* h_off = reinterpret_cast<uint32_t*>(static_cast<char*>(c->h_pinned) + qt_bytes);
-  std::memcpy(h_off, term_off, off_bytes);
-  {
-    auto* h_work = reinterpret_cast<uint4*>(static_cast<char*>(c->h_pinned) + qt_pad);
-    for (auto& w : seg_work) for (const WorkItem& it : w) *h_work++ = make_uint4(it.q, it.lo, it.len, it.list);
-    std::memcpy(static_cast<char*>(c->h_pinned) + qt_pad + work_bytes, list_off.data(), off_bytes);
-  }
-  if (total_chk) {
-    auto* h_x = reinterpret_cast<uint2*>(static_cast<char*>(c->h_pinned) + x_pos);
-    for (size_t si = 0; si < n_segs; ++si)
-      for (uint32_t i = 0; i < total_chk; ++i) h_x[si * total_chk + i] = excl_list(segs[si], chk_terms[i]);
-    std::memcpy(static_cast<char*>(c->h_pinned) + x_pos + x_lists, chk_off.data(), off_bytes);
-    if (term_grp) std::memcpy(static_cast<char*>(c->h_pinned) + x_pos + x_lists + off_bytes, chk_grp.data(), total_chk);
-  }
-  for (size_t si = 0; si < n_segs; ++si) {
-    const sdbg_segment* s = segs[si];
-    QTermDev* dst = h_qt + si * total_terms;
-    for (size_t q = 0; q < nq; ++q) {
-      const uint32_t t_begin = term_off[q], t_end = term_off[q + 1];
-      for (uint32_t i = t_begin; i < t_end; ++i) {
-        fill_qterm(s, terms[i], k1, b, dst[i]);
-      }
-      std::stable_sort(dst + t_begin, dst + t_end, [](const QTermDev& x, const QTermDev& y) { return x.docs_count < y.docs_count; });
-    }
-  }
-  DevBuf& b_qt = c->scratch[0]; DevBuf& b_theta = c->scratch[1]; DevBuf& b_cand = c->scratch[2];
-  DevBuf& b_candn = c->scratch[3]; DevBuf& b_keys = c->scratch[4]; DevBuf& b_small = c->scratch[5];
-  if ((rc = ensure(c, b_qt, desc_bytes))) return rc;
-  if ((rc = ensure(c, b_theta, nq * 16))) return rc;  // theta[nq] | total[nq]
+  std::vector<uint4> work;
+  work.reserve(total_work);
+  for (auto& w : seg_work) for (const WorkItem& it : w) work.push_back(make_uint4(it.q, it.lo, it.len, it.list));
+  const TopkDesc D = topk_desc(segs, n_segs, Q, k1, b, work, list_off, chk_terms, chk_off, chk_grp);
+  DevBuf& b_qt = c->scratch[0]; DevBuf& b_theta = c->scratch[1]; DevBuf& b_cand = c->scratch[2]; DevBuf& b_candn = c->scratch[3];
+  int rc;
+  if ((rc = ensure(c, b_qt, D.h.size()))) return rc;
+  if ((rc = ensure(c, b_theta, nq * 16))) return rc;  // theta[nq] | total[nq] when out.total is NULL
   if ((rc = ensure(c, b_cand, size_t(total_lists) * pl.cap * 8))) return rc;
   if ((rc = ensure(c, b_candn, size_t(total_lists) * 4))) return rc;
-  if ((rc = ensure(c, b_keys, nq * size_t(k) * 8))) return rc;
-  if ((rc = ensure(c, b_small, nq * 4))) return rc;
-  CU(c, cudaMemcpyAsync(b_qt.p, c->h_pinned, desc_bytes, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(b_qt.p, D.h.data(), D.h.size(), cudaMemcpyHostToDevice, c->stream));
+  const char* d_desc = static_cast<const char*>(b_qt.p);
   auto* d_theta = static_cast<unsigned long long*>(b_theta.p);
-  auto* d_total = d_theta + nq;
+  auto* d_total = out.total ? out.total : d_theta + nq;
   uint32_t thr_bits; std::memcpy(&thr_bits, &threshold_in, 4);
   if (!(threshold_in >= 0.f)) thr_bits = 0;  // negative / NaN seeds accept every positive score
   fill_u64_kernel<<<64, 256, 0, c->stream>>>(d_theta, nq, (static_cast<unsigned long long>(thr_bits) << 32) | 0xFFFFFFFFull);
@@ -1371,21 +1578,15 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm2
       TopkParams P;
       P.seg = postings_view(s, base);
       if ((rc = filter_view(s, filt, &P.filt))) return rc;
-      P.qterms = static_cast<const QTermDev*>(b_qt.p) + si * total_terms;
-      P.qterm_off = reinterpret_cast<const uint32_t*>(static_cast<const char*>(b_qt.p) + qt_bytes);
+      D.params(d_desc, si, work_done, P);
+      const uint4* const work0 = P.work;
+      work_done += seg_work[si].size();
       P.theta = d_theta; P.total = d_total;
       P.cand = static_cast<unsigned long long*>(b_cand.p);
       P.cand_n = static_cast<uint32_t*>(b_candn.p);
       P.k = k; P.cap = pl.cap; P.conjunction = kind == SDBG_QUERY_AND ? 1 : 0;
       P.claim = nullptr;
-      if (total_chk) {
-        P.excl = reinterpret_cast<const uint2*>(static_cast<const char*>(b_qt.p) + x_pos) + si * total_chk;
-        P.excl_off = reinterpret_cast<const uint32_t*>(static_cast<const char*>(b_qt.p) + x_pos + x_lists);
-        if (term_grp) P.excl_grp = reinterpret_cast<const uint8_t*>(static_cast<const char*>(b_qt.p) + x_pos + x_lists + off_bytes);
-      }
       const int wand = seg_wand(s);
-      const uint4* const work0 = reinterpret_cast<const uint4*>(static_cast<const char*>(b_qt.p) + qt_pad) + work_done;
-      work_done += seg_work[si].size();
       std::array<size_t, kAllClasses> cls_off{};
       { size_t o = 0; for (uint32_t cls = 0; cls < kAllClasses; ++cls) { cls_off[cls] = o; o += n_cls[si][cls]; } }
       auto launch_merge = [&](uint32_t T, size_t n, cudaStream_t st) {
@@ -1460,38 +1661,107 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm2
   MergeParams M;
   M.cand = static_cast<const unsigned long long*>(b_cand.p);
   M.cand_n = static_cast<const uint32_t*>(b_candn.p);
-  M.list_off = reinterpret_cast<const uint32_t*>(static_cast<const char*>(b_qt.p) + qt_pad + work_bytes);
+  M.list_off = reinterpret_cast<const uint32_t*>(d_desc + D.list_pos);
   M.G = 0; M.stride = pl.cap; M.k = k; M.cap = pl.cap;
-  M.keys_out = static_cast<unsigned long long*>(b_keys.p);
-  M.n_out = static_cast<uint32_t*>(b_small.p);
+  M.keys_out = out.keys;
+  M.n_out = out.n_out;
   { ProfScope ps_(c, kProfMerge);
     topk_merge_kernel<<<unsigned(nq), kTopkThreads, size_t(pl.cap) * 8, c->stream>>>(M); }
   ++c->launches;
   CU(c, cudaGetLastError());
-  dev->keys = M.keys_out; dev->n_out = M.n_out; dev->total = d_total;
   return SDBG_OK;
 }
 
-// keys -> hits on the host. `bases` = first ordinal of each segment.
-void keys_to_hits(const unsigned long long* keys, uint32_t n, const std::vector<uint64_t>& bases, sdbg_hit* out) {
-  if (bases.size() == 1) {                      // one segment: no search for the owner of an ordinal
-    const uint32_t b0 = uint32_t(bases[0]);
-    for (uint32_t i = 0; i < n; ++i) {
-      const uint32_t bits = uint32_t(keys[i] >> 32);
-      std::memcpy(&out[i].score, &bits, 4);
-      out[i].seg = 0;
-      out[i].doc = ~uint32_t(keys[i]) - b0;
+// Copies a top-k result d back through the pinned staging, [keys | total (when d.total) | n_out], and converts it into
+// the caller's arrays: hit i of query q is keys[q][i] as {score bits, decode(ordinal)}, with total_matches[q] (NULL: not
+// wanted) when d has totals. Turning keys into hits is a few ns per hit; a large batch (millions of hits) is cut into
+// per-thread query ranges whose keys are copied back one after the other, each followed by an event: a thread converts
+// its range as soon as it has landed, while the later ranges are still on the wire. One wait at the end.
+template <class Decode>
+int topk_to_host(sdbg_ctx* c, const TopkDevOut& d, size_t nq, uint32_t k, Decode decode, sdbg_hit* out, uint32_t* n_out,
+                 uint64_t* total_matches) {
+  const size_t kb = nq * size_t(k) * 8, tb = d.total ? nq * 8 : 0, nb = nq * 4;
+  if (int rc = ensure_pinned(c, kb + tb + nb)) return rc;
+  char* h = static_cast<char*>(c->h_pinned);
+  const size_t n_thr = std::max<size_t>(1, std::min<size_t>({size_t(env_int("SDBG_HOST_THREADS", 16)), (nq * size_t(k)) / 65536, size_t(kMaxCopyEvents)}));
+  if (tb) CU(c, cudaMemcpyAsync(h + kb, d.total, tb, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaMemcpyAsync(h + kb + tb, d.n_out, nb, cudaMemcpyDeviceToHost, c->stream));
+  for (size_t t = 0; t < n_thr; ++t) {
+    const size_t q0 = nq * t / n_thr, q1 = nq * (t + 1) / n_thr;
+    CU(c, cudaMemcpyAsync(h + q0 * k * 8, d.keys + q0 * k, (q1 - q0) * k * 8, cudaMemcpyDeviceToHost, c->stream));
+    if (n_thr > 1) {
+      if (!c->ev_copy[t]) CU(c, cudaEventCreateWithFlags(&c->ev_copy[t], cudaEventDisableTiming));
+      CU(c, cudaEventRecord(c->ev_copy[t], c->stream));
     }
-    return;
   }
-  for (uint32_t i = 0; i < n; ++i) {
-    const uint32_t bits = uint32_t(keys[i] >> 32);
-    const uint32_t ordinal = ~uint32_t(keys[i]);
-    size_t seg = std::upper_bound(bases.begin(), bases.end(), uint64_t(ordinal) - 1) - bases.begin() - 1;
-    std::memcpy(&out[i].score, &bits, 4);
-    out[i].seg = uint32_t(seg);
-    out[i].doc = uint32_t(ordinal - bases[seg]);
+  const auto* keys = reinterpret_cast<const unsigned long long*>(h);
+  const auto* tot = reinterpret_cast<const unsigned long long*>(h + kb);
+  const auto* cnt = reinterpret_cast<const uint32_t*>(h + kb + tb);
+  auto convert = [&](size_t q0, size_t q1) {
+    for (size_t q = q0; q < q1; ++q) {
+      n_out[q] = cnt[q];
+      for (uint32_t i = 0; i < cnt[q]; ++i) {
+        const unsigned long long key = keys[q * k + i];
+        const uint32_t bits = uint32_t(key >> 32);
+        sdbg_hit& hit = out[q * k + i];
+        std::memcpy(&hit.score, &bits, 4);
+        const uint2 sd = decode(~uint32_t(key));
+        hit.seg = sd.x;
+        hit.doc = sd.y;
+      }
+      if (tb && total_matches) total_matches[q] = tot[q];
+    }
+  };
+  if (n_thr <= 1) {
+    CU(c, cudaStreamSynchronize(c->stream));
+    convert(0, nq);
+  } else {
+    std::atomic<int> err{0};
+    std::vector<std::thread> pool;
+    for (size_t t = 0; t < n_thr; ++t)
+      pool.emplace_back([&, t] {
+        if (cudaSetDevice(c->device) != cudaSuccess || cudaEventSynchronize(c->ev_copy[t]) != cudaSuccess) { err = 1; return; }
+        convert(nq * t / n_thr, nq * (t + 1) / n_thr);
+      });
+    for (auto& th : pool) th.join();
+    CU(c, cudaStreamSynchronize(c->stream));
+    if (err) return fail(c, SDBG_ECUDA, "copying the hits back failed");
   }
+  return SDBG_OK;
+}
+
+// The host top-k entries after topk_args and their batch (B): runs it into the call's region in c->pass[0], [keys
+// [nq][k] | total [nq] | n_out [nq]] (topk_run for a whole batch, else shape by shape through shapes_run), and copies
+// it back (topk_to_host) with each ordinal decoded into {segment, doc}.
+int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_bm25_term>& B, float k1, float b,
+                    const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
+                    uint64_t* total_matches) {
+  if (int rc = topk_checked(segs, n_segs, B)) return rc;
+  sdbg_ctx* c = segs[0]->ctx;
+  const size_t nq = B.nq, kb = nq * size_t(k) * 8;
+  if (int rc = ensure(c, c->pass[0], kb + nq * 12)) return rc;
+  char* d = static_cast<char*>(c->pass[0].p);
+  const TopkDevOut dev{reinterpret_cast<unsigned long long*>(d), reinterpret_cast<uint32_t*>(d + kb + nq * 8),
+                       reinterpret_cast<unsigned long long*>(d + kb)};
+  int rc;
+  if (B.whole.nq) {
+    rc = topk_run(segs, n_segs, B.whole, B.total_excl, k1, b, filt, k, threshold_in, dev);
+  } else {
+    rc = shapes_run(c, B.S, {size_t(k) * 8, 8, 4}, {dev.keys, dev.total, dev.n_out}, [&](int sh, void* const* part) {
+      const TopkDevOut o{static_cast<unsigned long long*>(part[0]), static_cast<uint32_t*>(part[2]),
+                         static_cast<unsigned long long*>(part[1])};
+      return topk_run(segs, n_segs, B.S.view(sh), B.S.total_excl[sh], k1, b, filt, k, threshold_in, o);
+    });
+  }
+  if (rc) return rc;
+  std::vector<uint64_t> bases(n_segs);   // the first ordinal of each segment
+  uint64_t ord0 = 0;
+  for (size_t si = 0; si < n_segs; ++si) { bases[si] = ord0; ord0 += segs[si]->n_docs; }
+  return topk_to_host(c, dev, nq, k, [&](uint32_t ordinal) {
+    if (n_segs == 1) return make_uint2(0u, ordinal);   // one segment: no search for the owner of an ordinal
+    const size_t seg = std::upper_bound(bases.begin(), bases.end(), uint64_t(ordinal) - 1) - bases.begin() - 1;
+    return make_uint2(uint32_t(seg), uint32_t(ordinal - bases[seg]));
+  }, out, n_out, total_matches);
 }
 
 }  // namespace
@@ -1533,230 +1803,35 @@ extern "C" int sdbg_tfidf_topk_batch(sdbg_segment* const* segs, size_t n_segs, i
                               total_matches);
 }
 
-namespace {
-int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm25_term>& Q, float k1, float b,
-                    const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
-                    uint64_t* total_matches) {
-  if (!out || !n_out) return SDBG_EINVAL;
-  TopkDevOut dev{};
-  int rc = topk_run(segs, n_segs, Q, k1, b, filt, k, threshold_in, &dev);
-  if (rc) return rc;
-  sdbg_ctx* c = segs[0]->ctx;
-  const size_t nq = Q.nq;
-  const size_t kb = nq * size_t(k) * 8, nb = nq * 4, tb = nq * 8;
-  // results come back through a dedicated pinned block (the query descriptors are done with by now)
-  if ((rc = ensure_pinned(c, kb + nb + tb + 64))) return rc;
-  char* h = static_cast<char*>(c->h_pinned);
-  // key -> {segment, doc, score} is a few ns per hit; a large batch (millions of hits) is cut into per-thread query
-  // ranges whose keys are copied back one after the other, each followed by an event: a thread converts its range as
-  // soon as it has landed, while the later ranges are still on the wire.
-  const size_t n_thr = std::max<size_t>(1, std::min<size_t>({size_t(env_int("SDBG_HOST_THREADS", 16)), (nq * size_t(k)) / 65536, size_t(kMaxCopyEvents)}));
-  CU(c, cudaMemcpyAsync(h + kb, dev.total, tb, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaMemcpyAsync(h + kb + tb, dev.n_out, nb, cudaMemcpyDeviceToHost, c->stream));
-  for (size_t t = 0; t < n_thr; ++t) {
-    const size_t q0 = nq * t / n_thr, q1 = nq * (t + 1) / n_thr;
-    CU(c, cudaMemcpyAsync(h + q0 * k * 8, dev.keys + q0 * k, (q1 - q0) * k * 8, cudaMemcpyDeviceToHost, c->stream));
-    if (n_thr > 1) {
-      if (!c->ev_copy[t]) CU(c, cudaEventCreateWithFlags(&c->ev_copy[t], cudaEventDisableTiming));
-      CU(c, cudaEventRecord(c->ev_copy[t], c->stream));
-    }
-  }
-  std::vector<uint64_t> bases(n_segs);
-  uint64_t ord0 = 0;
-  for (size_t si = 0; si < n_segs; ++si) { bases[si] = ord0; ord0 += segs[si]->n_docs; }
-  const auto* keys = reinterpret_cast<const unsigned long long*>(h);
-  const auto* tot = reinterpret_cast<const unsigned long long*>(h + kb);
-  const auto* cnt = reinterpret_cast<const uint32_t*>(h + kb + tb);
-  auto convert = [&](size_t q0, size_t q1) {
-    for (size_t q = q0; q < q1; ++q) {
-      n_out[q] = cnt[q];
-      keys_to_hits(keys + q * k, cnt[q], bases, out + q * k);
-      if (total_matches) total_matches[q] = tot[q];
-    }
-  };
-  if (n_thr <= 1) {
-    CU(c, cudaStreamSynchronize(c->stream));
-    convert(0, nq);
-  } else {
-    std::atomic<int> err{0};
-    std::vector<std::thread> pool;
-    for (size_t t = 0; t < n_thr; ++t)
-      pool.emplace_back([&, t] {
-        if (cudaSetDevice(c->device) != cudaSuccess || cudaEventSynchronize(c->ev_copy[t]) != cudaSuccess) { err = 1; return; }
-        convert(nq * t / n_thr, nq * (t + 1) / n_thr);
-      });
-    for (auto& th : pool) th.join();
-    CU(c, cudaStreamSynchronize(c->stream));
-    if (err) return fail(c, SDBG_ECUDA, "copying the hits back failed");
-  }
-  return SDBG_OK;
-}
-}  // namespace
-
 extern "C" int sdbg_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
                                     const uint32_t* term_off, size_t nq, float k1, float b, const sdbg_col_pred* filt,
                                     uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
                                     uint64_t* total_matches) {
-  return topk_batch_host(segs, n_segs, {kind, terms, term_off, nq, nullptr, nullptr, nullptr}, k1, b, filt, k, threshold_in, out,
-                         n_out, total_matches);
+  if (!out || !n_out) return SDBG_EINVAL;
+  if (int rc = topk_args(segs, n_segs, nq, k)) return rc;
+  const PassBatch<sdbg_bm25_term> B(segs, n_segs, {kind, terms, term_off, nq, nullptr, nullptr, nullptr}, filt);
+  return topk_batch_host(segs, n_segs, B, k1, b, filt, k, threshold_in, out, n_out, total_matches);
 }
 
 extern "C" int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
                                          const uint32_t* term_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
                                          float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
                                          uint32_t* n_out, uint64_t* total_matches) {
-  if (!excl_off) return SDBG_EINVAL;
-  return topk_batch_host(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, k1, b, filt, k, threshold_in,
-                         out, n_out, total_matches);
+  if (!excl_off || !out || !n_out) return SDBG_EINVAL;
+  if (int rc = topk_args(segs, n_segs, nq, k)) return rc;
+  const PassBatch<sdbg_bm25_term> B(segs, n_segs, {kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  return topk_batch_host(segs, n_segs, B, k1, b, filt, k, threshold_in, out, n_out, total_matches);
 }
-
-// ---- conjunctions of OR groups (`a & (b | c) & !d`) ----
-namespace {
-// A batch of group queries split by shape. Shape 0: one group, run as the flat OR of its terms; 1: every group one term,
-// run as the AND; 2: a true nested query, run with its groups (term_grp). Each shape becomes a batch of the existing
-// entry points' form: terms / term_off / excl_terms / excl_off over its queries, in batch order.
-template <class Term>
-struct GroupSplit {
-  std::vector<uint32_t> qs[3];   // the batch positions of each shape's queries
-  std::vector<Term> terms[3];
-  std::vector<uint32_t> term_off[3], excl_terms[3], excl_off[3];
-  std::vector<uint8_t> term_grp[3];
-  uint32_t total_excl[3] = {};   // per shape, as check_query_batch sets it
-  int whole = -1;                 // the shape of a batch of one shape; -1: several
-
-  QueryBatch<Term> view(int sh) const {
-    return {sh == 1 ? SDBG_QUERY_AND : SDBG_QUERY_OR, terms[sh].data(), term_off[sh].data(), qs[sh].size(),
-            excl_terms[sh].empty() ? nullptr : excl_terms[sh].data(), excl_off[sh].data(),
-            sh == 2 ? term_grp[sh].data() : nullptr};
-  }
-};
-
-// Splits a batch of sdbg_*_batch_groups(_min) by shape and checks it, every shape included, before anything is queued:
-// non-decreasing query_group_off / group_off / excl_off, 1..16 groups, 1..16 positive terms and at most 16 excluded ones
-// per query, no empty group, no positive term id twice in a query, 1 <= group_min[g] <= the group's size; then
-// check_query_batch on every shape.
-// group_min (NULL: every group 1) is normalised first: a group that needs all its s terms is s single-term groups, so
-// that a query whose groups then all need 1 term takes the shapes above with exactly their results. The remaining queries
-// (some group needs 2 <= m < s terms, so m <= 15) run with their groups, and each term's tag carries m - 1 in its high
-// nibble (kCheckExcl's comment).
-template <class Term>
-int split_groups(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* group_off,
-                 const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
-                 const uint32_t* excl_off, const sdbg_col_pred* filt, GroupSplit<Term>& S) {
-  sdbg_ctx* c = segs[0]->ctx;
-  for (size_t q = 0; q < nq; ++q) {
-    if (query_group_off[q + 1] < query_group_off[q]) return fail(c, SDBG_EINVAL, "query_group_off must be non-decreasing");
-    for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g)
-      if (group_off[g + 1] < group_off[g]) return fail(c, SDBG_EINVAL, "group_off must be non-decreasing");
-    if (excl_off && excl_off[q + 1] < excl_off[q]) return fail(c, SDBG_EINVAL, "excl_off must be non-decreasing");
-  }
-  for (size_t q = 0; q < nq; ++q) {
-    const uint32_t ng = query_group_off[q + 1] - query_group_off[q];
-    if (ng == 0 || ng > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 groups");
-    const uint32_t t0 = group_off[query_group_off[q]], t1 = group_off[query_group_off[q + 1]];
-    if (t1 - t0 > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query needs 1..16 terms");
-    if (excl_off && excl_off[q + 1] - excl_off[q] > kMaxQueryTerms) return fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
-  }
-  for (size_t q = 0; q < nq; ++q) {
-    for (uint32_t g = query_group_off[q]; g < query_group_off[q + 1]; ++g) {
-      if (group_off[g + 1] == group_off[g]) return fail(c, SDBG_EINVAL, "empty OR group");
-      if (group_min && (group_min[g] == 0 || group_min[g] > group_off[g + 1] - group_off[g]))
-        return fail(c, SDBG_EINVAL, "a group's minimum match count must be 1..its number of terms");
-    }
-    const uint32_t t0 = group_off[query_group_off[q]], t1 = group_off[query_group_off[q + 1]];
-    if (!terms) return fail(c, SDBG_EINVAL, "terms is NULL");
-    if (excl_off && excl_off[q + 1] > excl_off[q] && !excl_terms) return fail(c, SDBG_EINVAL, "excl_terms is NULL");
-    std::array<uint32_t, kMaxQueryTerms> ids;
-    for (uint32_t i = t0; i < t1; ++i) ids[i - t0] = term_id(terms[i]);
-    std::sort(ids.begin(), ids.begin() + (t1 - t0));
-    if (std::adjacent_find(ids.begin(), ids.begin() + (t1 - t0)) != ids.begin() + (t1 - t0))
-      return fail(c, SDBG_EINVAL, "a positive term id occurs twice in a query");
-  }
-  for (int sh = 0; sh < 3; ++sh) { S.term_off[sh].assign(1, 0u); S.excl_off[sh].assign(1, 0u); }
-  for (size_t q = 0; q < nq; ++q) {
-    const uint32_t g0 = query_group_off[q], g1 = query_group_off[q + 1];
-    const uint32_t t0 = group_off[g0], t1 = group_off[g1];
-    // normalised groups: m == s becomes s single-term groups; a group of 2 <= m < s keeps its m
-    uint32_t n_groups = 0;
-    bool min_group = false;
-    for (uint32_t g = g0; g < g1; ++g) {
-      const uint32_t s = group_off[g + 1] - group_off[g], m = group_min ? group_min[g] : 1u;
-      if (m == s) n_groups += s;
-      else { ++n_groups; min_group |= m > 1u; }
-    }
-    const int sh = min_group ? 2 : n_groups == 1 ? 0 : (t1 - t0 == n_groups ? 1 : 2);
-    S.qs[sh].push_back(uint32_t(q));
-    uint32_t gi = 0;
-    for (uint32_t g = g0; g < g1; ++g) {
-      const uint32_t s = group_off[g + 1] - group_off[g], m = group_min ? group_min[g] : 1u;
-      for (uint32_t i = group_off[g]; i < group_off[g + 1]; ++i) {
-        S.terms[sh].push_back(terms[i]);
-        if (sh == 2) S.term_grp[sh].push_back(m == s ? uint8_t(gi++) : uint8_t(gi | ((m - 1u) << 4)));
-      }
-      if (m != s) ++gi;
-    }
-    S.term_off[sh].push_back(uint32_t(S.terms[sh].size()));
-    if (excl_off)
-      for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) S.excl_terms[sh].push_back(excl_terms[i]);
-    S.excl_off[sh].push_back(uint32_t(S.excl_terms[sh].size()));
-  }
-  for (int sh = 0; sh < 3; ++sh) {
-    if (S.qs[sh].empty()) continue;
-    if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &S.total_excl[sh])) return rc;
-    if (S.qs[sh].size() == nq) S.whole = sh;
-  }
-  return SDBG_OK;
-}
-
-// One per-query output array of a group entry: query q's row is the `bytes` bytes at p + q * bytes (p NULL: not wanted).
-struct OutRows {
-  void* p;
-  size_t bytes;
-};
-
-// Runs a batch of group top-k queries: splits and checks it (split_groups), then runs each shape as a batch of the flat
-// form, run(view, rows). A batch of one shape writes straight into the caller's rows; otherwise each shape writes
-// temporary rows, which go to the caller's query positions. Checks of the result that every shape would make alike (k)
-// are the caller's, before this call.
-template <class Term, size_t N, class Run>
-int run_groups(sdbg_segment* const* segs, size_t n_segs, const Term* terms, const uint32_t* group_off,
-               const uint32_t* query_group_off, const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
-               const uint32_t* excl_off, const sdbg_col_pred* filt, const OutRows (&rows)[N], Run run) {
-  GroupSplit<Term> S;
-  if (int rc = split_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, S)) return rc;
-  if (S.whole >= 0) return run(S.view(S.whole), rows);
-  for (int sh = 0; sh < 3; ++sh) {
-    const std::vector<uint32_t>& qs = S.qs[sh];
-    if (qs.empty()) continue;
-    std::vector<char> tmp[N];
-    OutRows part[N];
-    for (size_t i = 0; i < N; ++i) {
-      if (rows[i].p) tmp[i].resize(qs.size() * rows[i].bytes);
-      part[i] = {rows[i].p ? tmp[i].data() : nullptr, rows[i].bytes};
-    }
-    if (int rc = run(S.view(sh), part)) return rc;
-    for (size_t i = 0; i < N; ++i)
-      if (rows[i].p)
-        for (size_t j = 0; j < qs.size(); ++j)
-          std::memcpy(static_cast<char*>(rows[i].p) + qs[j] * rows[i].bytes, tmp[i].data() + j * rows[i].bytes, rows[i].bytes);
-  }
-  return SDBG_OK;
-}
-}  // namespace
 
 extern "C" int sdbg_bm25_topk_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
                                                const uint32_t* group_off, const uint32_t* query_group_off, const uint32_t* group_min,
                                                size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, float k1, float b,
                                                const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
                                                uint32_t* n_out, uint64_t* total_matches) {
-  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !out || !n_out) return SDBG_EINVAL;
-  if (int rc = topk_limits(segs[0]->ctx, nq, k)) return rc;
-  return run_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt,
-                    {{out, k * sizeof(sdbg_hit)}, {n_out, 4}, {total_matches, 8}},
-                    [&](const QueryBatch<sdbg_bm25_term>& Q, const OutRows* r) {
-                      return topk_batch_host(segs, n_segs, Q, k1, b, filt, k, threshold_in, static_cast<sdbg_hit*>(r[0].p),
-                                             static_cast<uint32_t*>(r[1].p), static_cast<uint64_t*>(r[2].p));
-                    });
+  if (!group_off || !query_group_off || !out || !n_out) return SDBG_EINVAL;
+  if (int rc = topk_args(segs, n_segs, nq, k)) return rc;
+  const PassBatch<sdbg_bm25_term> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  return topk_batch_host(segs, n_segs, B, k1, b, filt, k, threshold_in, out, n_out, total_matches);
 }
 
 extern "C" int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
@@ -2352,85 +2427,15 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
   return SDBG_OK;
 }
 
-// dst row to[j] = src row j, rows of row_words words.
-template <class Word>
-__global__ void __launch_bounds__(256) scatter_rows_kernel(const Word* __restrict__ src, Word* __restrict__ dst,
-                                                           const uint32_t* __restrict__ to, size_t n_rows, size_t row_words) {
-  const size_t n = n_rows * row_words;
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
-    const size_t j = i / row_words;
-    dst[size_t(to[j]) * row_words + (i - j * row_words)] = src[i];
-  }
-}
-
-// The queries of one pass, checked before anything is queued (rc: the checks' result): a batch count_run takes whole (a
-// flat batch, or a group batch of one shape), or a group batch of several shapes (S; whole.nq == 0).
-struct PassBatch {
-  int rc;
-  size_t nq;
-  QueryBatch<uint32_t> whole{};
-  uint32_t total_excl = 0;   // whole's, as check_query_batch sets it
-  GroupSplit<uint32_t> S;
-
-  PassBatch(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_t>& Q, const sdbg_col_pred* filt) : nq(Q.nq), whole(Q) {
-    rc = !segs || !n_segs || !Q.terms || !Q.term_off || !Q.nq ? SDBG_EINVAL : check_query_batch(segs, n_segs, Q, filt, &total_excl);
-  }
-  PassBatch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* group_off, const uint32_t* query_group_off,
-            const uint32_t* group_min, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt)
-      : nq(nq) {
-    rc = split_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, S);
-    if (S.whole >= 0) { whole = S.view(S.whole); total_excl = S.total_excl[S.whole]; }
-  }
-  PassBatch(const PassBatch&) = delete;   // whole may point into S
-};
-
-// Runs a prepared pass over B into out: count_run for a whole batch; otherwise each shape into zeroed rows of its own
-// (c->pass[2]), which scatter_rows_kernel moves to the caller's query positions on the stream. Nothing waits.
-int pass_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, const CountJob& job,
+// Runs a prepared pass over B into out: count_run for a whole batch, else shape by shape through shapes_run. Nothing waits.
+int pass_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt, const CountJob& job,
              const CountOut& out) {
   if (B.whole.nq) return count_run(segs, n_segs, count_plan(segs, n_segs, B.whole, B.total_excl, filt, job), filt, job, out);
-  sdbg_ctx* c = segs[0]->ctx;
   const GroupSplit<uint32_t>& S = B.S;
-  const std::array<size_t, 3> row = job.rows(out.rank >= 0);
-  void* const dst[3] = {out.counts, out.bins, out.nulls};
-  const auto pad = [](size_t b) { return (b + 7) & ~size_t(7); };
-  // per shape: its query positions (u32), then its rows of each array, every part 8-byte aligned
-  size_t pos[3] = {}, bytes = 0;
-  for (int sh = 0; sh < 3; ++sh) {
-    const size_t n = S.qs[sh].size();
-    pos[sh] = bytes;
-    bytes += pad(n * 4);
-    for (size_t r : row) bytes += pad(n * r);
-  }
-  if (int rc = ensure(c, c->pass[2], bytes)) return rc;
-  char* d = static_cast<char*>(c->pass[2].p);
-  CU(c, cudaMemsetAsync(d, 0, bytes, c->stream));
-  for (int sh = 0; sh < 3; ++sh)   // pageable: consumed on return
-    if (!S.qs[sh].empty()) CU(c, cudaMemcpyAsync(d + pos[sh], S.qs[sh].data(), S.qs[sh].size() * 4, cudaMemcpyHostToDevice, c->stream));
-  for (int sh = 0; sh < 3; ++sh) {
-    const size_t n = S.qs[sh].size();
-    if (!n) continue;
-    const auto* to = reinterpret_cast<const uint32_t*>(d + pos[sh]);
-    void* part[3];
-    char* p = d + pos[sh] + pad(n * 4);
-    for (int i = 0; i < 3; ++i) { part[i] = p; p += pad(n * row[i]); }
+  return shapes_run(segs[0]->ctx, S, job.rows(out.rank >= 0), {out.counts, out.bins, out.nulls}, [&](int sh, void* const* part) {
     const CountOut o{part[0], part[1], part[2], out.oor, out.stats, out.rank};
-    if (int rc = count_run(segs, n_segs, count_plan(segs, n_segs, S.view(sh), S.total_excl[sh], filt, job), filt, job, o)) return rc;
-    for (int i = 0; i < 3; ++i) {
-      if (!row[i]) continue;
-      const size_t words = row[i] % 8 ? row[i] / 4 : row[i] / 8;
-      const unsigned grid = unsigned(std::min<size_t>((n * words + 255) / 256, size_t(c->sm_count) * 8));
-      if (row[i] % 8)   // the sorted scan's u32 n_out
-        scatter_rows_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const uint32_t*>(part[i]), static_cast<uint32_t*>(dst[i]),
-                                                         to, n, words);
-      else
-        scatter_rows_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const unsigned long long*>(part[i]),
-                                                         static_cast<unsigned long long*>(dst[i]), to, n, words);
-      ++c->launches;
-    }
-    CU(c, cudaGetLastError());
-  }
-  return SDBG_OK;
+    return count_run(segs, n_segs, count_plan(segs, n_segs, S.view(sh), S.total_excl[sh], filt, job), filt, job, o);
+  });
 }
 
 // The aggregate device form's buffer: this header, then AggCell [nq][span], then AggCell [nq] for the NULL key.
@@ -2503,7 +2508,7 @@ void facet_fill(const char* h, size_t nq, uint32_t span, uint64_t* counts, uint6
 // (pass_finish). The sorted scan's windows go to sdbg_scan_stats. A count batch that the plan answers entirely from
 // docs_count queues nothing: fill gets the plan's counts, which is where the count region starts.
 template <class Fill>
-int pass_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, CountJob& job,
+int pass_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt, CountJob& job,
                  const PassRegion& L, Fill fill) {
   if (B.rc) return B.rc;
   sdbg_ctx* c = segs[0]->ctx;
@@ -2534,7 +2539,7 @@ int pass_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, c
   return pass_finish(c, L, h, fill);
 }
 
-int sort_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, uint64_t field,
+int sort_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt, uint64_t field,
                  int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
   CountJob job{CountMode::sort, {field, descending, nulls_first, k, {}, {}}, {}, {}};
   const PassRegion L = sort_region(B.nq, k);
@@ -2544,7 +2549,7 @@ int sort_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, c
   });
 }
 
-int agg_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, uint64_t key_field,
+int agg_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt, uint64_t key_field,
                 int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out, sdbg_match_agg* null_out) {
   CountJob job{CountMode::agg, {}, {}, {{key_field, key_min, key_span, {}}, value_field, {}}};
   const PassRegion L = agg_region(B.nq, key_span);
@@ -2558,7 +2563,7 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
                                       const uint32_t* term_off, size_t nq, const uint32_t* excl_terms,
                                       const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
   if (!counts) return SDBG_EINVAL;
-  const PassBatch B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
   CountJob job{CountMode::count, {}, {}, {}};
   return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
 }
@@ -2569,7 +2574,7 @@ extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t
                                                int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
   if (!segs || !n_segs || !segs[0] || !k || !out || !n_out) return SDBG_EINVAL;
   if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
-  const PassBatch B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
   return sort_to_host(segs, n_segs, B, filt, sort_field, descending, nulls_first, k, out, n_out);
 }
 
@@ -2578,7 +2583,7 @@ extern "C" int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n
                                              const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
                                              int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
   if (!counts || !null_counts) return SDBG_EINVAL;
-  const PassBatch B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
   CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
   return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, key_span),
                       [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
@@ -2590,7 +2595,7 @@ extern "C" int sdbg_match_aggregate_batch(sdbg_segment* const* segs, size_t n_se
                                           int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
                                           sdbg_match_agg* null_out) {
   if (!out || !null_out) return SDBG_EINVAL;
-  const PassBatch B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
   return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out);
 }
 
@@ -2599,7 +2604,7 @@ extern "C" int sdbg_match_count_batch_groups_min(sdbg_segment* const* segs, size
                                                  const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
                                                  const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts) return SDBG_EINVAL;
-  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   CountJob job{CountMode::count, {}, {}, {}};
   return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
 }
@@ -2620,7 +2625,7 @@ extern "C" int sdbg_match_topk_by_column_batch_groups_min(sdbg_segment* const* s
                                                           uint32_t* n_out) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !k || !out || !n_out) return SDBG_EINVAL;
   if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
-  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   return sort_to_host(segs, n_segs, B, filt, sort_field, descending, nulls_first, k, out, n_out);
 }
 
@@ -2632,7 +2637,7 @@ extern "C" int sdbg_match_facet_counts_batch_groups_min(sdbg_segment* const* seg
                                                         uint64_t* null_counts) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !counts || !null_counts) return SDBG_EINVAL;
   if (int rc = facet_check_range(segs[0]->ctx, key_min, key_span)) return rc;   // before the rows are sized
-  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
   return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, key_span),
                       [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
@@ -2646,7 +2651,7 @@ extern "C" int sdbg_match_aggregate_batch_groups_min(sdbg_segment* const* segs, 
                                                      sdbg_match_agg* out, sdbg_match_agg* null_out) {
   if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq || !out || !null_out) return SDBG_EINVAL;
   if (int rc = agg_check_range(segs[0]->ctx, key_field, key_min, key_span)) return rc;   // before the rows are sized
-  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out);
 }
 
@@ -2719,7 +2724,7 @@ __global__ void __launch_bounds__(256) agg_merge_gathered_kernel(const char* __r
 // pass run into it, one all-reduce of int64 over it, then the host entries' finish (pass_finish). A rank whose checks or
 // pass fail still joins the collective, with its failure word set.
 template <class Fill>
-int dist_words(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, CountJob& job, Fill fill) {
+int dist_words(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt, CountJob& job, Fill fill) {
   sdbg_ctx* c = segs[0]->ctx;
   CU(c, cudaSetDevice(c->device));
   const PassRegion L = words_region(B.nq, job.mode == CountMode::facet ? job.facet.span : 0);
@@ -2735,7 +2740,7 @@ int dist_words(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, con
 // hdr, prepares the job and runs the pass into the buffer, with c->pass[3] zeroed for what the device forms do not
 // report (the aggregate pass's counts, the sorted scan's windows). When the checks or the pass fail, sets the header's
 // failure word (at byte `failed`), so that the rank still joins the collective and the merge fails.
-int rank_device(sdbg_segment* const* segs, size_t n_segs, const PassBatch& B, const sdbg_col_pred* filt, CountJob& job,
+int rank_device(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt, CountJob& job,
                 const void* hdr, size_t failed, const PassRegion& L, int64_t rank, void* d_buf) {
   sdbg_ctx* c = segs[0]->ctx;
   CU(c, cudaSetDevice(c->device));
@@ -2763,7 +2768,7 @@ extern "C" int sdbg_dist_match_count_batch_groups_min(sdbg_segment* const* segs,
   if (int rc = dist_check(segs, n_segs, group_off, query_group_off, nq)) return rc;
   if (!counts) return SDBG_EINVAL;
   CountJob job{CountMode::count, {}, {}, {}};
-  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   return dist_words(segs, n_segs, B, filt, job, [&](const char* h) { std::memcpy(counts, h, nq * 8); });
 }
 
@@ -2777,7 +2782,7 @@ extern "C" int sdbg_dist_match_facet_counts_batch_groups_min(sdbg_segment* const
   if (!counts || !null_counts) return SDBG_EINVAL;
   if (int rc = facet_check_range(segs[0]->ctx, key_min, key_span)) return rc;
   CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
-  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   return dist_words(segs, n_segs, B, filt, job, [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
 }
 
@@ -2792,7 +2797,7 @@ extern "C" int sdbg_match_aggregate_batch_groups_min_device(sdbg_segment* const*
   CountJob job{CountMode::agg, {}, {}, {{key_field, key_min, key_span, {}}, value_field, {}}};
   const auto it = segs[0]->cols.find(value_field);   // the header's type: UINT64_MAX when not staged
   const AggDistHeader h{it == segs[0]->cols.end() ? UINT64_MAX : uint64_t(it->second.type), key_span, nq, 0, 0, {}};
-  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   return rank_device(segs, n_segs, B, filt, job, &h, offsetof(AggDistHeader, failed), agg_region(nq, key_span), -1, d_cells);
 }
 
@@ -2857,7 +2862,7 @@ extern "C" int sdbg_match_topk_by_column_batch_groups_min_device(sdbg_segment* c
   const auto it = segs[0]->cols.find(sort_field);   // the header's type: UINT64_MAX when not staged
   const SortDistHeader h{it == segs[0]->cols.end() ? UINT64_MAX : uint64_t(it->second.type), descending ? 1u : 0u,
                          nulls_first ? 1u : 0u, k, nq, 0, {}};
-  const PassBatch B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   return rank_device(segs, n_segs, B, filt, job, &h, offsetof(SortDistHeader, failed), sort_rank_region(nq, k), rank, d_rows);
 }
 
@@ -2937,31 +2942,19 @@ int scan_run(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_te
   const uint32_t scan_cap = 1024;                                    // candidate buffer of the kernel: unused here, kept minimal
   const uint32_t g = std::max(1u, std::min(uint32_t(c->sm_count) * 3u, range / 4096u));
   const uint32_t chunk = uint32_t((uint64_t(range) + g - 1) / g);   // 64-bit: range reaches 2^32 - 2
-  // descriptors: [QTermDev x T][term_off x 2][pad][work x g][excluded lists x n_excl][excl_off x 2]
-  const size_t qt_bytes = size_t(T) * sizeof(QTermDev), off_bytes = 2 * sizeof(uint32_t);
-  const size_t qt_pad = (qt_bytes + off_bytes + 15) & ~size_t(15), work_bytes = size_t(g) * sizeof(uint4);
-  const size_t x_bytes = n_excl * sizeof(uint2);
-  const size_t desc_bytes = qt_pad + work_bytes + (n_excl ? x_bytes + off_bytes : 0);
-  int rc = ensure_pinned(c, desc_bytes);
-  if (rc) return rc;
-  auto* h_qt = static_cast<QTermDev*>(c->h_pinned);
-  for (uint32_t i = 0; i < T; ++i) {
+  for (uint32_t i = 0; i < T; ++i)
     if (terms[i].term + 1 >= s->term_blk_begin.size()) return fail(c, SDBG_EINVAL, "term id out of range");
-    fill_qterm(s, terms[i], k1, b, h_qt[i]);
-  }
-  std::stable_sort(h_qt, h_qt + T, [](const QTermDev& x, const QTermDev& y) { return x.docs_count < y.docs_count; });
-  auto* h_off = reinterpret_cast<uint32_t*>(static_cast<char*>(c->h_pinned) + qt_bytes);
-  h_off[0] = 0; h_off[1] = T;
-  auto* h_work = reinterpret_cast<uint4*>(static_cast<char*>(c->h_pinned) + qt_pad);
+  // one query, one candidate list per chain, its excluded terms as its check lists
+  std::vector<uint4> work(g);
   for (uint32_t j = 0; j < g; ++j) {
     const uint32_t lo = doc_min + j * chunk;
-    h_work[j] = make_uint4(0u, lo, lo < doc_max ? std::min(chunk, doc_max - lo) : 0u, j);
-    if (lo >= doc_max) h_work[j].y = s->n_docs + 1u;               // empty chain
+    work[j] = make_uint4(0u, lo, lo < doc_max ? std::min(chunk, doc_max - lo) : 0u, j);
+    if (lo >= doc_max) work[j].y = s->n_docs + 1u;               // empty chain
   }
-  auto* h_x = reinterpret_cast<uint2*>(static_cast<char*>(c->h_pinned) + qt_pad + work_bytes);
-  for (size_t i = 0; i < n_excl; ++i) h_x[i] = excl_list(s, excl_terms[i]);
-  auto* h_xoff = reinterpret_cast<uint32_t*>(h_x + n_excl);
-  if (n_excl) { h_xoff[0] = 0; h_xoff[1] = uint32_t(n_excl); }
+  const uint32_t term_off[2] = {0, T};
+  const TopkDesc D = topk_desc(&s, 1, {kind, terms, term_off, 1, nullptr, nullptr, nullptr}, k1, b, work, {0, g},
+                               std::vector<uint32_t>(excl_terms, excl_terms + n_excl), {0, uint32_t(n_excl)}, {});
+  int rc;
   DevBuf& b_qt = c->scratch[0]; DevBuf& b_theta = c->scratch[1]; DevBuf& b_cand = c->scratch[2]; DevBuf& b_candn = c->scratch[3];
   DevBuf& b_emit = c->scratch[12];
   const uint64_t room = std::max<uint64_t>(cap, 1);
@@ -2969,19 +2962,17 @@ int scan_run(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_te
   cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, static_cast<const uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr),
                                   static_cast<const float*>(nullptr), static_cast<float*>(nullptr), room, 0, 32, c->stream);
   const size_t pair_bytes = (size_t(room) * 4 + 255) & ~size_t(255);
-  if ((rc = ensure(c, b_qt, desc_bytes))) return rc;
+  if ((rc = ensure(c, b_qt, D.h.size()))) return rc;
   if ((rc = ensure(c, b_theta, 32))) return rc;                      // theta | total | cursor
   if ((rc = ensure(c, b_cand, size_t(g) * scan_cap * 8))) return rc;
   if ((rc = ensure(c, b_candn, size_t(g) * 4))) return rc;
   if ((rc = ensure(c, b_emit, 4 * pair_bytes + sort_bytes))) return rc;
-  CU(c, cudaMemcpyAsync(b_qt.p, c->h_pinned, desc_bytes, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(b_qt.p, D.h.data(), D.h.size(), cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaMemsetAsync(b_theta.p, 0, 32, c->stream));
   TopkParams P;
   P.seg = postings_view(s, 0);
   if ((rc = filter_view(s, filt, &P.filt))) return rc;
-  P.qterms = static_cast<const QTermDev*>(b_qt.p);
-  P.qterm_off = reinterpret_cast<const uint32_t*>(static_cast<const char*>(b_qt.p) + qt_bytes);
-  P.work = reinterpret_cast<const uint4*>(static_cast<const char*>(b_qt.p) + qt_pad);
+  D.params(static_cast<const char*>(b_qt.p), 0, 0, P);
   P.theta = static_cast<unsigned long long*>(b_theta.p);
   P.total = P.theta + 1;
   P.emit_count = P.theta + 2;
@@ -2989,10 +2980,6 @@ int scan_run(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_te
   P.cand_n = static_cast<uint32_t*>(b_candn.p);
   P.claim = nullptr;
   P.k = 1; P.cap = scan_cap; P.conjunction = conj ? 1 : 0; P.wand = 0;
-  if (n_excl) {
-    P.excl = reinterpret_cast<const uint2*>(static_cast<const char*>(b_qt.p) + qt_pad + work_bytes);
-    P.excl_off = reinterpret_cast<const uint32_t*>(P.excl + n_excl);
-  }
   char* e = static_cast<char*>(b_emit.p);
   P.emit_docs = reinterpret_cast<uint32_t*>(e);
   P.emit_scores = reinterpret_cast<float*>(e + pair_bytes);
@@ -3051,30 +3038,19 @@ extern "C" int sdbg_bm25_topk(sdbg_segment* const* segs, size_t n_segs, int kind
 }
 
 namespace {
-__global__ void shift_keys_kernel(const unsigned long long* __restrict__ in, unsigned long long* __restrict__ out, size_t n,
-                                  uint32_t add) {
+__global__ void shift_keys_kernel(unsigned long long* __restrict__ keys, size_t n, uint32_t add) {
   // Re-bases ordinals for a cross-rank gather: ordinal' = ordinal + add (keys keep their order within a rank).
   for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
-    const unsigned long long k = in[i];
-    out[i] = k ? ((k & 0xFFFFFFFF00000000ull) | static_cast<unsigned long long>(~(~uint32_t(k) + add))) : 0ull;
+    const unsigned long long k = keys[i];
+    keys[i] = k ? ((k & 0xFFFFFFFF00000000ull) | static_cast<unsigned long long>(~(~uint32_t(k) + add))) : 0ull;
   }
 }
-}  // namespace
 
-namespace {
-int topk_batch_device_impl(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
-                           size_t nq, float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, uint32_t rank,
-                           void* d_keys, void* d_totals, bool sync);
-}
-extern "C" int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
-                                           const uint32_t* term_off, size_t nq, float k1, float b, const sdbg_col_pred* filt,
-                                           uint32_t k, float threshold_in, uint32_t rank, void* d_keys, void* d_totals) {
-  return topk_batch_device_impl(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, rank, d_keys, d_totals, true);
-}
-namespace {
-int topk_batch_device_impl(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
-                           size_t nq, float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, uint32_t rank,
-                           void* d_keys, void* d_totals, bool sync) {
+// The device form: the batch's keys straight into d_keys, its ordinals shifted into the rank's slot there, and its
+// totals into d_totals (NULL: not wanted). sync: wait for the stream before returning.
+int topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms, const uint32_t* term_off,
+                      size_t nq, float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, uint32_t rank,
+                      void* d_keys, void* d_totals, bool sync) {
   if (!d_keys || !segs || !n_segs) return SDBG_EINVAL;
   for (size_t si = 0; si < n_segs; ++si) if (!segs[si]) return SDBG_EINVAL;
   sdbg_ctx* c = segs[0]->ctx;
@@ -3084,17 +3060,28 @@ int topk_batch_device_impl(sdbg_segment* const* segs, size_t n_segs, int kind, c
   for (size_t si = 0; si < n_segs; ++si) docs += segs[si]->n_docs;
   if (rank >= 15) return fail(c, SDBG_EUNSUPPORTED, "rank slot overflow (rank >= 15)");
   if (docs >= (1ull << 28)) return fail(c, SDBG_EUNSUPPORTED, "rank slot overflow (>= 2^28 docs per rank)");
-  TopkDevOut dev{};
-  int rc = topk_run(segs, n_segs, {kind, terms, term_off, nq, nullptr, nullptr, nullptr}, k1, b, filt, k, threshold_in, &dev);
-  if (rc) return rc;
-  shift_keys_kernel<<<256, 256, 0, c->stream>>>(dev.keys, static_cast<unsigned long long*>(d_keys), nq * size_t(k), rank << 28);
+  if (int rc = topk_args(segs, n_segs, nq, k)) return rc;
+  const PassBatch<sdbg_bm25_term> B(segs, n_segs, {kind, terms, term_off, nq, nullptr, nullptr, nullptr}, filt);
+  if (int rc = topk_checked(segs, n_segs, B)) return rc;
+  DevBuf& b_n_out = c->scratch[5];   // the hit counts, which the device form does not report
+  if (int rc = ensure(c, b_n_out, nq * 4)) return rc;
+  auto* keys = static_cast<unsigned long long*>(d_keys);
+  if (int rc = topk_run(segs, n_segs, B.whole, B.total_excl, k1, b, filt, k, threshold_in,
+                        {keys, static_cast<uint32_t*>(b_n_out.p), static_cast<unsigned long long*>(d_totals)}))
+    return rc;
+  shift_keys_kernel<<<256, 256, 0, c->stream>>>(keys, nq * size_t(k), rank << 28);
   ++c->launches;
   CU(c, cudaGetLastError());
-  if (d_totals) CU(c, cudaMemcpyAsync(d_totals, dev.total, nq * 8, cudaMemcpyDeviceToDevice, c->stream));
   if (sync) CU(c, cudaStreamSynchronize(c->stream));
   return SDBG_OK;
 }
 }  // namespace
+
+extern "C" int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
+                                           const uint32_t* term_off, size_t nq, float k1, float b, const sdbg_col_pred* filt,
+                                           uint32_t k, float threshold_in, uint32_t rank, void* d_keys, void* d_totals) {
+  return topk_batch_device(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, rank, d_keys, d_totals, true);
+}
 
 extern "C" int sdbg_topk_merge_gathered(sdbg_ctx* c, const void* d_keys_all, uint32_t n_ranks, size_t nq, uint32_t k,
                                         sdbg_hit* out, uint32_t* n_out) {
@@ -3124,37 +3111,9 @@ extern "C" int sdbg_topk_merge_gathered(sdbg_ctx* c, const void* d_keys_all, uin
   CU(c, cudaGetLastError());
   if (!out && !n_out) return SDBG_OK;                                       // enqueue only: results stay in HBM, nothing waits
   if (!out) { CU(c, cudaStreamSynchronize(c->stream)); return SDBG_OK; }   // results stay in HBM (scratch of this context)
-  const size_t kb = nq * size_t(k) * 8, nb = nq * 4;
-  if ((rc = ensure_pinned(c, kb + nb))) return rc;
-  char* h = static_cast<char*>(c->h_pinned);
-  CU(c, cudaMemcpyAsync(h, M.keys_out, kb, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaMemcpyAsync(h + kb, M.n_out, nb, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  const auto* keys = reinterpret_cast<const unsigned long long*>(h);
-  const auto* cnt = reinterpret_cast<const uint32_t*>(h + kb);
-  auto convert = [&](size_t q0, size_t q1) {
-    for (size_t q = q0; q < q1; ++q) {
-      n_out[q] = cnt[q];
-      for (uint32_t i = 0; i < cnt[q]; ++i) {
-        const unsigned long long key = keys[q * k + i];
-        const uint32_t bits = uint32_t(key >> 32), ordinal = ~uint32_t(key);
-        sdbg_hit& h2 = out[q * k + i];
-        std::memcpy(&h2.score, &bits, 4);
-        h2.seg = ordinal >> 28;             // rank slot
-        h2.doc = ordinal & ((1u << 28) - 1);  // ordinal within the rank (segment base + doc)
-      }
-    }
-  };
-  // a few ns per hit; a large batch (millions of hits) is split over host threads like sdbg_bm25_topk_batch does
-  const size_t n_thr = std::min<size_t>(size_t(env_int("SDBG_HOST_THREADS", 8)), (nq * size_t(k)) / 65536);
-  if (n_thr <= 1) {
-    convert(0, nq);
-  } else {
-    std::vector<std::thread> pool;
-    for (size_t t = 0; t < n_thr; ++t) pool.emplace_back(convert, nq * t / n_thr, nq * (t + 1) / n_thr);
-    for (auto& th : pool) th.join();
-  }
-  return SDBG_OK;
+  // an ordinal is its rank's slot (ordinal >> 28) and the ordinal within the rank (segment base + doc)
+  return topk_to_host(c, {M.keys_out, M.n_out, nullptr}, nq, k,
+                      [](uint32_t ordinal) { return make_uint2(ordinal >> 28, ordinal & ((1u << 28) - 1)); }, out, n_out, nullptr);
 }
 
 extern "C" int sdbg_decode_score_term(sdbg_segment* s, uint32_t term, float c0, float nc, float nl, uint32_t* docs,
@@ -4021,16 +3980,15 @@ extern "C" int sdbg_dist_bm25_topk_batch(sdbg_segment* const* segs, size_t n_seg
   sdbg_ctx* c = segs[0]->ctx;
   const uint32_t world = uint32_t(c->dist_world), rank = uint32_t(c->dist_rank);
   if (world > 1 && !c->nccl_comm) return fail(c, SDBG_EINVAL, "sdbg_dist_init has not run");
-  DevBuf& mine = c->scratch[6 + 6];  // scratch[12..]: see DevBuf scratch[] size
-  DevBuf& all = c->scratch[6 + 7];
+  DevBuf& mine = c->pass[0];   // this rank's keys
+  DevBuf& all = c->pass[1];    // every rank's, gathered
   int rc;
   const size_t bytes = nq * size_t(k) * 8;
   if ((rc = ensure(c, mine, bytes))) return rc;
   if ((rc = ensure(c, all, bytes * world))) return rc;
-  if ((rc = topk_batch_device_impl(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, rank, mine.p, nullptr, false))) return rc;
+  if ((rc = topk_batch_device(segs, n_segs, kind, terms, term_off, nq, k1, b, filt, k, threshold_in, rank, mine.p, nullptr, false))) return rc;
   if ((rc = sdbg_dist_allgather(c, mine.p, all.p, bytes))) return rc;
-  if (!out) return sdbg_topk_merge_gathered(c, all.p, world, nq, k, nullptr, nullptr);
-  return sdbg_topk_merge_gathered(c, all.p, world, nq, k, out, n_out);
+  return sdbg_topk_merge_gathered(c, all.p, world, nq, k, out, out ? n_out : nullptr);
 }
 
 extern "C" int sdbg_dist_groupby_merge(sdbg_ctx* c, void* d_i64, void* d_f64, uint64_t span, double abs_bound) {

@@ -1,12 +1,14 @@
-"""Per-call latency of the synchronous count, facet, aggregate and sorted-scan entries: the host clock around each call
+"""Per-call latency of the synchronous count, facet, aggregate, sorted-scan and BM25 top-k entries: the host clock around each call
 (every call ends with its one stream synchronisation), median over --calls calls after warm-up. The batch benchmarks time
 4096 queries per step, which hides per-call costs (plan staging, the copy back, the single-term shortcut); this times
 the small batches where those costs show:
   shortcut   sdbg_match_count_batch of one single-term query, answered from docs_count without a launch;
   nq = 1 / 64 two-term ORs (bench.make_queries) for count, facet (2001 keys), aggregate (ungrouped, bit-packed int64)
              and the sorted scan (k = 100);
-  mixed      a 64-query group batch of all three shapes (one group, single-term groups, true groups) for count, facet
-             and the sorted scan.
+  mixed      a 64-query group batch of all three shapes (one group, single-term groups, true groups) for count, facet,
+             the sorted scan and the top-k;
+  topk       sdbg_bm25_topk_batch (BM25, k = 100) of nq = 1 / 64 two-term ORs, and sdbg_topk_merge_gathered of 4096 x 1000
+             keys (one rank's sdbg_bm25_topk_batch_device output) to host hits.
 Prints one JSON line with microseconds per call and the GPU name and power limit read in the same run.
 
     python tools/pass_latency.py [--calls 200] [--docs 10000000]
@@ -26,7 +28,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import bench  # noqa: E402
 import serenedb_b200 as sdb  # noqa: E402
 from serenedb_b200 import _native as N  # noqa: E402
-from serenedb_b200.engine import _ptr, _seg_array  # noqa: E402
+from serenedb_b200.engine import FLT_MIN, PreparedBatch, _ptr, _query_args, _seg_array, merge_gathered  # noqa: E402
 from count_bench import gpu_info  # noqa: E402
 
 K = 100
@@ -114,6 +116,21 @@ def main():
         mixed.append([[a, b]] if i % 3 == 0 else [[a], [b]] if i % 3 == 1 else [[a, b], [c]])
     terms, goff, qoff = group_batch(mixed)
     entries("mixed_nq64", len(mixed), terms, None, (goff, qoff))
+
+    scorer = sdb.BM25()
+    for nq in (1, 64):
+        res["topk_or_nq%d" % nq] = median_us(PreparedBatch(reader, queries[:nq], sdb.OR, scorer, K).run_host, args.calls)
+    gargs = _query_args(mixed, None, groups=True, stats=lambda t: reader.stats(scorer, t))
+    hits, n_out, total = np.zeros(len(mixed) * K * 12, np.uint8), np.zeros(len(mixed), np.uint32), np.zeros(len(mixed), np.uint64)
+    res["topk_mixed_nq64"] = median_us(lambda: N.check(lib.sdbg_bm25_topk_batch_groups_min(
+        segs, 1, *gargs, scorer.k, scorer.b, None, K, FLT_MIN, _ptr(hits), _ptr(n_out), _ptr(total)), ctx._h), args.calls)
+    import torch
+    nq, k = 4096, 1000
+    d_keys = torch.zeros(nq * k, dtype=torch.int64, device="cuda")
+    torch.cuda.synchronize()
+    PreparedBatch(reader, bench.make_queries(nq), sdb.OR, scorer, k).run_device(0, d_keys.data_ptr())
+    res["topk_merge_4096x1000_to_host"] = median_us(lambda: merge_gathered(ctx, d_keys.data_ptr(), 1, nq, k),
+                                                    max(args.calls // 10, 5))
     print(json.dumps(out))
 
 
