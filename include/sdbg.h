@@ -158,6 +158,21 @@ int sdbg_segment_term_bytes(const sdbg_segment*, uint64_t* bytes_out, size_t n_t
  *     which holds for every non-NULL row; `= 2.5` holds for none and `<> 2.5` for every non-NULL row. */
 enum { SDBG_OP_LT = 0, SDBG_OP_LE, SDBG_OP_GT, SDBG_OP_GE, SDBG_OP_EQ, SDBG_OP_NE, SDBG_OP_BETWEEN,
        SDBG_OP_IS_NULL, SDBG_OP_IS_NOT_NULL };
+/* Filter chains (`WHERE body @@ '...' AND a < x AND b = y`). Every full-text entry's `filt` -- the top-k, scan, count,
+ * sorted, facet and aggregate entries, their *_device forms and the sdbg_dist_* entries -- points at a chain: when
+ * filt[i].op has SDBG_OP_AND_NEXT set, filt[i] is ANDed with filt[i + 1], and the chain ends at the first entry without
+ * the bit. A chain holds at most 4 predicates: the bit on the 4th gives SDBG_EUNSUPPORTED before anything is queued, and
+ * a 5th entry is never read. A chain of one is the single predicate; filt == NULL is no filter. Each predicate follows
+ * the rules above against its own column (int64 raw or bit-packed, int32 or double; NOT NULL or nullable); predicates
+ * may repeat a column. Every column needs at least as many rows as the segment has docs (else SDBG_EINVAL; a column
+ * that is not staged: SDBG_ENOTFOUND). Before any posting list is read, the chain is judged per 2048-row zone from the
+ * zonemaps of its NOT NULL columns (DESIGN.md §4.13): zones where it holds for no row are skipped and zones where it
+ * holds for every row are not read; results do not depend on it. The first call that judges a NOT NULL column's zones
+ * (and the first after its values change: restaging, sdbg_column_device_ptr) waits once for the context's stream, to
+ * copy the column's zonemap to the host; this holds for every entry taking `filt`, the *_device and sdbg_dist_* forms
+ * included. sdbg_col_pred_resolve and the columnar entries
+ * (preds, n_preds) take no chain: the bit there is an op outside SDBG_OP_* (SDBG_EINVAL). */
+#define SDBG_OP_AND_NEXT 0x100
 typedef struct {
   uint64_t field;
   int32_t op;
@@ -172,6 +187,8 @@ typedef struct {
 int sdbg_col_pred_resolve(const sdbg_col_pred* in, int type, sdbg_col_pred* out);
 
 /* ---- BM25 top-k (boundary B2, irs::DocIterator::Collect) ---- */
+/* `filt` of every entry below (top-k, scan, count, sorted, facet, aggregate; *_device and sdbg_dist_* forms): NULL or a
+ * filter chain, see SDBG_OP_AND_NEXT above. */
 enum { SDBG_QUERY_OR = 0, SDBG_QUERY_AND = 1 };
 typedef struct { float idf, norm_const, norm_length, boost; uint32_t term; } sdbg_bm25_term; /* BM25Stats (bm25.hpp:49-56) + boost */
 typedef struct { float score; uint32_t doc; uint32_t seg; } sdbg_hit;                          /* irs::ScoreDoc (iterators.hpp:93-101) */
@@ -526,14 +543,16 @@ int sdbg_dist_allgather(sdbg_ctx*, const void* d_send, void* d_recv, size_t byte
 int sdbg_dist_groupby_merge(sdbg_ctx*, void* d_i64, void* d_f64, uint64_t span, double abs_bound);
 /* BM25 top-k over the segments of ALL ranks: local scan -> one all-gather of the k best keys per query -> local
    selection, back to back on the context's stream. hit.seg = rank, hit.doc = ordinal within the rank. out == NULL:
-   nothing is copied and nothing waits (results stay in HBM). */
+   nothing is copied and nothing waits (results stay in HBM), except the once-per-column zonemap copy of a filter chain
+   (SDBG_OP_AND_NEXT). */
 int sdbg_dist_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
                               const uint32_t* term_off, size_t n_queries, float k1, float b, const sdbg_col_pred* filt,
                               uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out);
 /* Count, facet counts, aggregates and the sorted scan over the segments of ALL ranks (a corpus sharded by segment, one
    context per GPU): each rank runs the local pass over its own segments with the results left in HBM, then one collective
    and, for the aggregates and the sorted scan, a merge kernel, back to back on the context's stream; the one wait is the
-   copy back at the end (the sorted scan's zonemap planning also waits for its own small copies, before its launches).
+   copy back at the end (the sorted scan's zonemap planning also waits for its own small copies, before its launches,
+   and a filter chain's first use of a NOT NULL column waits once for its zonemap copy: SDBG_OP_AND_NEXT).
    The query parameters are those of the *_batch_groups_min entries. A flat query is a degenerate groups query (OR: one
    group, AND: single-term groups), which the groups entries run as the flat entries and with exactly their results
    (§ "Conjunctions of OR groups" above), so there are no flat-form dist entries. Results are those of the local entry

@@ -15,7 +15,9 @@
 //        same early end. A group that needs m >= 2 of its s lists (`2 of (a | b | c)`) leads with its s - m + 1 shortest
 //        lists; it decodes each list into `tmp` the same way, adds it into a bit-sliced counter, then acc &= counter >= m.
 //   NOT  the excluded lists' blocks whose range holds a bit of `acc` are decoded and their docs cleared.
-// Then acc &= ~deleted, the filter runs per remaining bit, and popcounts are summed: one 64-bit atomicAdd per CTA.
+// Then acc &= ~deleted, the filter chain runs per remaining bit, and popcounts are summed: one 64-bit atomicAdd per CTA.
+// With the chain's zone verdicts (ChainDev::zone), a window whose zones are all dead is skipped before any list is
+// decoded, the docs of dead zones are cleared before any column is read, and docs of pass zones skip the chain.
 // The facet pass (kFacet, bm25_facet.cuh) also counts each remaining bit in its key's shared-memory bin; the aggregate pass
 // (kAgg, bm25_agg.cuh) also adds its value to its key's shared-memory cell.
 // A window that no positive list reaches (OR), that the shortest list does not reach (AND) or that no list of the lead
@@ -39,7 +41,7 @@ constexpr uint32_t kCountMaxLists = 2u * kMaxQueryTerms;   // positive + exclude
 
 struct CountParams {
   PostingsDev seg;              // arena, blocks, deleted, n_docs
-  FilterDev filt;
+  ChainDev filt;
   // Per query q of this segment: positive lists lists[term_off[q] .. term_off[q + 1]) as {first BlockDesc, blocks},
   // ascending by docs_count; excluded lists lists[n_pos + excl_off[q] .. n_pos + excl_off[q + 1]) (0 blocks: a term the
   // segment does not hold). excl_off null: no exclusions.
@@ -163,7 +165,10 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   __shared__ uint32_t s_ws, s_done;
   __shared__ unsigned long long s_sum[kCountWarps];
   __shared__ unsigned long long s_thr[1];   // kSort: this item's best known k-th hi
-  __shared__ uint32_t s_fill[1], s_zmask[2];  // kSort: keys in the buffer (kFacet: NULL keys); the window's zones that can reach s_thr
+  __shared__ uint32_t s_fill[1];  // kSort: keys in the buffer (kFacet: NULL keys)
+  // the window's zones that hold docs that can count: not dead for the filter chain and (kSort) able to reach s_thr;
+  // the zones where the chain holds for every row; (kSort) the zones that can reach s_thr
+  __shared__ uint32_t s_zmask[2], s_pmask[2], s_smask[2];
   // kSort: hi[cap] | lo[cap]; kFacet: the u32 bins, padded to 16 B; kAgg: the cells; then (kGroups) the bit-sliced
   // counter planes
   extern __shared__ unsigned long long sort_buf[];
@@ -242,26 +247,55 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       s_resume[tid] = 0u;
       s_end[tid] = (e < l.y && __ldg(&LB[e].z) < wlast) ? e + 1u : e;   // block e straddles the window's end
     }
-    // kSort with a zonemap: zones zb .. zb + 32 hold the window's rows ws - 1 .. ws + 65534 (32 zones for ws = 0)
+    // Zone verdicts (the sort column's zonemap, the filter chain's): zones zb .. zb + 32 hold the window's rows
+    // ws - 1 .. ws + 65534 (32 zones for ws = 0)
     const uint32_t zb = ws == 0u ? 0u : (ws >> 11) - 1u;
-    if constexpr (kSort) {
-      if (P.sort.zone && tid < 64u) {
-        const uint32_t nz = ws == 0u ? 32u : 33u;
-        const bool comp = tid < nz && sort_zone_bound(P.sort, zb + tid) >= s_thr[0];
-        const uint32_t m = __ballot_sync(kFull, comp);
-        if (lane == 0) s_zmask[warp] = m;
+    const bool sort_zoned = kSort && P.sort.zone;
+    const bool zoned = sort_zoned || P.filt.zone;
+    if (zoned && tid < 64u) {
+      const uint32_t z = zb + tid;
+      const bool in = tid < (ws == 0u ? 32u : 33u);
+      bool comp = in, pass = false;
+      if constexpr (kSort) {
+        if (P.sort.zone) comp = in && sort_zone_bound(P.sort, z) >= s_thr[0];
       }
+      const uint32_t sm = __ballot_sync(kFull, comp);
+      if (P.filt.zone) {
+        const uint8_t v = in && z < P.filt.n_zones ? P.filt.zone[z] : kZoneDead;   // zones past the segment hold no doc
+        comp = comp && v != kZoneDead;
+        pass = v == kZonePass;
+      }
+      const uint32_t m = __ballot_sync(kFull, comp), p = __ballot_sync(kFull, pass);
+      if (lane == 0) { s_zmask[warp] = m; s_pmask[warp] = p; s_smask[warp] = sm; }
     }
     for (uint32_t i = tid; i < kCountWords; i += kCountThreads) acc[i] = 0u;
     __syncthreads();
     bool skip = false;
-    if constexpr (kSort) {
-      if (P.sort.zone) {
-        ++judged;
-        skip = (s_zmask[0] | s_zmask[1]) == 0u;
-        skipped += skip;
-      }
+    if (zoned) {
+      skip = (s_zmask[0] | s_zmask[1]) == 0u;
+      if (sort_zoned) { ++judged; skipped += (s_smask[0] | s_smask[1]) == 0u; }
     }
+    // the bits of acc word i whose zone is set in the zone mask zm: bit 0 is row ws + 32i - 1, which starts a zone when
+    // ws + 32i does
+    auto zone_bits = [&](const uint32_t* zm, uint32_t i) {
+      auto has = [&](uint32_t zr) { return (zm[zr >> 5] >> (zr & 31u)) & 1u; };
+      const uint32_t d0 = ws + 32u * i;
+      uint32_t bits = has((d0 >> 11) - zb) ? 0xFFFFFFFEu : 0u;
+      if (d0 != 0u && has(((d0 - 1u) >> 11) - zb)) bits |= 1u;
+      return bits;
+    };
+    // the docs of word i's bits v that pass the filter chain: dead zones are cleared first, pass zones are not read
+    auto chain_bits = [&](uint32_t v, uint32_t i) {
+      if (v && zoned) v &= zone_bits(s_zmask, i);
+      if (v && P.filt.ps.n) {
+        const uint32_t check = P.filt.zone ? v & ~zone_bits(s_pmask, i) : v;
+        for (uint32_t r = check; r; r &= r - 1u) {
+          const uint32_t bit = __ffs(r) - 1u;
+          if (!preds_row(P.filt.ps, uint64_t(ws + 32u * i + bit) - 1u)) v &= ~(1u << bit);
+        }
+      }
+      return v;
+    };
     if (!skip) {
 
     // Blocks [s_cur, s_end) of lists [lo, hi) spread over the warps; `filter`: only blocks whose range holds a bit of acc.
@@ -348,12 +382,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
         uint32_t v = acc[i];
         if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
-        if (v && P.filt.values) {
-          for (uint32_t r = v; r; r &= r - 1u) {
-            const uint32_t bit = __ffs(r) - 1u;
-            if (!filter_pass(P.filt, ws + 32u * i + bit)) v &= ~(1u << bit);
-          }
-        }
+        v = chain_bits(v, i);
         if constexpr (kFacet) {
           for (uint32_t r = v; r; r &= r - 1u) oor |= facet_add(P.facet, ws + 32u * i + (__ffs(r) - 1u), bins, &s_fill[0]);
         }
@@ -368,23 +397,11 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
         const uint32_t wbase = ws >> 5, cap = P.sort.cap;
         unsigned long long* hi = sort_buf;
         unsigned long long* lo = sort_buf + cap;
-        auto zone_ok = [&](uint32_t zr) { return (s_zmask[zr >> 5] >> (zr & 31u)) & 1u; };
         for (uint32_t base = 0; base < kCountWords; base += kCountThreads) {   // uniform trip count
           const uint32_t i = base + tid;
           uint32_t v = acc[i];
           if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
-          if (v && P.sort.zone) {   // bit 0 is row ws + 32i - 1, which starts a zone when ws + 32i does
-            const uint32_t d0 = ws + 32u * i;
-            uint32_t keep = zone_ok((d0 >> 11) - zb) ? 0xFFFFFFFEu : 0u;
-            if (d0 != 0u && zone_ok(((d0 - 1u) >> 11) - zb)) keep |= 1u;
-            v &= keep;
-          }
-          if (v && P.filt.values) {
-            for (uint32_t r = v; r; r &= r - 1u) {
-              const uint32_t bit = __ffs(r) - 1u;
-              if (!filter_pass(P.filt, ws + 32u * i + bit)) v &= ~(1u << bit);
-            }
-          }
+          v = chain_bits(v, i);
           for (;;) {   // a full buffer is cut to the k best and the remaining bits go on
             const unsigned long long thr = s_thr[0];
             for (; v; v &= v - 1u) {

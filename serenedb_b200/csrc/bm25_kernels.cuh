@@ -17,7 +17,7 @@
 // CTA-wide bitonic sort when full (the GPU analogue of nth_element at 2k).
 #pragma once
 
-#include "device_common.cuh"
+#include "column_kernels.cuh"
 
 namespace sdbg {
 
@@ -32,15 +32,6 @@ struct PostingsDev {
   uint32_t norm_width;    // 1, 2 or 4
   uint32_t n_docs;
   uint32_t ordinal_base;  // first global ordinal of this segment (keys carry base + doc)
-};
-
-struct FilterDev {  // one pushed column predicate for the hybrid path
-  const void* values;        // null => no filter
-  const uint64_t* validity;  // null => NOT NULL column
-  int32_t type;              // 0 i64, 1 f64, 2 i32
-  int32_t op;
-  int64_t lo_i, hi_i;
-  double lo_f, hi_f;
 };
 
 struct QTermDev {  // one term of one query over one segment, 40 bytes
@@ -227,30 +218,6 @@ __device__ __forceinline__ float bm25_plain(uint32_t freq, uint32_t norm, float 
   return __fsub_rn(c0, __fdiv_rn(__fmul_rn(c0, c1), __fadd_rn(c1, static_cast<float>(freq))));
 }
 
-__device__ __forceinline__ bool filter_pass(const FilterDev& f, uint32_t doc) {
-  if (f.values == nullptr) return true;
-  const size_t r = size_t(doc) - 1u;  // row = doc - 1 (index/column_extract.hpp:46-48)
-  const bool valid = f.validity == nullptr || ((f.validity[r >> 6] >> (r & 63)) & 1ull);
-  if (f.op == 7) return !valid;
-  if (f.op == 8) return valid;
-  if (!valid) return false;
-  if (f.type == 1) {
-    const double v = __ldg(static_cast<const double*>(f.values) + r);
-    switch (f.op) {
-      case 0: return v < f.lo_f; case 1: return v <= f.lo_f; case 2: return v > f.lo_f;
-      case 3: return v >= f.lo_f; case 4: return v == f.lo_f; case 5: return v != f.lo_f;
-      default: return v >= f.lo_f && v <= f.hi_f;
-    }
-  }
-  const long long v = f.type == 2 ? static_cast<long long>(__ldg(static_cast<const int*>(f.values) + r))
-                                  : __ldg(static_cast<const long long*>(f.values) + r);
-  switch (f.op) {
-    case 0: return v < f.lo_i; case 1: return v <= f.lo_i; case 2: return v > f.lo_i;
-    case 3: return v >= f.lo_i; case 4: return v == f.lo_i; case 5: return v != f.lo_i;
-    default: return v >= f.lo_i && v <= f.hi_i;
-  }
-}
-
 // ------------------------------------------------------------------------------------------
 // Probe kernel: decode + score one whole posting list (exhaustive). One warp per block.
 // ------------------------------------------------------------------------------------------
@@ -308,7 +275,7 @@ decode_score_kernel(PostingsDev seg, uint32_t blk_begin, uint32_t nblk, float c0
 // ------------------------------------------------------------------------------------------
 struct TopkParams {
   PostingsDev seg;
-  FilterDev filt;
+  ChainDev filt;
   const QTermDev* qterms;      // flattened, per query sorted by ascending docs_count
   const uint32_t* qterm_off;   // n_queries + 1
   unsigned long long* theta;   // per query running threshold key (shared by all chains / segments)
@@ -933,7 +900,7 @@ bm25_topk_kernel(const TopkParams P) {
     const uint32_t n_entries = n_items * 128u;
     const uint32_t emit_begin = P.conjunction ? s_phase[buf][T - 1u] * 128u : 0u;  // AND: only the last term's slots can be complete (never in driver mode)
     bool first_pass = true;
-    const bool plain = !P.conjunction && P.filt.values == nullptr && P.seg.deleted == nullptr && !kExcl;   // disjunction, no table filter, no deletes, no exclusions: 4 entries per lane
+    const bool plain = !P.conjunction && P.filt.ps.n == 0 && P.seg.deleted == nullptr && !kExcl;   // disjunction, no table filter, no deletes, no exclusions: 4 entries per lane
     for (;;) {
       const unsigned long long theta = s_theta;
       const uint32_t theta_hi = uint32_t(theta >> 32);
@@ -981,7 +948,7 @@ bm25_topk_kernel(const TopkParams P) {
         bool live = d - lo <= hi - lo;                       // in window, not padding / folded / already stored
         if (live && P.conjunction) live = e_cnt[e] == T - 1u;
         if (live && P.seg.deleted != nullptr) live = ((__ldg(P.seg.deleted + (d >> 5)) >> (d & 31u)) & 1u) == 0u;   // MaskDocIterator: neither scored nor counted
-        if (live && P.filt.values != nullptr) live = filter_pass(P.filt, d);
+        if (live && P.filt.ps.n) live = chain_pass(P.filt, d);
         if (kGroups && live) live = !excluded_doc(P.seg.arena, P.seg.blocks, P.seg.anchors, s_ex, s_exg, n_ex, d);
         else if (kExcl && live) live = !excluded_doc(P.seg.arena, P.seg.blocks, P.seg.anchors, s_ex, n_ex, d);   // neither collected nor counted
         // cheap pre-test on the score bits alone; the full 64-bit key only for the few that may qualify

@@ -483,7 +483,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
   // capacity): for small k the threshold then follows the running k-th best closely instead of waiting for 2048
   // accepted candidates, which is what block-max skipping lives on.
   const uint32_t lim = min(P.cap, (P.k + max(P.k, 256u) + kTopkThreads - 1u) / kTopkThreads * kTopkThreads);
-  const bool doc_checks = P.filt.values != nullptr || P.seg.deleted != nullptr;   // hybrid filter / DocumentMask on final docs
+  const bool doc_checks = P.filt.ps.n != 0 || P.seg.deleted != nullptr;   // hybrid filter / DocumentMask on final docs
   // Per-doc list checks (excluded terms, OR groups): a probe per doc costs a few dependent loads. With pruning and a top-k
   // sink only docs whose final score passes the threshold pre-test are probed (late): a rejected doc then never enters the
   // candidate buffer, so the threshold is raised by real results only and pruned == exhaustive, and `matched` counts only
@@ -532,7 +532,7 @@ bm25_stream_kernel(const __grid_constant__ TopkParams P) {
 
     auto doc_ok = [&](uint32_t d) {
       if (P.seg.deleted != nullptr && ((__ldg(P.seg.deleted + (d >> 5)) >> (d & 31u)) & 1u)) return false;   // MaskDocIterator
-      return filter_pass(P.filt, d);
+      return chain_pass(P.filt, d);
     };
     auto test_and_append = [&](bool alive, uint32_t dv, float sv) {
       if (P.emit_docs != nullptr) { stream_emit(P.emit_docs, P.emit_scores, P.emit_count, P.emit_cap, alive, dv, sv); return; }

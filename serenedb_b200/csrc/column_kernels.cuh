@@ -91,6 +91,36 @@ __device__ __forceinline__ uint32_t preds2(const PredSet& ps, uint64_t r, uint64
   return m;
 }
 
+// Predicate `p` of a filter chain on row r alone (the full-text kernels' per-doc test). The host hands chain predicates
+// over as `lo <= v <= hi` (SDBG_OP_BETWEEN), `NOT (lo <= v <= hi)` (SDBG_OP_NE) or a NULL test (filter_view).
+__device__ __forceinline__ bool pred1(const PredDev& p, uint64_t r) {
+  const bool valid = col_valid(p.col, r);
+  if (p.op >= 7) return (p.op == 8) == valid;
+  if (!valid) return false;
+  bool in;
+  if (p.col.type == 1) {
+    const double v = __ldg(static_cast<const double*>(p.col.values) + r);
+    in = v >= p.lo_f && v <= p.hi_f;
+  } else {
+    const long long v = p.col.type == 2 ? static_cast<long long>(__ldg(static_cast<const int*>(p.col.values) + r))
+                                        : __ldg(static_cast<const long long*>(p.col.values) + r);
+    in = v >= p.lo_i && v <= p.hi_i;
+  }
+  return in != (p.op == 5);
+}
+
+// Every predicate of `ps` on row r, in the caller's order, up to the first that fails.
+// The first predicate is read from fixed parameter offsets like a single one; the loop over the others is not unrolled,
+// so the callers' instruction streams hold two copies of pred1, not four.
+__device__ __forceinline__ bool preds_row(const PredSet& ps, uint64_t r) {
+  if (ps.n == 0) return true;
+  if (!pred1(ps.p[0], r)) return false;
+#pragma unroll 1
+  for (int i = 1; i < ps.n; ++i)
+    if (!pred1(ps.p[i], r)) return false;
+  return true;
+}
+
 __device__ __forceinline__ void load2_i64(const ColDev& c, uint64_t r, long long& a, long long& b) {
   if (c.type == 2) {
     const int2 v = *reinterpret_cast<const int2*>(static_cast<const int*>(c.values) + r);
@@ -720,35 +750,67 @@ zonemap_kernel(const unsigned char* __restrict__ values, uint64_t rows, long lon
   }
 }
 
+constexpr uint8_t kZoneCheck = 0, kZoneDead = 1, kZonePass = 2;   // zone verdicts
+
 struct ZoneVerdictParams {
   const long long* zone[kMaxPreds];   // per predicate: the column's zonemap (null: no verdict from this predicate)
   long long lo[kMaxPreds];
   unsigned long long span[kMaxPreds];
   int negate[kMaxPreds];
   int n_preds;
+  int pass;                           // 1: also judge zones where every predicate holds for every row
   uint64_t n_blocks;
 };
-// skip[b] = 1 when some predicate's range [lo, lo + span] misses the block's [min, max] entirely (a negated predicate,
-// SQL <>, only when the whole block equals the excluded value). counter += number of skipped blocks.
+// The verdict of block b from the blocks' [min, max] in zone[i] (per predicate; null: no verdict from it): kZoneDead when
+// some predicate's range [lo, lo + span] misses the block entirely (a negated predicate, SQL <>, only when the whole
+// block equals the excluded value); with Z.pass, kZonePass when every predicate has a zonemap and its range covers
+// [min, max] (negated: misses it); else kZoneCheck. zone is Z.zone on the device and host copies on the host.
+__host__ __device__ __forceinline__ uint8_t zone_verdict(const ZoneVerdictParams& Z, const long long* const* zone, uint64_t b) {
+  bool dead = false, all = Z.pass != 0;
+  for (int i = 0; i < Z.n_preds; ++i) {
+    if (zone[i] == nullptr) { all = false; continue; }
+    const long long mn = zone[i][2 * b], mx = zone[i][2 * b + 1];
+    const long long lo = Z.lo[i];
+    const bool hi_below = static_cast<unsigned long long>(mn - lo) > Z.span[i] && mn > lo;   // block starts beyond lo + span
+    const bool lo_above = mx < lo;                                                             // block ends before lo
+    const bool inside = mn >= lo && static_cast<unsigned long long>(mx - lo) <= Z.span[i];    // block within the range
+    if (Z.negate[i]) { dead |= Z.span[i] == 0ull && mn == lo && mx == lo; all &= hi_below || lo_above; }
+    else { dead |= hi_below || lo_above; all &= inside; }
+  }
+  return dead ? kZoneDead : all ? kZonePass : kZoneCheck;
+}
+
+// skip[b] = zone_verdict(Z, Z.zone, b); counter (null: none) += number of dead blocks.
 __global__ void __launch_bounds__(256)
 zone_verdict_kernel(const ZoneVerdictParams Z, uint8_t* __restrict__ skip, unsigned long long* __restrict__ counter) {
   unsigned long long mine = 0;
   for (uint64_t b = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; b < Z.n_blocks; b += uint64_t(gridDim.x) * blockDim.x) {
-    bool dead = false;
-    for (int i = 0; i < Z.n_preds; ++i) {
-      if (Z.zone[i] == nullptr) continue;
-      const long long mn = Z.zone[i][2 * b], mx = Z.zone[i][2 * b + 1];
-      const long long lo = Z.lo[i];
-      const bool hi_below = static_cast<unsigned long long>(mn - lo) > Z.span[i] && mn > lo;   // block starts beyond lo + span
-      const bool lo_above = mx < lo;                                                             // block ends before lo
-      if (Z.negate[i]) dead |= Z.span[i] == 0ull && mn == lo && mx == lo;
-      else dead |= hi_below || lo_above;
-    }
-    skip[b] = dead ? 1 : 0;
-    mine += dead ? 1ull : 0ull;
+    const uint8_t v = zone_verdict(Z, Z.zone, b);
+    skip[b] = v;
+    mine += v == kZoneDead ? 1ull : 0ull;
   }
+  if (counter == nullptr) return;
   mine = warp_sum64(mine);
   if ((threadIdx.x & 31u) == 0u && mine) atomicAdd(counter, mine);
+}
+
+// The pushed predicate chain of a full-text entry (SDBG_OP_AND_NEXT) over one segment; ps.n == 0: no filter. zone, when
+// set: the chain's verdict per kZoneRows rows of the segment (zone_verdict_kernel), n_zones of them.
+struct ChainDev {
+  PredSet ps;
+  const uint8_t* zone;
+  uint32_t n_zones;
+  uint32_t pad;
+};
+
+// Doc `doc` (row doc - 1) against a chain: its zone's verdict when the zone is decided, else every predicate.
+__device__ __forceinline__ bool chain_pass(const ChainDev& f, uint32_t doc) {
+  const uint64_t r = uint64_t(doc) - 1u;
+  if (f.zone != nullptr) {
+    const uint8_t v = __ldg(f.zone + r / kZoneRows);
+    if (v != kZoneCheck) return v == kZonePass;
+  }
+  return preds_row(f.ps, r);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -60,6 +60,7 @@ struct ColumnObj {
   int64_t mn = 0, mx = 0;
   long long* d_zone = nullptr;  // zonemap: {min, max} per 2048-row block in predicate key space (NOT NULL columns, built on first use)
   bool zone_ok = false;         // d_zone holds the current values' zonemap (a restage of the same shape keeps the allocation)
+  std::vector<long long> h_zone;  // host copy of the current zonemap, fetched on first use by the filter chains (empty: none)
   bool has_absmax = false;      // double columns: bits of the largest |value| (>= 0x7FF0... when NaN / inf occur)
   uint64_t absmax_bits = 0;
 };
@@ -134,6 +135,8 @@ struct sdbg_segment {
   uint64_t n_deleted = 0;
   // columns
   std::map<uint64_t, ColumnObj> cols;
+  // zone verdicts of the last full-text call's filter chain over this segment (chain_verdicts)
+  DevBuf verdict;
 };
 
 struct sdbg_writer {
@@ -351,6 +354,7 @@ extern "C" void sdbg_segment_destroy(sdbg_segment* s) {
   if (s->d_norms) cudaFree(s->d_norms);
   if (s->d_deleted) cudaFree(s->d_deleted);
   for (auto& kv : s->cols) free_column(kv.second);
+  if (s->verdict.p) cudaFree(s->verdict.p);
   delete s;
 }
 
@@ -558,7 +562,7 @@ int pack_column(sdbg_ctx* c, ColumnObj& col) {
   const auto* raw = static_cast<const long long*>(c->stage_raw.p);
   const unsigned grid = grid_per_group_warp(c, n_groups);
   for_stats_kernel<<<grid, 256, 0, c->stream>>>(raw, nullptr, nullptr, rows, col.d_zone, s_hdr, s_nw);
-  col.zone_ok = true;
+  col.zone_ok = true; col.h_zone.clear();
   ++c->launches;
   CU(c, cudaGetLastError());
   CU(c, cub::DeviceScan::ExclusiveSum(base + h_bytes + 2 * n_bytes, scan_bytes, s_nw, s_off, int(n_groups + 1), c->stream));
@@ -616,7 +620,7 @@ extern "C" int sdbg_stage_column(sdbg_segment* s, uint64_t field, sdbg_type t, c
     CU(c, cudaMalloc(&col.d_values, bytes + 64));  // slack: row pairs are loaded as one 16-byte vector
     CU(c, cudaMemsetAsync(static_cast<char*>(col.d_values) + bytes, 0, 64, c->stream));
   }
-  col.zone_ok = false;   // new values: the zonemap is built again on first use (into the same allocation)
+  col.zone_ok = false; col.h_zone.clear();   // new values: the zonemap is built again on first use (into the same allocation)
   col.type = t; col.rows = rows; col.owned = true; col.has_minmax = false; col.has_absmax = false;
   CU(c, cudaMemcpyAsync(col.d_values, values, bytes, cudaMemcpyHostToDevice, c->stream));
   if (validity) {
@@ -719,7 +723,7 @@ extern "C" int sdbg_stage_column_for(sdbg_segment* s, uint64_t field, const sdbg
     CU(c, cudaMemcpyAsync(const_cast<unsigned long long*>(for_words(col)), words, n_words * 8, cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaMemsetAsync(static_cast<char*>(col.d_packed) + packed_bytes - 64, 0, 64, c->stream));
     { int rc = ensure_zone(c, col); if (rc) return rc; }
-    col.zone_ok = true;
+    col.zone_ok = true; col.h_zone.clear();
     for_stats_kernel<<<grid_per_group_warp(c, n_groups), 256, 0, c->stream>>>(nullptr, for_headers(col), for_words(col), rows, col.d_zone,
                                                                               nullptr, nullptr);
     ++c->launches;
@@ -734,7 +738,7 @@ extern "C" int sdbg_stage_column_for(sdbg_segment* s, uint64_t field, const sdbg
   }
   if (col.d_validity) { cudaFree(col.d_validity); col.d_validity = nullptr; }
   col.type = SDBG_I64; col.rows = rows; col.owned = true; col.has_minmax = false; col.has_absmax = false;
-  col.zone_ok = false;
+  col.zone_ok = false; col.h_zone.clear();
   DevBuf& buf = c->scratch[12];
   const size_t hdr_bytes = (n_groups * sizeof(ForBlockDev) + 255) & ~size_t(255);
   int rc = ensure(c, buf, hdr_bytes + n_words * 8);
@@ -777,7 +781,7 @@ extern "C" int sdbg_column_device_ptr(sdbg_segment* s, uint64_t field, void** d_
     cudaFree(col.d_packed);
     col.d_packed = nullptr; col.packed_bytes = 0;
   }
-  col.has_minmax = false; col.has_absmax = false; col.zone_ok = false;
+  col.has_minmax = false; col.has_absmax = false; col.zone_ok = false; col.h_zone.clear();
   if (d_values) *d_values = p;
   if (rows) *rows = it->second.rows;
   return SDBG_OK;
@@ -947,19 +951,200 @@ PostingsDev postings_view(const sdbg_segment* s, uint32_t ordinal_base) {
   return p;
 }
 
-int filter_view(sdbg_segment* s, const sdbg_col_pred* f, FilterDev* out) {
+// packed_ok: a packed column is described as {values = its d_packed block, type = kTypeFor} (for the TMA GROUP BY);
+// otherwise every column is described by its raw values.
+int col_view(sdbg_segment* s, uint64_t field, ColDev* out, uint64_t* rows, bool packed_ok = false) {
+  auto it = s->cols.find(field);
+  if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "column " + std::to_string(field) + " not staged");
+  ColumnObj& col = it->second;
+  out->validity = col.d_validity; out->type = col.type; out->pad = 0;
+  if (packed_ok && col.d_packed) { out->values = col.d_packed; out->type = kTypeFor; }
+  else { const int rc = raw_values(s->ctx, col, const_cast<void**>(&out->values)); if (rc) return rc; }
+  if (rows) *rows = col.rows;
+  return SDBG_OK;
+}
+
+// One pushed predicate on segment s: its column's view (col_view) and its constants resolved against the column's type.
+// *rows: the column's length.
+int pred_dev(sdbg_segment* s, const sdbg_col_pred& in, PredDev* out, uint64_t* rows, bool packed_ok = false) {
+  if (int rc = col_view(s, in.field, &out->col, rows, packed_ok)) return rc;
+  sdbg_col_pred p;
+  const int type = out->col.type == kTypeFor ? SDBG_I64 : out->col.type;   // a packed column holds int64
+  if (sdbg_col_pred_resolve(&in, type, &p)) return fail(s->ctx, SDBG_EINVAL, "bad predicate op");
+  out->op = p.op; out->pad = 0;
+  out->lo_i = p.lo_i; out->hi_i = p.hi_i;
+  out->lo_f = p.lo_f; out->hi_f = p.hi_f;
+  return SDBG_OK;
+}
+
+// Rewrites a resolved comparison as the per-doc test of the full-text kernels takes it (pred1): `lo <= v <= hi`
+// (SDBG_OP_BETWEEN; lo > hi: no row), or its negation for SQL <> (SDBG_OP_NE, lo == hi). Exact: integers step by 1 and
+// doubles by one ulp; NaN bounds hold for no row, so `<> NaN` holds for every non-NULL row. Keeps the per-doc code one
+// range test whatever the op.
+void between_form(PredDev& p) {
+  if (p.op == SDBG_OP_BETWEEN || p.op >= SDBG_OP_IS_NULL) return;
+  if (p.col.type == SDBG_F64) {
+    const double x = p.lo_f;
+    double lo = -HUGE_VAL, hi = HUGE_VAL;
+    switch (p.op) {
+      case SDBG_OP_LT: if (x == -HUGE_VAL) lo = 1.0, hi = 0.0; else hi = std::nextafter(x, -HUGE_VAL); break;
+      case SDBG_OP_LE: hi = x; break;
+      case SDBG_OP_GT: if (x == HUGE_VAL) lo = 1.0, hi = 0.0; else lo = std::nextafter(x, HUGE_VAL); break;
+      case SDBG_OP_GE: lo = x; break;
+      default: lo = hi = x; break;   // = and <>
+    }
+    p.lo_f = lo; p.hi_f = hi;
+  } else {
+    const int64_t x = p.lo_i;
+    int64_t lo = INT64_MIN, hi = INT64_MAX;
+    switch (p.op) {
+      case SDBG_OP_LT: if (x == INT64_MIN) lo = 1, hi = 0; else hi = x - 1; break;
+      case SDBG_OP_LE: hi = x; break;
+      case SDBG_OP_GT: if (x == INT64_MAX) lo = 1, hi = 0; else lo = x + 1; break;
+      case SDBG_OP_GE: lo = x; break;
+      default: lo = hi = x; break;
+    }
+    p.lo_i = lo; p.hi_i = hi;
+  }
+  if (p.op != SDBG_OP_NE) p.op = SDBG_OP_BETWEEN;
+}
+
+// The filter chain `f` of a full-text entry over segment s (sdbg.h, SDBG_OP_AND_NEXT): at most kMaxPreds predicates,
+// each on a column of at least n_docs rows. Only reads and checks; the zone verdicts come from chain_verdicts.
+int filter_view(sdbg_segment* s, const sdbg_col_pred* f, ChainDev* out) {
   std::memset(out, 0, sizeof *out);
   if (!f) return SDBG_OK;
-  auto it = s->cols.find(f->field);
-  if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "filter column not staged");
-  if (it->second.rows < s->n_docs) return fail(s->ctx, SDBG_EINVAL, "filter column shorter than segment");
-  sdbg_col_pred p;
-  if (sdbg_col_pred_resolve(f, it->second.type, &p)) return fail(s->ctx, SDBG_EINVAL, "bad predicate op");
-  void* raw = nullptr;
-  const int rc = raw_values(s->ctx, it->second, &raw);
-  if (rc) return rc;
-  out->values = raw; out->validity = it->second.d_validity; out->type = it->second.type;
-  out->op = p.op; out->lo_i = p.lo_i; out->hi_i = p.hi_i; out->lo_f = p.lo_f; out->hi_f = p.hi_f;
+  int n = 1;
+  while (f[n - 1].op & SDBG_OP_AND_NEXT) {
+    if (n == kMaxPreds) return fail(s->ctx, SDBG_EUNSUPPORTED, "a filter chain holds at most 4 predicates");
+    ++n;
+  }
+  out->ps.n = n;
+  for (int i = 0; i < n; ++i) {
+    sdbg_col_pred p = f[i];
+    p.op &= ~SDBG_OP_AND_NEXT;
+    uint64_t rows = 0;
+    if (int rc = pred_dev(s, p, &out->ps.p[i], &rows)) return rc;
+    if (rows < s->n_docs) return fail(s->ctx, SDBG_EINVAL, "filter column shorter than segment");
+    between_form(out->ps.p[i]);
+  }
+  return SDBG_OK;
+}
+
+// The zonemap of a NOT NULL column ({min, max} per kZoneRows rows in predicate key space), built on first use and kept
+// until the values change (restaging, sdbg_column_device_ptr).
+int column_zonemap(sdbg_ctx* c, ColumnObj& col, const long long** out) {
+  if (!col.zone_ok) {
+    void* raw = nullptr;
+    if (int rc = raw_values(c, col, &raw)) return rc;
+    if (int rc = ensure_zone(c, col)) return rc;
+    const uint64_t n_zones = (col.rows + kZoneRows - 1) / kZoneRows;
+    const unsigned zg = unsigned(std::min<uint64_t>((n_zones + 7) / 8, uint64_t(c->sm_count) * 8));
+    const auto* vals = static_cast<const unsigned char*>(raw);
+    if (col.type == SDBG_F64) zonemap_kernel<1><<<zg, 256, 0, c->stream>>>(vals, col.rows, col.d_zone);
+    else if (col.type == SDBG_I32) zonemap_kernel<2><<<zg, 256, 0, c->stream>>>(vals, col.rows, col.d_zone);
+    else zonemap_kernel<0><<<zg, 256, 0, c->stream>>>(vals, col.rows, col.d_zone);
+    ++c->launches;
+    CU(c, cudaGetLastError());
+    col.zone_ok = true; col.h_zone.clear();
+  }
+  *out = col.d_zone;
+  return SDBG_OK;
+}
+
+// Host copy of a NOT NULL column's zonemap (column_zonemap), fetched once per version of the values: one wait for the
+// stream, on first use only.
+int column_zonemap_host(sdbg_ctx* c, ColumnObj& col, const std::vector<long long>** out) {
+  if (col.h_zone.empty()) {
+    const long long* d = nullptr;
+    if (int rc = column_zonemap(c, col, &d)) return rc;
+    std::vector<long long> h(2 * ((col.rows + kZoneRows - 1) / kZoneRows));
+    CU(c, cudaMemcpyAsync(h.data(), d, h.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    col.h_zone = std::move(h);
+  }
+  *out = &col.h_zone;
+  return SDBG_OK;
+}
+
+// A resolved comparison (op < SDBG_OP_IS_NULL) as a closed range [*lo, *lo + *span] in the int64 key space of the
+// zonemaps (integers as they are, doubles through fkey()), from its between_form. *neg = 1 for SQL <>, which holds
+// outside the range. kKeyAll: the comparison holds for every non-NULL row; kKeyNone: for none.
+enum KeyRange { kKeyRange, kKeyAll, kKeyNone };
+KeyRange key_range(const PredDev& in, int64_t* lo, uint64_t* span, int* neg) {
+  PredDev pd = in;
+  between_form(pd);
+  *neg = pd.op == SDBG_OP_NE ? 1 : 0;
+  int64_t l, h;
+  if (pd.col.type == SDBG_F64) {
+    double lf = pd.lo_f, hf = pd.hi_f;
+    if (std::isnan(lf) || std::isnan(hf) || lf > hf) return *neg ? kKeyAll : kKeyNone;   // comparisons with NaN are false
+    if (lf == 0.0) lf = -0.0;                                      // -0.0 == +0.0: the range must cover both keys
+    if (hf == 0.0) hf = 0.0;
+    int64_t bl, bh; std::memcpy(&bl, &lf, 8); std::memcpy(&bh, &hf, 8);
+    l = fkey(bl); h = fkey(bh);
+  } else {
+    l = pd.lo_i; h = pd.hi_i;
+    if (l > h) return *neg ? kKeyAll : kKeyNone;
+  }
+  *lo = l; *span = static_cast<uint64_t>(h) - static_cast<uint64_t>(l);
+  return kKeyRange;
+}
+
+// Queues the zone verdicts of segment s's chain f (filter_view of `filt`): one verdict byte per kZoneRows-row zone, in
+// s->verdict. A predicate on a nullable column decides no zone; IS NULL / IS NOT NULL on a NOT NULL column holds for no
+// row / every row. Whether any zone is decided is known on the host from the zonemaps' host copies: when none is,
+// f->zone stays null and nothing is queued, so the per-doc kernels (top-k, scan) test nothing but the chain.
+int chain_verdicts(sdbg_segment* s, const sdbg_col_pred* filt, ChainDev* f) {
+  sdbg_ctx* c = s->ctx;
+  const uint64_t n_zones = (uint64_t(s->n_docs) + kZoneRows - 1) / kZoneRows;
+  if (!f->ps.n || !n_zones) return SDBG_OK;
+  ZoneVerdictParams Z;
+  std::memset(&Z, 0, sizeof Z);
+  Z.n_blocks = n_zones;
+  Z.pass = 1;
+  const long long* hz[kMaxPreds] = {};
+  bool never = false;
+  for (int i = 0; i < f->ps.n && !never; ++i) {
+    const PredDev& pd = f->ps.p[i];
+    ColumnObj& col = s->cols.find(filt[i].field)->second;
+    if (col.d_validity) { Z.pass = 0; continue; }
+    if (pd.op == SDBG_OP_IS_NULL) { never = true; continue; }
+    if (pd.op == SDBG_OP_IS_NOT_NULL) continue;
+    int64_t lo = 0; uint64_t span = 0; int neg = 0;
+    const KeyRange kr = key_range(pd, &lo, &span, &neg);
+    if (kr == kKeyAll) continue;
+    if (kr == kKeyNone) { never = true; continue; }
+    const int k = Z.n_preds++;
+    if (int rc = column_zonemap(c, col, &Z.zone[k])) return rc;
+    const std::vector<long long>* h = nullptr;
+    if (int rc = column_zonemap_host(c, col, &h)) return rc;
+    hz[k] = h->data();
+    Z.lo[k] = lo; Z.span[k] = span; Z.negate[k] = neg;
+  }
+  bool decided = never || (Z.pass && !Z.n_preds);   // some predicate holds for no row, or every one for every row
+  for (uint64_t z = 0; z < n_zones && !decided; ++z) decided = zone_verdict(Z, hz, z) != kZoneCheck;
+  if (!decided) return SDBG_OK;
+  if (int rc = ensure(c, s->verdict, n_zones)) return rc;
+  auto* v = static_cast<uint8_t*>(s->verdict.p);
+  f->zone = v; f->n_zones = uint32_t(n_zones);
+  if (never || !Z.n_preds) {
+    CU(c, cudaMemsetAsync(v, never ? kZoneDead : kZonePass, n_zones, c->stream));
+    return SDBG_OK;
+  }
+  const unsigned vg = unsigned(std::min<uint64_t>((n_zones + 255) / 256, uint64_t(c->sm_count) * 4));
+  zone_verdict_kernel<<<vg, 256, 0, c->stream>>>(Z, v, nullptr);
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  return SDBG_OK;
+}
+
+// The filter chains of a call's segments with their zone verdicts (out[n_segs]).
+int filter_chains(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred* filt, ChainDev* out) {
+  for (size_t si = 0; si < n_segs; ++si) {
+    if (int rc = filter_view(segs[si], filt, &out[si])) return rc;
+    if (int rc = chain_verdicts(segs[si], filt, &out[si])) return rc;
+  }
   return SDBG_OK;
 }
 
@@ -1119,7 +1304,7 @@ int check_query_batch(sdbg_segment* const* segs, size_t n_segs, const QueryBatch
   for (size_t si = 0; si < n_segs; ++si)
     for (uint32_t i = term_off[0]; i < term_off[nq]; ++i)
       if (size_t(term_id(terms[i])) + 1 >= segs[si]->term_blk_begin.size()) return fail(c, SDBG_EINVAL, "term id out of range");
-  FilterDev fv;
+  ChainDev fv;
   for (size_t si = 0; si < n_segs; ++si)
     if (int rc = filter_view(segs[si], filt, &fv)) return rc;
   return SDBG_OK;
@@ -1570,6 +1755,8 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm2
   uint64_t classes_present = 0;
   for (size_t si = 0; si < n_segs; ++si) for (uint32_t k2 = 0; k2 < kAllClasses; ++k2) if (n_cls[si][k2]) classes_present |= 1ull << k2;
   const bool two_lanes = (classes_present & (classes_present - 1u)) != 0u;
+  std::vector<ChainDev> chains(n_segs);
+  if ((rc = filter_chains(segs, n_segs, filt, chains.data()))) return rc;
   {
     ProfScope ps_(c, kProfTopk);   // one span for all top-k launches of the call
     uint32_t lane_no = 0;
@@ -1577,7 +1764,7 @@ int topk_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm2
       sdbg_segment* s = segs[si];
       TopkParams P;
       P.seg = postings_view(s, base);
-      if ((rc = filter_view(s, filt, &P.filt))) return rc;
+      P.filt = chains[si];
       D.params(d_desc, si, work_done, P);
       const uint4* const work0 = P.work;
       work_done += seg_work[si].size();
@@ -1994,18 +2181,8 @@ int sort_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, SortJob&
     base += segs[si]->n_docs;
     if (!c->wand || col.d_validity || !col.rows) continue;
     const uint64_t n_zones = (col.rows + kZoneRows - 1) / kZoneRows;
-    if (!col.zone_ok) {
-      if (int rc = ensure_zone(c, col)) return rc;
-      const unsigned zg = unsigned(std::min<uint64_t>((n_zones + 7) / 8, uint64_t(c->sm_count) * 8));
-      const auto* vals = static_cast<const unsigned char*>(raw);
-      if (col.type == SDBG_F64) zonemap_kernel<1><<<zg, 256, 0, c->stream>>>(vals, col.rows, col.d_zone);
-      else if (col.type == SDBG_I32) zonemap_kernel<2><<<zg, 256, 0, c->stream>>>(vals, col.rows, col.d_zone);
-      else zonemap_kernel<0><<<zg, 256, 0, c->stream>>>(vals, col.rows, col.d_zone);
-      ++c->launches;
-      CU(c, cudaGetLastError());
-      col.zone_ok = true;
-    }
-    S.zone = col.d_zone; S.n_zones = uint32_t(n_zones);
+    if (int rc = column_zonemap(c, col, &S.zone)) return rc;
+    S.n_zones = uint32_t(n_zones);
   }
   // host copies of the zonemaps last, and always waited for: J.zone must outlive every queued copy
   cudaError_t e = cudaSuccess;
@@ -2134,9 +2311,9 @@ struct CountPlan {
   }
 
   // The parameters of segment si's launch over its work items from `first` on, d the device copy of the staging.
-  int params(const char* d, sdbg_segment* s, size_t si, size_t first, const sdbg_col_pred* filt, CountParams* P) const {
+  void params(const char* d, sdbg_segment* s, size_t si, size_t first, const ChainDev& filt, CountParams* P) const {
     P->seg = postings_view(s, 0);
-    if (int rc = filter_view(s, filt, &P->filt)) return rc;
+    P->filt = filt;
     P->lists = reinterpret_cast<const uint2*>(d + lists_pos) + si * n_lists();
     P->term_off = reinterpret_cast<const uint32_t*>(d);
     P->excl_off = total_excl ? reinterpret_cast<const uint32_t*>(d + off_bytes) : nullptr;
@@ -2146,7 +2323,6 @@ struct CountPlan {
       P->grp_off = reinterpret_cast<const uint32_t*>(d + grp_pos);
       P->grp_end = reinterpret_cast<const uint32_t*>(d + grp_pos + off_bytes) + si * grp_off[Q.nq];
     }
-    return SDBG_OK;
   }
 
   // The bm25_count_kernel instantiation of this plan's launches in `mode`, with its dynamic shared memory: the mode's
@@ -2367,6 +2543,8 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
                                                            : 0;
   const auto [kernel, smem] = pl.kernel(job.mode, mode_bytes);
   CU(c, fit_dynamic_smem(kernel, smem));
+  std::vector<ChainDev> chains(n_segs);
+  if (int rc = filter_chains(segs, n_segs, filt, chains.data())) return rc;
   for (int phase = 0; phase < 2; ++phase) {   // seeds (sorted scan only), then the rest
     size_t begin = 0;
     for (size_t si = 0; si < n_segs; ++si) {
@@ -2376,7 +2554,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
       begin += w.size();
       if (!n) continue;
       CountParams P;
-      if (int rc = pl.params(d, segs[si], si, first, filt, &P)) return rc;
+      pl.params(d, segs[si], si, first, chains[si], &P);
       P.counts = static_cast<unsigned long long*>(out.counts);
       if (sort) {
         P.counts = nullptr;
@@ -2944,6 +3122,8 @@ int scan_run(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_te
   const uint32_t chunk = uint32_t((uint64_t(range) + g - 1) / g);   // 64-bit: range reaches 2^32 - 2
   for (uint32_t i = 0; i < T; ++i)
     if (terms[i].term + 1 >= s->term_blk_begin.size()) return fail(c, SDBG_EINVAL, "term id out of range");
+  ChainDev chain;
+  if (int rc = filter_chains(&s, 1, filt, &chain)) return rc;
   // one query, one candidate list per chain, its excluded terms as its check lists
   std::vector<uint4> work(g);
   for (uint32_t j = 0; j < g; ++j) {
@@ -2971,7 +3151,7 @@ int scan_run(sdbg_segment* s, int kind, const sdbg_bm25_term* terms, size_t n_te
   CU(c, cudaMemsetAsync(b_theta.p, 0, 32, c->stream));
   TopkParams P;
   P.seg = postings_view(s, 0);
-  if ((rc = filter_view(s, filt, &P.filt))) return rc;
+  P.filt = chain;
   D.params(static_cast<const char*>(b_qt.p), 0, 0, P);
   P.theta = static_cast<unsigned long long*>(b_theta.p);
   P.total = P.theta + 1;
@@ -3147,35 +3327,15 @@ extern "C" int sdbg_decode_score_term(sdbg_segment* s, uint32_t term, float c0, 
 // ------------------------------------------------------------------------------------------
 namespace {
 
-// packed_ok: a packed column is described as {values = its d_packed block, type = kTypeFor} (for the TMA GROUP BY);
-// otherwise every column is described by its raw values.
-int col_view(sdbg_segment* s, uint64_t field, ColDev* out, uint64_t* rows, bool packed_ok = false) {
-  auto it = s->cols.find(field);
-  if (it == s->cols.end()) return fail(s->ctx, SDBG_ENOTFOUND, "column " + std::to_string(field) + " not staged");
-  ColumnObj& col = it->second;
-  out->validity = col.d_validity; out->type = col.type; out->pad = 0;
-  if (packed_ok && col.d_packed) { out->values = col.d_packed; out->type = kTypeFor; }
-  else { const int rc = raw_values(s->ctx, col, const_cast<void**>(&out->values)); if (rc) return rc; }
-  if (rows) *rows = col.rows;
-  return SDBG_OK;
-}
-
 int pred_set(sdbg_segment* s, const sdbg_col_pred* preds, size_t n, PredSet* ps, uint64_t* rows, bool packed_ok = false) {
   if (n > size_t(kMaxPreds)) return fail(s->ctx, SDBG_EUNSUPPORTED, "more than 4 pushed predicates");
   std::memset(ps, 0, sizeof *ps);
   ps->n = int(n);
   for (size_t i = 0; i < n; ++i) {
     uint64_t r = 0;
-    const int rc = col_view(s, preds[i].field, &ps->p[i].col, &r, packed_ok);
-    if (rc) return rc;
+    if (int rc = pred_dev(s, preds[i], &ps->p[i], &r, packed_ok)) return rc;
     if (*rows == 0) *rows = r;
     if (r != *rows) return fail(s->ctx, SDBG_EINVAL, "columns of one segment differ in length");
-    sdbg_col_pred p;
-    const int type = ps->p[i].col.type == kTypeFor ? SDBG_I64 : ps->p[i].col.type;   // a packed column holds int64
-    if (sdbg_col_pred_resolve(&preds[i], type, &p)) return fail(s->ctx, SDBG_EINVAL, "bad predicate op");
-    ps->p[i].op = p.op;
-    ps->p[i].lo_i = p.lo_i; ps->p[i].hi_i = p.hi_i;
-    ps->p[i].lo_f = p.lo_f; ps->p[i].hi_f = p.hi_f;
   }
   return SDBG_OK;
 }
@@ -3485,56 +3645,21 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
         }
         return n;
       };
-      // Every comparison becomes a closed range [lo, lo + span] in an int64 key space (integers as they
-      // are, doubles through fkey()): exact, because integers step by 1 and doubles by one ulp. Predicates
-      // that hold for every row are dropped; one that holds for none makes the segment contribute nothing.
+      // Every comparison becomes a closed range of the zonemaps' key space (key_range). Predicates that hold for every
+      // row are dropped; one that holds for none makes the segment contribute nothing.
       bool never = false;
       int stream_idx[kMaxPreds];
       T.n_preds = 0;
       for (int i = 0; i < P.ps.n; ++i) {
         const PredDev& pd = P.ps.p[i];
-        int64_t lo, hi; int neg = 0; bool empty = false;
-        if (pd.col.type == SDBG_F64) {
-          double lf = -HUGE_VAL, hf = HUGE_VAL;
-          const double x = pd.lo_f;
-          if (std::isnan(x) || (pd.op == SDBG_OP_BETWEEN && std::isnan(pd.hi_f))) empty = true;   // comparisons with NaN are false
-          switch (pd.op) {
-            case SDBG_OP_LT: if (x == -HUGE_VAL) empty = true; else hf = std::nextafter(x, -HUGE_VAL); break;
-            case SDBG_OP_LE: hf = x; break;
-            case SDBG_OP_GT: if (x == HUGE_VAL) empty = true; else lf = std::nextafter(x, HUGE_VAL); break;
-            case SDBG_OP_GE: lf = x; break;
-            case SDBG_OP_EQ: lf = hf = x; break;
-            case SDBG_OP_NE: lf = hf = x; neg = 1; break;
-            default: lf = x; hf = pd.hi_f; break;
-          }
-          if (pd.op == SDBG_OP_NE && std::isnan(x)) continue;      // v <> NaN holds for every row
-          if (!empty && lf > hf) empty = true;
-          if (!empty) {
-            if (lf == 0.0) lf = -0.0;                               // -0.0 == +0.0: the range must cover both keys
-            if (hf == 0.0) hf = 0.0;
-            int64_t bl, bh; std::memcpy(&bl, &lf, 8); std::memcpy(&bh, &hf, 8);
-            lo = fkey(bl); hi = fkey(bh);
-          }
-        } else {
-          int64_t li = INT64_MIN, hi_ = INT64_MAX;
-          const int64_t x = pd.lo_i;
-          switch (pd.op) {
-            case SDBG_OP_LT: if (x == INT64_MIN) empty = true; else hi_ = x - 1; break;
-            case SDBG_OP_LE: hi_ = x; break;
-            case SDBG_OP_GT: if (x == INT64_MAX) empty = true; else li = x + 1; break;
-            case SDBG_OP_GE: li = x; break;
-            case SDBG_OP_EQ: li = hi_ = x; break;
-            case SDBG_OP_NE: li = hi_ = x; neg = 1; break;
-            default: li = x; hi_ = pd.hi_i; break;
-          }
-          if (li > hi_) empty = true;
-          lo = li; hi = hi_;
-        }
-        if (empty) { if (neg) continue; never = true; break; }
+        int64_t lo = 0; uint64_t span = 0; int neg = 0;
+        const KeyRange kr = key_range(pd, &lo, &span, &neg);
+        if (kr == kKeyAll) continue;
+        if (kr == kKeyNone) { never = true; break; }
         const int k = T.n_preds++;
         stream_idx[k] = stream_of(pd.col);
         T.pred_type[k] = pd.col.type; T.pred_negate[k] = neg;
-        T.pred_lo[k] = lo; T.pred_span[k] = static_cast<uint64_t>(hi) - static_cast<uint64_t>(lo);
+        T.pred_lo[k] = lo; T.pred_span[k] = span;
       }
       if (never) continue;   // WHERE is false for every row of this segment
       // Zonemap verdicts: blocks whose min / max miss a predicate's range are skipped by producer and consumers alike.
@@ -3549,17 +3674,7 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
           Z.lo[k2] = T.pred_lo[k2]; Z.span[k2] = T.pred_span[k2]; Z.negate[k2] = T.pred_negate[k2];
           ColumnObj* co = column_of(stream_id[stream_idx[k2]]);
           if (!co || co->d_validity) continue;
-          if (!co->zone_ok) {
-            if (!co->d_zone) CU(c, cudaMalloc(reinterpret_cast<void**>(&co->d_zone), Z.n_blocks * 16));
-            co->zone_ok = true;
-            const unsigned zg = unsigned(std::min<uint64_t>((Z.n_blocks + 7) / 8, uint64_t(c->sm_count) * 8));
-            const auto* vals = static_cast<const unsigned char*>(co->d_values);
-            if (co->type == SDBG_F64) zonemap_kernel<1><<<zg, 256, 0, c->stream>>>(vals, rows, co->d_zone);
-            else if (co->type == SDBG_I32) zonemap_kernel<2><<<zg, 256, 0, c->stream>>>(vals, rows, co->d_zone);
-            else zonemap_kernel<0><<<zg, 256, 0, c->stream>>>(vals, rows, co->d_zone);
-            ++c->launches;
-          }
-          Z.zone[k2] = co->d_zone;
+          if ((rc = column_zonemap(c, *co, &Z.zone[k2]))) return rc;
           any_zone = true;
         }
         if (any_zone) {

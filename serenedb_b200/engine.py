@@ -503,8 +503,24 @@ def _one(x):
     return None if x is None else [list(x)]
 
 
+AND_NEXT = 0x100   # sdbg.h SDBG_OP_AND_NEXT
+
+
 def _ref(filt):
-    return C.byref(filt) if filt is not None else None
+    """The `filt` argument of every full-text entry: None, one pred(), or a list / tuple of up to 4 of them ANDed
+    together, passed as one contiguous chain whose entries but the last carry SDBG_OP_AND_NEXT (sdbg.h). A list of one is
+    that pred, [] is no filter; more than 4 is refused by the library (SDBG_EUNSUPPORTED)."""
+    if filt is None:
+        return None
+    preds = [filt] if isinstance(filt, N.ColPred) else list(filt)
+    if not preds:
+        return None
+    chain = (N.ColPred * len(preds))()
+    for i, p in enumerate(preds):
+        chain[i] = p
+        if i + 1 < len(preds):
+            chain[i].op |= AND_NEXT
+    return chain
 
 
 def ExecuteTopKBatch(reader, queries, kind, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
@@ -1012,7 +1028,7 @@ def StreamScoredDocs(reader, seg_idx, query, kind, scorer, filt=None, doc_min=1,
     seg = reader.segments[seg_idx]
     x = np.ascontiguousarray(list(exclude) if exclude else [], dtype=np.uint32)
     terms = (N.BM25Term * len(query))(*[reader.stats(scorer, t) for t in query])
-    fp = C.byref(filt) if filt is not None else None
+    fp = _ref(filt)
     hi = int(doc_max) if doc_max is not None else 0xFFFFFFFF
     n = C.c_uint64(0)
     cap = 0
@@ -1050,7 +1066,7 @@ class PreparedBatch:
     """Query descriptors marshalled once (terms + statistics), reusable across steps."""
 
     def __init__(self, reader, queries, kind, scorer, k, filt=None, threshold=FLT_MIN, exclude=None):
-        self.reader, self.kind, self.scorer, self.k, self.filt, self.threshold = reader, int(kind), scorer, int(k), filt, float(threshold)
+        self.reader, self.kind, self.scorer, self.k, self.filt, self.threshold = reader, int(kind), scorer, int(k), _ref(filt), float(threshold)
         self.nq = len(queries)
         self.terms, self.off = _flatten_queries(reader, queries, scorer)
         self.excl = _exclusions(exclude, self.nq)   # None: no query excludes anything
@@ -1061,7 +1077,7 @@ class PreparedBatch:
     def run_host(self):
         """Full API call: host descriptors in, host hits out."""
         r = self.reader
-        fp = C.byref(self.filt) if self.filt is not None else None
+        fp = self.filt
         if self.excl is None:
             N.check(N.lib().sdbg_bm25_topk_batch(_seg_array(r.segments), len(r.segments), self.kind, self.terms,
                                                  _ptr(self.off), self.nq, self.scorer.k, self.scorer.b, fp, self.k, self.threshold,
@@ -1079,10 +1095,11 @@ class PreparedBatch:
 
     def run_dist(self, to_host=True):
         """Distributed top-k (sdbg_dist_bm25_topk_batch): local scan, one all-gather, local selection -- all enqueued by
-        the library on its stream. to_host=False leaves the merged keys in HBM and returns without waiting."""
+        the library on its stream. to_host=False leaves the merged keys in HBM and returns without waiting (except the
+        once-per-column zonemap copy of a filter chain, sdbg.h SDBG_OP_AND_NEXT)."""
         self._no_exclusions("run_dist")
         r = self.reader
-        fp = C.byref(self.filt) if self.filt is not None else None
+        fp = self.filt
         if to_host:
             hits = np.zeros((self.nq, self.k), HIT_DTYPE)
             n_out = np.zeros(self.nq, np.uint32)
@@ -1098,7 +1115,7 @@ class PreparedBatch:
         """Results stay in HBM as sortable keys (for the multi-GPU gather + merge)."""
         self._no_exclusions("run_device")
         r = self.reader
-        fp = C.byref(self.filt) if self.filt is not None else None
+        fp = self.filt
         N.check(N.lib().sdbg_bm25_topk_batch_device(_seg_array(r.segments), len(r.segments), self.kind, self.terms,
                                                     _ptr(self.off), self.nq, self.scorer.k, self.scorer.b, fp, self.k, self.threshold,
                                                     int(rank), C.c_void_p(int(d_keys_ptr)),

@@ -7,7 +7,9 @@
 // (tests/test_gpu_min_match.py); with "sorted", only the sorted scan (GpuSortedScan, tests/test_gpu_sort_by_column.py); with
 // "facet", only the facet counts (GpuFacetScan, tests/test_gpu_facets.py). "sorted groups" / "facet groups" run those two
 // with group queries (tests/test_gpu_groups_column.py). "aggregate" / "aggregate groups" run the aggregates over the matches
-// (GpuMatchAggScan, tests/test_gpu_match_aggregates.py).
+// (GpuMatchAggScan, tests/test_gpu_match_aggregates.py). "chain" runs a pushed filter chain (SDBG_OP_AND_NEXT) through the
+// top-k, streaming and count adapters next to the same calls filtered by an indicator column of the chain
+// (tests/test_gpu_filter_chains.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -44,6 +46,53 @@ int main(int argc, char** argv) {
   const uint32_t ids[2] = {2, 5};
   for (int i = 0; i < 2; ++i) { sdbg_bm25_collect(n_docs, sum_dl, dc[ids[i]], 1.2f, 0.75f, &terms[size_t(i)]); terms[size_t(i)].term = ids[i]; }
   sdbg_col_pred filt{}; filt.field = 9; filt.op = SDBG_OP_BETWEEN; filt.lo_i = 250000; filt.hi_i = 749999;
+  if (argc > 2 && std::string(argv[2]) == "chain") {
+    // `9 BETWEEN 250000 AND 749999 AND 20 < n_docs / 2 AND 9 <> 500000` (field 20: value = row, doc-ordered), then the
+    // indicator column 21 = 1 where the chain holds (int32, nullable with every row valid) as the single predicate
+    std::vector<int32_t> v9(n_docs);
+    std::vector<int64_t> v20(n_docs);
+    sdbg_column_to_host(seg, 9, v9.data(), n_docs);
+    std::vector<int32_t> m(n_docs);
+    for (uint32_t r = 0; r < n_docs; ++r) {
+      v20[r] = int64_t(r);
+      m[r] = v9[r] >= 250000 && v9[r] <= 749999 && v20[r] < int64_t(n_docs / 2) && v9[r] != 500000;
+    }
+    std::vector<uint64_t> valid((n_docs + 63) / 64, ~0ull);
+    sdbg_stage_column(seg, 20, SDBG_I64, v20.data(), nullptr, n_docs);
+    sdbg_stage_column(seg, 21, SDBG_I32, m.data(), valid.data(), n_docs);
+    sdbg_col_pred chain[3] = {filt, {}, {}};
+    chain[0].op |= SDBG_OP_AND_NEXT;
+    chain[1].field = 20; chain[1].op = SDBG_OP_LT | SDBG_OP_AND_NEXT; chain[1].lo_i = n_docs / 2;
+    chain[2].field = 9; chain[2].op = SDBG_OP_NE; chain[2].lo_i = 500000;
+    sdbg_col_pred ind{}; ind.field = 21; ind.op = SDBG_OP_EQ; ind.lo_i = 1;
+    irs::ScoreFunction sf; irs::ColumnArgsFetcher fetcher;
+    for (int indicator = 0; indicator < 2; ++indicator) {
+      const sdbg_col_pred* f = indicator ? &ind : chain;
+      ListCollector col;
+      sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_OR, terms, 1.2f, 0.75f, 100, f);
+      it.Collect(sf, fetcher, col);
+      std::printf("{\"indicator\": %d, \"topk\": [", indicator);
+      for (size_t i = 0; i < col.docs.size(); ++i) std::printf("%s[%u, %.9g]", i ? ", " : "", col.docs[i].doc, double(col.docs[i].score));
+      sdbg_host::GpuTopKIterator st(seg, SDBG_QUERY_OR, terms, 1.2f, 0.75f, 0, f);
+      std::vector<irs::doc_id_t> d(2048);
+      std::vector<irs::score_t> sc(2048);
+      uint64_t n = 0, doc_sum = 0;
+      for (irs::doc_id_t lo = 1; lo <= n_docs; lo += 2048) {
+        const uint32_t got = st.EmitScoredDocs(d.data(), sc.data(), lo + 2048, sf, &fetcher, lo);
+        for (uint32_t i = 0; i < got; ++i) doc_sum += d[i];
+        n += got;
+      }
+      sdbg_host::GpuCountScan scan({seg}, SDBG_QUERY_OR, {2, 5}, {}, f);
+      duckdb::DataChunkMock chunk;
+      scan.Scan(chunk);
+      std::printf("], \"total\": %llu, \"stream_n\": %llu, \"stream_doc_sum\": %llu, \"count\": %lld}\n",
+                  static_cast<unsigned long long>(it.total_matches()), static_cast<unsigned long long>(n),
+                  static_cast<unsigned long long>(doc_sum), chunk.size ? static_cast<long long>(chunk.count[0]) : -1ll);
+    }
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
   if (argc > 2 && std::string(argv[2]) == "excl") {
     // `t2 | t5` minus the docs of t3: Collect (top-100) and the streaming mode (k = 0), without and with the table filter
     ListCollector col;

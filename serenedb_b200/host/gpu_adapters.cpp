@@ -26,12 +26,17 @@ const uint32_t* group_minimums(const std::vector<uint32_t>& mins, size_t n_group
 }
 }  // namespace
 
+FilterChain::FilterChain(const sdbg_col_pred* table_filter) {
+  // a 4th entry that still carries the bit is kept: the library refuses the chain (SDBG_EUNSUPPORTED)
+  for (const sdbg_col_pred* f = table_filter; f; f = (f->op & SDBG_OP_AND_NEXT) && preds.size() < 4 ? f + 1 : nullptr)
+    preds.push_back(*f);
+}
+
 GpuTopKIterator::GpuTopKIterator(sdbg_segment* segment, int kind, std::vector<sdbg_bm25_term> terms, float k1, float b,
                                  uint32_t k, const sdbg_col_pred* table_filter, std::vector<uint32_t> excluded_terms,
                                  std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)
     : seg_(segment), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)), groups_(std::move(group_sizes)),
-      group_min_(std::move(group_min_match)), k1_(k1), b_(b), k_(k), has_filter_(table_filter != nullptr) {
-  if (table_filter) filter_ = *table_filter;
+      group_min_(std::move(group_min_match)), k1_(k1), b_(b), k_(k), filter_(table_filter) {
   threshold_.value = FLT_MIN;  // doc_collector.hpp:102
   // the streaming scan (sdbg_bm25_scan*) has no grouped form
   if (!groups_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "OR groups need k > 0: the streaming scan has no grouped form");
@@ -44,7 +49,7 @@ void GpuTopKIterator::run() {
     std::vector<uint32_t> docs;
     std::vector<float> scores;
     for (;;) {
-      const sdbg_col_pred* f = has_filter_ ? &filter_ : nullptr;
+      const sdbg_col_pred* f = filter_.data();
       const int rc = excluded_.empty()
                          ? sdbg_bm25_scan(seg_, kind_, terms_.data(), terms_.size(), k1_, b_, f, 1, UINT32_MAX, docs.data(), scores.data(), cap, &n)
                          : sdbg_bm25_scan_excl(seg_, kind_, terms_.data(), terms_.size(), excluded_.data(), excluded_.size(), k1_, b_, f, 1,
@@ -69,17 +74,17 @@ void GpuTopKIterator::run() {
     const uint32_t query_group_off[2] = {0, uint32_t(groups_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
     check(sdbg_bm25_topk_batch_groups_min(segs, 1, terms_.data(), group_off.data(), query_group_off,
                                           group_minimums(group_min_, groups_.size()), 1, excluded_.data(), excl_off, k1_, b_,
-                                          has_filter_ ? &filter_ : nullptr, k_, threshold_.value, hits_.data(), &n, &total_),
+                                          filter_.data(), k_, threshold_.value, hits_.data(), &n, &total_),
           "sdbg_bm25_topk_batch_groups_min");
     thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;
   } else if (excluded_.empty()) {
-    check(sdbg_bm25_topk(segs, 1, kind_, terms_.data(), terms_.size(), k1_, b_, has_filter_ ? &filter_ : nullptr, k_,
+    check(sdbg_bm25_topk(segs, 1, kind_, terms_.data(), terms_.size(), k1_, b_, filter_.data(), k_,
                          threshold_.value, hits_.data(), &n, &total_, &thr_out),
           "sdbg_bm25_topk");
   } else {
     const uint32_t term_off[2] = {0, uint32_t(terms_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
     check(sdbg_bm25_topk_batch_excl(segs, 1, kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off, k1_, b_,
-                                    has_filter_ ? &filter_ : nullptr, k_, threshold_.value, hits_.data(), &n, &total_),
+                                    filter_.data(), k_, threshold_.value, hits_.data(), &n, &total_),
           "sdbg_bm25_topk_batch_excl");
     thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;   // as sdbg_bm25_topk derives it
   }
@@ -202,8 +207,7 @@ GpuCountScan::GpuCountScan(std::vector<sdbg_segment*> segments, int kind, std::v
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, std::vector<uint32_t> group_sizes,
                            std::vector<uint32_t> group_min_match)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      groups_(std::move(group_sizes)), group_min_(std::move(group_min_match)), has_filter_(table_filter != nullptr) {
-  if (table_filter) filter_ = *table_filter;
+      groups_(std::move(group_sizes)), group_min_(std::move(group_min_match)), filter_(table_filter) {
 }
 
 void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
@@ -216,14 +220,14 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
   const char* what;
   if (groups_.empty()) {
     rc = sdbg_match_count_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
-                                has_filter_ ? &filter_ : nullptr, &n);
+                                filter_.data(), &n);
     what = "sdbg_match_count_batch: ";
   } else {                                                    // an And of Ors: kind_ is not used
     const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
     const uint32_t query_group_off[2] = {0, uint32_t(groups_.size())};
     rc = sdbg_match_count_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
                                            group_minimums(group_min_, groups_.size()), 1, excluded_.data(), excl_off,
-                                           has_filter_ ? &filter_ : nullptr, &n);
+                                           filter_.data(), &n);
     what = "sdbg_match_count_batch_groups_min: ";
   }
   if (rc != SDBG_OK) throw GpuError(rc, std::string(what) + sdbg_last_error(sdbg_segment_context(segs_[0])));
@@ -237,9 +241,8 @@ GpuSortedScan::GpuSortedScan(std::vector<sdbg_segment*> segments, int kind, std:
                              bool descending, bool nulls_first, uint32_t k, std::vector<uint32_t> group_sizes,
                              std::vector<uint32_t> group_min_match)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), has_filter_(table_filter != nullptr),
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), filter_(table_filter),
       field_(sort_field), desc_(descending), nulls_first_(nulls_first), k_(k) {
-  if (table_filter) filter_ = *table_filter;
 }
 
 void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
@@ -253,7 +256,7 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
     const char* what;
     if (group_sizes_.empty()) {
       rc = sdbg_match_topk_by_column_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
-                                           has_filter_ ? &filter_ : nullptr, field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
+                                           filter_.data(), field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
                                            hits_.data(), &n);
       what = "sdbg_match_topk_by_column_batch: ";
     } else {                                                  // an And of Ors: kind_ is not used
@@ -261,7 +264,7 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
       const uint32_t query_group_off[2] = {0, uint32_t(group_sizes_.size())};
       rc = sdbg_match_topk_by_column_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
                                                       group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(),
-                                                      excl_off, has_filter_ ? &filter_ : nullptr, field_, desc_ ? 1 : 0,
+                                                      excl_off, filter_.data(), field_, desc_ ? 1 : 0,
                                                       nulls_first_ ? 1 : 0, k_, hits_.data(), &n);
       what = "sdbg_match_topk_by_column_batch_groups_min: ";
     }
@@ -285,9 +288,8 @@ GpuFacetScan::GpuFacetScan(std::vector<sdbg_segment*> segments, int kind, std::v
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
                            std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), has_filter_(table_filter != nullptr),
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), filter_(table_filter),
       field_(key_field) {
-  if (table_filter) filter_ = *table_filter;
 }
 
 void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
@@ -312,14 +314,14 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
     const char* what;
     if (group_sizes_.empty()) {
       rc = sdbg_match_facet_counts_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
-                                         has_filter_ ? &filter_ : nullptr, field_, lo, uint32_t(span), counts.data(), &nulls_);
+                                         filter_.data(), field_, lo, uint32_t(span), counts.data(), &nulls_);
       what = "sdbg_match_facet_counts_batch: ";
     } else {                                                  // an And of Ors: kind_ is not used
       const std::vector<uint32_t> group_off = group_offsets(group_sizes_, terms_.size());
       const uint32_t query_group_off[2] = {0, uint32_t(group_sizes_.size())};
       rc = sdbg_match_facet_counts_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
                                                     group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(),
-                                                    excl_off, has_filter_ ? &filter_ : nullptr, field_, lo, uint32_t(span),
+                                                    excl_off, filter_.data(), field_, lo, uint32_t(span),
                                                     counts.data(), &nulls_);
       what = "sdbg_match_facet_counts_batch_groups_min: ";
     }
@@ -345,9 +347,8 @@ GpuMatchAggScan::GpuMatchAggScan(std::vector<sdbg_segment*> segments, int kind, 
                                  uint64_t value_field, sdbg_type value_type, std::vector<uint32_t> group_sizes,
                                  std::vector<uint32_t> group_min_match)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), has_filter_(table_filter != nullptr),
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), filter_(table_filter),
       key_field_(key_field), value_field_(value_field), value_type_(value_type) {
-  if (table_filter) filter_ = *table_filter;
 }
 
 void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
@@ -379,7 +380,7 @@ void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
     const char* what;
     if (group_sizes_.empty()) {
       rc = sdbg_match_aggregate_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
-                                      has_filter_ ? &filter_ : nullptr, key_field_, lo, uint32_t(span), value_field_, cells.data(),
+                                      filter_.data(), key_field_, lo, uint32_t(span), value_field_, cells.data(),
                                       &null_cell);
       what = "sdbg_match_aggregate_batch: ";
     } else {                                                  // an And of Ors: kind_ is not used
@@ -387,7 +388,7 @@ void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
       const uint32_t query_group_off[2] = {0, uint32_t(group_sizes_.size())};
       rc = sdbg_match_aggregate_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
                                                  group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(), excl_off,
-                                                 has_filter_ ? &filter_ : nullptr, key_field_, lo, uint32_t(span), value_field_,
+                                                 filter_.data(), key_field_, lo, uint32_t(span), value_field_,
                                                  cells.data(), &null_cell);
       what = "sdbg_match_aggregate_batch_groups_min: ";
     }

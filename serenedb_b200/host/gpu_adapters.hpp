@@ -31,6 +31,16 @@ struct GpuError : std::runtime_error {
   GpuError(int c, const std::string& what) : std::runtime_error(what), code(c) {}
 };
 
+// A pushed filter as the adapters keep it: the whole chain at `table_filter` (sdbg.h, SDBG_OP_AND_NEXT; the conjunction
+// of a ConjunctionAndFilter's comparison children), copied entry by entry up to the first without the bit or the 4th.
+// data() is what the ABI takes: NULL for no filter.
+struct FilterChain {
+  std::vector<sdbg_col_pred> preds;
+  FilterChain() = default;
+  explicit FilterChain(const sdbg_col_pred* table_filter);
+  const sdbg_col_pred* data() const { return preds.empty() ? nullptr : preds.data(); }
+};
+
 // One scored query over one staged segment.
 class GpuTopKIterator final : public irs::DocIterator {
  public:
@@ -77,8 +87,7 @@ class GpuTopKIterator final : public irs::DocIterator {
   std::vector<uint32_t> group_min_;   // their minimum match counts (empty: all 1)
   float k1_, b_;
   uint32_t k_;
-  bool has_filter_;
-  sdbg_col_pred filter_{};
+  FilterChain filter_;
   irs::ScoreThresholdAttr threshold_;
   irs::CostAttr cost_;
   std::vector<sdbg_hit> hits_;   // sorted by (score desc, doc asc) after run()
@@ -124,8 +133,7 @@ class GpuCountScan {
   std::vector<sdbg_segment*> segs_;
   int kind_;
   std::vector<uint32_t> terms_, excluded_, groups_, group_min_;
-  bool has_filter_;
-  sdbg_col_pred filter_{};
+  FilterChain filter_;
   bool done_ = false;
 };
 
@@ -148,8 +156,7 @@ class GpuSortedScan {
   std::vector<sdbg_segment*> segs_;
   int kind_;
   std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
-  bool has_filter_;
-  sdbg_col_pred filter_{};
+  FilterChain filter_;
   uint64_t field_;
   bool desc_, nulls_first_;
   uint32_t k_;
@@ -177,8 +184,7 @@ class GpuFacetScan {
   std::vector<sdbg_segment*> segs_;
   int kind_;
   std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
-  bool has_filter_;
-  sdbg_col_pred filter_{};
+  FilterChain filter_;
   uint64_t field_;
   std::vector<std::pair<int64_t, uint64_t>> groups_;   // (key, count) of the non-empty groups
   uint64_t nulls_ = 0;                                 // the NULL group's count
@@ -209,8 +215,7 @@ class GpuMatchAggScan {
   std::vector<sdbg_segment*> segs_;
   int kind_;
   std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
-  bool has_filter_;
-  sdbg_col_pred filter_{};
+  FilterChain filter_;
   uint64_t key_field_, value_field_;
   sdbg_type value_type_;
   std::vector<std::pair<int64_t, sdbg_match_agg>> groups_;   // (key, cell) of the rows to emit
