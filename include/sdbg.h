@@ -243,8 +243,8 @@ int sdbg_bm25_scan(sdbg_segment*, int kind, const sdbg_bm25_term* terms, size_t 
  * there. An empty set everywhere gives exactly sdbg_bm25_topk_batch's result. More than 16 excluded terms in a query:
  * SDBG_EUNSUPPORTED; a decreasing excl_off, or NULL excl_terms with a non-empty range: SDBG_EINVAL.
  * sdbg_bm25_scan_excl: sdbg_bm25_scan minus the docs of excl_terms[0 .. n_excl).
- * sdbg_bm25_topk_batch_device and sdbg_dist_bm25_topk_batch have no exclusion form yet; they run the same dispatch as
- * sdbg_bm25_topk_batch, so adding one means passing the exclusion lists through. */
+ * The top-k of queries with exclusions across GPUs: sdbg_dist_bm25_topk_batch_groups_min (a flat query is a degenerate
+ * groups query); sdbg_bm25_topk_batch_device and sdbg_dist_bm25_topk_batch take flat queries without exclusions only. */
 int sdbg_bm25_topk_batch_excl(sdbg_segment* const* segs, size_t n_segs, int kind, const sdbg_bm25_term* terms,
                               const uint32_t* term_off, size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off,
                               float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in,
@@ -330,8 +330,9 @@ int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int 
  * sdbg_match_facet_counts_batch_groups_min below.
  * Memory: as sdbg_bm25_topk_batch; a batch whose queries take several of the shapes above also holds its per-shape rows
  * in HBM (n_queries * (8k + 12) B) before they go to query order on the device.
- * Not supported yet: the streaming scan (sdbg_bm25_scan*), grouped forms of sdbg_bm25_topk_batch_device and
- * sdbg_dist_bm25_topk_batch, deeper nesting (an OR of ANDs), more than 16 positive terms, phrases. */
+ * The top-k of group queries across GPUs: sdbg_dist_bm25_topk_batch_groups_min below.
+ * Not supported yet: the streaming scan (sdbg_bm25_scan*), deeper nesting (an OR of ANDs), more than 16 positive terms,
+ * phrases. */
 int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
                                 const uint32_t* group_off, const uint32_t* query_group_off, size_t n_queries,
                                 const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
@@ -604,9 +605,32 @@ int sdbg_dist_bm25_topk_batch(sdbg_segment* const* segs, size_t n_segs, int kind
    sdbg_dist_match_topk_by_column_batch_groups_min: the device form, one sdbg_dist_allgather, the merge; hit.seg = rank.
    Device scratch: the local entry's, (1 + world) device-form buffers of 64 + n_queries * (8 + 24 k) B (8 ranks, 4096
    queries, k = 1000: 787 MB gathered), n_queries * k * 24 B of merged hits, and as much pinned host memory.
-   Not supported: exclusion / group forms of sdbg_bm25_topk_batch_device and sdbg_dist_bm25_topk_batch (they run on the
-   top-k path with 2^28-ordinal rank slots), the streaming scan across ranks, a sort threshold exchanged between ranks
-   during the scan. */
+   sdbg_bm25_topk_batch_groups_min_device: this rank's result of sdbg_bm25_topk_batch_groups_min (same query and scorer
+   parameters, threshold_in included: flat OR / AND, groups, min-match, exclusions, filter chains, deleted docs; BM25, BM15,
+   BM1 and TFIDF) left in d_buf with no wait: a 64-byte header {k, n_queries, failure word, 5 zero words}, then the keys
+   (u64 [n_queries][k], best first: score bits << 32 | ~ordinal, the ordinal being the docs of the rank's earlier segments
+   plus the doc id, up to 2^32 - 2), total_matches (u64 [n_queries]) and the hit counts (u32 [n_queries]), padded to a multiple of 8 B: 64 +
+   8 * ceil(n_queries * (8k + 12) / 8) B. The counts say how many keys are real: under BM1 every score is 0, so a key's value marks nothing. There is
+   no rank parameter and no rank slot: a rank is its buffer's position in the gathered array, and a rank holds up to
+   2^32 - 2 docs per call, as the local entry. Errors of the call's scalar arguments (NULL offsets or d_buf, k == 0,
+   n_queries == 0: SDBG_EINVAL; k > 8192, n_queries > 65535: SDBG_EUNSUPPORTED) return before anything is queued; any
+   other failure of the local pass returns its code and sets the failure word.
+   sdbg_bm25_topk_merge_gathered: per query the k best hits of n_ranks such buffers back to back (rank order), ordered by
+   (score desc, rank asc, ordinal asc), as sdbg_hit with seg = the rank and doc = the ordinal within the rank; n_out =
+   min(k, hits) and total_matches (NULL: not wanted) the sum of the ranks' totals. With ranks holding consecutive segments
+   in corpus order, the hits are those of the local entry over the unsharded corpus. The lists are re-keyed by position
+   (score bits << 32 | ~(rank * k + index)), selected with the local merge kernel and mapped back, which is exact while
+   n_ranks * k < 2^32 (k = 8192: 2^19 ranks). The headers are read first (one small copy and a wait): headers that
+   disagree (k, n_queries) or any rank's failure word: SDBG_EINVAL with nothing queued. n_ranks == 0, k == 0, n_queries ==
+   0: SDBG_EINVAL; k > 8192, n_queries > 65535, n_ranks * k >= 2^32: SDBG_EUNSUPPORTED. Synchronous on the context's stream.
+   sdbg_dist_bm25_topk_batch_groups_min: the device form, one sdbg_dist_allgather, the merge, with the errors above; hit.seg
+   = rank. Caller's contract, besides the one above: every rank passes the same term statistics (corpus-wide, as
+   dist.global_term_stats computes them), scorer and threshold_in, so that a doc scores the same on every rank. Device
+   scratch: the local entry's, (1 + world) device-form buffers (4096 queries at k = 1000: 33 MB per rank, 262 MB gathered
+   at 8 ranks), the re-keyed lists (about one more gathered buffer), n_queries * k * 8 B of merged keys and n_queries * (12k
+   + 12) B of hits, with as much pinned host memory for the copy back.
+   sdbg_bm25_topk_batch_device and sdbg_dist_bm25_topk_batch keep their flat queries and 2^28-ordinal rank slots.
+   Not supported: the streaming scan across ranks, a score or sort threshold exchanged between ranks during the scan. */
 int sdbg_dist_match_count_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
                                            const uint32_t* group_off, const uint32_t* query_group_off,
                                            const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
@@ -654,6 +678,22 @@ int sdbg_dist_match_aggregate_batch_groups_min(sdbg_segment* const* segs, size_t
                                                uint32_t key_span, uint64_t value_field,
                                                sdbg_match_agg* out /* n_queries * key_span */,
                                                sdbg_match_agg* null_out /* n_queries */);
+int sdbg_bm25_topk_batch_groups_min_device(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                           const uint32_t* group_off, const uint32_t* query_group_off,
+                                           const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                           const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                           float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in,
+                                           void* d_buf /* 64 + 8 * ceil(n_queries * (8 * k + 12) / 8) B */);
+int sdbg_bm25_topk_merge_gathered(sdbg_ctx*, const void* d_all /* n_ranks device-form buffers */, uint32_t n_ranks,
+                                  size_t n_queries, uint32_t k, sdbg_hit* out /* n_queries * k */,
+                                  uint32_t* n_out /* n_queries */, uint64_t* total_matches /* n_queries, or NULL */);
+int sdbg_dist_bm25_topk_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                         const uint32_t* group_off, const uint32_t* query_group_off,
+                                         const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                         const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                         float k1, float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in,
+                                         sdbg_hit* out /* n_queries * k */, uint32_t* n_out /* n_queries */,
+                                         uint64_t* total_matches /* n_queries, or NULL */);
 
 #ifdef __cplusplus
 }

@@ -135,6 +135,11 @@ SIGNATURES = {
     "sdbg_match_topk_by_column_merge_gathered": (C.c_int, [_vp, _vp, C.c_uint32, _sz, C.c_uint32, _vp, _vp]),
     "sdbg_dist_match_topk_by_column_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
                                                                   C.c_int, C.c_int, C.c_uint32, _vp, _vp]),
+    "sdbg_bm25_topk_batch_groups_min_device": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, C.c_float, C.c_float, _vp,
+                                                         C.c_uint32, C.c_float, _vp]),
+    "sdbg_bm25_topk_merge_gathered": (C.c_int, [_vp, _vp, C.c_uint32, _sz, C.c_uint32, _vp, _vp, _vp]),
+    "sdbg_dist_bm25_topk_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, C.c_float, C.c_float, _vp,
+                                                       C.c_uint32, C.c_float, _vp, _vp, _vp]),
     "sdbg_topk_merge_gathered": (C.c_int, [_vp, _vp, C.c_uint32, _sz, C.c_uint32, _vp, _vp]),
     "sdbg_decode_score_term": (C.c_int, [_vp, C.c_uint32, C.c_float, C.c_float, C.c_float, _vp, _vp, _vp]),
     "sdbg_col_pred_resolve": (C.c_int, [C.POINTER(ColPred), C.c_int, C.POINTER(ColPred)]),

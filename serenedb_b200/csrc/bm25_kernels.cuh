@@ -1089,4 +1089,65 @@ topk_merge_kernel(const MergeParams P) {
   if (tid == 0) P.n_out[q] = s_real;
 }
 
+// ---- the BM25 top-k across ranks ----
+// A rank's buffer (sdbg_bm25_topk_batch_groups_min_device): this header, then the region the local entries fill, keys
+// [nq][k] (score bits << 32 | ~ordinal within the rank, best first) | total_matches u64 [nq] | hit counts u32 [nq], padded
+// to a multiple of 8 bytes so that every rank's keys stay 8-byte aligned in the gathered array.
+struct TopkDistHeader {
+  unsigned long long k, nq;
+  unsigned long long failed;   // non-zero: this rank's local pass failed
+  unsigned long long pad[5];
+};
+static_assert(sizeof(TopkDistHeader) == 64, "the keys stay 8-byte aligned");
+
+__host__ __device__ __forceinline__ size_t topk_dist_bytes(size_t nq, uint32_t k) {
+  return sizeof(TopkDistHeader) + ((nq * (size_t(k) * 8 + 12) + 7) & ~size_t(7));
+}
+
+// Rank and ordinal do not fit in 32 bits together, so the merge orders by position instead: list (q, r) of the gathered
+// buffers becomes row q * n_ranks + r of `keys`, key i of it score_bits << 32 | ~(r * k + i). Within a rank the keys are
+// sorted by (score desc, ordinal asc), so the positional keys order by (score desc, rank asc, ordinal asc) and are never
+// zero while n_ranks * k < 2^32. cand_n[row] = the list's hit count (at most k).
+__global__ void __launch_bounds__(256) topk_rekey_gathered_kernel(const char* __restrict__ all, size_t rank_bytes, uint32_t n_ranks,
+                                                                  uint32_t nq, uint32_t k, unsigned long long* __restrict__ keys,
+                                                                  uint32_t* __restrict__ cand_n) {
+  const size_t rows = size_t(nq) * n_ranks;
+  for (size_t row = blockIdx.x; row < rows; row += gridDim.x) {
+    const uint32_t q = uint32_t(row / n_ranks), r = uint32_t(row - size_t(q) * n_ranks);
+    const char* b = all + r * rank_bytes + sizeof(TopkDistHeader);
+    const auto* src = reinterpret_cast<const unsigned long long*>(b) + size_t(q) * k;
+    const uint32_t n = min(reinterpret_cast<const uint32_t*>(b + size_t(nq) * (size_t(k) * 8 + 8))[q], k);
+    unsigned long long* dst = keys + row * k;
+    const uint32_t pos0 = r * k;
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
+      dst[i] = (src[i] & 0xFFFFFFFF00000000ull) | static_cast<unsigned long long>(~(pos0 + i));
+    if (threadIdx.x == 0) cand_n[row] = n;
+  }
+}
+
+// One CTA per query: the merged positional keys back to hits {score, ordinal within the rank, rank} (the layout of
+// sdbg_hit), and the query's total_matches summed over the ranks.
+__global__ void __launch_bounds__(256) topk_hits_gathered_kernel(const char* __restrict__ all, size_t rank_bytes, uint32_t n_ranks,
+                                                                 uint32_t nq, uint32_t k, const unsigned long long* __restrict__ merged,
+                                                                 const uint32_t* __restrict__ n_out, uint3* __restrict__ hits,
+                                                                 unsigned long long* __restrict__ totals) {
+  __shared__ unsigned long long s_total;
+  const uint32_t q = blockIdx.x;
+  if (threadIdx.x == 0) s_total = 0ull;
+  __syncthreads();
+  const uint32_t n = n_out[q];
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const unsigned long long key = merged[size_t(q) * k + i];
+    const uint32_t pos = ~uint32_t(key), r = pos / k, j = pos - r * k;
+    const auto* src = reinterpret_cast<const unsigned long long*>(all + r * rank_bytes + sizeof(TopkDistHeader));
+    hits[size_t(q) * k + i] = make_uint3(uint32_t(key >> 32), ~uint32_t(src[size_t(q) * k + j]), r);
+  }
+  unsigned long long t = 0;
+  for (uint32_t r = threadIdx.x; r < n_ranks; r += blockDim.x)
+    t += reinterpret_cast<const unsigned long long*>(all + r * rank_bytes + sizeof(TopkDistHeader) + size_t(nq) * k * 8)[q];
+  if (t) atomicAdd(&s_total, t);
+  __syncthreads();
+  if (threadIdx.x == 0) totals[q] = s_total;
+}
+
 }  // namespace sdbg

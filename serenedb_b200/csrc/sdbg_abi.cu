@@ -1917,30 +1917,37 @@ int topk_to_host(sdbg_ctx* c, const TopkDevOut& d, size_t nq, uint32_t k, Decode
   return SDBG_OK;
 }
 
-// The host top-k entries after topk_args and their batch (B): runs it into the call's region in c->pass[0], [keys
-// [nq][k] | total [nq] | n_out [nq]] (topk_run for a whole batch, else shape by shape through shapes_run), and copies
-// it back (topk_to_host) with each ordinal decoded into {segment, doc}.
+// The top-k entries' region at d: [keys [nq][k] | total [nq] | n_out [nq]], nq * (8k + 12) bytes.
+TopkDevOut topk_region(void* d, size_t nq, uint32_t k) {
+  char* p = static_cast<char*>(d);
+  const size_t kb = nq * size_t(k) * 8;
+  return {reinterpret_cast<unsigned long long*>(p), reinterpret_cast<uint32_t*>(p + kb + nq * 8),
+          reinterpret_cast<unsigned long long*>(p + kb)};
+}
+
+// Queues a batch that passed topk_args and topk_checked into the region dev: topk_run for a whole batch, else shape by
+// shape through shapes_run. Nothing waits.
+int topk_batch_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_bm25_term>& B, float k1, float b,
+                   const sdbg_col_pred* filt, uint32_t k, float threshold_in, const TopkDevOut& dev) {
+  if (B.whole.nq) return topk_run(segs, n_segs, B.whole, B.total_excl, k1, b, filt, k, threshold_in, dev);
+  return shapes_run(segs[0]->ctx, B.S, {size_t(k) * 8, 8, 4}, {dev.keys, dev.total, dev.n_out}, [&](int sh, void* const* part) {
+    const TopkDevOut o{static_cast<unsigned long long*>(part[0]), static_cast<uint32_t*>(part[2]),
+                       static_cast<unsigned long long*>(part[1])};
+    return topk_run(segs, n_segs, B.S.view(sh), B.S.total_excl[sh], k1, b, filt, k, threshold_in, o);
+  });
+}
+
+// The host top-k entries after topk_args and their batch (B): runs it into the call's region in c->pass[0]
+// (topk_region, topk_batch_run), and copies it back (topk_to_host) with each ordinal decoded into {segment, doc}.
 int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_bm25_term>& B, float k1, float b,
                     const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
                     uint64_t* total_matches) {
   if (int rc = topk_checked(segs, n_segs, B)) return rc;
   sdbg_ctx* c = segs[0]->ctx;
-  const size_t nq = B.nq, kb = nq * size_t(k) * 8;
-  if (int rc = ensure(c, c->pass[0], kb + nq * 12)) return rc;
-  char* d = static_cast<char*>(c->pass[0].p);
-  const TopkDevOut dev{reinterpret_cast<unsigned long long*>(d), reinterpret_cast<uint32_t*>(d + kb + nq * 8),
-                       reinterpret_cast<unsigned long long*>(d + kb)};
-  int rc;
-  if (B.whole.nq) {
-    rc = topk_run(segs, n_segs, B.whole, B.total_excl, k1, b, filt, k, threshold_in, dev);
-  } else {
-    rc = shapes_run(c, B.S, {size_t(k) * 8, 8, 4}, {dev.keys, dev.total, dev.n_out}, [&](int sh, void* const* part) {
-      const TopkDevOut o{static_cast<unsigned long long*>(part[0]), static_cast<uint32_t*>(part[2]),
-                         static_cast<unsigned long long*>(part[1])};
-      return topk_run(segs, n_segs, B.S.view(sh), B.S.total_excl[sh], k1, b, filt, k, threshold_in, o);
-    });
-  }
-  if (rc) return rc;
+  const size_t nq = B.nq;
+  if (int rc = ensure(c, c->pass[0], nq * (size_t(k) * 8 + 12))) return rc;
+  const TopkDevOut dev = topk_region(c->pass[0].p, nq, k);
+  if (int rc = topk_batch_run(segs, n_segs, B, k1, b, filt, k, threshold_in, dev)) return rc;
   std::vector<uint64_t> bases(n_segs);   // the first ordinal of each segment
   uint64_t ord0 = 0;
   for (size_t si = 0; si < n_segs; ++si) { bases[si] = ord0; ord0 += segs[si]->n_docs; }
@@ -3294,6 +3301,107 @@ extern "C" int sdbg_topk_merge_gathered(sdbg_ctx* c, const void* d_keys_all, uin
   // an ordinal is its rank's slot (ordinal >> 28) and the ordinal within the rank (segment base + doc)
   return topk_to_host(c, {M.keys_out, M.n_out, nullptr}, nq, k,
                       [](uint32_t ordinal) { return make_uint2(ordinal >> 28, ordinal & ((1u << 28) - 1)); }, out, n_out, nullptr);
+}
+
+// ---- the BM25 top-k of group queries across GPUs: no rank slots (TopkDistHeader, bm25_kernels.cuh) ----
+extern "C" int sdbg_bm25_topk_batch_groups_min_device(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                                      const uint32_t* group_off, const uint32_t* query_group_off,
+                                                      const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                      const uint32_t* excl_off, float k1, float b, const sdbg_col_pred* filt,
+                                                      uint32_t k, float threshold_in, void* d_buf) {
+  if (!group_off || !query_group_off || !d_buf) return SDBG_EINVAL;
+  if (int rc = topk_args(segs, n_segs, nq, k)) return rc;
+  sdbg_ctx* c = segs[0]->ctx;
+  const PassBatch<sdbg_bm25_term> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  const TopkDistHeader h{k, nq, 0, {}};
+  CU(c, cudaMemsetAsync(d_buf, 0, topk_dist_bytes(nq, k), c->stream));
+  CU(c, cudaMemcpyAsync(d_buf, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
+  int rc = topk_checked(segs, n_segs, B);
+  if (!rc) rc = topk_batch_run(segs, n_segs, B, k1, b, filt, k, threshold_in,
+                               topk_region(static_cast<char*>(d_buf) + sizeof(TopkDistHeader), nq, k));
+  if (rc) CU(c, cudaMemsetAsync(static_cast<char*>(d_buf) + offsetof(TopkDistHeader, failed), 1, 1, c->stream));
+  return rc;
+}
+
+// Checks the n_ranks headers on the host (one small copy and a wait) so that a bad gather queues no kernel, then re-keys
+// the lists by position (topk_rekey_gathered_kernel), selects each query's k best with topk_merge_kernel and maps them back
+// to hits (topk_hits_gathered_kernel); one copy back of [totals | hits | n_out] through the pinned staging.
+extern "C" int sdbg_bm25_topk_merge_gathered(sdbg_ctx* c, const void* d_all, uint32_t n_ranks, size_t nq, uint32_t k,
+                                             sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
+  if (!c || !d_all || !n_ranks || !nq || !k || !out || !n_out) return SDBG_EINVAL;
+  if (int rc = topk_limits(c, nq, k)) return rc;
+  if (uint64_t(n_ranks) * k >= (1ull << 32)) return fail(c, SDBG_EUNSUPPORTED, "n_ranks * k >= 2^32");
+  CU(c, cudaSetDevice(c->device));
+  static_assert(sizeof(sdbg_hit) == sizeof(uint3), "topk_hits_gathered_kernel writes sdbg_hit as uint3");
+  const size_t rank_bytes = topk_dist_bytes(nq, k), hits_bytes = nq * size_t(k) * sizeof(sdbg_hit);
+  const size_t out_bytes = nq * 8 + hits_bytes + nq * 4;
+  if (int rc = ensure_pinned(c, std::max(size_t(n_ranks) * sizeof(TopkDistHeader), out_bytes))) return rc;
+  CU(c, cudaMemcpy2DAsync(c->h_pinned, sizeof(TopkDistHeader), d_all, rank_bytes, sizeof(TopkDistHeader), n_ranks,
+                          cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  const auto* hdr = static_cast<const TopkDistHeader*>(c->h_pinned);
+  for (uint32_t r = 0; r < n_ranks; ++r) {
+    if (hdr[r].k != k || hdr[r].nq != nq) return fail(c, SDBG_EINVAL, "the ranks' top-k headers disagree (k or n_queries)");
+    if (hdr[r].failed) return fail(c, SDBG_EINVAL, "the top-k pass failed on a rank");
+  }
+  const size_t rows = nq * n_ranks;
+  DevBuf& b_in = c->scratch[6]; DevBuf& b_keys = c->scratch[7];
+  int rc;
+  if ((rc = ensure(c, b_in, rows * size_t(k) * 8 + rows * 4))) return rc;
+  if ((rc = ensure(c, b_keys, nq * size_t(k) * 8))) return rc;
+  if ((rc = ensure(c, c->pass[3], out_bytes))) return rc;
+  if ((rc = topk_smem_attrs(c))) return rc;
+  auto* pos_keys = static_cast<unsigned long long*>(b_in.p);
+  auto* cand_n = reinterpret_cast<uint32_t*>(pos_keys + rows * k);
+  char* m = static_cast<char*>(c->pass[3].p);   // [totals u64 [nq] | hits [nq][k] | n_out u32 [nq]]
+  auto* d_totals = reinterpret_cast<unsigned long long*>(m);
+  auto* d_hits = reinterpret_cast<uint3*>(m + nq * 8);
+  auto* d_n_out = reinterpret_cast<uint32_t*>(m + nq * 8 + hits_bytes);
+  const char* all = static_cast<const char*>(d_all);
+  const unsigned grid = unsigned(std::min<size_t>(rows, size_t(c->sm_count) * 16));
+  topk_rekey_gathered_kernel<<<grid, 256, 0, c->stream>>>(all, rank_bytes, n_ranks, uint32_t(nq), k, pos_keys, cand_n);
+  ++c->launches;
+  const uint32_t cap = std::max(next_pow2(k + 1024), 4096u);   // as sdbg_topk_merge_gathered
+  MergeParams M;
+  M.cand = pos_keys; M.cand_n = cand_n; M.list_off = nullptr;
+  M.G = n_ranks; M.stride = k; M.k = k; M.cap = cap;
+  M.keys_out = static_cast<unsigned long long*>(b_keys.p); M.n_out = d_n_out;
+  topk_merge_kernel<<<unsigned(nq), kTopkThreads, size_t(cap) * 8, c->stream>>>(M);
+  ++c->launches;
+  topk_hits_gathered_kernel<<<unsigned(nq), 256, 0, c->stream>>>(all, rank_bytes, n_ranks, uint32_t(nq), k, M.keys_out, d_n_out,
+                                                                 d_hits, d_totals);
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  CU(c, cudaMemcpyAsync(c->h_pinned, m, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  const char* h = static_cast<const char*>(c->h_pinned);
+  std::memcpy(n_out, h + nq * 8 + hits_bytes, nq * 4);
+  if (total_matches) std::memcpy(total_matches, h, nq * 8);
+  const auto* hits = reinterpret_cast<const sdbg_hit*>(h + nq * 8);
+  for (size_t q = 0; q < nq; ++q) std::memcpy(out + q * k, hits + q * k, n_out[q] * sizeof(sdbg_hit));
+  return SDBG_OK;
+}
+
+extern "C" int sdbg_dist_bm25_topk_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                                    const uint32_t* group_off, const uint32_t* query_group_off,
+                                                    const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                    const uint32_t* excl_off, float k1, float b, const sdbg_col_pred* filt,
+                                                    uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
+                                                    uint64_t* total_matches) {
+  if (int rc = dist_check(segs, n_segs, group_off, query_group_off, nq)) return rc;
+  if (!k || !out || !n_out) return SDBG_EINVAL;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (int rc = topk_limits(c, nq, k)) return rc;
+  const uint32_t world = uint32_t(c->dist_world);
+  if (uint64_t(world) * k >= (1ull << 32)) return fail(c, SDBG_EUNSUPPORTED, "n_ranks * k >= 2^32");
+  const size_t bytes = topk_dist_bytes(nq, k);
+  if (int rc = ensure(c, c->pass[0], bytes)) return rc;
+  if (int rc = ensure(c, c->pass[1], bytes * world)) return rc;
+  const int rc_local = sdbg_bm25_topk_batch_groups_min_device(segs, n_segs, terms, group_off, query_group_off, group_min, nq,
+                                                              excl_terms, excl_off, k1, b, filt, k, threshold_in, c->pass[0].p);
+  if (int rc = sdbg_dist_allgather(c, c->pass[0].p, c->pass[1].p, bytes)) return rc_local ? rc_local : rc;
+  const int rc = sdbg_bm25_topk_merge_gathered(c, c->pass[1].p, world, nq, k, out, n_out, total_matches);
+  return rc_local ? rc_local : rc;
 }
 
 extern "C" int sdbg_decode_score_term(sdbg_segment* s, uint32_t term, float c0, float nc, float nl, uint32_t* docs,

@@ -1005,6 +1005,49 @@ def merge_topk_by_column_gathered(ctx, d_all_ptr, n_ranks, nq, k, value_type):
     return _sort_result(hits, n_out, int(nq), int(k), _SORT_VALUE_DTYPE[value_type])
 
 
+def ExecuteDistTopKGroupsBatch(reader, queries, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, min_match=None):
+    """ExecuteTopKGroupsBatch over the segments of every rank (sdbg_dist_bm25_topk_batch_groups_min): each rank's k best
+    keys are all-gathered and merged on the device. Every rank passes the same queries, scorer, k and threshold, and a
+    reader whose statistics are corpus-wide (dist.global_term_stats). Returns (hits [Q, k], n_out [Q], total_matches [Q]),
+    with seg = the rank and doc = the ordinal within the rank (its earlier segments' docs plus the doc id); the same on
+    every rank."""
+    args = _query_args(queries, exclude, min_match, groups=True, stats=lambda t: reader.stats(scorer, t))
+    nq = len(queries)
+    hits = np.zeros((max(nq, 1), max(int(k), 1)), HIT_DTYPE)
+    n_out = np.zeros(max(nq, 1), np.uint32)
+    total = np.zeros(max(nq, 1), np.uint64)
+    N.check(N.lib().sdbg_dist_bm25_topk_batch_groups_min(_seg_array(reader.segments), len(reader.segments), *args, scorer.k,
+                                                         scorer.b, _ref(filt), int(k), float(threshold), _ptr(hits),
+                                                         _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
+    return hits[:nq], n_out[:nq], total[:nq]
+
+
+def topk_groups_device_bytes(nq, k):
+    """Bytes of one rank's buffer of TopKGroupsDevice: a 64-byte header, then nq * k keys of 8 bytes, nq totals of 8 and
+    nq hit counts of 4, padded to a multiple of 8 bytes."""
+    return 64 + (int(nq) * (8 * int(k) + 12) + 7) // 8 * 8
+
+
+def TopKGroupsDevice(reader, queries, scorer, k, d_buf_ptr, filt=None, threshold=FLT_MIN, exclude=None, min_match=None):
+    """This rank's top-k keys, totals and hit counts left in HBM at d_buf_ptr (topk_groups_device_bytes), for an all-gather
+    and merge_topk_groups_gathered (sdbg_bm25_topk_batch_groups_min_device). Nothing waits."""
+    N.check(N.lib().sdbg_bm25_topk_batch_groups_min_device(
+        _seg_array(reader.segments), len(reader.segments),
+        *_query_args(queries, exclude, min_match, groups=True, stats=lambda t: reader.stats(scorer, t)), scorer.k, scorer.b,
+        _ref(filt), int(k), float(threshold), C.c_void_p(int(d_buf_ptr))), reader.segments[0].ctx._h)
+
+
+def merge_topk_groups_gathered(ctx, d_all_ptr, n_ranks, nq, k):
+    """The top-k of n_ranks ranks' TopKGroupsDevice buffers, back to back in HBM (sdbg_bm25_topk_merge_gathered). Returns
+    (hits [nq, k], n_out [nq], total_matches [nq]) as ExecuteDistTopKGroupsBatch does."""
+    hits = np.zeros((max(int(nq), 1), max(int(k), 1)), HIT_DTYPE)
+    n_out = np.zeros(max(int(nq), 1), np.uint32)
+    total = np.zeros(max(int(nq), 1), np.uint64)
+    N.check(N.lib().sdbg_bm25_topk_merge_gathered(ctx._h, C.c_void_p(int(d_all_ptr)), int(n_ranks), int(nq), int(k), _ptr(hits),
+                                                  _ptr(n_out), _ptr(total)), ctx._h)
+    return hits[:int(nq)], n_out[:int(nq)], total[:int(nq)]
+
+
 FOR_BLOCK_DTYPE =np.dtype([("base", "<i8"), ("bits", "<u4"), ("off8", "<u4")])
 
 
