@@ -331,8 +331,8 @@ int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int 
  * Memory: as sdbg_bm25_topk_batch; a batch whose queries take several of the shapes above also holds its per-shape rows
  * in HBM (n_queries * (8k + 12) B) before they go to query order on the device.
  * The top-k of group queries across GPUs: sdbg_dist_bm25_topk_batch_groups_min below.
- * Not supported yet: the streaming scan (sdbg_bm25_scan*), deeper nesting (an OR of ANDs), more than 16 positive terms,
- * phrases. */
+ * The streaming scan of group queries, batched over segments: sdbg_match_scan_batch_groups_min below.
+ * Not supported yet: deeper nesting (an OR of ANDs), more than 16 positive terms, phrases. */
 int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
                                 const uint32_t* group_off, const uint32_t* query_group_off, size_t n_queries,
                                 const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
@@ -430,6 +430,35 @@ int sdbg_match_aggregate_batch_groups_min(sdbg_segment* const* segs, size_t n_se
                                           const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
                                           uint64_t value_field, sdbg_match_agg* out /* n_queries * key_span */,
                                           sdbg_match_agg* null_out /* n_queries */);
+/* Match scan (the Stream mode of the search scan: SELECT id [, bm25(...)] ... WHERE body @@ '...' [LIMIT n OFFSET o]
+ * without ORDER BY): per query, its matches themselves, a page at a time. The query parameters are those of
+ * sdbg_match_count_batch_groups_min (a flat OR is one group, a flat AND single-term groups); terms are sdbg_bm25_term.
+ * Which docs: exactly the docs sdbg_match_count_batch_groups_min counts for the query, with the same normalisation and
+ * degenerate shapes. Order: by (segment index in segs ascending, doc ascending).
+ * Output: total[q] is the exact number of matches (that count). out[q * limit ..] holds the matches at ordinals
+ * offset[q] .. offset[q] + limit - 1 of that order (offset NULL: all 0), n_out[q] = min(limit, total[q] - offset[q]),
+ * and 0 when the offset is at or past the end. A hit is {score, doc, seg}: seg indexes segs, doc is segment-local.
+ * Identical at every pruning level: nothing is pruned.
+ * Scores: with scored != 0, a hit's score is bit for bit the score sdbg_bm25_topk_batch_groups_min gives that doc at
+ * pruning level 0: the sum of the query's positive terms whose lists hold the doc, in ascending docs_count order in the
+ * doc's segment (stable), from 0. k1 and b select BM25, BM15 (b = 0), BM1 (k1 = 0) or TFIDF (k1 = -1; b != 0:
+ * normalised) as in the other batch entries; excluded terms never score. With scored == 0 no frequency, norm or scorer
+ * parameter is read (k1, b and the terms' statistics are ignored) and every score is 0.
+ * Errors, all found before anything is queued: those of sdbg_match_count_batch_groups_min; limit == 0, or NULL out, n_out
+ * or total: SDBG_EINVAL; when scored, those of the top-k entries' limits (more than 65535 queries, or more than
+ * 2^32 - 2 docs over the segments: SDBG_EUNSUPPORTED). Synchronous on the context's stream, with one wait per call.
+ * Device scratch: n_queries * (limit * 12 + 12) B for the pages, totals and counts (4096 queries at limit 1000: 49 MB),
+ * 12 B per work item (windows of one query in one segment, at most 2 x SMs per query and segment), and as much pinned
+ * host memory as the pages for the copy back; a batch whose queries take several shapes also holds its per-shape rows in
+ * HBM (the same bytes again) before they go to query order. Split larger batches.
+ * sdbg_bm25_scan / sdbg_bm25_scan_excl stay the per-segment doc-window form with their own limits. */
+int sdbg_match_scan_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                     const uint32_t* group_off, const uint32_t* query_group_off,
+                                     const uint32_t* group_min /* NULL: all 1 */, size_t n_queries,
+                                     const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                     float k1, float b, const sdbg_col_pred* filt,
+                                     const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit, int scored,
+                                     sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

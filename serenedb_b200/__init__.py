@@ -13,7 +13,7 @@ from .engine import ExecuteDistTopKGroupsBatch, TopKGroupsDevice, merge_topk_gro
 from .engine import (AND, OR, BM25, TFIDF, FLT_MIN, Context, ExecuteCount, ExecuteCountBatch, ExecuteCountGroups,
                      ExecuteCountGroupsBatch, ExecuteFacetCounts, ExecuteFacetCountsBatch, ExecuteFacetCountsGroups,
                      ExecuteFacetCountsGroupsBatch, ExecuteMatchAggregates, ExecuteMatchAggregatesBatch,
-                     ExecuteMatchAggregatesGroups, ExecuteMatchAggregatesGroupsBatch, ExecuteTopK, ExecuteTopKBatch, ExecuteTopKByColumn, ExecuteTopKByColumnBatch,
+                     ExecuteMatchAggregatesGroups, ExecuteMatchAggregatesGroupsBatch, ExecuteMatchScanBatch, ExecuteMatchScanGroupsBatch, ExecuteTopK, ExecuteTopKBatch, ExecuteTopKByColumn, ExecuteTopKByColumnBatch,
                      ExecuteTopKByColumnGroups, ExecuteTopKByColumnGroupsBatch, ExecuteTopKGroups, ExecuteTopKGroupsBatch, IndexReader, IResearchScan, PostingsWriter, PreparedBatch, Segment, merge_gathered, pred,
                      resolve_pred, stage_parse_host, sum_i128, StreamScoredDocs, pack_for)
 
@@ -22,7 +22,7 @@ _native.lib()  # fail loudly at import time when the CUDA extension is missing
 __all__ = ["AND", "OR", "BM25", "TFIDF", "FLT_MIN", "Context", "ExecuteCount", "ExecuteCountBatch", "ExecuteCountGroups",
            "ExecuteCountGroupsBatch", "ExecuteFacetCounts", "ExecuteFacetCountsBatch", "ExecuteFacetCountsGroups",
            "ExecuteFacetCountsGroupsBatch", "ExecuteMatchAggregates", "ExecuteMatchAggregatesBatch",
-           "ExecuteMatchAggregatesGroups", "ExecuteMatchAggregatesGroupsBatch", "ExecuteTopK", "ExecuteTopKBatch", "ExecuteTopKByColumn", "ExecuteTopKByColumnBatch",
+           "ExecuteMatchAggregatesGroups", "ExecuteMatchAggregatesGroupsBatch", "ExecuteMatchScanBatch", "ExecuteMatchScanGroupsBatch", "ExecuteTopK", "ExecuteTopKBatch", "ExecuteTopKByColumn", "ExecuteTopKByColumnBatch",
            "ExecuteTopKByColumnGroups", "ExecuteTopKByColumnGroupsBatch", "ExecuteTopKGroups", "ExecuteTopKGroupsBatch", "IndexReader", "IResearchScan", "PostingsWriter", "PreparedBatch", "Segment", "merge_gathered",
            "pred", "resolve_pred", "stage_parse_host", "sum_i128", "StreamScoredDocs", "pack_for",
            "ExecuteDistCountGroupsBatch", "ExecuteDistFacetCountsGroupsBatch", "ExecuteDistMatchAggregatesGroupsBatch",

@@ -118,6 +118,8 @@ SIGNATURES = {
                                                              C.c_int, C.c_int, C.c_uint32, _vp, _vp]),
     "sdbg_match_facet_counts_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
                                                            C.c_int64, C.c_uint32, _vp, _vp]),
+    "sdbg_match_scan_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, C.c_float, C.c_float, _vp,
+                                                   _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
     "sdbg_match_aggregate_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,
                                              C.c_uint32, C.c_uint64, _vp, _vp]),
     "sdbg_match_aggregate_batch_groups_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,

@@ -19,7 +19,8 @@
 // With the chain's zone verdicts (ChainDev::zone), a window whose zones are all dead is skipped before any list is
 // decoded, the docs of dead zones are cleared before any column is read, and docs of pass zones skip the chain.
 // The facet pass (kFacet, bm25_facet.cuh) also counts each remaining bit in its key's shared-memory bin; the aggregate pass
-// (kAgg, bm25_agg.cuh) also adds its value to its key's shared-memory cell.
+// (kAgg, bm25_agg.cuh) also adds its value to its key's shared-memory cell. The match scan (kEmit, bm25_emit.cuh) counts
+// each item's matches, then writes the docs whose ordinal falls in the query's page.
 // A window that no positive list reaches (OR), that the shortest list does not reach (AND) or that no list of the lead
 // group reaches (GROUPS) is never touched: the CTA
 // jumps to the window of the next block's first possible doc, so a sparse query costs in proportion to its blocks.
@@ -27,6 +28,7 @@
 
 #include "bm25_kernels.cuh"
 #include "bm25_agg.cuh"
+#include "bm25_emit.cuh"
 #include "bm25_facet.cuh"
 #include "bm25_sort.cuh"
 
@@ -61,6 +63,7 @@ struct CountParams {
   SortSink sort;                // kSort: the sorted scan's sink (work item .w = its output slot)
   FacetSink facet;              // kFacet: the facet pass's sink
   AggSink agg;                  // kAgg: the aggregate pass's sink
+  EmitSink emit;                // kEmit: the match scan's sink (work item .w = its count and base slot)
 };
 
 __device__ __forceinline__ uint32_t warp_min(uint32_t v) {
@@ -145,14 +148,21 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
 // kAgg: the aggregate pass (bm25_agg.cuh). Besides the popcount, every surviving doc's value is added to its key's cell
 // among the item's P.agg.key.span + 1 cells in dynamic shared memory (ungrouped: to the thread's register cell), flushed
 // to the query's output cells at the end.
+// kEmit: the match scan (bm25_emit.cuh). Pass A (P.emit.base null) writes the item's match count to
+// P.emit.item_n[item.w] instead of adding it to P.counts. Pass B ranks the surviving docs of each window in doc order:
+// each thread takes kCountWords / kCountThreads consecutive words, and a block-wide exclusive scan of their popcounts
+// gives each doc its ordinal, base[item.w] plus the matches of the item's earlier windows; the docs whose ordinal lies in
+// [offset[q], offset[q] + limit) go to their row of P.emit.out, unscored. An item whose ordinals miss the page exits
+// before it decodes anything, and an item stops after the window that fills the page.
 // The sinks take kGroups queries: the groups narrow `acc` before the sink reads the column, and the bit-sliced counter
 // planes follow the sink's region of dynamic shared memory (16 * cap B, 4 * span B or agg_cells_bytes(span), rounded up
 // to 16 B).
-template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false, bool kAgg = false>
+template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false, bool kAgg = false, bool kEmit = false>
 __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
   static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
   static_assert(!(kFacet && kSort), "the facet pass has its own sink");
   static_assert(!(kAgg && (kSort || kFacet)), "the aggregate pass has its own sink");
+  static_assert(!(kEmit && (kSort || kFacet || kAgg)), "the match scan has its own sink");
   __shared__ uint32_t acc[kCountWords];
   __shared__ uint32_t tmp[kAnd || kGroups ? kCountWords : 1];
   __shared__ uint32_t stage[kCountWarps][128];
@@ -189,6 +199,16 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   const uint32_t n_lead = kGroups ? (gend0 & 0xFFu) - (gend0 >> 8) : kAnd ? 1u : n_pos;
   const uint4* const B = P.seg.blocks;
   const uint32_t del_words = (P.seg.n_docs >> 5) + 2u;   // (n_docs + 32) / 32 + 1, the host bitmap's words, without wrapping
+  // kEmit pass B: the ordinal of the item's next match and the end of the query's page
+  unsigned long long e_run = 0, e_end = 0;
+  if constexpr (kEmit) {
+    if (P.emit.base) {
+      const unsigned long long b = P.emit.base[item.w], n = P.emit.item_n[item.w], off = P.emit.offset[q];
+      e_run = b;
+      e_end = off + P.emit.limit;
+      if (b + n <= off || b >= e_end) return;   // the whole block: nothing has been read or synchronised yet
+    }
+  }
 
   if (tid < n_lists) {
     const uint2 l = tid < n_pos ? P.lists[P.term_off[q] + tid] : P.lists[P.n_pos + P.excl_off[q] + (tid - n_pos)];
@@ -377,7 +397,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       run_lists(n_pos, n_lists, acc, true, true);
       __syncthreads();
     }
-    if (live && !kSort) {
+    if (live && !kSort && !(kEmit && P.emit.base)) {
       const uint32_t wbase = ws >> 5;
       for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
         uint32_t v = acc[i];
@@ -390,6 +410,35 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
           for (uint32_t r = v; r; r &= r - 1u) oor |= agg_add(P.agg, ws + 32u * i + (__ffs(r) - 1u), cells, mine);
         }
         count += __popc(v);
+      }
+    }
+    if constexpr (kEmit) {
+      if (live && P.emit.base) {
+        constexpr uint32_t kRun = kCountWords / kCountThreads;
+        const uint32_t wbase = ws >> 5, i0 = tid * kRun;
+        uint32_t v[kRun], n = 0;
+#pragma unroll
+        for (uint32_t j = 0; j < kRun; ++j) {
+          uint32_t x = acc[i0 + j];
+          if (x && P.seg.deleted && wbase + i0 + j < del_words) x &= ~__ldg(P.seg.deleted + wbase + i0 + j);
+          v[j] = chain_bits(x, i0 + j);
+          n += __popc(v[j]);
+        }
+        const uint32_t incl = warp_incl_scan(n, lane);
+        if (lane == 31u) s_sum[warp] = incl;   // s_sum is free until the end of the kernel
+        __syncthreads();
+        unsigned long long before = 0, all = 0;
+        for (uint32_t w = 0; w < kCountWarps; ++w) { before += w < warp ? s_sum[w] : 0ull; all += s_sum[w]; }
+        unsigned long long r = e_run + before + (incl - n);   // ordinal of this thread's first doc
+        const unsigned long long off = P.emit.offset[q];
+        if (r < e_end && r + n > off) {
+          EmitHit* out = P.emit.out + size_t(q) * P.emit.limit;
+#pragma unroll
+          for (uint32_t j = 0; j < kRun; ++j)
+            for (uint32_t x = v[j]; x && r < e_end; x &= x - 1u, ++r)
+              if (r >= off) out[r - off] = EmitHit{0.f, ws + 32u * (i0 + j) + uint32_t(__ffs(x) - 1), P.emit.seg};
+        }
+        e_run += all;
       }
     }
     if constexpr (kSort) {
@@ -420,7 +469,10 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       }
     }
     }   // !skip
-    __syncthreads();   // acc / tmp / cursors are rewritten by the next window
+    __syncthreads();   // acc / tmp / cursors (kEmit: s_sum) are rewritten by the next window
+    if constexpr (kEmit) {
+      if (P.emit.base && e_run >= e_end) return;   // the page is full
+    }
     if (wlast == 0xFFFFFFFFu || (wlast >> kCountWindowLog) + 1u >= w_end) break;
     ws = wlast + 1u;
   }
@@ -460,13 +512,17 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
     }
     if (oor) *P.agg.out_of_range = 1u;
   }
+  if constexpr (kEmit) {
+    if (P.emit.base) return;
+  }
   count = warp_sum64(count);
   if (lane == 0) s_sum[warp] = count;
   __syncthreads();
   if (tid == 0) {
     unsigned long long s = 0;
     for (uint32_t w = 0; w < kCountWarps; ++w) s += s_sum[w];
-    if (s) atomicAdd(P.counts + q, s);
+    if constexpr (kEmit) P.emit.item_n[item.w] = uint32_t(s);   // an item's docs lie in one segment: fewer than 2^32
+    else if (s) atomicAdd(P.counts + q, s);
   }
 }
 

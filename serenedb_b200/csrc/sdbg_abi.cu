@@ -1509,6 +1509,20 @@ int topk_checked(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_
   return SDBG_OK;
 }
 
+// Each query's terms over each segment as QTermDev, dst[segment][term], by ascending docs_count in that segment (stable,
+// conjunction.hpp:520-523): the order in which the top-k kernels sum a doc's term scores.
+void qterms_by_cost(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm25_term>& Q, float k1, float b, QTermDev* qt) {
+  const size_t nq = Q.nq, n_terms = Q.term_off[nq];
+  for (size_t si = 0; si < n_segs; ++si) {
+    QTermDev* dst = qt + si * n_terms;
+    for (size_t q = 0; q < nq; ++q) {
+      const uint32_t t_begin = Q.term_off[q], t_end = Q.term_off[q + 1];
+      for (uint32_t i = t_begin; i < t_end; ++i) fill_qterm(segs[si], Q.terms[i], k1, b, dst[i]);
+      std::stable_sort(dst + t_begin, dst + t_end, [](const QTermDev& x, const QTermDev& y) { return x.docs_count < y.docs_count; });
+    }
+  }
+}
+
 // The descriptor block of the top-k kernels (TopkParams, MergeParams::list_off), staged in pageable memory for one copy:
 // [QTermDev [segment][term_off[nq]], each query's terms by ascending docs_count (conjunction.hpp:520-523) | term_off
 // [nq + 1] | from 16 B on, the work items {query, first doc, docs, candidate list} | list_off [nq + 1] | when some query
@@ -1546,14 +1560,7 @@ TopkDesc topk_desc(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sd
   D.grp_pos = D.chk_off_pos + off_bytes;
   D.h.resize(n_chk ? D.grp_pos + (D.grp ? n_chk : 0) : D.list_pos + off_bytes);
   char* h = D.h.data();
-  for (size_t si = 0; si < n_segs; ++si) {
-    QTermDev* dst = reinterpret_cast<QTermDev*>(h) + si * n_terms;
-    for (size_t q = 0; q < nq; ++q) {
-      const uint32_t t_begin = Q.term_off[q], t_end = Q.term_off[q + 1];
-      for (uint32_t i = t_begin; i < t_end; ++i) fill_qterm(segs[si], Q.terms[i], k1, b, dst[i]);
-      std::stable_sort(dst + t_begin, dst + t_end, [](const QTermDev& x, const QTermDev& y) { return x.docs_count < y.docs_count; });
-    }
-  }
+  qterms_by_cost(segs, n_segs, Q, k1, b, reinterpret_cast<QTermDev*>(h));
   std::memcpy(h + D.off_pos, Q.term_off, off_bytes);
   std::memcpy(h + D.work_pos, work.data(), work.size() * sizeof(uint4));
   std::memcpy(h + D.list_pos, list_off.data(), off_bytes);
@@ -2237,7 +2244,13 @@ uint32_t count_planes(uint32_t max_min) {
 }
 
 using CountKernel = void (*)(CountParams);
-enum class CountMode { count, sort, facet, agg };
+enum class CountMode { count, sort, facet, agg, emit };
+
+// The match scan's part of a count_run call: the page of each query of the plan's batch.
+struct EmitJob {
+  uint32_t limit;
+  const unsigned long long* offset;   // host [nq]: the first ordinal of each query's page
+};
 
 // One pass of count_run: its mode and that mode's parameters. job_prepare checks them and fills the sinks, once per call.
 struct CountJob {
@@ -2245,6 +2258,7 @@ struct CountJob {
   SortJob sort;     // CountMode::sort
   FacetJob facet;   // CountMode::facet
   AggJob agg;       // CountMode::agg
+  EmitJob emit;     // CountMode::emit
 
   // Bytes per query of count_run's per-query arrays {counts, bins, nulls} (CountOut); rank: the sorted scan's rank form.
   std::array<size_t, 3> rows(bool rank) const {
@@ -2252,6 +2266,7 @@ struct CountJob {
       case CountMode::sort: return {rank ? 8u : 4u, size_t(sort.k) * (rank ? sizeof(SortDistRow) : sizeof(SortHitDev)), 0};
       case CountMode::facet: return {8, size_t(facet.span) * 8, 8};
       case CountMode::agg: return {8, size_t(agg.key.span) * sizeof(AggCell), sizeof(AggCell)};
+      case CountMode::emit: return {8, size_t(emit.limit) * sizeof(EmitHit), 4};
       default: return {8, 0, 0};
     }
   }
@@ -2270,10 +2285,10 @@ int job_prepare(sdbg_ctx* c, sdbg_segment* const* segs, size_t n_segs, CountJob&
 // back and nothing waits (the sorted scan's zonemap planning in sort_prepare excepted), so a collective can follow.
 struct CountOut {
   void* counts;                // [nq]: count u64 counts; facet / aggregate u64 scratch; sorted scan u32 n_out (rank < 0) or
-                               // u64 row counts
+                               // u64 row counts; match scan u64 totals
   void* bins;                  // facet u64 [nq][span], aggregate AggCell [nq][span]; sorted scan SortHitDev [nq][k] (rank < 0)
-                               // or SortDistRow [nq][k]
-  void* nulls;                 // facet u64 [nq], aggregate AggCell [nq]
+                               // or SortDistRow [nq][k]; match scan EmitHit [nq][limit]
+  void* nulls;                 // facet u64 [nq], aggregate AggCell [nq]; match scan u32 n_out [nq]
   unsigned int* oor;           // facet / aggregate: set to 1 when a matching doc's key lies outside the range
   unsigned long long* stats;   // sorted scan: windows judged / skipped by the zonemaps
   int64_t rank;                // sorted scan: < 0 hits, else this rank's rows (sort_dist_rows_kernel)
@@ -2335,13 +2350,13 @@ struct CountPlan {
   // The bm25_count_kernel instantiation of this plan's launches in `mode`, with its dynamic shared memory: the mode's
   // own bytes (facet bins, sorted keys, aggregate cells; none for a count), then the counter planes.
   std::pair<CountKernel, size_t> kernel(CountMode mode, size_t mode_bytes) const {
-    static const CountKernel kernels[3][4] = {   // [OR | AND | OR groups][count | sort | facet | agg]
+    static const CountKernel kernels[3][5] = {   // [OR | AND | OR groups][count | sort | facet | agg | emit]
         {bm25_count_kernel<false>, bm25_count_kernel<false, false, true>, bm25_count_kernel<false, false, false, true>,
-         bm25_count_kernel<false, false, false, false, true>},
+         bm25_count_kernel<false, false, false, false, true>, bm25_count_kernel<false, false, false, false, false, true>},
         {bm25_count_kernel<true>, bm25_count_kernel<true, false, true>, bm25_count_kernel<true, false, false, true>,
-         bm25_count_kernel<true, false, false, false, true>},
+         bm25_count_kernel<true, false, false, false, true>, bm25_count_kernel<true, false, false, false, false, true>},
         {bm25_count_kernel<false, true>, bm25_count_kernel<false, true, true>, bm25_count_kernel<false, true, false, true>,
-         bm25_count_kernel<false, true, false, false, true>}};
+         bm25_count_kernel<false, true, false, false, true>, bm25_count_kernel<false, true, false, false, false, true>}};
     const int shape = Q.term_grp ? 2 : Q.kind == SDBG_QUERY_AND ? 1 : 0;
     return {kernels[shape][int(mode)], mode_bytes + size_t(planes) * kCountWords * 4u};
   }
@@ -2494,27 +2509,30 @@ CountPlan count_plan(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<
 // Queues a pass over its plan into out. A count pass first sets out.counts to the single-term shortcut's counts. The
 // sorted scan launches per segment its seed items first (all segments), then the rest, each item writing its k best to
 // its own slot (its index in the work array); then sort_merge_kernel per query, and for a rank sort_dist_rows_kernel.
+// The match scan launches its items twice (bm25_emit.cuh): pass A, emit_bases_kernel over each query's items in
+// (segment, first window) order, pass B.
 // The plan is staged from pageable memory, which the copy has consumed when it returns, so calls can follow one another
 // without a wait (a host group entry queues its shapes back to back).
 int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt, const CountJob& job,
               const CountOut& out) {
   sdbg_ctx* c = segs[0]->ctx;
   const size_t nq = pl.Q.nq, total = pl.items;
-  const bool sort = job.mode == CountMode::sort;
+  const bool sort = job.mode == CountMode::sort, emit = job.mode == CountMode::emit;
   if (std::any_of(pl.host.begin(), pl.host.end(), [](uint64_t v) { return v != 0; }))   // else out.counts is zero already
     CU(c, cudaMemcpyAsync(out.counts, pl.host.data(), nq * 8, cudaMemcpyHostToDevice, c->stream));
   if (!total && !sort) return SDBG_OK;
   const SortJob& J = job.sort;
   const uint32_t k = J.k, cap = sort ? J.sink[0].cap : 0u;
-  // host staging: the plan's, then for the sorted scan [slot_off | slots | segments]
+  // host staging: the plan's, then for the sorted scan [slot_off | slots | segments], for the match scan [slot_off |
+  // slots | offsets]
   const size_t slot_off_pos = pl.staged;
   const size_t slots_pos = slot_off_pos + pl.off_bytes;
   const size_t segs_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
-  const size_t bytes = sort ? segs_pos + n_segs * sizeof(SortSegDev) : pl.staged;
+  const size_t bytes = sort ? segs_pos + n_segs * sizeof(SortSegDev) : emit ? segs_pos + nq * 8 : pl.staged;
   std::vector<char> staging(bytes);
   char* h = staging.data();
   pl.write(h);
-  if (sort) {
+  if (sort || emit) {   // each query's items in work order, i.e. by segment, then first window
     auto* hw = reinterpret_cast<uint4*>(h + pl.work_pos);
     auto* h_slot_off = reinterpret_cast<uint32_t*>(h + slot_off_pos);
     auto* h_slots = reinterpret_cast<uint32_t*>(h + slots_pos);
@@ -2523,6 +2541,9 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
     for (size_t q = 0; q < nq; ++q) h_slot_off[q + 1] += h_slot_off[q];
     std::vector<uint32_t> fillq(h_slot_off, h_slot_off + nq);
     for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
+  }
+  if (emit) std::memcpy(h + segs_pos, job.emit.offset, nq * 8);
+  if (sort) {
     auto* h_segs = reinterpret_cast<SortSegDev*>(h + segs_pos);
     for (size_t si = 0; si < n_segs; ++si) {
       const SortSink& S = J.sink[si];
@@ -2537,6 +2558,8 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
   DevBuf& b_desc = c->scratch[0]; DevBuf& b_out = c->scratch[1];
   if (int rc = ensure(c, b_desc, bytes)) return rc;
   if (int rc = sort ? ensure(c, b_out, out.rank < 0 ? hits_pos : n_out_pos + nq * 4) : SDBG_OK) return rc;
+  // the match scan's device scratch: [item bases u64 | item counts u32]
+  if (int rc = emit ? ensure(c, b_out, total * 12) : SDBG_OK) return rc;
   char* d = static_cast<char*>(b_desc.p);
   char* o = static_cast<char*>(b_out.p);
   auto* thr = reinterpret_cast<unsigned long long*>(o + thr_pos);
@@ -2552,39 +2575,55 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
   CU(c, fit_dynamic_smem(kernel, smem));
   std::vector<ChainDev> chains(n_segs);
   if (int rc = filter_chains(segs, n_segs, filt, chains.data())) return rc;
-  for (int phase = 0; phase < 2; ++phase) {   // seeds (sorted scan only), then the rest
-    size_t begin = 0;
-    for (size_t si = 0; si < n_segs; ++si) {
-      const auto& w = pl.seg_work[si];
-      const size_t n_seed = size_t(std::count_if(w.begin(), w.end(), [](const CountItem& x) { return x.seed; }));
-      const size_t first = begin + (phase ? n_seed : 0), n = phase ? w.size() - n_seed : n_seed;
-      begin += w.size();
-      if (!n) continue;
-      CountParams P;
-      pl.params(d, segs[si], si, first, chains[si], &P);
-      P.counts = static_cast<unsigned long long*>(out.counts);
-      if (sort) {
-        P.counts = nullptr;
-        P.sort = J.sink[si];
-        P.sort.thr = c->wand ? thr : nullptr;
-        P.sort.out = reinterpret_cast<ulonglong2*>(o);
-        P.sort.out_n = reinterpret_cast<uint32_t*>(o + keys_n_pos);
-        P.sort.stats = out.stats;
-      }
-      if (job.mode == CountMode::facet) {
-        P.facet = job.facet.sink[si];
-        P.facet.counts = static_cast<unsigned long long*>(out.bins);
-        P.facet.nulls = static_cast<unsigned long long*>(out.nulls);
-        P.facet.out_of_range = out.oor;
-      }
-      if (job.mode == CountMode::agg) {
-        P.agg = job.agg.sink[si];
-        P.agg.cells = static_cast<AggCell*>(out.bins);
-        P.agg.nulls = static_cast<AggCell*>(out.nulls);
-        P.agg.out_of_range = out.oor;
-      }
-      kernel<<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
+  auto* e_base = reinterpret_cast<unsigned long long*>(o);
+  auto* e_n = reinterpret_cast<uint32_t*>(o + total * 8);
+  const auto* e_off = reinterpret_cast<const unsigned long long*>(d + segs_pos);
+  for (int pass = 0; pass < (emit ? 2 : 1); ++pass) {   // the match scan: pass A, the bases, pass B
+    if (pass) {
+      emit_bases_kernel<<<unsigned(nq), 32, 0, c->stream>>>(e_n, reinterpret_cast<const uint32_t*>(d + slot_off_pos),
+                                                            reinterpret_cast<const uint32_t*>(d + slots_pos), e_off, job.emit.limit,
+                                                            e_base, static_cast<unsigned long long*>(out.counts),
+                                                            static_cast<uint32_t*>(out.nulls));
       ++c->launches;
+    }
+    for (int phase = 0; phase < 2; ++phase) {   // seeds (sorted scan only), then the rest
+      size_t begin = 0;
+      for (size_t si = 0; si < n_segs; ++si) {
+        const auto& w = pl.seg_work[si];
+        const size_t n_seed = size_t(std::count_if(w.begin(), w.end(), [](const CountItem& x) { return x.seed; }));
+        const size_t first = begin + (phase ? n_seed : 0), n = phase ? w.size() - n_seed : n_seed;
+        begin += w.size();
+        if (!n) continue;
+        CountParams P;
+        pl.params(d, segs[si], si, first, chains[si], &P);
+        P.counts = static_cast<unsigned long long*>(out.counts);
+        if (sort) {
+          P.counts = nullptr;
+          P.sort = J.sink[si];
+          P.sort.thr = c->wand ? thr : nullptr;
+          P.sort.out = reinterpret_cast<ulonglong2*>(o);
+          P.sort.out_n = reinterpret_cast<uint32_t*>(o + keys_n_pos);
+          P.sort.stats = out.stats;
+        }
+        if (job.mode == CountMode::facet) {
+          P.facet = job.facet.sink[si];
+          P.facet.counts = static_cast<unsigned long long*>(out.bins);
+          P.facet.nulls = static_cast<unsigned long long*>(out.nulls);
+          P.facet.out_of_range = out.oor;
+        }
+        if (job.mode == CountMode::agg) {
+          P.agg = job.agg.sink[si];
+          P.agg.cells = static_cast<AggCell*>(out.bins);
+          P.agg.nulls = static_cast<AggCell*>(out.nulls);
+          P.agg.out_of_range = out.oor;
+        }
+        if (emit) {
+          P.counts = nullptr;
+          P.emit = EmitSink{e_n, pass ? e_base : nullptr, e_off, static_cast<EmitHit*>(out.bins), job.emit.limit, uint32_t(si)};
+        }
+        kernel<<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
+        ++c->launches;
+      }
     }
   }
   CU(c, cudaGetLastError());
@@ -2838,6 +2877,118 @@ extern "C" int sdbg_match_aggregate_batch_groups_min(sdbg_segment* const* segs, 
   if (int rc = agg_check_range(segs[0]->ctx, key_field, key_min, key_span)) return rc;   // before the rows are sized
   const PassBatch<uint32_t> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out);
+}
+
+// ---- the match scan (Stream mode) ----
+namespace {
+static_assert(sizeof(sdbg_hit) == sizeof(EmitHit), "sdbg_hit layout");
+
+struct ScanArgs {
+  const uint64_t* offset;   // per query of the call (NULL: all 0)
+  uint32_t limit;
+  int scored;
+  float k1, b;
+};
+
+// The match scan's region: [totals u64 [nq] | hits EmitHit [nq][limit] | n_out u32 [nq]].
+PassRegion scan_region(size_t nq, uint32_t limit) {
+  const size_t n_out = nq * 8 + nq * size_t(limit) * sizeof(EmitHit);
+  return {0, nq * 8, n_out, kNone, kNone, n_out + nq * 4};
+}
+
+// Queues the match scan of a batch of one shape (checked; total_excl as check_query_batch set it) into out, zeroed:
+// the emit pass over its count plan, then, when scored, emit_score_kernel over the pages. qpos: the call's position of
+// each query (NULL: the same), which picks its offset.
+int scan_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm25_term>& Q, uint32_t total_excl, const uint32_t* qpos,
+             const sdbg_col_pred* filt, const ScanArgs& A, const CountOut& out) {
+  sdbg_ctx* c = segs[0]->ctx;
+  const size_t nq = Q.nq, n_terms = Q.term_off[nq];
+  std::vector<uint32_t> ids(n_terms);
+  for (size_t i = 0; i < n_terms; ++i) ids[i] = Q.terms[i].term;
+  std::vector<unsigned long long> offs(nq, 0ull);
+  if (A.offset)
+    for (size_t q = 0; q < nq; ++q) offs[q] = A.offset[qpos ? qpos[q] : q];
+  const QueryBatch<uint32_t> Qi{Q.kind, ids.data(), Q.term_off, nq, Q.excl_terms, Q.excl_off, Q.term_grp};
+  CountJob job{CountMode::emit, {}, {}, {}, {A.limit, offs.data()}};
+  if (int rc = count_run(segs, n_segs, count_plan(segs, n_segs, Qi, total_excl, filt, job), filt, job, out)) return rc;
+  if (!A.scored) return SDBG_OK;
+  // the scorer's staging: [PostingsDev [n_segs] | QTermDev [n_segs][n_terms] | qterm_off [nq + 1]]
+  const size_t qt_pos = (n_segs * sizeof(PostingsDev) + 15) & ~size_t(15);
+  const size_t off_pos = qt_pos + n_segs * n_terms * sizeof(QTermDev);
+  std::vector<char> h(off_pos + (nq + 1) * 4);
+  for (size_t si = 0; si < n_segs; ++si) {
+    const PostingsDev p = postings_view(segs[si], 0);
+    std::memcpy(h.data() + si * sizeof(PostingsDev), &p, sizeof(p));
+  }
+  qterms_by_cost(segs, n_segs, Q, A.k1, A.b, reinterpret_cast<QTermDev*>(h.data() + qt_pos));
+  std::memcpy(h.data() + off_pos, Q.term_off, (nq + 1) * 4);
+  DevBuf& b_sc = c->scratch[4];
+  if (int rc = ensure(c, b_sc, h.size())) return rc;
+  CU(c, cudaMemcpyAsync(b_sc.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
+  const char* d = static_cast<const char*>(b_sc.p);
+  EmitScoreParams P;
+  P.segs = reinterpret_cast<const PostingsDev*>(d);
+  P.qterms = reinterpret_cast<const QTermDev*>(d + qt_pos);
+  P.qterm_off = reinterpret_cast<const uint32_t*>(d + off_pos);
+  P.n_terms = uint32_t(n_terms);
+  P.blocks_per_query = (A.limit + kEmitScoreHits - 1) / kEmitScoreHits;
+  P.limit = A.limit;
+  P.out = static_cast<EmitHit*>(out.bins);
+  P.n_out = static_cast<const uint32_t*>(out.nulls);
+  emit_score_kernel<<<unsigned(nq * P.blocks_per_query), kEmitScoreThreads, 0, c->stream>>>(P);
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  return SDBG_OK;
+}
+
+// The match scan of a checked batch B: scan_run for a whole batch, else shape by shape through shapes_run, into the
+// call's region in c->pass[0]; then one copy back through the pinned staging, one wait, and pass_finish.
+int scan_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_bm25_term>& B, const sdbg_col_pred* filt,
+                 const ScanArgs& A, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
+  if (B.rc) return B.rc;
+  sdbg_ctx* c = segs[0]->ctx;
+  CU(c, cudaSetDevice(c->device));
+  const size_t nq = B.nq;
+  const PassRegion L = scan_region(nq, A.limit);
+  if (int rc = ensure(c, c->pass[0], L.bytes)) return rc;
+  if (int rc = ensure_pinned(c, L.bytes)) return rc;
+  const CountOut o = L.at(c->pass[0].p);
+  CU(c, cudaMemsetAsync(c->pass[0].p, 0, L.bytes, c->stream));
+  int rc;
+  if (B.whole.nq) {
+    rc = scan_run(segs, n_segs, B.whole, B.total_excl, nullptr, filt, A, o);
+  } else {
+    const CountJob job{CountMode::emit, {}, {}, {}, {A.limit, nullptr}};
+    rc = shapes_run(c, B.S, job.rows(false), {o.counts, o.bins, o.nulls}, [&](int sh, void* const* part) {
+      return scan_run(segs, n_segs, B.S.view(sh), B.S.total_excl[sh], B.S.qs[sh].data(), filt, A,
+                      CountOut{part[0], part[1], part[2], nullptr, nullptr, -1});
+    });
+  }
+  if (rc) return rc;
+  CU(c, cudaMemcpyAsync(c->h_pinned, c->pass[0].p, L.bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  return pass_finish(c, L, static_cast<const char*>(c->h_pinned), [&](const char* h) {
+    std::memcpy(total, h + L.counts, nq * 8);
+    std::memcpy(out, h + L.bins, nq * size_t(A.limit) * sizeof(sdbg_hit));
+    std::memcpy(n_out, h + L.nulls, nq * 4);
+  });
+}
+}  // namespace
+
+extern "C" int sdbg_match_scan_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
+                                                const uint32_t* group_off, const uint32_t* query_group_off,
+                                                const uint32_t* group_min, size_t nq, const uint32_t* excl_terms,
+                                                const uint32_t* excl_off, float k1, float b, const sdbg_col_pred* filt,
+                                                const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out,
+                                                uint32_t* n_out, uint64_t* total) {
+  if (!segs || !n_segs || !segs[0] || !group_off || !query_group_off || !nq) return SDBG_EINVAL;
+  if (!limit || !out || !n_out || !total) return SDBG_EINVAL;
+  if (scored)
+    if (int rc = topk_limits(segs[0]->ctx, nq, 1)) return rc;
+  const PassBatch<sdbg_bm25_term> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
+  if (scored)
+    if (int rc = topk_checked(segs, n_segs, B)) return rc;
+  return scan_to_host(segs, n_segs, B, filt, {offset, limit, scored, k1, b}, out, n_out, total);
 }
 
 // ---- the count, facet, aggregate and sorted passes across GPUs ----

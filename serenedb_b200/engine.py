@@ -805,6 +805,39 @@ def ExecuteCountGroups(reader, groups, filt=None, exclude=None, min_match=None):
     return int(ExecuteCountGroupsBatch(reader, _one_groups(groups), filt, exclude=_one(exclude), min_match=_one(min_match))[0])
 
 
+def ExecuteMatchScanGroupsBatch(reader, queries, scorer=None, limit=1 << 20, offset=None, filt=None, exclude=None,
+                               min_match=None):
+    """Stream mode of the search scan (`SELECT id [, bm25(...)] ... WHERE body @@ '...' LIMIT n OFFSET o`,
+    sdbg_match_scan_batch_groups_min): per query, the docs ExecuteCountGroupsBatch counts for it, in (segment, doc) order,
+    from ordinal offset[q] (None: 0) on, at most `limit` of them. scorer: BM25 / TFIDF to score each hit exactly as
+    ExecuteTopKGroupsBatch scores it at pruning level 0; None: unscored (every score 0). queries, filt, exclude and
+    min_match as in ExecuteTopKGroupsBatch. Returns per query ((seg u32, doc u32, score f32) arrays, total matches)."""
+    nq = len(queries)
+    if scorer is None:
+        stats = lambda t: N.BM25Term(0.0, 0.0, 0.0, 0.0, int(t))   # noqa: E731  (unscored: only the term id is read)
+    else:
+        stats = lambda t: reader.stats(scorer, t)   # noqa: E731
+    args = _query_args(queries, exclude, min_match, groups=True, stats=stats)
+    offs = None if offset is None else np.ascontiguousarray(offset, dtype=np.uint64)
+    if offs is not None and offs.shape != (nq,):
+        raise ValueError("offset needs one value per query")
+    hits = np.zeros((nq, max(int(limit), 1)), HIT_DTYPE)
+    n_out = np.zeros(nq, np.uint32)
+    total = np.zeros(nq, np.uint64)
+    k1, b = (0.0, 0.0) if scorer is None else (scorer.k, scorer.b)
+    N.check(N.lib().sdbg_match_scan_batch_groups_min(_seg_array(reader.segments), len(reader.segments), *args, k1, b,
+                                                     _ref(filt), _ptr(offs), int(limit), int(scorer is not None), _ptr(hits),
+                                                     _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
+    return [((hits["seg"][q, :n_out[q]].copy(), hits["doc"][q, :n_out[q]].copy(), hits["score"][q, :n_out[q]].copy()),
+             int(total[q])) for q in range(nq)]
+
+
+def ExecuteMatchScanBatch(reader, queries, kind, scorer=None, limit=1 << 20, offset=None, filt=None, exclude=None):
+    """ExecuteMatchScanGroupsBatch for flat queries (lists of term ids): an OR is one group, an AND single-term groups."""
+    groups = [[list(q)] if kind == OR else [[t] for t in q] for q in queries]
+    return ExecuteMatchScanGroupsBatch(reader, groups, scorer, limit, offset, filt, exclude)
+
+
 def ExecuteTopKByColumnGroupsBatch(reader, queries, sort_field, k, descending=False, nulls_first=False, filt=None,
                                    exclude=None, min_match=None):
     """Sorted scan of conjunctions of OR groups (`WHERE body @@ 'a & (b | c)' ORDER BY col LIMIT k`,

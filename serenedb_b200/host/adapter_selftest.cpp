@@ -9,7 +9,8 @@
 // with group queries (tests/test_gpu_groups_column.py). "aggregate" / "aggregate groups" run the aggregates over the matches
 // (GpuMatchAggScan, tests/test_gpu_match_aggregates.py). "chain" runs a pushed filter chain (SDBG_OP_AND_NEXT) through the
 // top-k, streaming and count adapters next to the same calls filtered by an indicator column of the chain
-// (tests/test_gpu_filter_chains.py).
+// (tests/test_gpu_filter_chains.py). "scan" runs the Stream mode (GpuMatchScan) for flat, grouped and min-match queries
+// (tests/test_gpu_match_scan.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -186,6 +187,49 @@ int main(int argc, char** argv) {
       scan.Scan(chunk);
     } catch (const sdbg_host::GpuError& e) { code = e.code; }
     std::printf("{\"min_error\": %d}\n", code);
+    sdbg_segment_destroy(seg);
+    sdbg_destroy(ctx);
+    return 0;
+  }
+  if (argc > 2 && std::string(argv[2]) == "scan") {
+    // the Stream mode (GpuMatchScan): `t2 | t5` scored, `t1 & 2 of (t2 | t5 | t6)` unscored, `t2 & (t5 | t6)` scored; every
+    // row in chunk order
+    struct Case { std::vector<uint32_t> ids, sizes, mins; bool scored; };
+    const Case cases[3] = {{{2, 5}, {2}, {1}, true}, {{1, 2, 5, 6}, {1, 3}, {1, 2}, false}, {{2, 5, 6}, {1, 2}, {1, 1}, true}};
+    for (const Case& cs : cases) {
+      std::vector<sdbg_bm25_term> t(cs.ids.size());
+      for (size_t i = 0; i < t.size(); ++i) { sdbg_bm25_collect(n_docs, sum_dl, dc[cs.ids[i]], 1.2f, 0.75f, &t[i]); t[i].term = cs.ids[i]; }
+      sdbg_host::GpuMatchScan scan({seg}, t, {}, nullptr, 1.2f, 0.75f, cs.scored, cs.sizes, cs.mins);
+      std::vector<uint64_t> chunks;
+      std::vector<uint32_t> docs, segs;
+      std::vector<float> scores;
+      duckdb::DataChunkMock chunk;
+      for (scan.Scan(chunk); chunk.size; scan.Scan(chunk)) {
+        chunks.push_back(chunk.size);
+        docs.insert(docs.end(), chunk.doc.begin(), chunk.doc.end());
+        segs.insert(segs.end(), chunk.segment.begin(), chunk.segment.end());
+        scores.insert(scores.end(), chunk.score.begin(), chunk.score.end());
+      }
+      scan.Scan(chunk);
+      std::printf("{\"groups\": [");
+      for (size_t g = 0, o = 0; g < cs.sizes.size(); o += cs.sizes[g++]) {
+        std::printf("%s[", g ? ", " : "");
+        for (uint32_t i = 0; i < cs.sizes[g]; ++i) std::printf("%s%u", i ? ", " : "", cs.ids[o + i]);
+        std::printf("]");
+      }
+      std::printf("], \"mins\": [");
+      for (size_t g = 0; g < cs.mins.size(); ++g) std::printf("%s%u", g ? ", " : "", cs.mins[g]);
+      std::printf("], \"scored\": %d, \"chunks\": [", cs.scored ? 1 : 0);
+      for (size_t i = 0; i < chunks.size(); ++i) std::printf("%s%llu", i ? ", " : "", static_cast<unsigned long long>(chunks[i]));
+      std::printf("], \"docs\": [");
+      for (size_t i = 0; i < docs.size(); ++i) std::printf("%s%u", i ? ", " : "", docs[i]);
+      std::printf("], \"segs\": [");
+      for (size_t i = 0; i < segs.size(); ++i) std::printf("%s%u", i ? ", " : "", segs[i]);
+      std::printf("], \"scores\": [");
+      for (size_t i = 0; i < scores.size(); ++i) std::printf("%s%.9g", i ? ", " : "", double(scores[i]));
+      std::printf("], \"total\": %llu, \"rows_after\": %llu}\n", static_cast<unsigned long long>(scan.total_matches()),
+                  static_cast<unsigned long long>(chunk.size));
+    }
     sdbg_segment_destroy(seg);
     sdbg_destroy(ctx);
     return 0;

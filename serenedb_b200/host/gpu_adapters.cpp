@@ -284,6 +284,46 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
   cursor_ += take;
 }
 
+GpuMatchScan::GpuMatchScan(std::vector<sdbg_segment*> segments, std::vector<sdbg_bm25_term> terms,
+                           std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, float k1, float b, bool scored,
+                           std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)
+    : segs_(std::move(segments)), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
+      group_sizes_(group_sizes.empty() ? std::vector<uint32_t>{uint32_t(terms_.size())} : std::move(group_sizes)),
+      group_min_(std::move(group_min_match)), filter_(table_filter), k1_(k1), b_(b), scored_(scored) {
+}
+
+void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kPage - 1
+  const std::vector<uint32_t> group_off = group_offsets(group_sizes_, terms_.size());
+  const uint32_t query_group_off[2] = {0, uint32_t(group_sizes_.size())};
+  const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
+  page_.resize(kPage);
+  uint32_t n = 0;
+  const int rc = sdbg_match_scan_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
+                                                  group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(), excl_off,
+                                                  k1_, b_, filter_.data(), &offset_, kPage, scored_ ? 1 : 0, page_.data(), &n,
+                                                  &total_);
+  if (rc != SDBG_OK)
+    throw GpuError(rc, std::string("sdbg_match_scan_batch_groups_min: ") + sdbg_last_error(sdbg_segment_context(segs_[0])));
+  page_.resize(n);
+  offset_ += kPage;
+  cursor_ = 0;
+  ran_ = true;
+}
+
+void GpuMatchScan::Scan(duckdb::DataChunkMock& output) {
+  output.Reset();
+  if (!ran_ || (cursor_ == page_.size() && page_.size() == kPage && offset_ < total_)) Fetch();
+  const size_t take = std::min<size_t>(duckdb::STANDARD_VECTOR_SIZE, page_.size() - cursor_);   // 0: end of scan
+  for (size_t i = 0; i < take; ++i) {
+    const sdbg_hit& h = page_[cursor_ + i];
+    output.doc.push_back(h.doc);
+    output.segment.push_back(h.seg);
+    output.score.push_back(h.score);
+  }
+  output.size = take;
+  cursor_ += take;
+}
+
 GpuFacetScan::GpuFacetScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
                            std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)

@@ -165,6 +165,36 @@ class GpuSortedScan {
   bool ran_ = false;
 };
 
+// SELECT id [, bm25(...)] FROM t WHERE body @@ '<query>' [AND <pushed filter>] [LIMIT n OFFSET o] without ORDER BY -- the
+// body of the Stream scan mode (duckdb_search_full_scan.cpp RunStreamingScan :2370-2403) for flat, grouped and min-match
+// queries over every segment. Pages of kPage matches come from sdbg_match_scan_batch_groups_min (offset += kPage); Scan
+// emits rows (doc, segment, score) of at most STANDARD_VECTOR_SIZE in (segment, doc) order, cardinality 0 at the end.
+// Scores are those of the top-k at pruning level 0 when `scored`, else 0 (no frequency or norm is read).
+class GpuMatchScan {
+ public:
+  static constexpr uint32_t kPage = 1u << 20;
+  GpuMatchScan(std::vector<sdbg_segment*> segments, std::vector<sdbg_bm25_term> terms /* statistics unused when unscored */,
+               std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
+               float k1, float b, bool scored,
+               std::vector<uint32_t> group_sizes = {} /* an And of Ors over `terms`; empty = one group (a flat OR) */,
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
+  void Scan(duckdb::DataChunkMock& output);
+  uint64_t total_matches() const { return total_; }
+
+ private:
+  void Fetch();
+  std::vector<sdbg_segment*> segs_;
+  std::vector<sdbg_bm25_term> terms_;
+  std::vector<uint32_t> excluded_, group_sizes_, group_min_;
+  FilterChain filter_;
+  float k1_, b_;
+  bool scored_;
+  std::vector<sdbg_hit> page_;
+  uint64_t offset_ = 0, total_ = 0;   // ordinal of page_[0]'s successor page; the query's matches
+  size_t cursor_ = 0;
+  bool ran_ = false;
+};
+
 // SELECT col, count(*) FROM t WHERE body @@ '<query>' [AND <pushed filter>] GROUP BY col -- the body of the
 // HASH_GROUP_BY(col; count_star()) <- IRESEARCH_SCAN(text query) plan shape (facet counts). The first Scan takes the key
 // range from sdbg_column_minmax_i64 over the segments and runs one sdbg_match_facet_counts_batch call

@@ -235,11 +235,12 @@ struct DataChunkMock {          // stands in for duckdb::DataChunk with flat vec
   std::vector<uint32_t> segment;//   the double's bits) and validity (0 = NULL)
   std::vector<int64_t> value;
   std::vector<uint8_t> valid;
+  std::vector<float> score;     // match scan: the hit's score (0 when unscored)
   uint64_t size = 0;
   void Reset() {
     key.clear(); count.clear(); sum_lo.clear(); sum_hi.clear(); avg.clear();
     count_value.clear(); sum_f64.clear(); min.clear(); max.clear();
-    doc.clear(); segment.clear(); value.clear(); valid.clear();
+    doc.clear(); segment.clear(); value.clear(); valid.clear(); score.clear();
     size = 0;
   }
 };
