@@ -127,11 +127,11 @@ typedef enum { SDBG_I64 = 0, SDBG_F64 = 1, SDBG_I32 = 2 } sdbg_type;
 int sdbg_stage_column(sdbg_segment*, uint64_t field, sdbg_type t, const void* values,
                       const uint64_t* validity, uint64_t rows);
 /* Same, but `d_values` already lives in device memory (borrowed, not copied, not freed). The library caches statistics
-   of the values (min / max, largest magnitude, zonemap): once the owner's writes to the buffer are complete, it calls this
+   of the values (min / max, zonemap): once the owner's writes to the buffer are complete, it calls this
    again with the same buffer before the next query, which drops them. The values must be complete when this is called. */
 int sdbg_stage_column_device(sdbg_segment*, uint64_t field, sdbg_type t, const void* d_values, uint64_t rows);
 /* Device address of a staged column's raw values, for callers that write them in place. The call means "about to
-   write": it drops the cached statistics of the values (min / max, largest magnitude, zonemap), and a bit-packed column
+   write": it drops the cached statistics of the values (min / max, zonemap), and a bit-packed column
    drops its packed form, so the raw values at this address are the column until it is restaged. Writes go on after the
    context's queued work (sdbg_sync) and must be complete before the next call that reads the column; a caller that writes
    again later calls this again first. */

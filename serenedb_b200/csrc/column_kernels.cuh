@@ -404,12 +404,6 @@ struct TmaGroupByParams {
   // (1..3) words of the slot by tile index when one word would not be enough.
   int32_t pack_shift, pack_tables;
   int64_t pack_bias;
-  // Fixed-point SUM(double) (kFix kernels): a 64-bit floating-point RED costs several integer ones in L2,
-  // so |w| / 2^fix_eunit is truncated to a 2*fix_limb-bit integer and its two limbs are added with integer
-  // REDs into words 2 and 3 of the slot. The host picks fix_eunit from the column's largest magnitude so
-  // that nothing overflows; the sum is exact to 2^-(2*fix_limb) of that magnitude and independent of the
-  // order of the updates. Columns with NaN / infinities keep the floating-point RED.
-  int32_t fix_limb, fix_eunit;
   int64_t key_min;
   uint64_t key_span;
   uint64_t rows;
@@ -434,7 +428,7 @@ constexpr uint32_t kZoneRows = 2048;   // rows per zonemap block = the reference
 __host__ __device__ __forceinline__ long long fkey(long long bits) { return bits ^ ((bits >> 63) & 0x7FFFFFFFFFFFFFFFll); }
 
 // |w| / 2^eunit truncated to an integer below 2^(2*limb), split into two limbs carrying w's sign.
-// Requires |w| < 2^(eunit + 2*limb) and w finite (the host checks both against the column statistics).
+// Requires |w| < 2^(eunit + 2*limb) and w finite (the caller checks both).
 __device__ __forceinline__ void fix_limbs(double w, int limb, int eunit, long long& l0, long long& l1) {
   const long long bits = __double_as_longlong(w);
   const int ex = int((bits >> 52) & 0x7FF);
@@ -502,16 +496,18 @@ __device__ __forceinline__ uint32_t range2_for(const unsigned char* col, uint32_
   return (static_cast<unsigned long long>(v[0] - lo) <= span ? 1u : 0u) | (static_cast<unsigned long long>(v[1] - lo) <= span ? 2u : 0u);
 }
 
-// kQuad (opt-in, SDBG_GROUPBY_QUAD=1): every accumulator of the slot is an integer (fixed-point SUM(double) or
-// no double sum), and the four words of a row's slot are updated by four adjacent lanes of ONE RED
-// instruction: one L2 request per passing row, sums independent of update order (bit-reproducible), at the
-// cost of a compaction through shared memory and limb arithmetic in the consumer warps. Off by default.
+// Shape of filter_groupby_tma_kernel: a ring of kGroupByStages tiles of kGroupByTileRows rows, filled by one producer
+// warp and read by kGroupByConsumerWarps consumer warps. 3 x 20 KB stages -> 3 CTAs (24 consumer warps) per SM; on an
+// H100 (400 W) ring depths 3 and 4 tie, 2 is 7 % slower.
+constexpr int kGroupByStages = 3;
+constexpr int kGroupByTileRows = 512;
+constexpr int kGroupByConsumerWarps = 8;
 // kFor: some streams are FOR bit-packed (TmaGroupByParams::hdr); needs kTileRows to divide kForGroupRows with 16-byte
-// aligned tile slices, i.e. the default 512-row shape. The group headers of the stages live behind the ring (and behind
-// the quad area): kStages * kMaxStreams * 16 bytes.
-template <int kStages, int kTileRows, int kConsumerWarps, bool kPacked, bool kQuad, bool kFor = false>
-__global__ void __launch_bounds__((kConsumerWarps + 1) * 32)
+// aligned tile slices. The group headers of the stages live behind the ring: kStages * kMaxStreams * 16 bytes.
+template <bool kPacked, bool kFor>
+__global__ void __launch_bounds__((kGroupByConsumerWarps + 1) * 32)
 filter_groupby_tma_kernel(const TmaGroupByParams P) {
+  constexpr int kStages = kGroupByStages, kTileRows = kGroupByTileRows, kConsumerWarps = kGroupByConsumerWarps;
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages];
   static_assert(!kFor || (kForGroupRows % kTileRows == 0 && kTileRows % 128 == 0), "a tile's packed slice must be 16-byte aligned");
@@ -524,7 +520,7 @@ filter_groupby_tma_kernel(const TmaGroupByParams P) {
   __syncthreads();
   const uint32_t stage_bytes = P.off[P.n_streams];
   const uint64_t n_tiles = (P.rows + kTileRows - 1) / kTileRows;
-  uint4* const pk_hdr = reinterpret_cast<uint4*>(smem + size_t(kStages) * stage_bytes + (kQuad ? size_t(kConsumerWarps) * (2048u + 256u) : 0u));
+  uint4* const pk_hdr = reinterpret_cast<uint4*>(smem + size_t(kStages) * stage_bytes);
 
   if (warp == kConsumerWarps) {
     if (kFor) {
@@ -596,9 +592,6 @@ filter_groupby_tma_kernel(const TmaGroupByParams P) {
   }
 
   // ===== consumers =====
-  // quad mode: per-warp staging area behind the ring, 64 entries x (4 addends + slot index)
-  unsigned long long* const q_words = reinterpret_cast<unsigned long long*>(smem + size_t(kStages) * stage_bytes) + size_t(warp) * 256u;
-  uint32_t* const q_idx = reinterpret_cast<uint32_t*>(smem + size_t(kStages) * stage_bytes + size_t(kConsumerWarps) * 2048u) + size_t(warp) * 64u;
   // Each lane owns two consecutive rows of a 64-row strip, so every staged column is read with one
   // 16-byte (8-byte for int32) shared load per lane and the column type is a warp-uniform switch
   // outside the per-row work.
@@ -630,7 +623,7 @@ filter_groupby_tma_kernel(const TmaGroupByParams P) {
           m &= P.pred_negate[i] ? ~in : in;
         }
       }
-      if (!kQuad && m == 0u) continue;          // quad mode: every lane takes part in the warp-wide compaction
+      if (m == 0u) continue;
       long long key[2], v[2] = {0, 0};
       double w[2] = {0.0, 0.0};
       if (kFor && P.key_type == kTypeFor) unpack2(base + P.key_off, r, hst[P.key_stream], key);
@@ -642,59 +635,6 @@ filter_groupby_tma_kernel(const TmaGroupByParams P) {
       if (P.has_sum_f) {
         const double2 x = *reinterpret_cast<const double2*>(base + P.sum_f_off + size_t(r) * 8u);
         w[0] = x.x; w[1] = x.y;
-      }
-      if (kQuad) {
-        // Stage {slot index, 4 addends} of every passing row compacted in shared memory, then let lane
-        // 4q + f add word f of entry q: eight sectors per RED instruction, one request per passing row.
-        unsigned long long a[2][4];
-        uint32_t gi[2] = {0u, 0u};
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          if (!(m & (1u << j))) continue;
-          const unsigned long long idx = static_cast<unsigned long long>(key[j] - P.key_min);
-          if (idx >= P.key_span) { atomicAdd(P.out_of_range, 1ull); m &= ~(1u << j); continue; }
-          gi[j] = uint32_t(idx);                                   // dense tables span <= 2^26 groups
-          if (kPacked) {
-            const unsigned long long pk = (1ull << P.pack_shift) + static_cast<unsigned long long>(v[j] - P.pack_bias);
-            a[j][0] = pack_word == 0u ? pk : 0ull;
-            a[j][1] = pack_word == 1u ? pk : 0ull;
-            a[j][2] = pack_word == 2u ? pk : 0ull;
-          } else {
-            a[j][0] = 1ull;
-            a[j][1] = !P.has_sum_i ? 0ull : P.wide_int ? (static_cast<unsigned long long>(v[j]) & 0xFFFFFFFFull) : static_cast<unsigned long long>(v[j]);
-            a[j][2] = P.has_sum_i && P.wide_int ? static_cast<unsigned long long>(v[j] >> 32) : 0ull;
-          }
-          a[j][3] = 0ull;
-          if (P.fix_limb) {                                        // fixed-point SUM(double): words 2 and 3
-            long long l0, l1;
-            fix_limbs(w[j], P.fix_limb, P.fix_eunit, l0, l1);
-            a[j][2] = static_cast<unsigned long long>(l0);
-            a[j][3] = static_cast<unsigned long long>(l1);
-          }
-        }
-        const uint32_t b0 = __ballot_sync(kFull, (m & 1u) != 0u), b1 = __ballot_sync(kFull, (m & 2u) != 0u);
-        const uint32_t lt = (1u << lane) - 1u;
-        uint32_t pos = __popc(b0 & lt) + __popc(b1 & lt);
-        const uint32_t total = __popc(b0) + __popc(b1);
-        if (m & 1u) {
-          reinterpret_cast<ulonglong2*>(q_words)[pos * 2u] = make_ulonglong2(a[0][0], a[0][1]);
-          reinterpret_cast<ulonglong2*>(q_words)[pos * 2u + 1u] = make_ulonglong2(a[0][2], a[0][3]);
-          q_idx[pos++] = gi[0];
-        }
-        if (m & 2u) {
-          reinterpret_cast<ulonglong2*>(q_words)[pos * 2u] = make_ulonglong2(a[1][0], a[1][1]);
-          reinterpret_cast<ulonglong2*>(q_words)[pos * 2u + 1u] = make_ulonglong2(a[1][2], a[1][3]);
-          q_idx[pos] = gi[1];
-        }
-        __syncwarp();
-        if (!(P.debug_skip & 7)) {
-          for (uint32_t e = lane >> 2; e < total; e += 8u) {
-            const unsigned long long val = q_words[e * 4u + (lane & 3u)];
-            if (val) atomicAdd(reinterpret_cast<unsigned long long*>(P.table + q_idx[e]) + (lane & 3u), val);
-          }
-        }
-        __syncwarp();
-        continue;
       }
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
@@ -901,17 +841,11 @@ filter_groupby_hash_kernel(const HashGroupByParams P) {
 __global__ void __launch_bounds__(256)
 groupby_pack_kernel(const GroupSlot* __restrict__ table, const unsigned long long* __restrict__ cnt_f,
                     uint64_t span, long long* __restrict__ d_i64, double* __restrict__ d_f64,
-                    int pack_shift, int pack_tables, long long pack_bias, int fix_limb, int fix_eunit) {
+                    int pack_shift, int pack_tables, long long pack_bias) {
   for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < span; i += uint64_t(gridDim.x) * blockDim.x) {
     GroupSlot g = table[i];
-    if (fix_limb) {     // fixed-point SUM(double): words 2, 3 hold the two limb sums (so at most two packed words)
-      const long long s0 = g.sum_hi;
-      long long s1; memcpy(&s1, &g.sum_f, 8);
-      g.sum_f = fix_total(s0, s1, fix_limb, fix_eunit);
-      g.sum_hi = 0;
-    }
     if (pack_tables) {  // packed accumulators: split count << shift | sum(v - bias) back into the plain fields
-      const unsigned long long w[3] = {g.count, static_cast<unsigned long long>(g.sum_lo), static_cast<unsigned long long>(g.sum_hi)};   // sum_hi is 0 in fix mode
+      const unsigned long long w[3] = {g.count, static_cast<unsigned long long>(g.sum_lo), static_cast<unsigned long long>(g.sum_hi)};
       const unsigned long long mask = (1ull << pack_shift) - 1ull;
       unsigned long long cnt = 0, sum = 0;
       for (int t = 0; t < pack_tables; ++t) { cnt += w[t] >> pack_shift; sum += w[t] & mask; }
@@ -941,20 +875,6 @@ minmax_i64_kernel(const ColDev col, uint64_t rows, long long* __restrict__ out /
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) { mn = min(mn, __shfl_xor_sync(kFull, mn, o)); mx = max(mx, __shfl_xor_sync(kFull, mx, o)); }
   if ((threadIdx.x & 31u) == 0) { atomicMin(out, mn); atomicMax(out + 1, mx); }
-}
-
-// Largest |w| of a double column as raw bits (non-negative doubles order like their bit patterns; any
-// NaN or infinity yields a value >= 0x7FF0000000000000).
-__global__ void __launch_bounds__(256)
-absmax_f64_kernel(const ColDev col, uint64_t rows, unsigned long long* __restrict__ out) {
-  unsigned long long mx = 0ull;
-  for (uint64_t r = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; r < rows; r += uint64_t(gridDim.x) * blockDim.x) {
-    if (!col_valid(col, r)) continue;
-    mx = max(mx, static_cast<const unsigned long long*>(col.values)[r] & 0x7FFFFFFFFFFFFFFFull);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) mx = max(mx, __shfl_xor_sync(kFull, mx, o));
-  if ((threadIdx.x & 31u) == 0) atomicMax(out, mx);
 }
 
 // ------------------------------------------------------------------------------------------

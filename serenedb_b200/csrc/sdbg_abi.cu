@@ -49,7 +49,7 @@ struct ColumnObj {
   void* d_values = nullptr;
   // Owned NOT NULL int64 columns whose frame-of-reference bit-packed form is smaller than the raw one stay packed:
   // ForBlockDev headers (packed_hdr_bytes, 256-aligned) | word stream (every group 16-byte aligned) | 64 B of slack.
-  // The default-shape TMA GROUP BY reads this directly; every other reader goes through raw_values().
+  // The TMA GROUP BY reads this directly; every other reader goes through raw_values().
   void* d_packed = nullptr;
   size_t packed_bytes = 0;
   uint64_t* d_validity = nullptr;
@@ -61,8 +61,6 @@ struct ColumnObj {
   long long* d_zone = nullptr;  // zonemap: {min, max} per 2048-row block in predicate key space (NOT NULL columns, built on first use)
   bool zone_ok = false;         // d_zone holds the current values' zonemap (a restage of the same shape keeps the allocation)
   std::vector<long long> h_zone;  // host copy of the current zonemap, fetched on first use by the filter chains (empty: none)
-  bool has_absmax = false;      // double columns: bits of the largest |value| (>= 0x7FF0... when NaN / inf occur)
-  uint64_t absmax_bits = 0;
 };
 
 }  // namespace
@@ -621,7 +619,7 @@ extern "C" int sdbg_stage_column(sdbg_segment* s, uint64_t field, sdbg_type t, c
     CU(c, cudaMemsetAsync(static_cast<char*>(col.d_values) + bytes, 0, 64, c->stream));
   }
   col.zone_ok = false; col.h_zone.clear();   // new values: the zonemap is built again on first use (into the same allocation)
-  col.type = t; col.rows = rows; col.owned = true; col.has_minmax = false; col.has_absmax = false;
+  col.type = t; col.rows = rows; col.owned = true; col.has_minmax = false;
   CU(c, cudaMemcpyAsync(col.d_values, values, bytes, cudaMemcpyHostToDevice, c->stream));
   if (validity) {
     const size_t vb = ((rows + 63) / 64) * 8;
@@ -718,7 +716,7 @@ extern "C" int sdbg_stage_column_for(sdbg_segment* s, uint64_t field, const sdbg
       col.rows = rows; col.packed_bytes = packed_bytes;
       CU(c, cudaMalloc(&col.d_packed, packed_bytes));
     }
-    col.type = SDBG_I64; col.rows = rows; col.owned = true; col.has_minmax = false; col.has_absmax = false;
+    col.type = SDBG_I64; col.rows = rows; col.owned = true; col.has_minmax = false;
     CU(c, cudaMemcpyAsync(col.d_packed, headers, n_groups * sizeof(ForBlockDev), cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaMemcpyAsync(const_cast<unsigned long long*>(for_words(col)), words, n_words * 8, cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaMemsetAsync(static_cast<char*>(col.d_packed) + packed_bytes - 64, 0, 64, c->stream));
@@ -737,7 +735,7 @@ extern "C" int sdbg_stage_column_for(sdbg_segment* s, uint64_t field, const sdbg
     CU(c, cudaMemsetAsync(static_cast<char*>(col.d_values) + bytes, 0, 64, c->stream));
   }
   if (col.d_validity) { cudaFree(col.d_validity); col.d_validity = nullptr; }
-  col.type = SDBG_I64; col.rows = rows; col.owned = true; col.has_minmax = false; col.has_absmax = false;
+  col.type = SDBG_I64; col.rows = rows; col.owned = true; col.has_minmax = false;
   col.zone_ok = false; col.h_zone.clear();
   DevBuf& buf = c->scratch[12];
   const size_t hdr_bytes = (n_groups * sizeof(ForBlockDev) + 255) & ~size_t(255);
@@ -781,7 +779,7 @@ extern "C" int sdbg_column_device_ptr(sdbg_segment* s, uint64_t field, void** d_
     cudaFree(col.d_packed);
     col.d_packed = nullptr; col.packed_bytes = 0;
   }
-  col.has_minmax = false; col.has_absmax = false; col.zone_ok = false; col.h_zone.clear();
+  col.has_minmax = false; col.zone_ok = false; col.h_zone.clear();
   if (d_values) *d_values = p;
   if (rows) *rows = it->second.rows;
   return SDBG_OK;
@@ -3627,30 +3625,6 @@ int column_minmax(sdbg_segment* s, uint64_t field, int64_t* mn, int64_t* mx) {
   return SDBG_OK;
 }
 
-// Largest magnitude of a double column (raw bits), computed once per column like the integer min/max.
-int column_absmax(sdbg_segment* s, uint64_t field, uint64_t* bits) {
-  sdbg_ctx* c = s->ctx;
-  auto it = s->cols.find(field);
-  if (it == s->cols.end()) return fail(c, SDBG_ENOTFOUND, "column not staged");
-  ColumnObj& col = it->second;
-  if (col.type != SDBG_F64) return fail(c, SDBG_EINVAL, "absmax statistics are kept for double columns");
-  if (!col.has_absmax) {
-    int rc;
-    if ((rc = ensure(c, c->scratch[10], 16))) return rc;
-    CU(c, cudaMemsetAsync(c->scratch[10].p, 0, 16, c->stream));
-    ColDev cd; cd.values = col.d_values; cd.validity = col.d_validity; cd.type = col.type; cd.pad = 0;
-    absmax_f64_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(cd, col.rows, static_cast<unsigned long long*>(c->scratch[10].p));
-    ++c->launches;
-    CU(c, cudaGetLastError());
-    unsigned long long res = 0;
-    CU(c, cudaMemcpyAsync(&res, c->scratch[10].p, 8, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    col.absmax_bits = res; col.has_absmax = true;
-  }
-  *bits = col.absmax_bits;
-  return SDBG_OK;
-}
-
 }  // namespace
 
 extern "C" int sdbg_column_minmax_i64(sdbg_segment* s, uint64_t field, int64_t* mn, int64_t* mx) {
@@ -3760,13 +3734,11 @@ extern "C" int sdbg_filter_count_sum(sdbg_segment* const* segs, size_t n_segs, c
 
 namespace {
 
-struct GroupPlan { int wide_int = 0; int count_f = 0; int pack_shift = 0; int pack_tables = 0; int64_t pack_bias = 0; int fix_limb = 0; int fix_eunit = 0; int quad = 0; };
-constexpr int kGroupByDefaultStages = 3;   // 3 x 20 KB stages -> 3 CTAs (24 consumer warps) per SM; on an H100 (400 W) 3 and 4 tie, 2 is 7 % slower
-constexpr int kGroupByTileRows = 512;   // tile of the default TMA shape; packed accumulators are only planned for it
+struct GroupPlan { int wide_int = 0; int count_f = 0; int pack_shift = 0; int pack_tables = 0; int64_t pack_bias = 0; };
 
 int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred* preds, size_t n_preds, uint64_t key_field,
                    int64_t key_min, uint64_t span, uint64_t sum_int_field, uint64_t avg_f64_field, void* d_i64, void* d_f64,
-                   GroupPlan* plan_out, bool defer_check = false) {
+                   bool defer_check = false) {
   sdbg_ctx* c = segs[0]->ctx;
   int rc;
   // table | cnt_f | out_of_range
@@ -3779,8 +3751,7 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
   GroupPlan plan;
   uint64_t total_rows = 0;
   int64_t sum_mn = INT64_MAX, sum_mx = INT64_MIN;
-  uint64_t absmax_bits = 0;
-  bool all_tma = env_int("SDBG_GROUPBY_TMA", 1) != 0 && env_int("SDBG_GROUPBY_TMA_SHAPE", 0) == 0;
+  bool all_tma = env_int("SDBG_GROUPBY_TMA", 1) != 0;
   for (size_t si = 0; si < n_segs; ++si) {  // statistics decide the accumulator shape
     sdbg_segment* s = segs[si];
     if (sum_int_field != UINT64_MAX) {
@@ -3799,9 +3770,6 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
       auto it = s->cols.find(avg_f64_field);
       if (it == s->cols.end()) return fail(c, SDBG_ENOTFOUND, "avg column not staged");
       if (it->second.d_validity) { plan.count_f = 1; all_tma = false; }
-      uint64_t ab = 0;
-      if (it->second.type == SDBG_F64 && all_tma && env_int("SDBG_GROUPBY_QUAD", 0)) { if ((rc = column_absmax(s, avg_f64_field, &ab))) return rc; }   // statistic only the fixed-point path needs
-      absmax_bits = std::max(absmax_bits, ab);
     }
     auto kit = s->cols.find(key_field);
     if (kit == s->cols.end()) return fail(c, SDBG_ENOTFOUND, "key column not staged");
@@ -3815,7 +3783,7 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
   // consumer warps run into). Rows are dealt to 1..3 words of the slot by tile index.
   if (sum_int_field != UINT64_MAX && !plan.wide_int && all_tma && total_rows && sum_mx >= sum_mn && env_int("SDBG_GROUPBY_PACKED", 1)) {
     const unsigned __int128 range = static_cast<unsigned __int128>(static_cast<uint64_t>(sum_mx) - static_cast<uint64_t>(sum_mn));
-    const int max_tables = avg_f64_field != UINT64_MAX ? 2 : 3;   // words 2, 3 are kept free for the fixed-point SUM(double) limbs
+    const int max_tables = avg_f64_field != UINT64_MAX ? 2 : 3;   // with a SUM(double) at most two words: a third is free, but that plan has not been measured
     for (int nt = std::max(1, env_int("SDBG_GROUPBY_PACK_TABLES_MIN", 1)); nt <= max_tables && !plan.pack_tables; ++nt) {   // env: test hook
       uint64_t cap_rows = 0;   // most rows any one word can receive: its share of every segment's tiles
       for (size_t si = 0; si < n_segs; ++si) {
@@ -3828,30 +3796,12 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
       if (shift < 63 && cap_rows < (1ull << (64 - shift))) { plan.pack_tables = nt; plan.pack_shift = shift; plan.pack_bias = sum_mn; }
     }
   }
-  // Fixed-point SUM(double): two integer limb REDs instead of one floating-point RED (see TmaGroupByParams).
-  // Needs words 2 and 3 of the slot (no wide integer sum, at most two packed words) and a finite column.
-  if (avg_f64_field != UINT64_MAX && all_tma && !plan.wide_int && total_rows && absmax_bits < 0x7FF0000000000000ull &&
-      env_int("SDBG_GROUPBY_FIXED", 1)) {
-    int row_bits = 1;
-    while ((1ull << row_bits) <= total_rows) ++row_bits;
-    plan.fix_limb = std::min(37, 63 - row_bits);                     // |limb sum| <= rows * 2^limb < 2^63
-    double mx; std::memcpy(&mx, &absmax_bits, 8);
-    int e = 0;
-    if (mx > 0) std::frexp(mx, &e);                                  // mx < 2^e
-    // |w| / 2^eunit < 2^(2*limb); never below 2^-1074, the unit of every double: a finer unit would shift a subnormal's
-    // mantissa 64 bits or more (fix_limbs) and gains nothing, since every value is already an integer multiple of it
-    plan.fix_eunit = std::max(e - 2 * plan.fix_limb, -1074);
-  }
-  // All accumulators integer => the four words of a slot go out as one RED request per passing row.
-  plan.quad = all_tma && (avg_f64_field == UINT64_MAX || plan.fix_limb) && env_int("SDBG_GROUPBY_QUAD", 0);
-  if (!plan.quad) plan.fix_limb = 0, plan.fix_eunit = 0;            // separate REDs: one f64 RED beats two integer ones
-  const int shape = env_int("SDBG_GROUPBY_TMA_SHAPE", 0);
   for (size_t si = 0; si < n_segs; ++si) {
     sdbg_segment* s = segs[si];
-    // Packed columns are read packed by the default-shape TMA kernel, which takes segments without nullable columns;
-    // every other path reads their raw view.
+    // Packed columns are read packed by the TMA kernel, which takes segments without nullable columns; every other
+    // path reads their raw view.
     auto nullable = [&](uint64_t f) { auto it = s->cols.find(f); return it != s->cols.end() && it->second.d_validity != nullptr; };
-    bool packed_ok = env_int("SDBG_GROUPBY_TMA", 1) != 0 && shape == 0 && !nullable(key_field) &&
+    bool packed_ok = env_int("SDBG_GROUPBY_TMA", 1) != 0 && !nullable(key_field) &&
                      (sum_int_field == UINT64_MAX || !nullable(sum_int_field)) && (avg_f64_field == UINT64_MAX || !nullable(avg_f64_field));
     for (size_t i = 0; i < n_preds; ++i) packed_ok = packed_ok && preds[i].op < 7 && !nullable(preds[i].field);
     GroupByParams P;
@@ -3956,62 +3906,35 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
       T.debug_skip = env_int("SDBG_GROUPBY_DEBUG", 0);
       T.wide_int = plan.wide_int; T.key_min = key_min; T.key_span = span; T.rows = rows; T.table = table; T.out_of_range = oor;
       T.pack_shift = plan.pack_shift; T.pack_tables = plan.pack_tables; T.pack_bias = plan.pack_bias;
-      T.fix_limb = plan.fix_limb; T.fix_eunit = plan.fix_eunit;
       for (int i = 0; i < T.n_preds; ++i) T.pred_stream[i] = stream_idx[i];
       T.key_stream = key_s; T.sum_i_stream = sum_i_s >= 0 ? sum_i_s : 0;
       bool any_for = false;
       for (int i = 0; i < T.n_streams; ++i) any_for |= T.hdr[i] != nullptr;
-      // Stream offsets inside a stage depend on the tile shape. A packed stream keeps its raw slot size, so the
-      // shared-memory footprint, ring depth and CTAs per SM are those of the raw scan.
-      auto set_offsets = [&](int tile_rows) {
-        uint32_t o = 0;
-        for (int i = 0; i < T.n_streams; ++i) { T.off[i] = o; o += uint32_t(T.elem[i]) * uint32_t(tile_rows); }
-        T.off[T.n_streams] = o;
-        for (int i = 0; i < T.n_preds; ++i) T.pred_off[i] = T.off[stream_idx[i]];
-        T.key_off = T.off[key_s];
-        T.sum_i_off = sum_i_s >= 0 ? T.off[sum_i_s] : 0;
-        T.sum_f_off = sum_f_s >= 0 ? T.off[sum_f_s] : 0;
-      };
-      const bool quad = plan.quad != 0;
-      auto launch = [&](auto kern, int stages, int tile_rows, int consumer_warps) -> int {
-        set_offsets(tile_rows);
-        const size_t smem = size_t(stages) * size_t(T.off[T.n_streams]) + (quad ? size_t(consumer_warps) * (2048 + 256) : 0) +
-                            (any_for ? size_t(stages) * kMaxStreams * 16 : 0);
+      // A packed stream keeps its raw slot size, so the shared-memory footprint and CTAs per SM are those of the raw scan.
+      uint32_t o = 0;
+      for (int i = 0; i < T.n_streams; ++i) { T.off[i] = o; o += uint32_t(T.elem[i]) * uint32_t(kGroupByTileRows); }
+      T.off[T.n_streams] = o;
+      for (int i = 0; i < T.n_preds; ++i) T.pred_off[i] = T.off[stream_idx[i]];
+      T.key_off = T.off[key_s];
+      T.sum_i_off = sum_i_s >= 0 ? T.off[sum_i_s] : 0;
+      T.sum_f_off = sum_f_s >= 0 ? T.off[sum_f_s] : 0;
+      constexpr int threads = (kGroupByConsumerWarps + 1) * 32;
+      const size_t smem = size_t(kGroupByStages) * size_t(T.off[T.n_streams]) + (any_for ? size_t(kGroupByStages) * kMaxStreams * 16 : 0);
+      auto launch = [&](auto kern) -> int {
         CU(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
         const size_t fit = std::max<size_t>(1, (220 * 1024) / (smem + 2048));
-        const size_t by_threads = std::max<size_t>(1, 2048 / (size_t(consumer_warps + 1) * 32));
         int resident = 0;   // persistent CTAs: never more per SM than can be resident at once (registers included)
-        CU(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, (consumer_warps + 1) * 32, smem));
-        const unsigned per_sm = unsigned(std::max<size_t>(1, std::min<size_t>({fit, by_threads, size_t(env_int("SDBG_GROUPBY_TMA_CTAS", 8)), size_t(resident)})));
-        const unsigned grid = unsigned(c->sm_count) * per_sm;
+        CU(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, threads, smem));
+        const unsigned per_sm = unsigned(std::max<size_t>(1, std::min<size_t>({fit, size_t(2048 / threads), size_t(resident)})));
         ProfScope ps_(c, kProfGroupBy);
-        kern<<<grid, (consumer_warps + 1) * 32, smem, c->stream>>>(T);
+        kern<<<unsigned(c->sm_count) * per_sm, threads, smem, c->stream>>>(T);
         return SDBG_OK;
       };
-      int lrc;
-      switch (shape) {
-        case 1: lrc = launch(filter_groupby_tma_kernel<4, 256, 8, false, false>, 4, 256, 8); break;
-        case 2: lrc = launch(filter_groupby_tma_kernel<4, 512, 16, false, false>, 4, 512, 16); break;
-        case 3: lrc = launch(filter_groupby_tma_kernel<3, 256, 8, false, false>, 3, 256, 8); break;
-        case 4: lrc = launch(filter_groupby_tma_kernel<4, 1024, 16, false, false>, 4, 1024, 16); break;
-        default: {
-          // default shape: 512-row tiles, 8 consumer warps; ring depth by SDBG_GROUPBY_TMA_STAGES (the CTAs per
-          // SM follow from the shared-memory footprint, so fewer stages = more resident consumer warps)
-#define SDBG_GB_LAUNCH(ST, FOR) \
-          (plan.pack_tables ? (quad ? launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, true, true, FOR>, ST, kGroupByTileRows, 8) \
-                                    : launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, true, false, FOR>, ST, kGroupByTileRows, 8)) \
-                            : (quad ? launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, false, true, FOR>, ST, kGroupByTileRows, 8) \
-                                    : launch(filter_groupby_tma_kernel<ST, kGroupByTileRows, 8, false, false, FOR>, ST, kGroupByTileRows, 8)))
-          const int stages = env_int("SDBG_GROUPBY_TMA_STAGES", kGroupByDefaultStages);
-          if (any_for) lrc = stages == 2 ? SDBG_GB_LAUNCH(2, true) : stages == 3 ? SDBG_GB_LAUNCH(3, true) : SDBG_GB_LAUNCH(4, true);
-          else lrc = stages == 2 ? SDBG_GB_LAUNCH(2, false) : stages == 3 ? SDBG_GB_LAUNCH(3, false) : SDBG_GB_LAUNCH(4, false);
-#undef SDBG_GB_LAUNCH
-          break;
-        }
-      }
+      const int lrc = plan.pack_tables ? (any_for ? launch(filter_groupby_tma_kernel<true, true>) : launch(filter_groupby_tma_kernel<true, false>))
+                                       : (any_for ? launch(filter_groupby_tma_kernel<false, true>) : launch(filter_groupby_tma_kernel<false, false>));
       if (lrc) return lrc;
     } else {
-      const unsigned grid = unsigned(c->sm_count) * unsigned(env_int("SDBG_GROUPBY_CTAS_PER_SM", 8));
+      const unsigned grid = unsigned(c->sm_count) * 8u;
       ProfScope ps_(c, kProfGroupBy);
       filter_groupby_kernel<2><<<grid, 256, 0, c->stream>>>(P);
     }
@@ -4020,7 +3943,7 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
   }
   groupby_pack_kernel<<<c->sm_count * 2, 256, 0, c->stream>>>(table, plan.count_f ? cnt_f : nullptr, span,
                                                                static_cast<long long*>(d_i64), static_cast<double*>(d_f64),
-                                                               plan.pack_shift, plan.pack_tables, plan.pack_bias, plan.fix_limb, plan.fix_eunit);
+                                                               plan.pack_shift, plan.pack_tables, plan.pack_bias);
   ++c->launches;
   CU(c, cudaGetLastError());
   if (defer_check) {
@@ -4035,7 +3958,6 @@ int groupby_launch(sdbg_segment* const* segs, size_t n_segs, const sdbg_col_pred
     CU(c, cudaStreamSynchronize(c->stream));
     if (h_oor) return fail(c, SDBG_EINVAL, "GROUP BY key outside [key_min, key_min + span)");
   }
-  if (plan_out) *plan_out = plan;
   return SDBG_OK;
 }
 
@@ -4129,10 +4051,9 @@ extern "C" int sdbg_filter_groupby_partial(sdbg_segment* const* segs, size_t n_s
                                            uint64_t avg_f64_field, void* d_i64, void* d_f64) {
   if (!segs || !n_segs || !d_i64 || !d_f64 || !key_span || (!preds && n_preds)) return SDBG_EINVAL;
   CU(segs[0]->ctx, cudaSetDevice(segs[0]->ctx->device));
-  GroupPlan plan;
   // asynchronous: nothing here waits for the GPU (SUM(int) leaves as two limbs, total = hi * 2^32 + lo; a narrow sum
   // keeps the whole value in lo -- sdbg_dist_groupby_merge normalises the limbs before they are all-reduced)
-  return groupby_launch(segs, n_segs, preds, n_preds, key_field, key_min, key_span, sum_int_field, avg_f64_field, d_i64, d_f64, &plan, true);
+  return groupby_launch(segs, n_segs, preds, n_preds, key_field, key_min, key_span, sum_int_field, avg_f64_field, d_i64, d_f64, true);
 }
 
 extern "C" int sdbg_groupby_finalize(sdbg_ctx* c, int64_t key_min, uint64_t span, const void* d_i64, const void* d_f64,
@@ -4197,8 +4118,7 @@ extern "C" int sdbg_filter_groupby(sdbg_segment* const* segs, size_t n_segs, con
   if ((rc = ensure(c, c->scratch[8], span * 40 + 64))) return rc;
   void* d_i64 = c->scratch[8].p;
   void* d_f64 = static_cast<char*>(c->scratch[8].p) + span * 32;
-  GroupPlan plan;
-  if ((rc = groupby_launch(segs, n_segs, preds, n_preds, key_field, kmin, span, sum_int_field, avg_f64_field, d_i64, d_f64, &plan))) return rc;
+  if ((rc = groupby_launch(segs, n_segs, preds, n_preds, key_field, kmin, span, sum_int_field, avg_f64_field, d_i64, d_f64))) return rc;
   return sdbg_groupby_finalize(c, kmin, span, d_i64, d_f64, out, cap, n_out);
 }
 

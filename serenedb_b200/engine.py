@@ -322,7 +322,7 @@ class Segment:
 
     def column_device_ptr(self, field):
         """(device address, rows) of the column's raw values, for writing them in place. The call means "about to
-        write": the column's cached min / max, largest magnitude and zonemap are dropped, and a bit-packed column is held
+        write": the column's cached min / max and zonemap are dropped, and a bit-packed column is held
         as these raw values until it is restaged. Write after ctx.sync(), finish before the next query, and call this
         again before writing again. A borrowed column (stage_column_device) is instead restaged after its owner writes it."""
         p, r = C.c_void_p(), C.c_uint64()

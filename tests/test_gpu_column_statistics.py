@@ -1,6 +1,5 @@
 """Plans chosen from cached column statistics: the min / max (dense range, wide limbs, packed COUNT|SUM word, facet key
-range), the largest magnitude (fixed-point SUM(double)), the zonemaps (skip verdicts) and the bit-packed words. Each
-reader is compared with NumPy over the column's current values (exact Python-int sums) after the values change in every
+range), the zonemaps (skip verdicts) and the bit-packed words. Each reader is compared with NumPy over the column's current values (exact Python-int sums) after the values change in every
 way the library allows, and each statistics-gated choice is placed on both sides of its limit, up to the GROUP BY's row
 limit of 2^31 - 1 rows per GPU."""
 import json
@@ -21,10 +20,9 @@ pytestmark = pytest.mark.gpu
 
 INT32_MIN, INT32_MAX = -2**31, 2**31 - 1
 INT64_MIN, INT64_MAX = -2**63, 2**63 - 1
-DBL_MAX = float(np.finfo(np.float64).max)
 N = 200_000                      # 98 zonemap blocks of 2048 rows
 KEY, SUBJ = 1, 2                 # the GROUP BY key column and the column whose values change
-TILE = 512                       # rows per tile of the default TMA GROUP BY (packed words are dealt by tile)
+TILE = 512                       # rows per tile of the TMA GROUP BY (packed words are dealt by tile)
 
 # GROUP BY paths: default (TMA, packed COUNT|SUM words when the statistics allow), TMA with plain words, the
 # register-staged kernel, the hash table
@@ -111,7 +109,7 @@ def _kernels_per_call(calls):
 
 
 def _tma_args(names):
-    """Template arguments of each filter_groupby_tma_kernel launch: [stages, tile, warps, kPacked, kQuad, kFor]."""
+    """Template arguments of each filter_groupby_tma_kernel launch: [kPacked, kFor]."""
     out = []
     for n in names:
         if "filter_groupby_tma_kernel" in n:
@@ -121,8 +119,7 @@ def _tma_args(names):
 
 
 def _env(monkeypatch, env):
-    for k in ("SDBG_GROUPBY_PACKED", "SDBG_GROUPBY_TMA", "SDBG_GROUPBY_FORCE_HASH", "SDBG_GROUPBY_PACK_TABLES_MIN",
-              "SDBG_GROUPBY_QUAD"):
+    for k in ("SDBG_GROUPBY_PACKED", "SDBG_GROUPBY_TMA", "SDBG_GROUPBY_FORCE_HASH", "SDBG_GROUPBY_PACK_TABLES_MIN"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)
@@ -294,7 +291,7 @@ def check_readers(monkeypatch, seg, reader, keys, vals, valid=None):
 
 def _old_new(dtype):
     """(old, new): old ascends in clusters of 100 from 1000 to 2999; new descends in clusters of 8 from 12_999 to
-    -12_000. The new values move the min and the max, the largest magnitude and every zonemap block, and a stale plan
+    -12_000. The new values move the min and the max and every zonemap block, and a stale plan
     gives a different answer rather than an error (a stale packing bias above the new minimum carries the sum field into
     the count). Both ranges fit the facet bins."""
     i = np.arange(N)
@@ -511,43 +508,14 @@ def test_dense_or_hash_at_the_span_limits(monkeypatch, span, hint, dense):
     segs[0].close()
 
 
-def _quad_values(kind, rows, rng):
-    if kind == "pow2":
-        w = rng.uniform(-1024.0, 1024.0, rows)
-        w[:2] = 1024.0, -1024.0
-    elif kind == "subnormal":
-        w = rng.integers(-2, 2, rows, endpoint=True).astype(np.float64) * 5e-324    # multiples of 2^-1074
-        w[:2] = 2 * 5e-324, -5e-324                                     # the largest: 2^-1073, two mantissa bits
-    else:
-        w = rng.uniform(-1.0, 1.0, rows) * 2.0**1000
-        w[:2] = DBL_MAX, -DBL_MAX
-    return w
-
-
-@pytest.mark.parametrize("kind", ["pow2", "subnormal", "dbl_max"])
-def test_fixed_point_sum_double_at_magnitude_edges(monkeypatch, kind):
-    """Fixed-point SUM(double) (SDBG_GROUPBY_QUAD=1) sized from the largest magnitude: exactly a power of two, subnormal
-    (the unit never goes below 2^-1074), and DBL_MAX."""
-    rows = 70_002
-    rng = np.random.default_rng(len(kind))
-    cols = [{1: rng.integers(0, 7, rows).astype(np.int64), 3: _quad_values(kind, rows, rng)}]
-    cols[0][1][:2] = 0                                                  # +-DBL_MAX in one key: a finite sum
-    segs = _segments(cols)
-    _env(monkeypatch, {"SDBG_GROUPBY_QUAD": "1"})
-    _run_groupby(segs, cols, 1, sf=3)
-    _env(monkeypatch, {})
-    segs[0].close()
-
-
 def _plan_checks():
     """(ok, detail) per limit case: the kernels it launches, from one profiler session. The packed COUNT|SUM word at its
     fill limit in 1, 2 and 3 words and on both sides of the count-field limit; wide limbs (no packed word) exactly past
-    the int32 range; the dense table up to max(2^20, 8 x hint) and 2^26 keys, the hash table past them; the fixed-point
-    SUM(double) at every magnitude edge."""
+    the int32 range; the dense table up to max(2^20, 8 x hint) and 2^26 keys, the hash table past them."""
     cases = []                                            # (segments, groupby kwargs, env, check of the kernel names)
 
     def packed(flag):
-        return lambda names: bool(_tma_args(names)) and all(a[3] == flag for a in _tma_args(names))
+        return lambda names: bool(_tma_args(names)) and all(a[0] == flag for a in _tma_args(names))
     for nt in (1, 2, 3):
         cases.append((_segments(_pack_fill([7, 5, 1, 2], nt, 43)[0]), dict(sum_int_field=2),
                       {"SDBG_GROUPBY_PACK_TABLES_MIN": str(nt)}, packed("true")))
@@ -567,10 +535,6 @@ def _plan_checks():
         cases.append((_segments([{1: k, 2: np.ones(4096, np.int64)}]), dict(sum_int_field=2, n_groups_hint=hint), {},
                       (lambda d: lambda names: bool(_tma_args(names)) == d and
                        any("filter_groupby_hash_kernel" in n for n in names) != d)(dense)))
-    for kind in ("pow2", "subnormal", "dbl_max"):
-        w = _quad_values(kind, 4096, np.random.default_rng(1))
-        cases.append((_segments([{1: np.zeros(4096, np.int64), 3: w}]), dict(avg_f64_field=3), {"SDBG_GROUPBY_QUAD": "1"},
-                      lambda names: bool(_tma_args(names)) and all(a[4] == "true" for a in _tma_args(names))))
 
     def call(segs, kw, env):
         def fn():
@@ -600,7 +564,7 @@ def test_plans_flip_at_their_limits():
     res = subprocess.run(args, capture_output=True, text=True, timeout=900)
     assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
     out = json.loads(res.stdout.strip().splitlines()[-1])
-    assert len(out) == 17 and all(ok for ok, _ in out), [(i, detail) for i, (ok, detail) in enumerate(out) if not ok]
+    assert len(out) == 14 and all(ok for ok, _ in out), [(i, detail) for i, (ok, detail) in enumerate(out) if not ok]
 
 
 # ---------------------------------------------------------------------------------------------------------------------

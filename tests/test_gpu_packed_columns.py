@@ -228,7 +228,7 @@ def _kernels_of(fn):
 
 
 def test_groupby_reads_the_packed_words():
-    """The default-shape GROUP BY over packed columns runs the kFor instantiation and never decodes a raw view."""
+    """The TMA GROUP BY over packed columns runs the kFor instantiation and never decodes a raw view."""
     packed, raw, host, keep = _tables([70_002], [9], [20], [11], seed=7)
     preds = [sdb.pred(2, "LT", int(np.median(host[0][2])))]
     names = _kernels_of(lambda: sdb.IResearchScan(packed).groupby(preds, 1, sum_int_field=4, avg_f64_field=3))
