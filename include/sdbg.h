@@ -104,6 +104,16 @@ int sdbg_stage_postings(sdbg_segment*, const uint8_t* doc_file, size_t n, const 
  * scored, collected nor counted by the BM25 calls, like SegmentReaderImpl::mask wrapping the query iterator
  * (segment_reader_impl.cpp:95-157,318-326; duckdb_search_full_scan.cpp:1898). n == 0 clears the mask. */
 int sdbg_stage_docs_mask(sdbg_segment*, const uint32_t* deleted_docs, size_t n);
+/* Term positions of the segment's field, for phrase queries (sdbg_phrase_*_batch): term t's positions are
+ * positions[term_pos_off[t] .. term_pos_off[t+1]) (term_pos_off has n_terms + 1 entries), in posting order, posting i of
+ * the term contributing exactly its freq_i positions, strictly ascending within the posting: the values the reference's
+ * position iterator yields (PosAttr::value()), decoded once at load time. Call after sdbg_stage_postings; restaging the
+ * postings drops the positions, restaging the positions replaces them. HBM layout (DESIGN.md §3): 8 B per posting block,
+ * 4 B per posting and 4 B per position. Errors: NULL segment or term_pos_off, postings not staged, n_terms different from
+ * the staged term count, a decreasing term_pos_off, or NULL positions with a non-empty range: SDBG_EINVAL; a term whose
+ * position count differs from the sum of its postings' frequencies, or positions not strictly ascending within a
+ * posting: SDBG_EFORMAT (the segment keeps the positions it had). Synchronous. */
+int sdbg_stage_positions(sdbg_segment*, const uint32_t* positions, const uint64_t* term_pos_off, size_t n_terms);
 /* The b of the BM25 scorer the segment's block-max (wand) entries were written for (wand_writer.hpp:142-175; default
    0.75). Block-max pruning is used only for queries whose scorer has the same b -- the check Scorer::equals makes in
    PostingsReaderImpl::WandIterator (formats/posting/reader.hpp:457-501); any other scorer is evaluated exhaustively. */
@@ -332,7 +342,7 @@ int sdbg_match_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, int 
  * in HBM (n_queries * (8k + 12) B) before they go to query order on the device.
  * The top-k of group queries across GPUs: sdbg_dist_bm25_topk_batch_groups_min below.
  * The streaming scan of group queries, batched over segments: sdbg_match_scan_batch_groups_min below.
- * Not supported yet: deeper nesting (an OR of ANDs), more than 16 positive terms, phrases. */
+ * Not supported yet: deeper nesting (an OR of ANDs), more than 16 positive terms. Phrases: sdbg_phrase_*_batch below. */
 int sdbg_bm25_topk_batch_groups(sdbg_segment* const* segs, size_t n_segs, const sdbg_bm25_term* terms,
                                 const uint32_t* group_off, const uint32_t* query_group_off, size_t n_queries,
                                 const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
@@ -459,6 +469,38 @@ int sdbg_match_scan_batch_groups_min(sdbg_segment* const* segs, size_t n_segs, c
                                      float k1, float b, const sdbg_col_pred* filt,
                                      const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit, int scored,
                                      sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
+/* Exact phrase queries (`body @@ '"new york"'`: by_phrase / FixedPhraseQuery of plain terms, slop 0). Query q is the phrase
+ * of slots phrase_off[q] .. phrase_off[q+1]) (1..16): slot i is term terms[i] at relative position rel_pos[i], rel_pos
+ * starting at 0 in each phrase and strictly increasing (rel_pos NULL: 0, 1, 2, ..., adjacent words; gaps express removed
+ * stop words). A term may repeat (`"to be or not to be"`); at most 16 distinct terms. Doc d matches when some anchor p has
+ * p + rel_pos[i] among term terms[i]'s positions in d for every slot i, d is not deleted, passes the filter chain and is
+ * in none of the lists of excl_terms[excl_off[q] .. excl_off[q+1]) (0..16 ids; excl_off NULL: none). The phrase frequency
+ * is the number of such anchors, overlaps included (`"a a"` in `a a a`: 2). A term a segment holds no postings for makes
+ * the phrase match nothing there. Every segment needs staged positions (sdbg_stage_positions).
+ * sdbg_phrase_count_batch: counts[q] = the number of matching docs over the segments.
+ * sdbg_phrase_topk_batch: the k best matches by score, scored bm25(phrase frequency, norm(d)) with phrase_stats[q] (one
+ * per query, .term ignored; engine.py sums the terms' idfs), under BM25, BM15 (b = 0), BM1 (k1 = 0) or TFIDF (k1 = -1)
+ * as in the other batch entries; out / n_out / total_matches / threshold_in as sdbg_bm25_topk_batch (score desc, segment
+ * asc, doc asc; scores > threshold_in). Nothing is pruned: identical at every pruning level, total_matches exact and equal
+ * to the count. A one-slot phrase gives exactly its term's flat result.
+ * Errors, all found before anything is queued: an empty phrase, rel_pos not starting at 0 or not increasing, a
+ * decreasing offset array, or NULL arrays with non-empty ranges: SDBG_EINVAL; more than 16 slots or 16 excluded ids:
+ * SDBG_EUNSUPPORTED; a segment without positions: SDBG_ENOTFOUND; otherwise the errors and limits of
+ * sdbg_match_count_batch (kind AND) and, for the top-k, of sdbg_bm25_topk_batch, with k capped at 4096 (each work item
+ * keeps 2 * next_pow2(k) 16-byte candidate keys in shared memory): SDBG_EUNSUPPORTED above. Synchronous.
+ * Device scratch: as sdbg_match_count_batch; the top-k adds k keys of 8 B per work item (a range of 65 536-doc windows of
+ * one query in one segment, at most 2 x SMs per query and segment) and n_queries * (8k + 12) B for the results, with as
+ * much pinned host memory for the copy back. */
+int sdbg_phrase_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                            const uint32_t* rel_pos /* NULL: adjacent */, const uint32_t* phrase_off, size_t n_queries,
+                            const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                            uint64_t* counts);
+int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                           const uint32_t* rel_pos /* NULL: adjacent */, const uint32_t* phrase_off, size_t n_queries,
+                           const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                           const sdbg_bm25_term* phrase_stats /* n_queries */, float k1, float b, const sdbg_col_pred* filt,
+                           uint32_t k, float threshold_in, sdbg_hit* out /* n_queries * k */, uint32_t* n_out,
+                           uint64_t* total_matches);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

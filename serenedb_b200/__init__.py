@@ -10,6 +10,7 @@ from .engine import (ExecuteDistCountGroupsBatch, ExecuteDistFacetCountsGroupsBa
                      ExecuteDistTopKByColumnGroupsBatch, MatchAggregatesDevice, TopKByColumnDevice, match_aggregate_device_bytes,
                      merge_aggregates_gathered, merge_topk_by_column_gathered, topk_by_column_device_bytes)
 from .engine import ExecuteDistTopKGroupsBatch, TopKGroupsDevice, merge_topk_groups_gathered, topk_groups_device_bytes
+from .engine import ExecutePhraseCount, ExecutePhraseCountBatch, ExecutePhraseTopK, ExecutePhraseTopKBatch
 from .engine import (AND, OR, BM25, TFIDF, FLT_MIN, Context, ExecuteCount, ExecuteCountBatch, ExecuteCountGroups,
                      ExecuteCountGroupsBatch, ExecuteFacetCounts, ExecuteFacetCountsBatch, ExecuteFacetCountsGroups,
                      ExecuteFacetCountsGroupsBatch, ExecuteMatchAggregates, ExecuteMatchAggregatesBatch,
@@ -29,4 +30,5 @@ __all__ = ["AND", "OR", "BM25", "TFIDF", "FLT_MIN", "Context", "ExecuteCount", "
            "MatchAggregatesDevice", "match_aggregate_device_bytes", "merge_aggregates_gathered",
            "ExecuteDistTopKByColumnGroupsBatch", "TopKByColumnDevice", "topk_by_column_device_bytes",
            "merge_topk_by_column_gathered", "ExecuteDistTopKGroupsBatch", "TopKGroupsDevice", "topk_groups_device_bytes",
-           "merge_topk_groups_gathered"]
+           "merge_topk_groups_gathered", "ExecutePhraseCount", "ExecutePhraseCountBatch", "ExecutePhraseTopK",
+           "ExecutePhraseTopKBatch"]

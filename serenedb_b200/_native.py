@@ -66,6 +66,7 @@ SIGNATURES = {
     "sdbg_segment_destroy": (None, [_vp]),
     "sdbg_stage_postings": (C.c_int, [_vp, _vp, _sz, _vp, _sz, C.c_int]),
     "sdbg_stage_norms": (C.c_int, [_vp, _vp, _sz, _vp, _sz]),
+    "sdbg_stage_positions": (C.c_int, [_vp, _vp, _vp, _sz]),
     "sdbg_stage_column": (C.c_int, [_vp, C.c_uint64, C.c_int, _vp, _vp, C.c_uint64]),
     "sdbg_stage_column_device": (C.c_int, [_vp, C.c_uint64, C.c_int, _vp, C.c_uint64]),
     "sdbg_column_device_ptr": (C.c_int, [_vp, C.c_uint64, C.POINTER(_vp), _u64p]),
@@ -104,6 +105,9 @@ SIGNATURES = {
     "sdbg_bm25_scan_excl": (C.c_int, [_vp, C.c_int, _vp, _sz, _vp, _sz, C.c_float, C.c_float, _vp, C.c_uint32, C.c_uint32, _vp,
                                       _vp, C.c_uint64, _u64p]),
     "sdbg_match_count_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "sdbg_phrase_count_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "sdbg_phrase_topk_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_float, C.c_float, _vp, C.c_uint32,
+                                         C.c_float, _vp, _vp, _vp]),
     "sdbg_match_topk_by_column_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int, C.c_int,
                                                   C.c_uint32, _vp, _vp]),
     "sdbg_match_facet_counts_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,

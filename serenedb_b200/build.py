@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "_lib")
 LIB_PATH = os.path.join(LIB_DIR, "libsdbg.so")
 SOURCES = [os.path.join(CSRC, "sdbg_abi.cu"), os.path.join(CSRC, "posting_format.cpp")]
-DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("bm25_kernels.cuh", "bm25_stream.cuh", "bm25_merge.cuh", "bm25_count.cuh", "bm25_emit.cuh", "bm25_agg.cuh", "bm25_facet.cuh", "bm25_sort.cuh", "column_kernels.cuh", "device_common.cuh",
+DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("bm25_kernels.cuh", "bm25_stream.cuh", "bm25_merge.cuh", "bm25_count.cuh", "bm25_emit.cuh", "bm25_agg.cuh", "bm25_facet.cuh", "bm25_sort.cuh", "bm25_phrase.cuh", "column_kernels.cuh", "device_common.cuh",
                                                    "posting_format.hpp")] + [
     os.path.join(os.path.dirname(HERE), "include", "sdbg.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",

@@ -30,6 +30,7 @@
 #include "bm25_agg.cuh"
 #include "bm25_emit.cuh"
 #include "bm25_facet.cuh"
+#include "bm25_phrase.cuh"
 #include "bm25_sort.cuh"
 
 namespace sdbg {
@@ -64,6 +65,7 @@ struct CountParams {
   FacetSink facet;              // kFacet: the facet pass's sink
   AggSink agg;                  // kAgg: the aggregate pass's sink
   EmitSink emit;                // kEmit: the match scan's sink (work item .w = its count and base slot)
+  PhraseSink phrase;            // kPhrase: the phrase check and its top-k (work item .w = its output slot)
 };
 
 __device__ __forceinline__ uint32_t warp_min(uint32_t v) {
@@ -154,15 +156,21 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
 // gives each doc its ordinal, base[item.w] plus the matches of the item's earlier windows; the docs whose ordinal lies in
 // [offset[q], offset[q] + limit) go to their row of P.emit.out, unscored. An item whose ordinals miss the page exits
 // before it decodes anything, and an item stops after the window that fills the page.
+// kPhrase (with kAnd): the phrase check (bm25_phrase.cuh). Every doc that survives the conjunction, the exclusions, the
+// deleted docs and the filter chain is probed in each slot's list for its positions; a doc of phrase frequency 0 is
+// dropped, the others are counted and, with P.phrase.cap, scored from their phrase frequency and kept in a buffer of
+// P.phrase.cap keys in dynamic shared memory as the sorted scan keeps its keys; the item's k best go to slot item.w.
 // The sinks take kGroups queries: the groups narrow `acc` before the sink reads the column, and the bit-sliced counter
 // planes follow the sink's region of dynamic shared memory (16 * cap B, 4 * span B or agg_cells_bytes(span), rounded up
 // to 16 B).
-template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false, bool kAgg = false, bool kEmit = false>
+template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false, bool kAgg = false, bool kEmit = false,
+          bool kPhrase = false>
 __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
   static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
   static_assert(!(kFacet && kSort), "the facet pass has its own sink");
   static_assert(!(kAgg && (kSort || kFacet)), "the aggregate pass has its own sink");
   static_assert(!(kEmit && (kSort || kFacet || kAgg)), "the match scan has its own sink");
+  static_assert(!kPhrase || (kAnd && !kSort && !kFacet && !kAgg && !kEmit), "a phrase is checked on its terms' conjunction");
   __shared__ uint32_t acc[kCountWords];
   __shared__ uint32_t tmp[kAnd || kGroups ? kCountWords : 1];
   __shared__ uint32_t stage[kCountWarps][128];
@@ -174,7 +182,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   __shared__ uint32_t s_gend[kGroups ? kMaxQueryTerms : 1];
   __shared__ uint32_t s_ws, s_done;
   __shared__ unsigned long long s_sum[kCountWarps];
-  __shared__ unsigned long long s_thr[1];   // kSort: this item's best known k-th hi
+  __shared__ unsigned long long s_thr[1];   // kSort: this item's best known k-th hi (kPhrase: k-th key)
   __shared__ uint32_t s_fill[1];  // kSort: keys in the buffer (kFacet: NULL keys)
   // the window's zones that hold docs that can count: not dead for the filter chain and (kSort) able to reach s_thr;
   // the zones where the chain holds for every row; (kSort) the zones that can reach s_thr
@@ -226,6 +234,10 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
     for (uint32_t i = tid; i < 2u * P.sort.cap; i += kCountThreads) sort_buf[i] = 0ull;
     if (tid == 0) { s_thr[0] = 0ull; s_fill[0] = 0u; }
   }
+  if constexpr (kPhrase) {
+    for (uint32_t i = tid; i < 2u * P.phrase.cap; i += kCountThreads) sort_buf[i] = 0ull;
+    if (tid == 0) { s_thr[0] = P.phrase.cap ? P.phrase.thr[q] : 0ull; s_fill[0] = 0u; }
+  }
   if constexpr (kFacet) {
     for (uint32_t i = tid; i < P.facet.span; i += kCountThreads) bins[i] = 0u;
     if (tid == 0) s_fill[0] = 0u;
@@ -250,6 +262,9 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       s_ws = (nxt >> kCountWindowLog) << kCountWindowLog;
       if constexpr (kSort) {
         if (P.sort.thr) s_thr[0] = max(s_thr[0], *reinterpret_cast<volatile unsigned long long*>(P.sort.thr + q));
+      }
+      if constexpr (kPhrase) {
+        if (P.phrase.cap) s_thr[0] = max(s_thr[0], *reinterpret_cast<volatile unsigned long long*>(P.phrase.thr + q));
       }
     }
     __syncthreads();
@@ -397,7 +412,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       run_lists(n_pos, n_lists, acc, true, true);
       __syncthreads();
     }
-    if (live && !kSort && !(kEmit && P.emit.base)) {
+    if (live && !kSort && !kPhrase && !(kEmit && P.emit.base)) {
       const uint32_t wbase = ws >> 5;
       for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
         uint32_t v = acc[i];
@@ -468,6 +483,41 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
         }
       }
     }
+    if constexpr (kPhrase) {
+      if (live) {
+        const PhraseSink& F = P.phrase;
+        const uint32_t wbase = ws >> 5, cap = F.cap, s0 = F.slot_off[q], ns = F.slot_off[q + 1] - s0;
+        unsigned long long* hi = sort_buf;
+        unsigned long long* lo = sort_buf + cap;
+        for (uint32_t base = 0; base < kCountWords; base += kCountThreads) {   // uniform trip count
+          const uint32_t i = base + tid;
+          uint32_t v = acc[i];
+          if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
+          v = chain_bits(v, i);
+          for (;;) {   // a full buffer is cut to the k best and the remaining bits go on
+            const unsigned long long thr = s_thr[0];
+            for (; v; v &= v - 1u) {
+              const uint32_t doc = ws + 32u * i + (__ffs(v) - 1u);
+              const uint32_t f = phrase_freq(P.seg, F, s0, ns, doc);
+              if (!f) continue;
+              if (cap) {
+                const unsigned long long key = phrase_key(P.seg, F, q, doc, f);
+                if (key > thr) {
+                  const uint32_t slot = atomicAdd(&s_fill[0], 1u);
+                  if (slot >= cap) break;   // this bit is checked again after the cut
+                  hi[slot] = key;
+                }
+              }
+              ++count;
+            }
+            if (!cap || !__syncthreads_or(v != 0u)) break;
+            const unsigned long long kth = sort_select(hi, lo, cap, F.k, &s_fill[0]);
+            if (tid == 0 && kth > s_thr[0]) { s_thr[0] = kth; atomicMax(F.thr + q, kth); }
+            __syncthreads();
+          }
+        }
+      }
+    }
     }   // !skip
     __syncthreads();   // acc / tmp / cursors (kEmit: s_sum) are rewritten by the next window
     if constexpr (kEmit) {
@@ -514,6 +564,17 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   }
   if constexpr (kEmit) {
     if (P.emit.base) return;
+  }
+  if constexpr (kPhrase) {
+    if (P.phrase.cap) {
+      const unsigned long long kth = sort_select(sort_buf, sort_buf + P.phrase.cap, P.phrase.cap, P.phrase.k, &s_fill[0]);
+      const uint32_t n = s_fill[0];
+      for (uint32_t i = tid; i < n; i += kCountThreads) P.phrase.out[size_t(item.w) * P.phrase.k + i] = sort_buf[i];
+      if (tid == 0) {
+        P.phrase.out_n[item.w] = n;
+        if (kth) atomicMax(P.phrase.thr + q, kth);
+      }
+    }
   }
   count = warp_sum64(count);
   if (lane == 0) s_sum[warp] = count;

@@ -123,6 +123,31 @@ __device__ __forceinline__ unsigned long long sort_select(unsigned long long* hi
   return kth;
 }
 
+// Gathers the keys of query q's work items (slots[slot_off[q] .. slot_off[q + 1]), keys_n[slot] keys each, load(slot, i)
+// the i-th as {hi, lo}) into hi / lo and keeps the k best (sort_select); *fill ends at their number. Whole CTA; the
+// buffer of cap >= 2k slots is zeroed first.
+template <class Load>
+__device__ __forceinline__ void merge_item_keys(unsigned long long* hi, unsigned long long* lo, uint32_t cap, uint32_t k, uint32_t q,
+                                                const uint32_t* slot_off, const uint32_t* slots, const uint32_t* keys_n,
+                                                uint32_t* fill, Load load) {
+  for (uint32_t i = threadIdx.x; i < cap; i += blockDim.x) { hi[i] = 0ull; lo[i] = 0ull; }
+  if (threadIdx.x == 0) *fill = 0u;
+  __syncthreads();
+  for (uint32_t si = slot_off[q]; si < slot_off[q + 1]; ++si) {
+    const uint32_t slot = slots[si], n = keys_n[slot];
+    if (*fill + n > cap) sort_select(hi, lo, cap, k, fill);   // n <= k and cap >= 2k: room after a select
+    const uint32_t f = *fill;
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+      const ulonglong2 v = load(slot, i);
+      hi[f + i] = v.x; lo[f + i] = v.y;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *fill = f + n;
+    __syncthreads();
+  }
+  sort_select(hi, lo, cap, k, fill);
+}
+
 // One row of sdbg_sort_hit.
 struct SortHitDev {
   long long value;
@@ -155,22 +180,8 @@ __global__ void __launch_bounds__(256) sort_merge_kernel(SortMergeParams P) {
   unsigned long long* hi = sm_keys;
   unsigned long long* lo = sm_keys + P.cap;
   const uint32_t q = blockIdx.x, k = P.k, cap = P.cap;
-  for (uint32_t i = threadIdx.x; i < cap; i += blockDim.x) { hi[i] = 0ull; lo[i] = 0ull; }
-  if (threadIdx.x == 0) s_fill = 0u;
-  __syncthreads();
-  for (uint32_t si = P.slot_off[q]; si < P.slot_off[q + 1]; ++si) {
-    const uint32_t slot = P.slots[si], n = P.keys_n[slot];
-    if (s_fill + n > cap) sort_select(hi, lo, cap, k, &s_fill);   // n <= k and cap >= 2k: room after a select
-    const uint32_t f = s_fill;
-    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
-      const ulonglong2 v = P.keys[size_t(slot) * k + i];
-      hi[f + i] = v.x; lo[f + i] = v.y;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) s_fill = f + n;
-    __syncthreads();
-  }
-  sort_select(hi, lo, cap, k, &s_fill);
+  merge_item_keys(hi, lo, cap, k, q, P.slot_off, P.slots, P.keys_n, &s_fill,
+                  [&](uint32_t slot, uint32_t i) { return P.keys[size_t(slot) * k + i]; });
   const uint32_t n = s_fill;
   for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
     const uint32_t ord = ~static_cast<uint32_t>(lo[i]);

@@ -115,6 +115,9 @@ struct sdbg_segment {
   void* d_blocks = nullptr;
   void* d_anchor = nullptr;
   void* d_blkmax = nullptr;
+  // positions (sdbg_stage_positions, bm25_phrase.cuh): per block + sentinel a u64 base into d_pos; null: not staged
+  void* d_pos_base = nullptr;
+  void* d_pos = nullptr;
   std::vector<uint32_t> term_blk_begin, term_docs;
   std::vector<MaxPair> term_max;
   std::vector<uint8_t> term_probe;
@@ -327,6 +330,11 @@ extern "C" int sdbg_segment_create(sdbg_ctx* c, uint32_t docs_count, sdbg_segmen
 }
 
 namespace {
+void free_positions(sdbg_segment* s) {   // they index the posting blocks: restaging the postings drops them
+  if (s->d_pos_base) cudaFree(s->d_pos_base);
+  if (s->d_pos) cudaFree(s->d_pos);
+  s->d_pos_base = s->d_pos = nullptr;
+}
 void free_postings(sdbg_segment* s) {
   if (s->d_arena) cudaFree(s->d_arena);
   if (s->d_blocks) cudaFree(s->d_blocks);
@@ -334,6 +342,7 @@ void free_postings(sdbg_segment* s) {
   s->d_anchor = nullptr;
   if (s->d_blkmax) cudaFree(s->d_blkmax);
   s->d_arena = s->d_blocks = s->d_blkmax = nullptr;
+  free_positions(s);
 }
 void free_column(ColumnObj& c) {
   if (c.d_zone) { cudaFree(c.d_zone); c.d_zone = nullptr; }
@@ -452,6 +461,84 @@ extern "C" int sdbg_stage_postings(sdbg_segment* s, const uint8_t* doc_file, siz
     if (terms[t].docs_count && sp.blocks[sp.term_blk_begin[t + 1] - 1].last_doc > s->n_docs)
       return fail(s->ctx, SDBG_EFORMAT, "doc id beyond segment size");
   return upload_postings(s, sp);
+}
+
+extern "C" int sdbg_stage_positions(sdbg_segment* s, const uint32_t* positions, const uint64_t* term_pos_off, size_t n_terms) {
+  if (!s) return SDBG_EINVAL;
+  sdbg_ctx* c = s->ctx;
+  if (!s->d_blocks) return fail(c, SDBG_EINVAL, "stage the postings before the positions");
+  if (!term_pos_off || n_terms + 1 != s->term_blk_begin.size()) return fail(c, SDBG_EINVAL, "n_terms differs from the staged term count");
+  for (size_t t = 0; t < n_terms; ++t)
+    if (term_pos_off[t + 1] < term_pos_off[t]) return fail(c, SDBG_EINVAL, "term_pos_off must be non-decreasing");
+  const uint64_t n_pos = term_pos_off[n_terms] - term_pos_off[0];
+  if (n_pos && !positions) return fail(c, SDBG_EINVAL, "positions is NULL");
+  CU(c, cudaSetDevice(c->device));
+  const uint64_t nb = s->n_blocks;
+  const unsigned grid = unsigned(std::max<uint64_t>(1, (nb * 32 + 255) / 256));
+  // per block its frequency sum (device) and its length (descriptors)
+  std::vector<unsigned long long> fsum(nb);
+  std::vector<BlockDesc> desc(nb);
+  DevBuf& b_sum = c->scratch[0];
+  if (int rc = ensure(c, b_sum, std::max<uint64_t>(nb, 1) * 8)) return rc;
+  if (nb) {
+    phrase_freq_sums_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const uint4*>(s->d_arena), static_cast<const uint4*>(s->d_blocks), nb,
+                                                         static_cast<unsigned long long*>(b_sum.p));
+    ++c->launches;
+    CU(c, cudaGetLastError());
+    CU(c, cudaMemcpyAsync(fsum.data(), b_sum.p, nb * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaMemcpyAsync(desc.data(), s->d_blocks, nb * sizeof(BlockDesc), cudaMemcpyDeviceToHost, c->stream));
+  }
+  CU(c, cudaStreamSynchronize(c->stream));
+  // src_off: each block's first position in `positions`; base: its region in the arena (prefixes, then positions)
+  std::vector<unsigned long long> src_off(std::max<uint64_t>(nb, 1)), base(nb + 1);
+  unsigned long long at = 0;
+  for (size_t t = 0; t < n_terms; ++t) {
+    unsigned long long got = 0;
+    for (uint32_t g = s->term_blk_begin[t]; g < s->term_blk_begin[t + 1]; ++g) {
+      if (fsum[g] > 0xFFFFFFFFull) return fail(c, SDBG_EFORMAT, "more than 2^32 - 1 positions in one posting block");
+      src_off[g] = term_pos_off[t] - term_pos_off[0] + got;
+      got += fsum[g];
+      base[g] = at;
+      at += ((desc[g].packed >> 12) & 127u) + 1u + fsum[g];
+    }
+    if (got != term_pos_off[t + 1] - term_pos_off[t])
+      return fail(c, SDBG_EFORMAT, "a term's position count differs from the sum of its postings' frequencies");
+  }
+  base[nb] = at;
+  void* d_base = nullptr; void* d_pos = nullptr; void* d_src = nullptr; void* d_src_off = nullptr;
+  auto cleanup = [&]() { for (void* p : {d_base, d_pos, d_src, d_src_off}) if (p) cudaFree(p); };
+  auto run = [&]() -> int {
+    CU(c, cudaMalloc(&d_base, (nb + 1) * 8));
+    CU(c, cudaMalloc(&d_pos, std::max<unsigned long long>(at, 1) * 4));
+    CU(c, cudaMalloc(&d_src, std::max<uint64_t>(n_pos, 1) * 4));
+    CU(c, cudaMalloc(&d_src_off, src_off.size() * 8));
+    CU(c, cudaMemcpyAsync(d_base, base.data(), (nb + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(d_src_off, src_off.data(), src_off.size() * 8, cudaMemcpyHostToDevice, c->stream));
+    if (n_pos) CU(c, cudaMemcpyAsync(d_src, positions + term_pos_off[0], n_pos * 4, cudaMemcpyHostToDevice, c->stream));
+    unsigned int* d_bad = static_cast<unsigned int*>(b_sum.p);
+    CU(c, cudaMemsetAsync(d_bad, 0, 4, c->stream));
+    if (nb) {
+      phrase_fill_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const uint4*>(s->d_arena), static_cast<const uint4*>(s->d_blocks), nb,
+                                                      static_cast<const unsigned long long*>(d_base),
+                                                      static_cast<const unsigned long long*>(d_src_off), static_cast<const uint32_t*>(d_src),
+                                                      static_cast<uint32_t*>(d_pos), d_bad);
+      ++c->launches;
+      CU(c, cudaGetLastError());
+    }
+    unsigned int bad = 0;
+    CU(c, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    if (bad) return fail(c, SDBG_EFORMAT, "positions do not ascend strictly within a posting");
+    return SDBG_OK;
+  };
+  const int rc = run();
+  cudaFree(d_src); cudaFree(d_src_off);
+  d_src = d_src_off = nullptr;
+  if (rc) { cleanup(); return rc; }
+  free_positions(s);
+  s->d_pos_base = d_base;
+  s->d_pos = d_pos;
+  return SDBG_OK;
 }
 
 extern "C" int sdbg_stage_norms(sdbg_segment* s, const uint8_t* bytes, size_t n, const sdbg_norm_rg* rgs, size_t n_rg) {
@@ -1942,6 +2029,9 @@ int topk_batch_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdb
   });
 }
 
+int topk_hits_to_host(sdbg_segment* const* segs, size_t n_segs, const TopkDevOut& dev, size_t nq, uint32_t k, sdbg_hit* out,
+                      uint32_t* n_out, uint64_t* total_matches);
+
 // The host top-k entries after topk_args and their batch (B): runs it into the call's region in c->pass[0]
 // (topk_region, topk_batch_run), and copies it back (topk_to_host) with each ordinal decoded into {segment, doc}.
 int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_bm25_term>& B, float k1, float b,
@@ -1953,6 +2043,13 @@ int topk_batch_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sd
   if (int rc = ensure(c, c->pass[0], nq * (size_t(k) * 8 + 12))) return rc;
   const TopkDevOut dev = topk_region(c->pass[0].p, nq, k);
   if (int rc = topk_batch_run(segs, n_segs, B, k1, b, filt, k, threshold_in, dev)) return rc;
+  return topk_hits_to_host(segs, n_segs, dev, nq, k, out, n_out, total_matches);
+}
+
+// topk_to_host for the local entries: each ordinal decoded into {segment, doc}.
+int topk_hits_to_host(sdbg_segment* const* segs, size_t n_segs, const TopkDevOut& dev, size_t nq, uint32_t k, sdbg_hit* out,
+                      uint32_t* n_out, uint64_t* total_matches) {
+  sdbg_ctx* c = segs[0]->ctx;
   std::vector<uint64_t> bases(n_segs);   // the first ordinal of each segment
   uint64_t ord0 = 0;
   for (size_t si = 0; si < n_segs; ++si) { bases[si] = ord0; ord0 += segs[si]->n_docs; }
@@ -2242,12 +2339,24 @@ uint32_t count_planes(uint32_t max_min) {
 }
 
 using CountKernel = void (*)(CountParams);
-enum class CountMode { count, sort, facet, agg, emit };
+enum class CountMode { count, sort, facet, agg, emit, phrase };
 
 // The match scan's part of a count_run call: the page of each query of the plan's batch.
 struct EmitJob {
   uint32_t limit;
   const unsigned long long* offset;   // host [nq]: the first ordinal of each query's page
+};
+
+// The phrase pass's part of a count_run call (the plan's batch is the AND of each phrase's distinct terms): query q's
+// slots are slot_term / slot_rel [slot_off[q] .. slot_off[q + 1]). k == 0: count only; else the top-k, scored with
+// consts[q] = {c0, norm_const, norm_length} and seeded with the key of threshold_in.
+struct PhraseJob {
+  const uint32_t* slot_term = nullptr;
+  const uint32_t* slot_rel = nullptr;
+  const uint32_t* slot_off = nullptr;
+  std::vector<float4> consts;
+  uint32_t k = 0;
+  unsigned long long seed = 0;
 };
 
 // One pass of count_run: its mode and that mode's parameters. job_prepare checks them and fills the sinks, once per call.
@@ -2257,6 +2366,7 @@ struct CountJob {
   FacetJob facet;   // CountMode::facet
   AggJob agg;       // CountMode::agg
   EmitJob emit;     // CountMode::emit
+  PhraseJob phrase; // CountMode::phrase
 
   // Bytes per query of count_run's per-query arrays {counts, bins, nulls} (CountOut); rank: the sorted scan's rank form.
   std::array<size_t, 3> rows(bool rank) const {
@@ -2355,6 +2465,7 @@ struct CountPlan {
          bm25_count_kernel<true, false, false, false, true>, bm25_count_kernel<true, false, false, false, false, true>},
         {bm25_count_kernel<false, true>, bm25_count_kernel<false, true, true>, bm25_count_kernel<false, true, false, true>,
          bm25_count_kernel<false, true, false, false, true>, bm25_count_kernel<false, true, false, false, false, true>}};
+    if (mode == CountMode::phrase) return {bm25_count_kernel<true, false, false, false, false, false, true>, mode_bytes};
     const int shape = Q.term_grp ? 2 : Q.kind == SDBG_QUERY_AND ? 1 : 0;
     return {kernels[shape][int(mode)], mode_bytes + size_t(planes) * kCountWords * 4u};
   }
@@ -2504,6 +2615,102 @@ CountPlan count_plan(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<
   return pl;
 }
 
+// The item slots of the plan's staging h: each work item's output slot is its index (work item .w), and query q's items
+// are slots[slot_off[q] .. slot_off[q + 1]) in work order, i.e. by segment, then first window.
+void item_slots(const CountPlan& pl, char* h, size_t slot_off_pos, size_t slots_pos) {
+  const size_t nq = pl.Q.nq, total = pl.items;
+  auto* hw = reinterpret_cast<uint4*>(h + pl.work_pos);
+  auto* h_slot_off = reinterpret_cast<uint32_t*>(h + slot_off_pos);
+  auto* h_slots = reinterpret_cast<uint32_t*>(h + slots_pos);
+  std::fill(h_slot_off, h_slot_off + nq + 1, 0u);
+  for (uint32_t i = 0; i < total; ++i) { hw[i].w = i; ++h_slot_off[hw[i].x + 1]; }
+  for (size_t q = 0; q < nq; ++q) h_slot_off[q + 1] += h_slot_off[q];
+  std::vector<uint32_t> fillq(h_slot_off, h_slot_off + nq);
+  for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
+}
+
+// The phrase pass of count_run (CountMode::phrase) over a plan with work items: bm25_count_kernel<kAnd, .., kPhrase> per
+// segment, the count into out.counts; with a top-k (job.k) each item writes its k best keys to its own slot, then
+// phrase_merge_kernel keeps each query's k best in out.bins (u64 keys [nq][k]) with their number in out.nulls (u32 [nq]).
+// Host staging: the plan's, then [slot_off | slots | query slot offsets | per segment the slots' lists | consts].
+int phrase_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt, const PhraseJob& job,
+               const CountOut& out) {
+  sdbg_ctx* c = segs[0]->ctx;
+  const size_t nq = pl.Q.nq, total = pl.items;
+  const uint32_t k = job.k, n_slots = job.slot_off[nq];
+  uint32_t cap = 0;
+  if (k) { uint32_t kp = 1; while (kp < k) kp <<= 1; cap = std::max(256u, 2u * kp); }
+  const size_t slot_off_pos = pl.staged;
+  const size_t slots_pos = slot_off_pos + pl.off_bytes;
+  const size_t poff_pos = slots_pos + total * 4;
+  const size_t lists_pos = (poff_pos + pl.off_bytes + 15) & ~size_t(15);
+  const size_t consts_pos = lists_pos + n_segs * n_slots * sizeof(uint4);
+  const size_t bytes = consts_pos + nq * sizeof(float4);
+  std::vector<char> staging(bytes);
+  char* h = staging.data();
+  pl.write(h);
+  item_slots(pl, h, slot_off_pos, slots_pos);
+  std::memcpy(h + poff_pos, job.slot_off, pl.off_bytes);
+  auto* h_lists = reinterpret_cast<uint4*>(h + lists_pos);   // slots before job.slot_off[0] belong to no query: left 0
+  for (size_t si = 0; si < n_segs; ++si)
+    for (uint32_t i = job.slot_off[0]; i < n_slots; ++i) {
+      const uint2 l = excl_list(segs[si], job.slot_term[i]);
+      h_lists[si * n_slots + i] = make_uint4(l.x, l.y, job.slot_rel[i], 0u);
+    }
+  if (k) std::memcpy(h + consts_pos, job.consts.data(), nq * sizeof(float4));
+  // device scratch: [item keys [items][k] | item key counts | thresholds [nq]]
+  const size_t keys_n_pos = total * size_t(k) * 8;
+  const size_t thr_pos = (keys_n_pos + total * 4 + 15) & ~size_t(15);
+  DevBuf& b_desc = c->scratch[0]; DevBuf& b_out = c->scratch[1];
+  if (int rc = ensure(c, b_desc, bytes)) return rc;
+  if (int rc = k ? ensure(c, b_out, thr_pos + nq * 8) : SDBG_OK) return rc;
+  char* d = static_cast<char*>(b_desc.p);
+  char* o = static_cast<char*>(b_out.p);
+  auto* thr = reinterpret_cast<unsigned long long*>(o + thr_pos);
+  CU(c, cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, c->stream));
+  if (k) {
+    fill_u64_kernel<<<64, 256, 0, c->stream>>>(thr, nq, job.seed);
+    ++c->launches;
+  }
+  const auto [kernel, smem] = pl.kernel(CountMode::phrase, size_t(cap) * 16);
+  CU(c, fit_dynamic_smem(kernel, smem));
+  std::vector<ChainDev> chains(n_segs);
+  if (int rc = filter_chains(segs, n_segs, filt, chains.data())) return rc;
+  size_t first = 0;
+  uint64_t base = 0;   // ordinals of the earlier segments (at most 2^32 - 2 docs per call)
+  for (size_t si = 0; si < n_segs; ++si) {
+    const size_t n = pl.seg_work[si].size();
+    CountParams P;
+    pl.params(d, segs[si], si, first, chains[si], &P);
+    P.counts = static_cast<unsigned long long*>(out.counts);
+    PhraseSink& F = P.phrase;
+    F.pos_base = static_cast<const unsigned long long*>(segs[si]->d_pos_base);
+    F.pos = static_cast<const uint32_t*>(segs[si]->d_pos);
+    F.slots = reinterpret_cast<const uint4*>(d + lists_pos) + si * n_slots;
+    F.slot_off = reinterpret_cast<const uint32_t*>(d + poff_pos);
+    F.consts = reinterpret_cast<const float4*>(d + consts_pos);
+    F.ordinal_base = uint32_t(base);
+    F.k = k; F.cap = cap; F.thr = thr;
+    F.out = reinterpret_cast<unsigned long long*>(o);
+    F.out_n = reinterpret_cast<uint32_t*>(o + keys_n_pos);
+    base += segs[si]->n_docs;
+    first += n;
+    if (!n) continue;
+    kernel<<<unsigned(n), kCountThreads, smem, c->stream>>>(P);
+    ++c->launches;
+  }
+  CU(c, cudaGetLastError());
+  if (!k) return SDBG_OK;
+  CU(c, fit_dynamic_smem(phrase_merge_kernel, size_t(cap) * 16));
+  phrase_merge_kernel<<<unsigned(nq), 256, size_t(cap) * 16, c->stream>>>(
+      reinterpret_cast<const unsigned long long*>(o), reinterpret_cast<const uint32_t*>(o + keys_n_pos),
+      reinterpret_cast<const uint32_t*>(d + slot_off_pos), reinterpret_cast<const uint32_t*>(d + slots_pos), k, cap,
+      static_cast<unsigned long long*>(out.bins), static_cast<uint32_t*>(out.nulls));
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  return SDBG_OK;
+}
+
 // Queues a pass over its plan into out. A count pass first sets out.counts to the single-term shortcut's counts. The
 // sorted scan launches per segment its seed items first (all segments), then the rest, each item writing its k best to
 // its own slot (its index in the work array); then sort_merge_kernel per query, and for a rank sort_dist_rows_kernel.
@@ -2515,10 +2722,11 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
               const CountOut& out) {
   sdbg_ctx* c = segs[0]->ctx;
   const size_t nq = pl.Q.nq, total = pl.items;
-  const bool sort = job.mode == CountMode::sort, emit = job.mode == CountMode::emit;
+  const bool sort = job.mode == CountMode::sort, emit = job.mode == CountMode::emit, phrase = job.mode == CountMode::phrase;
   if (std::any_of(pl.host.begin(), pl.host.end(), [](uint64_t v) { return v != 0; }))   // else out.counts is zero already
     CU(c, cudaMemcpyAsync(out.counts, pl.host.data(), nq * 8, cudaMemcpyHostToDevice, c->stream));
   if (!total && !sort) return SDBG_OK;
+  if (phrase) return phrase_run(segs, n_segs, pl, filt, job.phrase, out);
   const SortJob& J = job.sort;
   const uint32_t k = J.k, cap = sort ? J.sink[0].cap : 0u;
   // host staging: the plan's, then for the sorted scan [slot_off | slots | segments], for the match scan [slot_off |
@@ -2530,16 +2738,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
   std::vector<char> staging(bytes);
   char* h = staging.data();
   pl.write(h);
-  if (sort || emit) {   // each query's items in work order, i.e. by segment, then first window
-    auto* hw = reinterpret_cast<uint4*>(h + pl.work_pos);
-    auto* h_slot_off = reinterpret_cast<uint32_t*>(h + slot_off_pos);
-    auto* h_slots = reinterpret_cast<uint32_t*>(h + slots_pos);
-    std::fill(h_slot_off, h_slot_off + nq + 1, 0u);
-    for (uint32_t i = 0; i < total; ++i) { hw[i].w = i; ++h_slot_off[hw[i].x + 1]; }
-    for (size_t q = 0; q < nq; ++q) h_slot_off[q + 1] += h_slot_off[q];
-    std::vector<uint32_t> fillq(h_slot_off, h_slot_off + nq);
-    for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
-  }
+  if (sort || emit) item_slots(pl, h, slot_off_pos, slots_pos);
   if (emit) std::memcpy(h + segs_pos, job.emit.offset, nq * 8);
   if (sort) {
     auto* h_segs = reinterpret_cast<SortSegDev*>(h + segs_pos);
@@ -2788,6 +2987,111 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
   const PassBatch<uint32_t> B(segs, n_segs, QueryBatch<uint32_t>{kind, terms, term_off, nq, excl_terms, excl_off, nullptr}, filt);
   CountJob job{CountMode::count, {}, {}, {}};
   return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
+}
+
+namespace {
+// A batch of phrases (sdbg_phrase_*_batch), checked before anything is queued: query q's slots are terms / rel_pos
+// [phrase_off[q] .. phrase_off[q + 1]); `ids` / `id_off` hold each phrase's distinct term ids, in slot order, which run as
+// the AND the phrase check starts from.
+struct PhraseBatch {
+  int rc = SDBG_OK;
+  std::vector<uint32_t> ids, id_off, rel;
+
+  PhraseBatch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* phrase_off,
+              size_t nq) {
+    if (!segs || !n_segs || !segs[0] || !nq || !phrase_off) { rc = SDBG_EINVAL; return; }
+    sdbg_ctx* c = segs[0]->ctx;
+    for (size_t q = 0; q < nq && !rc; ++q) {
+      if (phrase_off[q + 1] < phrase_off[q]) rc = fail(c, SDBG_EINVAL, "phrase_off must be non-decreasing");
+      else if (phrase_off[q + 1] == phrase_off[q]) rc = fail(c, SDBG_EINVAL, "empty phrase");
+    }
+    for (size_t q = 0; q < nq && !rc; ++q)
+      if (phrase_off[q + 1] - phrase_off[q] > kMaxPhraseSlots) rc = fail(c, SDBG_EUNSUPPORTED, "a phrase holds 1..16 slots");
+    if (!rc && !terms) rc = fail(c, SDBG_EINVAL, "terms is NULL");
+    if (rc) return;
+    id_off.assign(1, 0u);
+    rel.resize(phrase_off[nq]);
+    for (size_t q = 0; q < nq; ++q) {
+      const uint32_t s0 = phrase_off[q], s1 = phrase_off[q + 1];
+      for (uint32_t i = s0; i < s1; ++i) {
+        rel[i] = rel_pos ? rel_pos[i] : i - s0;
+        if (i == s0 ? rel[i] != 0u : rel[i] <= rel[i - 1]) {
+          rc = fail(c, SDBG_EINVAL, "rel_pos must start at 0 and increase");
+          return;
+        }
+        if (std::find(ids.begin() + id_off.back(), ids.end(), terms[i]) == ids.end()) ids.push_back(terms[i]);
+      }
+      id_off.push_back(uint32_t(ids.size()));
+    }
+  }
+
+  QueryBatch<uint32_t> conj(size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off) const {
+    return {SDBG_QUERY_AND, ids.data(), id_off.data(), nq, excl_terms, excl_off, nullptr};
+  }
+};
+
+// Every segment holds positions (sdbg_stage_positions).
+int phrase_positions_staged(sdbg_segment* const* segs, size_t n_segs) {
+  for (size_t si = 0; si < n_segs; ++si)
+    if (!segs[si]->d_pos) return fail(segs[0]->ctx, SDBG_ENOTFOUND, "segment has no staged positions");
+  return SDBG_OK;
+}
+}  // namespace
+
+extern "C" int sdbg_phrase_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                       const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
+                                       const sdbg_col_pred* filt, uint64_t* counts) {
+  if (!counts) return SDBG_EINVAL;
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  if (PB.rc) return PB.rc;
+  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  if (B.rc) return B.rc;
+  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
+  CountJob job{CountMode::count, {}, {}, {}};
+  job.mode = CountMode::phrase;
+  job.phrase.slot_term = terms; job.phrase.slot_rel = PB.rel.data(); job.phrase.slot_off = phrase_off;
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
+}
+
+extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                      const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
+                                      const sdbg_bm25_term* phrase_stats, float k1, float b, const sdbg_col_pred* filt, uint32_t k,
+                                      float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
+  if (!out || !n_out || !phrase_stats) return SDBG_EINVAL;
+  if (int rc = topk_args(segs, n_segs, nq, k)) return rc;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  if (PB.rc) return PB.rc;
+  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  if (B.rc) return B.rc;
+  uint64_t ord = 0;
+  for (size_t si = 0; si < n_segs; ++si) ord += segs[si]->n_docs;
+  if (ord > kMaxDocId) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-2 docs per call");
+  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
+  CountJob job{CountMode::count, {}, {}, {}};
+  job.mode = CountMode::phrase;
+  PhraseJob& J = job.phrase;
+  J.slot_term = terms; J.slot_rel = PB.rel.data(); J.slot_off = phrase_off; J.k = k;
+  J.consts.resize(nq);
+  for (size_t q = 0; q < nq; ++q) {   // the scorer form of fill_qterm, with the phrase's statistics
+    sdbg_bm25_term t = phrase_stats[q];
+    t.term = terms[phrase_off[q]];
+    QTermDev d;
+    fill_qterm(segs[0], t, k1, b, d);
+    J.consts[q] = make_float4(d.c0, d.norm_const, d.norm_length, 0.f);
+  }
+  uint32_t thr_bits; std::memcpy(&thr_bits, &threshold_in, 4);
+  if (!(threshold_in >= 0.f)) thr_bits = 0;  // negative / NaN seeds accept every positive score, as the top-k entries
+  J.seed = (static_cast<unsigned long long>(thr_bits) << 32) | 0xFFFFFFFFull;
+  if (int rc = job_prepare(c, segs, n_segs, job)) return rc;
+  if (int rc = ensure(c, c->pass[0], nq * (size_t(k) * 8 + 12))) return rc;
+  const TopkDevOut dev = topk_region(c->pass[0].p, nq, k);
+  CU(c, cudaMemsetAsync(c->pass[0].p, 0, nq * (size_t(k) * 8 + 12), c->stream));
+  const CountPlan pl = count_plan(segs, n_segs, B.whole, B.total_excl, filt, job);
+  const CountOut o{dev.total, dev.keys, dev.n_out, nullptr, nullptr, -1};
+  if (int rc = count_run(segs, n_segs, pl, filt, job, o)) return rc;
+  return topk_hits_to_host(segs, n_segs, dev, nq, k, out, n_out, total_matches);
 }
 
 extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,

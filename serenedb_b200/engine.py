@@ -274,6 +274,14 @@ class Segment:
         N.check(N.lib().sdbg_segment_set_wand_b(self._h, float(wand_b)), self.ctx._h)   # pruning only for scorers with this b
         self.term_docs = metas["docs_count"].astype(np.uint64)
 
+    def stage_positions(self, positions, term_pos_off):
+        """Term positions for phrase queries (sdbg_stage_positions), after stage_postings: term t's positions are
+        positions[term_pos_off[t]:term_pos_off[t + 1]], posting after posting, each posting's freq positions ascending."""
+        positions = np.ascontiguousarray(positions, dtype=np.uint32)
+        term_pos_off = np.ascontiguousarray(term_pos_off, dtype=np.uint64)
+        N.check(N.lib().sdbg_stage_positions(self._h, _ptr(positions), _ptr(term_pos_off), max(len(term_pos_off) - 1, 0)),
+                self.ctx._h)
+
     def stage_norms(self, norm_bytes, byte_width):
         norm_bytes = np.ascontiguousarray(norm_bytes, dtype=np.uint8)
         rg = N.NormRg(byte_width, self.n_docs, 0)
@@ -461,6 +469,19 @@ class IndexReader:
         return scorer.collect(self.docs_with_field, self.total_term_freq, int(self.docs_with_term[term]), term, boost)
 
 
+    def phrase_stats(self, scorer, terms, boost=1.0):
+        """The statistics of a phrase (collectors.cpp:116-128 restated): its terms' statistics with the idfs summed in
+        float32 in slot order, a repeated term counted once per slot; the first term's norm constants and `boost`."""
+        ts = [self.stats(scorer, t) for t in terms]
+        out = ts[0]
+        idf = np.float32(0)
+        for t in ts:
+            idf = np.float32(idf + np.float32(t.idf))
+        out.idf = float(idf)
+        out.boost = float(boost)
+        return out
+
+
 def _exclusions(exclude, nq):
     """Per-query excluded term ids -> (flat ids u32, offsets u32 [nq + 1]), or None when no query excludes anything."""
     if exclude is None:
@@ -555,6 +576,59 @@ def ExecuteCountBatch(reader, queries, kind, filt=None, exclude=None):
 def ExecuteCount(reader, query_terms, kind, filt=None, exclude=None):
     """ExecuteCountBatch for one query: its match count as an int."""
     return int(ExecuteCountBatch(reader, _one(query_terms), kind, filt, exclude=_one(exclude))[0])
+
+
+def _phrase_args(phrases, rel_pos, exclude):
+    """(terms, rel_pos, phrase_off, nq, excl_terms, excl_off) of the phrase entries. rel_pos: None (adjacent words), or
+    one list of relative positions (or None) per phrase."""
+    nq = len(phrases)
+    flat = np.ascontiguousarray([t for p in phrases for t in p], dtype=np.uint32)
+    off = np.zeros(nq + 1, np.uint32)
+    off[1:] = np.cumsum([len(p) for p in phrases])
+    rel = None
+    if rel_pos is not None:
+        if len(rel_pos) != nq:
+            raise ValueError("rel_pos needs one list (or None) per phrase")
+        rel = np.ascontiguousarray([r for p, rp in zip(phrases, rel_pos) for r in (range(len(p)) if rp is None else rp)],
+                                   dtype=np.uint32)
+    x = _exclusions(exclude, nq) or (None, None)
+    return (_ptr(flat) if len(flat) else None, _ptr(rel), _ptr(off), nq, _ptr(x[0]), _ptr(x[1]))
+
+
+def ExecutePhraseCountBatch(reader, phrases, rel_pos=None, filt=None, exclude=None):
+    """Count of exact phrase queries (`SELECT count(*) ... WHERE body @@ '"new york"'`, sdbg_phrase_count_batch): per
+    phrase (a list of term ids, a term may repeat), the docs over all segments where its terms occur at consecutive
+    positions (or at `rel_pos`), not deleted, passing `filt` and holding none of its `exclude` ids. Returns uint64[Q]."""
+    counts = np.zeros(len(phrases), np.uint64)
+    N.check(N.lib().sdbg_phrase_count_batch(_seg_array(reader.segments), len(reader.segments), *_phrase_args(phrases, rel_pos, exclude),
+                                            _ref(filt), _ptr(counts)), reader.segments[0].ctx._h)
+    return counts
+
+
+def ExecutePhraseCount(reader, phrase, rel_pos=None, filt=None, exclude=None):
+    """ExecutePhraseCountBatch for one phrase: its match count as an int."""
+    return int(ExecutePhraseCountBatch(reader, [list(phrase)], _one(rel_pos), filt, exclude=_one(exclude))[0])
+
+
+def ExecutePhraseTopKBatch(reader, phrases, scorer, k, rel_pos=None, filt=None, threshold=FLT_MIN, exclude=None, boost=1.0):
+    """Top-k of exact phrase queries (sdbg_phrase_topk_batch), scored by the phrase frequency with
+    IndexReader.phrase_stats. Returns (hits [Q, k] structured, n_out [Q], total_matches [Q]) as ExecuteTopKBatch."""
+    nq = len(phrases)
+    stats = (N.BM25Term * nq)(*[reader.phrase_stats(scorer, p, boost) for p in phrases])
+    hits = np.zeros((nq, k), HIT_DTYPE)
+    n_out = np.zeros(nq, np.uint32)
+    total = np.zeros(nq, np.uint64)
+    N.check(N.lib().sdbg_phrase_topk_batch(_seg_array(reader.segments), len(reader.segments), *_phrase_args(phrases, rel_pos, exclude),
+                                           stats, scorer.k, scorer.b, _ref(filt), int(k), float(threshold), _ptr(hits),
+                                           _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
+    return hits, n_out, total
+
+
+def ExecutePhraseTopK(reader, phrase, scorer, k, rel_pos=None, filt=None, threshold=FLT_MIN, exclude=None, boost=1.0):
+    """ExecutePhraseTopKBatch for one phrase: (hits [n_out], total_matches)."""
+    hits, n_out, total = ExecutePhraseTopKBatch(reader, [list(phrase)], scorer, k, _one(rel_pos), filt, threshold,
+                                                _one(exclude), boost)
+    return hits[0, :n_out[0]], int(total[0])
 
 
 SORT_HIT_DTYPE = np.dtype([("value", "<i8"), ("doc", "<u4"), ("seg", "<u4"), ("is_null", "u1"), ("pad", "V7")])

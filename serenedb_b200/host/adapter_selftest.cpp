@@ -10,7 +10,8 @@
 // (GpuMatchAggScan, tests/test_gpu_match_aggregates.py). "chain" runs a pushed filter chain (SDBG_OP_AND_NEXT) through the
 // top-k, streaming and count adapters next to the same calls filtered by an indicator column of the chain
 // (tests/test_gpu_filter_chains.py). "scan" runs the Stream mode (GpuMatchScan) for flat, grouped and min-match queries
-// (tests/test_gpu_match_scan.py).
+// (tests/test_gpu_match_scan.py). "phrase" runs a phrase through the top-k and count adapters on a token corpus of its own
+// (tests/test_gpu_phrase.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -28,6 +29,78 @@ struct ListCollector final : irs::ScoreCollector {  // a trivial ScoreCollector:
   void AddWindow(const irs::score_t*, const uint64_t*, irs::doc_id_t, size_t, bool) override {}
   void AddDocs(const irs::doc_id_t* d, size_t n, const irs::score_t* s) override { for (size_t i = 0; i < n; ++i) docs.push_back({s[i], d[i], 0}); }
 };
+// "phrase": a by_phrase through GpuTopKIterator (top-50) and GpuCountScan on a token corpus of its own, which
+// tests/test_gpu_phrase.py rebuilds: doc i (1-based) has 1 + r % 16 tokens, each token r % 6, r the next value of
+// r = r * 1664525 + 1013904223 (mod 2^32) >> 16 from state 12345, docs in order. Norms are the doc lengths. One line per
+// phrase: its slots and positions, the excluded term, the hits, total_matches and the count.
+int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs) {
+  uint32_t state = 12345u;
+  auto next = [&]() { state = state * 1664525u + 1013904223u; return state >> 16; };
+  constexpr uint32_t kVocab = 6;
+  std::vector<std::vector<uint32_t>> docs(kVocab), freqs(kVocab), pos(kVocab);
+  std::vector<uint32_t> norms(n_docs);
+  uint64_t sum_len = 0;
+  for (uint32_t d = 1; d <= n_docs; ++d) {
+    const uint32_t len = 1 + next() % 16;
+    norms[d - 1] = len;
+    sum_len += len;
+    std::vector<std::vector<uint32_t>> at(kVocab);
+    for (uint32_t p = 0; p < len; ++p) at[next() % kVocab].push_back(p);
+    for (uint32_t t = 0; t < kVocab; ++t) {
+      if (at[t].empty()) continue;
+      docs[t].push_back(d); freqs[t].push_back(uint32_t(at[t].size()));
+      pos[t].insert(pos[t].end(), at[t].begin(), at[t].end());
+    }
+  }
+  sdbg_writer* w = nullptr;
+  sdbg_segment* seg = nullptr;
+  const uint8_t* doc_file = nullptr; const sdbg_term_meta* metas = nullptr;
+  size_t n_bytes = 0, n_terms = 0;
+  int rc = sdbg_writer_create(n_docs, 1, 0.75f, norms.data(), &w);
+  for (uint32_t t = 0; t < kVocab && !rc; ++t) rc = sdbg_writer_add_term(w, docs[t].data(), freqs[t].data(), uint32_t(docs[t].size()));
+  if (!rc) rc = sdbg_writer_finish(w, &doc_file, &n_bytes, &metas, &n_terms);
+  if (!rc) rc = sdbg_segment_create(ctx, n_docs, &seg);
+  if (!rc) rc = sdbg_stage_postings(seg, doc_file, n_bytes, metas, n_terms, 1);
+  std::vector<uint8_t> nb(norms.begin(), norms.end());
+  const sdbg_norm_rg rg{1, n_docs, 0};
+  if (!rc) rc = sdbg_stage_norms(seg, nb.data(), nb.size(), &rg, 1);
+  std::vector<uint32_t> flat;
+  std::vector<uint64_t> off(1, 0);
+  for (uint32_t t = 0; t < kVocab; ++t) { flat.insert(flat.end(), pos[t].begin(), pos[t].end()); off.push_back(flat.size()); }
+  if (!rc) rc = sdbg_stage_positions(seg, flat.data(), off.data(), kVocab);
+  if (w) sdbg_writer_destroy(w);
+  if (rc) { std::printf("{\"error\": %d}\n", rc); return 1; }
+  struct Case { std::vector<uint32_t> slots, rel, excl; };
+  const Case cases[] = {{{1, 0}, {0, 1}, {}}, {{2, 2, 4}, {0, 1, 3}, {5}}};
+  ListCollector col;
+  irs::ScoreFunction sf; irs::ColumnArgsFetcher fetcher;
+  for (const Case& cs : cases) {
+    std::vector<sdbg_bm25_term> terms(cs.slots.size());
+    for (size_t i = 0; i < terms.size(); ++i) {
+      sdbg_bm25_collect(n_docs, sum_len, docs[cs.slots[i]].size(), 1.2f, 0.75f, &terms[i]);
+      terms[i].term = cs.slots[i];
+    }
+    sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_AND, terms, 1.2f, 0.75f, 50, nullptr, cs.excl, {}, {}, cs.rel);
+    col.docs.clear();
+    it.Collect(sf, fetcher, col);
+    sdbg_host::GpuCountScan cnt({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, {}, {}, cs.rel);
+    duckdb::DataChunkMock out;
+    cnt.Scan(out);
+    std::printf("{\"slots\": [");
+    for (size_t i = 0; i < cs.slots.size(); ++i) std::printf("%s%u", i ? ", " : "", cs.slots[i]);
+    std::printf("], \"rel\": [");
+    for (size_t i = 0; i < cs.rel.size(); ++i) std::printf("%s%u", i ? ", " : "", cs.rel[i]);
+    std::printf("], \"excl\": [");
+    for (size_t i = 0; i < cs.excl.size(); ++i) std::printf("%s%u", i ? ", " : "", cs.excl[i]);
+    std::printf("], \"topk\": [");
+    for (size_t i = 0; i < col.docs.size(); ++i) std::printf("%s[%u, %.9g]", i ? ", " : "", col.docs[i].doc, double(col.docs[i].score));
+    std::printf("], \"total\": %llu, \"count\": %lld}\n", static_cast<unsigned long long>(it.total_matches()),
+                static_cast<long long>(out.count.empty() ? -1 : out.count[0]));
+  }
+  sdbg_segment_destroy(seg);
+  sdbg_destroy(ctx);
+  return 0;
+}
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -35,6 +108,7 @@ int main(int argc, char** argv) {
   sdbg_ctx* ctx = nullptr;
   int rc = sdbg_init(0, &ctx);
   if (rc != SDBG_OK) { std::printf("{\"error\": %d}\n", rc); return rc == SDBG_ENODEVICE ? 3 : 1; }
+  if (argc > 2 && std::string(argv[2]) == "phrase") return phrase_mode(ctx, n_docs);
   sdbg_segment* seg = nullptr;
   sdbg_segment_create(ctx, n_docs, &seg);
   std::vector<uint32_t> dc(8);

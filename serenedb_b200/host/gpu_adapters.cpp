@@ -24,6 +24,23 @@ const uint32_t* group_minimums(const std::vector<uint32_t>& mins, size_t n_group
   if (mins.size() != n_groups) throw GpuError(SDBG_EINVAL, "one minimum match count per OR group");
   return mins.data();
 }
+
+// A phrase's relative positions: one per slot and no OR groups (the library checks their order).
+void check_phrase(const std::vector<uint32_t>& phrase, size_t n_terms, bool groups) {
+  if (phrase.empty()) return;
+  if (phrase.size() != n_terms) throw GpuError(SDBG_EINVAL, "one phrase position per term");
+  if (groups) throw GpuError(SDBG_EUNSUPPORTED, "a phrase has no OR groups");
+}
+
+// The statistics of a phrase (collectors.cpp:116-128): the slots' idfs summed in float32 in slot order, a repeated term
+// once per slot; the first slot's norm constants and boost (the field's, shared by every slot).
+sdbg_bm25_term phrase_stats(const std::vector<sdbg_bm25_term>& slots) {
+  sdbg_bm25_term s = slots[0];
+  float idf = 0.f;
+  for (const sdbg_bm25_term& t : slots) idf += t.idf;
+  s.idf = idf;
+  return s;
+}
 }  // namespace
 
 FilterChain::FilterChain(const sdbg_col_pred* table_filter) {
@@ -34,10 +51,13 @@ FilterChain::FilterChain(const sdbg_col_pred* table_filter) {
 
 GpuTopKIterator::GpuTopKIterator(sdbg_segment* segment, int kind, std::vector<sdbg_bm25_term> terms, float k1, float b,
                                  uint32_t k, const sdbg_col_pred* table_filter, std::vector<uint32_t> excluded_terms,
-                                 std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)
+                                 std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
+                                 std::vector<uint32_t> phrase_positions)
     : seg_(segment), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)), groups_(std::move(group_sizes)),
-      group_min_(std::move(group_min_match)), k1_(k1), b_(b), k_(k), filter_(table_filter) {
+      group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)), k1_(k1), b_(b), k_(k), filter_(table_filter) {
   threshold_.value = FLT_MIN;  // doc_collector.hpp:102
+  check_phrase(phrase_, terms_.size(), !groups_.empty());
+  if (!phrase_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "phrases need k > 0: the streaming scan has no phrase form");
   // the streaming scan (sdbg_bm25_scan*) has no grouped form
   if (!groups_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "OR groups need k > 0: the streaming scan has no grouped form");
 }
@@ -69,7 +89,16 @@ void GpuTopKIterator::run() {
   uint32_t n = 0;
   float thr_out = 0;
   sdbg_segment* segs[1] = {seg_};
-  if (!groups_.empty()) {
+  if (!phrase_.empty()) {
+    std::vector<uint32_t> ids(terms_.size());
+    for (size_t i = 0; i < ids.size(); ++i) ids[i] = terms_[i].term;
+    const sdbg_bm25_term stats = phrase_stats(terms_);
+    const uint32_t phrase_off[2] = {0, uint32_t(ids.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
+    check(sdbg_phrase_topk_batch(segs, 1, ids.data(), phrase_.data(), phrase_off, 1, excluded_.data(), excl_off, &stats, k1_, b_,
+                                 filter_.data(), k_, threshold_.value, hits_.data(), &n, &total_),
+          "sdbg_phrase_topk_batch");
+    thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;
+  } else if (!groups_.empty()) {
     const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
     const uint32_t query_group_off[2] = {0, uint32_t(groups_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
     check(sdbg_bm25_topk_batch_groups_min(segs, 1, terms_.data(), group_off.data(), query_group_off,
@@ -205,9 +234,11 @@ void GpuAggScan::Scan(duckdb::DataChunkMock& output) {
 
 GpuCountScan::GpuCountScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, std::vector<uint32_t> group_sizes,
-                           std::vector<uint32_t> group_min_match)
+                           std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      groups_(std::move(group_sizes)), group_min_(std::move(group_min_match)), filter_(table_filter) {
+      groups_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
+      filter_(table_filter) {
+  check_phrase(phrase_, terms_.size(), !groups_.empty());
 }
 
 void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
@@ -218,7 +249,12 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
   uint64_t n = 0;
   int rc;
   const char* what;
-  if (groups_.empty()) {
+  if (!phrase_.empty()) {
+    const uint32_t phrase_off[2] = {0, uint32_t(terms_.size())};
+    rc = sdbg_phrase_count_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), phrase_off, 1, excluded_.data(), excl_off,
+                                 filter_.data(), &n);
+    what = "sdbg_phrase_count_batch: ";
+  } else if (groups_.empty()) {
     rc = sdbg_match_count_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                 filter_.data(), &n);
     what = "sdbg_match_count_batch: ";

@@ -50,7 +50,9 @@ class GpuTopKIterator final : public irs::DocIterator {
                   const sdbg_col_pred* table_filter /* nullable: the ColFilter wrap */,
                   std::vector<uint32_t> excluded_terms = {} /* term ids of the And's Not children (irs exclusion.hpp) */,
                   std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */,
-                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
+                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+                  std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
+                                                                 relative positions (0 first, increasing); needs k > 0 */);
 
   // Scored top-k: the hot path.
   void Collect(const irs::ScoreFunction&, irs::ColumnArgsFetcher&, irs::ScoreCollector& collector) override;
@@ -85,6 +87,7 @@ class GpuTopKIterator final : public irs::DocIterator {
   std::vector<uint32_t> excluded_;
   std::vector<uint32_t> groups_;   // sizes of the OR groups over terms_ (empty: the flat `kind_` query)
   std::vector<uint32_t> group_min_;   // their minimum match counts (empty: all 1)
+  std::vector<uint32_t> phrase_;      // a phrase's relative positions, one per term (empty: not a phrase)
   float k1_, b_;
   uint32_t k_;
   FilterChain filter_;
@@ -125,14 +128,16 @@ class GpuCountScan {
   GpuCountScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */,
-               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+               std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
+                                                              relative positions (0 first, increasing) */);
   // Fills `output` with one row, count[0] = the number of matches; the next call leaves it empty (end of scan).
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, groups_, group_min_;
+  std::vector<uint32_t> terms_, excluded_, groups_, group_min_, phrase_;
   FilterChain filter_;
   bool done_ = false;
 };

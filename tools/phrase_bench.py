@@ -1,0 +1,108 @@
+"""Cost of the phrase check: exact phrase queries against the AND of the same terms, on a seeded token corpus.
+
+The corpus: --docs docs (10 M by default) of 4..28 tokens each (uniform), tokens drawn from a Zipf(1.1) vocabulary of
+--vocab terms, norms = doc lengths, one segment. Two batches of --queries phrases, windows of the corpus's own token
+sequence (a window is picked with its frequency, so frequent adjacent pairs dominate): two-word phrases, and three- and
+four-word phrases. For each batch it reports ms per step (CUDA events on the library's stream, L2 flushed before every step, after
+warm-up) of
+  phrase count (sdbg_phrase_count_batch)   against   AND count of the same terms (sdbg_match_count_batch)
+  phrase top-1000 (sdbg_phrase_topk_batch) against   AND top-1000 (sdbg_bm25_topk_batch at pruning level 0)
+and the matches of both. The AND is the phrase's candidate set, so the gap is the cost of checking positions. Prints one
+JSON line with the GPU name and power limit read in the same run.
+
+    python tools/phrase_bench.py [--steps 5] [--warmup 2] [--docs 10000000] [--queries 4096]
+"""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+import serenedb_b200 as sdb  # noqa: E402
+from count_bench import gpu_info, timed  # noqa: E402
+
+
+def corpus(n_docs, vocab, seed):
+    # the sort key below packs (term, doc, position) into 64 bits: 29 bits of term, 30 of doc, 5 of position (< 32)
+    if not 0 < n_docs < 1 << 30 or not 0 < vocab <= 1 << 29:
+        raise SystemExit("--docs must be below 2^30 and --vocab at most 2^29")
+    rng = np.random.default_rng(seed)
+    lens = rng.integers(4, 29, n_docs).astype(np.int64)   # positions 0..27: 5 bits
+    n_tok = int(lens.sum())
+    terms = ((rng.zipf(1.1, n_tok) - 1) % vocab).astype(np.uint64)   # the tail past the vocabulary folds back onto it
+    starts = np.concatenate([[0], np.cumsum(lens)[:-1]])
+    doc = np.repeat(np.arange(1, n_docs + 1, dtype=np.uint64), lens)
+    pos = np.arange(n_tok, dtype=np.uint64) - np.repeat(starts.astype(np.uint64), lens)
+    # one sort by (term, doc, position) gives the postings and, per posting, its positions in order
+    key = np.sort((terms << np.uint64(35)) | (doc << np.uint64(5)) | pos)
+    t_of, d_of, p_of = key >> np.uint64(35), (key >> np.uint64(5)) & np.uint64((1 << 30) - 1), (key & np.uint64(31)).astype(np.uint32)
+    td = key >> np.uint64(5)
+    first = np.flatnonzero(np.concatenate([[True], td[1:] != td[:-1]]))
+    freqs = np.diff(np.concatenate([first, [len(key)]])).astype(np.uint32)
+    post_t, post_d = t_of[first].astype(np.int64), d_of[first].astype(np.uint32)
+    w = sdb.PostingsWriter(n_docs, norms=lens.astype(np.uint32))
+    tb = np.searchsorted(post_t, np.arange(vocab + 1))
+    pb = np.searchsorted(t_of.astype(np.int64), np.arange(vocab + 1))
+    for t in range(vocab):
+        w.add_term(post_d[tb[t]:tb[t + 1]], freqs[tb[t]:tb[t + 1]])
+    doc_bytes, metas = w.finish()
+    return dict(n=n_docs, lens=lens, terms=terms, doc=doc, doc_bytes=doc_bytes, metas=metas, positions=p_of,
+                term_pos_off=pb.astype(np.uint64), dwt=(tb[1:] - tb[:-1]))
+
+
+def phrases(c, n, length, rng):
+    """n phrases of `length` tokens, each a window of the corpus starting at a uniformly drawn token whose window stays in
+    its doc: frequent word sequences are drawn in proportion to their frequency."""
+    terms, doc = c["terms"], c["doc"]
+    out = []
+    while len(out) < n:
+        i = rng.integers(0, len(terms) - length, n)
+        ok = doc[i] == doc[i + length - 1]
+        for j in i[ok][: n - len(out)]:
+            out.append([int(x) for x in terms[j:j + length]])
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--docs", type=int, default=10_000_000)
+    ap.add_argument("--vocab", type=int, default=100_000)
+    ap.add_argument("--queries", type=int, default=4096)
+    a = ap.parse_args()
+    c = corpus(a.docs, a.vocab, 7)
+    ctx = sdb.Context(0)
+    seg = sdb.Segment(ctx, c["n"])
+    seg.stage_postings(c["doc_bytes"], c["metas"])
+    seg.stage_norms(c["lens"].astype(np.uint8), 1)
+    seg.stage_positions(c["positions"], c["term_pos_off"])
+    reader = sdb.IndexReader([seg], c["n"], int(c["lens"].sum()), c["dwt"])
+    scorer = sdb.BM25()
+    rng = np.random.default_rng(11)
+    out = {"gpu": gpu_info(), "docs": c["n"], "tokens": int(c["lens"].sum()), "queries": a.queries, "batches": {}}
+    ctx.set_wand(0)
+    for name, qs in (("2-word", phrases(c, a.queries, 2, rng)),
+                     ("3/4-word", phrases(c, a.queries // 2, 3, rng) + phrases(c, a.queries - a.queries // 2, 4, rng))):
+        conj = [sorted(set(q)) for q in qs]
+        pc = sdb.ExecutePhraseCountBatch(reader, qs)
+        ac = sdb.ExecuteCountBatch(reader, conj, sdb.AND)
+        _, _, pt = sdb.ExecutePhraseTopKBatch(reader, qs, scorer, 1000)
+        if not np.array_equal(pc, pt) or np.any(pc > ac):
+            raise SystemExit("phrase count / top-k total mismatch")
+        r = {"phrase_matches": int(pc.sum()), "and_matches": int(ac.sum())}
+        r["phrase_count_ms"] = timed(ctx, lambda: sdb.ExecutePhraseCountBatch(reader, qs), a.steps, a.warmup)
+        r["and_count_ms"] = timed(ctx, lambda: sdb.ExecuteCountBatch(reader, conj, sdb.AND), a.steps, a.warmup)
+        r["phrase_top1000_ms"] = timed(ctx, lambda: sdb.ExecutePhraseTopKBatch(reader, qs, scorer, 1000), a.steps, a.warmup)
+        r["and_top1000_ms"] = timed(ctx, lambda: sdb.ExecuteTopKBatch(reader, conj, sdb.AND, scorer, 1000), a.steps, a.warmup)
+        out["batches"][name] = r
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
