@@ -501,6 +501,47 @@ int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint3
                            const sdbg_bm25_term* phrase_stats /* n_queries */, float k1, float b, const sdbg_col_pred* filt,
                            uint32_t k, float threshold_in, sdbg_hit* out /* n_queries * k */, uint32_t* n_out,
                            uint64_t* total_matches);
+/* Sorted scan, facet counts, aggregates and match scan of phrases (`WHERE body @@ '"new york"' ORDER BY col LIMIT k`,
+ * `... GROUP BY col`, `SELECT id [, bm25(...)] ... LIMIT n OFFSET o`): the phrase parameters of sdbg_phrase_count_batch
+ * (terms, rel_pos, phrase_off, n_queries, excl_terms, excl_off, filt), then the pass parameters and outputs of the flat
+ * entry each mirrors: sdbg_match_topk_by_column_batch (k 1..4096), sdbg_match_facet_counts_batch,
+ * sdbg_match_aggregate_batch and sdbg_match_scan_batch_groups_min. Which docs: exactly the docs sdbg_phrase_count_batch
+ * counts for the query. Order, ties, NULL rules, key ranges, the dense layouts, the out-of-range report, pages and totals
+ * are those of the mirrored entry; identical at every pruning level (the sorted scan prunes as its flat entry does).
+ * sum(counts[q, :]) + null_counts[q], COUNT(*) over the groups and total[q] equal the phrase count. A one-slot phrase
+ * gives exactly the flat AND entry's result for its term.
+ * sdbg_phrase_scan_batch scores with phrase_stats, k1, b as sdbg_phrase_topk_batch does: with scored != 0 a hit's score is
+ * bit for bit the score sdbg_phrase_topk_batch gives that doc; with scored == 0 every score is 0 and phrase_stats may be
+ * NULL.
+ * Errors, all found before anything is queued except the facet and aggregate passes' out-of-range key: those of
+ * sdbg_phrase_count_batch (SDBG_ENOTFOUND for a segment without positions) and those of the mirrored entry; a scored scan
+ * with NULL phrase_stats: SDBG_EINVAL. Synchronous on the context's stream.
+ * Device scratch: the mirrored entry's, plus the slots' lists, 16 B per slot and segment; a scored scan stages the same
+ * again with one PostingsDev and one 80-byte sink per segment and 16 B per query. The phrase check runs per doc that
+ * survives the conjunction, the exclusions, the deleted docs and the filter chain (the sorted scan: once its key has
+ * passed the threshold), and a page deep into the result repeats it in the scan's second pass. */
+int sdbg_phrase_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                     const uint32_t* rel_pos /* NULL: adjacent */, const uint32_t* phrase_off, size_t n_queries,
+                                     const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                     const sdbg_col_pred* filt, uint64_t sort_field, int descending, int nulls_first,
+                                     uint32_t k, sdbg_sort_hit* out /* n_queries * k */, uint32_t* n_out);
+int sdbg_phrase_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                   const uint32_t* rel_pos /* NULL: adjacent */, const uint32_t* phrase_off, size_t n_queries,
+                                   const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                   const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                   uint64_t* counts /* n_queries * key_span */, uint64_t* null_counts /* n_queries */);
+int sdbg_phrase_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                const uint32_t* rel_pos /* NULL: adjacent */, const uint32_t* phrase_off, size_t n_queries,
+                                const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                uint64_t value_field, sdbg_match_agg* out /* n_queries * key_span */,
+                                sdbg_match_agg* null_out /* n_queries */);
+int sdbg_phrase_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                           const uint32_t* rel_pos /* NULL: adjacent */, const uint32_t* phrase_off, size_t n_queries,
+                           const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                           const sdbg_bm25_term* phrase_stats /* n_queries; NULL when scored == 0 */, float k1, float b,
+                           const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit, int scored,
+                           sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

@@ -11,6 +11,9 @@ from .engine import (ExecuteDistCountGroupsBatch, ExecuteDistFacetCountsGroupsBa
                      merge_aggregates_gathered, merge_topk_by_column_gathered, topk_by_column_device_bytes)
 from .engine import ExecuteDistTopKGroupsBatch, TopKGroupsDevice, merge_topk_groups_gathered, topk_groups_device_bytes
 from .engine import ExecutePhraseCount, ExecutePhraseCountBatch, ExecutePhraseTopK, ExecutePhraseTopKBatch
+from .engine import (ExecutePhraseTopKByColumn, ExecutePhraseTopKByColumnBatch, ExecutePhraseFacetCounts,
+                     ExecutePhraseFacetCountsBatch, ExecutePhraseMatchAggregates, ExecutePhraseMatchAggregatesBatch,
+                     ExecutePhraseMatchScan, ExecutePhraseMatchScanBatch)
 from .engine import (AND, OR, BM25, TFIDF, FLT_MIN, Context, ExecuteCount, ExecuteCountBatch, ExecuteCountGroups,
                      ExecuteCountGroupsBatch, ExecuteFacetCounts, ExecuteFacetCountsBatch, ExecuteFacetCountsGroups,
                      ExecuteFacetCountsGroupsBatch, ExecuteMatchAggregates, ExecuteMatchAggregatesBatch,
@@ -31,4 +34,6 @@ __all__ = ["AND", "OR", "BM25", "TFIDF", "FLT_MIN", "Context", "ExecuteCount", "
            "ExecuteDistTopKByColumnGroupsBatch", "TopKByColumnDevice", "topk_by_column_device_bytes",
            "merge_topk_by_column_gathered", "ExecuteDistTopKGroupsBatch", "TopKGroupsDevice", "topk_groups_device_bytes",
            "merge_topk_groups_gathered", "ExecutePhraseCount", "ExecutePhraseCountBatch", "ExecutePhraseTopK",
-           "ExecutePhraseTopKBatch"]
+           "ExecutePhraseTopKBatch", "ExecutePhraseTopKByColumn", "ExecutePhraseTopKByColumnBatch", "ExecutePhraseFacetCounts",
+           "ExecutePhraseFacetCountsBatch", "ExecutePhraseMatchAggregates", "ExecutePhraseMatchAggregatesBatch",
+           "ExecutePhraseMatchScan", "ExecutePhraseMatchScanBatch"]

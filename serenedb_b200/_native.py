@@ -108,7 +108,15 @@ SIGNATURES = {
     "sdbg_phrase_count_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
     "sdbg_phrase_topk_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_float, C.c_float, _vp, C.c_uint32,
                                          C.c_float, _vp, _vp, _vp]),
-    "sdbg_match_topk_by_column_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int, C.c_int,
+    "sdbg_phrase_topk_by_column_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int, C.c_int,
+                                                   C.c_uint32, _vp, _vp]),
+    "sdbg_phrase_facet_counts_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,
+                                                 C.c_uint32, _vp, _vp]),
+    "sdbg_phrase_aggregate_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64, C.c_uint32,
+                                              C.c_uint64, _vp, _vp]),
+    "sdbg_phrase_scan_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _vp,
+                                         C.c_uint32, C.c_int, _vp, _vp, _vp]),
+    "sdbg_match_topk_by_column_batch":(C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int, C.c_int,
                                                   C.c_uint32, _vp, _vp]),
     "sdbg_match_facet_counts_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,
                                                 C.c_uint32, _vp, _vp]),

@@ -137,6 +137,10 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
   return __any_sync(kFull, any != 0u);
 }
 
+// The phrase check inlined into the sorted scan's and the facet pass's sinks spills a word under ptxas's own register
+// choice; at least 4 CTAs per SM (64 registers) it does not. Every other instantiation has no minimum.
+constexpr int kPhraseMinBlocks = 4;
+
 // kAnd: conjunction (else disjunction). kGroups: conjunction of OR groups (CountParams::grp_end). The term loops are not
 // unrolled: 1..16 terms share one instantiation.
 // kSort: the sorted scan (bm25_sort.cuh). Instead of popcounting, every surviving doc's sort key enters a buffer of
@@ -160,17 +164,24 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
 // deleted docs and the filter chain is probed in each slot's list for its positions; a doc of phrase frequency 0 is
 // dropped, the others are counted and, with P.phrase.cap, scored from their phrase frequency and kept in a buffer of
 // P.phrase.cap keys in dynamic shared memory as the sorted scan keeps its keys; the item's k best go to slot item.w.
+// kPhrase with one other sink: with kFacet, kAgg or kEmit the phrase check is a stage that narrows `acc` after the
+// exclusions (deleted docs, filter chain, then phrase_freq per surviving bit, written back), so the sink reads only phrase
+// matches and emit passes A and B see the same set. With kSort it runs inside the sink, on a doc whose key has passed
+// s_thr: a doc that cannot enter the buffer is never probed for positions.
 // The sinks take kGroups queries: the groups narrow `acc` before the sink reads the column, and the bit-sliced counter
 // planes follow the sink's region of dynamic shared memory (16 * cap B, 4 * span B or agg_cells_bytes(span), rounded up
 // to 16 B).
 template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false, bool kAgg = false, bool kEmit = false,
           bool kPhrase = false>
-__global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P) {
+__global__ void __launch_bounds__(kCountThreads, kPhrase && (kSort || kFacet) ? kPhraseMinBlocks : 0) bm25_count_kernel(CountParams P) {
   static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
   static_assert(!(kFacet && kSort), "the facet pass has its own sink");
   static_assert(!(kAgg && (kSort || kFacet)), "the aggregate pass has its own sink");
   static_assert(!(kEmit && (kSort || kFacet || kAgg)), "the match scan has its own sink");
-  static_assert(!kPhrase || (kAnd && !kSort && !kFacet && !kAgg && !kEmit), "a phrase is checked on its terms' conjunction");
+  static_assert(!kPhrase || (kAnd && int(kSort) + int(kFacet) + int(kAgg) + int(kEmit) <= 1),
+                "a phrase is checked on its terms' conjunction");
+  constexpr bool kPhraseSink = kPhrase && !kSort && !kFacet && !kAgg && !kEmit;   // count / top-k of phrase matches
+  constexpr bool kPhraseStage = kPhrase && (kFacet || kAgg || kEmit);           // narrows acc before the sink
   __shared__ uint32_t acc[kCountWords];
   __shared__ uint32_t tmp[kAnd || kGroups ? kCountWords : 1];
   __shared__ uint32_t stage[kCountWarps][128];
@@ -234,7 +245,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
     for (uint32_t i = tid; i < 2u * P.sort.cap; i += kCountThreads) sort_buf[i] = 0ull;
     if (tid == 0) { s_thr[0] = 0ull; s_fill[0] = 0u; }
   }
-  if constexpr (kPhrase) {
+  if constexpr (kPhraseSink) {
     for (uint32_t i = tid; i < 2u * P.phrase.cap; i += kCountThreads) sort_buf[i] = 0ull;
     if (tid == 0) { s_thr[0] = P.phrase.cap ? P.phrase.thr[q] : 0ull; s_fill[0] = 0u; }
   }
@@ -263,7 +274,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       if constexpr (kSort) {
         if (P.sort.thr) s_thr[0] = max(s_thr[0], *reinterpret_cast<volatile unsigned long long*>(P.sort.thr + q));
       }
-      if constexpr (kPhrase) {
+      if constexpr (kPhraseSink) {
         if (P.phrase.cap) s_thr[0] = max(s_thr[0], *reinterpret_cast<volatile unsigned long long*>(P.phrase.thr + q));
       }
     }
@@ -412,12 +423,30 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
       run_lists(n_pos, n_lists, acc, true, true);
       __syncthreads();
     }
-    if (live && !kSort && !kPhrase && !(kEmit && P.emit.base)) {
+    if constexpr (kPhraseStage) {
+      if (live) {
+        const uint32_t wbase = ws >> 5, s0 = P.phrase.slot_off[q], ns = P.phrase.slot_off[q + 1] - s0;
+        for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
+          uint32_t v = acc[i];
+          if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
+          v = chain_bits(v, i);
+          for (uint32_t r = v; r; r &= r - 1u) {
+            const uint32_t bit = __ffs(r) - 1u;
+            if (!phrase_freq(P.seg, P.phrase, s0, ns, ws + 32u * i + bit)) v &= ~(1u << bit);
+          }
+          acc[i] = v;
+        }
+        __syncthreads();
+      }
+    }
+    if (live && !kSort && !kPhraseSink && !(kEmit && P.emit.base)) {
       const uint32_t wbase = ws >> 5;
       for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
         uint32_t v = acc[i];
-        if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
-        v = chain_bits(v, i);
+        if constexpr (!kPhraseStage) {   // else the stage has applied them
+          if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
+          v = chain_bits(v, i);
+        }
         if constexpr (kFacet) {
           for (uint32_t r = v; r; r &= r - 1u) oor |= facet_add(P.facet, ws + 32u * i + (__ffs(r) - 1u), bins, &s_fill[0]);
         }
@@ -435,8 +464,11 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
 #pragma unroll
         for (uint32_t j = 0; j < kRun; ++j) {
           uint32_t x = acc[i0 + j];
-          if (x && P.seg.deleted && wbase + i0 + j < del_words) x &= ~__ldg(P.seg.deleted + wbase + i0 + j);
-          v[j] = chain_bits(x, i0 + j);
+          if constexpr (!kPhraseStage) {
+            if (x && P.seg.deleted && wbase + i0 + j < del_words) x &= ~__ldg(P.seg.deleted + wbase + i0 + j);
+            x = chain_bits(x, i0 + j);
+          }
+          v[j] = x;
           n += __popc(v[j]);
         }
         const uint32_t incl = warp_incl_scan(n, lane);
@@ -459,6 +491,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
     if constexpr (kSort) {
       if (live) {
         const uint32_t wbase = ws >> 5, cap = P.sort.cap;
+        const uint32_t s0 = kPhrase ? P.phrase.slot_off[q] : 0u, ns = kPhrase ? P.phrase.slot_off[q + 1] - s0 : 0u;
         unsigned long long* hi = sort_buf;
         unsigned long long* lo = sort_buf + cap;
         for (uint32_t base = 0; base < kCountWords; base += kCountThreads) {   // uniform trip count
@@ -469,8 +502,12 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
           for (;;) {   // a full buffer is cut to the k best and the remaining bits go on
             const unsigned long long thr = s_thr[0];
             for (; v; v &= v - 1u) {
-              const ulonglong2 key = sort_key(P.sort, ws + 32u * i + (__ffs(v) - 1u));
+              const uint32_t doc = ws + 32u * i + (__ffs(v) - 1u);
+              const ulonglong2 key = sort_key(P.sort, doc);
               if (key.x < thr) continue;
+              if constexpr (kPhrase) {
+                if (!phrase_freq(P.seg, P.phrase, s0, ns, doc)) continue;
+              }
               const uint32_t slot = atomicAdd(&s_fill[0], 1u);
               if (slot >= cap) break;
               hi[slot] = key.x; lo[slot] = key.y;
@@ -483,7 +520,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
         }
       }
     }
-    if constexpr (kPhrase) {
+    if constexpr (kPhraseSink) {
       if (live) {
         const PhraseSink& F = P.phrase;
         const uint32_t wbase = ws >> 5, cap = F.cap, s0 = F.slot_off[q], ns = F.slot_off[q + 1] - s0;
@@ -565,7 +602,7 @@ __global__ void __launch_bounds__(kCountThreads) bm25_count_kernel(CountParams P
   if constexpr (kEmit) {
     if (P.emit.base) return;
   }
-  if constexpr (kPhrase) {
+  if constexpr (kPhraseSink) {
     if (P.phrase.cap) {
       const unsigned long long kth = sort_select(sort_buf, sort_buf + P.phrase.cap, P.phrase.cap, P.phrase.k, &s_fill[0]);
       const uint32_t n = s_fill[0];

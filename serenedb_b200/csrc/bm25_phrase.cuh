@@ -1,6 +1,8 @@
-// bm25_phrase.cuh -- exact phrase queries (sdbg_phrase_count_batch / sdbg_phrase_topk_batch): the positions layout in
-// HBM, the kernels that build it at staging, and the per-doc phrase check that bm25_count_kernel runs (kPhrase) on the
-// docs that survive the conjunction of the phrase's terms, the deleted docs, the filter chain and the exclusions.
+// bm25_phrase.cuh -- exact phrase queries (sdbg_phrase_*_batch): the positions layout in HBM, the kernels that build it
+// at staging, and the per-doc phrase check that bm25_count_kernel runs (kPhrase) on the docs that survive the
+// conjunction of the phrase's terms, the deleted docs, the filter chain and the exclusions: in its own sink (count,
+// top-k), as a stage that narrows the window before the facet, aggregate and match-scan sinks, or inside the sorted
+// scan's sink once a doc's key has passed the threshold.
 //
 // Positions layout (DESIGN.md §3): per posting block g a 64-bit base pos_base[g] into the u32 arena `pos` (one sentinel
 // behind the last block), and at pos[pos_base[g] ..] first the block's len exclusive prefix sums of its frequencies, then
@@ -17,7 +19,8 @@ namespace sdbg {
 
 constexpr uint32_t kMaxPhraseSlots = 16;
 
-// bm25_count_kernel's phrase sink (kPhrase). cap == 0: count only; else the top-k of the phrase matches by score.
+// bm25_count_kernel's phrase sink (kPhrase). cap == 0: count only; else the top-k of the phrase matches by score. With
+// another sink (kSort, kFacet, kAgg, kEmit) only the positions and slots are read.
 struct PhraseSink {
   const unsigned long long* pos_base = nullptr;   // per block + sentinel
   const uint32_t* pos = nullptr;
@@ -78,10 +81,15 @@ __device__ __forceinline__ uint32_t phrase_freq(const PostingsDev& S, const Phra
   return freq;
 }
 
+// The score of a phrase match of frequency f: bm25(f, norm(d)) with query q's phrase statistics.
+__device__ __forceinline__ float phrase_score(const PostingsDev& S, const PhraseSink& F, uint32_t q, uint32_t d, uint32_t f) {
+  const float4 c = __ldg(F.consts + q);
+  return bm25(f, load_norm(S.norms, S.norm_width, d), c.x, c.y, c.z);
+}
+
 // The top-k key of a phrase match: score bits, then ~ordinal (ties: segment asc, doc asc), as bm25_topk's keys.
 __device__ __forceinline__ unsigned long long phrase_key(const PostingsDev& S, const PhraseSink& F, uint32_t q, uint32_t d, uint32_t f) {
-  const float4 c = __ldg(F.consts + q);
-  const float s = bm25(f, load_norm(S.norms, S.norm_width, d), c.x, c.y, c.z);
+  const float s = phrase_score(S, F, q, d, f);
   return (static_cast<unsigned long long>(__float_as_uint(s)) << 32) | (~(F.ordinal_base + d) & 0xFFFFFFFFull);
 }
 

@@ -2456,8 +2456,9 @@ struct CountPlan {
   }
 
   // The bm25_count_kernel instantiation of this plan's launches in `mode`, with its dynamic shared memory: the mode's
-  // own bytes (facet bins, sorted keys, aggregate cells; none for a count), then the counter planes.
-  std::pair<CountKernel, size_t> kernel(CountMode mode, size_t mode_bytes) const {
+  // own bytes (facet bins, sorted keys, aggregate cells; none for a count), then the counter planes. phrased: the plan's
+  // batch is the AND of phrases' terms, checked by the phrase sink (CountMode::phrase) or before / in another sink.
+  std::pair<CountKernel, size_t> kernel(CountMode mode, size_t mode_bytes, bool phrased = false) const {
     static const CountKernel kernels[3][5] = {   // [OR | AND | OR groups][count | sort | facet | agg | emit]
         {bm25_count_kernel<false>, bm25_count_kernel<false, false, true>, bm25_count_kernel<false, false, false, true>,
          bm25_count_kernel<false, false, false, false, true>, bm25_count_kernel<false, false, false, false, false, true>},
@@ -2465,7 +2466,12 @@ struct CountPlan {
          bm25_count_kernel<true, false, false, false, true>, bm25_count_kernel<true, false, false, false, false, true>},
         {bm25_count_kernel<false, true>, bm25_count_kernel<false, true, true>, bm25_count_kernel<false, true, false, true>,
          bm25_count_kernel<false, true, false, false, true>, bm25_count_kernel<false, true, false, false, false, true>}};
-    if (mode == CountMode::phrase) return {bm25_count_kernel<true, false, false, false, false, false, true>, mode_bytes};
+    static const CountKernel phrase_kernels[5] = {   // [phrase sink | sort | facet | agg | emit] of a phrase's conjunction
+        bm25_count_kernel<true, false, false, false, false, false, true>, bm25_count_kernel<true, false, true, false, false, false, true>,
+        bm25_count_kernel<true, false, false, true, false, false, true>, bm25_count_kernel<true, false, false, false, true, false, true>,
+        bm25_count_kernel<true, false, false, false, false, true, true>};
+    if (mode == CountMode::phrase) return {phrase_kernels[0], mode_bytes};
+    if (phrased) return {phrase_kernels[int(mode)], mode_bytes};
     const int shape = Q.term_grp ? 2 : Q.kind == SDBG_QUERY_AND ? 1 : 0;
     return {kernels[shape][int(mode)], mode_bytes + size_t(planes) * kCountWords * 4u};
   }
@@ -2629,6 +2635,27 @@ void item_slots(const CountPlan& pl, char* h, size_t slot_off_pos, size_t slots_
   for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
 }
 
+// The phrase's slot lists of every segment for the kernel's PhraseSink::slots, h_lists[segment][slot]: {first BlockDesc,
+// blocks, rel_pos, 0}. Slots before job.slot_off[0] belong to no query and are left as they are.
+void phrase_slot_lists(sdbg_segment* const* segs, size_t n_segs, const PhraseJob& job, size_t nq, uint4* h_lists) {
+  const uint32_t n_slots = job.slot_off[nq];
+  for (size_t si = 0; si < n_segs; ++si)
+    for (uint32_t i = job.slot_off[0]; i < n_slots; ++i) {
+      const uint2 l = excl_list(segs[si], job.slot_term[i]);
+      h_lists[si * n_slots + i] = make_uint4(l.x, l.y, job.slot_rel[i], 0u);
+    }
+}
+
+// The positions and slots of segment si for the kernels' PhraseSink; d_slot_off / d_lists: device copies of
+// job.slot_off and of phrase_slot_lists' array.
+void phrase_sink(sdbg_segment* const* segs, size_t si, uint32_t n_slots, const uint32_t* d_slot_off, const uint4* d_lists,
+                 PhraseSink& F) {
+  F.pos_base = static_cast<const unsigned long long*>(segs[si]->d_pos_base);
+  F.pos = static_cast<const uint32_t*>(segs[si]->d_pos);
+  F.slots = d_lists + si * n_slots;
+  F.slot_off = d_slot_off;
+}
+
 // The phrase pass of count_run (CountMode::phrase) over a plan with work items: bm25_count_kernel<kAnd, .., kPhrase> per
 // segment, the count into out.counts; with a top-k (job.k) each item writes its k best keys to its own slot, then
 // phrase_merge_kernel keeps each query's k best in out.bins (u64 keys [nq][k]) with their number in out.nulls (u32 [nq]).
@@ -2651,12 +2678,7 @@ int phrase_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, co
   pl.write(h);
   item_slots(pl, h, slot_off_pos, slots_pos);
   std::memcpy(h + poff_pos, job.slot_off, pl.off_bytes);
-  auto* h_lists = reinterpret_cast<uint4*>(h + lists_pos);   // slots before job.slot_off[0] belong to no query: left 0
-  for (size_t si = 0; si < n_segs; ++si)
-    for (uint32_t i = job.slot_off[0]; i < n_slots; ++i) {
-      const uint2 l = excl_list(segs[si], job.slot_term[i]);
-      h_lists[si * n_slots + i] = make_uint4(l.x, l.y, job.slot_rel[i], 0u);
-    }
+  phrase_slot_lists(segs, n_segs, job, nq, reinterpret_cast<uint4*>(h + lists_pos));
   if (k) std::memcpy(h + consts_pos, job.consts.data(), nq * sizeof(float4));
   // device scratch: [item keys [items][k] | item key counts | thresholds [nq]]
   const size_t keys_n_pos = total * size_t(k) * 8;
@@ -2684,10 +2706,7 @@ int phrase_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, co
     pl.params(d, segs[si], si, first, chains[si], &P);
     P.counts = static_cast<unsigned long long*>(out.counts);
     PhraseSink& F = P.phrase;
-    F.pos_base = static_cast<const unsigned long long*>(segs[si]->d_pos_base);
-    F.pos = static_cast<const uint32_t*>(segs[si]->d_pos);
-    F.slots = reinterpret_cast<const uint4*>(d + lists_pos) + si * n_slots;
-    F.slot_off = reinterpret_cast<const uint32_t*>(d + poff_pos);
+    phrase_sink(segs, si, n_slots, reinterpret_cast<const uint32_t*>(d + poff_pos), reinterpret_cast<const uint4*>(d + lists_pos), F);
     F.consts = reinterpret_cast<const float4*>(d + consts_pos);
     F.ordinal_base = uint32_t(base);
     F.k = k; F.cap = cap; F.thr = thr;
@@ -2715,7 +2734,8 @@ int phrase_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, co
 // sorted scan launches per segment its seed items first (all segments), then the rest, each item writing its k best to
 // its own slot (its index in the work array); then sort_merge_kernel per query, and for a rank sort_dist_rows_kernel.
 // The match scan launches its items twice (bm25_emit.cuh): pass A, emit_bases_kernel over each query's items in
-// (segment, first window) order, pass B.
+// (segment, first window) order, pass B. A job with phrase slots (job.phrase.slot_off; the plan's batch is the AND of the
+// phrases' terms) runs the phrase instantiations of its mode and stages the slot lists.
 // The plan is staged from pageable memory, which the copy has consumed when it returns, so calls can follow one another
 // without a wait (a host group entry queues its shapes back to back).
 int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt, const CountJob& job,
@@ -2729,17 +2749,26 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
   if (phrase) return phrase_run(segs, n_segs, pl, filt, job.phrase, out);
   const SortJob& J = job.sort;
   const uint32_t k = J.k, cap = sort ? J.sink[0].cap : 0u;
+  const bool phrased = job.phrase.slot_off != nullptr;
+  const uint32_t n_slots = phrased ? job.phrase.slot_off[nq] : 0u;
   // host staging: the plan's, then for the sorted scan [slot_off | slots | segments], for the match scan [slot_off |
-  // slots | offsets]
+  // slots | offsets]; then for a phrase [query slot offsets | per segment the slots' lists]
   const size_t slot_off_pos = pl.staged;
   const size_t slots_pos = slot_off_pos + pl.off_bytes;
   const size_t segs_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
-  const size_t bytes = sort ? segs_pos + n_segs * sizeof(SortSegDev) : emit ? segs_pos + nq * 8 : pl.staged;
+  const size_t mode_end = sort ? segs_pos + n_segs * sizeof(SortSegDev) : emit ? segs_pos + nq * 8 : pl.staged;
+  const size_t poff_pos = (mode_end + 15) & ~size_t(15);
+  const size_t plists_pos = (poff_pos + pl.off_bytes + 15) & ~size_t(15);
+  const size_t bytes = phrased ? plists_pos + n_segs * n_slots * sizeof(uint4) : mode_end;
   std::vector<char> staging(bytes);
   char* h = staging.data();
   pl.write(h);
   if (sort || emit) item_slots(pl, h, slot_off_pos, slots_pos);
   if (emit) std::memcpy(h + segs_pos, job.emit.offset, nq * 8);
+  if (phrased) {
+    std::memcpy(h + poff_pos, job.phrase.slot_off, pl.off_bytes);
+    phrase_slot_lists(segs, n_segs, job.phrase, nq, reinterpret_cast<uint4*>(h + plists_pos));
+  }
   if (sort) {
     auto* h_segs = reinterpret_cast<SortSegDev*>(h + segs_pos);
     for (size_t si = 0; si < n_segs; ++si) {
@@ -2768,7 +2797,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
                             : job.mode == CountMode::facet ? (size_t(job.facet.span) * 4 + 15) & ~size_t(15)
                             : job.mode == CountMode::agg   ? agg_cells_bytes(job.agg.key.span)
                                                            : 0;
-  const auto [kernel, smem] = pl.kernel(job.mode, mode_bytes);
+  const auto [kernel, smem] = pl.kernel(job.mode, mode_bytes, phrased);
   CU(c, fit_dynamic_smem(kernel, smem));
   std::vector<ChainDev> chains(n_segs);
   if (int rc = filter_chains(segs, n_segs, filt, chains.data())) return rc;
@@ -2794,6 +2823,9 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
         CountParams P;
         pl.params(d, segs[si], si, first, chains[si], &P);
         P.counts = static_cast<unsigned long long*>(out.counts);
+        if (phrased)
+          phrase_sink(segs, si, n_slots, reinterpret_cast<const uint32_t*>(d + poff_pos), reinterpret_cast<const uint4*>(d + plists_pos),
+                      P.phrase);
         if (sort) {
           P.counts = nullptr;
           P.sort = J.sink[si];
@@ -2960,9 +2992,11 @@ int pass_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint3
   return pass_finish(c, L, h, fill);
 }
 
+// phrase: the job's phrase slots (PhraseBatch::job) when B is the AND of phrases' terms.
 int sort_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt, uint64_t field,
-                 int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
+                 int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out, const PhraseJob& phrase = {}) {
   CountJob job{CountMode::sort, {field, descending, nulls_first, k, {}, {}}, {}, {}};
+  job.phrase = phrase;
   const PassRegion L = sort_region(B.nq, k);
   return pass_to_host(segs, n_segs, B, filt, job, L, [&](const char* h) {
     std::memcpy(n_out, h + L.counts, B.nq * 4);
@@ -2971,8 +3005,10 @@ int sort_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint3
 }
 
 int agg_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt, uint64_t key_field,
-                int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out, sdbg_match_agg* null_out) {
+                int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out, sdbg_match_agg* null_out,
+                const PhraseJob& phrase = {}) {
   CountJob job{CountMode::agg, {}, {}, {{key_field, key_min, key_span, {}}, value_field, {}}};
+  job.phrase = phrase;
   const PassRegion L = agg_region(B.nq, key_span);
   return pass_to_host(segs, n_segs, B, filt, job, L, [&](const char* h) {
     agg_results(reinterpret_cast<const AggCell*>(h + L.bins), B.nq, key_span, job.agg.sink[0].type, out, null_out);
@@ -3028,7 +3064,29 @@ struct PhraseBatch {
   QueryBatch<uint32_t> conj(size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off) const {
     return {SDBG_QUERY_AND, ids.data(), id_off.data(), nq, excl_terms, excl_off, nullptr};
   }
+
+  // The phrase slots of a count_run job over conj(): count only until k or consts are set.
+  PhraseJob job(const uint32_t* terms, const uint32_t* phrase_off) const {
+    PhraseJob J;
+    J.slot_term = terms; J.slot_rel = rel.data(); J.slot_off = phrase_off;
+    return J;
+  }
 };
+
+// consts[q] = {c0, norm_const, norm_length, 0} of phrase q's statistics phrase_stats[q]: the scorer form of fill_qterm,
+// as the phrase top-k and the scored phrase scan score a match.
+std::vector<float4> phrase_consts(sdbg_segment* const* segs, const uint32_t* terms, const uint32_t* phrase_off, size_t nq,
+                                  const sdbg_bm25_term* phrase_stats, float k1, float b) {
+  std::vector<float4> consts(nq);
+  for (size_t q = 0; q < nq; ++q) {
+    sdbg_bm25_term t = phrase_stats[q];
+    t.term = terms[phrase_off[q]];
+    QTermDev d;
+    fill_qterm(segs[0], t, k1, b, d);
+    consts[q] = make_float4(d.c0, d.norm_const, d.norm_length, 0.f);
+  }
+  return consts;
+}
 
 // Every segment holds positions (sdbg_stage_positions).
 int phrase_positions_staged(sdbg_segment* const* segs, size_t n_segs) {
@@ -3049,7 +3107,7 @@ extern "C" int sdbg_phrase_count_batch(sdbg_segment* const* segs, size_t n_segs,
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
   CountJob job{CountMode::count, {}, {}, {}};
   job.mode = CountMode::phrase;
-  job.phrase.slot_term = terms; job.phrase.slot_rel = PB.rel.data(); job.phrase.slot_off = phrase_off;
+  job.phrase = PB.job(terms, phrase_off);
   return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
 }
 
@@ -3072,15 +3130,9 @@ extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, 
   CountJob job{CountMode::count, {}, {}, {}};
   job.mode = CountMode::phrase;
   PhraseJob& J = job.phrase;
-  J.slot_term = terms; J.slot_rel = PB.rel.data(); J.slot_off = phrase_off; J.k = k;
-  J.consts.resize(nq);
-  for (size_t q = 0; q < nq; ++q) {   // the scorer form of fill_qterm, with the phrase's statistics
-    sdbg_bm25_term t = phrase_stats[q];
-    t.term = terms[phrase_off[q]];
-    QTermDev d;
-    fill_qterm(segs[0], t, k1, b, d);
-    J.consts[q] = make_float4(d.c0, d.norm_const, d.norm_length, 0.f);
-  }
+  J = PB.job(terms, phrase_off);
+  J.k = k;
+  J.consts = phrase_consts(segs, terms, phrase_off, nq, phrase_stats, k1, b);
   uint32_t thr_bits; std::memcpy(&thr_bits, &threshold_in, 4);
   if (!(threshold_in >= 0.f)) thr_bits = 0;  // negative / NaN seeds accept every positive score, as the top-k entries
   J.seed = (static_cast<unsigned long long>(thr_bits) << 32) | 0xFFFFFFFFull;
@@ -3092,6 +3144,52 @@ extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, 
   const CountOut o{dev.total, dev.keys, dev.n_out, nullptr, nullptr, -1};
   if (int rc = count_run(segs, n_segs, pl, filt, job, o)) return rc;
   return topk_hits_to_host(segs, n_segs, dev, nq, k, out, n_out, total_matches);
+}
+
+// The sorted scan, facet counts and aggregates of phrases: the phrase entries' checks (PhraseBatch, the AND of the
+// phrases' terms, staged positions), then the flat entry's pass with the phrase slots on its job.
+extern "C" int sdbg_phrase_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                                const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms,
+                                                const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
+                                                int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
+  if (!segs || !n_segs || !segs[0] || !k || !out || !n_out) return SDBG_EINVAL;
+  if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  if (PB.rc) return PB.rc;
+  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  if (B.rc) return B.rc;
+  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
+  return sort_to_host(segs, n_segs, B, filt, sort_field, descending, nulls_first, k, out, n_out, PB.job(terms, phrase_off));
+}
+
+extern "C" int sdbg_phrase_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                              const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms,
+                                              const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                              int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
+  if (!counts || !null_counts) return SDBG_EINVAL;
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  if (PB.rc) return PB.rc;
+  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  if (B.rc) return B.rc;
+  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
+  CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
+  job.phrase = PB.job(terms, phrase_off);
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, key_span),
+                      [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
+}
+
+extern "C" int sdbg_phrase_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                           const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms,
+                                           const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                           int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
+                                           sdbg_match_agg* null_out) {
+  if (!out || !null_out) return SDBG_EINVAL;
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  if (PB.rc) return PB.rc;
+  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  if (B.rc) return B.rc;
+  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
+  return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out, PB.job(terms, phrase_off));
 }
 
 extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -3243,37 +3341,85 @@ int scan_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<sdbg_bm2
   return SDBG_OK;
 }
 
-// The match scan of a checked batch B: scan_run for a whole batch, else shape by shape through shapes_run, into the
-// call's region in c->pass[0]; then one copy back through the pinned staging, one wait, and pass_finish.
-int scan_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_bm25_term>& B, const sdbg_col_pred* filt,
-                 const ScanArgs& A, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
-  if (B.rc) return B.rc;
-  sdbg_ctx* c = segs[0]->ctx;
+// The match scan of a checked batch of nq queries: run(o) queues it into the call's region in c->pass[0], zeroed; then
+// one copy back through the pinned staging, one wait, and pass_finish.
+template <class Run>
+int scan_to_host(sdbg_ctx* c, size_t nq, uint32_t limit, Run run, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
   CU(c, cudaSetDevice(c->device));
-  const size_t nq = B.nq;
-  const PassRegion L = scan_region(nq, A.limit);
+  const PassRegion L = scan_region(nq, limit);
   if (int rc = ensure(c, c->pass[0], L.bytes)) return rc;
   if (int rc = ensure_pinned(c, L.bytes)) return rc;
-  const CountOut o = L.at(c->pass[0].p);
   CU(c, cudaMemsetAsync(c->pass[0].p, 0, L.bytes, c->stream));
-  int rc;
-  if (B.whole.nq) {
-    rc = scan_run(segs, n_segs, B.whole, B.total_excl, nullptr, filt, A, o);
-  } else {
-    const CountJob job{CountMode::emit, {}, {}, {}, {A.limit, nullptr}};
-    rc = shapes_run(c, B.S, job.rows(false), {o.counts, o.bins, o.nulls}, [&](int sh, void* const* part) {
-      return scan_run(segs, n_segs, B.S.view(sh), B.S.total_excl[sh], B.S.qs[sh].data(), filt, A,
-                      CountOut{part[0], part[1], part[2], nullptr, nullptr, -1});
-    });
-  }
-  if (rc) return rc;
+  if (int rc = run(L.at(c->pass[0].p))) return rc;
   CU(c, cudaMemcpyAsync(c->h_pinned, c->pass[0].p, L.bytes, cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
   return pass_finish(c, L, static_cast<const char*>(c->h_pinned), [&](const char* h) {
     std::memcpy(total, h + L.counts, nq * 8);
-    std::memcpy(out, h + L.bins, nq * size_t(A.limit) * sizeof(sdbg_hit));
+    std::memcpy(out, h + L.bins, nq * size_t(limit) * sizeof(sdbg_hit));
     std::memcpy(n_out, h + L.nulls, nq * 4);
   });
+}
+
+// The match scan of a checked batch B: scan_run for a whole batch, else shape by shape through shapes_run.
+int scan_batch_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch<sdbg_bm25_term>& B, const sdbg_col_pred* filt,
+                       const ScanArgs& A, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
+  if (B.rc) return B.rc;
+  sdbg_ctx* c = segs[0]->ctx;
+  return scan_to_host(c, B.nq, A.limit, [&](const CountOut& o) {
+    if (B.whole.nq) return scan_run(segs, n_segs, B.whole, B.total_excl, nullptr, filt, A, o);
+    const CountJob job{CountMode::emit, {}, {}, {}, {A.limit, nullptr}};
+    return shapes_run(c, B.S, job.rows(false), {o.counts, o.bins, o.nulls}, [&](int sh, void* const* part) {
+      return scan_run(segs, n_segs, B.S.view(sh), B.S.total_excl[sh], B.S.qs[sh].data(), filt, A,
+                      CountOut{part[0], part[1], part[2], nullptr, nullptr, -1});
+    });
+  }, out, n_out, total);
+}
+
+// Queues the match scan of a checked phrase batch (B: the AND of the phrases' terms) into out, zeroed: the emit pass with
+// the phrase slots, then, when scored (J.consts set), phrase_score_kernel over the pages.
+// The scorer's staging: [PostingsDev [n_segs] | PhraseSink [n_segs] | slot_off | per segment the slots' lists].
+int phrase_scan_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt,
+                    const PhraseJob& J, const uint64_t* offset, uint32_t limit, const CountOut& out) {
+  sdbg_ctx* c = segs[0]->ctx;
+  const size_t nq = B.nq;
+  std::vector<unsigned long long> offs(nq, 0ull);
+  if (offset) std::copy(offset, offset + nq, offs.begin());
+  CountJob job{CountMode::emit, {}, {}, {}, {limit, offs.data()}};
+  job.phrase = J;
+  if (int rc = count_run(segs, n_segs, count_plan(segs, n_segs, B.whole, B.total_excl, filt, job), filt, job, out)) return rc;
+  if (J.consts.empty()) return SDBG_OK;
+  const uint32_t n_slots = J.slot_off[nq];
+  const size_t sinks_pos = (n_segs * sizeof(PostingsDev) + 15) & ~size_t(15);
+  const size_t off_pos = sinks_pos + n_segs * sizeof(PhraseSink);
+  const size_t lists_pos = (off_pos + (nq + 1) * 4 + 15) & ~size_t(15);
+  const size_t consts_pos = lists_pos + n_segs * n_slots * sizeof(uint4);
+  std::vector<char> h(consts_pos + nq * sizeof(float4));
+  DevBuf& b_sc = c->scratch[4];
+  if (int rc = ensure(c, b_sc, h.size())) return rc;
+  const char* d = static_cast<const char*>(b_sc.p);
+  for (size_t si = 0; si < n_segs; ++si) {
+    const PostingsDev p = postings_view(segs[si], 0);
+    std::memcpy(h.data() + si * sizeof(PostingsDev), &p, sizeof(p));
+    PhraseSink F;
+    phrase_sink(segs, si, n_slots, reinterpret_cast<const uint32_t*>(d + off_pos), reinterpret_cast<const uint4*>(d + lists_pos), F);
+    F.consts = reinterpret_cast<const float4*>(d + consts_pos);
+    std::memcpy(h.data() + sinks_pos + si * sizeof(PhraseSink), &F, sizeof(F));
+  }
+  std::memcpy(h.data() + off_pos, J.slot_off, (nq + 1) * 4);
+  phrase_slot_lists(segs, n_segs, J, nq, reinterpret_cast<uint4*>(h.data() + lists_pos));
+  std::memcpy(h.data() + consts_pos, J.consts.data(), nq * sizeof(float4));
+  CU(c, cudaMemcpyAsync(b_sc.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
+  PhraseScoreParams P;
+  P.segs = reinterpret_cast<const PostingsDev*>(d);
+  P.sinks = reinterpret_cast<const PhraseSink*>(d + sinks_pos);
+  P.blocks_per_query = (limit + kEmitScoreThreads - 1) / kEmitScoreThreads;
+  P.limit = limit;
+  P.out = static_cast<EmitHit*>(out.bins);
+  P.n_out = static_cast<const uint32_t*>(out.nulls);
+  phrase_score_kernel<<<unsigned(nq * P.blocks_per_query), kEmitScoreThreads, 0, c->stream>>>(P);
+  ++c->launches;
+  CU(c, cudaGetLastError());
+  return SDBG_OK;
 }
 }  // namespace
 
@@ -3290,7 +3436,32 @@ extern "C" int sdbg_match_scan_batch_groups_min(sdbg_segment* const* segs, size_
   const PassBatch<sdbg_bm25_term> B(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt);
   if (scored)
     if (int rc = topk_checked(segs, n_segs, B)) return rc;
-  return scan_to_host(segs, n_segs, B, filt, {offset, limit, scored, k1, b}, out, n_out, total);
+  return scan_batch_to_host(segs, n_segs, B, filt, {offset, limit, scored, k1, b}, out, n_out, total);
+}
+
+extern "C" int sdbg_phrase_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                      const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
+                                      const sdbg_col_pred* filt, const sdbg_bm25_term* phrase_stats, float k1, float b,
+                                      const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out,
+                                      uint64_t* total) {
+  if (!limit || !out || !n_out || !total || (scored && !phrase_stats)) return SDBG_EINVAL;
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  if (PB.rc) return PB.rc;
+  sdbg_ctx* c = segs[0]->ctx;
+  if (scored)
+    if (int rc = topk_limits(c, nq, 1)) return rc;
+  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  if (B.rc) return B.rc;
+  if (scored) {
+    uint64_t ord = 0;
+    for (size_t si = 0; si < n_segs; ++si) ord += segs[si]->n_docs;
+    if (ord > kMaxDocId) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-2 docs per call");
+  }
+  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
+  PhraseJob J = PB.job(terms, phrase_off);
+  if (scored) J.consts = phrase_consts(segs, terms, phrase_off, nq, phrase_stats, k1, b);
+  return scan_to_host(c, nq, limit, [&](const CountOut& o) { return phrase_scan_run(segs, n_segs, B, filt, J, offset, limit, o); },
+                      out, n_out, total);
 }
 
 // ---- the count, facet, aggregate and sorted passes across GPUs ----

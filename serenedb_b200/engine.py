@@ -631,7 +631,107 @@ def ExecutePhraseTopK(reader, phrase, scorer, k, rel_pos=None, filt=None, thresh
     return hits[0, :n_out[0]], int(total[0])
 
 
-SORT_HIT_DTYPE = np.dtype([("value", "<i8"), ("doc", "<u4"), ("seg", "<u4"), ("is_null", "u1"), ("pad", "V7")])
+def ExecutePhraseTopKByColumnBatch(reader, phrases, sort_field, k, descending=False, nulls_first=False, rel_pos=None,
+                                   filt=None, exclude=None):
+    """Sorted scan of exact phrase queries (`WHERE body @@ '"new york"' ORDER BY col LIMIT k`,
+    sdbg_phrase_topk_by_column_batch): per phrase, the first k of the docs ExecutePhraseCountBatch counts, in the order of
+    ExecuteTopKByColumnBatch. phrases / rel_pos / exclude as in ExecutePhraseCountBatch. Returns the dict
+    ExecuteTopKByColumnBatch returns."""
+    vt = _sort_value_type(reader, sort_field)
+    nq = len(phrases)
+    hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
+    n_out = np.zeros(max(nq, 1), np.uint32)
+    N.check(N.lib().sdbg_phrase_topk_by_column_batch(_seg_array(reader.segments), len(reader.segments),
+                                                     *_phrase_args(phrases, rel_pos, exclude), _ref(filt), int(sort_field),
+                                                     int(bool(descending)), int(bool(nulls_first)), int(k), _ptr(hits),
+                                                     _ptr(n_out)), reader.segments[0].ctx._h)
+    return _sort_result(hits, n_out, nq, k, vt)
+
+
+def ExecutePhraseTopKByColumn(reader, phrase, sort_field, k, descending=False, nulls_first=False, rel_pos=None, filt=None,
+                              exclude=None):
+    """ExecutePhraseTopKByColumnBatch for one phrase: dict of docs, segs, values, nulls."""
+    return _sort_row(ExecutePhraseTopKByColumnBatch(reader, [list(phrase)], sort_field, k, descending, nulls_first,
+                                                    _one(rel_pos), filt, _one(exclude)))
+
+
+def ExecutePhraseFacetCountsBatch(reader, phrases, key_field, key_min=None, key_span=None, rel_pos=None, filt=None,
+                                  exclude=None):
+    """Facet counts of exact phrase queries (`WHERE body @@ '"new york"' GROUP BY col`, sdbg_phrase_facet_counts_batch):
+    per phrase, how the docs ExecutePhraseCountBatch counts split over the values of column `key_field`. The key range as
+    in ExecuteFacetCountsBatch. Returns the dict ExecuteFacetCountsBatch returns."""
+    key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
+    nq = len(phrases)
+    counts = np.zeros((max(nq, 1), max(int(key_span), 1)), np.uint64)
+    nulls = np.zeros(max(nq, 1), np.uint64)
+    N.check(N.lib().sdbg_phrase_facet_counts_batch(_seg_array(reader.segments), len(reader.segments),
+                                                   *_phrase_args(phrases, rel_pos, exclude), _ref(filt), int(key_field),
+                                                   int(key_min), int(key_span), _ptr(counts), _ptr(nulls)),
+            reader.segments[0].ctx._h)
+    return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
+
+
+def ExecutePhraseFacetCounts(reader, phrase, key_field, key_min=None, key_span=None, rel_pos=None, filt=None, exclude=None):
+    """ExecutePhraseFacetCountsBatch for one phrase: {key: count} plus {None: n} for NULL keys, as ExecuteFacetCounts."""
+    return _facet_row(ExecutePhraseFacetCountsBatch(reader, [list(phrase)], key_field, key_min, key_span, _one(rel_pos), filt,
+                                                    _one(exclude)))
+
+
+def ExecutePhraseMatchAggregatesBatch(reader, phrases, value_field, key_field=None, key_min=None, key_span=None, rel_pos=None,
+                                      filt=None, exclude=None):
+    """Aggregates over the matches of exact phrase queries (sdbg_phrase_aggregate_batch): per phrase, over the docs
+    ExecutePhraseCountBatch counts; the grouping and the result as in ExecuteMatchAggregatesBatch."""
+    vt, kf, key_min, key_span = _agg_args(reader, value_field, key_field, key_min, key_span)
+    nq = len(phrases)
+    out = np.zeros((max(nq, 1), max(int(key_span), 1)), MATCH_AGG_DTYPE)
+    null_out = np.zeros(max(nq, 1), MATCH_AGG_DTYPE)
+    N.check(N.lib().sdbg_phrase_aggregate_batch(_seg_array(reader.segments), len(reader.segments),
+                                                *_phrase_args(phrases, rel_pos, exclude), _ref(filt), kf, int(key_min),
+                                                int(key_span), int(value_field), _ptr(out), _ptr(null_out)),
+            reader.segments[0].ctx._h)
+    return _agg_result(out, null_out, nq, key_min, vt)
+
+
+def ExecutePhraseMatchAggregates(reader, phrase, value_field, key_field=None, key_min=None, key_span=None, rel_pos=None,
+                                 filt=None, exclude=None):
+    """ExecutePhraseMatchAggregatesBatch for one phrase, in the form ExecuteMatchAggregates returns."""
+    return _agg_row(ExecutePhraseMatchAggregatesBatch(reader, [list(phrase)], value_field, key_field, key_min, key_span,
+                                                      _one(rel_pos), filt, _one(exclude)), key_field is not None)
+
+
+def ExecutePhraseMatchScanBatch(reader, phrases, scorer=None, limit=1 << 20, offset=None, rel_pos=None, filt=None,
+                                exclude=None, boost=1.0):
+    """Stream mode of exact phrase queries (`SELECT id [, bm25(...)] ... WHERE body @@ '"new york"' LIMIT n OFFSET o`,
+    sdbg_phrase_scan_batch): per phrase, the docs ExecutePhraseCountBatch counts, in (segment, doc) order, from ordinal
+    offset[q] (None: 0) on, at most `limit` of them. scorer: BM25 / TFIDF to score each hit exactly as
+    ExecutePhraseTopKBatch scores it; None: unscored (every score 0). Returns what ExecuteMatchScanGroupsBatch returns."""
+    nq = len(phrases)
+    stats = None
+    if scorer is not None:
+        stats = (N.BM25Term * nq)(*[reader.phrase_stats(scorer, p, boost) for p in phrases])
+    offs = None if offset is None else np.ascontiguousarray(offset, dtype=np.uint64)
+    if offs is not None and offs.shape != (nq,):
+        raise ValueError("offset needs one value per query")
+    hits = np.zeros((nq, max(int(limit), 1)), HIT_DTYPE)
+    n_out = np.zeros(nq, np.uint32)
+    total = np.zeros(nq, np.uint64)
+    k1, b = (0.0, 0.0) if scorer is None else (scorer.k, scorer.b)
+    N.check(N.lib().sdbg_phrase_scan_batch(_seg_array(reader.segments), len(reader.segments),
+                                           *_phrase_args(phrases, rel_pos, exclude), _ref(filt), stats, k1, b, _ptr(offs),
+                                           int(limit), int(scorer is not None), _ptr(hits), _ptr(n_out), _ptr(total)),
+            reader.segments[0].ctx._h)
+    return [((hits["seg"][q, :n_out[q]].copy(), hits["doc"][q, :n_out[q]].copy(), hits["score"][q, :n_out[q]].copy()),
+             int(total[q])) for q in range(nq)]
+
+
+def ExecutePhraseMatchScan(reader, phrase, scorer=None, limit=1 << 20, offset=0, rel_pos=None, filt=None, exclude=None,
+                           boost=1.0):
+    """ExecutePhraseMatchScanBatch for one phrase: ((seg, doc, score) arrays, total matches)."""
+    return ExecutePhraseMatchScanBatch(reader, [list(phrase)], scorer, limit, [offset], _one(rel_pos), filt, _one(exclude),
+                                       boost)[0]
+
+
+SORT_HIT_DTYPE =np.dtype([("value", "<i8"), ("doc", "<u4"), ("seg", "<u4"), ("is_null", "u1"), ("pad", "V7")])
 _SORT_VALUE_DTYPE = {0: np.int64, 1: np.float64, 2: np.int32}
 
 

@@ -11,7 +11,8 @@
 // top-k, streaming and count adapters next to the same calls filtered by an indicator column of the chain
 // (tests/test_gpu_filter_chains.py). "scan" runs the Stream mode (GpuMatchScan) for flat, grouped and min-match queries
 // (tests/test_gpu_match_scan.py). "phrase" runs a phrase through the top-k and count adapters on a token corpus of its own
-// (tests/test_gpu_phrase.py).
+// (tests/test_gpu_phrase.py); "phrase columns" runs the same phrases through the sorted, facet, aggregate and Stream
+// adapters instead (tests/test_gpu_phrase_column.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -33,7 +34,11 @@ struct ListCollector final : irs::ScoreCollector {  // a trivial ScoreCollector:
 // tests/test_gpu_phrase.py rebuilds: doc i (1-based) has 1 + r % 16 tokens, each token r % 6, r the next value of
 // r = r * 1664525 + 1013904223 (mod 2^32) >> 16 from state 12345, docs in order. Norms are the doc lengths. One line per
 // phrase: its slots and positions, the excluded term, the hits, total_matches and the count.
-int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs) {
+// With `columns`, the int64 column 20 holds (d * 7919) % 23 - 11 for doc d, NULL when d % 5 == 0, and each line holds
+// instead: GpuSortedScan ORDER BY column 20 DESC NULLS LAST LIMIT 30 (docs, values, valid), GpuFacetScan GROUP BY column 20
+// (keys, counts, valid), GpuMatchAggScan of column 20 without GROUP BY (count, count_value, sum_lo, min, max), and the
+// scored GpuMatchScan (docs, scores, total).
+int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns) {
   uint32_t state = 12345u;
   auto next = [&]() { state = state * 1664525u + 1013904223u; return state >> 16; };
   constexpr uint32_t kVocab = 6;
@@ -69,7 +74,19 @@ int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs) {
   for (uint32_t t = 0; t < kVocab; ++t) { flat.insert(flat.end(), pos[t].begin(), pos[t].end()); off.push_back(flat.size()); }
   if (!rc) rc = sdbg_stage_positions(seg, flat.data(), off.data(), kVocab);
   if (w) sdbg_writer_destroy(w);
+  std::vector<int64_t> key(n_docs);
+  std::vector<uint64_t> valid_bits((n_docs + 63) / 64, 0);
+  for (uint32_t d = 1; d <= n_docs; ++d) {
+    key[d - 1] = int64_t((uint64_t(d) * 7919u) % 23u) - 11;
+    if (d % 5u) valid_bits[(d - 1) / 64] |= uint64_t(1) << ((d - 1) % 64);
+  }
+  if (!rc && columns) rc = sdbg_stage_column(seg, 20, SDBG_I64, key.data(), valid_bits.data(), n_docs);
   if (rc) { std::printf("{\"error\": %d}\n", rc); return 1; }
+  auto ints = [](const char* f, const auto& v) {
+    std::printf(", \"%s\": [", f);
+    for (size_t i = 0; i < v.size(); ++i) std::printf("%s%lld", i ? ", " : "", static_cast<long long>(v[i]));
+    std::printf("]");
+  };
   struct Case { std::vector<uint32_t> slots, rel, excl; };
   const Case cases[] = {{{1, 0}, {0, 1}, {}}, {{2, 2, 4}, {0, 1, 3}, {5}}};
   ListCollector col;
@@ -79,6 +96,40 @@ int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs) {
     for (size_t i = 0; i < terms.size(); ++i) {
       sdbg_bm25_collect(n_docs, sum_len, docs[cs.slots[i]].size(), 1.2f, 0.75f, &terms[i]);
       terms[i].term = cs.slots[i];
+    }
+    if (columns) {
+      std::printf("{\"slots\": [");
+      for (size_t i = 0; i < cs.slots.size(); ++i) std::printf("%s%u", i ? ", " : "", cs.slots[i]);
+      std::printf("]");
+      ints("rel", cs.rel);
+      ints("excl", cs.excl);
+      duckdb::DataChunkMock out;
+      sdbg_host::GpuSortedScan sorted({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, 20, true, false, 30, {}, {}, cs.rel);
+      for (sorted.Scan(out); out.size; sorted.Scan(out)) { ints("sorted_docs", out.doc); ints("sorted_values", out.value); ints("sorted_valid", out.valid); }
+      sdbg_host::GpuFacetScan facet({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, 20, {}, {}, cs.rel);
+      std::vector<int64_t> keys, counts, valid;
+      for (facet.Scan(out); out.size; facet.Scan(out)) {
+        keys.insert(keys.end(), out.key.begin(), out.key.end());
+        counts.insert(counts.end(), out.count.begin(), out.count.end());
+        valid.insert(valid.end(), out.valid.begin(), out.valid.end());
+      }
+      ints("facet_keys", keys); ints("facet_counts", counts); ints("facet_valid", valid);
+      sdbg_host::GpuMatchAggScan agg({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, UINT64_MAX, 20, SDBG_I64, {}, {}, cs.rel);
+      agg.Scan(out);
+      ints("agg_count", out.count); ints("agg_count_value", out.count_value); ints("agg_sum_lo", out.sum_lo);
+      ints("agg_min", out.min); ints("agg_max", out.max);
+      sdbg_host::GpuMatchScan scan({seg}, terms, cs.excl, nullptr, 1.2f, 0.75f, true, {}, {}, cs.rel);
+      std::vector<uint32_t> sdocs;
+      std::vector<float> sscores;
+      for (scan.Scan(out); out.size; scan.Scan(out)) {
+        sdocs.insert(sdocs.end(), out.doc.begin(), out.doc.end());
+        sscores.insert(sscores.end(), out.score.begin(), out.score.end());
+      }
+      ints("scan_docs", sdocs);
+      std::printf(", \"scan_scores\": [");
+      for (size_t i = 0; i < sscores.size(); ++i) std::printf("%s%.9g", i ? ", " : "", double(sscores[i]));
+      std::printf("], \"scan_total\": %llu}\n", static_cast<unsigned long long>(scan.total_matches()));
+      continue;
     }
     sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_AND, terms, 1.2f, 0.75f, 50, nullptr, cs.excl, {}, {}, cs.rel);
     col.docs.clear();
@@ -108,7 +159,7 @@ int main(int argc, char** argv) {
   sdbg_ctx* ctx = nullptr;
   int rc = sdbg_init(0, &ctx);
   if (rc != SDBG_OK) { std::printf("{\"error\": %d}\n", rc); return rc == SDBG_ENODEVICE ? 3 : 1; }
-  if (argc > 2 && std::string(argv[2]) == "phrase") return phrase_mode(ctx, n_docs);
+  if (argc > 2 && std::string(argv[2]) == "phrase") return phrase_mode(ctx, n_docs, argc > 3 && std::string(argv[3]) == "columns");
   sdbg_segment* seg = nullptr;
   sdbg_segment_create(ctx, n_docs, &seg);
   std::vector<uint32_t> dc(8);

@@ -275,10 +275,11 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
 GpuSortedScan::GpuSortedScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                              std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t sort_field,
                              bool descending, bool nulls_first, uint32_t k, std::vector<uint32_t> group_sizes,
-                             std::vector<uint32_t> group_min_match)
+                             std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), filter_(table_filter),
-      field_(sort_field), desc_(descending), nulls_first_(nulls_first), k_(k) {
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
+      filter_(table_filter), field_(sort_field), desc_(descending), nulls_first_(nulls_first), k_(k) {
+  check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
 }
 
 void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
@@ -290,7 +291,13 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
     uint32_t n = 0;
     int rc;
     const char* what;
-    if (group_sizes_.empty()) {
+    if (!phrase_.empty()) {
+      const uint32_t phrase_off[2] = {0, uint32_t(terms_.size())};
+      rc = sdbg_phrase_topk_by_column_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), phrase_off, 1, excluded_.data(),
+                                            excl_off, filter_.data(), field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
+                                            hits_.data(), &n);
+      what = "sdbg_phrase_topk_by_column_batch: ";
+    } else if (group_sizes_.empty()) {
       rc = sdbg_match_topk_by_column_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                            filter_.data(), field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
                                            hits_.data(), &n);
@@ -322,10 +329,13 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
 
 GpuMatchScan::GpuMatchScan(std::vector<sdbg_segment*> segments, std::vector<sdbg_bm25_term> terms,
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, float k1, float b, bool scored,
-                           std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)
+                           std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
+                           std::vector<uint32_t> phrase_positions)
     : segs_(std::move(segments)), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(group_sizes.empty() ? std::vector<uint32_t>{uint32_t(terms_.size())} : std::move(group_sizes)),
-      group_min_(std::move(group_min_match)), filter_(table_filter), k1_(k1), b_(b), scored_(scored) {
+      group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)), filter_(table_filter), k1_(k1), b_(b),
+      scored_(scored) {
+  check_phrase(phrase_, terms_.size(), group_sizes_.size() > 1 || !group_min_.empty());
 }
 
 void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kPage - 1
@@ -334,12 +344,24 @@ void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kP
   const uint32_t excl_off[2] = {0, uint32_t(excluded_.size())};
   page_.resize(kPage);
   uint32_t n = 0;
-  const int rc = sdbg_match_scan_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
-                                                  group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(), excl_off,
-                                                  k1_, b_, filter_.data(), &offset_, kPage, scored_ ? 1 : 0, page_.data(), &n,
-                                                  &total_);
-  if (rc != SDBG_OK)
-    throw GpuError(rc, std::string("sdbg_match_scan_batch_groups_min: ") + sdbg_last_error(sdbg_segment_context(segs_[0])));
+  int rc;
+  const char* what;
+  if (!phrase_.empty()) {
+    std::vector<uint32_t> ids(terms_.size());
+    for (size_t i = 0; i < ids.size(); ++i) ids[i] = terms_[i].term;
+    const sdbg_bm25_term stats = phrase_stats(terms_);
+    const uint32_t phrase_off[2] = {0, uint32_t(ids.size())};
+    rc = sdbg_phrase_scan_batch(segs_.data(), segs_.size(), ids.data(), phrase_.data(), phrase_off, 1, excluded_.data(), excl_off,
+                                filter_.data(), scored_ ? &stats : nullptr, k1_, b_, &offset_, kPage, scored_ ? 1 : 0,
+                                page_.data(), &n, &total_);
+    what = "sdbg_phrase_scan_batch: ";
+  } else {
+    rc = sdbg_match_scan_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
+                                          group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(), excl_off,
+                                          k1_, b_, filter_.data(), &offset_, kPage, scored_ ? 1 : 0, page_.data(), &n, &total_);
+    what = "sdbg_match_scan_batch_groups_min: ";
+  }
+  if (rc != SDBG_OK) throw GpuError(rc, std::string(what) + sdbg_last_error(sdbg_segment_context(segs_[0])));
   page_.resize(n);
   offset_ += kPage;
   cursor_ = 0;
@@ -362,10 +384,12 @@ void GpuMatchScan::Scan(duckdb::DataChunkMock& output) {
 
 GpuFacetScan::GpuFacetScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
-                           std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match)
+                           std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
+                           std::vector<uint32_t> phrase_positions)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), filter_(table_filter),
-      field_(key_field) {
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
+      filter_(table_filter), field_(key_field) {
+  check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
 }
 
 void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
@@ -388,7 +412,12 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
     std::vector<uint64_t> counts(span);
     int rc;
     const char* what;
-    if (group_sizes_.empty()) {
+    if (!phrase_.empty()) {
+      const uint32_t phrase_off[2] = {0, uint32_t(terms_.size())};
+      rc = sdbg_phrase_facet_counts_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), phrase_off, 1, excluded_.data(),
+                                          excl_off, filter_.data(), field_, lo, uint32_t(span), counts.data(), &nulls_);
+      what = "sdbg_phrase_facet_counts_batch: ";
+    } else if (group_sizes_.empty()) {
       rc = sdbg_match_facet_counts_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                          filter_.data(), field_, lo, uint32_t(span), counts.data(), &nulls_);
       what = "sdbg_match_facet_counts_batch: ";
@@ -421,10 +450,11 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
 GpuMatchAggScan::GpuMatchAggScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                                  std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
                                  uint64_t value_field, sdbg_type value_type, std::vector<uint32_t> group_sizes,
-                                 std::vector<uint32_t> group_min_match)
+                                 std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
-      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), filter_(table_filter),
-      key_field_(key_field), value_field_(value_field), value_type_(value_type) {
+      group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
+      filter_(table_filter), key_field_(key_field), value_field_(value_field), value_type_(value_type) {
+  check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
 }
 
 void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
@@ -454,7 +484,13 @@ void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
     sdbg_match_agg null_cell{};
     int rc;
     const char* what;
-    if (group_sizes_.empty()) {
+    if (!phrase_.empty()) {
+      const uint32_t phrase_off[2] = {0, uint32_t(terms_.size())};
+      rc = sdbg_phrase_aggregate_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), phrase_off, 1, excluded_.data(),
+                                       excl_off, filter_.data(), key_field_, lo, uint32_t(span), value_field_, cells.data(),
+                                       &null_cell);
+      what = "sdbg_phrase_aggregate_batch: ";
+    } else if (group_sizes_.empty()) {
       rc = sdbg_match_aggregate_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                       filter_.data(), key_field_, lo, uint32_t(span), value_field_, cells.data(),
                                       &null_cell);

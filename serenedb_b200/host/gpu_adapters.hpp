@@ -145,7 +145,7 @@ class GpuCountScan {
 // SELECT ... FROM t WHERE body @@ '<query>' [AND <pushed filter>] ORDER BY col [DESC] [NULLS FIRST|LAST] LIMIT k -- the body
 // of the TOP_N(col) <- IRESEARCH_SCAN(Stream) plan shape (duckdb_search_full_scan.cpp IResearchSetScanOrder :1711-1762 pushes
 // only score orders; RunStreamingScan :2370-2403 serves the rest under TOP_N). One sdbg_match_topk_by_column_batch call
-// (sdbg_match_topk_by_column_batch_groups_min with group_sizes) on the first Scan; then rows (doc, segment, value, valid) in TOP_N's order, <= STANDARD_VECTOR_SIZE per call,
+// (sdbg_match_topk_by_column_batch_groups_min with group_sizes, sdbg_phrase_topk_by_column_batch with phrase_positions) on the first Scan; then rows (doc, segment, value, valid) in TOP_N's order, <= STANDARD_VECTOR_SIZE per call,
 // cardinality 0 at the end.
 class GpuSortedScan {
  public:
@@ -154,13 +154,15 @@ class GpuSortedScan {
                 uint64_t sort_field, bool descending, bool nulls_first /* the plan's resolved OrderByNullType */,
                 uint32_t k /* LIMIT (+ OFFSET), 1..4096 */,
                 std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
-                std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
+                std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+                std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
+                                                               relative positions (0 first, increasing) */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_;
   FilterChain filter_;
   uint64_t field_;
   bool desc_, nulls_first_;
@@ -172,7 +174,8 @@ class GpuSortedScan {
 
 // SELECT id [, bm25(...)] FROM t WHERE body @@ '<query>' [AND <pushed filter>] [LIMIT n OFFSET o] without ORDER BY -- the
 // body of the Stream scan mode (duckdb_search_full_scan.cpp RunStreamingScan :2370-2403) for flat, grouped and min-match
-// queries over every segment. Pages of kPage matches come from sdbg_match_scan_batch_groups_min (offset += kPage); Scan
+// queries and phrases over every segment. Pages of kPage matches come from sdbg_match_scan_batch_groups_min
+// (sdbg_phrase_scan_batch with phrase_positions, scored with the phrase's summed idfs) (offset += kPage); Scan
 // emits rows (doc, segment, score) of at most STANDARD_VECTOR_SIZE in (segment, doc) order, cardinality 0 at the end.
 // Scores are those of the top-k at pruning level 0 when `scored`, else 0 (no frequency or norm is read).
 class GpuMatchScan {
@@ -182,7 +185,9 @@ class GpuMatchScan {
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
                float k1, float b, bool scored,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors over `terms`; empty = one group (a flat OR) */,
-               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+               std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
+                                                              relative positions (0 first, increasing) */);
   void Scan(duckdb::DataChunkMock& output);
   uint64_t total_matches() const { return total_; }
 
@@ -190,7 +195,7 @@ class GpuMatchScan {
   void Fetch();
   std::vector<sdbg_segment*> segs_;
   std::vector<sdbg_bm25_term> terms_;
-  std::vector<uint32_t> excluded_, group_sizes_, group_min_;
+  std::vector<uint32_t> excluded_, group_sizes_, group_min_, phrase_;
   FilterChain filter_;
   float k1_, b_;
   bool scored_;
@@ -203,7 +208,7 @@ class GpuMatchScan {
 // SELECT col, count(*) FROM t WHERE body @@ '<query>' [AND <pushed filter>] GROUP BY col -- the body of the
 // HASH_GROUP_BY(col; count_star()) <- IRESEARCH_SCAN(text query) plan shape (facet counts). The first Scan takes the key
 // range from sdbg_column_minmax_i64 over the segments and runs one sdbg_match_facet_counts_batch call
-// (sdbg_match_facet_counts_batch_groups_min with group_sizes); then the non-empty
+// (sdbg_match_facet_counts_batch_groups_min with group_sizes, sdbg_phrase_facet_counts_batch with phrase_positions); then the non-empty
 // groups as rows (key, count, valid) in ascending key order, the NULL group (valid = 0) last, <= STANDARD_VECTOR_SIZE per
 // call, cardinality 0 at the end. A key range wider than 32768 throws GpuError(SDBG_EUNSUPPORTED): the plan stays on the CPU.
 class GpuFacetScan {
@@ -212,13 +217,15 @@ class GpuFacetScan {
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
                uint64_t key_field /* int64 or int32 */,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
-               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+               std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
+                                                              relative positions (0 first, increasing) */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_;
   FilterChain filter_;
   uint64_t field_;
   std::vector<std::pair<int64_t, uint64_t>> groups_;   // (key, count) of the non-empty groups
@@ -231,7 +238,7 @@ class GpuFacetScan {
 // [GROUP BY col] -- the body of the HASH_GROUP_BY(col; count_star(), count(v), sum(v), avg(v), min(v), max(v)) and
 // UNGROUPED_AGGREGATE(...) <- IRESEARCH_SCAN(text query) plan shapes, for one value column (two columns: two scans). The
 // first Scan takes the key range as GpuFacetScan does and runs one sdbg_match_aggregate_batch call
-// (sdbg_match_aggregate_batch_groups_min with group_sizes). Grouped, it then emits the non-empty groups as rows (key, count,
+// (sdbg_match_aggregate_batch_groups_min with group_sizes, sdbg_phrase_aggregate_batch with phrase_positions). Grouped, it then emits the non-empty groups as rows (key, count,
 // count_value, sum_lo / sum_hi or sum_f64, avg, min, max, valid) in ascending key order, the NULL group (valid = 0) last;
 // ungrouped (key_field UINT64_MAX), one row. <= STANDARD_VECTOR_SIZE rows per call, cardinality 0 at the end. A row with
 // count_value 0 has NULL sum, avg, min and max (emitted as 0). A key range wider than 4096 values throws
@@ -243,13 +250,15 @@ class GpuMatchAggScan {
                   uint64_t key_field /* int64 or int32; UINT64_MAX: no GROUP BY */, uint64_t value_field,
                   sdbg_type value_type /* as staged: picks sum_f64 or the 128-bit sum for avg */,
                   std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
-                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */);
+                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+                  std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
+                                                                 relative positions (0 first, increasing) */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_;
   FilterChain filter_;
   uint64_t key_field_, value_field_;
   sdbg_type value_type_;

@@ -7,8 +7,15 @@ four-word phrases. For each batch it reports ms per step (CUDA events on the lib
 warm-up) of
   phrase count (sdbg_phrase_count_batch)   against   AND count of the same terms (sdbg_match_count_batch)
   phrase top-1000 (sdbg_phrase_topk_batch) against   AND top-1000 (sdbg_bm25_topk_batch at pruning level 0)
-and the matches of both. The AND is the phrase's candidate set, so the gap is the cost of checking positions. Prints one
-JSON line with the GPU name and power limit read in the same run.
+and the matches of both. The AND is the phrase's candidate set, so the gap is the cost of checking positions. Then the
+four passes of the phrases' matches, next to the phrase count, over two staged columns (an int64 column `ts` of uniform
+values and an int32 column `cat` of 100 values):
+  sorted LIMIT 1000 by ts (sdbg_phrase_topk_by_column_batch, pruning level 2 as shipped)
+  facets GROUP BY cat (sdbg_phrase_facet_counts_batch)
+  SUM / AVG(ts) GROUP BY cat (sdbg_phrase_aggregate_batch)
+  the first scan page of 1000, unscored and scored (sdbg_phrase_scan_batch), and an unscored page of 1000 from the
+  middle of each phrase's matches (a page deep in the result repeats the phrase check over the items before it).
+Prints one JSON line with the GPU name and power limit read in the same run.
 
     python tools/phrase_bench.py [--steps 5] [--warmup 2] [--docs 10000000] [--queries 4096]
 """
@@ -82,6 +89,9 @@ def main():
     seg.stage_postings(c["doc_bytes"], c["metas"])
     seg.stage_norms(c["lens"].astype(np.uint8), 1)
     seg.stage_positions(c["positions"], c["term_pos_off"])
+    crng = np.random.default_rng(13)
+    seg.stage_column(1, crng.integers(0, 1 << 40, c["n"]).astype(np.int64))   # ts
+    seg.stage_column(2, crng.integers(0, 100, c["n"]).astype(np.int32))       # cat
     reader = sdb.IndexReader([seg], c["n"], int(c["lens"].sum()), c["dwt"])
     scorer = sdb.BM25()
     rng = np.random.default_rng(11)
@@ -100,6 +110,26 @@ def main():
         r["and_count_ms"] = timed(ctx, lambda: sdb.ExecuteCountBatch(reader, conj, sdb.AND), a.steps, a.warmup)
         r["phrase_top1000_ms"] = timed(ctx, lambda: sdb.ExecutePhraseTopKBatch(reader, qs, scorer, 1000), a.steps, a.warmup)
         r["and_top1000_ms"] = timed(ctx, lambda: sdb.ExecuteTopKBatch(reader, conj, sdb.AND, scorer, 1000), a.steps, a.warmup)
+        # the four passes over the same phrases; each is checked against the count before it is timed
+        ctx.set_wand(2)
+        srt = sdb.ExecutePhraseTopKByColumnBatch(reader, qs, 1, 1000)
+        fac = sdb.ExecutePhraseFacetCountsBatch(reader, qs, 2, 0, 100)
+        agg = sdb.ExecutePhraseMatchAggregatesBatch(reader, qs, 1, 2, 0, 100)
+        scan = sdb.ExecutePhraseMatchScanBatch(reader, qs, None, 1000)
+        mid = np.ascontiguousarray(pc // 2, dtype=np.uint64)
+        if (not np.array_equal(srt["n_out"], np.minimum(pc, 1000)) or not np.array_equal(fac["counts"].sum(1), pc)
+                or not np.array_equal(agg["count"].sum(1), pc) or [t for _, t in scan] != pc.tolist()):
+            raise SystemExit("phrase pass / count mismatch")
+        r["phrase_sorted1000_ms"] = timed(ctx, lambda: sdb.ExecutePhraseTopKByColumnBatch(reader, qs, 1, 1000), a.steps, a.warmup)
+        ctx.set_wand(0)
+        r["phrase_facets_ms"] = timed(ctx, lambda: sdb.ExecutePhraseFacetCountsBatch(reader, qs, 2, 0, 100), a.steps, a.warmup)
+        r["phrase_sum_avg_ms"] = timed(ctx, lambda: sdb.ExecutePhraseMatchAggregatesBatch(reader, qs, 1, 2, 0, 100), a.steps,
+                                       a.warmup)
+        r["phrase_scan1000_ms"] = timed(ctx, lambda: sdb.ExecutePhraseMatchScanBatch(reader, qs, None, 1000), a.steps, a.warmup)
+        r["phrase_scan1000_scored_ms"] = timed(ctx, lambda: sdb.ExecutePhraseMatchScanBatch(reader, qs, scorer, 1000), a.steps,
+                                               a.warmup)
+        r["phrase_scan1000_mid_ms"] = timed(ctx, lambda: sdb.ExecutePhraseMatchScanBatch(reader, qs, None, 1000, mid), a.steps,
+                                            a.warmup)
         out["batches"][name] = r
     print(json.dumps(out))
 
