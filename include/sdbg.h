@@ -542,6 +542,70 @@ int sdbg_phrase_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint3
                            const sdbg_bm25_term* phrase_stats /* n_queries; NULL when scored == 0 */, float k1, float b,
                            const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit, int scored,
                            sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
+/* Conjunctions of phrases, terms and negated phrases (`"new york" & pizza & !"deep dish"`). Query q is an AND of the
+ * clauses query_clause_off[q] .. query_clause_off[q+1]) (at least one), plus excl_terms / excl_off and the filter chain
+ * as above. Clause j is a phrase exactly as above, of slots clause_off[j] .. clause_off[j+1]) (at least one; rel_pos
+ * starting at 0 in each clause and strictly increasing; rel_pos NULL: adjacent within each clause); a one-slot clause is a
+ * plain term. Clause j is negated when clause_negated[j] != 0 (clause_negated NULL: none); a query needs a positive
+ * clause. At most 16 slots per query, positive and negated clauses together. Doc d matches when every positive clause
+ * has phrase frequency > 0 in d, every negated clause phrase frequency 0, d is not deleted, passes the filter chain and
+ * holds none of the excluded terms. A term of a positive clause that a segment holds no postings for makes the query match
+ * nothing there; a term of a negated clause that a segment does not hold makes that clause exclude nothing there (a
+ * one-slot negated clause behaves exactly as that term among excl_terms).
+ * Score (the top-k, and the scan with scored != 0): the fp32 sum, from 0, of bm25(phrase frequency, norm(d)) over the
+ * positive clauses, each with its own statistics clause_stats[j] (one per clause, .term ignored, negated clauses' entries
+ * ignored; engine.py sums each clause's idfs in slot order), in ascending cost order within d's segment: a clause costs the
+ * smallest docs_count of its terms in that segment, ties in the query's clause order. For queries of one-slot clauses of
+ * distinct terms that is the order of sdbg_bm25_topk_batch's conjunctions, whose results these entries then reproduce
+ * bit for bit at pruning level 0; a query of one positive clause gives exactly the sdbg_phrase_* result for that phrase
+ * (which is how those entries run). Nothing is pruned: identical at every pruning level, k <= 4096.
+ * Each entry takes the parameters of its sdbg_phrase_* counterpart, with (terms, rel_pos, phrase_off) replaced by
+ * (terms, rel_pos, clause_off, clause_negated, query_clause_off) and phrase_stats by clause_stats; outputs, orders, NULL
+ * rules and scratch are the counterpart's (the clause tables add 16 B per clause and segment, and 16 B of statistics per
+ * clause when scored). Errors, all found before anything is queued: an empty clause, a query without a clause or without
+ * a positive clause, bad rel_pos, decreasing offsets, NULL arrays with non-empty ranges, NULL clause_stats where a score
+ * is needed: SDBG_EINVAL; more than 16 slots in a query, more than 16 excluded ids, k > 4096: SDBG_EUNSUPPORTED; a
+ * segment without staged positions: SDBG_ENOTFOUND; otherwise the counterpart's. Synchronous. */
+int sdbg_phrase_and_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                const uint32_t* rel_pos /* NULL: adjacent within each clause */, const uint32_t* clause_off,
+                                const uint8_t* clause_negated /* NULL: none */, const uint32_t* query_clause_off,
+                                size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                const sdbg_col_pred* filt, uint64_t* counts);
+int sdbg_phrase_and_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                               const uint32_t* rel_pos /* NULL: adjacent within each clause */, const uint32_t* clause_off,
+                               const uint8_t* clause_negated /* NULL: none */, const uint32_t* query_clause_off,
+                               size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                               const sdbg_bm25_term* clause_stats /* one per clause */, float k1, float b,
+                               const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out /* n_queries * k */,
+                               uint32_t* n_out, uint64_t* total_matches);
+int sdbg_phrase_and_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                         const uint32_t* rel_pos /* NULL: adjacent within each clause */,
+                                         const uint32_t* clause_off, const uint8_t* clause_negated /* NULL: none */,
+                                         const uint32_t* query_clause_off, size_t n_queries, const uint32_t* excl_terms,
+                                         const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                                         uint64_t sort_field, int descending, int nulls_first, uint32_t k,
+                                         sdbg_sort_hit* out /* n_queries * k */, uint32_t* n_out);
+int sdbg_phrase_and_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                       const uint32_t* rel_pos /* NULL: adjacent within each clause */,
+                                       const uint32_t* clause_off, const uint8_t* clause_negated /* NULL: none */,
+                                       const uint32_t* query_clause_off, size_t n_queries, const uint32_t* excl_terms,
+                                       const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt, uint64_t key_field,
+                                       int64_t key_min, uint32_t key_span, uint64_t* counts /* n_queries * key_span */,
+                                       uint64_t* null_counts /* n_queries */);
+int sdbg_phrase_and_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                    const uint32_t* rel_pos /* NULL: adjacent within each clause */,
+                                    const uint32_t* clause_off, const uint8_t* clause_negated /* NULL: none */,
+                                    const uint32_t* query_clause_off, size_t n_queries, const uint32_t* excl_terms,
+                                    const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt, uint64_t key_field,
+                                    int64_t key_min, uint32_t key_span, uint64_t value_field,
+                                    sdbg_match_agg* out /* n_queries * key_span */, sdbg_match_agg* null_out /* n_queries */);
+int sdbg_phrase_and_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                               const uint32_t* rel_pos /* NULL: adjacent within each clause */, const uint32_t* clause_off,
+                               const uint8_t* clause_negated /* NULL: none */, const uint32_t* query_clause_off,
+                               size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                               const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats /* NULL when scored == 0 */,
+                               float k1, float b, const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit,
+                               int scored, sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

@@ -14,6 +14,8 @@ from .engine import ExecutePhraseCount, ExecutePhraseCountBatch, ExecutePhraseTo
 from .engine import (ExecutePhraseTopKByColumn, ExecutePhraseTopKByColumnBatch, ExecutePhraseFacetCounts,
                      ExecutePhraseFacetCountsBatch, ExecutePhraseMatchAggregates, ExecutePhraseMatchAggregatesBatch,
                      ExecutePhraseMatchScan, ExecutePhraseMatchScanBatch)
+from .engine import (ExecutePhraseAndCount, ExecutePhraseAndCountBatch, ExecutePhraseAndTopK, ExecutePhraseAndTopKBatch, ExecutePhraseAndTopKByColumn, ExecutePhraseAndTopKByColumnBatch,
+                     ExecutePhraseAndFacetCounts, ExecutePhraseAndFacetCountsBatch, ExecutePhraseAndMatchAggregates, ExecutePhraseAndMatchAggregatesBatch, ExecutePhraseAndMatchScan, ExecutePhraseAndMatchScanBatch)
 from .engine import (AND, OR, BM25, TFIDF, FLT_MIN, Context, ExecuteCount, ExecuteCountBatch, ExecuteCountGroups,
                      ExecuteCountGroupsBatch, ExecuteFacetCounts, ExecuteFacetCountsBatch, ExecuteFacetCountsGroups,
                      ExecuteFacetCountsGroupsBatch, ExecuteMatchAggregates, ExecuteMatchAggregatesBatch,
@@ -36,4 +38,5 @@ __all__ = ["AND", "OR", "BM25", "TFIDF", "FLT_MIN", "Context", "ExecuteCount", "
            "merge_topk_groups_gathered", "ExecutePhraseCount", "ExecutePhraseCountBatch", "ExecutePhraseTopK",
            "ExecutePhraseTopKBatch", "ExecutePhraseTopKByColumn", "ExecutePhraseTopKByColumnBatch", "ExecutePhraseFacetCounts",
            "ExecutePhraseFacetCountsBatch", "ExecutePhraseMatchAggregates", "ExecutePhraseMatchAggregatesBatch",
-           "ExecutePhraseMatchScan", "ExecutePhraseMatchScanBatch"]
+           "ExecutePhraseMatchScan", "ExecutePhraseMatchScanBatch", "ExecutePhraseAndCount", "ExecutePhraseAndCountBatch", "ExecutePhraseAndTopK", "ExecutePhraseAndTopKBatch",
+           "ExecutePhraseAndTopKByColumn", "ExecutePhraseAndTopKByColumnBatch", "ExecutePhraseAndFacetCounts", "ExecutePhraseAndFacetCountsBatch", "ExecutePhraseAndMatchAggregates", "ExecutePhraseAndMatchAggregatesBatch", "ExecutePhraseAndMatchScan", "ExecutePhraseAndMatchScanBatch"]

@@ -116,6 +116,18 @@ SIGNATURES = {
                                               C.c_uint64, _vp, _vp]),
     "sdbg_phrase_scan_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _vp,
                                          C.c_uint32, C.c_int, _vp, _vp, _vp]),
+    # the clause conjunctions: (terms, rel_pos, clause_off, clause_negated, query_clause_off, n_queries) for the phrase args
+    "sdbg_phrase_and_count_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "sdbg_phrase_and_topk_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_float, C.c_float, _vp,
+                                             C.c_uint32, C.c_float, _vp, _vp, _vp]),
+    "sdbg_phrase_and_topk_by_column_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int,
+                                                       C.c_int, C.c_uint32, _vp, _vp]),
+    "sdbg_phrase_and_facet_counts_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,
+                                                     C.c_uint32, _vp, _vp]),
+    "sdbg_phrase_and_aggregate_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,
+                                                  C.c_uint32, C.c_uint64, _vp, _vp]),
+    "sdbg_phrase_and_scan_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, C.c_float, C.c_float,
+                                             _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
     "sdbg_match_topk_by_column_batch":(C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int, C.c_int,
                                                   C.c_uint32, _vp, _vp]),
     "sdbg_match_facet_counts_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,

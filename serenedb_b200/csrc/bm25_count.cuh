@@ -137,8 +137,9 @@ __device__ __forceinline__ bool range_has_bits(const uint32_t* bm, const uint4& 
   return __any_sync(kFull, any != 0u);
 }
 
-// The phrase check inlined into the sorted scan's and the facet pass's sinks spills a word under ptxas's own register
-// choice; at least 4 CTAs per SM (64 registers) it does not. Every other instantiation has no minimum.
+// The clause check inlined into the phrase instantiations spills under ptxas's own register choice (the phrase sink, the
+// sorted scan's and the facet pass's); at least 4 CTAs per SM (64 registers) none does. Every other instantiation has no
+// minimum.
 constexpr int kPhraseMinBlocks = 4;
 
 // kAnd: conjunction (else disjunction). kGroups: conjunction of OR groups (CountParams::grp_end). The term loops are not
@@ -160,12 +161,14 @@ constexpr int kPhraseMinBlocks = 4;
 // gives each doc its ordinal, base[item.w] plus the matches of the item's earlier windows; the docs whose ordinal lies in
 // [offset[q], offset[q] + limit) go to their row of P.emit.out, unscored. An item whose ordinals miss the page exits
 // before it decodes anything, and an item stops after the window that fills the page.
-// kPhrase (with kAnd): the phrase check (bm25_phrase.cuh). Every doc that survives the conjunction, the exclusions, the
-// deleted docs and the filter chain is probed in each slot's list for its positions; a doc of phrase frequency 0 is
-// dropped, the others are counted and, with P.phrase.cap, scored from their phrase frequency and kept in a buffer of
-// P.phrase.cap keys in dynamic shared memory as the sorted scan keeps its keys; the item's k best go to slot item.w.
-// kPhrase with one other sink: with kFacet, kAgg or kEmit the phrase check is a stage that narrows `acc` after the
-// exclusions (deleted docs, filter chain, then phrase_freq per surviving bit, written back), so the sink reads only phrase
+// kPhrase (with kAnd, the conjunction of the positive clauses' terms): the clause check (phrase_clauses,
+// bm25_phrase.cuh). Every doc that survives the conjunction, the exclusions, the deleted docs and the filter chain is
+// probed, clause after clause of the query's clause table, in each slot's list for its positions; a doc that fails a
+// clause is dropped, the others are counted and, with P.phrase.cap, scored as the sum of their positive clauses' scores
+// and kept in a buffer of P.phrase.cap keys in dynamic shared memory as the sorted scan keeps its keys; the item's k best
+// go to slot item.w. Without a score the one-slot positive clauses, which the conjunction guarantees, are skipped.
+// kPhrase with one other sink: with kFacet, kAgg or kEmit the clause check is a stage that narrows `acc` after the
+// exclusions (deleted docs, filter chain, then the check per surviving bit, written back), so the sink reads only
 // matches and emit passes A and B see the same set. With kSort it runs inside the sink, on a doc whose key has passed
 // s_thr: a doc that cannot enter the buffer is never probed for positions.
 // The sinks take kGroups queries: the groups narrow `acc` before the sink reads the column, and the bit-sliced counter
@@ -173,7 +176,7 @@ constexpr int kPhraseMinBlocks = 4;
 // to 16 B).
 template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false, bool kAgg = false, bool kEmit = false,
           bool kPhrase = false>
-__global__ void __launch_bounds__(kCountThreads, kPhrase && (kSort || kFacet) ? kPhraseMinBlocks : 0) bm25_count_kernel(CountParams P) {
+__global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0) bm25_count_kernel(CountParams P) {
   static_assert(!(kAnd && kGroups), "groups generalise the conjunction");
   static_assert(!(kFacet && kSort), "the facet pass has its own sink");
   static_assert(!(kAgg && (kSort || kFacet)), "the aggregate pass has its own sink");
@@ -425,14 +428,16 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase && (kSort || kFacet) ? 
     }
     if constexpr (kPhraseStage) {
       if (live) {
-        const uint32_t wbase = ws >> 5, s0 = P.phrase.slot_off[q], ns = P.phrase.slot_off[q + 1] - s0;
+        const uint32_t wbase = ws >> 5;
+        const PhraseQuery PQ = phrase_query(P.phrase, q);
+        float unused;
         for (uint32_t i = tid; i < kCountWords; i += kCountThreads) {
           uint32_t v = acc[i];
           if (v && P.seg.deleted && wbase + i < del_words) v &= ~__ldg(P.seg.deleted + wbase + i);
           v = chain_bits(v, i);
           for (uint32_t r = v; r; r &= r - 1u) {
             const uint32_t bit = __ffs(r) - 1u;
-            if (!phrase_freq(P.seg, P.phrase, s0, ns, ws + 32u * i + bit)) v &= ~(1u << bit);
+            if (!phrase_clauses(P.seg, P.phrase, PQ, ws + 32u * i + bit, PhraseMode::check, unused)) v &= ~(1u << bit);
           }
           acc[i] = v;
         }
@@ -491,7 +496,8 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase && (kSort || kFacet) ? 
     if constexpr (kSort) {
       if (live) {
         const uint32_t wbase = ws >> 5, cap = P.sort.cap;
-        const uint32_t s0 = kPhrase ? P.phrase.slot_off[q] : 0u, ns = kPhrase ? P.phrase.slot_off[q + 1] - s0 : 0u;
+        PhraseQuery PQ{};
+        if constexpr (kPhrase) PQ = phrase_query(P.phrase, q);
         unsigned long long* hi = sort_buf;
         unsigned long long* lo = sort_buf + cap;
         for (uint32_t base = 0; base < kCountWords; base += kCountThreads) {   // uniform trip count
@@ -506,7 +512,8 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase && (kSort || kFacet) ? 
               const ulonglong2 key = sort_key(P.sort, doc);
               if (key.x < thr) continue;
               if constexpr (kPhrase) {
-                if (!phrase_freq(P.seg, P.phrase, s0, ns, doc)) continue;
+                float unused;
+                if (!phrase_clauses(P.seg, P.phrase, PQ, doc, PhraseMode::check, unused)) continue;
               }
               const uint32_t slot = atomicAdd(&s_fill[0], 1u);
               if (slot >= cap) break;
@@ -523,7 +530,9 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase && (kSort || kFacet) ? 
     if constexpr (kPhraseSink) {
       if (live) {
         const PhraseSink& F = P.phrase;
-        const uint32_t wbase = ws >> 5, cap = F.cap, s0 = F.slot_off[q], ns = F.slot_off[q + 1] - s0;
+        const uint32_t wbase = ws >> 5, cap = F.cap;
+        const PhraseQuery PQ = phrase_query(F, q);
+        const PhraseMode mode = cap ? PhraseMode::score : PhraseMode::check;
         unsigned long long* hi = sort_buf;
         unsigned long long* lo = sort_buf + cap;
         for (uint32_t base = 0; base < kCountWords; base += kCountThreads) {   // uniform trip count
@@ -535,10 +544,10 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase && (kSort || kFacet) ? 
             const unsigned long long thr = s_thr[0];
             for (; v; v &= v - 1u) {
               const uint32_t doc = ws + 32u * i + (__ffs(v) - 1u);
-              const uint32_t f = phrase_freq(P.seg, F, s0, ns, doc);
-              if (!f) continue;
+              float s;
+              if (!phrase_clauses(P.seg, F, PQ, doc, mode, s)) continue;
               if (cap) {
-                const unsigned long long key = phrase_key(P.seg, F, q, doc, f);
+                const unsigned long long key = phrase_key(F, doc, s);
                 if (key > thr) {
                   const uint32_t slot = atomicAdd(&s_fill[0], 1u);
                   if (slot >= cap) break;   // this bit is checked again after the cut

@@ -1,8 +1,9 @@
-// bm25_phrase.cuh -- exact phrase queries (sdbg_phrase_*_batch): the positions layout in HBM, the kernels that build it
-// at staging, and the per-doc phrase check that bm25_count_kernel runs (kPhrase) on the docs that survive the
-// conjunction of the phrase's terms, the deleted docs, the filter chain and the exclusions: in its own sink (count,
-// top-k), as a stage that narrows the window before the facet, aggregate and match-scan sinks, or inside the sorted
-// scan's sink once a doc's key has passed the threshold.
+// bm25_phrase.cuh -- exact phrase queries and conjunctions of phrase clauses (sdbg_phrase_*_batch,
+// sdbg_phrase_and_*_batch): the positions layout in HBM, the kernels that build it at staging, and the per-doc clause
+// check that bm25_count_kernel runs (kPhrase) on the docs that survive the conjunction of the positive clauses' terms,
+// the deleted docs, the filter chain and the exclusions: in its own sink (count, top-k), as a stage that narrows the
+// window before the facet, aggregate and match-scan sinks, or inside the sorted scan's sink once a doc's key has passed
+// the threshold. A single phrase is a query of one positive clause.
 //
 // Positions layout (DESIGN.md §3): per posting block g a 64-bit base pos_base[g] into the u32 arena `pos` (one sentinel
 // behind the last block), and at pos[pos_base[g] ..] first the block's len exclusive prefix sums of its frequencies, then
@@ -19,15 +20,17 @@ namespace sdbg {
 
 constexpr uint32_t kMaxPhraseSlots = 16;
 
-// bm25_count_kernel's phrase sink (kPhrase). cap == 0: count only; else the top-k of the phrase matches by score. With
-// another sink (kSort, kFacet, kAgg, kEmit) only the positions and slots are read.
+// bm25_count_kernel's phrase sink (kPhrase). cap == 0: count only; else the top-k of the matches by score. With another
+// sink (kSort, kFacet, kAgg, kEmit) only the positions, slots and clauses are read.
 struct PhraseSink {
   const unsigned long long* pos_base = nullptr;   // per block + sentinel
   const uint32_t* pos = nullptr;
-  // query q's slots slots[slot_off[q] .. slot_off[q + 1]) of this segment: {first BlockDesc, blocks, rel_pos, 0}
-  const uint4* slots = nullptr;
-  const uint32_t* slot_off = nullptr;
-  const float4* consts = nullptr;                 // per query {c0, norm_const, norm_length, 0} of the phrase statistics
+  const uint4* slots = nullptr;                   // this segment's slots: {first BlockDesc, blocks, rel_pos, 0}
+  // query q's clauses clauses[clause_off[q] .. clause_off[q + 1]) in this segment's cost order (ascending smallest
+  // docs_count of the clause's terms, ties in query order): {first slot, slots, negated, statistics index}
+  const uint4* clauses = nullptr;
+  const uint32_t* clause_off = nullptr;
+  const float4* consts = nullptr;                 // per statistics index {c0, norm_const, norm_length, 0} of a positive clause
   uint32_t ordinal_base = 0;                      // docs of the earlier segments: key = score bits << 32 | ~(base + doc)
   uint32_t k = 0, cap = 0;                        // cap: buffer slots, a power of two >= 2k (0: count only)
   unsigned long long* thr = nullptr;              // per query: the best known k-th key, seeded with the threshold
@@ -66,6 +69,7 @@ __device__ __forceinline__ uint32_t phrase_freq(const PostingsDev& S, const Phra
     rel[i] = sl.z;
     cur[i] = 0u;
   }
+  if (ns == 1u) return cnt[0];   // a term: its frequency, without walking its positions
   uint32_t freq = 0;
   for (uint32_t j = 0; j < cnt[0]; ++j) {
     const unsigned long long p = __ldg(F.pos + at[0] + j);
@@ -81,15 +85,50 @@ __device__ __forceinline__ uint32_t phrase_freq(const PostingsDev& S, const Phra
   return freq;
 }
 
-// The score of a phrase match of frequency f: bm25(f, norm(d)) with query q's phrase statistics.
-__device__ __forceinline__ float phrase_score(const PostingsDev& S, const PhraseSink& F, uint32_t q, uint32_t d, uint32_t f) {
-  const float4 c = __ldg(F.consts + q);
-  return bm25(f, load_norm(S.norms, S.norm_width, d), c.x, c.y, c.z);
+// Query q's clause range and its first clause, read once per window outside the per-doc loops: a single phrase (one
+// clause) then reads no clause table per doc.
+struct PhraseQuery {
+  uint32_t c0, c1;
+  uint4 first;
+};
+
+__device__ __forceinline__ PhraseQuery phrase_query(const PhraseSink& F, uint32_t q) {
+  PhraseQuery Q;
+  Q.c0 = __ldg(F.clause_off + q);
+  Q.c1 = __ldg(F.clause_off + q + 1);
+  Q.first = __ldg(F.clauses + Q.c0);
+  return Q;
 }
 
-// The top-k key of a phrase match: score bits, then ~ordinal (ties: segment asc, doc asc), as bm25_topk's keys.
-__device__ __forceinline__ unsigned long long phrase_key(const PostingsDev& S, const PhraseSink& F, uint32_t q, uint32_t d, uint32_t f) {
-  const float s = phrase_score(S, F, q, d, f);
+// How phrase_clauses treats doc d: check only (one-slot positive clauses skipped, since the conjunction of the positive
+// terms holds d already), check and score, or score a doc known to match (negated clauses skipped).
+enum class PhraseMode { check, score, score_match };
+
+// The clause check of doc d for query Q, clause after clause in table order, dropping d at the first that fails: a
+// positive clause needs phrase frequency > 0, a negated one 0. Scoring modes: s = the sum of bm25(frequency, norm(d)) of
+// the positive clauses with their statistics, in table order from 0 (a one-slot clause's frequency is its term's
+// position count).
+__device__ __forceinline__ bool phrase_clauses(const PostingsDev& S, const PhraseSink& F, const PhraseQuery& Q, uint32_t d,
+                                               PhraseMode mode, float& s) {
+  s = 0.f;
+  uint4 cl = Q.first;
+  for (uint32_t c = Q.c0;;) {
+    const bool skip = cl.z ? mode == PhraseMode::score_match : mode == PhraseMode::check && cl.y == 1u;
+    if (!skip) {
+      const uint32_t f = phrase_freq(S, F, cl.x, cl.y, d);
+      if ((f != 0u) == (cl.z != 0u)) return false;
+      if (mode != PhraseMode::check && !cl.z) {
+        const float4 k = __ldg(F.consts + cl.w);
+        s = __fadd_rn(s, bm25(f, load_norm(S.norms, S.norm_width, d), k.x, k.y, k.z));
+      }
+    }
+    if (++c >= Q.c1) return true;
+    cl = __ldg(F.clauses + c);
+  }
+}
+
+// The top-k key of a match of score s: score bits, then ~ordinal (ties: segment asc, doc asc), as bm25_topk's keys.
+__device__ __forceinline__ unsigned long long phrase_key(const PhraseSink& F, uint32_t d, float s) {
   return (static_cast<unsigned long long>(__float_as_uint(s)) << 32) | (~(F.ordinal_base + d) & 0xFFFFFFFFull);
 }
 

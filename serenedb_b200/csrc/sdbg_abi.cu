@@ -2347,16 +2347,41 @@ struct EmitJob {
   const unsigned long long* offset;   // host [nq]: the first ordinal of each query's page
 };
 
-// The phrase pass's part of a count_run call (the plan's batch is the AND of each phrase's distinct terms): query q's
-// slots are slot_term / slot_rel [slot_off[q] .. slot_off[q + 1]). k == 0: count only; else the top-k, scored with
-// consts[q] = {c0, norm_const, norm_length} and seeded with the key of threshold_in.
+// The phrase pass's part of a count_run call (the plan's batch is the AND of the distinct terms of each query's positive
+// clauses): query q's clauses are [query_off[q] .. query_off[q + 1]), clause j's slots slot_term / slot_rel
+// [clause_off[j] .. clause_off[j + 1]), negated when clause_neg[j] (clause_neg null: none). k == 0: count only; else the
+// top-k, scored with consts[j] = {c0, norm_const, norm_length} per clause and seeded with the key of threshold_in.
 struct PhraseJob {
   const uint32_t* slot_term = nullptr;
   const uint32_t* slot_rel = nullptr;
-  const uint32_t* slot_off = nullptr;
+  const uint32_t* clause_off = nullptr;
+  const uint8_t* clause_neg = nullptr;
+  const uint32_t* query_off = nullptr;
+  size_t nq = 0;
   std::vector<float4> consts;
   uint32_t k = 0;
   unsigned long long seed = 0;
+
+  uint32_t n_clauses() const { return query_off[nq]; }
+  uint32_t n_slots() const { return clause_off[n_clauses()]; }
+
+  // The job's device tables, staged as [query clause offsets | per segment the clause tables | per segment the slots'
+  // lists | per clause consts], from a 16-B aligned offset.
+  size_t clauses_pos() const { return ((nq + 1) * 4 + 15) & ~size_t(15); }
+  size_t lists_pos(size_t n_segs) const { return clauses_pos() + n_segs * n_clauses() * sizeof(uint4); }
+  size_t consts_pos(size_t n_segs) const { return lists_pos(n_segs) + n_segs * n_slots() * sizeof(uint4); }
+  size_t bytes(size_t n_segs) const { return consts_pos(n_segs) + (consts.empty() ? 0 : n_clauses() * sizeof(float4)); }
+  void write(sdbg_segment* const* segs, size_t n_segs, char* h) const;
+
+  // Segment si's view of the tables staged at d for the kernels' PhraseSink.
+  void sink(sdbg_segment* const* segs, size_t n_segs, size_t si, const char* d, PhraseSink& F) const {
+    F.pos_base = static_cast<const unsigned long long*>(segs[si]->d_pos_base);
+    F.pos = static_cast<const uint32_t*>(segs[si]->d_pos);
+    F.clause_off = reinterpret_cast<const uint32_t*>(d);
+    F.clauses = reinterpret_cast<const uint4*>(d + clauses_pos()) + si * n_clauses();
+    F.slots = reinterpret_cast<const uint4*>(d + lists_pos(n_segs)) + si * n_slots();
+    F.consts = consts.empty() ? nullptr : reinterpret_cast<const float4*>(d + consts_pos(n_segs));
+  }
 };
 
 // One pass of count_run: its mode and that mode's parameters. job_prepare checks them and fills the sinks, once per call.
@@ -2635,51 +2660,59 @@ void item_slots(const CountPlan& pl, char* h, size_t slot_off_pos, size_t slots_
   for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
 }
 
-// The phrase's slot lists of every segment for the kernel's PhraseSink::slots, h_lists[segment][slot]: {first BlockDesc,
-// blocks, rel_pos, 0}. Slots before job.slot_off[0] belong to no query and are left as they are.
-void phrase_slot_lists(sdbg_segment* const* segs, size_t n_segs, const PhraseJob& job, size_t nq, uint4* h_lists) {
-  const uint32_t n_slots = job.slot_off[nq];
-  for (size_t si = 0; si < n_segs; ++si)
-    for (uint32_t i = job.slot_off[0]; i < n_slots; ++i) {
-      const uint2 l = excl_list(segs[si], job.slot_term[i]);
-      h_lists[si * n_slots + i] = make_uint4(l.x, l.y, job.slot_rel[i], 0u);
+// The tables of PhraseJob::bytes at h. Per segment: each slot's list {first BlockDesc, blocks, rel_pos, 0}, and each
+// query's clauses {first slot, slots, negated, clause index} in that segment's cost order, the smallest docs_count of the
+// clause's terms (a term the segment does not hold costs 0), ascending, ties in query order: the order of a conjunction of
+// the terms' lists (conjunction.hpp:185-195), in which the scores of the positive clauses are summed. Slots and clauses
+// before the first query's are left as they are.
+void PhraseJob::write(sdbg_segment* const* segs, size_t n_segs, char* h) const {
+  const uint32_t nc = n_clauses(), ns = n_slots(), c0 = query_off[0];
+  std::memcpy(h, query_off, (nq + 1) * 4);
+  auto* lists = reinterpret_cast<uint4*>(h + lists_pos(n_segs));
+  auto* tables = reinterpret_cast<uint4*>(h + clauses_pos());
+  std::vector<uint32_t> cost(nc);
+  for (size_t si = 0; si < n_segs; ++si) {
+    const sdbg_segment* sg = segs[si];
+    for (uint32_t i = clause_off[c0]; i < ns; ++i) {
+      const uint2 l = excl_list(sg, slot_term[i]);
+      lists[si * ns + i] = make_uint4(l.x, l.y, slot_rel[i], 0u);
     }
-}
-
-// The positions and slots of segment si for the kernels' PhraseSink; d_slot_off / d_lists: device copies of
-// job.slot_off and of phrase_slot_lists' array.
-void phrase_sink(sdbg_segment* const* segs, size_t si, uint32_t n_slots, const uint32_t* d_slot_off, const uint4* d_lists,
-                 PhraseSink& F) {
-  F.pos_base = static_cast<const unsigned long long*>(segs[si]->d_pos_base);
-  F.pos = static_cast<const uint32_t*>(segs[si]->d_pos);
-  F.slots = d_lists + si * n_slots;
-  F.slot_off = d_slot_off;
+    for (uint32_t j = c0; j < nc; ++j) {
+      uint32_t m = 0xFFFFFFFFu;
+      for (uint32_t i = clause_off[j]; i < clause_off[j + 1]; ++i)
+        m = std::min(m, slot_term[i] < sg->term_docs.size() ? sg->term_docs[slot_term[i]] : 0u);
+      cost[j] = m;
+    }
+    uint4* T = tables + si * nc;
+    for (size_t q = 0; q < nq; ++q) {
+      for (uint32_t j = query_off[q]; j < query_off[q + 1]; ++j)
+        T[j] = make_uint4(clause_off[j], clause_off[j + 1] - clause_off[j], clause_neg && clause_neg[j] ? 1u : 0u, j);
+      std::stable_sort(T + query_off[q], T + query_off[q + 1], [&](const uint4& x, const uint4& y) { return cost[x.w] < cost[y.w]; });
+    }
+  }
+  if (!consts.empty()) std::memcpy(h + consts_pos(n_segs), consts.data(), nc * sizeof(float4));
 }
 
 // The phrase pass of count_run (CountMode::phrase) over a plan with work items: bm25_count_kernel<kAnd, .., kPhrase> per
 // segment, the count into out.counts; with a top-k (job.k) each item writes its k best keys to its own slot, then
 // phrase_merge_kernel keeps each query's k best in out.bins (u64 keys [nq][k]) with their number in out.nulls (u32 [nq]).
-// Host staging: the plan's, then [slot_off | slots | query slot offsets | per segment the slots' lists | consts].
+// Host staging: the plan's, then [slot_off | slots | the job's tables (PhraseJob::bytes)].
 int phrase_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt, const PhraseJob& job,
                const CountOut& out) {
   sdbg_ctx* c = segs[0]->ctx;
   const size_t nq = pl.Q.nq, total = pl.items;
-  const uint32_t k = job.k, n_slots = job.slot_off[nq];
+  const uint32_t k = job.k;
   uint32_t cap = 0;
   if (k) { uint32_t kp = 1; while (kp < k) kp <<= 1; cap = std::max(256u, 2u * kp); }
   const size_t slot_off_pos = pl.staged;
   const size_t slots_pos = slot_off_pos + pl.off_bytes;
-  const size_t poff_pos = slots_pos + total * 4;
-  const size_t lists_pos = (poff_pos + pl.off_bytes + 15) & ~size_t(15);
-  const size_t consts_pos = lists_pos + n_segs * n_slots * sizeof(uint4);
-  const size_t bytes = consts_pos + nq * sizeof(float4);
+  const size_t tables_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
+  const size_t bytes = tables_pos + job.bytes(n_segs);
   std::vector<char> staging(bytes);
   char* h = staging.data();
   pl.write(h);
   item_slots(pl, h, slot_off_pos, slots_pos);
-  std::memcpy(h + poff_pos, job.slot_off, pl.off_bytes);
-  phrase_slot_lists(segs, n_segs, job, nq, reinterpret_cast<uint4*>(h + lists_pos));
-  if (k) std::memcpy(h + consts_pos, job.consts.data(), nq * sizeof(float4));
+  job.write(segs, n_segs, h + tables_pos);
   // device scratch: [item keys [items][k] | item key counts | thresholds [nq]]
   const size_t keys_n_pos = total * size_t(k) * 8;
   const size_t thr_pos = (keys_n_pos + total * 4 + 15) & ~size_t(15);
@@ -2706,8 +2739,7 @@ int phrase_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, co
     pl.params(d, segs[si], si, first, chains[si], &P);
     P.counts = static_cast<unsigned long long*>(out.counts);
     PhraseSink& F = P.phrase;
-    phrase_sink(segs, si, n_slots, reinterpret_cast<const uint32_t*>(d + poff_pos), reinterpret_cast<const uint4*>(d + lists_pos), F);
-    F.consts = reinterpret_cast<const float4*>(d + consts_pos);
+    job.sink(segs, n_segs, si, d + tables_pos, F);
     F.ordinal_base = uint32_t(base);
     F.k = k; F.cap = cap; F.thr = thr;
     F.out = reinterpret_cast<unsigned long long*>(o);
@@ -2734,8 +2766,8 @@ int phrase_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, co
 // sorted scan launches per segment its seed items first (all segments), then the rest, each item writing its k best to
 // its own slot (its index in the work array); then sort_merge_kernel per query, and for a rank sort_dist_rows_kernel.
 // The match scan launches its items twice (bm25_emit.cuh): pass A, emit_bases_kernel over each query's items in
-// (segment, first window) order, pass B. A job with phrase slots (job.phrase.slot_off; the plan's batch is the AND of the
-// phrases' terms) runs the phrase instantiations of its mode and stages the slot lists.
+// (segment, first window) order, pass B. A job with phrase clauses (job.phrase.query_off; the plan's batch is the AND of
+// the positive clauses' terms) runs the phrase instantiations of its mode and stages the phrase tables.
 // The plan is staged from pageable memory, which the copy has consumed when it returns, so calls can follow one another
 // without a wait (a host group entry queues its shapes back to back).
 int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, const sdbg_col_pred* filt, const CountJob& job,
@@ -2749,26 +2781,21 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
   if (phrase) return phrase_run(segs, n_segs, pl, filt, job.phrase, out);
   const SortJob& J = job.sort;
   const uint32_t k = J.k, cap = sort ? J.sink[0].cap : 0u;
-  const bool phrased = job.phrase.slot_off != nullptr;
-  const uint32_t n_slots = phrased ? job.phrase.slot_off[nq] : 0u;
+  const bool phrased = job.phrase.query_off != nullptr;
   // host staging: the plan's, then for the sorted scan [slot_off | slots | segments], for the match scan [slot_off |
-  // slots | offsets]; then for a phrase [query slot offsets | per segment the slots' lists]
+  // slots | offsets]; then for a phrase its tables (PhraseJob::bytes)
   const size_t slot_off_pos = pl.staged;
   const size_t slots_pos = slot_off_pos + pl.off_bytes;
   const size_t segs_pos = (slots_pos + total * 4 + 15) & ~size_t(15);
   const size_t mode_end = sort ? segs_pos + n_segs * sizeof(SortSegDev) : emit ? segs_pos + nq * 8 : pl.staged;
-  const size_t poff_pos = (mode_end + 15) & ~size_t(15);
-  const size_t plists_pos = (poff_pos + pl.off_bytes + 15) & ~size_t(15);
-  const size_t bytes = phrased ? plists_pos + n_segs * n_slots * sizeof(uint4) : mode_end;
+  const size_t tables_pos = (mode_end + 15) & ~size_t(15);
+  const size_t bytes = phrased ? tables_pos + job.phrase.bytes(n_segs) : mode_end;
   std::vector<char> staging(bytes);
   char* h = staging.data();
   pl.write(h);
   if (sort || emit) item_slots(pl, h, slot_off_pos, slots_pos);
   if (emit) std::memcpy(h + segs_pos, job.emit.offset, nq * 8);
-  if (phrased) {
-    std::memcpy(h + poff_pos, job.phrase.slot_off, pl.off_bytes);
-    phrase_slot_lists(segs, n_segs, job.phrase, nq, reinterpret_cast<uint4*>(h + plists_pos));
-  }
+  if (phrased) job.phrase.write(segs, n_segs, h + tables_pos);
   if (sort) {
     auto* h_segs = reinterpret_cast<SortSegDev*>(h + segs_pos);
     for (size_t si = 0; si < n_segs; ++si) {
@@ -2823,9 +2850,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
         CountParams P;
         pl.params(d, segs[si], si, first, chains[si], &P);
         P.counts = static_cast<unsigned long long*>(out.counts);
-        if (phrased)
-          phrase_sink(segs, si, n_slots, reinterpret_cast<const uint32_t*>(d + poff_pos), reinterpret_cast<const uint4*>(d + plists_pos),
-                      P.phrase);
+        if (phrased) job.phrase.sink(segs, n_segs, si, d + tables_pos, P.phrase);
         if (sort) {
           P.counts = nullptr;
           P.sort = J.sink[si];
@@ -3026,67 +3051,88 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
 }
 
 namespace {
-// A batch of phrases (sdbg_phrase_*_batch), checked before anything is queued: query q's slots are terms / rel_pos
-// [phrase_off[q] .. phrase_off[q + 1]); `ids` / `id_off` hold each phrase's distinct term ids, in slot order, which run as
-// the AND the phrase check starts from.
+// A batch of clause conjunctions (sdbg_phrase_and_*_batch; a phrase of sdbg_phrase_*_batch is a query of one positive
+// clause, query_clause_off null), checked before anything is queued: query q's clauses are [qoff[q] .. qoff[q + 1]),
+// clause j's slots terms / rel_pos [clause_off[j] .. clause_off[j + 1]), negated when clause_neg[j]. `ids` / `id_off` hold
+// the distinct term ids of each query's positive clauses, in slot order, which run as the AND the clause check starts from.
 struct PhraseBatch {
   int rc = SDBG_OK;
-  std::vector<uint32_t> ids, id_off, rel;
+  std::vector<uint32_t> ids, id_off, rel, qoff;
+  const uint32_t* terms = nullptr;
+  const uint32_t* clause_off = nullptr;
+  const uint8_t* clause_neg = nullptr;
 
-  PhraseBatch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* phrase_off,
-              size_t nq) {
-    if (!segs || !n_segs || !segs[0] || !nq || !phrase_off) { rc = SDBG_EINVAL; return; }
+  PhraseBatch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms_, const uint32_t* rel_pos, const uint32_t* clause_off_,
+              const uint8_t* clause_neg_, const uint32_t* query_clause_off, size_t nq)
+      : terms(terms_), clause_off(clause_off_), clause_neg(clause_neg_) {
+    if (!segs || !n_segs || !segs[0] || !nq || !clause_off) { rc = SDBG_EINVAL; return; }
     sdbg_ctx* c = segs[0]->ctx;
+    qoff.resize(nq + 1);
+    for (size_t q = 0; q <= nq; ++q) qoff[q] = query_clause_off ? query_clause_off[q] : uint32_t(q);
     for (size_t q = 0; q < nq && !rc; ++q) {
-      if (phrase_off[q + 1] < phrase_off[q]) rc = fail(c, SDBG_EINVAL, "phrase_off must be non-decreasing");
-      else if (phrase_off[q + 1] == phrase_off[q]) rc = fail(c, SDBG_EINVAL, "empty phrase");
+      if (qoff[q + 1] < qoff[q]) rc = fail(c, SDBG_EINVAL, "query_clause_off must be non-decreasing");
+      else if (qoff[q + 1] == qoff[q]) rc = fail(c, SDBG_EINVAL, "a query without a clause");
+    }
+    for (uint32_t j = qoff[0]; j < qoff[nq] && !rc; ++j) {
+      if (clause_off[j + 1] < clause_off[j]) rc = fail(c, SDBG_EINVAL, "clause_off must be non-decreasing");
+      else if (clause_off[j + 1] == clause_off[j]) rc = fail(c, SDBG_EINVAL, "empty clause");
+    }
+    for (size_t q = 0; q < nq && !rc; ++q) {
+      bool pos = false;
+      for (uint32_t j = qoff[q]; j < qoff[q + 1]; ++j) pos |= !negated(j);
+      if (!pos) rc = fail(c, SDBG_EINVAL, "a query without a positive clause");
     }
     for (size_t q = 0; q < nq && !rc; ++q)
-      if (phrase_off[q + 1] - phrase_off[q] > kMaxPhraseSlots) rc = fail(c, SDBG_EUNSUPPORTED, "a phrase holds 1..16 slots");
+      if (clause_off[qoff[q + 1]] - clause_off[qoff[q]] > kMaxPhraseSlots) rc = fail(c, SDBG_EUNSUPPORTED, "a query holds 1..16 slots");
     if (!rc && !terms) rc = fail(c, SDBG_EINVAL, "terms is NULL");
     if (rc) return;
     id_off.assign(1, 0u);
-    rel.resize(phrase_off[nq]);
+    rel.resize(clause_off[qoff[nq]]);
     for (size_t q = 0; q < nq; ++q) {
-      const uint32_t s0 = phrase_off[q], s1 = phrase_off[q + 1];
-      for (uint32_t i = s0; i < s1; ++i) {
-        rel[i] = rel_pos ? rel_pos[i] : i - s0;
-        if (i == s0 ? rel[i] != 0u : rel[i] <= rel[i - 1]) {
-          rc = fail(c, SDBG_EINVAL, "rel_pos must start at 0 and increase");
-          return;
+      for (uint32_t j = qoff[q]; j < qoff[q + 1]; ++j) {
+        const uint32_t s0 = clause_off[j], s1 = clause_off[j + 1];
+        for (uint32_t i = s0; i < s1; ++i) {
+          rel[i] = rel_pos ? rel_pos[i] : i - s0;
+          if (i == s0 ? rel[i] != 0u : rel[i] <= rel[i - 1]) {
+            rc = fail(c, SDBG_EINVAL, "rel_pos must start at 0 and increase");
+            return;
+          }
+          if (!negated(j) && std::find(ids.begin() + id_off.back(), ids.end(), terms[i]) == ids.end()) ids.push_back(terms[i]);
         }
-        if (std::find(ids.begin() + id_off.back(), ids.end(), terms[i]) == ids.end()) ids.push_back(terms[i]);
       }
       id_off.push_back(uint32_t(ids.size()));
     }
   }
 
+  bool negated(uint32_t j) const { return clause_neg && clause_neg[j]; }
+
   QueryBatch<uint32_t> conj(size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off) const {
     return {SDBG_QUERY_AND, ids.data(), id_off.data(), nq, excl_terms, excl_off, nullptr};
   }
 
-  // The phrase slots of a count_run job over conj(): count only until k or consts are set.
-  PhraseJob job(const uint32_t* terms, const uint32_t* phrase_off) const {
+  // The clauses of a count_run job over conj(): count only until k or consts are set.
+  PhraseJob job() const {
     PhraseJob J;
-    J.slot_term = terms; J.slot_rel = rel.data(); J.slot_off = phrase_off;
+    J.slot_term = terms; J.slot_rel = rel.data(); J.clause_off = clause_off; J.clause_neg = clause_neg;
+    J.query_off = qoff.data(); J.nq = qoff.size() - 1;
     return J;
   }
-};
 
-// consts[q] = {c0, norm_const, norm_length, 0} of phrase q's statistics phrase_stats[q]: the scorer form of fill_qterm,
-// as the phrase top-k and the scored phrase scan score a match.
-std::vector<float4> phrase_consts(sdbg_segment* const* segs, const uint32_t* terms, const uint32_t* phrase_off, size_t nq,
-                                  const sdbg_bm25_term* phrase_stats, float k1, float b) {
-  std::vector<float4> consts(nq);
-  for (size_t q = 0; q < nq; ++q) {
-    sdbg_bm25_term t = phrase_stats[q];
-    t.term = terms[phrase_off[q]];
-    QTermDev d;
-    fill_qterm(segs[0], t, k1, b, d);
-    consts[q] = make_float4(d.c0, d.norm_const, d.norm_length, 0.f);
+  // consts[j] = {c0, norm_const, norm_length, 0} of positive clause j's statistics clause_stats[j] (negated clauses: 0):
+  // the scorer form of fill_qterm, as the phrase top-k and the scored phrase scan score a match.
+  std::vector<float4> consts(sdbg_segment* const* segs, const sdbg_bm25_term* clause_stats, float k1, float b) const {
+    std::vector<float4> out(qoff.back(), make_float4(0.f, 0.f, 0.f, 0.f));
+    for (uint32_t j = qoff[0]; j < qoff.back(); ++j) {
+      if (negated(j)) continue;
+      sdbg_bm25_term t = clause_stats[j];
+      t.term = terms[clause_off[j]];
+      QTermDev d;
+      fill_qterm(segs[0], t, k1, b, d);
+      out[j] = make_float4(d.c0, d.norm_const, d.norm_length, 0.f);
+    }
+    return out;
   }
-  return consts;
-}
+};
 
 // Every segment holds positions (sdbg_stage_positions).
 int phrase_positions_staged(sdbg_segment* const* segs, size_t n_segs) {
@@ -3094,32 +3140,34 @@ int phrase_positions_staged(sdbg_segment* const* segs, size_t n_segs) {
     if (!segs[si]->d_pos) return fail(segs[0]->ctx, SDBG_ENOTFOUND, "segment has no staged positions");
   return SDBG_OK;
 }
-}  // namespace
 
-extern "C" int sdbg_phrase_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                                       const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
-                                       const sdbg_col_pred* filt, uint64_t* counts) {
+// The count, top-k, sorted scan, facet counts and aggregates of a batch of clause conjunctions (query_clause_off null:
+// one clause per query, the sdbg_phrase_* entries): PhraseBatch's checks, the AND of the positive clauses' terms, staged
+// positions, then the flat entry's pass with the clauses on its job.
+int phrase_count(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* clause_off,
+                 const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
+                 const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
   if (!counts) return SDBG_EINVAL;
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
   if (PB.rc) return PB.rc;
   const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
   if (B.rc) return B.rc;
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
   CountJob job{CountMode::count, {}, {}, {}};
   job.mode = CountMode::phrase;
-  job.phrase = PB.job(terms, phrase_off);
+  job.phrase = PB.job();
   return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
 }
 
-extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                                      const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
-                                      const sdbg_bm25_term* phrase_stats, float k1, float b, const sdbg_col_pred* filt, uint32_t k,
-                                      float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
-  if (!out || !n_out || !phrase_stats) return SDBG_EINVAL;
+int phrase_topk(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* clause_off,
+                const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
+                const uint32_t* excl_off, const sdbg_bm25_term* clause_stats, float k1, float b, const sdbg_col_pred* filt, uint32_t k,
+                float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
+  if (!out || !n_out || !clause_stats) return SDBG_EINVAL;
   if (int rc = topk_args(segs, n_segs, nq, k)) return rc;
   sdbg_ctx* c = segs[0]->ctx;
   if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
   if (PB.rc) return PB.rc;
   const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
   if (B.rc) return B.rc;
@@ -3130,9 +3178,9 @@ extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, 
   CountJob job{CountMode::count, {}, {}, {}};
   job.mode = CountMode::phrase;
   PhraseJob& J = job.phrase;
-  J = PB.job(terms, phrase_off);
+  J = PB.job();
   J.k = k;
-  J.consts = phrase_consts(segs, terms, phrase_off, nq, phrase_stats, k1, b);
+  J.consts = PB.consts(segs, clause_stats, k1, b);
   uint32_t thr_bits; std::memcpy(&thr_bits, &threshold_in, 4);
   if (!(threshold_in >= 0.f)) thr_bits = 0;  // negative / NaN seeds accept every positive score, as the top-k entries
   J.seed = (static_cast<unsigned long long>(thr_bits) << 32) | 0xFFFFFFFFull;
@@ -3146,36 +3194,116 @@ extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, 
   return topk_hits_to_host(segs, n_segs, dev, nq, k, out, n_out, total_matches);
 }
 
-// The sorted scan, facet counts and aggregates of phrases: the phrase entries' checks (PhraseBatch, the AND of the
-// phrases' terms, staged positions), then the flat entry's pass with the phrase slots on its job.
-extern "C" int sdbg_phrase_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                                                const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms,
-                                                const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
-                                                int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
+int phrase_topk_by_column(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                          const uint32_t* clause_off, const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq,
+                          const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
+                          int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
   if (!segs || !n_segs || !segs[0] || !k || !out || !n_out) return SDBG_EINVAL;
   if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
   if (PB.rc) return PB.rc;
   const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
   if (B.rc) return B.rc;
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
-  return sort_to_host(segs, n_segs, B, filt, sort_field, descending, nulls_first, k, out, n_out, PB.job(terms, phrase_off));
+  return sort_to_host(segs, n_segs, B, filt, sort_field, descending, nulls_first, k, out, n_out, PB.job());
+}
+
+int phrase_facet_counts(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                        const uint32_t* clause_off, const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq,
+                        const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                        int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
+  if (!counts || !null_counts) return SDBG_EINVAL;
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
+  if (PB.rc) return PB.rc;
+  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  if (B.rc) return B.rc;
+  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
+  CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
+  job.phrase = PB.job();
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, key_span),
+                      [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
+}
+
+int phrase_aggregate(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* clause_off,
+                     const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
+                     const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
+                     uint64_t value_field, sdbg_match_agg* out, sdbg_match_agg* null_out) {
+  if (!out || !null_out) return SDBG_EINVAL;
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
+  if (PB.rc) return PB.rc;
+  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  if (B.rc) return B.rc;
+  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
+  return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out, PB.job());
+}
+}  // namespace
+
+extern "C" int sdbg_phrase_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                       const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
+                                       const sdbg_col_pred* filt, uint64_t* counts) {
+  return phrase_count(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, counts);
+}
+
+extern "C" int sdbg_phrase_and_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                           const uint32_t* clause_off, const uint8_t* clause_negated, const uint32_t* query_clause_off,
+                                           size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                           uint64_t* counts) {
+  if (!query_clause_off) return SDBG_EINVAL;
+  return phrase_count(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt, counts);
+}
+
+extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                      const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
+                                      const sdbg_bm25_term* phrase_stats, float k1, float b, const sdbg_col_pred* filt, uint32_t k,
+                                      float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
+  return phrase_topk(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, phrase_stats, k1, b, filt, k,
+                     threshold_in, out, n_out, total_matches);
+}
+
+extern "C" int sdbg_phrase_and_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                          const uint32_t* clause_off, const uint8_t* clause_negated, const uint32_t* query_clause_off,
+                                          size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
+                                          const sdbg_bm25_term* clause_stats, float k1, float b, const sdbg_col_pred* filt, uint32_t k,
+                                          float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
+  if (!query_clause_off) return SDBG_EINVAL;
+  return phrase_topk(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, clause_stats,
+                     k1, b, filt, k, threshold_in, out, n_out, total_matches);
+}
+
+extern "C" int sdbg_phrase_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                                const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms,
+                                                const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
+                                                int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
+  return phrase_topk_by_column(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, sort_field,
+                               descending, nulls_first, k, out, n_out);
+}
+
+extern "C" int sdbg_phrase_and_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                    const uint32_t* rel_pos, const uint32_t* clause_off, const uint8_t* clause_negated,
+                                                    const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
+                                                    const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
+                                                    int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
+  if (!query_clause_off) return SDBG_EINVAL;
+  return phrase_topk_by_column(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt,
+                               sort_field, descending, nulls_first, k, out, n_out);
 }
 
 extern "C" int sdbg_phrase_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
                                               const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms,
                                               const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
                                               int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
-  if (!counts || !null_counts) return SDBG_EINVAL;
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
-  if (PB.rc) return PB.rc;
-  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
-  if (B.rc) return B.rc;
-  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
-  CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
-  job.phrase = PB.job(terms, phrase_off);
-  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, key_span),
-                      [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
+  return phrase_facet_counts(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, key_field,
+                             key_min, key_span, counts, null_counts);
+}
+
+extern "C" int sdbg_phrase_and_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                                  const uint32_t* clause_off, const uint8_t* clause_negated,
+                                                  const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
+                                                  const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                                  int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
+  if (!query_clause_off) return SDBG_EINVAL;
+  return phrase_facet_counts(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt,
+                             key_field, key_min, key_span, counts, null_counts);
 }
 
 extern "C" int sdbg_phrase_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3183,13 +3311,19 @@ extern "C" int sdbg_phrase_aggregate_batch(sdbg_segment* const* segs, size_t n_s
                                            const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
                                            int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
                                            sdbg_match_agg* null_out) {
-  if (!out || !null_out) return SDBG_EINVAL;
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
-  if (PB.rc) return PB.rc;
-  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
-  if (B.rc) return B.rc;
-  if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
-  return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out, PB.job(terms, phrase_off));
+  return phrase_aggregate(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, key_field, key_min,
+                          key_span, value_field, out, null_out);
+}
+
+extern "C" int sdbg_phrase_and_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                               const uint32_t* clause_off, const uint8_t* clause_negated,
+                                               const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
+                                               const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                               int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
+                                               sdbg_match_agg* null_out) {
+  if (!query_clause_off) return SDBG_EINVAL;
+  return phrase_aggregate(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt,
+                          key_field, key_min, key_span, value_field, out, null_out);
 }
 
 extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -3377,7 +3511,7 @@ int scan_batch_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch
 
 // Queues the match scan of a checked phrase batch (B: the AND of the phrases' terms) into out, zeroed: the emit pass with
 // the phrase slots, then, when scored (J.consts set), phrase_score_kernel over the pages.
-// The scorer's staging: [PostingsDev [n_segs] | PhraseSink [n_segs] | slot_off | per segment the slots' lists].
+// The scorer's staging: [PostingsDev [n_segs] | PhraseSink [n_segs] | the job's tables (PhraseJob::bytes)].
 int phrase_scan_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt,
                     const PhraseJob& J, const uint64_t* offset, uint32_t limit, const CountOut& out) {
   sdbg_ctx* c = segs[0]->ctx;
@@ -3388,12 +3522,9 @@ int phrase_scan_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<ui
   job.phrase = J;
   if (int rc = count_run(segs, n_segs, count_plan(segs, n_segs, B.whole, B.total_excl, filt, job), filt, job, out)) return rc;
   if (J.consts.empty()) return SDBG_OK;
-  const uint32_t n_slots = J.slot_off[nq];
   const size_t sinks_pos = (n_segs * sizeof(PostingsDev) + 15) & ~size_t(15);
-  const size_t off_pos = sinks_pos + n_segs * sizeof(PhraseSink);
-  const size_t lists_pos = (off_pos + (nq + 1) * 4 + 15) & ~size_t(15);
-  const size_t consts_pos = lists_pos + n_segs * n_slots * sizeof(uint4);
-  std::vector<char> h(consts_pos + nq * sizeof(float4));
+  const size_t tables_pos = (sinks_pos + n_segs * sizeof(PhraseSink) + 15) & ~size_t(15);
+  std::vector<char> h(tables_pos + J.bytes(n_segs));
   DevBuf& b_sc = c->scratch[4];
   if (int rc = ensure(c, b_sc, h.size())) return rc;
   const char* d = static_cast<const char*>(b_sc.p);
@@ -3401,13 +3532,10 @@ int phrase_scan_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<ui
     const PostingsDev p = postings_view(segs[si], 0);
     std::memcpy(h.data() + si * sizeof(PostingsDev), &p, sizeof(p));
     PhraseSink F;
-    phrase_sink(segs, si, n_slots, reinterpret_cast<const uint32_t*>(d + off_pos), reinterpret_cast<const uint4*>(d + lists_pos), F);
-    F.consts = reinterpret_cast<const float4*>(d + consts_pos);
+    J.sink(segs, n_segs, si, d + tables_pos, F);
     std::memcpy(h.data() + sinks_pos + si * sizeof(PhraseSink), &F, sizeof(F));
   }
-  std::memcpy(h.data() + off_pos, J.slot_off, (nq + 1) * 4);
-  phrase_slot_lists(segs, n_segs, J, nq, reinterpret_cast<uint4*>(h.data() + lists_pos));
-  std::memcpy(h.data() + consts_pos, J.consts.data(), nq * sizeof(float4));
+  J.write(segs, n_segs, h.data() + tables_pos);
   CU(c, cudaMemcpyAsync(b_sc.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
   PhraseScoreParams P;
   P.segs = reinterpret_cast<const PostingsDev*>(d);
@@ -3439,13 +3567,13 @@ extern "C" int sdbg_match_scan_batch_groups_min(sdbg_segment* const* segs, size_
   return scan_batch_to_host(segs, n_segs, B, filt, {offset, limit, scored, k1, b}, out, n_out, total);
 }
 
-extern "C" int sdbg_phrase_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                                      const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
-                                      const sdbg_col_pred* filt, const sdbg_bm25_term* phrase_stats, float k1, float b,
-                                      const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out,
-                                      uint64_t* total) {
-  if (!limit || !out || !n_out || !total || (scored && !phrase_stats)) return SDBG_EINVAL;
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, phrase_off, nq);
+namespace {
+int phrase_scan(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* clause_off,
+                const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
+                const uint32_t* excl_off, const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats, float k1, float b,
+                const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
+  if (!limit || !out || !n_out || !total || (scored && !clause_stats)) return SDBG_EINVAL;
+  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
   if (PB.rc) return PB.rc;
   sdbg_ctx* c = segs[0]->ctx;
   if (scored)
@@ -3458,10 +3586,30 @@ extern "C" int sdbg_phrase_scan_batch(sdbg_segment* const* segs, size_t n_segs, 
     if (ord > kMaxDocId) return fail(c, SDBG_EUNSUPPORTED, "more than 2^32-2 docs per call");
   }
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
-  PhraseJob J = PB.job(terms, phrase_off);
-  if (scored) J.consts = phrase_consts(segs, terms, phrase_off, nq, phrase_stats, k1, b);
+  PhraseJob J = PB.job();
+  if (scored) J.consts = PB.consts(segs, clause_stats, k1, b);
   return scan_to_host(c, nq, limit, [&](const CountOut& o) { return phrase_scan_run(segs, n_segs, B, filt, J, offset, limit, o); },
                       out, n_out, total);
+}
+}  // namespace
+
+extern "C" int sdbg_phrase_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                      const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
+                                      const sdbg_col_pred* filt, const sdbg_bm25_term* phrase_stats, float k1, float b,
+                                      const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out,
+                                      uint64_t* total) {
+  return phrase_scan(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, phrase_stats, k1, b,
+                     offset, limit, scored, out, n_out, total);
+}
+
+extern "C" int sdbg_phrase_and_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                          const uint32_t* clause_off, const uint8_t* clause_negated, const uint32_t* query_clause_off,
+                                          size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                          const sdbg_bm25_term* clause_stats, float k1, float b, const uint64_t* offset,
+                                          uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
+  if (!query_clause_off) return SDBG_EINVAL;
+  return phrase_scan(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt,
+                     clause_stats, k1, b, offset, limit, scored, out, n_out, total);
 }
 
 // ---- the count, facet, aggregate and sorted passes across GPUs ----

@@ -589,6 +589,8 @@ def _phrase_args(phrases, rel_pos, exclude):
     if rel_pos is not None:
         if len(rel_pos) != nq:
             raise ValueError("rel_pos needs one list (or None) per phrase")
+        if any(rp is not None and len(rp) != len(p) for p, rp in zip(phrases, rel_pos)):
+            raise ValueError("a phrase's rel_pos needs one position per term")
         rel = np.ascontiguousarray([r for p, rp in zip(phrases, rel_pos) for r in (range(len(p)) if rp is None else rp)],
                                    dtype=np.uint32)
     x = _exclusions(exclude, nq) or (None, None)
@@ -729,6 +731,195 @@ def ExecutePhraseMatchScan(reader, phrase, scorer=None, limit=1 << 20, offset=0,
     """ExecutePhraseMatchScanBatch for one phrase: ((seg, doc, score) arrays, total matches)."""
     return ExecutePhraseMatchScanBatch(reader, [list(phrase)], scorer, limit, [offset], _one(rel_pos), filt, _one(exclude),
                                        boost)[0]
+
+
+def _clause(c):
+    """A clause as (term ids, rel_pos or None): a list of term ids, or a pair (term ids, rel_pos)."""
+    if isinstance(c, tuple) and len(c) == 2 and not isinstance(c[0], (int, np.integer)):
+        terms, rel = [int(t) for t in c[0]], (None if c[1] is None else [int(r) for r in c[1]])
+        if rel is not None and len(rel) != len(terms):
+            raise ValueError("a clause's rel_pos needs one position per term")
+        return terms, rel
+    return [int(t) for t in c], None
+
+
+def _phrase_and_clauses(queries, exclude_phrases):
+    """Per query its clauses as [(terms, rel_pos or None, negated)]: the positive clauses of queries[q], then the
+    negated clauses exclude_phrases[q]."""
+    if exclude_phrases is not None and len(exclude_phrases) != len(queries):
+        raise ValueError("exclude_phrases needs one list (or None) per query")
+    out = []
+    for q, query in enumerate(queries):
+        neg = exclude_phrases[q] if exclude_phrases is not None and exclude_phrases[q] is not None else []
+        out.append([_clause(c) + (False,) for c in query] + [_clause(c) + (True,) for c in neg])
+    return out
+
+
+def _phrase_and_args(clauses, exclude):
+    """(terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off) of the clause-conjunction
+    entries, and the arrays they point into (kept alive by the caller)."""
+    nq = len(clauses)
+    flat = [c for q in clauses for c in q]
+    terms = np.ascontiguousarray([t for ts, _, _ in flat for t in ts], dtype=np.uint32)
+    rel = np.ascontiguousarray([r for ts, rp, _ in flat for r in (range(len(ts)) if rp is None else rp)], dtype=np.uint32)
+    coff = np.zeros(len(flat) + 1, np.uint32)
+    coff[1:] = np.cumsum([len(ts) for ts, _, _ in flat])
+    neg = np.ascontiguousarray([1 if n else 0 for _, _, n in flat], dtype=np.uint8)
+    qoff = np.zeros(nq + 1, np.uint32)
+    qoff[1:] = np.cumsum([len(q) for q in clauses])
+    x = _exclusions(exclude, nq) or (None, None)
+    keep = (terms, rel, coff, neg, qoff, x)
+    return (_ptr(terms) if len(terms) else None, _ptr(rel) if len(rel) else None, _ptr(coff), _ptr(neg) if len(neg) else None,
+            _ptr(qoff), nq, _ptr(x[0]), _ptr(x[1])), keep
+
+
+def _clause_stats(reader, clauses, scorer, boost):
+    """One BM25Term per clause: reader.phrase_stats of each positive clause, zeros for the negated ones."""
+    flat = [c for q in clauses for c in q]
+    return (N.BM25Term * max(len(flat), 1))(*[N.BM25Term() if n else reader.phrase_stats(scorer, ts, boost) for ts, _, n in flat])
+
+
+def ExecutePhraseAndCountBatch(reader, queries, filt=None, exclude=None, exclude_phrases=None):
+    """Count of conjunctions of phrases, terms and negated phrases (`"new york" & pizza & !"deep dish"`,
+    sdbg_phrase_and_count_batch). queries: per query its positive clauses, each a list of term ids (a phrase of adjacent
+    words; one id: a plain term) or a pair (term ids, rel_pos); exclude_phrases: per query its negated clauses in the same
+    form (or None); exclude: per query excluded term ids, as in ExecutePhraseCountBatch. A doc matches when every positive
+    clause occurs in it and no negated clause does. Returns uint64[Q]."""
+    clauses = _phrase_and_clauses(queries, exclude_phrases)
+    args, keep = _phrase_and_args(clauses, exclude)
+    counts = np.zeros(len(queries), np.uint64)
+    N.check(N.lib().sdbg_phrase_and_count_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), _ptr(counts)),
+            reader.segments[0].ctx._h)
+    return counts
+
+
+def ExecutePhraseAndCount(reader, query, filt=None, exclude=None, exclude_phrases=None):
+    """ExecutePhraseAndCountBatch for one query: its match count as an int."""
+    return int(ExecutePhraseAndCountBatch(reader, [list(query)], filt, _one(exclude), _one(exclude_phrases))[0])
+
+
+def ExecutePhraseAndTopKBatch(reader, queries, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, exclude_phrases=None,
+                              boost=1.0):
+    """Top-k of clause conjunctions (sdbg_phrase_and_topk_batch): a match scores the sum of its positive clauses' scores,
+    each bm25(phrase frequency, norm) with IndexReader.phrase_stats of that clause. Returns (hits [Q, k] structured,
+    n_out [Q], total_matches [Q]) as ExecuteTopKBatch."""
+    clauses = _phrase_and_clauses(queries, exclude_phrases)
+    args, keep = _phrase_and_args(clauses, exclude)
+    stats = _clause_stats(reader, clauses, scorer, boost)
+    nq = len(queries)
+    hits = np.zeros((nq, k), HIT_DTYPE)
+    n_out = np.zeros(nq, np.uint32)
+    total = np.zeros(nq, np.uint64)
+    N.check(N.lib().sdbg_phrase_and_topk_batch(_seg_array(reader.segments), len(reader.segments), *args, stats, scorer.k, scorer.b,
+                                               _ref(filt), int(k), float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)),
+            reader.segments[0].ctx._h)
+    return hits, n_out, total
+
+
+def ExecutePhraseAndTopK(reader, query, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, exclude_phrases=None, boost=1.0):
+    """ExecutePhraseAndTopKBatch for one query: (hits [n_out], total_matches)."""
+    hits, n_out, total = ExecutePhraseAndTopKBatch(reader, [list(query)], scorer, k, filt, threshold, _one(exclude),
+                                                   _one(exclude_phrases), boost)
+    return hits[0, :n_out[0]], int(total[0])
+
+
+def ExecutePhraseAndTopKByColumnBatch(reader, queries, sort_field, k, descending=False, nulls_first=False, filt=None,
+                                      exclude=None, exclude_phrases=None):
+    """Sorted scan of clause conjunctions (sdbg_phrase_and_topk_by_column_batch): the first k of the docs
+    ExecutePhraseAndCountBatch counts, in the order of ExecuteTopKByColumnBatch. Returns its dict."""
+    vt = _sort_value_type(reader, sort_field)
+    clauses = _phrase_and_clauses(queries, exclude_phrases)
+    args, keep = _phrase_and_args(clauses, exclude)
+    nq = len(queries)
+    hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
+    n_out = np.zeros(max(nq, 1), np.uint32)
+    N.check(N.lib().sdbg_phrase_and_topk_by_column_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt),
+                                                         int(sort_field), int(bool(descending)), int(bool(nulls_first)), int(k),
+                                                         _ptr(hits), _ptr(n_out)), reader.segments[0].ctx._h)
+    return _sort_result(hits, n_out, nq, k, vt)
+
+
+def ExecutePhraseAndTopKByColumn(reader, query, sort_field, k, descending=False, nulls_first=False, filt=None, exclude=None,
+                                 exclude_phrases=None):
+    """ExecutePhraseAndTopKByColumnBatch for one query: dict of docs, segs, values, nulls."""
+    return _sort_row(ExecutePhraseAndTopKByColumnBatch(reader, [list(query)], sort_field, k, descending, nulls_first, filt,
+                                                       _one(exclude), _one(exclude_phrases)))
+
+
+def ExecutePhraseAndFacetCountsBatch(reader, queries, key_field, key_min=None, key_span=None, filt=None, exclude=None,
+                                     exclude_phrases=None):
+    """Facet counts of clause conjunctions (sdbg_phrase_and_facet_counts_batch): how the docs ExecutePhraseAndCountBatch
+    counts split over the values of column `key_field`. Returns the dict ExecuteFacetCountsBatch returns."""
+    key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
+    clauses = _phrase_and_clauses(queries, exclude_phrases)
+    args, keep = _phrase_and_args(clauses, exclude)
+    nq = len(queries)
+    counts = np.zeros((max(nq, 1), max(int(key_span), 1)), np.uint64)
+    nulls = np.zeros(max(nq, 1), np.uint64)
+    N.check(N.lib().sdbg_phrase_and_facet_counts_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt),
+                                                       int(key_field), int(key_min), int(key_span), _ptr(counts), _ptr(nulls)),
+            reader.segments[0].ctx._h)
+    return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
+
+
+def ExecutePhraseAndFacetCounts(reader, query, key_field, key_min=None, key_span=None, filt=None, exclude=None,
+                                exclude_phrases=None):
+    """ExecutePhraseAndFacetCountsBatch for one query: {key: count} plus {None: n} for NULL keys."""
+    return _facet_row(ExecutePhraseAndFacetCountsBatch(reader, [list(query)], key_field, key_min, key_span, filt, _one(exclude),
+                                                       _one(exclude_phrases)))
+
+
+def ExecutePhraseAndMatchAggregatesBatch(reader, queries, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                                         exclude=None, exclude_phrases=None):
+    """Aggregates over the matches of clause conjunctions (sdbg_phrase_and_aggregate_batch): over the docs
+    ExecutePhraseAndCountBatch counts; the grouping and the result as in ExecuteMatchAggregatesBatch."""
+    vt, kf, key_min, key_span = _agg_args(reader, value_field, key_field, key_min, key_span)
+    clauses = _phrase_and_clauses(queries, exclude_phrases)
+    args, keep = _phrase_and_args(clauses, exclude)
+    nq = len(queries)
+    out = np.zeros((max(nq, 1), max(int(key_span), 1)), MATCH_AGG_DTYPE)
+    null_out = np.zeros(max(nq, 1), MATCH_AGG_DTYPE)
+    N.check(N.lib().sdbg_phrase_and_aggregate_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), kf,
+                                                    int(key_min), int(key_span), int(value_field), _ptr(out), _ptr(null_out)),
+            reader.segments[0].ctx._h)
+    return _agg_result(out, null_out, nq, key_min, vt)
+
+
+def ExecutePhraseAndMatchAggregates(reader, query, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                                    exclude=None, exclude_phrases=None):
+    """ExecutePhraseAndMatchAggregatesBatch for one query, in the form ExecuteMatchAggregates returns."""
+    return _agg_row(ExecutePhraseAndMatchAggregatesBatch(reader, [list(query)], value_field, key_field, key_min, key_span, filt,
+                                                         _one(exclude), _one(exclude_phrases)), key_field is not None)
+
+
+def ExecutePhraseAndMatchScanBatch(reader, queries, scorer=None, limit=1 << 20, offset=None, filt=None, exclude=None,
+                                   exclude_phrases=None, boost=1.0):
+    """Stream mode of clause conjunctions (sdbg_phrase_and_scan_batch): the docs ExecutePhraseAndCountBatch counts, in
+    (segment, doc) order, from ordinal offset[q] (None: 0) on, at most `limit` of them, scored as
+    ExecutePhraseAndTopKBatch scores them (scorer None: unscored). Returns what ExecuteMatchScanGroupsBatch returns."""
+    clauses = _phrase_and_clauses(queries, exclude_phrases)
+    args, keep = _phrase_and_args(clauses, exclude)
+    nq = len(queries)
+    stats = None if scorer is None else _clause_stats(reader, clauses, scorer, boost)
+    offs = None if offset is None else np.ascontiguousarray(offset, dtype=np.uint64)
+    if offs is not None and offs.shape != (nq,):
+        raise ValueError("offset needs one value per query")
+    hits = np.zeros((nq, max(int(limit), 1)), HIT_DTYPE)
+    n_out = np.zeros(nq, np.uint32)
+    total = np.zeros(nq, np.uint64)
+    k1, b = (0.0, 0.0) if scorer is None else (scorer.k, scorer.b)
+    N.check(N.lib().sdbg_phrase_and_scan_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), stats, k1, b,
+                                               _ptr(offs), int(limit), int(scorer is not None), _ptr(hits), _ptr(n_out),
+                                               _ptr(total)), reader.segments[0].ctx._h)
+    return [((hits["seg"][q, :n_out[q]].copy(), hits["doc"][q, :n_out[q]].copy(), hits["score"][q, :n_out[q]].copy()),
+             int(total[q])) for q in range(nq)]
+
+
+def ExecutePhraseAndMatchScan(reader, query, scorer=None, limit=1 << 20, offset=0, filt=None, exclude=None, exclude_phrases=None,
+                              boost=1.0):
+    """ExecutePhraseAndMatchScanBatch for one query: ((seg, doc, score) arrays, total matches)."""
+    return ExecutePhraseAndMatchScanBatch(reader, [list(query)], scorer, limit, [offset], filt, _one(exclude),
+                                          _one(exclude_phrases), boost)[0]
 
 
 SORT_HIT_DTYPE =np.dtype([("value", "<i8"), ("doc", "<u4"), ("seg", "<u4"), ("is_null", "u1"), ("pad", "V7")])

@@ -12,7 +12,8 @@
 // (tests/test_gpu_filter_chains.py). "scan" runs the Stream mode (GpuMatchScan) for flat, grouped and min-match queries
 // (tests/test_gpu_match_scan.py). "phrase" runs a phrase through the top-k and count adapters on a token corpus of its own
 // (tests/test_gpu_phrase.py); "phrase columns" runs the same phrases through the sorted, facet, aggregate and Stream
-// adapters instead (tests/test_gpu_phrase_column.py).
+// adapters instead (tests/test_gpu_phrase_column.py); "phrase and" runs conjunctions of phrases, terms and negated phrases
+// (clause_sizes / clause_negated) through all six phrase adapters (tests/test_gpu_phrase_and.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -38,7 +39,11 @@ struct ListCollector final : irs::ScoreCollector {  // a trivial ScoreCollector:
 // instead: GpuSortedScan ORDER BY column 20 DESC NULLS LAST LIMIT 30 (docs, values, valid), GpuFacetScan GROUP BY column 20
 // (keys, counts, valid), GpuMatchAggScan of column 20 without GROUP BY (count, count_value, sum_lo, min, max), and the
 // scored GpuMatchScan (docs, scores, total).
-int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns) {
+// With `clauses` ("phrase and"), the column is staged too and each case is an And of clauses (clause_sizes over the
+// slots, clause_negated); each line holds its slots, positions, sizes, negations and excluded terms, then the top-50
+// (GpuTopKIterator), total and count (GpuCountScan), the sorted docs, the facet keys and counts, the aggregate count
+// and the scored scan's docs, scores and total, as above.
+int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns, bool clauses) {
   uint32_t state = 12345u;
   auto next = [&]() { state = state * 1664525u + 1013904223u; return state >> 16; };
   constexpr uint32_t kVocab = 6;
@@ -80,7 +85,7 @@ int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns) {
     key[d - 1] = int64_t((uint64_t(d) * 7919u) % 23u) - 11;
     if (d % 5u) valid_bits[(d - 1) / 64] |= uint64_t(1) << ((d - 1) % 64);
   }
-  if (!rc && columns) rc = sdbg_stage_column(seg, 20, SDBG_I64, key.data(), valid_bits.data(), n_docs);
+  if (!rc && (columns || clauses)) rc = sdbg_stage_column(seg, 20, SDBG_I64, key.data(), valid_bits.data(), n_docs);
   if (rc) { std::printf("{\"error\": %d}\n", rc); return 1; }
   auto ints = [](const char* f, const auto& v) {
     std::printf(", \"%s\": [", f);
@@ -91,7 +96,60 @@ int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns) {
   const Case cases[] = {{{1, 0}, {0, 1}, {}}, {{2, 2, 4}, {0, 1, 3}, {5}}};
   ListCollector col;
   irs::ScoreFunction sf; irs::ColumnArgsFetcher fetcher;
-  for (const Case& cs : cases) {
+  if (clauses) {
+    // "1 0" & 2;  "2 2" & 4 & !"3 1" & !5;  0 & 1 & !3
+    struct AndCase { std::vector<uint32_t> slots, rel, sizes; std::vector<uint8_t> neg; std::vector<uint32_t> excl; };
+    const AndCase and_cases[] = {{{1, 0, 2}, {0, 1, 0}, {2, 1}, {0, 0}, {}},
+                                 {{2, 2, 4, 3, 1}, {0, 1, 0, 0, 1}, {2, 1, 2}, {0, 0, 1}, {5}},
+                                 {{0, 1, 3}, {0, 0, 0}, {1, 1, 1}, {0, 0, 1}, {}}};
+    for (const AndCase& cs : and_cases) {
+      std::vector<sdbg_bm25_term> terms(cs.slots.size());
+      for (size_t i = 0; i < terms.size(); ++i) {
+        sdbg_bm25_collect(n_docs, sum_len, docs[cs.slots[i]].size(), 1.2f, 0.75f, &terms[i]);
+        terms[i].term = cs.slots[i];
+      }
+      std::printf("{\"slots\": [");
+      for (size_t i = 0; i < cs.slots.size(); ++i) std::printf("%s%u", i ? ", " : "", cs.slots[i]);
+      std::printf("]");
+      ints("rel", cs.rel); ints("sizes", cs.sizes); ints("neg", cs.neg); ints("excl", cs.excl);
+      sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_AND, terms, 1.2f, 0.75f, 50, nullptr, cs.excl, {}, {}, cs.rel, cs.sizes, cs.neg);
+      col.docs.clear();
+      it.Collect(sf, fetcher, col);
+      std::printf(", \"topk\": [");
+      for (size_t i = 0; i < col.docs.size(); ++i) std::printf("%s[%u, %.9g]", i ? ", " : "", col.docs[i].doc, double(col.docs[i].score));
+      std::printf("], \"total\": %llu", static_cast<unsigned long long>(it.total_matches()));
+      duckdb::DataChunkMock out;
+      sdbg_host::GpuCountScan cnt({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, {}, {}, cs.rel, cs.sizes, cs.neg);
+      cnt.Scan(out);
+      std::printf(", \"count\": %lld", static_cast<long long>(out.count.empty() ? -1 : out.count[0]));
+      sdbg_host::GpuSortedScan sorted({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, 20, true, false, 30, {}, {}, cs.rel, cs.sizes,
+                                      cs.neg);
+      for (sorted.Scan(out); out.size; sorted.Scan(out)) ints("sorted_docs", out.doc);
+      sdbg_host::GpuFacetScan facet({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, 20, {}, {}, cs.rel, cs.sizes, cs.neg);
+      std::vector<int64_t> keys, counts;
+      for (facet.Scan(out); out.size; facet.Scan(out)) {
+        keys.insert(keys.end(), out.key.begin(), out.key.end());
+        counts.insert(counts.end(), out.count.begin(), out.count.end());
+      }
+      ints("facet_keys", keys); ints("facet_counts", counts);
+      sdbg_host::GpuMatchAggScan agg({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, UINT64_MAX, 20, SDBG_I64, {}, {}, cs.rel,
+                                     cs.sizes, cs.neg);
+      agg.Scan(out);
+      ints("agg_count", out.count);
+      sdbg_host::GpuMatchScan scan({seg}, terms, cs.excl, nullptr, 1.2f, 0.75f, true, {}, {}, cs.rel, cs.sizes, cs.neg);
+      std::vector<uint32_t> sdocs;
+      std::vector<float> sscores;
+      for (scan.Scan(out); out.size; scan.Scan(out)) {
+        sdocs.insert(sdocs.end(), out.doc.begin(), out.doc.end());
+        sscores.insert(sscores.end(), out.score.begin(), out.score.end());
+      }
+      ints("scan_docs", sdocs);
+      std::printf(", \"scan_scores\": [");
+      for (size_t i = 0; i < sscores.size(); ++i) std::printf("%s%.9g", i ? ", " : "", double(sscores[i]));
+      std::printf("], \"scan_total\": %llu}\n", static_cast<unsigned long long>(scan.total_matches()));
+    }
+  }
+  for (const Case& cs : clauses ? std::vector<Case>{} : std::vector<Case>(std::begin(cases), std::end(cases))) {
     std::vector<sdbg_bm25_term> terms(cs.slots.size());
     for (size_t i = 0; i < terms.size(); ++i) {
       sdbg_bm25_collect(n_docs, sum_len, docs[cs.slots[i]].size(), 1.2f, 0.75f, &terms[i]);
@@ -159,7 +217,8 @@ int main(int argc, char** argv) {
   sdbg_ctx* ctx = nullptr;
   int rc = sdbg_init(0, &ctx);
   if (rc != SDBG_OK) { std::printf("{\"error\": %d}\n", rc); return rc == SDBG_ENODEVICE ? 3 : 1; }
-  if (argc > 2 && std::string(argv[2]) == "phrase") return phrase_mode(ctx, n_docs, argc > 3 && std::string(argv[3]) == "columns");
+  if (argc > 2 && std::string(argv[2]) == "phrase")
+    return phrase_mode(ctx, n_docs, argc > 3 && std::string(argv[3]) == "columns", argc > 3 && std::string(argv[3]) == "and");
   sdbg_segment* seg = nullptr;
   sdbg_segment_create(ctx, n_docs, &seg);
   std::vector<uint32_t> dc(8);

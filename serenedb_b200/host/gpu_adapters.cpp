@@ -32,6 +32,26 @@ void check_phrase(const std::vector<uint32_t>& phrase, size_t n_terms, bool grou
   if (groups) throw GpuError(SDBG_EUNSUPPORTED, "a phrase has no OR groups");
 }
 
+// The clauses of a phrase query over its n_terms slots for the sdbg_phrase_and_* entries: clause_off (clause j is slots
+// off[j] .. off[j + 1]) and each clause's negation. Empty sizes and negations: the slots are one positive clause (a single
+// phrase). Not a phrase (no positions): no clauses.
+void phrase_clauses(const std::vector<uint32_t>& phrase, size_t n_terms, const std::vector<uint32_t>& sizes,
+                    const std::vector<uint8_t>& negated, std::vector<uint32_t>& off, std::vector<uint8_t>& neg) {
+  if (phrase.empty()) {
+    if (!sizes.empty() || !negated.empty()) throw GpuError(SDBG_EINVAL, "clause_sizes / clause_negated need phrase_positions");
+    return;
+  }
+  if (sizes.empty() && !negated.empty()) throw GpuError(SDBG_EINVAL, "clause_negated needs clause_sizes");
+  const std::vector<uint32_t> one{uint32_t(n_terms)};
+  const std::vector<uint32_t>& sz = sizes.empty() ? one : sizes;
+  if (!negated.empty() && negated.size() != sz.size()) throw GpuError(SDBG_EINVAL, "one clause_negated entry per clause");
+  off.assign(1, 0u);
+  for (uint32_t x : sz) off.push_back(off.back() + x);
+  if (off.back() != n_terms) throw GpuError(SDBG_EINVAL, "clause_sizes must cover the terms");
+  neg.assign(sz.size(), 0u);
+  for (size_t j = 0; j < negated.size(); ++j) neg[j] = negated[j] ? 1u : 0u;
+}
+
 // The statistics of a phrase (collectors.cpp:116-128): the slots' idfs summed in float32 in slot order, a repeated term
 // once per slot; the first slot's norm constants and boost (the field's, shared by every slot).
 sdbg_bm25_term phrase_stats(const std::vector<sdbg_bm25_term>& slots) {
@@ -40,6 +60,22 @@ sdbg_bm25_term phrase_stats(const std::vector<sdbg_bm25_term>& slots) {
   for (const sdbg_bm25_term& t : slots) idf += t.idf;
   s.idf = idf;
   return s;
+}
+
+// One statistics entry per clause: the phrase statistics of its slots (a one-slot clause: its term's own); negated
+// clauses never score and get zeros.
+std::vector<sdbg_bm25_term> clause_stats(const std::vector<sdbg_bm25_term>& terms, const std::vector<uint32_t>& off,
+                                         const std::vector<uint8_t>& neg) {
+  std::vector<sdbg_bm25_term> out(neg.size(), sdbg_bm25_term{});
+  for (size_t j = 0; j < neg.size(); ++j)
+    if (!neg[j]) out[j] = phrase_stats(std::vector<sdbg_bm25_term>(terms.begin() + off[j], terms.begin() + off[j + 1]));
+  return out;
+}
+
+std::vector<uint32_t> term_ids(const std::vector<sdbg_bm25_term>& terms) {
+  std::vector<uint32_t> ids(terms.size());
+  for (size_t i = 0; i < ids.size(); ++i) ids[i] = terms[i].term;
+  return ids;
 }
 }  // namespace
 
@@ -52,11 +88,13 @@ FilterChain::FilterChain(const sdbg_col_pred* table_filter) {
 GpuTopKIterator::GpuTopKIterator(sdbg_segment* segment, int kind, std::vector<sdbg_bm25_term> terms, float k1, float b,
                                  uint32_t k, const sdbg_col_pred* table_filter, std::vector<uint32_t> excluded_terms,
                                  std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
-                                 std::vector<uint32_t> phrase_positions)
+                                 std::vector<uint32_t> phrase_positions,
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
     : seg_(segment), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)), groups_(std::move(group_sizes)),
       group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)), k1_(k1), b_(b), k_(k), filter_(table_filter) {
   threshold_.value = FLT_MIN;  // doc_collector.hpp:102
   check_phrase(phrase_, terms_.size(), !groups_.empty());
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
   if (!phrase_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "phrases need k > 0: the streaming scan has no phrase form");
   // the streaming scan (sdbg_bm25_scan*) has no grouped form
   if (!groups_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "OR groups need k > 0: the streaming scan has no grouped form");
@@ -90,13 +128,13 @@ void GpuTopKIterator::run() {
   float thr_out = 0;
   sdbg_segment* segs[1] = {seg_};
   if (!phrase_.empty()) {
-    std::vector<uint32_t> ids(terms_.size());
-    for (size_t i = 0; i < ids.size(); ++i) ids[i] = terms_[i].term;
-    const sdbg_bm25_term stats = phrase_stats(terms_);
-    const uint32_t phrase_off[2] = {0, uint32_t(ids.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
-    check(sdbg_phrase_topk_batch(segs, 1, ids.data(), phrase_.data(), phrase_off, 1, excluded_.data(), excl_off, &stats, k1_, b_,
-                                 filter_.data(), k_, threshold_.value, hits_.data(), &n, &total_),
-          "sdbg_phrase_topk_batch");
+    const std::vector<uint32_t> ids = term_ids(terms_);
+    const std::vector<sdbg_bm25_term> stats = clause_stats(terms_, clause_off_, clause_neg_);
+    const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
+    check(sdbg_phrase_and_topk_batch(segs, 1, ids.data(), phrase_.data(), clause_off_.data(), clause_neg_.data(), query_clause_off, 1,
+                                     excluded_.data(), excl_off, stats.data(), k1_, b_, filter_.data(), k_, threshold_.value,
+                                     hits_.data(), &n, &total_),
+          "sdbg_phrase_and_topk_batch");
     thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;
   } else if (!groups_.empty()) {
     const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
@@ -234,11 +272,13 @@ void GpuAggScan::Scan(duckdb::DataChunkMock& output) {
 
 GpuCountScan::GpuCountScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, std::vector<uint32_t> group_sizes,
-                           std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions)
+                           std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions,
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       groups_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
       filter_(table_filter) {
   check_phrase(phrase_, terms_.size(), !groups_.empty());
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
 }
 
 void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
@@ -250,10 +290,10 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
   int rc;
   const char* what;
   if (!phrase_.empty()) {
-    const uint32_t phrase_off[2] = {0, uint32_t(terms_.size())};
-    rc = sdbg_phrase_count_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), phrase_off, 1, excluded_.data(), excl_off,
-                                 filter_.data(), &n);
-    what = "sdbg_phrase_count_batch: ";
+    const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
+    rc = sdbg_phrase_and_count_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), clause_neg_.data(),
+                                     query_clause_off, 1, excluded_.data(), excl_off, filter_.data(), &n);
+    what = "sdbg_phrase_and_count_batch: ";
   } else if (groups_.empty()) {
     rc = sdbg_match_count_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                 filter_.data(), &n);
@@ -275,11 +315,13 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
 GpuSortedScan::GpuSortedScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                              std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t sort_field,
                              bool descending, bool nulls_first, uint32_t k, std::vector<uint32_t> group_sizes,
-                             std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions)
+                             std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions,
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
       filter_(table_filter), field_(sort_field), desc_(descending), nulls_first_(nulls_first), k_(k) {
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
 }
 
 void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
@@ -292,11 +334,11 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
     int rc;
     const char* what;
     if (!phrase_.empty()) {
-      const uint32_t phrase_off[2] = {0, uint32_t(terms_.size())};
-      rc = sdbg_phrase_topk_by_column_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), phrase_off, 1, excluded_.data(),
-                                            excl_off, filter_.data(), field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
-                                            hits_.data(), &n);
-      what = "sdbg_phrase_topk_by_column_batch: ";
+      const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
+      rc = sdbg_phrase_and_topk_by_column_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
+                                                clause_neg_.data(), query_clause_off, 1, excluded_.data(), excl_off, filter_.data(),
+                                                field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_, hits_.data(), &n);
+      what = "sdbg_phrase_and_topk_by_column_batch: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_topk_by_column_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                            filter_.data(), field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
@@ -330,12 +372,14 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
 GpuMatchScan::GpuMatchScan(std::vector<sdbg_segment*> segments, std::vector<sdbg_bm25_term> terms,
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, float k1, float b, bool scored,
                            std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
-                           std::vector<uint32_t> phrase_positions)
+                           std::vector<uint32_t> phrase_positions,
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
     : segs_(std::move(segments)), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(group_sizes.empty() ? std::vector<uint32_t>{uint32_t(terms_.size())} : std::move(group_sizes)),
       group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)), filter_(table_filter), k1_(k1), b_(b),
       scored_(scored) {
   check_phrase(phrase_, terms_.size(), group_sizes_.size() > 1 || !group_min_.empty());
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
 }
 
 void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kPage - 1
@@ -347,14 +391,13 @@ void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kP
   int rc;
   const char* what;
   if (!phrase_.empty()) {
-    std::vector<uint32_t> ids(terms_.size());
-    for (size_t i = 0; i < ids.size(); ++i) ids[i] = terms_[i].term;
-    const sdbg_bm25_term stats = phrase_stats(terms_);
-    const uint32_t phrase_off[2] = {0, uint32_t(ids.size())};
-    rc = sdbg_phrase_scan_batch(segs_.data(), segs_.size(), ids.data(), phrase_.data(), phrase_off, 1, excluded_.data(), excl_off,
-                                filter_.data(), scored_ ? &stats : nullptr, k1_, b_, &offset_, kPage, scored_ ? 1 : 0,
-                                page_.data(), &n, &total_);
-    what = "sdbg_phrase_scan_batch: ";
+    const std::vector<uint32_t> ids = term_ids(terms_);
+    const std::vector<sdbg_bm25_term> stats = clause_stats(terms_, clause_off_, clause_neg_);
+    const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
+    rc = sdbg_phrase_and_scan_batch(segs_.data(), segs_.size(), ids.data(), phrase_.data(), clause_off_.data(), clause_neg_.data(),
+                                    query_clause_off, 1, excluded_.data(), excl_off, filter_.data(), scored_ ? stats.data() : nullptr,
+                                    k1_, b_, &offset_, kPage, scored_ ? 1 : 0, page_.data(), &n, &total_);
+    what = "sdbg_phrase_and_scan_batch: ";
   } else {
     rc = sdbg_match_scan_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
                                           group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(), excl_off,
@@ -385,11 +428,13 @@ void GpuMatchScan::Scan(duckdb::DataChunkMock& output) {
 GpuFacetScan::GpuFacetScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
                            std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
-                           std::vector<uint32_t> phrase_positions)
+                           std::vector<uint32_t> phrase_positions,
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
       filter_(table_filter), field_(key_field) {
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
 }
 
 void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
@@ -413,10 +458,11 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
     int rc;
     const char* what;
     if (!phrase_.empty()) {
-      const uint32_t phrase_off[2] = {0, uint32_t(terms_.size())};
-      rc = sdbg_phrase_facet_counts_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), phrase_off, 1, excluded_.data(),
-                                          excl_off, filter_.data(), field_, lo, uint32_t(span), counts.data(), &nulls_);
-      what = "sdbg_phrase_facet_counts_batch: ";
+      const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
+      rc = sdbg_phrase_and_facet_counts_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
+                                              clause_neg_.data(), query_clause_off, 1, excluded_.data(), excl_off, filter_.data(),
+                                              field_, lo, uint32_t(span), counts.data(), &nulls_);
+      what = "sdbg_phrase_and_facet_counts_batch: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_facet_counts_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                          filter_.data(), field_, lo, uint32_t(span), counts.data(), &nulls_);
@@ -450,11 +496,13 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
 GpuMatchAggScan::GpuMatchAggScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                                  std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
                                  uint64_t value_field, sdbg_type value_type, std::vector<uint32_t> group_sizes,
-                                 std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions)
+                                 std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions,
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
       filter_(table_filter), key_field_(key_field), value_field_(value_field), value_type_(value_type) {
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
 }
 
 void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
@@ -485,11 +533,11 @@ void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
     int rc;
     const char* what;
     if (!phrase_.empty()) {
-      const uint32_t phrase_off[2] = {0, uint32_t(terms_.size())};
-      rc = sdbg_phrase_aggregate_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), phrase_off, 1, excluded_.data(),
-                                       excl_off, filter_.data(), key_field_, lo, uint32_t(span), value_field_, cells.data(),
-                                       &null_cell);
-      what = "sdbg_phrase_aggregate_batch: ";
+      const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
+      rc = sdbg_phrase_and_aggregate_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
+                                           clause_neg_.data(), query_clause_off, 1, excluded_.data(), excl_off, filter_.data(),
+                                           key_field_, lo, uint32_t(span), value_field_, cells.data(), &null_cell);
+      what = "sdbg_phrase_and_aggregate_batch: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_aggregate_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                       filter_.data(), key_field_, lo, uint32_t(span), value_field_, cells.data(),

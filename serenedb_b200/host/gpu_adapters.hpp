@@ -51,8 +51,12 @@ class GpuTopKIterator final : public irs::DocIterator {
                   std::vector<uint32_t> excluded_terms = {} /* term ids of the And's Not children (irs exclusion.hpp) */,
                   std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */,
                   std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+
                   std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
-                                                                 relative positions (0 first, increasing); needs k > 0 */);
+                                                                 relative positions (0 first, increasing); needs k > 0 */,
+                  std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
+                                                            phrase_positions (a one-slot clause is a term); empty: one phrase */,
+                  std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
 
   // Scored top-k: the hot path.
   void Collect(const irs::ScoreFunction&, irs::ColumnArgsFetcher&, irs::ScoreCollector& collector) override;
@@ -88,6 +92,8 @@ class GpuTopKIterator final : public irs::DocIterator {
   std::vector<uint32_t> groups_;   // sizes of the OR groups over terms_ (empty: the flat `kind_` query)
   std::vector<uint32_t> group_min_;   // their minimum match counts (empty: all 1)
   std::vector<uint32_t> phrase_;      // a phrase's relative positions, one per term (empty: not a phrase)
+  std::vector<uint32_t> clause_off_;  // the clauses over terms_ / phrase_ (a single phrase: one clause)
+  std::vector<uint8_t> clause_neg_;   // per clause: negated
   float k1_, b_;
   uint32_t k_;
   FilterChain filter_;
@@ -129,15 +135,20 @@ class GpuCountScan {
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */,
                std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+
                std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
-                                                              relative positions (0 first, increasing) */);
+                                                              relative positions (0 first, increasing) */,
+               std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
+                                                         phrase_positions (a one-slot clause is a term); empty: one phrase */,
+               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
   // Fills `output` with one row, count[0] = the number of matches; the next call leaves it empty (end of scan).
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, groups_, group_min_, phrase_;
+  std::vector<uint32_t> terms_, excluded_, groups_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
+  std::vector<uint8_t> clause_neg_;
   FilterChain filter_;
   bool done_ = false;
 };
@@ -155,14 +166,19 @@ class GpuSortedScan {
                 uint32_t k /* LIMIT (+ OFFSET), 1..4096 */,
                 std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
                 std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+
                 std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
-                                                               relative positions (0 first, increasing) */);
+                                                               relative positions (0 first, increasing) */,
+                std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
+                                                          phrase_positions (a one-slot clause is a term); empty: one phrase */,
+                std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
+  std::vector<uint8_t> clause_neg_;
   FilterChain filter_;
   uint64_t field_;
   bool desc_, nulls_first_;
@@ -186,8 +202,12 @@ class GpuMatchScan {
                float k1, float b, bool scored,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors over `terms`; empty = one group (a flat OR) */,
                std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+
                std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
-                                                              relative positions (0 first, increasing) */);
+                                                              relative positions (0 first, increasing) */,
+               std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
+                                                         phrase_positions (a one-slot clause is a term); empty: one phrase */,
+               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
   void Scan(duckdb::DataChunkMock& output);
   uint64_t total_matches() const { return total_; }
 
@@ -195,7 +215,8 @@ class GpuMatchScan {
   void Fetch();
   std::vector<sdbg_segment*> segs_;
   std::vector<sdbg_bm25_term> terms_;
-  std::vector<uint32_t> excluded_, group_sizes_, group_min_, phrase_;
+  std::vector<uint32_t> excluded_, group_sizes_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
+  std::vector<uint8_t> clause_neg_;
   FilterChain filter_;
   float k1_, b_;
   bool scored_;
@@ -218,14 +239,19 @@ class GpuFacetScan {
                uint64_t key_field /* int64 or int32 */,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
                std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+
                std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
-                                                              relative positions (0 first, increasing) */);
+                                                              relative positions (0 first, increasing) */,
+               std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
+                                                         phrase_positions (a one-slot clause is a term); empty: one phrase */,
+               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
+  std::vector<uint8_t> clause_neg_;
   FilterChain filter_;
   uint64_t field_;
   std::vector<std::pair<int64_t, uint64_t>> groups_;   // (key, count) of the non-empty groups
@@ -251,14 +277,19 @@ class GpuMatchAggScan {
                   sdbg_type value_type /* as staged: picks sum_f64 or the 128-bit sum for avg */,
                   std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
                   std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+
                   std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
-                                                                 relative positions (0 first, increasing) */);
+                                                                 relative positions (0 first, increasing) */,
+                  std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
+                                                            phrase_positions (a one-slot clause is a term); empty: one phrase */,
+                  std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
-  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_;
+  std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
+  std::vector<uint8_t> clause_neg_;
   FilterChain filter_;
   uint64_t key_field_, value_field_;
   sdbg_type value_type_;

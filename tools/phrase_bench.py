@@ -15,9 +15,14 @@ values and an int32 column `cat` of 100 values):
   SUM / AVG(ts) GROUP BY cat (sdbg_phrase_aggregate_batch)
   the first scan page of 1000, unscored and scored (sdbg_phrase_scan_batch), and an unscored page of 1000 from the
   middle of each phrase's matches (a page deep in the result repeats the phrase check over the items before it).
+A third batch, "phrase-and", times conjunctions of a phrase with a term (sdbg_phrase_and_*_batch): --queries
+queries `"w1 w2" & t`, t a token drawn from the phrase's own doc, and the same with `& !"w3 w4"` added, w3 w4 a window
+drawn as the phrases are. For each it reports the count, the top-1000 and the facets GROUP BY cat, next to the phrase
+"w1 w2" alone and the AND of w1, w2 and t (and of w3, w4 not excluded: the AND of w1, w2, t is the candidate set).
+--batches picks the batches to run (comma-separated; all by default).
 Prints one JSON line with the GPU name and power limit read in the same run.
 
-    python tools/phrase_bench.py [--steps 5] [--warmup 2] [--docs 10000000] [--queries 4096]
+    python tools/phrase_bench.py [--steps 5] [--warmup 2] [--docs 10000000] [--queries 4096] [--batches 2-word,phrase-and]
 """
 import argparse
 import json
@@ -75,6 +80,48 @@ def phrases(c, n, length, rng):
     return out
 
 
+def phrase_and_rows(c, reader, ctx, scorer, n, rng, steps, warmup):
+    """The "phrase-and" batch: `"w1 w2" & t` and `"w1 w2" & t & !"w3 w4"` next to "w1 w2" and the AND of w1, w2, t."""
+    terms, doc = c["terms"], c["doc"]
+    ph, ts = [], []
+    while len(ph) < n:
+        i = int(rng.integers(0, len(terms) - 2))
+        if doc[i] != doc[i + 1]:
+            continue
+        same = np.flatnonzero(doc[max(0, i - 28):i + 30] == doc[i]) + max(0, i - 28)
+        ph.append([int(terms[i]), int(terms[i + 1])])
+        ts.append(int(terms[int(same[int(rng.integers(0, len(same)))])]))
+    neg = phrases(c, n, 2, rng)
+    plain = [[p, [t]] for p, t in zip(ph, ts)]
+    conj = [sorted(set(p + [t])) for p, t in zip(ph, ts)]
+    pc = sdb.ExecutePhraseCountBatch(reader, ph)
+    ac = sdb.ExecuteCountBatch(reader, conj, sdb.AND)
+    qc = sdb.ExecutePhraseAndCountBatch(reader, plain)
+    nc = sdb.ExecutePhraseAndCountBatch(reader, plain, exclude_phrases=[[x] for x in neg])
+    _, _, qt = sdb.ExecutePhraseAndTopKBatch(reader, plain, scorer, 1000)
+    fac = sdb.ExecutePhraseAndFacetCountsBatch(reader, plain, 2, 0, 100)
+    if (not np.array_equal(qc, qt) or not np.array_equal(fac["counts"].sum(1), qc) or np.any(qc > pc) or np.any(qc > ac)
+            or np.any(nc > qc)):
+        raise SystemExit("phrase-and count / top-k / facet mismatch")
+    r = {"phrase_matches": int(pc.sum()), "and_matches": int(ac.sum()), "phrase_and_matches": int(qc.sum()),
+         "phrase_and_not_matches": int(nc.sum())}
+    runs = (("phrase", lambda: sdb.ExecutePhraseCountBatch(reader, ph), lambda: sdb.ExecutePhraseTopKBatch(reader, ph, scorer, 1000),
+             lambda: sdb.ExecutePhraseFacetCountsBatch(reader, ph, 2, 0, 100)),
+            ("and", lambda: sdb.ExecuteCountBatch(reader, conj, sdb.AND), lambda: sdb.ExecuteTopKBatch(reader, conj, sdb.AND, scorer, 1000),
+             lambda: sdb.ExecuteFacetCountsBatch(reader, conj, sdb.AND, 2, 0, 100)),
+            ("phrase_and", lambda: sdb.ExecutePhraseAndCountBatch(reader, plain),
+             lambda: sdb.ExecutePhraseAndTopKBatch(reader, plain, scorer, 1000),
+             lambda: sdb.ExecutePhraseAndFacetCountsBatch(reader, plain, 2, 0, 100)),
+            ("phrase_and_not", lambda: sdb.ExecutePhraseAndCountBatch(reader, plain, exclude_phrases=[[x] for x in neg]),
+             lambda: sdb.ExecutePhraseAndTopKBatch(reader, plain, scorer, 1000, exclude_phrases=[[x] for x in neg]),
+             lambda: sdb.ExecutePhraseAndFacetCountsBatch(reader, plain, 2, 0, 100, exclude_phrases=[[x] for x in neg])))
+    for name, cnt, top, facets in runs:
+        r[name + "_count_ms"] = timed(ctx, cnt, steps, warmup)
+        r[name + "_top1000_ms"] = timed(ctx, top, steps, warmup)
+        r[name + "_facets_ms"] = timed(ctx, facets, steps, warmup)
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
@@ -82,7 +129,9 @@ def main():
     ap.add_argument("--docs", type=int, default=10_000_000)
     ap.add_argument("--vocab", type=int, default=100_000)
     ap.add_argument("--queries", type=int, default=4096)
+    ap.add_argument("--batches", default="2-word,3/4-word,phrase-and")
     a = ap.parse_args()
+    want = set(a.batches.split(","))
     c = corpus(a.docs, a.vocab, 7)
     ctx = sdb.Context(0)
     seg = sdb.Segment(ctx, c["n"])
@@ -99,6 +148,8 @@ def main():
     ctx.set_wand(0)
     for name, qs in (("2-word", phrases(c, a.queries, 2, rng)),
                      ("3/4-word", phrases(c, a.queries // 2, 3, rng) + phrases(c, a.queries - a.queries // 2, 4, rng))):
+        if name not in want:
+            continue
         conj = [sorted(set(q)) for q in qs]
         pc = sdb.ExecutePhraseCountBatch(reader, qs)
         ac = sdb.ExecuteCountBatch(reader, conj, sdb.AND)
@@ -131,6 +182,8 @@ def main():
         r["phrase_scan1000_mid_ms"] = timed(ctx, lambda: sdb.ExecutePhraseMatchScanBatch(reader, qs, None, 1000, mid), a.steps,
                                             a.warmup)
         out["batches"][name] = r
+    if "phrase-and" in want:
+        out["batches"]["phrase-and"] = phrase_and_rows(c, reader, ctx, scorer, a.queries, np.random.default_rng(17), a.steps, a.warmup)
     print(json.dumps(out))
 
 
