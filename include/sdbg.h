@@ -606,6 +606,77 @@ int sdbg_phrase_and_scan_batch(sdbg_segment* const* segs, size_t n_segs, const u
                                const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats /* NULL when scored == 0 */,
                                float k1, float b, const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit,
                                int scored, sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
+/* Conjunctions of OR groups of phrases and terms (`("new york" | nyc) & pizza & !"deep dish"`; the shape synonym
+ * expansion of multi-word synonyms produces). Query q is an AND of the groups query_group_off[q] .. query_group_off[q+1])
+ * (1..16), plus excl_terms / excl_off and the filter chain as above. Group g is an OR of the alternatives group_off[g] ..
+ * group_off[g+1]) (1..16); it is negated when group_negated[g] != 0 (group_negated NULL: none), and a query needs a
+ * positive group. Alternative j is a phrase exactly as a clause of sdbg_phrase_and_*: slots clause_off[j] ..
+ * clause_off[j+1]) at rel_pos starting at 0 and strictly increasing (rel_pos NULL: adjacent), gaps and repeated terms
+ * allowed; a one-slot alternative is a plain term. At most 16 slots per query, every alternative of every group counted.
+ * Doc d matches when every positive group has an alternative with phrase frequency > 0 in d, no alternative of a negated
+ * group has (`!(A | B)` is `!A & !B`), d is not deleted, passes the filter chain and holds none of the excluded terms. An
+ * alternative with a term a segment holds no postings for matches nothing there (a positive group all of whose
+ * alternatives are so matches nothing, so neither does the query) and, negated, excludes nothing there.
+ * Score (the top-k, and the scan with scored != 0): the fp32 sum, from 0, of bm25(phrase frequency, norm(d)) over the
+ * positive alternatives with frequency > 0 in d, whatever their group, each with its own statistics clause_stats[j] (one
+ * per alternative, .term ignored, negated groups' entries ignored), in ascending cost order within d's segment: an
+ * alternative costs the smallest docs_count of its terms there, ties in the query's alternative order, flattened group by
+ * group. Duplicate alternatives are each scored; negated groups never score. Every group of one alternative gives exactly
+ * sdbg_phrase_and_* (which, with sdbg_phrase_*, runs as this case); one-slot alternatives of distinct terms give exactly
+ * the *_groups_min entries with every minimum 1 (the top-k bit for bit at pruning level 0); one group of one-slot
+ * alternatives gives exactly the flat OR entries. Nothing is pruned: identical at every pruning level, k <= 4096.
+ * Each entry takes the parameters of its sdbg_phrase_and_* counterpart, with (clause_off, clause_negated,
+ * query_clause_off) replaced by (clause_off, group_off, group_negated, query_group_off); outputs, orders, NULL rules and
+ * scratch are the counterpart's. Errors, all found before anything is queued: an empty group or clause, a query without
+ * a group or without a positive group, bad rel_pos, decreasing offsets, NULL arrays with non-empty ranges, NULL
+ * clause_stats where a score is needed: SDBG_EINVAL; more than 16 slots, groups or excluded ids in a query, k > 4096:
+ * SDBG_EUNSUPPORTED; a segment without staged positions: SDBG_ENOTFOUND; otherwise the counterpart's. Synchronous. */
+int sdbg_phrase_groups_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                   const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                   const uint32_t* clause_off, const uint32_t* group_off,
+                                   const uint8_t* group_negated /* NULL: none */, const uint32_t* query_group_off,
+                                   size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                   const sdbg_col_pred* filt, uint64_t* counts);
+int sdbg_phrase_groups_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                  const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                  const uint32_t* clause_off, const uint32_t* group_off,
+                                  const uint8_t* group_negated /* NULL: none */, const uint32_t* query_group_off,
+                                  size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                  const sdbg_bm25_term* clause_stats /* one per alternative */, float k1, float b,
+                                  const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out /* n_queries * k */,
+                                  uint32_t* n_out, uint64_t* total_matches);
+int sdbg_phrase_groups_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                            const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                            const uint32_t* clause_off, const uint32_t* group_off,
+                                            const uint8_t* group_negated /* NULL: none */, const uint32_t* query_group_off,
+                                            size_t n_queries, const uint32_t* excl_terms,
+                                            const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                                            uint64_t sort_field, int descending, int nulls_first, uint32_t k,
+                                            sdbg_sort_hit* out /* n_queries * k */, uint32_t* n_out);
+int sdbg_phrase_groups_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                          const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                          const uint32_t* clause_off, const uint32_t* group_off,
+                                          const uint8_t* group_negated /* NULL: none */, const uint32_t* query_group_off,
+                                          size_t n_queries, const uint32_t* excl_terms,
+                                          const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                                          uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                          uint64_t* counts /* n_queries * key_span */, uint64_t* null_counts /* n_queries */);
+int sdbg_phrase_groups_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                       const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                       const uint32_t* clause_off, const uint32_t* group_off,
+                                       const uint8_t* group_negated /* NULL: none */, const uint32_t* query_group_off,
+                                       size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                       const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                       uint64_t value_field, sdbg_match_agg* out /* n_queries * key_span */,
+                                       sdbg_match_agg* null_out /* n_queries */);
+int sdbg_phrase_groups_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                  const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                  const uint32_t* clause_off, const uint32_t* group_off,
+                                  const uint8_t* group_negated /* NULL: none */, const uint32_t* query_group_off,
+                                  size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                  const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats /* NULL when scored == 0 */,
+                                  float k1, float b, const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit,
+                                  int scored, sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

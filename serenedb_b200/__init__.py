@@ -16,6 +16,10 @@ from .engine import (ExecutePhraseTopKByColumn, ExecutePhraseTopKByColumnBatch, 
                      ExecutePhraseMatchScan, ExecutePhraseMatchScanBatch)
 from .engine import (ExecutePhraseAndCount, ExecutePhraseAndCountBatch, ExecutePhraseAndTopK, ExecutePhraseAndTopKBatch, ExecutePhraseAndTopKByColumn, ExecutePhraseAndTopKByColumnBatch,
                      ExecutePhraseAndFacetCounts, ExecutePhraseAndFacetCountsBatch, ExecutePhraseAndMatchAggregates, ExecutePhraseAndMatchAggregatesBatch, ExecutePhraseAndMatchScan, ExecutePhraseAndMatchScanBatch)
+from .engine import (ExecutePhraseGroupsCount, ExecutePhraseGroupsCountBatch, ExecutePhraseGroupsTopK, ExecutePhraseGroupsTopKBatch,
+                     ExecutePhraseGroupsTopKByColumn, ExecutePhraseGroupsTopKByColumnBatch, ExecutePhraseGroupsFacetCounts,
+                     ExecutePhraseGroupsFacetCountsBatch, ExecutePhraseGroupsMatchAggregates, ExecutePhraseGroupsMatchAggregatesBatch,
+                     ExecutePhraseGroupsMatchScan, ExecutePhraseGroupsMatchScanBatch)
 from .engine import (AND, OR, BM25, TFIDF, FLT_MIN, Context, ExecuteCount, ExecuteCountBatch, ExecuteCountGroups,
                      ExecuteCountGroupsBatch, ExecuteFacetCounts, ExecuteFacetCountsBatch, ExecuteFacetCountsGroups,
                      ExecuteFacetCountsGroupsBatch, ExecuteMatchAggregates, ExecuteMatchAggregatesBatch,
@@ -39,4 +43,8 @@ __all__ = ["AND", "OR", "BM25", "TFIDF", "FLT_MIN", "Context", "ExecuteCount", "
            "ExecutePhraseTopKBatch", "ExecutePhraseTopKByColumn", "ExecutePhraseTopKByColumnBatch", "ExecutePhraseFacetCounts",
            "ExecutePhraseFacetCountsBatch", "ExecutePhraseMatchAggregates", "ExecutePhraseMatchAggregatesBatch",
            "ExecutePhraseMatchScan", "ExecutePhraseMatchScanBatch", "ExecutePhraseAndCount", "ExecutePhraseAndCountBatch", "ExecutePhraseAndTopK", "ExecutePhraseAndTopKBatch",
-           "ExecutePhraseAndTopKByColumn", "ExecutePhraseAndTopKByColumnBatch", "ExecutePhraseAndFacetCounts", "ExecutePhraseAndFacetCountsBatch", "ExecutePhraseAndMatchAggregates", "ExecutePhraseAndMatchAggregatesBatch", "ExecutePhraseAndMatchScan", "ExecutePhraseAndMatchScanBatch"]
+           "ExecutePhraseAndTopKByColumn", "ExecutePhraseAndTopKByColumnBatch", "ExecutePhraseAndFacetCounts", "ExecutePhraseAndFacetCountsBatch", "ExecutePhraseAndMatchAggregates", "ExecutePhraseAndMatchAggregatesBatch", "ExecutePhraseAndMatchScan", "ExecutePhraseAndMatchScanBatch",
+           "ExecutePhraseGroupsCount", "ExecutePhraseGroupsCountBatch", "ExecutePhraseGroupsTopK", "ExecutePhraseGroupsTopKBatch",
+           "ExecutePhraseGroupsTopKByColumn", "ExecutePhraseGroupsTopKByColumnBatch", "ExecutePhraseGroupsFacetCounts",
+           "ExecutePhraseGroupsFacetCountsBatch", "ExecutePhraseGroupsMatchAggregates", "ExecutePhraseGroupsMatchAggregatesBatch",
+           "ExecutePhraseGroupsMatchScan", "ExecutePhraseGroupsMatchScanBatch"]

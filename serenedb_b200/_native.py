@@ -128,6 +128,18 @@ SIGNATURES = {
                                                   C.c_uint32, C.c_uint64, _vp, _vp]),
     "sdbg_phrase_and_scan_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, C.c_float, C.c_float,
                                              _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
+    # the OR groups: (terms, rel_pos, clause_off, group_off, group_negated, query_group_off, n_queries) for the phrase args
+    "sdbg_phrase_groups_count_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "sdbg_phrase_groups_topk_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_float, C.c_float,
+                                                _vp, C.c_uint32, C.c_float, _vp, _vp, _vp]),
+    "sdbg_phrase_groups_topk_by_column_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
+                                                          C.c_int, C.c_int, C.c_uint32, _vp, _vp]),
+    "sdbg_phrase_groups_facet_counts_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
+                                                        C.c_int64, C.c_uint32, _vp, _vp]),
+    "sdbg_phrase_groups_aggregate_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64,
+                                                     C.c_int64, C.c_uint32, C.c_uint64, _vp, _vp]),
+    "sdbg_phrase_groups_scan_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, C.c_float,
+                                                C.c_float, _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
     "sdbg_match_topk_by_column_batch":(C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int, C.c_int,
                                                   C.c_uint32, _vp, _vp]),
     "sdbg_match_facet_counts_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,

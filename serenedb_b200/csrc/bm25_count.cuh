@@ -161,12 +161,13 @@ constexpr int kPhraseMinBlocks = 4;
 // gives each doc its ordinal, base[item.w] plus the matches of the item's earlier windows; the docs whose ordinal lies in
 // [offset[q], offset[q] + limit) go to their row of P.emit.out, unscored. An item whose ordinals miss the page exits
 // before it decodes anything, and an item stops after the window that fills the page.
-// kPhrase (with kAnd, the conjunction of the positive clauses' terms): the clause check (phrase_clauses,
-// bm25_phrase.cuh). Every doc that survives the conjunction, the exclusions, the deleted docs and the filter chain is
-// probed, clause after clause of the query's clause table, in each slot's list for its positions; a doc that fails a
-// clause is dropped, the others are counted and, with P.phrase.cap, scored as the sum of their positive clauses' scores
-// and kept in a buffer of P.phrase.cap keys in dynamic shared memory as the sorted scan keeps its keys; the item's k best
-// go to slot item.w. Without a score the one-slot positive clauses, which the conjunction guarantees, are skipped.
+// kPhrase (on any candidate shape: the AND, the flat OR or the OR groups (m = 1) of the alternatives' proxy terms): the
+// alternative check (phrase_clauses, bm25_phrase.cuh). Every doc that survives the candidate scan, the exclusions, the
+// deleted docs and the filter chain is probed, entry after entry of the query's alternative table, in each slot's list
+// for its positions; a doc that fails its groups is dropped, the others are counted and, with P.phrase.cap, scored as the
+// sum of their matching positive alternatives' scores and kept in a buffer of P.phrase.cap keys in dynamic shared memory
+// as the sorted scan keeps its keys; the item's k best go to slot item.w. Without a score the entries of groups that the
+// candidate scan guarantees, or that an earlier entry satisfied, are skipped.
 // kPhrase with one other sink: with kFacet, kAgg or kEmit the clause check is a stage that narrows `acc` after the
 // exclusions (deleted docs, filter chain, then the check per surviving bit, written back), so the sink reads only
 // matches and emit passes A and B see the same set. With kSort it runs inside the sink, on a doc whose key has passed
@@ -181,8 +182,7 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0)
   static_assert(!(kFacet && kSort), "the facet pass has its own sink");
   static_assert(!(kAgg && (kSort || kFacet)), "the aggregate pass has its own sink");
   static_assert(!(kEmit && (kSort || kFacet || kAgg)), "the match scan has its own sink");
-  static_assert(!kPhrase || (kAnd && int(kSort) + int(kFacet) + int(kAgg) + int(kEmit) <= 1),
-                "a phrase is checked on its terms' conjunction");
+  static_assert(!kPhrase || int(kSort) + int(kFacet) + int(kAgg) + int(kEmit) <= 1, "the phrase check serves one sink");
   constexpr bool kPhraseSink = kPhrase && !kSort && !kFacet && !kAgg && !kEmit;   // count / top-k of phrase matches
   constexpr bool kPhraseStage = kPhrase && (kFacet || kAgg || kEmit);           // narrows acc before the sink
   __shared__ uint32_t acc[kCountWords];
@@ -379,11 +379,11 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0)
       }
     }
     if constexpr (kGroups) {
-      // the lead group is already in acc unless it needs m >= 2 of its lists
-      for (uint32_t g = (gend0 >> 8) ? 0u : 1u; g < n_groups; ++g) {
+      // the lead group is already in acc unless it needs m >= 2 of its lists (never for phrase candidates)
+      for (uint32_t g = !kPhrase && (gend0 >> 8) ? 0u : 1u; g < n_groups; ++g) {
         const uint32_t lo = g ? s_gend[g - 1] & 0xFFu : 0u, hi = s_gend[g] & 0xFFu, m = (s_gend[g] >> 8) + 1u;
         uint32_t nz = 0u;
-        if (m == 1u) {
+        if (kPhrase || m == 1u) {
           for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
           __syncthreads();
           run_lists(lo, hi, tmp, false, true);
@@ -437,7 +437,7 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0)
           v = chain_bits(v, i);
           for (uint32_t r = v; r; r &= r - 1u) {
             const uint32_t bit = __ffs(r) - 1u;
-            if (!phrase_clauses(P.seg, P.phrase, PQ, ws + 32u * i + bit, PhraseMode::check, unused)) v &= ~(1u << bit);
+            if (!phrase_clauses<!kAnd>(P.seg, P.phrase, PQ, ws + 32u * i + bit, PhraseMode::check, unused)) v &= ~(1u << bit);
           }
           acc[i] = v;
         }
@@ -513,7 +513,7 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0)
               if (key.x < thr) continue;
               if constexpr (kPhrase) {
                 float unused;
-                if (!phrase_clauses(P.seg, P.phrase, PQ, doc, PhraseMode::check, unused)) continue;
+                if (!phrase_clauses<!kAnd>(P.seg, P.phrase, PQ, doc, PhraseMode::check, unused)) continue;
               }
               const uint32_t slot = atomicAdd(&s_fill[0], 1u);
               if (slot >= cap) break;
@@ -545,7 +545,7 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0)
             for (; v; v &= v - 1u) {
               const uint32_t doc = ws + 32u * i + (__ffs(v) - 1u);
               float s;
-              if (!phrase_clauses(P.seg, F, PQ, doc, mode, s)) continue;
+              if (!phrase_clauses<!kAnd>(P.seg, F, PQ, doc, mode, s)) continue;
               if (cap) {
                 const unsigned long long key = phrase_key(F, doc, s);
                 if (key > thr) {

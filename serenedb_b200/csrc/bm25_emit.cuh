@@ -10,8 +10,9 @@
 //           write the docs whose ordinal falls in the page, and stop once it is full.
 // Scored calls then run emit_score_kernel over the page: each hit is probed in every positive list of its query, in the
 // order the top-k sums them (ascending docs_count per segment), and the scores are added from 0 with __fadd_rn. Scored
-// phrase scans (sdbg_phrase_scan_batch, sdbg_phrase_and_scan_batch) run phrase_score_kernel instead: each hit's positive
-// clauses' scores summed as the phrase top-k sums them.
+// phrase scans (sdbg_phrase_scan_batch, sdbg_phrase_and_scan_batch, sdbg_phrase_groups_scan_batch) run
+// phrase_score_kernel instead: the scores of each hit's positive alternatives that occur in it, summed as the phrase top-k
+// sums them.
 #pragma once
 
 #include "bm25_kernels.cuh"
@@ -129,15 +130,15 @@ __global__ void __launch_bounds__(kEmitScoreThreads) emit_score_kernel(EmitScore
 
 struct PhraseScoreParams {
   const PostingsDev* segs;    // [segments]
-  const PhraseSink* sinks;    // [segments]: positions, that segment's slots and clause tables, clause_off and consts
+  const PhraseSink* sinks;    // [segments]: positions, that segment's slots and alternative tables, offsets, masks, consts
   uint32_t blocks_per_query;  // ceil(limit / kEmitScoreThreads)
   uint32_t limit;
   EmitHit* out;               // [queries][limit], n_out[q] hits each
   const uint32_t* n_out;
 };
 
-// Grid: queries x blocks_per_query, one thread per hit: phrase_clauses of the hit's doc over its segment's clause table,
-// scored as the phrase top-k scores it. At least 4 CTAs per SM (64 registers): no spill around the position walk.
+// Grid: queries x blocks_per_query, one thread per hit: phrase_clauses of the hit's doc over its segment's alternative
+// table, scored as the phrase top-k scores it (negated entries skipped, alternatives of frequency 0 add nothing). At least 4 CTAs per SM (64 registers): no spill around the position walk.
 __global__ void __launch_bounds__(kEmitScoreThreads, 4) phrase_score_kernel(PhraseScoreParams P) {
   const uint32_t q = blockIdx.x / P.blocks_per_query;
   const uint32_t i = (blockIdx.x % P.blocks_per_query) * kEmitScoreThreads + threadIdx.x;
@@ -147,7 +148,7 @@ __global__ void __launch_bounds__(kEmitScoreThreads, 4) phrase_score_kernel(Phra
   const PostingsDev& S = P.segs[h.seg];
   const PhraseSink& F = P.sinks[h.seg];
   float s;
-  phrase_clauses(S, F, phrase_query(F, q), d, PhraseMode::score_match, s);   // the hit matched: every clause holds
+  phrase_clauses<true>(S, F, phrase_query(F, q), d, PhraseMode::score_match, s);   // the hit matched: every group holds
   h.score = s;
 }
 

@@ -1,9 +1,11 @@
-// bm25_phrase.cuh -- exact phrase queries and conjunctions of phrase clauses (sdbg_phrase_*_batch,
-// sdbg_phrase_and_*_batch): the positions layout in HBM, the kernels that build it at staging, and the per-doc clause
-// check that bm25_count_kernel runs (kPhrase) on the docs that survive the conjunction of the positive clauses' terms,
-// the deleted docs, the filter chain and the exclusions: in its own sink (count, top-k), as a stage that narrows the
-// window before the facet, aggregate and match-scan sinks, or inside the sorted scan's sink once a doc's key has passed
-// the threshold. A single phrase is a query of one positive clause.
+// bm25_phrase.cuh -- exact phrase queries, conjunctions of phrase clauses and conjunctions of OR groups of phrases
+// (sdbg_phrase_*_batch, sdbg_phrase_and_*_batch, sdbg_phrase_groups_*_batch): the positions layout in HBM, the kernels
+// that build it at staging, and the per-doc check of a query's alternatives that bm25_count_kernel runs (kPhrase) on the
+// docs that survive its candidate scan (the AND, the flat OR or the OR groups of the alternatives' proxy terms), the
+// deleted docs, the filter chain and the exclusions: in its own sink (count, top-k), as a stage that narrows the window
+// before the facet, aggregate and match-scan sinks, or inside the sorted scan's sink once a doc's key has passed the
+// threshold. A single phrase is a query of one positive group of one alternative; a clause conjunction is a query of
+// groups of one alternative each.
 //
 // Positions layout (DESIGN.md §3): per posting block g a 64-bit base pos_base[g] into the u32 arena `pos` (one sentinel
 // behind the last block), and at pos[pos_base[g] ..] first the block's len exclusive prefix sums of its frequencies, then
@@ -26,11 +28,12 @@ struct PhraseSink {
   const unsigned long long* pos_base = nullptr;   // per block + sentinel
   const uint32_t* pos = nullptr;
   const uint4* slots = nullptr;                   // this segment's slots: {first BlockDesc, blocks, rel_pos, 0}
-  // query q's clauses clauses[clause_off[q] .. clause_off[q + 1]) in this segment's cost order (ascending smallest
-  // docs_count of the clause's terms, ties in query order): {first slot, slots, negated, statistics index}
+  // query q's alternatives clauses[clause_off[q] .. clause_off[q + 1]) in this segment's cost order (ascending smallest
+  // docs_count of the alternative's terms, ties in query order, flattened group by group): {first slot, slots, flags
+  // (kAlt*), statistics index}
   const uint4* clauses = nullptr;
   const uint32_t* clause_off = nullptr;
-  const float4* consts = nullptr;                 // per statistics index {c0, norm_const, norm_length, 0} of a positive clause
+  const float4* consts = nullptr;                 // per statistics index {c0, norm_const, norm_length, 0} of a positive alternative
   uint32_t ordinal_base = 0;                      // docs of the earlier segments: key = score bits << 32 | ~(base + doc)
   uint32_t k = 0, cap = 0;                        // cap: buffer slots, a power of two >= 2k (0: count only)
   unsigned long long* thr = nullptr;              // per query: the best known k-th key, seeded with the threshold
@@ -85,8 +88,12 @@ __device__ __forceinline__ uint32_t phrase_freq(const PostingsDev& S, const Phra
   return freq;
 }
 
-// Query q's clause range and its first clause, read once per window outside the per-doc loops: a single phrase (one
-// clause) then reads no clause table per doc.
+// The flags of an alternative table entry: negated; its group (bits 1..4) of the query; the candidate scan guarantees its
+// group (check mode need not look); the last positive entry of its group in table order.
+constexpr uint32_t kAltNegated = 1u, kAltGuaranteed = 1u << 5, kAltLast = 1u << 6;
+
+// Query q's alternative range and its first alternative, read once per window outside the per-doc loops: a single phrase
+// (one alternative) then reads no table per doc.
 struct PhraseQuery {
   uint32_t c0, c1;
   uint4 first;
@@ -100,30 +107,61 @@ __device__ __forceinline__ PhraseQuery phrase_query(const PhraseSink& F, uint32_
   return Q;
 }
 
-// How phrase_clauses treats doc d: check only (one-slot positive clauses skipped, since the conjunction of the positive
-// terms holds d already), check and score, or score a doc known to match (negated clauses skipped).
+// How phrase_clauses treats doc d: check only (entries of a group that the candidate scan guarantees or that an earlier
+// entry satisfied are skipped), check and score, or score a doc known to match (negated entries skipped).
 enum class PhraseMode { check, score, score_match };
 
-// The clause check of doc d for query Q, clause after clause in table order, dropping d at the first that fails: a
-// positive clause needs phrase frequency > 0, a negated one 0. Scoring modes: s = the sum of bm25(frequency, norm(d)) of
-// the positive clauses with their statistics, in table order from 0 (a one-slot clause's frequency is its term's
-// position count).
+// The check of doc d for query Q, entry after entry in table order. kAlts false, for the candidate AND (every positive
+// group one alternative, table flags only kAltNegated): a clause conjunction's walk, dropping d at the first entry that
+// fails (positive: frequency 0; negated: frequency > 0); check mode skips the one-slot positive entries, which the AND
+// holds. kAlts true, for the flat OR and OR-group candidates, with the mask `sat` of the positive groups satisfied so far:
+// a negated entry with phrase frequency > 0 drops d; a positive entry with frequency > 0 satisfies its group, and one
+// with frequency 0 that is the last of a group not yet satisfied drops d. Every positive group has a last entry, so a doc
+// that reaches the table's end has every positive group satisfied (or guaranteed): it matches, and no mask of the
+// query's groups needs to stay live. Scoring modes evaluate every positive entry: s = the sum of bm25(frequency,
+// norm(d)) of those with frequency > 0, with their statistics, in table order from 0 (a one-slot entry's frequency is its
+// term's position count). The kAlts walk scores a conjunction's table too, so phrase_score_kernel takes every shape.
+template <bool kAlts>
 __device__ __forceinline__ bool phrase_clauses(const PostingsDev& S, const PhraseSink& F, const PhraseQuery& Q, uint32_t d,
                                                PhraseMode mode, float& s) {
   s = 0.f;
-  uint4 cl = Q.first;
-  for (uint32_t c = Q.c0;;) {
-    const bool skip = cl.z ? mode == PhraseMode::score_match : mode == PhraseMode::check && cl.y == 1u;
-    if (!skip) {
-      const uint32_t f = phrase_freq(S, F, cl.x, cl.y, d);
-      if ((f != 0u) == (cl.z != 0u)) return false;
-      if (mode != PhraseMode::check && !cl.z) {
-        const float4 k = __ldg(F.consts + cl.w);
-        s = __fadd_rn(s, bm25(f, load_norm(S.norms, S.norm_width, d), k.x, k.y, k.z));
+  if constexpr (!kAlts) {
+    uint4 cl = Q.first;
+    for (uint32_t c = Q.c0;;) {
+      const bool skip = cl.z ? mode == PhraseMode::score_match : mode == PhraseMode::check && cl.y == 1u;
+      if (!skip) {
+        const uint32_t f = phrase_freq(S, F, cl.x, cl.y, d);
+        if ((f != 0u) == (cl.z != 0u)) return false;
+        if (mode != PhraseMode::check && !cl.z) {
+          const float4 k = __ldg(F.consts + cl.w);
+          s = __fadd_rn(s, bm25(f, load_norm(S.norms, S.norm_width, d), k.x, k.y, k.z));
+        }
       }
+      if (++c >= Q.c1) return true;
+      cl = __ldg(F.clauses + c);
     }
-    if (++c >= Q.c1) return true;
-    cl = __ldg(F.clauses + c);
+  } else {
+    uint4 cl = __ldg(F.clauses + Q.c0);   // Q.first is not kept live across the window: the candidate scan's state is
+    uint32_t sat = 0u;
+    for (uint32_t c = Q.c0;;) {
+      const bool neg = cl.z & kAltNegated;
+      const uint32_t g = 1u << ((cl.z >> 1) & 15u);
+      const bool skip = neg ? mode == PhraseMode::score_match
+                            : mode == PhraseMode::check && ((cl.z & kAltGuaranteed) || (sat & g));
+      if (!skip) {
+        const uint32_t f = phrase_freq(S, F, cl.x, cl.y, d);
+        if (f != 0u ? neg : (cl.z & kAltLast) && !(sat & g)) return false;
+        if (f != 0u) {
+          sat |= g;
+          if (mode != PhraseMode::check) {
+            const float4 k = __ldg(F.consts + cl.w);
+            s = __fadd_rn(s, bm25(f, load_norm(S.norms, S.norm_width, d), k.x, k.y, k.z));
+          }
+        }
+      }
+      if (++c >= Q.c1) return true;
+      cl = __ldg(F.clauses + c);
+    }
   }
 }
 

@@ -1420,6 +1420,17 @@ struct GroupSplit {
   }
 };
 
+// check_query_batch on every shape of a split batch of nq queries; sets S.whole.
+template <class Term>
+int check_shapes(sdbg_segment* const* segs, size_t n_segs, size_t nq, const sdbg_col_pred* filt, GroupSplit<Term>& S) {
+  for (int sh = 0; sh < 3; ++sh) {
+    if (S.qs[sh].empty()) continue;
+    if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &S.total_excl[sh])) return rc;
+    if (S.qs[sh].size() == nq) S.whole = sh;
+  }
+  return SDBG_OK;
+}
+
 // Splits a batch of sdbg_*_batch_groups(_min) by shape and checks it, every shape included, before anything is queued:
 // non-decreasing query_group_off / group_off / excl_off, 1..16 groups, 1..16 positive terms and at most 16 excluded ones
 // per query, no empty group, no positive term id twice in a query, 1 <= group_min[g] <= the group's size; then
@@ -1489,12 +1500,7 @@ int split_groups(sdbg_segment* const* segs, size_t n_segs, const Term* terms, co
       for (uint32_t i = excl_off[q]; i < excl_off[q + 1]; ++i) S.excl_terms[sh].push_back(excl_terms[i]);
     S.excl_off[sh].push_back(uint32_t(S.excl_terms[sh].size()));
   }
-  for (int sh = 0; sh < 3; ++sh) {
-    if (S.qs[sh].empty()) continue;
-    if (int rc = check_query_batch(segs, n_segs, S.view(sh), filt, &S.total_excl[sh])) return rc;
-    if (S.qs[sh].size() == nq) S.whole = sh;
-  }
-  return SDBG_OK;
+  return check_shapes(segs, n_segs, nq, filt, S);
 }
 
 // The queries of one call, checked before anything is queued (rc: the checks' result): a batch that runs whole (a flat
@@ -1515,6 +1521,12 @@ struct PassBatch {
             const uint32_t* group_min, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt)
       : nq(nq) {
     rc = split_groups(segs, n_segs, terms, group_off, query_group_off, group_min, nq, excl_terms, excl_off, filt, S);
+    if (S.whole >= 0) { whole = S.view(S.whole); total_excl = S.total_excl[S.whole]; }
+  }
+  // A batch its caller has split (S_: every query in one shape, no term twice in a query; PhraseBatch::candidates).
+  PassBatch(sdbg_segment* const* segs, size_t n_segs, GroupSplit<Term>&& S_, size_t nq, const sdbg_col_pred* filt)
+      : nq(nq), S(std::move(S_)) {
+    rc = check_shapes(segs, n_segs, nq, filt, S);
     if (S.whole >= 0) { whole = S.view(S.whole); total_excl = S.total_excl[S.whole]; }
   }
   PassBatch(const PassBatch&) = delete;   // whole may point into S
@@ -2347,31 +2359,44 @@ struct EmitJob {
   const unsigned long long* offset;   // host [nq]: the first ordinal of each query's page
 };
 
-// The phrase pass's part of a count_run call (the plan's batch is the AND of the distinct terms of each query's positive
-// clauses): query q's clauses are [query_off[q] .. query_off[q + 1]), clause j's slots slot_term / slot_rel
-// [clause_off[j] .. clause_off[j + 1]), negated when clause_neg[j] (clause_neg null: none). k == 0: count only; else the
-// top-k, scored with consts[j] = {c0, norm_const, norm_length} per clause and seeded with the key of threshold_in.
+// The phrase pass's part of a count_run call (the plan's batch is the candidate batch of PhraseBatch::candidates): batch
+// query b's alternatives are [query_off[b] .. query_off[b + 1]), alternative j's slots slot_term / slot_rel
+// [clause_off[j] .. clause_off[j + 1]), with flags[j] = kAltNegated | group << 1 | kAltGuaranteed (bm25_phrase.cuh).
+// The job's queries are the batch's at positions qpos (null: all of them), so a
+// shape of a mixed batch runs the job of its own queries. k == 0: count only; else the top-k, scored with consts[j] =
+// {c0, norm_const, norm_length} per alternative and seeded with the key of threshold_in.
 struct PhraseJob {
   const uint32_t* slot_term = nullptr;
   const uint32_t* slot_rel = nullptr;
   const uint32_t* clause_off = nullptr;
-  const uint8_t* clause_neg = nullptr;
+  const uint32_t* flags = nullptr;
   const uint32_t* query_off = nullptr;
-  size_t nq = 0;
+  const uint32_t* qpos = nullptr;
+  size_t nq = 0;        // the job's queries
+  uint32_t n_alts = 0;  // the batch's alternatives, query_off[its nq]
   std::vector<float4> consts;
   uint32_t k = 0;
   unsigned long long seed = 0;
 
-  uint32_t n_clauses() const { return query_off[nq]; }
-  uint32_t n_slots() const { return clause_off[n_clauses()]; }
+  uint32_t n_clauses() const { return n_alts; }
+  uint32_t n_slots() const { return clause_off[n_alts]; }
+  uint32_t batch_query(size_t q) const { return qpos ? qpos[q] : uint32_t(q); }
 
-  // The job's device tables, staged as [query clause offsets | per segment the clause tables | per segment the slots'
-  // lists | per clause consts], from a 16-B aligned offset.
+  // The job for the batch's queries at positions qs.
+  PhraseJob on(const std::vector<uint32_t>& qs) const {
+    PhraseJob J = *this;
+    J.qpos = qs.data();
+    J.nq = qs.size();
+    return J;
+  }
+
+  // The job's device tables, staged as [per query its table offsets | per segment the alternative tables | per segment
+  // the slots' lists | per alternative consts], from a 16-B aligned offset.
   size_t clauses_pos() const { return ((nq + 1) * 4 + 15) & ~size_t(15); }
   size_t lists_pos(size_t n_segs) const { return clauses_pos() + n_segs * n_clauses() * sizeof(uint4); }
   size_t consts_pos(size_t n_segs) const { return lists_pos(n_segs) + n_segs * n_slots() * sizeof(uint4); }
   size_t bytes(size_t n_segs) const { return consts_pos(n_segs) + (consts.empty() ? 0 : n_clauses() * sizeof(float4)); }
-  void write(sdbg_segment* const* segs, size_t n_segs, char* h) const;
+  void write(sdbg_segment* const* segs, size_t n_segs, char* h, bool conj) const;
 
   // Segment si's view of the tables staged at d for the kernels' PhraseSink.
   void sink(sdbg_segment* const* segs, size_t n_segs, size_t si, const char* d, PhraseSink& F) const {
@@ -2400,6 +2425,7 @@ struct CountJob {
       case CountMode::facet: return {8, size_t(facet.span) * 8, 8};
       case CountMode::agg: return {8, size_t(agg.key.span) * sizeof(AggCell), sizeof(AggCell)};
       case CountMode::emit: return {8, size_t(emit.limit) * sizeof(EmitHit), 4};
+      case CountMode::phrase: return {8, size_t(phrase.k) * 8, phrase.k ? 4u : 0u};
       default: return {8, 0, 0};
     }
   }
@@ -2482,7 +2508,8 @@ struct CountPlan {
 
   // The bm25_count_kernel instantiation of this plan's launches in `mode`, with its dynamic shared memory: the mode's
   // own bytes (facet bins, sorted keys, aggregate cells; none for a count), then the counter planes. phrased: the plan's
-  // batch is the AND of phrases' terms, checked by the phrase sink (CountMode::phrase) or before / in another sink.
+  // batch is the candidates of phrase alternatives, checked by the phrase sink (CountMode::phrase) or before / in another
+  // sink.
   std::pair<CountKernel, size_t> kernel(CountMode mode, size_t mode_bytes, bool phrased = false) const {
     static const CountKernel kernels[3][5] = {   // [OR | AND | OR groups][count | sort | facet | agg | emit]
         {bm25_count_kernel<false>, bm25_count_kernel<false, false, true>, bm25_count_kernel<false, false, false, true>,
@@ -2491,13 +2518,20 @@ struct CountPlan {
          bm25_count_kernel<true, false, false, false, true>, bm25_count_kernel<true, false, false, false, false, true>},
         {bm25_count_kernel<false, true>, bm25_count_kernel<false, true, true>, bm25_count_kernel<false, true, false, true>,
          bm25_count_kernel<false, true, false, false, true>, bm25_count_kernel<false, true, false, false, false, true>}};
-    static const CountKernel phrase_kernels[5] = {   // [phrase sink | sort | facet | agg | emit] of a phrase's conjunction
-        bm25_count_kernel<true, false, false, false, false, false, true>, bm25_count_kernel<true, false, true, false, false, false, true>,
-        bm25_count_kernel<true, false, false, true, false, false, true>, bm25_count_kernel<true, false, false, false, true, false, true>,
-        bm25_count_kernel<true, false, false, false, false, true, true>};
-    if (mode == CountMode::phrase) return {phrase_kernels[0], mode_bytes};
-    if (phrased) return {phrase_kernels[int(mode)], mode_bytes};
+    // [OR | AND | OR groups][phrase sink | sort | facet | agg | emit] of phrase alternatives' candidates
+    static const CountKernel phrase_kernels[3][5] = {
+        {bm25_count_kernel<false, false, false, false, false, false, true>, bm25_count_kernel<false, false, true, false, false, false, true>,
+         bm25_count_kernel<false, false, false, true, false, false, true>, bm25_count_kernel<false, false, false, false, true, false, true>,
+         bm25_count_kernel<false, false, false, false, false, true, true>},
+        {bm25_count_kernel<true, false, false, false, false, false, true>, bm25_count_kernel<true, false, true, false, false, false, true>,
+         bm25_count_kernel<true, false, false, true, false, false, true>, bm25_count_kernel<true, false, false, false, true, false, true>,
+         bm25_count_kernel<true, false, false, false, false, true, true>},
+        {bm25_count_kernel<false, true, false, false, false, false, true>, bm25_count_kernel<false, true, true, false, false, false, true>,
+         bm25_count_kernel<false, true, false, true, false, false, true>, bm25_count_kernel<false, true, false, false, true, false, true>,
+         bm25_count_kernel<false, true, false, false, false, true, true>}};
     const int shape = Q.term_grp ? 2 : Q.kind == SDBG_QUERY_AND ? 1 : 0;
+    if (mode == CountMode::phrase) return {phrase_kernels[shape][0], mode_bytes};
+    if (phrased) return {phrase_kernels[shape][int(mode)], mode_bytes};   // candidate groups need 1 list: no counter planes
     return {kernels[shape][int(mode)], mode_bytes + size_t(planes) * kCountWords * 4u};
   }
 };
@@ -2660,14 +2694,22 @@ void item_slots(const CountPlan& pl, char* h, size_t slot_off_pos, size_t slots_
   for (uint32_t i = 0; i < total; ++i) h_slots[fillq[hw[i].x]++] = i;
 }
 
-// The tables of PhraseJob::bytes at h. Per segment: each slot's list {first BlockDesc, blocks, rel_pos, 0}, and each
-// query's clauses {first slot, slots, negated, clause index} in that segment's cost order, the smallest docs_count of the
-// clause's terms (a term the segment does not hold costs 0), ascending, ties in query order: the order of a conjunction of
-// the terms' lists (conjunction.hpp:185-195), in which the scores of the positive clauses are summed. Slots and clauses
-// before the first query's are left as they are.
-void PhraseJob::write(sdbg_segment* const* segs, size_t n_segs, char* h) const {
+// The tables of PhraseJob::bytes at h. Per query of the job its table offsets. Per segment: each
+// slot's list {first BlockDesc, blocks, rel_pos, 0}, and each query's alternatives {first slot, slots, flags, alternative
+// index} in that segment's cost order, the smallest docs_count of the alternative's terms (a term the segment does not
+// hold costs 0), ascending, ties in query order: the order of a conjunction of the terms' lists
+// (conjunction.hpp:185-195), in which the scores of the matching positive alternatives are summed; the last positive
+// entry of each group gets kAltLast. conj: the job's candidates are the AND (every positive group one alternative), whose
+// walk (phrase_clauses<false>) reads the flags as the negated bit alone. Slots before the batch's first query's are left
+// as they are.
+void PhraseJob::write(sdbg_segment* const* segs, size_t n_segs, char* h, bool conj) const {
   const uint32_t nc = n_clauses(), ns = n_slots(), c0 = query_off[0];
-  std::memcpy(h, query_off, (nq + 1) * 4);
+  auto* off = reinterpret_cast<uint32_t*>(h);
+  off[0] = 0;
+  for (size_t q = 0; q < nq; ++q) {
+    const uint32_t b = batch_query(q);
+    off[q + 1] = off[q] + (query_off[b + 1] - query_off[b]);
+  }
   auto* lists = reinterpret_cast<uint4*>(h + lists_pos(n_segs));
   auto* tables = reinterpret_cast<uint4*>(h + clauses_pos());
   std::vector<uint32_t> cost(nc);
@@ -2685,9 +2727,20 @@ void PhraseJob::write(sdbg_segment* const* segs, size_t n_segs, char* h) const {
     }
     uint4* T = tables + si * nc;
     for (size_t q = 0; q < nq; ++q) {
-      for (uint32_t j = query_off[q]; j < query_off[q + 1]; ++j)
-        T[j] = make_uint4(clause_off[j], clause_off[j + 1] - clause_off[j], clause_neg && clause_neg[j] ? 1u : 0u, j);
-      std::stable_sort(T + query_off[q], T + query_off[q + 1], [&](const uint4& x, const uint4& y) { return cost[x.w] < cost[y.w]; });
+      const uint32_t b = batch_query(q);
+      uint4* E = T + off[q];
+      const uint32_t n = off[q + 1] - off[q];
+      for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t j = query_off[b] + i;
+        E[i] = make_uint4(clause_off[j], clause_off[j + 1] - clause_off[j], conj ? flags[j] & kAltNegated : flags[j], j);
+      }
+      std::stable_sort(E, E + n, [&](const uint4& x, const uint4& y) { return cost[x.w] < cost[y.w]; });
+      if (conj) continue;
+      uint32_t seen = 0;
+      for (uint32_t i = n; i-- > 0;) {
+        const uint32_t g = 1u << ((E[i].z >> 1) & 15u);
+        if (!(E[i].z & kAltNegated) && !(seen & g)) { E[i].z |= kAltLast; seen |= g; }
+      }
     }
   }
   if (!consts.empty()) std::memcpy(h + consts_pos(n_segs), consts.data(), nc * sizeof(float4));
@@ -2712,7 +2765,7 @@ int phrase_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, co
   char* h = staging.data();
   pl.write(h);
   item_slots(pl, h, slot_off_pos, slots_pos);
-  job.write(segs, n_segs, h + tables_pos);
+  job.write(segs, n_segs, h + tables_pos, pl.Q.kind == SDBG_QUERY_AND);
   // device scratch: [item keys [items][k] | item key counts | thresholds [nq]]
   const size_t keys_n_pos = total * size_t(k) * 8;
   const size_t thr_pos = (keys_n_pos + total * 4 + 15) & ~size_t(15);
@@ -2795,7 +2848,7 @@ int count_run(sdbg_segment* const* segs, size_t n_segs, const CountPlan& pl, con
   pl.write(h);
   if (sort || emit) item_slots(pl, h, slot_off_pos, slots_pos);
   if (emit) std::memcpy(h + segs_pos, job.emit.offset, nq * 8);
-  if (phrased) job.phrase.write(segs, n_segs, h + tables_pos);
+  if (phrased) job.phrase.write(segs, n_segs, h + tables_pos, pl.Q.kind == SDBG_QUERY_AND);
   if (sort) {
     auto* h_segs = reinterpret_cast<SortSegDev*>(h + segs_pos);
     for (size_t si = 0; si < n_segs; ++si) {
@@ -2912,7 +2965,11 @@ int pass_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>
   const GroupSplit<uint32_t>& S = B.S;
   return shapes_run(segs[0]->ctx, S, job.rows(out.rank >= 0), {out.counts, out.bins, out.nulls}, [&](int sh, void* const* part) {
     const CountOut o{part[0], part[1], part[2], out.oor, out.stats, out.rank};
-    return count_run(segs, n_segs, count_plan(segs, n_segs, S.view(sh), S.total_excl[sh], filt, job), filt, job, o);
+    if (!job.phrase.query_off)
+      return count_run(segs, n_segs, count_plan(segs, n_segs, S.view(sh), S.total_excl[sh], filt, job), filt, job, o);
+    CountJob js = job;   // the phrase tables of this shape's queries
+    js.phrase = job.phrase.on(S.qs[sh]);
+    return count_run(segs, n_segs, count_plan(segs, n_segs, S.view(sh), S.total_excl[sh], filt, js), filt, js, o);
   });
 }
 
@@ -3051,79 +3108,194 @@ extern "C" int sdbg_match_count_batch(sdbg_segment* const* segs, size_t n_segs, 
 }
 
 namespace {
-// A batch of clause conjunctions (sdbg_phrase_and_*_batch; a phrase of sdbg_phrase_*_batch is a query of one positive
-// clause, query_clause_off null), checked before anything is queued: query q's clauses are [qoff[q] .. qoff[q + 1]),
-// clause j's slots terms / rel_pos [clause_off[j] .. clause_off[j + 1]), negated when clause_neg[j]. `ids` / `id_off` hold
-// the distinct term ids of each query's positive clauses, in slot order, which run as the AND the clause check starts from.
+// The phrase entries' queries as their callers pass them. Query q is an AND of the groups [query_group_off[q] ..
+// query_group_off[q + 1]) (null: group q), group g an OR of the alternatives [group_off[g] .. group_off[g + 1]) (null:
+// alternative g), negated when group_neg[g] (null: none), alternative j the phrase of slots terms / rel_pos [clause_off[j]
+// .. clause_off[j + 1]) (rel_pos null: adjacent); excl_terms / excl_off as the flat entries take them.
+struct PhraseQueries {
+  const uint32_t* terms;
+  const uint32_t* rel_pos;
+  const uint32_t* clause_off;
+  const uint32_t* group_off;
+  const uint8_t* group_neg;
+  const uint32_t* query_group_off;
+  size_t nq;
+  const uint32_t* excl_terms;
+  const uint32_t* excl_off;
+};
+
+// A batch of phrase queries (PhraseQueries), checked before anything is queued, with its candidate batch S: per query
+// a superset of its matches that the existing candidate scans find, which the alternative check then narrows exactly.
+//   every positive group has one alternative: the AND of the distinct terms of the positive groups (shape 1);
+//   else, exactly one group kept: the flat OR of its proxies (shape 0); otherwise OR groups of proxies (shape 2).
+// A positive group of one alternative contributes each of its distinct terms as a one-list group. A group of several
+// alternatives contributes, per one-slot alternative, its term, and per phrase alternative one of its terms, the cheapest
+// by docs_count summed over the call's segments among those the query has not used yet (none when the group holds one of
+// its terms already). A term stays in one group of a query, so a group that cannot avoid a repeat is left out and only
+// checked per doc. The one-alternative groups are always kept, and so is the first group of several when there are
+// none, so the candidate batch always holds a group. A group is
+// guaranteed (kAltGuaranteed) when it is kept and all its alternatives are one slot.
+// Per alternative j: flags[j] (PhraseJob); per query: its alternatives [aoff[q] .. aoff[q + 1]).
 struct PhraseBatch {
   int rc = SDBG_OK;
-  std::vector<uint32_t> ids, id_off, rel, qoff;
-  const uint32_t* terms = nullptr;
-  const uint32_t* clause_off = nullptr;
-  const uint8_t* clause_neg = nullptr;
+  size_t nq;
+  std::vector<uint32_t> rel, qoff, goff, aoff, flags;
+  const uint32_t* terms;
+  const uint32_t* clause_off;
+  GroupSplit<uint32_t> S;
 
-  PhraseBatch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms_, const uint32_t* rel_pos, const uint32_t* clause_off_,
-              const uint8_t* clause_neg_, const uint32_t* query_clause_off, size_t nq)
-      : terms(terms_), clause_off(clause_off_), clause_neg(clause_neg_) {
+  PhraseBatch(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A)
+      : nq(A.nq), terms(A.terms), clause_off(A.clause_off) {
     if (!segs || !n_segs || !segs[0] || !nq || !clause_off) { rc = SDBG_EINVAL; return; }
     sdbg_ctx* c = segs[0]->ctx;
     qoff.resize(nq + 1);
-    for (size_t q = 0; q <= nq; ++q) qoff[q] = query_clause_off ? query_clause_off[q] : uint32_t(q);
+    for (size_t q = 0; q <= nq; ++q) qoff[q] = A.query_group_off ? A.query_group_off[q] : uint32_t(q);
     for (size_t q = 0; q < nq && !rc; ++q) {
-      if (qoff[q + 1] < qoff[q]) rc = fail(c, SDBG_EINVAL, "query_clause_off must be non-decreasing");
+      if (qoff[q + 1] < qoff[q]) rc = fail(c, SDBG_EINVAL, "query offsets must be non-decreasing");
       else if (qoff[q + 1] == qoff[q]) rc = fail(c, SDBG_EINVAL, "a query without a clause");
+      else if (qoff[q + 1] - qoff[q] > kMaxQueryTerms) rc = fail(c, SDBG_EUNSUPPORTED, "a query holds 1..16 groups");
     }
-    for (uint32_t j = qoff[0]; j < qoff[nq] && !rc; ++j) {
+    if (rc) return;
+    goff.assign(size_t(qoff[nq]) + 1, 0u);
+    for (uint32_t g = qoff[0]; g <= qoff[nq]; ++g) goff[g] = A.group_off ? A.group_off[g] : g;
+    for (uint32_t g = qoff[0]; g < qoff[nq] && !rc; ++g) {
+      if (goff[g + 1] < goff[g]) rc = fail(c, SDBG_EINVAL, "group_off must be non-decreasing");
+      else if (goff[g + 1] == goff[g]) rc = fail(c, SDBG_EINVAL, "empty OR group");
+    }
+    for (uint32_t j = goff[qoff[0]]; j < goff[qoff[nq]] && !rc; ++j) {
       if (clause_off[j + 1] < clause_off[j]) rc = fail(c, SDBG_EINVAL, "clause_off must be non-decreasing");
       else if (clause_off[j + 1] == clause_off[j]) rc = fail(c, SDBG_EINVAL, "empty clause");
     }
     for (size_t q = 0; q < nq && !rc; ++q) {
       bool pos = false;
-      for (uint32_t j = qoff[q]; j < qoff[q + 1]; ++j) pos |= !negated(j);
+      for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) pos |= !negated_group(A, g);
       if (!pos) rc = fail(c, SDBG_EINVAL, "a query without a positive clause");
     }
     for (size_t q = 0; q < nq && !rc; ++q)
-      if (clause_off[qoff[q + 1]] - clause_off[qoff[q]] > kMaxPhraseSlots) rc = fail(c, SDBG_EUNSUPPORTED, "a query holds 1..16 slots");
+      if (clause_off[goff[qoff[q + 1]]] - clause_off[goff[qoff[q]]] > kMaxPhraseSlots) rc = fail(c, SDBG_EUNSUPPORTED, "a query holds 1..16 slots");
     if (!rc && !terms) rc = fail(c, SDBG_EINVAL, "terms is NULL");
     if (rc) return;
-    id_off.assign(1, 0u);
-    rel.resize(clause_off[qoff[nq]]);
+    aoff.resize(nq + 1);
+    flags.assign(goff[qoff[nq]], 0u);
+    rel.resize(clause_off[goff[qoff[nq]]]);
+    for (size_t q = 0; q <= nq; ++q) aoff[q] = goff[qoff[q]];
     for (size_t q = 0; q < nq; ++q) {
-      for (uint32_t j = qoff[q]; j < qoff[q + 1]; ++j) {
-        const uint32_t s0 = clause_off[j], s1 = clause_off[j + 1];
-        for (uint32_t i = s0; i < s1; ++i) {
-          rel[i] = rel_pos ? rel_pos[i] : i - s0;
-          if (i == s0 ? rel[i] != 0u : rel[i] <= rel[i - 1]) {
-            rc = fail(c, SDBG_EINVAL, "rel_pos must start at 0 and increase");
-            return;
+      for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) {
+        const bool neg = negated_group(A, g);
+        for (uint32_t j = goff[g]; j < goff[g + 1]; ++j) {
+          flags[j] = (neg ? kAltNegated : 0u) | ((g - qoff[q]) << 1);
+          const uint32_t s0 = clause_off[j], s1 = clause_off[j + 1];
+          for (uint32_t i = s0; i < s1; ++i) {
+            rel[i] = A.rel_pos ? A.rel_pos[i] : i - s0;
+            if (i == s0 ? rel[i] != 0u : rel[i] <= rel[i - 1]) {
+              rc = fail(c, SDBG_EINVAL, "rel_pos must start at 0 and increase");
+              return;
+            }
+            if (!neg)
+              for (size_t si = 0; si < n_segs; ++si)
+                if (size_t(terms[i]) + 1 >= segs[si]->term_blk_begin.size()) {
+                  rc = fail(c, SDBG_EINVAL, "term id out of range");
+                  return;
+                }
           }
-          if (!negated(j) && std::find(ids.begin() + id_off.back(), ids.end(), terms[i]) == ids.end()) ids.push_back(terms[i]);
         }
       }
-      id_off.push_back(uint32_t(ids.size()));
+    }
+    if (A.excl_off)
+      for (size_t q = 0; q < nq && !rc; ++q) {
+        if (A.excl_off[q + 1] < A.excl_off[q]) rc = fail(c, SDBG_EINVAL, "excl_off must be non-decreasing");
+        else if (A.excl_off[q + 1] - A.excl_off[q] > kMaxQueryTerms) rc = fail(c, SDBG_EUNSUPPORTED, "a query excludes at most 16 terms");
+        else if (A.excl_off[q + 1] > A.excl_off[q] && !A.excl_terms) rc = fail(c, SDBG_EINVAL, "excl_terms is NULL");
+      }
+    if (!rc) candidates(segs, n_segs, A);
+  }
+
+  static bool negated_group(const PhraseQueries& A, uint32_t g) { return A.group_neg && A.group_neg[g]; }
+  uint32_t slots(uint32_t j) const { return clause_off[j + 1] - clause_off[j]; }
+
+  void candidates(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A) {
+    const auto docs = [&](uint32_t t) {
+      uint64_t n = 0;
+      for (size_t si = 0; si < n_segs; ++si) n += segs[si]->term_docs[t];
+      return n;
+    };
+    for (int sh = 0; sh < 3; ++sh) { S.term_off[sh].assign(1, 0u); S.excl_off[sh].assign(1, 0u); }
+    std::vector<std::vector<uint32_t>> groups;
+    std::vector<uint32_t> used;
+    const auto in = [](const std::vector<uint32_t>& v, uint32_t t) { return std::find(v.begin(), v.end(), t) != v.end(); };
+    for (size_t q = 0; q < nq; ++q) {
+      groups.clear();
+      used.clear();
+      bool single = true;
+      for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g)
+        if (!negated_group(A, g)) single &= goff[g + 1] - goff[g] == 1u;
+      for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) {
+        if (negated_group(A, g) || goff[g + 1] - goff[g] != 1u) continue;
+        const uint32_t j = goff[g];
+        for (uint32_t i = clause_off[j]; i < clause_off[j + 1]; ++i)
+          if (!in(used, terms[i])) { used.push_back(terms[i]); groups.push_back({terms[i]}); }
+        if (slots(j) == 1u) flags[j] |= kAltGuaranteed;
+      }
+      for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) {
+        if (negated_group(A, g) || goff[g + 1] - goff[g] == 1u) continue;
+        std::vector<uint32_t> G;
+        bool ok = true, terms_only = true;
+        for (uint32_t j = goff[g]; j < goff[g + 1] && ok; ++j) {
+          if (slots(j) != 1u) { terms_only = false; continue; }
+          const uint32_t t = terms[clause_off[j]];
+          if (in(G, t)) continue;
+          ok = !in(used, t);
+          G.push_back(t);
+        }
+        for (uint32_t j = goff[g]; j < goff[g + 1] && ok; ++j) {
+          if (slots(j) == 1u) continue;
+          bool covered = false;
+          uint32_t best = 0;
+          uint64_t best_docs = UINT64_MAX;
+          for (uint32_t i = clause_off[j]; i < clause_off[j + 1]; ++i) {
+            covered |= in(G, terms[i]);
+            if (in(used, terms[i])) continue;
+            const uint64_t n = docs(terms[i]);
+            if (n < best_docs) { best_docs = n; best = terms[i]; }
+          }
+          if (covered) continue;
+          ok = best_docs != UINT64_MAX;
+          G.push_back(best);
+        }
+        if (!ok) continue;
+        used.insert(used.end(), G.begin(), G.end());
+        groups.push_back(std::move(G));
+        if (terms_only)
+          for (uint32_t j = goff[g]; j < goff[g + 1]; ++j) flags[j] |= kAltGuaranteed;
+      }
+      const int sh = single ? 1 : groups.size() == 1 ? 0 : 2;
+      S.qs[sh].push_back(uint32_t(q));
+      for (size_t gi = 0; gi < groups.size(); ++gi)
+        for (uint32_t t : groups[gi]) {
+          S.terms[sh].push_back(t);
+          if (sh == 2) S.term_grp[sh].push_back(uint8_t(gi));
+        }
+      S.term_off[sh].push_back(uint32_t(S.terms[sh].size()));
+      if (A.excl_off)
+        for (uint32_t i = A.excl_off[q]; i < A.excl_off[q + 1]; ++i) S.excl_terms[sh].push_back(A.excl_terms[i]);
+      S.excl_off[sh].push_back(uint32_t(S.excl_terms[sh].size()));
     }
   }
 
-  bool negated(uint32_t j) const { return clause_neg && clause_neg[j]; }
-
-  QueryBatch<uint32_t> conj(size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off) const {
-    return {SDBG_QUERY_AND, ids.data(), id_off.data(), nq, excl_terms, excl_off, nullptr};
-  }
-
-  // The clauses of a count_run job over conj(): count only until k or consts are set.
+  // The alternatives of a count_run job over the candidate batch: count only until k or consts are set.
   PhraseJob job() const {
     PhraseJob J;
-    J.slot_term = terms; J.slot_rel = rel.data(); J.clause_off = clause_off; J.clause_neg = clause_neg;
-    J.query_off = qoff.data(); J.nq = qoff.size() - 1;
+    J.slot_term = terms; J.slot_rel = rel.data(); J.clause_off = clause_off; J.flags = flags.data();
+    J.query_off = aoff.data(); J.nq = nq; J.n_alts = aoff[nq];
     return J;
   }
 
-  // consts[j] = {c0, norm_const, norm_length, 0} of positive clause j's statistics clause_stats[j] (negated clauses: 0):
+  // consts[j] = {c0, norm_const, norm_length, 0} of positive alternative j's statistics clause_stats[j] (negated ones: 0):
   // the scorer form of fill_qterm, as the phrase top-k and the scored phrase scan score a match.
   std::vector<float4> consts(sdbg_segment* const* segs, const sdbg_bm25_term* clause_stats, float k1, float b) const {
-    std::vector<float4> out(qoff.back(), make_float4(0.f, 0.f, 0.f, 0.f));
-    for (uint32_t j = qoff[0]; j < qoff.back(); ++j) {
-      if (negated(j)) continue;
+    std::vector<float4> out(aoff[nq], make_float4(0.f, 0.f, 0.f, 0.f));
+    for (uint32_t j = aoff[0]; j < aoff[nq]; ++j) {
+      if (flags[j] & kAltNegated) continue;
       sdbg_bm25_term t = clause_stats[j];
       t.term = terms[clause_off[j]];
       QTermDev d;
@@ -3141,35 +3313,32 @@ int phrase_positions_staged(sdbg_segment* const* segs, size_t n_segs) {
   return SDBG_OK;
 }
 
-// The count, top-k, sorted scan, facet counts and aggregates of a batch of clause conjunctions (query_clause_off null:
-// one clause per query, the sdbg_phrase_* entries): PhraseBatch's checks, the AND of the positive clauses' terms, staged
-// positions, then the flat entry's pass with the clauses on its job.
-int phrase_count(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* clause_off,
-                 const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
-                 const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
+// The count, top-k, sorted scan, facet counts and aggregates of a batch of phrase queries (PhraseQueries): PhraseBatch's
+// checks, its candidate batch, staged positions, then the flat entry's pass with the alternatives on its job.
+int phrase_count(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A, const sdbg_col_pred* filt, uint64_t* counts) {
   if (!counts) return SDBG_EINVAL;
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
+  PhraseBatch PB(segs, n_segs, A);
   if (PB.rc) return PB.rc;
-  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  const PassBatch<uint32_t> B(segs, n_segs, std::move(PB.S), A.nq, filt);
   if (B.rc) return B.rc;
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
   CountJob job{CountMode::count, {}, {}, {}};
   job.mode = CountMode::phrase;
   job.phrase = PB.job();
-  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, 0), [&](const char* h) { std::memcpy(counts, h, nq * 8); });
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(A.nq, 0), [&](const char* h) { std::memcpy(counts, h, A.nq * 8); });
 }
 
-int phrase_topk(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* clause_off,
-                const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
-                const uint32_t* excl_off, const sdbg_bm25_term* clause_stats, float k1, float b, const sdbg_col_pred* filt, uint32_t k,
-                float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
+int phrase_topk(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A, const sdbg_bm25_term* clause_stats, float k1,
+                float b, const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
+                uint64_t* total_matches) {
   if (!out || !n_out || !clause_stats) return SDBG_EINVAL;
+  const size_t nq = A.nq;
   if (int rc = topk_args(segs, n_segs, nq, k)) return rc;
   sdbg_ctx* c = segs[0]->ctx;
   if (k > kSortMaxK) return fail(c, SDBG_EUNSUPPORTED, "k > 4096");
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
+  PhraseBatch PB(segs, n_segs, A);
   if (PB.rc) return PB.rc;
-  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  const PassBatch<uint32_t> B(segs, n_segs, std::move(PB.S), nq, filt);
   if (B.rc) return B.rc;
   uint64_t ord = 0;
   for (size_t si = 0; si < n_segs; ++si) ord += segs[si]->n_docs;
@@ -3188,60 +3357,61 @@ int phrase_topk(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
   if (int rc = ensure(c, c->pass[0], nq * (size_t(k) * 8 + 12))) return rc;
   const TopkDevOut dev = topk_region(c->pass[0].p, nq, k);
   CU(c, cudaMemsetAsync(c->pass[0].p, 0, nq * (size_t(k) * 8 + 12), c->stream));
-  const CountPlan pl = count_plan(segs, n_segs, B.whole, B.total_excl, filt, job);
   const CountOut o{dev.total, dev.keys, dev.n_out, nullptr, nullptr, -1};
-  if (int rc = count_run(segs, n_segs, pl, filt, job, o)) return rc;
+  if (int rc = pass_run(segs, n_segs, B, filt, job, o)) return rc;
   return topk_hits_to_host(segs, n_segs, dev, nq, k, out, n_out, total_matches);
 }
 
-int phrase_topk_by_column(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                          const uint32_t* clause_off, const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq,
-                          const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
-                          int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
+int phrase_topk_by_column(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A, const sdbg_col_pred* filt,
+                          uint64_t sort_field, int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
   if (!segs || !n_segs || !segs[0] || !k || !out || !n_out) return SDBG_EINVAL;
   if (k > kSortMaxK) return fail(segs[0]->ctx, SDBG_EUNSUPPORTED, "k > 4096");
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
+  PhraseBatch PB(segs, n_segs, A);
   if (PB.rc) return PB.rc;
-  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  const PassBatch<uint32_t> B(segs, n_segs, std::move(PB.S), A.nq, filt);
   if (B.rc) return B.rc;
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
   return sort_to_host(segs, n_segs, B, filt, sort_field, descending, nulls_first, k, out, n_out, PB.job());
 }
 
-int phrase_facet_counts(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                        const uint32_t* clause_off, const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq,
-                        const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+int phrase_facet_counts(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A, const sdbg_col_pred* filt, uint64_t key_field,
                         int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
   if (!counts || !null_counts) return SDBG_EINVAL;
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
+  PhraseBatch PB(segs, n_segs, A);
   if (PB.rc) return PB.rc;
-  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  const PassBatch<uint32_t> B(segs, n_segs, std::move(PB.S), A.nq, filt);
   if (B.rc) return B.rc;
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
   CountJob job{CountMode::facet, {}, {key_field, key_min, key_span, {}}, {}};
   job.phrase = PB.job();
-  return pass_to_host(segs, n_segs, B, filt, job, words_region(nq, key_span),
-                      [&](const char* h) { facet_fill(h, nq, key_span, counts, null_counts); });
+  return pass_to_host(segs, n_segs, B, filt, job, words_region(A.nq, key_span),
+                      [&](const char* h) { facet_fill(h, A.nq, key_span, counts, null_counts); });
 }
 
-int phrase_aggregate(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* clause_off,
-                     const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
-                     const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
-                     uint64_t value_field, sdbg_match_agg* out, sdbg_match_agg* null_out) {
+int phrase_aggregate(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A, const sdbg_col_pred* filt, uint64_t key_field,
+                     int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out, sdbg_match_agg* null_out) {
   if (!out || !null_out) return SDBG_EINVAL;
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
+  PhraseBatch PB(segs, n_segs, A);
   if (PB.rc) return PB.rc;
-  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  const PassBatch<uint32_t> B(segs, n_segs, std::move(PB.S), A.nq, filt);
   if (B.rc) return B.rc;
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
   return agg_to_host(segs, n_segs, B, filt, key_field, key_min, key_span, value_field, out, null_out, PB.job());
 }
 }  // namespace
 
+namespace {
+// The queries of the sdbg_phrase_* entries: each one positive group of one alternative.
+PhraseQueries phrase_one(const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* phrase_off, size_t nq,
+                         const uint32_t* excl_terms, const uint32_t* excl_off) {
+  return {terms, rel_pos, phrase_off, nullptr, nullptr, nullptr, nq, excl_terms, excl_off};
+}
+}  // namespace
+
 extern "C" int sdbg_phrase_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
                                        const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
                                        const sdbg_col_pred* filt, uint64_t* counts) {
-  return phrase_count(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, counts);
+  return phrase_count(segs, n_segs, phrase_one(terms, rel_pos, phrase_off, nq, excl_terms, excl_off), filt, counts);
 }
 
 extern "C" int sdbg_phrase_and_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3249,14 +3419,24 @@ extern "C" int sdbg_phrase_and_count_batch(sdbg_segment* const* segs, size_t n_s
                                            size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
                                            uint64_t* counts) {
   if (!query_clause_off) return SDBG_EINVAL;
-  return phrase_count(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt, counts);
+  return phrase_count(segs, n_segs, {terms, rel_pos, clause_off, nullptr, clause_negated, query_clause_off, nq, excl_terms, excl_off},
+                      filt, counts);
+}
+
+extern "C" int sdbg_phrase_groups_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                              const uint32_t* clause_off, const uint32_t* group_off, const uint8_t* group_negated,
+                                              const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
+                                              const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
+  if (!group_off || !query_group_off) return SDBG_EINVAL;
+  return phrase_count(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off},
+                      filt, counts);
 }
 
 extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
                                       const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms, const uint32_t* excl_off,
                                       const sdbg_bm25_term* phrase_stats, float k1, float b, const sdbg_col_pred* filt, uint32_t k,
                                       float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
-  return phrase_topk(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, phrase_stats, k1, b, filt, k,
+  return phrase_topk(segs, n_segs, phrase_one(terms, rel_pos, phrase_off, nq, excl_terms, excl_off), phrase_stats, k1, b, filt, k,
                      threshold_in, out, n_out, total_matches);
 }
 
@@ -3266,15 +3446,26 @@ extern "C" int sdbg_phrase_and_topk_batch(sdbg_segment* const* segs, size_t n_se
                                           const sdbg_bm25_term* clause_stats, float k1, float b, const sdbg_col_pred* filt, uint32_t k,
                                           float threshold_in, sdbg_hit* out, uint32_t* n_out, uint64_t* total_matches) {
   if (!query_clause_off) return SDBG_EINVAL;
-  return phrase_topk(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, clause_stats,
-                     k1, b, filt, k, threshold_in, out, n_out, total_matches);
+  return phrase_topk(segs, n_segs, {terms, rel_pos, clause_off, nullptr, clause_negated, query_clause_off, nq, excl_terms, excl_off},
+                     clause_stats, k1, b, filt, k, threshold_in, out, n_out, total_matches);
+}
+
+extern "C" int sdbg_phrase_groups_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                             const uint32_t* clause_off, const uint32_t* group_off, const uint8_t* group_negated,
+                                             const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
+                                             const uint32_t* excl_off, const sdbg_bm25_term* clause_stats, float k1, float b,
+                                             const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
+                                             uint64_t* total_matches) {
+  if (!group_off || !query_group_off) return SDBG_EINVAL;
+  return phrase_topk(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off},
+                     clause_stats, k1, b, filt, k, threshold_in, out, n_out, total_matches);
 }
 
 extern "C" int sdbg_phrase_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
                                                 const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms,
                                                 const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
                                                 int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
-  return phrase_topk_by_column(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, sort_field,
+  return phrase_topk_by_column(segs, n_segs, phrase_one(terms, rel_pos, phrase_off, nq, excl_terms, excl_off), filt, sort_field,
                                descending, nulls_first, k, out, n_out);
 }
 
@@ -3284,16 +3475,27 @@ extern "C" int sdbg_phrase_and_topk_by_column_batch(sdbg_segment* const* segs, s
                                                     const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
                                                     int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
   if (!query_clause_off) return SDBG_EINVAL;
-  return phrase_topk_by_column(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt,
-                               sort_field, descending, nulls_first, k, out, n_out);
+  return phrase_topk_by_column(segs, n_segs, {terms, rel_pos, clause_off, nullptr, clause_negated, query_clause_off, nq, excl_terms,
+                                              excl_off}, filt, sort_field, descending, nulls_first, k, out, n_out);
+}
+
+extern "C" int sdbg_phrase_groups_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                       const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                                       const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
+                                                       const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                                       uint64_t sort_field, int descending, int nulls_first, uint32_t k,
+                                                       sdbg_sort_hit* out, uint32_t* n_out) {
+  if (!group_off || !query_group_off) return SDBG_EINVAL;
+  return phrase_topk_by_column(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms,
+                                              excl_off}, filt, sort_field, descending, nulls_first, k, out, n_out);
 }
 
 extern "C" int sdbg_phrase_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
                                               const uint32_t* phrase_off, size_t nq, const uint32_t* excl_terms,
                                               const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
                                               int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
-  return phrase_facet_counts(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, key_field,
-                             key_min, key_span, counts, null_counts);
+  return phrase_facet_counts(segs, n_segs, phrase_one(terms, rel_pos, phrase_off, nq, excl_terms, excl_off), filt, key_field, key_min,
+                             key_span, counts, null_counts);
 }
 
 extern "C" int sdbg_phrase_and_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3302,8 +3504,19 @@ extern "C" int sdbg_phrase_and_facet_counts_batch(sdbg_segment* const* segs, siz
                                                   const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
                                                   int64_t key_min, uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
   if (!query_clause_off) return SDBG_EINVAL;
-  return phrase_facet_counts(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt,
-                             key_field, key_min, key_span, counts, null_counts);
+  return phrase_facet_counts(segs, n_segs, {terms, rel_pos, clause_off, nullptr, clause_negated, query_clause_off, nq, excl_terms,
+                                            excl_off}, filt, key_field, key_min, key_span, counts, null_counts);
+}
+
+extern "C" int sdbg_phrase_groups_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                     const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                                     const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
+                                                     const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                                     uint64_t key_field, int64_t key_min, uint32_t key_span, uint64_t* counts,
+                                                     uint64_t* null_counts) {
+  if (!group_off || !query_group_off) return SDBG_EINVAL;
+  return phrase_facet_counts(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms,
+                                            excl_off}, filt, key_field, key_min, key_span, counts, null_counts);
 }
 
 extern "C" int sdbg_phrase_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3311,7 +3524,7 @@ extern "C" int sdbg_phrase_aggregate_batch(sdbg_segment* const* segs, size_t n_s
                                            const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
                                            int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
                                            sdbg_match_agg* null_out) {
-  return phrase_aggregate(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, key_field, key_min,
+  return phrase_aggregate(segs, n_segs, phrase_one(terms, rel_pos, phrase_off, nq, excl_terms, excl_off), filt, key_field, key_min,
                           key_span, value_field, out, null_out);
 }
 
@@ -3322,8 +3535,19 @@ extern "C" int sdbg_phrase_and_aggregate_batch(sdbg_segment* const* segs, size_t
                                                int64_t key_min, uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
                                                sdbg_match_agg* null_out) {
   if (!query_clause_off) return SDBG_EINVAL;
-  return phrase_aggregate(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt,
-                          key_field, key_min, key_span, value_field, out, null_out);
+  return phrase_aggregate(segs, n_segs, {terms, rel_pos, clause_off, nullptr, clause_negated, query_clause_off, nq, excl_terms, excl_off},
+                          filt, key_field, key_min, key_span, value_field, out, null_out);
+}
+
+extern "C" int sdbg_phrase_groups_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                  const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                                  const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
+                                                  const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                                  uint64_t key_field, int64_t key_min, uint32_t key_span, uint64_t value_field,
+                                                  sdbg_match_agg* out, sdbg_match_agg* null_out) {
+  if (!group_off || !query_group_off) return SDBG_EINVAL;
+  return phrase_aggregate(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off},
+                          filt, key_field, key_min, key_span, value_field, out, null_out);
 }
 
 extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -3509,18 +3733,20 @@ int scan_batch_to_host(sdbg_segment* const* segs, size_t n_segs, const PassBatch
   }, out, n_out, total);
 }
 
-// Queues the match scan of a checked phrase batch (B: the AND of the phrases' terms) into out, zeroed: the emit pass with
-// the phrase slots, then, when scored (J.consts set), phrase_score_kernel over the pages.
+// Queues the match scan of one shape Q of a checked phrase batch (total_excl as check_query_batch set it; J: the job of
+// its queries) into out, zeroed: the emit pass with the alternatives, then, when scored (J.consts set),
+// phrase_score_kernel over the pages. qpos: the call's position of each query (NULL: the same), which picks its offset.
 // The scorer's staging: [PostingsDev [n_segs] | PhraseSink [n_segs] | the job's tables (PhraseJob::bytes)].
-int phrase_scan_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<uint32_t>& B, const sdbg_col_pred* filt,
-                    const PhraseJob& J, const uint64_t* offset, uint32_t limit, const CountOut& out) {
+int phrase_scan_run(sdbg_segment* const* segs, size_t n_segs, const QueryBatch<uint32_t>& Q, uint32_t total_excl, const uint32_t* qpos,
+                    const sdbg_col_pred* filt, const PhraseJob& J, const uint64_t* offset, uint32_t limit, const CountOut& out) {
   sdbg_ctx* c = segs[0]->ctx;
-  const size_t nq = B.nq;
+  const size_t nq = Q.nq;
   std::vector<unsigned long long> offs(nq, 0ull);
-  if (offset) std::copy(offset, offset + nq, offs.begin());
+  if (offset)
+    for (size_t q = 0; q < nq; ++q) offs[q] = offset[qpos ? qpos[q] : q];
   CountJob job{CountMode::emit, {}, {}, {}, {limit, offs.data()}};
   job.phrase = J;
-  if (int rc = count_run(segs, n_segs, count_plan(segs, n_segs, B.whole, B.total_excl, filt, job), filt, job, out)) return rc;
+  if (int rc = count_run(segs, n_segs, count_plan(segs, n_segs, Q, total_excl, filt, job), filt, job, out)) return rc;
   if (J.consts.empty()) return SDBG_OK;
   const size_t sinks_pos = (n_segs * sizeof(PostingsDev) + 15) & ~size_t(15);
   const size_t tables_pos = (sinks_pos + n_segs * sizeof(PhraseSink) + 15) & ~size_t(15);
@@ -3535,7 +3761,7 @@ int phrase_scan_run(sdbg_segment* const* segs, size_t n_segs, const PassBatch<ui
     J.sink(segs, n_segs, si, d + tables_pos, F);
     std::memcpy(h.data() + sinks_pos + si * sizeof(PhraseSink), &F, sizeof(F));
   }
-  J.write(segs, n_segs, h.data() + tables_pos);
+  J.write(segs, n_segs, h.data() + tables_pos, Q.kind == SDBG_QUERY_AND);
   CU(c, cudaMemcpyAsync(b_sc.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));   // pageable: consumed on return
   PhraseScoreParams P;
   P.segs = reinterpret_cast<const PostingsDev*>(d);
@@ -3568,17 +3794,17 @@ extern "C" int sdbg_match_scan_batch_groups_min(sdbg_segment* const* segs, size_
 }
 
 namespace {
-int phrase_scan(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos, const uint32_t* clause_off,
-                const uint8_t* clause_negated, const uint32_t* query_clause_off, size_t nq, const uint32_t* excl_terms,
-                const uint32_t* excl_off, const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats, float k1, float b,
-                const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
+int phrase_scan(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A, const sdbg_col_pred* filt,
+                const sdbg_bm25_term* clause_stats, float k1, float b, const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out,
+                uint32_t* n_out, uint64_t* total) {
   if (!limit || !out || !n_out || !total || (scored && !clause_stats)) return SDBG_EINVAL;
-  const PhraseBatch PB(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq);
+  const size_t nq = A.nq;
+  PhraseBatch PB(segs, n_segs, A);
   if (PB.rc) return PB.rc;
   sdbg_ctx* c = segs[0]->ctx;
   if (scored)
     if (int rc = topk_limits(c, nq, 1)) return rc;
-  const PassBatch<uint32_t> B(segs, n_segs, PB.conj(nq, excl_terms, excl_off), filt);
+  const PassBatch<uint32_t> B(segs, n_segs, std::move(PB.S), nq, filt);
   if (B.rc) return B.rc;
   if (scored) {
     uint64_t ord = 0;
@@ -3588,8 +3814,14 @@ int phrase_scan(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
   if (int rc = phrase_positions_staged(segs, n_segs)) return rc;
   PhraseJob J = PB.job();
   if (scored) J.consts = PB.consts(segs, clause_stats, k1, b);
-  return scan_to_host(c, nq, limit, [&](const CountOut& o) { return phrase_scan_run(segs, n_segs, B, filt, J, offset, limit, o); },
-                      out, n_out, total);
+  return scan_to_host(c, nq, limit, [&](const CountOut& o) {
+    if (B.whole.nq) return phrase_scan_run(segs, n_segs, B.whole, B.total_excl, nullptr, filt, J, offset, limit, o);
+    const CountJob job{CountMode::emit, {}, {}, {}, {limit, nullptr}};
+    return shapes_run(c, B.S, job.rows(false), {o.counts, o.bins, o.nulls}, [&](int sh, void* const* part) {
+      return phrase_scan_run(segs, n_segs, B.S.view(sh), B.S.total_excl[sh], B.S.qs[sh].data(), filt, J.on(B.S.qs[sh]), offset, limit,
+                             CountOut{part[0], part[1], part[2], nullptr, nullptr, -1});
+    });
+  }, out, n_out, total);
 }
 }  // namespace
 
@@ -3598,8 +3830,8 @@ extern "C" int sdbg_phrase_scan_batch(sdbg_segment* const* segs, size_t n_segs, 
                                       const sdbg_col_pred* filt, const sdbg_bm25_term* phrase_stats, float k1, float b,
                                       const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out,
                                       uint64_t* total) {
-  return phrase_scan(segs, n_segs, terms, rel_pos, phrase_off, nullptr, nullptr, nq, excl_terms, excl_off, filt, phrase_stats, k1, b,
-                     offset, limit, scored, out, n_out, total);
+  return phrase_scan(segs, n_segs, phrase_one(terms, rel_pos, phrase_off, nq, excl_terms, excl_off), filt, phrase_stats, k1, b, offset,
+                     limit, scored, out, n_out, total);
 }
 
 extern "C" int sdbg_phrase_and_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3608,8 +3840,19 @@ extern "C" int sdbg_phrase_and_scan_batch(sdbg_segment* const* segs, size_t n_se
                                           const sdbg_bm25_term* clause_stats, float k1, float b, const uint64_t* offset,
                                           uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
   if (!query_clause_off) return SDBG_EINVAL;
-  return phrase_scan(segs, n_segs, terms, rel_pos, clause_off, clause_negated, query_clause_off, nq, excl_terms, excl_off, filt,
-                     clause_stats, k1, b, offset, limit, scored, out, n_out, total);
+  return phrase_scan(segs, n_segs, {terms, rel_pos, clause_off, nullptr, clause_negated, query_clause_off, nq, excl_terms, excl_off},
+                     filt, clause_stats, k1, b, offset, limit, scored, out, n_out, total);
+}
+
+extern "C" int sdbg_phrase_groups_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
+                                             const uint32_t* clause_off, const uint32_t* group_off, const uint8_t* group_negated,
+                                             const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
+                                             const uint32_t* excl_off, const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats,
+                                             float k1, float b, const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out,
+                                             uint32_t* n_out, uint64_t* total) {
+  if (!group_off || !query_group_off) return SDBG_EINVAL;
+  return phrase_scan(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off},
+                     filt, clause_stats, k1, b, offset, limit, scored, out, n_out, total);
 }
 
 // ---- the count, facet, aggregate and sorted passes across GPUs ----

@@ -922,6 +922,199 @@ def ExecutePhraseAndMatchScan(reader, query, scorer=None, limit=1 << 20, offset=
                                           _one(exclude_phrases), boost)[0]
 
 
+def _phrase_groups(queries, exclude_phrases):
+    """Per query its groups as [([(terms, rel_pos or None)], negated)]: the OR groups of queries[q], each a non-empty list
+    of alternatives in the forms _clause takes, then one negated group per alternative of exclude_phrases[q]."""
+    if exclude_phrases is not None and len(exclude_phrases) != len(queries):
+        raise ValueError("exclude_phrases needs one list (or None) per query")
+    out = []
+    for q, query in enumerate(queries):
+        groups = []
+        for g in query:
+            if isinstance(g, (int, np.integer)) or len(g) == 0:
+                raise ValueError("a group is a non-empty list of alternatives")
+            groups.append(([_clause(a) for a in g], False))
+        neg = exclude_phrases[q] if exclude_phrases is not None and exclude_phrases[q] is not None else []
+        groups += [([_clause(c)], True) for c in neg]
+        if not groups:
+            raise ValueError("a query needs a group")
+        if any(len(ts) == 0 for alts, _ in groups for ts, _ in alts):
+            raise ValueError("an alternative needs a term")
+        out.append(groups)
+    return out
+
+
+def _phrase_groups_args(groups, exclude):
+    """(terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off) of the OR-group
+    entries, and the arrays they point into (kept alive by the caller)."""
+    nq = len(groups)
+    flat_g = [g for q in groups for g in q]
+    flat = [a for alts, _ in flat_g for a in alts]
+    terms = np.ascontiguousarray([t for ts, _ in flat for t in ts], dtype=np.uint32)
+    rel = np.ascontiguousarray([r for ts, rp in flat for r in (range(len(ts)) if rp is None else rp)], dtype=np.uint32)
+    coff = np.zeros(len(flat) + 1, np.uint32)
+    coff[1:] = np.cumsum([len(ts) for ts, _ in flat])
+    goff = np.zeros(len(flat_g) + 1, np.uint32)
+    goff[1:] = np.cumsum([len(alts) for alts, _ in flat_g])
+    neg = np.ascontiguousarray([1 if n else 0 for _, n in flat_g], dtype=np.uint8)
+    qoff = np.zeros(nq + 1, np.uint32)
+    qoff[1:] = np.cumsum([len(q) for q in groups])
+    x = _exclusions(exclude, nq) or (None, None)
+    keep = (terms, rel, coff, goff, neg, qoff, x)
+    return (_ptr(terms), _ptr(rel), _ptr(coff), _ptr(goff), _ptr(neg), _ptr(qoff), nq, _ptr(x[0]), _ptr(x[1])), keep
+
+
+def _alternative_stats(reader, groups, scorer, boost):
+    """One BM25Term per alternative: reader.phrase_stats of each positive alternative, zeros for the negated ones."""
+    flat = [(ts, n) for q in groups for alts, n in q for ts, _ in alts]
+    return (N.BM25Term * max(len(flat), 1))(*[N.BM25Term() if n else reader.phrase_stats(scorer, ts, boost) for ts, n in flat])
+
+
+def ExecutePhraseGroupsCountBatch(reader, queries, filt=None, exclude=None, exclude_phrases=None):
+    """Count of conjunctions of OR groups of phrases and terms (`("new york" | nyc) & pizza & !"deep dish"`,
+    sdbg_phrase_groups_count_batch). queries: per query its groups, each a list of alternatives; an alternative is a list
+    of term ids (a phrase of adjacent words; one id: a plain term) or a pair (term ids, rel_pos). exclude_phrases: per
+    query negated alternatives in the same form (or None), each excluded on its own; exclude: per query excluded term ids,
+    as in ExecutePhraseCountBatch. A doc matches when every group has an alternative that occurs in it and no negated
+    alternative does. Returns uint64[Q]."""
+    groups = _phrase_groups(queries, exclude_phrases)
+    args, keep = _phrase_groups_args(groups, exclude)
+    counts = np.zeros(len(queries), np.uint64)
+    N.check(N.lib().sdbg_phrase_groups_count_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), _ptr(counts)),
+            reader.segments[0].ctx._h)
+    return counts
+
+
+def ExecutePhraseGroupsCount(reader, query, filt=None, exclude=None, exclude_phrases=None):
+    """ExecutePhraseGroupsCountBatch for one query: its match count as an int."""
+    return int(ExecutePhraseGroupsCountBatch(reader, [list(query)], filt, _one(exclude), _one(exclude_phrases))[0])
+
+
+def ExecutePhraseGroupsTopKBatch(reader, queries, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, exclude_phrases=None,
+                                 boost=1.0):
+    """Top-k of OR-group queries (sdbg_phrase_groups_topk_batch): a match scores the sum of the scores of its positive
+    alternatives that occur in it, each bm25(phrase frequency, norm) with IndexReader.phrase_stats of that alternative.
+    Returns (hits [Q, k] structured, n_out [Q], total_matches [Q]) as ExecuteTopKBatch."""
+    groups = _phrase_groups(queries, exclude_phrases)
+    args, keep = _phrase_groups_args(groups, exclude)
+    stats = _alternative_stats(reader, groups, scorer, boost)
+    nq = len(queries)
+    hits = np.zeros((nq, k), HIT_DTYPE)
+    n_out = np.zeros(nq, np.uint32)
+    total = np.zeros(nq, np.uint64)
+    N.check(N.lib().sdbg_phrase_groups_topk_batch(_seg_array(reader.segments), len(reader.segments), *args, stats, scorer.k, scorer.b,
+                                                  _ref(filt), int(k), float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)),
+            reader.segments[0].ctx._h)
+    return hits, n_out, total
+
+
+def ExecutePhraseGroupsTopK(reader, query, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, exclude_phrases=None, boost=1.0):
+    """ExecutePhraseGroupsTopKBatch for one query: (hits [n_out], total_matches)."""
+    hits, n_out, total = ExecutePhraseGroupsTopKBatch(reader, [list(query)], scorer, k, filt, threshold, _one(exclude),
+                                                      _one(exclude_phrases), boost)
+    return hits[0, :n_out[0]], int(total[0])
+
+
+def ExecutePhraseGroupsTopKByColumnBatch(reader, queries, sort_field, k, descending=False, nulls_first=False, filt=None,
+                                         exclude=None, exclude_phrases=None):
+    """Sorted scan of OR-group queries (sdbg_phrase_groups_topk_by_column_batch): the first k of the docs
+    ExecutePhraseGroupsCountBatch counts, in the order of ExecuteTopKByColumnBatch. Returns its dict."""
+    vt = _sort_value_type(reader, sort_field)
+    groups = _phrase_groups(queries, exclude_phrases)
+    args, keep = _phrase_groups_args(groups, exclude)
+    nq = len(queries)
+    hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
+    n_out = np.zeros(max(nq, 1), np.uint32)
+    N.check(N.lib().sdbg_phrase_groups_topk_by_column_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt),
+                                                            int(sort_field), int(bool(descending)), int(bool(nulls_first)), int(k),
+                                                            _ptr(hits), _ptr(n_out)), reader.segments[0].ctx._h)
+    return _sort_result(hits, n_out, nq, k, vt)
+
+
+def ExecutePhraseGroupsTopKByColumn(reader, query, sort_field, k, descending=False, nulls_first=False, filt=None, exclude=None,
+                                    exclude_phrases=None):
+    """ExecutePhraseGroupsTopKByColumnBatch for one query: dict of docs, segs, values, nulls."""
+    return _sort_row(ExecutePhraseGroupsTopKByColumnBatch(reader, [list(query)], sort_field, k, descending, nulls_first, filt,
+                                                          _one(exclude), _one(exclude_phrases)))
+
+
+def ExecutePhraseGroupsFacetCountsBatch(reader, queries, key_field, key_min=None, key_span=None, filt=None, exclude=None,
+                                        exclude_phrases=None):
+    """Facet counts of OR-group queries (sdbg_phrase_groups_facet_counts_batch): how the docs
+    ExecutePhraseGroupsCountBatch counts split over the values of column `key_field`. Returns the dict
+    ExecuteFacetCountsBatch returns."""
+    key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
+    groups = _phrase_groups(queries, exclude_phrases)
+    args, keep = _phrase_groups_args(groups, exclude)
+    nq = len(queries)
+    counts = np.zeros((max(nq, 1), max(int(key_span), 1)), np.uint64)
+    nulls = np.zeros(max(nq, 1), np.uint64)
+    N.check(N.lib().sdbg_phrase_groups_facet_counts_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt),
+                                                          int(key_field), int(key_min), int(key_span), _ptr(counts), _ptr(nulls)),
+            reader.segments[0].ctx._h)
+    return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
+
+
+def ExecutePhraseGroupsFacetCounts(reader, query, key_field, key_min=None, key_span=None, filt=None, exclude=None,
+                                   exclude_phrases=None):
+    """ExecutePhraseGroupsFacetCountsBatch for one query: {key: count} plus {None: n} for NULL keys."""
+    return _facet_row(ExecutePhraseGroupsFacetCountsBatch(reader, [list(query)], key_field, key_min, key_span, filt, _one(exclude),
+                                                          _one(exclude_phrases)))
+
+
+def ExecutePhraseGroupsMatchAggregatesBatch(reader, queries, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                                            exclude=None, exclude_phrases=None):
+    """Aggregates over the matches of OR-group queries (sdbg_phrase_groups_aggregate_batch): over the docs
+    ExecutePhraseGroupsCountBatch counts; the grouping and the result as in ExecuteMatchAggregatesBatch."""
+    vt, kf, key_min, key_span = _agg_args(reader, value_field, key_field, key_min, key_span)
+    groups = _phrase_groups(queries, exclude_phrases)
+    args, keep = _phrase_groups_args(groups, exclude)
+    nq = len(queries)
+    out = np.zeros((max(nq, 1), max(int(key_span), 1)), MATCH_AGG_DTYPE)
+    null_out = np.zeros(max(nq, 1), MATCH_AGG_DTYPE)
+    N.check(N.lib().sdbg_phrase_groups_aggregate_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), kf,
+                                                       int(key_min), int(key_span), int(value_field), _ptr(out), _ptr(null_out)),
+            reader.segments[0].ctx._h)
+    return _agg_result(out, null_out, nq, key_min, vt)
+
+
+def ExecutePhraseGroupsMatchAggregates(reader, query, value_field, key_field=None, key_min=None, key_span=None, filt=None,
+                                       exclude=None, exclude_phrases=None):
+    """ExecutePhraseGroupsMatchAggregatesBatch for one query, in the form ExecuteMatchAggregates returns."""
+    return _agg_row(ExecutePhraseGroupsMatchAggregatesBatch(reader, [list(query)], value_field, key_field, key_min, key_span, filt,
+                                                            _one(exclude), _one(exclude_phrases)), key_field is not None)
+
+
+def ExecutePhraseGroupsMatchScanBatch(reader, queries, scorer=None, limit=1 << 20, offset=None, filt=None, exclude=None,
+                                      exclude_phrases=None, boost=1.0):
+    """Stream mode of OR-group queries (sdbg_phrase_groups_scan_batch): the docs ExecutePhraseGroupsCountBatch counts, in
+    (segment, doc) order, from ordinal offset[q] (None: 0) on, at most `limit` of them, scored as
+    ExecutePhraseGroupsTopKBatch scores them (scorer None: unscored). Returns what ExecuteMatchScanGroupsBatch returns."""
+    groups = _phrase_groups(queries, exclude_phrases)
+    args, keep = _phrase_groups_args(groups, exclude)
+    nq = len(queries)
+    stats = None if scorer is None else _alternative_stats(reader, groups, scorer, boost)
+    offs = None if offset is None else np.ascontiguousarray(offset, dtype=np.uint64)
+    if offs is not None and offs.shape != (nq,):
+        raise ValueError("offset needs one value per query")
+    hits = np.zeros((nq, max(int(limit), 1)), HIT_DTYPE)
+    n_out = np.zeros(nq, np.uint32)
+    total = np.zeros(nq, np.uint64)
+    k1, b = (0.0, 0.0) if scorer is None else (scorer.k, scorer.b)
+    N.check(N.lib().sdbg_phrase_groups_scan_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), stats, k1, b,
+                                                  _ptr(offs), int(limit), int(scorer is not None), _ptr(hits), _ptr(n_out),
+                                                  _ptr(total)), reader.segments[0].ctx._h)
+    return [((hits["seg"][q, :n_out[q]].copy(), hits["doc"][q, :n_out[q]].copy(), hits["score"][q, :n_out[q]].copy()),
+             int(total[q])) for q in range(nq)]
+
+
+def ExecutePhraseGroupsMatchScan(reader, query, scorer=None, limit=1 << 20, offset=0, filt=None, exclude=None, exclude_phrases=None,
+                                 boost=1.0):
+    """ExecutePhraseGroupsMatchScanBatch for one query: ((seg, doc, score) arrays, total matches)."""
+    return ExecutePhraseGroupsMatchScanBatch(reader, [list(query)], scorer, limit, [offset], filt, _one(exclude),
+                                             _one(exclude_phrases), boost)[0]
+
+
 SORT_HIT_DTYPE =np.dtype([("value", "<i8"), ("doc", "<u4"), ("seg", "<u4"), ("is_null", "u1"), ("pad", "V7")])
 _SORT_VALUE_DTYPE = {0: np.int64, 1: np.float64, 2: np.int32}
 

@@ -32,13 +32,17 @@ void check_phrase(const std::vector<uint32_t>& phrase, size_t n_terms, bool grou
   if (groups) throw GpuError(SDBG_EUNSUPPORTED, "a phrase has no OR groups");
 }
 
-// The clauses of a phrase query over its n_terms slots for the sdbg_phrase_and_* entries: clause_off (clause j is slots
-// off[j] .. off[j + 1]) and each clause's negation. Empty sizes and negations: the slots are one positive clause (a single
-// phrase). Not a phrase (no positions): no clauses.
+// The clauses of a phrase query over its n_terms slots for the sdbg_phrase_groups_* entries: clause_off (clause j is
+// slots off[j] .. off[j + 1]), each clause's negation, and the OR groups over the clauses: group_off (group g is clauses
+// goff[g] .. goff[g + 1]) and each group's negation, which all its clauses share. Empty sizes and negations: the slots are
+// one positive clause (a single phrase); empty group sizes: one clause per group (an And of the clauses). Not a phrase
+// (no positions): no clauses.
 void phrase_clauses(const std::vector<uint32_t>& phrase, size_t n_terms, const std::vector<uint32_t>& sizes,
-                    const std::vector<uint8_t>& negated, std::vector<uint32_t>& off, std::vector<uint8_t>& neg) {
+                    const std::vector<uint8_t>& negated, const std::vector<uint32_t>& group_sizes, std::vector<uint32_t>& off,
+                    std::vector<uint8_t>& neg, std::vector<uint32_t>& goff, std::vector<uint8_t>& gneg) {
   if (phrase.empty()) {
-    if (!sizes.empty() || !negated.empty()) throw GpuError(SDBG_EINVAL, "clause_sizes / clause_negated need phrase_positions");
+    if (!sizes.empty() || !negated.empty() || !group_sizes.empty())
+      throw GpuError(SDBG_EINVAL, "clause_sizes / clause_negated / clause_group_sizes need phrase_positions");
     return;
   }
   if (sizes.empty() && !negated.empty()) throw GpuError(SDBG_EINVAL, "clause_negated needs clause_sizes");
@@ -50,6 +54,20 @@ void phrase_clauses(const std::vector<uint32_t>& phrase, size_t n_terms, const s
   if (off.back() != n_terms) throw GpuError(SDBG_EINVAL, "clause_sizes must cover the terms");
   neg.assign(sz.size(), 0u);
   for (size_t j = 0; j < negated.size(); ++j) neg[j] = negated[j] ? 1u : 0u;
+  goff.assign(1, 0u);
+  if (group_sizes.empty())
+    for (size_t j = 0; j < sz.size(); ++j) goff.push_back(goff.back() + 1u);
+  for (uint32_t x : group_sizes) {
+    if (x == 0) throw GpuError(SDBG_EINVAL, "an empty OR group");
+    goff.push_back(goff.back() + x);
+  }
+  if (goff.back() != sz.size()) throw GpuError(SDBG_EINVAL, "clause_group_sizes must cover the clauses");
+  gneg.assign(goff.size() - 1, 0u);
+  for (size_t g = 0; g + 1 < goff.size(); ++g) {
+    gneg[g] = neg[goff[g]];
+    for (uint32_t j = goff[g]; j < goff[g + 1]; ++j)
+      if (neg[j] != gneg[g]) throw GpuError(SDBG_EINVAL, "the clauses of an OR group share their clause_negated flag");
+  }
 }
 
 // The statistics of a phrase (collectors.cpp:116-128): the slots' idfs summed in float32 in slot order, a repeated term
@@ -89,12 +107,14 @@ GpuTopKIterator::GpuTopKIterator(sdbg_segment* segment, int kind, std::vector<sd
                                  uint32_t k, const sdbg_col_pred* table_filter, std::vector<uint32_t> excluded_terms,
                                  std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
                                  std::vector<uint32_t> phrase_positions,
-    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated,
+    std::vector<uint32_t> clause_group_sizes)
     : seg_(segment), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)), groups_(std::move(group_sizes)),
       group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)), k1_(k1), b_(b), k_(k), filter_(table_filter) {
   threshold_.value = FLT_MIN;  // doc_collector.hpp:102
   check_phrase(phrase_, terms_.size(), !groups_.empty());
-  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
+                 group_off_, group_neg_);
   if (!phrase_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "phrases need k > 0: the streaming scan has no phrase form");
   // the streaming scan (sdbg_bm25_scan*) has no grouped form
   if (!groups_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "OR groups need k > 0: the streaming scan has no grouped form");
@@ -130,11 +150,11 @@ void GpuTopKIterator::run() {
   if (!phrase_.empty()) {
     const std::vector<uint32_t> ids = term_ids(terms_);
     const std::vector<sdbg_bm25_term> stats = clause_stats(terms_, clause_off_, clause_neg_);
-    const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
-    check(sdbg_phrase_and_topk_batch(segs, 1, ids.data(), phrase_.data(), clause_off_.data(), clause_neg_.data(), query_clause_off, 1,
+    const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
+    check(sdbg_phrase_groups_topk_batch(segs, 1, ids.data(), phrase_.data(), clause_off_.data(), group_off_.data(), group_neg_.data(), query_group_off, 1,
                                      excluded_.data(), excl_off, stats.data(), k1_, b_, filter_.data(), k_, threshold_.value,
                                      hits_.data(), &n, &total_),
-          "sdbg_phrase_and_topk_batch");
+          "sdbg_phrase_groups_topk_batch");
     thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;
   } else if (!groups_.empty()) {
     const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
@@ -273,12 +293,14 @@ void GpuAggScan::Scan(duckdb::DataChunkMock& output) {
 GpuCountScan::GpuCountScan(std::vector<sdbg_segment*> segments, int kind, std::vector<uint32_t> terms,
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, std::vector<uint32_t> group_sizes,
                            std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions,
-    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated,
+    std::vector<uint32_t> clause_group_sizes)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       groups_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
       filter_(table_filter) {
   check_phrase(phrase_, terms_.size(), !groups_.empty());
-  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
+                 group_off_, group_neg_);
 }
 
 void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
@@ -290,10 +312,10 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
   int rc;
   const char* what;
   if (!phrase_.empty()) {
-    const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
-    rc = sdbg_phrase_and_count_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), clause_neg_.data(),
-                                     query_clause_off, 1, excluded_.data(), excl_off, filter_.data(), &n);
-    what = "sdbg_phrase_and_count_batch: ";
+    const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
+    rc = sdbg_phrase_groups_count_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), group_off_.data(), group_neg_.data(),
+                                     query_group_off, 1, excluded_.data(), excl_off, filter_.data(), &n);
+    what = "sdbg_phrase_groups_count_batch: ";
   } else if (groups_.empty()) {
     rc = sdbg_match_count_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                 filter_.data(), &n);
@@ -316,12 +338,14 @@ GpuSortedScan::GpuSortedScan(std::vector<sdbg_segment*> segments, int kind, std:
                              std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t sort_field,
                              bool descending, bool nulls_first, uint32_t k, std::vector<uint32_t> group_sizes,
                              std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions,
-    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated,
+    std::vector<uint32_t> clause_group_sizes)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
       filter_(table_filter), field_(sort_field), desc_(descending), nulls_first_(nulls_first), k_(k) {
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
-  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
+                 group_off_, group_neg_);
 }
 
 void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
@@ -334,11 +358,11 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
     int rc;
     const char* what;
     if (!phrase_.empty()) {
-      const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
-      rc = sdbg_phrase_and_topk_by_column_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
-                                                clause_neg_.data(), query_clause_off, 1, excluded_.data(), excl_off, filter_.data(),
+      const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
+      rc = sdbg_phrase_groups_topk_by_column_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), group_off_.data(),
+                                                group_neg_.data(), query_group_off, 1, excluded_.data(), excl_off, filter_.data(),
                                                 field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_, hits_.data(), &n);
-      what = "sdbg_phrase_and_topk_by_column_batch: ";
+      what = "sdbg_phrase_groups_topk_by_column_batch: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_topk_by_column_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                            filter_.data(), field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
@@ -373,13 +397,15 @@ GpuMatchScan::GpuMatchScan(std::vector<sdbg_segment*> segments, std::vector<sdbg
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, float k1, float b, bool scored,
                            std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
                            std::vector<uint32_t> phrase_positions,
-    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated,
+    std::vector<uint32_t> clause_group_sizes)
     : segs_(std::move(segments)), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(group_sizes.empty() ? std::vector<uint32_t>{uint32_t(terms_.size())} : std::move(group_sizes)),
       group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)), filter_(table_filter), k1_(k1), b_(b),
       scored_(scored) {
   check_phrase(phrase_, terms_.size(), group_sizes_.size() > 1 || !group_min_.empty());
-  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
+                 group_off_, group_neg_);
 }
 
 void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kPage - 1
@@ -393,11 +419,11 @@ void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kP
   if (!phrase_.empty()) {
     const std::vector<uint32_t> ids = term_ids(terms_);
     const std::vector<sdbg_bm25_term> stats = clause_stats(terms_, clause_off_, clause_neg_);
-    const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
-    rc = sdbg_phrase_and_scan_batch(segs_.data(), segs_.size(), ids.data(), phrase_.data(), clause_off_.data(), clause_neg_.data(),
-                                    query_clause_off, 1, excluded_.data(), excl_off, filter_.data(), scored_ ? stats.data() : nullptr,
+    const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
+    rc = sdbg_phrase_groups_scan_batch(segs_.data(), segs_.size(), ids.data(), phrase_.data(), clause_off_.data(), group_off_.data(), group_neg_.data(),
+                                    query_group_off, 1, excluded_.data(), excl_off, filter_.data(), scored_ ? stats.data() : nullptr,
                                     k1_, b_, &offset_, kPage, scored_ ? 1 : 0, page_.data(), &n, &total_);
-    what = "sdbg_phrase_and_scan_batch: ";
+    what = "sdbg_phrase_groups_scan_batch: ";
   } else {
     rc = sdbg_match_scan_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
                                           group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(), excl_off,
@@ -429,12 +455,14 @@ GpuFacetScan::GpuFacetScan(std::vector<sdbg_segment*> segments, int kind, std::v
                            std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
                            std::vector<uint32_t> group_sizes, std::vector<uint32_t> group_min_match,
                            std::vector<uint32_t> phrase_positions,
-    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated,
+    std::vector<uint32_t> clause_group_sizes)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
       filter_(table_filter), field_(key_field) {
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
-  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
+                 group_off_, group_neg_);
 }
 
 void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
@@ -458,11 +486,11 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
     int rc;
     const char* what;
     if (!phrase_.empty()) {
-      const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
-      rc = sdbg_phrase_and_facet_counts_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
-                                              clause_neg_.data(), query_clause_off, 1, excluded_.data(), excl_off, filter_.data(),
+      const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
+      rc = sdbg_phrase_groups_facet_counts_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), group_off_.data(),
+                                              group_neg_.data(), query_group_off, 1, excluded_.data(), excl_off, filter_.data(),
                                               field_, lo, uint32_t(span), counts.data(), &nulls_);
-      what = "sdbg_phrase_and_facet_counts_batch: ";
+      what = "sdbg_phrase_groups_facet_counts_batch: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_facet_counts_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                          filter_.data(), field_, lo, uint32_t(span), counts.data(), &nulls_);
@@ -497,12 +525,14 @@ GpuMatchAggScan::GpuMatchAggScan(std::vector<sdbg_segment*> segments, int kind, 
                                  std::vector<uint32_t> excluded_terms, const sdbg_col_pred* table_filter, uint64_t key_field,
                                  uint64_t value_field, sdbg_type value_type, std::vector<uint32_t> group_sizes,
                                  std::vector<uint32_t> group_min_match, std::vector<uint32_t> phrase_positions,
-    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated)
+    std::vector<uint32_t> clause_sizes, std::vector<uint8_t> clause_negated,
+    std::vector<uint32_t> clause_group_sizes)
     : segs_(std::move(segments)), kind_(kind), terms_(std::move(terms)), excluded_(std::move(excluded_terms)),
       group_sizes_(std::move(group_sizes)), group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)),
       filter_(table_filter), key_field_(key_field), value_field_(value_field), value_type_(value_type) {
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
-  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_off_, clause_neg_);
+  phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
+                 group_off_, group_neg_);
 }
 
 void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
@@ -533,11 +563,11 @@ void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
     int rc;
     const char* what;
     if (!phrase_.empty()) {
-      const uint32_t query_clause_off[2] = {0, uint32_t(clause_neg_.size())};
-      rc = sdbg_phrase_and_aggregate_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
-                                           clause_neg_.data(), query_clause_off, 1, excluded_.data(), excl_off, filter_.data(),
+      const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
+      rc = sdbg_phrase_groups_aggregate_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), group_off_.data(),
+                                           group_neg_.data(), query_group_off, 1, excluded_.data(), excl_off, filter_.data(),
                                            key_field_, lo, uint32_t(span), value_field_, cells.data(), &null_cell);
-      what = "sdbg_phrase_and_aggregate_batch: ";
+      what = "sdbg_phrase_groups_aggregate_batch: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_aggregate_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                       filter_.data(), key_field_, lo, uint32_t(span), value_field_, cells.data(),

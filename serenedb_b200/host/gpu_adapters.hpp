@@ -56,7 +56,8 @@ class GpuTopKIterator final : public irs::DocIterator {
                                                                  relative positions (0 first, increasing); needs k > 0 */,
                   std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
                                                             phrase_positions (a one-slot clause is a term); empty: one phrase */,
-                  std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
+                  std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */,
+                  std::vector<uint32_t> clause_group_sizes = {} /* clauses per OR group, in order; empty: one per group */);
 
   // Scored top-k: the hot path.
   void Collect(const irs::ScoreFunction&, irs::ColumnArgsFetcher&, irs::ScoreCollector& collector) override;
@@ -94,6 +95,8 @@ class GpuTopKIterator final : public irs::DocIterator {
   std::vector<uint32_t> phrase_;      // a phrase's relative positions, one per term (empty: not a phrase)
   std::vector<uint32_t> clause_off_;  // the clauses over terms_ / phrase_ (a single phrase: one clause)
   std::vector<uint8_t> clause_neg_;   // per clause: negated
+  std::vector<uint32_t> group_off_;   // the OR groups over the clauses (clause_group_sizes)
+  std::vector<uint8_t> group_neg_;    // per group: negated
   float k1_, b_;
   uint32_t k_;
   FilterChain filter_;
@@ -140,7 +143,8 @@ class GpuCountScan {
                                                               relative positions (0 first, increasing) */,
                std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
                                                          phrase_positions (a one-slot clause is a term); empty: one phrase */,
-               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
+               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */,
+                  std::vector<uint32_t> clause_group_sizes = {} /* clauses per OR group, in order; empty: one per group */);
   // Fills `output` with one row, count[0] = the number of matches; the next call leaves it empty (end of scan).
   void Scan(duckdb::DataChunkMock& output);
 
@@ -148,7 +152,8 @@ class GpuCountScan {
   std::vector<sdbg_segment*> segs_;
   int kind_;
   std::vector<uint32_t> terms_, excluded_, groups_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
-  std::vector<uint8_t> clause_neg_;
+  std::vector<uint8_t> clause_neg_, group_neg_;
+  std::vector<uint32_t> group_off_;   // the OR groups over the clauses (clause_group_sizes)
   FilterChain filter_;
   bool done_ = false;
 };
@@ -171,14 +176,16 @@ class GpuSortedScan {
                                                                relative positions (0 first, increasing) */,
                 std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
                                                           phrase_positions (a one-slot clause is a term); empty: one phrase */,
-                std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
+                std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */,
+                  std::vector<uint32_t> clause_group_sizes = {} /* clauses per OR group, in order; empty: one per group */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
   std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
-  std::vector<uint8_t> clause_neg_;
+  std::vector<uint8_t> clause_neg_, group_neg_;
+  std::vector<uint32_t> group_off_;   // the OR groups over the clauses (clause_group_sizes)
   FilterChain filter_;
   uint64_t field_;
   bool desc_, nulls_first_;
@@ -207,7 +214,8 @@ class GpuMatchScan {
                                                               relative positions (0 first, increasing) */,
                std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
                                                          phrase_positions (a one-slot clause is a term); empty: one phrase */,
-               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
+               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */,
+                  std::vector<uint32_t> clause_group_sizes = {} /* clauses per OR group, in order; empty: one per group */);
   void Scan(duckdb::DataChunkMock& output);
   uint64_t total_matches() const { return total_; }
 
@@ -216,7 +224,8 @@ class GpuMatchScan {
   std::vector<sdbg_segment*> segs_;
   std::vector<sdbg_bm25_term> terms_;
   std::vector<uint32_t> excluded_, group_sizes_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
-  std::vector<uint8_t> clause_neg_;
+  std::vector<uint8_t> clause_neg_, group_neg_;
+  std::vector<uint32_t> group_off_;   // the OR groups over the clauses (clause_group_sizes)
   FilterChain filter_;
   float k1_, b_;
   bool scored_;
@@ -244,14 +253,16 @@ class GpuFacetScan {
                                                               relative positions (0 first, increasing) */,
                std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
                                                          phrase_positions (a one-slot clause is a term); empty: one phrase */,
-               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
+               std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */,
+                  std::vector<uint32_t> clause_group_sizes = {} /* clauses per OR group, in order; empty: one per group */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
   std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
-  std::vector<uint8_t> clause_neg_;
+  std::vector<uint8_t> clause_neg_, group_neg_;
+  std::vector<uint32_t> group_off_;   // the OR groups over the clauses (clause_group_sizes)
   FilterChain filter_;
   uint64_t field_;
   std::vector<std::pair<int64_t, uint64_t>> groups_;   // (key, count) of the non-empty groups
@@ -282,14 +293,16 @@ class GpuMatchAggScan {
                                                                  relative positions (0 first, increasing) */,
                   std::vector<uint32_t> clause_sizes = {} /* an And of clauses: consecutive clauses over `terms` /
                                                             phrase_positions (a one-slot clause is a term); empty: one phrase */,
-                  std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */);
+                  std::vector<uint8_t> clause_negated = {} /* per clause: 1 for a Not child; empty: none */,
+                  std::vector<uint32_t> clause_group_sizes = {} /* clauses per OR group, in order; empty: one per group */);
   void Scan(duckdb::DataChunkMock& output);
 
  private:
   std::vector<sdbg_segment*> segs_;
   int kind_;
   std::vector<uint32_t> terms_, excluded_, group_sizes_, group_min_, phrase_, clause_off_;   // clause_off_: the phrase's clauses
-  std::vector<uint8_t> clause_neg_;
+  std::vector<uint8_t> clause_neg_, group_neg_;
+  std::vector<uint32_t> group_off_;   // the OR groups over the clauses (clause_group_sizes)
   FilterChain filter_;
   uint64_t key_field_, value_field_;
   sdbg_type value_type_;

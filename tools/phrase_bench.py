@@ -19,10 +19,15 @@ A third batch, "phrase-and", times conjunctions of a phrase with a term (sdbg_ph
 queries `"w1 w2" & t`, t a token drawn from the phrase's own doc, and the same with `& !"w3 w4"` added, w3 w4 a window
 drawn as the phrases are. For each it reports the count, the top-1000 and the facets GROUP BY cat, next to the phrase
 "w1 w2" alone and the AND of w1, w2 and t (and of w3, w4 not excluded: the AND of w1, w2, t is the candidate set).
+A fourth batch, "phrase-groups", times phrases inside OR groups (sdbg_phrase_groups_*_batch), the shape synonym
+expansion produces: --queries queries each of `("w1 w2" | s) & t`, `"w1 w2" | s` and `("w1 w2" | s) & t & !"w3 w4"`,
+s a token of another doc, t a token of the phrase's doc (s, w1 and t distinct), next to `"w1 w2" & t` (phrase-and) and
+`(w1 | s) & t` (the OR-group count, top-k and facets of sdbg_*_groups). The proxy candidates of `"w1 w2" | s` are the
+docs of w1 or w2 (the cheaper) or s, wider than the phrase's own AND.
 --batches picks the batches to run (comma-separated; all by default).
 Prints one JSON line with the GPU name and power limit read in the same run.
 
-    python tools/phrase_bench.py [--steps 5] [--warmup 2] [--docs 10000000] [--queries 4096] [--batches 2-word,phrase-and]
+    python tools/phrase_bench.py [--steps 5] [--warmup 2] [--docs 10000000] [--queries 4096] [--batches 2-word,phrase-and,phrase-groups]
 """
 import argparse
 import json
@@ -122,6 +127,53 @@ def phrase_and_rows(c, reader, ctx, scorer, n, rng, steps, warmup):
     return r
 
 
+def phrase_groups_rows(c, reader, ctx, scorer, n, rng, steps, warmup):
+    """The "phrase-groups" batch: `("w1 w2" | s) & t`, `"w1 w2" | s`, `("w1 w2" | s) & t & !"w3 w4"` next to `"w1 w2" & t`
+    and `(w1 | s) & t`."""
+    terms, doc = c["terms"], c["doc"]
+    ph, ss, ts = [], [], []
+    while len(ph) < n:
+        i = int(rng.integers(0, len(terms) - 2))
+        if doc[i] != doc[i + 1]:
+            continue
+        same = np.flatnonzero(doc[max(0, i - 28):i + 30] == doc[i]) + max(0, i - 28)
+        t = int(terms[int(same[int(rng.integers(0, len(same)))])])
+        s = int(terms[int(rng.integers(0, len(terms)))])
+        if len({int(terms[i]), s, t}) < 3:
+            continue
+        ph.append([int(terms[i]), int(terms[i + 1])]); ss.append(s); ts.append(t)
+    neg = [[x] for x in phrases(c, n, 2, rng)]
+    and_t = [[[p], [[t]]] for p, t in zip(ph, ts)]
+    or_t = [[[p, [s]], [[t]]] for p, s, t in zip(ph, ss, ts)]
+    or_only = [[[p, [s]]] for p, s in zip(ph, ss)]
+    grp = [[[p[0], s], [t]] for p, s, t in zip(ph, ss, ts)]
+    pa = [[p, [t]] for p, t in zip(ph, ts)]
+    counts = {"phrase_and": sdb.ExecutePhraseGroupsCountBatch(reader, and_t), "or_and_t": sdb.ExecutePhraseGroupsCountBatch(reader, or_t),
+              "or": sdb.ExecutePhraseGroupsCountBatch(reader, or_only),
+              "or_and_t_not": sdb.ExecutePhraseGroupsCountBatch(reader, or_t, exclude_phrases=neg),
+              "groups": sdb.ExecuteCountGroupsBatch(reader, grp)}
+    _, _, tt = sdb.ExecutePhraseGroupsTopKBatch(reader, or_t, scorer, 1000)
+    fac = sdb.ExecutePhraseGroupsFacetCountsBatch(reader, or_t, 2, 0, 100)
+    if (not np.array_equal(counts["phrase_and"], sdb.ExecutePhraseAndCountBatch(reader, pa)) or not np.array_equal(tt, counts["or_and_t"])
+            or not np.array_equal(fac["counts"].sum(1), counts["or_and_t"]) or np.any(counts["or_and_t"] < counts["phrase_and"])
+            or np.any(counts["or_and_t_not"] > counts["or_and_t"])):
+        raise SystemExit("phrase-groups count / top-k / facet mismatch")
+    r = {k + "_matches": int(v.sum()) for k, v in counts.items()}
+    runs = (("phrase_and", lambda: sdb.ExecutePhraseAndCountBatch(reader, pa), lambda: sdb.ExecutePhraseAndTopKBatch(reader, pa, scorer, 1000),
+             lambda: sdb.ExecutePhraseAndFacetCountsBatch(reader, pa, 2, 0, 100)),
+            ("groups", lambda: sdb.ExecuteCountGroupsBatch(reader, grp), lambda: sdb.ExecuteTopKGroupsBatch(reader, grp, scorer, 1000),
+             lambda: sdb.ExecuteFacetCountsGroupsBatch(reader, grp, 2, 0, 100)))
+    runs += tuple((name, (lambda q=q, x=x: sdb.ExecutePhraseGroupsCountBatch(reader, q, exclude_phrases=x)),
+                   (lambda q=q, x=x: sdb.ExecutePhraseGroupsTopKBatch(reader, q, scorer, 1000, exclude_phrases=x)),
+                   (lambda q=q, x=x: sdb.ExecutePhraseGroupsFacetCountsBatch(reader, q, 2, 0, 100, exclude_phrases=x)))
+                  for name, q, x in (("or_and_t", or_t, None), ("or", or_only, None), ("or_and_t_not", or_t, neg)))
+    for name, cnt, top, facets in runs:
+        r[name + "_count_ms"] = timed(ctx, cnt, steps, warmup)
+        r[name + "_top1000_ms"] = timed(ctx, top, steps, warmup)
+        r[name + "_facets_ms"] = timed(ctx, facets, steps, warmup)
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
@@ -129,7 +181,7 @@ def main():
     ap.add_argument("--docs", type=int, default=10_000_000)
     ap.add_argument("--vocab", type=int, default=100_000)
     ap.add_argument("--queries", type=int, default=4096)
-    ap.add_argument("--batches", default="2-word,3/4-word,phrase-and")
+    ap.add_argument("--batches", default="2-word,3/4-word,phrase-and,phrase-groups")
     a = ap.parse_args()
     want = set(a.batches.split(","))
     c = corpus(a.docs, a.vocab, 7)
@@ -184,6 +236,9 @@ def main():
         out["batches"][name] = r
     if "phrase-and" in want:
         out["batches"]["phrase-and"] = phrase_and_rows(c, reader, ctx, scorer, a.queries, np.random.default_rng(17), a.steps, a.warmup)
+    if "phrase-groups" in want:
+        out["batches"]["phrase-groups"] = phrase_groups_rows(c, reader, ctx, scorer, a.queries, np.random.default_rng(19), a.steps,
+                                                             a.warmup)
     print(json.dumps(out))
 
 
