@@ -677,6 +677,76 @@ int sdbg_phrase_groups_scan_batch(sdbg_segment* const* segs, size_t n_segs, cons
                                   const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats /* NULL when scored == 0 */,
                                   float k1, float b, const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit,
                                   int scored, sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
+/* Minimum match counts over OR groups of phrases and terms (`2 of ("new york" | nyc | "big apple") & pizza`; the shape a
+ * minimum_should_match query with a multi-word synonym produces). Everything is as in sdbg_phrase_groups_*, with positive
+ * group g holding doc d when at least group_min[g] of its s_g alternatives have phrase frequency > 0 in d (group_min
+ * NULL: every minimum 1). Every alternative counts on its own: duplicate alternatives each count, as they are each
+ * scored. 1 <= group_min[g] <= s_g; a negated group keeps minimum 1 (`!(A | B)` is `!A & !B`). The score is unchanged:
+ * the fp32 sum, from 0, of bm25(phrase frequency, norm) over every positive alternative with frequency > 0 in d, in
+ * ascending alternative cost within d's segment, ties in flattened query order; a doc holding more than group_min[g]
+ * alternatives of a group is scored on all of them (as the term *_groups_min entries score). A positive group with
+ * group_min == s_g is s_g groups of one alternative, and at most 16 slots per query still bound the groups after that
+ * split. Every minimum 1 (or NULL) gives exactly sdbg_phrase_groups_* (which run as this case); group_min == s_g gives
+ * exactly sdbg_phrase_and_* with that group's alternatives as separate positive clauses; one-slot alternatives of
+ * distinct terms give exactly the term *_batch_groups_min entries (the top-k bit for bit at pruning level 0). Nothing is
+ * pruned: identical at every pruning level, total_matches exact, k <= 4096.
+ * Each entry takes the parameters of its sdbg_phrase_groups_* counterpart plus group_min right after group_negated;
+ * outputs, orders, NULL rules and scratch are the counterpart's. Errors, all found before anything is queued: a
+ * group_min[g] of 0 or above its group's size: SDBG_EINVAL; a negated group with group_min[g] != 1: SDBG_EUNSUPPORTED;
+ * otherwise the counterpart's. Synchronous. */
+int sdbg_phrase_groups_count_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                       const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                       const uint32_t* clause_off, const uint32_t* group_off,
+                                       const uint8_t* group_negated /* NULL: none */,
+                                       const uint32_t* group_min /* NULL: all 1 */, const uint32_t* query_group_off,
+                                       size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                       const sdbg_col_pred* filt, uint64_t* counts);
+int sdbg_phrase_groups_topk_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                      const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                      const uint32_t* clause_off, const uint32_t* group_off,
+                                      const uint8_t* group_negated /* NULL: none */,
+                                      const uint32_t* group_min /* NULL: all 1 */, const uint32_t* query_group_off,
+                                      size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                      const sdbg_bm25_term* clause_stats /* one per alternative */, float k1, float b,
+                                      const sdbg_col_pred* filt, uint32_t k, float threshold_in,
+                                      sdbg_hit* out /* n_queries * k */, uint32_t* n_out, uint64_t* total_matches);
+int sdbg_phrase_groups_topk_by_column_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                                const uint32_t* clause_off, const uint32_t* group_off,
+                                                const uint8_t* group_negated /* NULL: none */,
+                                                const uint32_t* group_min /* NULL: all 1 */, const uint32_t* query_group_off,
+                                                size_t n_queries, const uint32_t* excl_terms,
+                                                const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                                                uint64_t sort_field, int descending, int nulls_first, uint32_t k,
+                                                sdbg_sort_hit* out /* n_queries * k */, uint32_t* n_out);
+int sdbg_phrase_groups_facet_counts_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                              const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                              const uint32_t* clause_off, const uint32_t* group_off,
+                                              const uint8_t* group_negated /* NULL: none */,
+                                              const uint32_t* group_min /* NULL: all 1 */, const uint32_t* query_group_off,
+                                              size_t n_queries, const uint32_t* excl_terms,
+                                              const uint32_t* excl_off /* NULL: none */, const sdbg_col_pred* filt,
+                                              uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                              uint64_t* counts /* n_queries * key_span */, uint64_t* null_counts /* n_queries */);
+int sdbg_phrase_groups_aggregate_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                           const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                           const uint32_t* clause_off, const uint32_t* group_off,
+                                           const uint8_t* group_negated /* NULL: none */,
+                                           const uint32_t* group_min /* NULL: all 1 */, const uint32_t* query_group_off,
+                                           size_t n_queries, const uint32_t* excl_terms,
+                                           const uint32_t* excl_off /* NULL: none */,
+                                           const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min, uint32_t key_span,
+                                           uint64_t value_field, sdbg_match_agg* out /* n_queries * key_span */,
+                                           sdbg_match_agg* null_out /* n_queries */);
+int sdbg_phrase_groups_scan_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                      const uint32_t* rel_pos /* NULL: adjacent within each alternative */,
+                                      const uint32_t* clause_off, const uint32_t* group_off,
+                                      const uint8_t* group_negated /* NULL: none */,
+                                      const uint32_t* group_min /* NULL: all 1 */, const uint32_t* query_group_off,
+                                      size_t n_queries, const uint32_t* excl_terms, const uint32_t* excl_off /* NULL: none */,
+                                      const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats /* NULL when scored == 0 */,
+                                      float k1, float b, const uint64_t* offset /* n_queries; NULL: all 0 */, uint32_t limit,
+                                      int scored, sdbg_hit* out /* n_queries * limit */, uint32_t* n_out, uint64_t* total);
 /* Multi-GPU: leave each query's top-k on the device as sortable 64-bit keys + a base ordinal so a
  * collective can gather them; merge gathered keys from `n_ranks` ranks (see INTEGRATION.md). */
 int sdbg_bm25_topk_batch_device(sdbg_segment* const* segs, size_t n_segs, int kind,

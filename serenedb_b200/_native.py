@@ -140,6 +140,18 @@ SIGNATURES = {
                                                      C.c_int64, C.c_uint32, C.c_uint64, _vp, _vp]),
     "sdbg_phrase_groups_scan_batch": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, C.c_float,
                                                 C.c_float, _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
+    # the minimum match counts: the OR-group entries' arguments with group_min after group_negated
+    "sdbg_phrase_groups_count_batch_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "sdbg_phrase_groups_topk_batch_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, C.c_float,
+                                                    C.c_float, _vp, C.c_uint32, C.c_float, _vp, _vp, _vp]),
+    "sdbg_phrase_groups_topk_by_column_batch_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp,
+                                                              C.c_uint64, C.c_int, C.c_int, C.c_uint32, _vp, _vp]),
+    "sdbg_phrase_groups_facet_counts_batch_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp,
+                                                            C.c_uint64, C.c_int64, C.c_uint32, _vp, _vp]),
+    "sdbg_phrase_groups_aggregate_batch_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp,
+                                                         C.c_uint64, C.c_int64, C.c_uint32, C.c_uint64, _vp, _vp]),
+    "sdbg_phrase_groups_scan_batch_min": (C.c_int, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp,
+                                                    C.c_float, C.c_float, _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
     "sdbg_match_topk_by_column_batch":(C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int, C.c_int,
                                                   C.c_uint32, _vp, _vp]),
     "sdbg_match_facet_counts_batch": (C.c_int, [_vp, _sz, C.c_int, _vp, _vp, _sz, _vp, _vp, _vp, C.c_uint64, C.c_int64,

@@ -161,7 +161,7 @@ constexpr int kPhraseMinBlocks = 4;
 // gives each doc its ordinal, base[item.w] plus the matches of the item's earlier windows; the docs whose ordinal lies in
 // [offset[q], offset[q] + limit) go to their row of P.emit.out, unscored. An item whose ordinals miss the page exits
 // before it decodes anything, and an item stops after the window that fills the page.
-// kPhrase (on any candidate shape: the AND, the flat OR or the OR groups (m = 1) of the alternatives' proxy terms): the
+// kPhrase (on any candidate shape: the AND, the flat OR or the OR groups (m >= 1) of the alternatives' proxy terms): the
 // alternative check (phrase_clauses, bm25_phrase.cuh). Every doc that survives the candidate scan, the exclusions, the
 // deleted docs and the filter chain is probed, entry after entry of the query's alternative table, in each slot's list
 // for its positions; a doc that fails its groups is dropped, the others are counted and, with P.phrase.cap, scored as the
@@ -173,8 +173,8 @@ constexpr int kPhraseMinBlocks = 4;
 // matches and emit passes A and B see the same set. With kSort it runs inside the sink, on a doc whose key has passed
 // s_thr: a doc that cannot enter the buffer is never probed for positions.
 // The sinks take kGroups queries: the groups narrow `acc` before the sink reads the column, and the bit-sliced counter
-// planes follow the sink's region of dynamic shared memory (16 * cap B, 4 * span B or agg_cells_bytes(span), rounded up
-// to 16 B).
+// planes follow the sink's region of dynamic shared memory (16 * cap B of the sorted scan or the phrase sink, 4 * span B
+// or agg_cells_bytes(span), rounded up to 16 B).
 template <bool kAnd, bool kGroups = false, bool kSort = false, bool kFacet = false, bool kAgg = false, bool kEmit = false,
           bool kPhrase = false>
 __global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0) bm25_count_kernel(CountParams P) {
@@ -379,11 +379,11 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0)
       }
     }
     if constexpr (kGroups) {
-      // the lead group is already in acc unless it needs m >= 2 of its lists (never for phrase candidates)
-      for (uint32_t g = !kPhrase && (gend0 >> 8) ? 0u : 1u; g < n_groups; ++g) {
+      // the lead group is already in acc unless it needs m >= 2 of its lists
+      for (uint32_t g = (gend0 >> 8) ? 0u : 1u; g < n_groups; ++g) {
         const uint32_t lo = g ? s_gend[g - 1] & 0xFFu : 0u, hi = s_gend[g] & 0xFFu, m = (s_gend[g] >> 8) + 1u;
         uint32_t nz = 0u;
-        if (kPhrase || m == 1u) {
+        if (m == 1u) {
           for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
           __syncthreads();
           run_lists(lo, hi, tmp, false, true);
@@ -393,7 +393,7 @@ __global__ void __launch_bounds__(kCountThreads, kPhrase ? kPhraseMinBlocks : 0)
           // at least m of the lists: each list's bitmap is added into a saturating bit-sliced counter (plane p = bit p)
           const uint32_t np = 32u - __clz(m);
           uint32_t* const plane = bins + (kSort ? 4u * P.sort.cap : kFacet ? (P.facet.span + 3u) & ~3u
-                                                                  : kAgg ? agg_cells_bytes(P.agg.key.span) / 4u : 0u);
+                                          : kAgg ? agg_cells_bytes(P.agg.key.span) / 4u : kPhraseSink ? 4u * P.phrase.cap : 0u);
           for (uint32_t i = tid; i < np * kCountWords; i += kCountThreads) plane[i] = 0u;
           for (uint32_t i = tid; i < kCountWords; i += kCountThreads) tmp[i] = 0u;
           for (uint32_t li = lo; li < hi; ++li) {

@@ -89,8 +89,11 @@ __device__ __forceinline__ uint32_t phrase_freq(const PostingsDev& S, const Phra
 }
 
 // The flags of an alternative table entry: negated; its group (bits 1..4) of the query; the candidate scan guarantees its
-// group (check mode need not look); the last positive entry of its group in table order.
-constexpr uint32_t kAltNegated = 1u, kAltGuaranteed = 1u << 5, kAltLast = 1u << 6;
+// group (check mode need not look); `need` (bits 6..9), the count of matched entries its group must have before this
+// entry for the doc to survive this entry's frequency 0: max(0, m - rest), rest the positive entries of the group after
+// this one in table order (for m = 1: 1 on the group's last entry, else 0; negated entries 0); the group's minimum match
+// count m - 1 (bits 10..13; negated groups 0).
+constexpr uint32_t kAltNegated = 1u, kAltGuaranteed = 1u << 5, kAltNeedShift = 6, kAltMinShift = 10;
 
 // Query q's alternative range and its first alternative, read once per window outside the per-doc loops: a single phrase
 // (one alternative) then reads no table per doc.
@@ -114,13 +117,15 @@ enum class PhraseMode { check, score, score_match };
 // The check of doc d for query Q, entry after entry in table order. kAlts false, for the candidate AND (every positive
 // group one alternative, table flags only kAltNegated): a clause conjunction's walk, dropping d at the first entry that
 // fails (positive: frequency 0; negated: frequency > 0); check mode skips the one-slot positive entries, which the AND
-// holds. kAlts true, for the flat OR and OR-group candidates, with the mask `sat` of the positive groups satisfied so far:
-// a negated entry with phrase frequency > 0 drops d; a positive entry with frequency > 0 satisfies its group, and one
-// with frequency 0 that is the last of a group not yet satisfied drops d. Every positive group has a last entry, so a doc
-// that reaches the table's end has every positive group satisfied (or guaranteed): it matches, and no mask of the
-// query's groups needs to stay live. Scoring modes evaluate every positive entry: s = the sum of bm25(frequency,
-// norm(d)) of those with frequency > 0, with their statistics, in table order from 0 (a one-slot entry's frequency is its
-// term's position count). The kAlts walk scores a conjunction's table too, so phrase_score_kernel takes every shape.
+// holds. kAlts true, for the flat OR and OR-group candidates, with per positive group a 4-bit count `have` of its
+// entries of frequency > 0 so far (16 counters in `cnt`, counted until they reach m <= 15; a group is satisfied when
+// have == m): a negated entry with phrase frequency > 0 drops d; a positive entry with frequency > 0 counts for its
+// group, and one with frequency 0 drops d when have < need, i.e. the group's count plus the entries after this one cannot
+// reach m (for m = 1: the last entry of an unsatisfied group). A positive group's last entry has need m, so a doc that
+// reaches the table's end has every positive group satisfied (or guaranteed): it matches, and no state of the query's
+// groups needs to stay live. Scoring modes evaluate every positive entry: s = the
+// sum of bm25(frequency, norm(d)) of those with frequency > 0, with their statistics, in table order from 0 (a one-slot
+// entry's frequency is its term's position count). The kAlts walk scores a conjunction's table too, so phrase_score_kernel takes every shape.
 template <bool kAlts>
 __device__ __forceinline__ bool phrase_clauses(const PostingsDev& S, const PhraseSink& F, const PhraseQuery& Q, uint32_t d,
                                                PhraseMode mode, float& s) {
@@ -142,17 +147,18 @@ __device__ __forceinline__ bool phrase_clauses(const PostingsDev& S, const Phras
     }
   } else {
     uint4 cl = __ldg(F.clauses + Q.c0);   // Q.first is not kept live across the window: the candidate scan's state is
-    uint32_t sat = 0u;
+    unsigned long long cnt = 0ull;
     for (uint32_t c = Q.c0;;) {
       const bool neg = cl.z & kAltNegated;
-      const uint32_t g = 1u << ((cl.z >> 1) & 15u);
+      const uint32_t sh = 4u * ((cl.z >> 1) & 15u), have = uint32_t(cnt >> sh) & 15u;
+      const bool open = have <= ((cl.z >> kAltMinShift) & 15u);   // have < m
       const bool skip = neg ? mode == PhraseMode::score_match
-                            : mode == PhraseMode::check && ((cl.z & kAltGuaranteed) || (sat & g));
+                            : mode == PhraseMode::check && ((cl.z & kAltGuaranteed) || !open);
       if (!skip) {
         const uint32_t f = phrase_freq(S, F, cl.x, cl.y, d);
-        if (f != 0u ? neg : (cl.z & kAltLast) && !(sat & g)) return false;
+        if (f != 0u ? neg : have < ((cl.z >> kAltNeedShift) & 15u)) return false;
         if (f != 0u) {
-          sat |= g;
+          cnt += static_cast<unsigned long long>(open) << sh;
           if (mode != PhraseMode::check) {
             const float4 k = __ldg(F.consts + cl.w);
             s = __fadd_rn(s, bm25(f, load_norm(S.norms, S.norm_width, d), k.x, k.y, k.z));

@@ -2361,7 +2361,8 @@ struct EmitJob {
 
 // The phrase pass's part of a count_run call (the plan's batch is the candidate batch of PhraseBatch::candidates): batch
 // query b's alternatives are [query_off[b] .. query_off[b + 1]), alternative j's slots slot_term / slot_rel
-// [clause_off[j] .. clause_off[j + 1]), with flags[j] = kAltNegated | group << 1 | kAltGuaranteed (bm25_phrase.cuh).
+// [clause_off[j] .. clause_off[j + 1]), with flags[j] = kAltNegated | group << 1 | kAltGuaranteed | (m - 1) <<
+// kAltMinShift (bm25_phrase.cuh); write adds each entry's need.
 // The job's queries are the batch's at positions qpos (null: all of them), so a
 // shape of a mixed batch runs the job of its own queries. k == 0: count only; else the top-k, scored with consts[j] =
 // {c0, norm_const, norm_length} per alternative and seeded with the key of threshold_in.
@@ -2507,9 +2508,9 @@ struct CountPlan {
   }
 
   // The bm25_count_kernel instantiation of this plan's launches in `mode`, with its dynamic shared memory: the mode's
-  // own bytes (facet bins, sorted keys, aggregate cells; none for a count), then the counter planes. phrased: the plan's
-  // batch is the candidates of phrase alternatives, checked by the phrase sink (CountMode::phrase) or before / in another
-  // sink.
+  // own bytes (facet bins, sorted keys, aggregate cells, the phrase sink's keys; none for a count), then the counter
+  // planes. phrased: the plan's batch is the candidates of phrase alternatives, checked by the phrase sink
+  // (CountMode::phrase) or before / in another sink.
   std::pair<CountKernel, size_t> kernel(CountMode mode, size_t mode_bytes, bool phrased = false) const {
     static const CountKernel kernels[3][5] = {   // [OR | AND | OR groups][count | sort | facet | agg | emit]
         {bm25_count_kernel<false>, bm25_count_kernel<false, false, true>, bm25_count_kernel<false, false, false, true>,
@@ -2530,9 +2531,9 @@ struct CountPlan {
          bm25_count_kernel<false, true, false, true, false, false, true>, bm25_count_kernel<false, true, false, false, true, false, true>,
          bm25_count_kernel<false, true, false, false, false, true, true>}};
     const int shape = Q.term_grp ? 2 : Q.kind == SDBG_QUERY_AND ? 1 : 0;
-    if (mode == CountMode::phrase) return {phrase_kernels[shape][0], mode_bytes};
-    if (phrased) return {phrase_kernels[shape][int(mode)], mode_bytes};   // candidate groups need 1 list: no counter planes
-    return {kernels[shape][int(mode)], mode_bytes + size_t(planes) * kCountWords * 4u};
+    const CountKernel k = mode == CountMode::phrase ? phrase_kernels[shape][0] : phrased ? phrase_kernels[shape][int(mode)]
+                                                                                          : kernels[shape][int(mode)];
+    return {k, mode_bytes + size_t(planes) * kCountWords * 4u};
   }
 };
 
@@ -2698,8 +2699,9 @@ void item_slots(const CountPlan& pl, char* h, size_t slot_off_pos, size_t slots_
 // slot's list {first BlockDesc, blocks, rel_pos, 0}, and each query's alternatives {first slot, slots, flags, alternative
 // index} in that segment's cost order, the smallest docs_count of the alternative's terms (a term the segment does not
 // hold costs 0), ascending, ties in query order: the order of a conjunction of the terms' lists
-// (conjunction.hpp:185-195), in which the scores of the matching positive alternatives are summed; the last positive
-// entry of each group gets kAltLast. conj: the job's candidates are the AND (every positive group one alternative), whose
+// (conjunction.hpp:185-195), in which the scores of the matching positive alternatives are summed; each positive entry
+// gets its `need` (kAltNeedShift) from the positive entries of its group after it. conj: the job's candidates are the AND
+// (every positive group one alternative), whose
 // walk (phrase_clauses<false>) reads the flags as the negated bit alone. Slots before the batch's first query's are left
 // as they are.
 void PhraseJob::write(sdbg_segment* const* segs, size_t n_segs, char* h, bool conj) const {
@@ -2736,10 +2738,12 @@ void PhraseJob::write(sdbg_segment* const* segs, size_t n_segs, char* h, bool co
       }
       std::stable_sort(E, E + n, [&](const uint4& x, const uint4& y) { return cost[x.w] < cost[y.w]; });
       if (conj) continue;
-      uint32_t seen = 0;
+      std::array<uint32_t, kMaxQueryTerms> after{};   // per group: its positive entries after entry i
       for (uint32_t i = n; i-- > 0;) {
-        const uint32_t g = 1u << ((E[i].z >> 1) & 15u);
-        if (!(E[i].z & kAltNegated) && !(seen & g)) { E[i].z |= kAltLast; seen |= g; }
+        if (E[i].z & kAltNegated) continue;
+        const uint32_t g = (E[i].z >> 1) & 15u, m = ((E[i].z >> kAltMinShift) & 15u) + 1u;
+        E[i].z |= (m > after[g] ? m - after[g] : 0u) << kAltNeedShift;
+        ++after[g];
       }
     }
   }
@@ -3111,7 +3115,8 @@ namespace {
 // The phrase entries' queries as their callers pass them. Query q is an AND of the groups [query_group_off[q] ..
 // query_group_off[q + 1]) (null: group q), group g an OR of the alternatives [group_off[g] .. group_off[g + 1]) (null:
 // alternative g), negated when group_neg[g] (null: none), alternative j the phrase of slots terms / rel_pos [clause_off[j]
-// .. clause_off[j + 1]) (rel_pos null: adjacent); excl_terms / excl_off as the flat entries take them.
+// .. clause_off[j + 1]) (rel_pos null: adjacent); excl_terms / excl_off as the flat entries take them. Positive group g
+// needs group_min[g] of its alternatives (null: 1).
 struct PhraseQueries {
   const uint32_t* terms;
   const uint32_t* rel_pos;
@@ -3122,24 +3127,32 @@ struct PhraseQueries {
   size_t nq;
   const uint32_t* excl_terms;
   const uint32_t* excl_off;
+  const uint32_t* group_min = nullptr;
 };
 
 // A batch of phrase queries (PhraseQueries), checked before anything is queued, with its candidate batch S: per query
 // a superset of its matches that the existing candidate scans find, which the alternative check then narrows exactly.
+// The groups are normalised first, as split_groups does for terms: a positive group that needs all its s alternatives is
+// s groups of one (qoff / goff / gneg / gmin hold the normalised groups, alternatives in the caller's order).
 //   every positive group has one alternative: the AND of the distinct terms of the positive groups (shape 1);
-//   else, exactly one group kept: the flat OR of its proxies (shape 0); otherwise OR groups of proxies (shape 2).
+//   else, exactly one group kept, needing one of its lists: the flat OR of its proxies (shape 0); otherwise OR groups of
+//   proxies (shape 2).
 // A positive group of one alternative contributes each of its distinct terms as a one-list group. A group of several
 // alternatives contributes, per one-slot alternative, its term, and per phrase alternative one of its terms, the cheapest
 // by docs_count summed over the call's segments among those the query has not used yet (none when the group holds one of
-// its terms already). A term stays in one group of a query, so a group that cannot avoid a repeat is left out and only
-// checked per doc. The one-alternative groups are always kept, and so is the first group of several when there are
-// none, so the candidate batch always holds a group. A group is
-// guaranteed (kAltGuaranteed) when it is kept and all its alternatives are one slot.
+// its terms already, which then stands for it). With c_l alternatives standing on list l, the group needs the least
+// number m' of its lists whose c_l, largest first, sum to its minimum m: a doc in which m alternatives occur is in all
+// their lists, and fewer than m' lists cannot carry m alternatives. A term stays in one group of a query, so a group that
+// cannot avoid a repeat is left out and only checked per doc. The one-alternative groups are always kept, and so is the
+// first group of several when there are none, so the candidate batch always holds a group. A group is guaranteed
+// (kAltGuaranteed) when it is kept, all its alternatives are one slot and, for m >= 2, no two of them share a term
+// (m' == m).
 // Per alternative j: flags[j] (PhraseJob); per query: its alternatives [aoff[q] .. aoff[q + 1]).
 struct PhraseBatch {
   int rc = SDBG_OK;
   size_t nq;
-  std::vector<uint32_t> rel, qoff, goff, aoff, flags;
+  std::vector<uint32_t> rel, qoff, goff, aoff, flags, gmin;
+  std::vector<uint8_t> gneg;
   const uint32_t* terms;
   const uint32_t* clause_off;
   GroupSplit<uint32_t> S;
@@ -3159,16 +3172,23 @@ struct PhraseBatch {
     goff.assign(size_t(qoff[nq]) + 1, 0u);
     for (uint32_t g = qoff[0]; g <= qoff[nq]; ++g) goff[g] = A.group_off ? A.group_off[g] : g;
     for (uint32_t g = qoff[0]; g < qoff[nq] && !rc; ++g) {
+      const uint32_t m = A.group_min ? A.group_min[g] : 1u;
       if (goff[g + 1] < goff[g]) rc = fail(c, SDBG_EINVAL, "group_off must be non-decreasing");
       else if (goff[g + 1] == goff[g]) rc = fail(c, SDBG_EINVAL, "empty OR group");
+      else if (m == 0u || m > goff[g + 1] - goff[g])
+        rc = fail(c, SDBG_EINVAL, "a group's minimum match count must be 1..its number of alternatives");
+      else if (m != 1u && A.group_neg && A.group_neg[g])
+        rc = fail(c, SDBG_EUNSUPPORTED, "a negated group with a minimum match count other than 1");
     }
+    if (rc) return;
+    normalise(A);
     for (uint32_t j = goff[qoff[0]]; j < goff[qoff[nq]] && !rc; ++j) {
       if (clause_off[j + 1] < clause_off[j]) rc = fail(c, SDBG_EINVAL, "clause_off must be non-decreasing");
       else if (clause_off[j + 1] == clause_off[j]) rc = fail(c, SDBG_EINVAL, "empty clause");
     }
     for (size_t q = 0; q < nq && !rc; ++q) {
       bool pos = false;
-      for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) pos |= !negated_group(A, g);
+      for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) pos |= !gneg[g];
       if (!pos) rc = fail(c, SDBG_EINVAL, "a query without a positive clause");
     }
     for (size_t q = 0; q < nq && !rc; ++q)
@@ -3181,9 +3201,9 @@ struct PhraseBatch {
     for (size_t q = 0; q <= nq; ++q) aoff[q] = goff[qoff[q]];
     for (size_t q = 0; q < nq; ++q) {
       for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) {
-        const bool neg = negated_group(A, g);
+        const bool neg = gneg[g];
         for (uint32_t j = goff[g]; j < goff[g + 1]; ++j) {
-          flags[j] = (neg ? kAltNegated : 0u) | ((g - qoff[q]) << 1);
+          flags[j] = (neg ? kAltNegated : 0u) | ((g - qoff[q]) << 1) | ((gmin[g] - 1u) << kAltMinShift);
           const uint32_t s0 = clause_off[j], s1 = clause_off[j + 1];
           for (uint32_t i = s0; i < s1; ++i) {
             rel[i] = A.rel_pos ? A.rel_pos[i] : i - s0;
@@ -3210,8 +3230,31 @@ struct PhraseBatch {
     if (!rc) candidates(segs, n_segs, A);
   }
 
-  static bool negated_group(const PhraseQueries& A, uint32_t g) { return A.group_neg && A.group_neg[g]; }
   uint32_t slots(uint32_t j) const { return clause_off[j + 1] - clause_off[j]; }
+
+  // Replaces the caller's groups (checked) with the normalised ones: a positive group of s >= 2 alternatives with
+  // minimum s becomes s groups of one.
+  void normalise(const PhraseQueries& A) {
+    std::vector<uint32_t> q2{0u}, g2;
+    gneg.clear();
+    gmin.clear();
+    for (size_t q = 0; q < nq; ++q) {
+      for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) {
+        const uint32_t s = goff[g + 1] - goff[g], m = A.group_min ? A.group_min[g] : 1u;
+        const bool neg = A.group_neg && A.group_neg[g];
+        const bool split = !neg && m == s;
+        for (uint32_t j = goff[g]; j < goff[g + 1]; j += split ? 1u : s) {
+          g2.push_back(j);
+          gneg.push_back(neg);
+          gmin.push_back(split ? 1u : m);
+        }
+      }
+      q2.push_back(uint32_t(g2.size()));
+    }
+    g2.push_back(goff[qoff[nq]]);
+    qoff = std::move(q2);
+    goff = std::move(g2);
+  }
 
   void candidates(sdbg_segment* const* segs, size_t n_segs, const PhraseQueries& A) {
     const auto docs = [&](uint32_t t) {
@@ -3223,57 +3266,66 @@ struct PhraseBatch {
     std::vector<std::vector<uint32_t>> groups;
     std::vector<uint32_t> used;
     const auto in = [](const std::vector<uint32_t>& v, uint32_t t) { return std::find(v.begin(), v.end(), t) != v.end(); };
+    std::vector<uint32_t> need;   // per kept group: its minimum number of lists m'
     for (size_t q = 0; q < nq; ++q) {
       groups.clear();
       used.clear();
+      need.clear();
       bool single = true;
       for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g)
-        if (!negated_group(A, g)) single &= goff[g + 1] - goff[g] == 1u;
+        if (!gneg[g]) single &= goff[g + 1] - goff[g] == 1u;
       for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) {
-        if (negated_group(A, g) || goff[g + 1] - goff[g] != 1u) continue;
+        if (gneg[g] || goff[g + 1] - goff[g] != 1u) continue;
         const uint32_t j = goff[g];
         for (uint32_t i = clause_off[j]; i < clause_off[j + 1]; ++i)
-          if (!in(used, terms[i])) { used.push_back(terms[i]); groups.push_back({terms[i]}); }
+          if (!in(used, terms[i])) { used.push_back(terms[i]); groups.push_back({terms[i]}); need.push_back(1u); }
         if (slots(j) == 1u) flags[j] |= kAltGuaranteed;
       }
       for (uint32_t g = qoff[q]; g < qoff[q + 1]; ++g) {
-        if (negated_group(A, g) || goff[g + 1] - goff[g] == 1u) continue;
-        std::vector<uint32_t> G;
+        if (gneg[g] || goff[g + 1] - goff[g] == 1u) continue;
+        std::vector<uint32_t> G, cnt;   // the group's lists and the alternatives standing on each
         bool ok = true, terms_only = true;
+        const auto stand = [&](uint32_t t) {
+          const size_t l = std::find(G.begin(), G.end(), t) - G.begin();
+          if (l == G.size()) { G.push_back(t); cnt.push_back(0u); }
+          ++cnt[l];
+        };
         for (uint32_t j = goff[g]; j < goff[g + 1] && ok; ++j) {
           if (slots(j) != 1u) { terms_only = false; continue; }
           const uint32_t t = terms[clause_off[j]];
-          if (in(G, t)) continue;
-          ok = !in(used, t);
-          G.push_back(t);
+          ok = in(G, t) || !in(used, t);
+          stand(t);
         }
         for (uint32_t j = goff[g]; j < goff[g + 1] && ok; ++j) {
           if (slots(j) == 1u) continue;
+          uint32_t best = 0, cover = 0;
           bool covered = false;
-          uint32_t best = 0;
           uint64_t best_docs = UINT64_MAX;
           for (uint32_t i = clause_off[j]; i < clause_off[j + 1]; ++i) {
-            covered |= in(G, terms[i]);
+            if (!covered && in(G, terms[i])) { covered = true; cover = terms[i]; }
             if (in(used, terms[i])) continue;
             const uint64_t n = docs(terms[i]);
             if (n < best_docs) { best_docs = n; best = terms[i]; }
           }
-          if (covered) continue;
-          ok = best_docs != UINT64_MAX;
-          G.push_back(best);
+          ok = covered || best_docs != UINT64_MAX;
+          if (ok) stand(covered ? cover : best);
         }
         if (!ok) continue;
+        std::sort(cnt.begin(), cnt.end(), std::greater<uint32_t>());
+        uint32_t m2 = 0;
+        for (uint32_t sum = 0; sum < gmin[g]; sum += cnt[m2++]) {}
         used.insert(used.end(), G.begin(), G.end());
         groups.push_back(std::move(G));
-        if (terms_only)
+        need.push_back(m2);
+        if (terms_only && (gmin[g] == 1u || m2 == gmin[g]))
           for (uint32_t j = goff[g]; j < goff[g + 1]; ++j) flags[j] |= kAltGuaranteed;
       }
-      const int sh = single ? 1 : groups.size() == 1 ? 0 : 2;
+      const int sh = single ? 1 : groups.size() == 1 && need[0] == 1u ? 0 : 2;
       S.qs[sh].push_back(uint32_t(q));
       for (size_t gi = 0; gi < groups.size(); ++gi)
         for (uint32_t t : groups[gi]) {
           S.terms[sh].push_back(t);
-          if (sh == 2) S.term_grp[sh].push_back(uint8_t(gi));
+          if (sh == 2) S.term_grp[sh].push_back(uint8_t(gi | ((need[gi] - 1u) << 4)));
         }
       S.term_off[sh].push_back(uint32_t(S.terms[sh].size()));
       if (A.excl_off)
@@ -3423,13 +3475,24 @@ extern "C" int sdbg_phrase_and_count_batch(sdbg_segment* const* segs, size_t n_s
                       filt, counts);
 }
 
-extern "C" int sdbg_phrase_groups_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                                              const uint32_t* clause_off, const uint32_t* group_off, const uint8_t* group_negated,
-                                              const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
-                                              const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
+extern "C" int sdbg_phrase_groups_count_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                  const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                                  const uint8_t* group_negated, const uint32_t* group_min,
+                                                  const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
+                                                  const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t* counts) {
   if (!group_off || !query_group_off) return SDBG_EINVAL;
-  return phrase_count(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off},
+  return phrase_count(segs, n_segs,
+                      {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off, group_min},
                       filt, counts);
+}
+
+extern "C" int sdbg_phrase_groups_count_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                              const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                              const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
+                                              const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                              uint64_t* counts) {
+  return sdbg_phrase_groups_count_batch_min(segs, n_segs, terms, rel_pos, clause_off, group_off, group_negated, nullptr,
+                                            query_group_off, nq, excl_terms, excl_off, filt, counts);
 }
 
 extern "C" int sdbg_phrase_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3450,15 +3513,29 @@ extern "C" int sdbg_phrase_and_topk_batch(sdbg_segment* const* segs, size_t n_se
                      clause_stats, k1, b, filt, k, threshold_in, out, n_out, total_matches);
 }
 
-extern "C" int sdbg_phrase_groups_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                                             const uint32_t* clause_off, const uint32_t* group_off, const uint8_t* group_negated,
-                                             const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
-                                             const uint32_t* excl_off, const sdbg_bm25_term* clause_stats, float k1, float b,
-                                             const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
-                                             uint64_t* total_matches) {
+extern "C" int sdbg_phrase_groups_topk_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                 const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                                 const uint8_t* group_negated, const uint32_t* group_min,
+                                                 const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
+                                                 const uint32_t* excl_off, const sdbg_bm25_term* clause_stats, float k1, float b,
+                                                 const sdbg_col_pred* filt, uint32_t k, float threshold_in, sdbg_hit* out,
+                                                 uint32_t* n_out, uint64_t* total_matches) {
   if (!group_off || !query_group_off) return SDBG_EINVAL;
-  return phrase_topk(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off},
+  return phrase_topk(segs, n_segs,
+                     {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off, group_min},
                      clause_stats, k1, b, filt, k, threshold_in, out, n_out, total_matches);
+}
+
+extern "C" int sdbg_phrase_groups_topk_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                             const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                             const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
+                                             const uint32_t* excl_terms, const uint32_t* excl_off,
+                                             const sdbg_bm25_term* clause_stats, float k1, float b, const sdbg_col_pred* filt,
+                                             uint32_t k, float threshold_in, sdbg_hit* out, uint32_t* n_out,
+                                             uint64_t* total_matches) {
+  return sdbg_phrase_groups_topk_batch_min(segs, n_segs, terms, rel_pos, clause_off, group_off, group_negated, nullptr,
+                                           query_group_off, nq, excl_terms, excl_off, clause_stats, k1, b, filt, k, threshold_in,
+                                           out, n_out, total_matches);
 }
 
 extern "C" int sdbg_phrase_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3479,15 +3556,29 @@ extern "C" int sdbg_phrase_and_topk_by_column_batch(sdbg_segment* const* segs, s
                                               excl_off}, filt, sort_field, descending, nulls_first, k, out, n_out);
 }
 
-extern "C" int sdbg_phrase_groups_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
-                                                       const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
-                                                       const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
-                                                       const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
-                                                       uint64_t sort_field, int descending, int nulls_first, uint32_t k,
-                                                       sdbg_sort_hit* out, uint32_t* n_out) {
+extern "C" int sdbg_phrase_groups_topk_by_column_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                           const uint32_t* rel_pos, const uint32_t* clause_off,
+                                                           const uint32_t* group_off, const uint8_t* group_negated,
+                                                           const uint32_t* group_min, const uint32_t* query_group_off, size_t nq,
+                                                           const uint32_t* excl_terms, const uint32_t* excl_off,
+                                                           const sdbg_col_pred* filt, uint64_t sort_field, int descending,
+                                                           int nulls_first, uint32_t k, sdbg_sort_hit* out, uint32_t* n_out) {
   if (!group_off || !query_group_off) return SDBG_EINVAL;
-  return phrase_topk_by_column(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms,
-                                              excl_off}, filt, sort_field, descending, nulls_first, k, out, n_out);
+  return phrase_topk_by_column(segs, n_segs,
+                               {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off, group_min},
+                               filt, sort_field, descending, nulls_first, k, out, n_out);
+}
+
+extern "C" int sdbg_phrase_groups_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                       const uint32_t* rel_pos, const uint32_t* clause_off,
+                                                       const uint32_t* group_off, const uint8_t* group_negated,
+                                                       const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
+                                                       const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t sort_field,
+                                                       int descending, int nulls_first, uint32_t k, sdbg_sort_hit* out,
+                                                       uint32_t* n_out) {
+  return sdbg_phrase_groups_topk_by_column_batch_min(segs, n_segs, terms, rel_pos, clause_off, group_off, group_negated, nullptr,
+                                                     query_group_off, nq, excl_terms, excl_off, filt, sort_field, descending,
+                                                     nulls_first, k, out, n_out);
 }
 
 extern "C" int sdbg_phrase_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3508,15 +3599,29 @@ extern "C" int sdbg_phrase_and_facet_counts_batch(sdbg_segment* const* segs, siz
                                             excl_off}, filt, key_field, key_min, key_span, counts, null_counts);
 }
 
-extern "C" int sdbg_phrase_groups_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
-                                                     const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
-                                                     const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
-                                                     const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
-                                                     uint64_t key_field, int64_t key_min, uint32_t key_span, uint64_t* counts,
-                                                     uint64_t* null_counts) {
+extern "C" int sdbg_phrase_groups_facet_counts_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                         const uint32_t* rel_pos, const uint32_t* clause_off,
+                                                         const uint32_t* group_off, const uint8_t* group_negated,
+                                                         const uint32_t* group_min, const uint32_t* query_group_off, size_t nq,
+                                                         const uint32_t* excl_terms, const uint32_t* excl_off,
+                                                         const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min,
+                                                         uint32_t key_span, uint64_t* counts, uint64_t* null_counts) {
   if (!group_off || !query_group_off) return SDBG_EINVAL;
-  return phrase_facet_counts(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms,
-                                            excl_off}, filt, key_field, key_min, key_span, counts, null_counts);
+  return phrase_facet_counts(segs, n_segs,
+                             {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off, group_min},
+                             filt, key_field, key_min, key_span, counts, null_counts);
+}
+
+extern "C" int sdbg_phrase_groups_facet_counts_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                     const uint32_t* rel_pos, const uint32_t* clause_off,
+                                                     const uint32_t* group_off, const uint8_t* group_negated,
+                                                     const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
+                                                     const uint32_t* excl_off, const sdbg_col_pred* filt, uint64_t key_field,
+                                                     int64_t key_min, uint32_t key_span, uint64_t* counts,
+                                                     uint64_t* null_counts) {
+  return sdbg_phrase_groups_facet_counts_batch_min(segs, n_segs, terms, rel_pos, clause_off, group_off, group_negated, nullptr,
+                                                   query_group_off, nq, excl_terms, excl_off, filt, key_field, key_min, key_span,
+                                                   counts, null_counts);
 }
 
 extern "C" int sdbg_phrase_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
@@ -3539,15 +3644,29 @@ extern "C" int sdbg_phrase_and_aggregate_batch(sdbg_segment* const* segs, size_t
                           filt, key_field, key_min, key_span, value_field, out, null_out);
 }
 
+extern "C" int sdbg_phrase_groups_aggregate_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                      const uint32_t* rel_pos, const uint32_t* clause_off,
+                                                      const uint32_t* group_off, const uint8_t* group_negated,
+                                                      const uint32_t* group_min, const uint32_t* query_group_off, size_t nq,
+                                                      const uint32_t* excl_terms, const uint32_t* excl_off,
+                                                      const sdbg_col_pred* filt, uint64_t key_field, int64_t key_min,
+                                                      uint32_t key_span, uint64_t value_field, sdbg_match_agg* out,
+                                                      sdbg_match_agg* null_out) {
+  if (!group_off || !query_group_off) return SDBG_EINVAL;
+  return phrase_aggregate(segs, n_segs,
+                          {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off, group_min},
+                          filt, key_field, key_min, key_span, value_field, out, null_out);
+}
+
 extern "C" int sdbg_phrase_groups_aggregate_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
                                                   const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
                                                   const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
                                                   const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
                                                   uint64_t key_field, int64_t key_min, uint32_t key_span, uint64_t value_field,
                                                   sdbg_match_agg* out, sdbg_match_agg* null_out) {
-  if (!group_off || !query_group_off) return SDBG_EINVAL;
-  return phrase_aggregate(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off},
-                          filt, key_field, key_min, key_span, value_field, out, null_out);
+  return sdbg_phrase_groups_aggregate_batch_min(segs, n_segs, terms, rel_pos, clause_off, group_off, group_negated, nullptr,
+                                                query_group_off, nq, excl_terms, excl_off, filt, key_field, key_min, key_span,
+                                                value_field, out, null_out);
 }
 
 extern "C" int sdbg_match_topk_by_column_batch(sdbg_segment* const* segs, size_t n_segs, int kind, const uint32_t* terms,
@@ -3844,15 +3963,28 @@ extern "C" int sdbg_phrase_and_scan_batch(sdbg_segment* const* segs, size_t n_se
                      filt, clause_stats, k1, b, offset, limit, scored, out, n_out, total);
 }
 
-extern "C" int sdbg_phrase_groups_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms, const uint32_t* rel_pos,
-                                             const uint32_t* clause_off, const uint32_t* group_off, const uint8_t* group_negated,
-                                             const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
-                                             const uint32_t* excl_off, const sdbg_col_pred* filt, const sdbg_bm25_term* clause_stats,
-                                             float k1, float b, const uint64_t* offset, uint32_t limit, int scored, sdbg_hit* out,
-                                             uint32_t* n_out, uint64_t* total) {
+extern "C" int sdbg_phrase_groups_scan_batch_min(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                                 const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                                 const uint8_t* group_negated, const uint32_t* group_min,
+                                                 const uint32_t* query_group_off, size_t nq, const uint32_t* excl_terms,
+                                                 const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                                 const sdbg_bm25_term* clause_stats, float k1, float b, const uint64_t* offset,
+                                                 uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
   if (!group_off || !query_group_off) return SDBG_EINVAL;
-  return phrase_scan(segs, n_segs, {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off},
+  return phrase_scan(segs, n_segs,
+                     {terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off, group_min},
                      filt, clause_stats, k1, b, offset, limit, scored, out, n_out, total);
+}
+
+extern "C" int sdbg_phrase_groups_scan_batch(sdbg_segment* const* segs, size_t n_segs, const uint32_t* terms,
+                                             const uint32_t* rel_pos, const uint32_t* clause_off, const uint32_t* group_off,
+                                             const uint8_t* group_negated, const uint32_t* query_group_off, size_t nq,
+                                             const uint32_t* excl_terms, const uint32_t* excl_off, const sdbg_col_pred* filt,
+                                             const sdbg_bm25_term* clause_stats, float k1, float b, const uint64_t* offset,
+                                             uint32_t limit, int scored, sdbg_hit* out, uint32_t* n_out, uint64_t* total) {
+  return sdbg_phrase_groups_scan_batch_min(segs, n_segs, terms, rel_pos, clause_off, group_off, group_negated, nullptr,
+                                           query_group_off, nq, excl_terms, excl_off, filt, clause_stats, k1, b, offset, limit,
+                                           scored, out, n_out, total);
 }
 
 // ---- the count, facet, aggregate and sorted passes across GPUs ----

@@ -944,9 +944,28 @@ def _phrase_groups(queries, exclude_phrases):
     return out
 
 
-def _phrase_groups_args(groups, exclude):
+def _phrase_group_min(min_match, queries, groups):
+    """group_min u32 indexed like the group_off of _phrase_groups_args: min_match[q] gives one minimum per group of
+    queries[q], in order, and the negated groups of exclude_phrases take 1 (None: None)."""
+    if min_match is None:
+        return None
+    if len(min_match) != len(queries) or any(len(m) != len(q) for m, q in zip(min_match, queries)):
+        raise ValueError("min_match needs one value per group of each query")
+    if any(int(v) < 0 for m in min_match for v in m):
+        raise ValueError("a minimum match count is 1..its group's number of alternatives")
+    return np.ascontiguousarray([int(v) for m, g in zip(min_match, groups) for v in list(m) + [1] * (len(g) - len(m))],
+                                dtype=np.uint32)
+
+
+def _phrase_groups_entry(name, gmin):
+    """The OR-group entry `name`, or its _min form when there are minimums."""
+    return getattr(N.lib(), name if gmin is None else name + "_min")
+
+
+def _phrase_groups_args(groups, exclude, gmin=None):
     """(terms, rel_pos, clause_off, group_off, group_negated, query_group_off, nq, excl_terms, excl_off) of the OR-group
-    entries, and the arrays they point into (kept alive by the caller)."""
+    entries, with group_min after group_negated when gmin is given (_phrase_group_min), and the arrays they point into
+    (kept alive by the caller)."""
     nq = len(groups)
     flat_g = [g for q in groups for g in q]
     flat = [a for alts, _ in flat_g for a in alts]
@@ -960,8 +979,9 @@ def _phrase_groups_args(groups, exclude):
     qoff = np.zeros(nq + 1, np.uint32)
     qoff[1:] = np.cumsum([len(q) for q in groups])
     x = _exclusions(exclude, nq) or (None, None)
-    keep = (terms, rel, coff, goff, neg, qoff, x)
-    return (_ptr(terms), _ptr(rel), _ptr(coff), _ptr(goff), _ptr(neg), _ptr(qoff), nq, _ptr(x[0]), _ptr(x[1])), keep
+    keep = (terms, rel, coff, goff, neg, qoff, x, gmin)
+    mins = () if gmin is None else (_ptr(gmin),)
+    return (_ptr(terms), _ptr(rel), _ptr(coff), _ptr(goff), _ptr(neg), *mins, _ptr(qoff), nq, _ptr(x[0]), _ptr(x[1])), keep
 
 
 def _alternative_stats(reader, groups, scorer, boost):
@@ -970,128 +990,140 @@ def _alternative_stats(reader, groups, scorer, boost):
     return (N.BM25Term * max(len(flat), 1))(*[N.BM25Term() if n else reader.phrase_stats(scorer, ts, boost) for ts, n in flat])
 
 
-def ExecutePhraseGroupsCountBatch(reader, queries, filt=None, exclude=None, exclude_phrases=None):
+def ExecutePhraseGroupsCountBatch(reader, queries, filt=None, exclude=None, exclude_phrases=None, min_match=None):
     """Count of conjunctions of OR groups of phrases and terms (`("new york" | nyc) & pizza & !"deep dish"`,
     sdbg_phrase_groups_count_batch). queries: per query its groups, each a list of alternatives; an alternative is a list
     of term ids (a phrase of adjacent words; one id: a plain term) or a pair (term ids, rel_pos). exclude_phrases: per
     query negated alternatives in the same form (or None), each excluded on its own; exclude: per query excluded term ids,
     as in ExecutePhraseCountBatch. A doc matches when every group has an alternative that occurs in it and no negated
-    alternative does. Returns uint64[Q]."""
+    alternative does. min_match: per query one minimum per group of queries[q] (`2 of ("new york" | nyc | "big apple")`:
+    a doc needs that many of the group's alternatives, each counted on its own), 1..the group's size, run through
+    sdbg_phrase_groups_count_batch_min; None: 1 everywhere. The other OR-group functions take it alike. Returns
+    uint64[Q]."""
     groups = _phrase_groups(queries, exclude_phrases)
-    args, keep = _phrase_groups_args(groups, exclude)
+    gmin = _phrase_group_min(min_match, queries, groups)
+    args, keep = _phrase_groups_args(groups, exclude, gmin)
     counts = np.zeros(len(queries), np.uint64)
-    N.check(N.lib().sdbg_phrase_groups_count_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), _ptr(counts)),
-            reader.segments[0].ctx._h)
+    entry = _phrase_groups_entry("sdbg_phrase_groups_count_batch", gmin)
+    N.check(entry(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), _ptr(counts)), reader.segments[0].ctx._h)
     return counts
 
 
-def ExecutePhraseGroupsCount(reader, query, filt=None, exclude=None, exclude_phrases=None):
+def ExecutePhraseGroupsCount(reader, query, filt=None, exclude=None, exclude_phrases=None, min_match=None):
     """ExecutePhraseGroupsCountBatch for one query: its match count as an int."""
-    return int(ExecutePhraseGroupsCountBatch(reader, [list(query)], filt, _one(exclude), _one(exclude_phrases))[0])
+    return int(ExecutePhraseGroupsCountBatch(reader, [list(query)], filt, _one(exclude), _one(exclude_phrases),
+                                             _one(min_match))[0])
 
 
 def ExecutePhraseGroupsTopKBatch(reader, queries, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, exclude_phrases=None,
-                                 boost=1.0):
+                                 boost=1.0, min_match=None):
     """Top-k of OR-group queries (sdbg_phrase_groups_topk_batch): a match scores the sum of the scores of its positive
     alternatives that occur in it, each bm25(phrase frequency, norm) with IndexReader.phrase_stats of that alternative.
     Returns (hits [Q, k] structured, n_out [Q], total_matches [Q]) as ExecuteTopKBatch."""
     groups = _phrase_groups(queries, exclude_phrases)
-    args, keep = _phrase_groups_args(groups, exclude)
+    gmin = _phrase_group_min(min_match, queries, groups)
+    args, keep = _phrase_groups_args(groups, exclude, gmin)
     stats = _alternative_stats(reader, groups, scorer, boost)
     nq = len(queries)
     hits = np.zeros((nq, k), HIT_DTYPE)
     n_out = np.zeros(nq, np.uint32)
     total = np.zeros(nq, np.uint64)
-    N.check(N.lib().sdbg_phrase_groups_topk_batch(_seg_array(reader.segments), len(reader.segments), *args, stats, scorer.k, scorer.b,
-                                                  _ref(filt), int(k), float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)),
-            reader.segments[0].ctx._h)
+    entry = _phrase_groups_entry("sdbg_phrase_groups_topk_batch", gmin)
+    N.check(entry(_seg_array(reader.segments), len(reader.segments), *args, stats, scorer.k, scorer.b, _ref(filt), int(k),
+                  float(threshold), _ptr(hits), _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
     return hits, n_out, total
 
 
-def ExecutePhraseGroupsTopK(reader, query, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, exclude_phrases=None, boost=1.0):
+def ExecutePhraseGroupsTopK(reader, query, scorer, k, filt=None, threshold=FLT_MIN, exclude=None, exclude_phrases=None, boost=1.0,
+                            min_match=None):
     """ExecutePhraseGroupsTopKBatch for one query: (hits [n_out], total_matches)."""
     hits, n_out, total = ExecutePhraseGroupsTopKBatch(reader, [list(query)], scorer, k, filt, threshold, _one(exclude),
-                                                      _one(exclude_phrases), boost)
+                                                      _one(exclude_phrases), boost, _one(min_match))
     return hits[0, :n_out[0]], int(total[0])
 
 
 def ExecutePhraseGroupsTopKByColumnBatch(reader, queries, sort_field, k, descending=False, nulls_first=False, filt=None,
-                                         exclude=None, exclude_phrases=None):
+                                         exclude=None, exclude_phrases=None, min_match=None):
     """Sorted scan of OR-group queries (sdbg_phrase_groups_topk_by_column_batch): the first k of the docs
     ExecutePhraseGroupsCountBatch counts, in the order of ExecuteTopKByColumnBatch. Returns its dict."""
     vt = _sort_value_type(reader, sort_field)
     groups = _phrase_groups(queries, exclude_phrases)
-    args, keep = _phrase_groups_args(groups, exclude)
+    gmin = _phrase_group_min(min_match, queries, groups)
+    args, keep = _phrase_groups_args(groups, exclude, gmin)
     nq = len(queries)
     hits = np.zeros(max(nq, 1) * max(int(k), 1), SORT_HIT_DTYPE)
     n_out = np.zeros(max(nq, 1), np.uint32)
-    N.check(N.lib().sdbg_phrase_groups_topk_by_column_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt),
-                                                            int(sort_field), int(bool(descending)), int(bool(nulls_first)), int(k),
-                                                            _ptr(hits), _ptr(n_out)), reader.segments[0].ctx._h)
+    entry = _phrase_groups_entry("sdbg_phrase_groups_topk_by_column_batch", gmin)
+    N.check(entry(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), int(sort_field), int(bool(descending)),
+                  int(bool(nulls_first)), int(k), _ptr(hits), _ptr(n_out)), reader.segments[0].ctx._h)
     return _sort_result(hits, n_out, nq, k, vt)
 
 
 def ExecutePhraseGroupsTopKByColumn(reader, query, sort_field, k, descending=False, nulls_first=False, filt=None, exclude=None,
-                                    exclude_phrases=None):
+                                    exclude_phrases=None, min_match=None):
     """ExecutePhraseGroupsTopKByColumnBatch for one query: dict of docs, segs, values, nulls."""
     return _sort_row(ExecutePhraseGroupsTopKByColumnBatch(reader, [list(query)], sort_field, k, descending, nulls_first, filt,
-                                                          _one(exclude), _one(exclude_phrases)))
+                                                          _one(exclude), _one(exclude_phrases), _one(min_match)))
 
 
 def ExecutePhraseGroupsFacetCountsBatch(reader, queries, key_field, key_min=None, key_span=None, filt=None, exclude=None,
-                                        exclude_phrases=None):
+                                        exclude_phrases=None, min_match=None):
     """Facet counts of OR-group queries (sdbg_phrase_groups_facet_counts_batch): how the docs
     ExecutePhraseGroupsCountBatch counts split over the values of column `key_field`. Returns the dict
     ExecuteFacetCountsBatch returns."""
     key_min, key_span = _facet_key_range(reader, key_field, key_min, key_span)
     groups = _phrase_groups(queries, exclude_phrases)
-    args, keep = _phrase_groups_args(groups, exclude)
+    gmin = _phrase_group_min(min_match, queries, groups)
+    args, keep = _phrase_groups_args(groups, exclude, gmin)
     nq = len(queries)
     counts = np.zeros((max(nq, 1), max(int(key_span), 1)), np.uint64)
     nulls = np.zeros(max(nq, 1), np.uint64)
-    N.check(N.lib().sdbg_phrase_groups_facet_counts_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt),
-                                                          int(key_field), int(key_min), int(key_span), _ptr(counts), _ptr(nulls)),
-            reader.segments[0].ctx._h)
+    entry = _phrase_groups_entry("sdbg_phrase_groups_facet_counts_batch", gmin)
+    N.check(entry(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), int(key_field), int(key_min),
+                  int(key_span), _ptr(counts), _ptr(nulls)), reader.segments[0].ctx._h)
     return dict(key_min=int(key_min), counts=counts[:nq], nulls=nulls[:nq])
 
 
 def ExecutePhraseGroupsFacetCounts(reader, query, key_field, key_min=None, key_span=None, filt=None, exclude=None,
-                                   exclude_phrases=None):
+                                   exclude_phrases=None, min_match=None):
     """ExecutePhraseGroupsFacetCountsBatch for one query: {key: count} plus {None: n} for NULL keys."""
     return _facet_row(ExecutePhraseGroupsFacetCountsBatch(reader, [list(query)], key_field, key_min, key_span, filt, _one(exclude),
-                                                          _one(exclude_phrases)))
+                                                          _one(exclude_phrases), _one(min_match)))
 
 
 def ExecutePhraseGroupsMatchAggregatesBatch(reader, queries, value_field, key_field=None, key_min=None, key_span=None, filt=None,
-                                            exclude=None, exclude_phrases=None):
+                                            exclude=None, exclude_phrases=None, min_match=None):
     """Aggregates over the matches of OR-group queries (sdbg_phrase_groups_aggregate_batch): over the docs
     ExecutePhraseGroupsCountBatch counts; the grouping and the result as in ExecuteMatchAggregatesBatch."""
     vt, kf, key_min, key_span = _agg_args(reader, value_field, key_field, key_min, key_span)
     groups = _phrase_groups(queries, exclude_phrases)
-    args, keep = _phrase_groups_args(groups, exclude)
+    gmin = _phrase_group_min(min_match, queries, groups)
+    args, keep = _phrase_groups_args(groups, exclude, gmin)
     nq = len(queries)
     out = np.zeros((max(nq, 1), max(int(key_span), 1)), MATCH_AGG_DTYPE)
     null_out = np.zeros(max(nq, 1), MATCH_AGG_DTYPE)
-    N.check(N.lib().sdbg_phrase_groups_aggregate_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), kf,
-                                                       int(key_min), int(key_span), int(value_field), _ptr(out), _ptr(null_out)),
-            reader.segments[0].ctx._h)
+    entry = _phrase_groups_entry("sdbg_phrase_groups_aggregate_batch", gmin)
+    N.check(entry(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), kf, int(key_min), int(key_span),
+                  int(value_field), _ptr(out), _ptr(null_out)), reader.segments[0].ctx._h)
     return _agg_result(out, null_out, nq, key_min, vt)
 
 
 def ExecutePhraseGroupsMatchAggregates(reader, query, value_field, key_field=None, key_min=None, key_span=None, filt=None,
-                                       exclude=None, exclude_phrases=None):
+                                       exclude=None, exclude_phrases=None, min_match=None):
     """ExecutePhraseGroupsMatchAggregatesBatch for one query, in the form ExecuteMatchAggregates returns."""
     return _agg_row(ExecutePhraseGroupsMatchAggregatesBatch(reader, [list(query)], value_field, key_field, key_min, key_span, filt,
-                                                            _one(exclude), _one(exclude_phrases)), key_field is not None)
+                                                            _one(exclude), _one(exclude_phrases), _one(min_match)),
+                    key_field is not None)
 
 
 def ExecutePhraseGroupsMatchScanBatch(reader, queries, scorer=None, limit=1 << 20, offset=None, filt=None, exclude=None,
-                                      exclude_phrases=None, boost=1.0):
+                                      exclude_phrases=None, boost=1.0, min_match=None):
     """Stream mode of OR-group queries (sdbg_phrase_groups_scan_batch): the docs ExecutePhraseGroupsCountBatch counts, in
     (segment, doc) order, from ordinal offset[q] (None: 0) on, at most `limit` of them, scored as
     ExecutePhraseGroupsTopKBatch scores them (scorer None: unscored). Returns what ExecuteMatchScanGroupsBatch returns."""
     groups = _phrase_groups(queries, exclude_phrases)
-    args, keep = _phrase_groups_args(groups, exclude)
+    gmin = _phrase_group_min(min_match, queries, groups)
+    args, keep = _phrase_groups_args(groups, exclude, gmin)
     nq = len(queries)
     stats = None if scorer is None else _alternative_stats(reader, groups, scorer, boost)
     offs = None if offset is None else np.ascontiguousarray(offset, dtype=np.uint64)
@@ -1101,18 +1133,18 @@ def ExecutePhraseGroupsMatchScanBatch(reader, queries, scorer=None, limit=1 << 2
     n_out = np.zeros(nq, np.uint32)
     total = np.zeros(nq, np.uint64)
     k1, b = (0.0, 0.0) if scorer is None else (scorer.k, scorer.b)
-    N.check(N.lib().sdbg_phrase_groups_scan_batch(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), stats, k1, b,
-                                                  _ptr(offs), int(limit), int(scorer is not None), _ptr(hits), _ptr(n_out),
-                                                  _ptr(total)), reader.segments[0].ctx._h)
+    entry = _phrase_groups_entry("sdbg_phrase_groups_scan_batch", gmin)
+    N.check(entry(_seg_array(reader.segments), len(reader.segments), *args, _ref(filt), stats, k1, b, _ptr(offs), int(limit),
+                  int(scorer is not None), _ptr(hits), _ptr(n_out), _ptr(total)), reader.segments[0].ctx._h)
     return [((hits["seg"][q, :n_out[q]].copy(), hits["doc"][q, :n_out[q]].copy(), hits["score"][q, :n_out[q]].copy()),
              int(total[q])) for q in range(nq)]
 
 
 def ExecutePhraseGroupsMatchScan(reader, query, scorer=None, limit=1 << 20, offset=0, filt=None, exclude=None, exclude_phrases=None,
-                                 boost=1.0):
+                                 boost=1.0, min_match=None):
     """ExecutePhraseGroupsMatchScanBatch for one query: ((seg, doc, score) arrays, total matches)."""
     return ExecutePhraseGroupsMatchScanBatch(reader, [list(query)], scorer, limit, [offset], filt, _one(exclude),
-                                             _one(exclude_phrases), boost)[0]
+                                             _one(exclude_phrases), boost, _one(min_match))[0]
 
 
 SORT_HIT_DTYPE =np.dtype([("value", "<i8"), ("doc", "<u4"), ("seg", "<u4"), ("is_null", "u1"), ("pad", "V7")])

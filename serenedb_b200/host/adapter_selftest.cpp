@@ -14,7 +14,9 @@
 // (tests/test_gpu_phrase.py); "phrase columns" runs the same phrases through the sorted, facet, aggregate and Stream
 // adapters instead (tests/test_gpu_phrase_column.py); "phrase and" runs conjunctions of phrases, terms and negated phrases
 // (clause_sizes / clause_negated) through all six phrase adapters (tests/test_gpu_phrase_and.py); "phrase groups" runs
-// conjunctions of OR groups of phrases and terms (clause_group_sizes too) through them (tests/test_gpu_phrase_groups.py).
+// conjunctions of OR groups of phrases and terms (clause_group_sizes too) through them (tests/test_gpu_phrase_groups.py);
+// "phrase min" runs OR groups of phrases and terms with minimum match counts (group_min_match per clause group) through
+// them (tests/test_gpu_phrase_min_match.py).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -44,8 +46,9 @@ struct ListCollector final : irs::ScoreCollector {  // a trivial ScoreCollector:
 // slots, clause_negated); each line holds its slots, positions, sizes, negations and excluded terms, then the top-50
 // (GpuTopKIterator), total and count (GpuCountScan), the sorted docs, the facet keys and counts, the aggregate count
 // and the scored scan's docs, scores and total, as above. With `groups` ("phrase groups") the cases are And of OR groups of
-// clauses (clause_group_sizes), and each line also holds the group sizes ("gsizes").
-int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns, bool clauses, bool groups) {
+// clauses (clause_group_sizes), and each line also holds the group sizes ("gsizes"). With `mins` ("phrase min") the cases
+// are And of OR groups with minimum match counts (group_min_match), and each line also holds them ("gmin").
+int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns, bool clauses, bool groups, bool mins) {
   uint32_t state = 12345u;
   auto next = [&]() { state = state * 1664525u + 1013904223u; return state >> 16; };
   constexpr uint32_t kVocab = 6;
@@ -100,7 +103,7 @@ int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns, bool clauses, bool
   irs::ScoreFunction sf; irs::ColumnArgsFetcher fetcher;
   if (clauses) {
     // "1 0" & 2;  "2 2" & 4 & !"3 1" & !5;  0 & 1 & !3
-    struct AndCase { std::vector<uint32_t> slots, rel, sizes; std::vector<uint8_t> neg; std::vector<uint32_t> excl, gsizes; };
+    struct AndCase { std::vector<uint32_t> slots, rel, sizes; std::vector<uint8_t> neg; std::vector<uint32_t> excl, gsizes, gmin; };
     const std::vector<AndCase> and_cases = {{{1, 0, 2}, {0, 1, 0}, {2, 1}, {0, 0}, {}, {}},
                                             {{2, 2, 4, 3, 1}, {0, 1, 0, 0, 1}, {2, 1, 2}, {0, 0, 1}, {5}, {}},
                                             {{0, 1, 3}, {0, 0, 0}, {1, 1, 1}, {0, 0, 1}, {}, {}}};
@@ -108,7 +111,12 @@ int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns, bool clauses, bool
     const std::vector<AndCase> group_cases = {{{1, 0, 2, 4}, {0, 1, 0, 0}, {2, 1, 1}, {0, 0, 0}, {}, {2, 1}},
                                               {{2, 2, 3, 3, 1, 5}, {0, 1, 0, 0, 1, 0}, {2, 1, 2, 1}, {0, 0, 1, 1}, {}, {2, 2}},
                                               {{0, 1, 4, 1, 2, 3}, {0, 0, 1, 0, 0, 0}, {1, 2, 1, 1, 1}, {0, 0, 0, 0, 1}, {5}, {2, 2, 1}}};
-    for (const AndCase& cs : groups ? group_cases : and_cases) {
+    // 2 of ("1 0" | 2 | 4);  2 of ("2 2" | 3 | "1 4") & !("3 1" | 5);  3 of (0 | 1 | 2 | 3) & (4 | "5 0") & !5
+    const std::vector<AndCase> min_cases = {
+        {{1, 0, 2, 4}, {0, 1, 0, 0}, {2, 1, 1}, {0, 0, 0}, {}, {3}, {2}},
+        {{2, 2, 3, 1, 4, 3, 1, 5}, {0, 1, 0, 0, 1, 0, 1, 0}, {2, 1, 2, 2, 1}, {0, 0, 0, 1, 1}, {}, {3, 2}, {2, 1}},
+        {{0, 1, 2, 3, 4, 5, 0}, {0, 0, 0, 0, 0, 0, 1}, {1, 1, 1, 1, 1, 2}, {0, 0, 0, 0, 0, 0}, {5}, {4, 2}, {3, 1}}};
+    for (const AndCase& cs : mins ? min_cases : groups ? group_cases : and_cases) {
       std::vector<sdbg_bm25_term> terms(cs.slots.size());
       for (size_t i = 0; i < terms.size(); ++i) {
         sdbg_bm25_collect(n_docs, sum_len, docs[cs.slots[i]].size(), 1.2f, 0.75f, &terms[i]);
@@ -119,32 +127,35 @@ int phrase_mode(sdbg_ctx* ctx, uint32_t n_docs, bool columns, bool clauses, bool
       std::printf("]");
       ints("rel", cs.rel); ints("sizes", cs.sizes); ints("neg", cs.neg); ints("excl", cs.excl);
       if (groups) ints("gsizes", cs.gsizes);
-      sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_AND, terms, 1.2f, 0.75f, 50, nullptr, cs.excl, {}, {}, cs.rel, cs.sizes, cs.neg,
-                                  cs.gsizes);
+      if (mins) ints("gmin", cs.gmin);
+      sdbg_host::GpuTopKIterator it(seg, SDBG_QUERY_AND, terms, 1.2f, 0.75f, 50, nullptr, cs.excl, {}, cs.gmin, cs.rel, cs.sizes,
+                                  cs.neg, cs.gsizes);
       col.docs.clear();
       it.Collect(sf, fetcher, col);
       std::printf(", \"topk\": [");
       for (size_t i = 0; i < col.docs.size(); ++i) std::printf("%s[%u, %.9g]", i ? ", " : "", col.docs[i].doc, double(col.docs[i].score));
       std::printf("], \"total\": %llu", static_cast<unsigned long long>(it.total_matches()));
       duckdb::DataChunkMock out;
-      sdbg_host::GpuCountScan cnt({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, {}, {}, cs.rel, cs.sizes, cs.neg, cs.gsizes);
+      sdbg_host::GpuCountScan cnt({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, {}, cs.gmin, cs.rel, cs.sizes, cs.neg, cs.gsizes);
       cnt.Scan(out);
       std::printf(", \"count\": %lld", static_cast<long long>(out.count.empty() ? -1 : out.count[0]));
-      sdbg_host::GpuSortedScan sorted({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, 20, true, false, 30, {}, {}, cs.rel, cs.sizes,
-                                      cs.neg, cs.gsizes);
+      sdbg_host::GpuSortedScan sorted({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, 20, true, false, 30, {}, cs.gmin, cs.rel,
+                                      cs.sizes, cs.neg, cs.gsizes);
       for (sorted.Scan(out); out.size; sorted.Scan(out)) ints("sorted_docs", out.doc);
-      sdbg_host::GpuFacetScan facet({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, 20, {}, {}, cs.rel, cs.sizes, cs.neg, cs.gsizes);
+      sdbg_host::GpuFacetScan facet({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, 20, {}, cs.gmin, cs.rel, cs.sizes, cs.neg,
+                                    cs.gsizes);
       std::vector<int64_t> keys, counts;
       for (facet.Scan(out); out.size; facet.Scan(out)) {
         keys.insert(keys.end(), out.key.begin(), out.key.end());
         counts.insert(counts.end(), out.count.begin(), out.count.end());
       }
       ints("facet_keys", keys); ints("facet_counts", counts);
-      sdbg_host::GpuMatchAggScan agg({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, UINT64_MAX, 20, SDBG_I64, {}, {}, cs.rel,
+      sdbg_host::GpuMatchAggScan agg({seg}, SDBG_QUERY_AND, cs.slots, cs.excl, nullptr, UINT64_MAX, 20, SDBG_I64, {}, cs.gmin, cs.rel,
                                      cs.sizes, cs.neg, cs.gsizes);
       agg.Scan(out);
       ints("agg_count", out.count);
-      sdbg_host::GpuMatchScan scan({seg}, terms, cs.excl, nullptr, 1.2f, 0.75f, true, {}, {}, cs.rel, cs.sizes, cs.neg, cs.gsizes);
+      sdbg_host::GpuMatchScan scan({seg}, terms, cs.excl, nullptr, 1.2f, 0.75f, true, {}, cs.gmin, cs.rel, cs.sizes, cs.neg,
+                                   cs.gsizes);
       std::vector<uint32_t> sdocs;
       std::vector<float> sscores;
       for (scan.Scan(out); out.size; scan.Scan(out)) {
@@ -227,8 +238,9 @@ int main(int argc, char** argv) {
   if (rc != SDBG_OK) { std::printf("{\"error\": %d}\n", rc); return rc == SDBG_ENODEVICE ? 3 : 1; }
   if (argc > 2 && std::string(argv[2]) == "phrase")
     return phrase_mode(ctx, n_docs, argc > 3 && std::string(argv[3]) == "columns",
-                       argc > 3 && (std::string(argv[3]) == "and" || std::string(argv[3]) == "groups"),
-                       argc > 3 && std::string(argv[3]) == "groups");
+                       argc > 3 && (std::string(argv[3]) == "and" || std::string(argv[3]) == "groups" || std::string(argv[3]) == "min"),
+                       argc > 3 && (std::string(argv[3]) == "groups" || std::string(argv[3]) == "min"),
+                       argc > 3 && std::string(argv[3]) == "min");
   sdbg_segment* seg = nullptr;
   sdbg_segment_create(ctx, n_docs, &seg);
   std::vector<uint32_t> dc(8);

@@ -25,7 +25,14 @@ const uint32_t* group_minimums(const std::vector<uint32_t>& mins, size_t n_group
   return mins.data();
 }
 
-// A phrase's relative positions: one per slot and no OR groups (the library checks their order).
+// Per clause group of a phrase query (group_neg: one entry per group) its minimum match count, or none (every group 1).
+const uint32_t* phrase_minimums(const std::vector<uint32_t>& mins, const std::vector<uint8_t>& group_neg) {
+  if (mins.empty()) return nullptr;
+  if (mins.size() != group_neg.size()) throw GpuError(SDBG_EINVAL, "one minimum match count per clause group");
+  return mins.data();
+}
+
+// A phrase's relative positions: one per slot and no OR groups of terms (the library checks their order).
 void check_phrase(const std::vector<uint32_t>& phrase, size_t n_terms, bool groups) {
   if (phrase.empty()) return;
   if (phrase.size() != n_terms) throw GpuError(SDBG_EINVAL, "one phrase position per term");
@@ -115,6 +122,7 @@ GpuTopKIterator::GpuTopKIterator(sdbg_segment* segment, int kind, std::vector<sd
   check_phrase(phrase_, terms_.size(), !groups_.empty());
   phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
                  group_off_, group_neg_);
+  if (!phrase_.empty()) phrase_minimums(group_min_, group_neg_);
   if (!phrase_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "phrases need k > 0: the streaming scan has no phrase form");
   // the streaming scan (sdbg_bm25_scan*) has no grouped form
   if (!groups_.empty() && k_ == 0) throw GpuError(SDBG_EUNSUPPORTED, "OR groups need k > 0: the streaming scan has no grouped form");
@@ -151,10 +159,11 @@ void GpuTopKIterator::run() {
     const std::vector<uint32_t> ids = term_ids(terms_);
     const std::vector<sdbg_bm25_term> stats = clause_stats(terms_, clause_off_, clause_neg_);
     const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())}, excl_off[2] = {0, uint32_t(excluded_.size())};
-    check(sdbg_phrase_groups_topk_batch(segs, 1, ids.data(), phrase_.data(), clause_off_.data(), group_off_.data(), group_neg_.data(), query_group_off, 1,
-                                     excluded_.data(), excl_off, stats.data(), k1_, b_, filter_.data(), k_, threshold_.value,
-                                     hits_.data(), &n, &total_),
-          "sdbg_phrase_groups_topk_batch");
+    check(sdbg_phrase_groups_topk_batch_min(segs, 1, ids.data(), phrase_.data(), clause_off_.data(), group_off_.data(),
+                                            group_neg_.data(), phrase_minimums(group_min_, group_neg_), query_group_off, 1,
+                                            excluded_.data(), excl_off, stats.data(), k1_, b_, filter_.data(), k_, threshold_.value,
+                                            hits_.data(), &n, &total_),
+          "sdbg_phrase_groups_topk_batch_min");
     thr_out = n == k_ ? hits_[k_ - 1].score : threshold_.value;
   } else if (!groups_.empty()) {
     const std::vector<uint32_t> group_off = group_offsets(groups_, terms_.size());
@@ -301,6 +310,7 @@ GpuCountScan::GpuCountScan(std::vector<sdbg_segment*> segments, int kind, std::v
   check_phrase(phrase_, terms_.size(), !groups_.empty());
   phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
                  group_off_, group_neg_);
+  if (!phrase_.empty()) phrase_minimums(group_min_, group_neg_);
 }
 
 void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
@@ -313,9 +323,10 @@ void GpuCountScan::Scan(duckdb::DataChunkMock& output) {
   const char* what;
   if (!phrase_.empty()) {
     const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
-    rc = sdbg_phrase_groups_count_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), group_off_.data(), group_neg_.data(),
-                                     query_group_off, 1, excluded_.data(), excl_off, filter_.data(), &n);
-    what = "sdbg_phrase_groups_count_batch: ";
+    rc = sdbg_phrase_groups_count_batch_min(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
+                                            group_off_.data(), group_neg_.data(), phrase_minimums(group_min_, group_neg_),
+                                            query_group_off, 1, excluded_.data(), excl_off, filter_.data(), &n);
+    what = "sdbg_phrase_groups_count_batch_min: ";
   } else if (groups_.empty()) {
     rc = sdbg_match_count_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                 filter_.data(), &n);
@@ -346,6 +357,7 @@ GpuSortedScan::GpuSortedScan(std::vector<sdbg_segment*> segments, int kind, std:
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
   phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
                  group_off_, group_neg_);
+  if (!phrase_.empty()) phrase_minimums(group_min_, group_neg_);
 }
 
 void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
@@ -359,10 +371,11 @@ void GpuSortedScan::Scan(duckdb::DataChunkMock& output) {
     const char* what;
     if (!phrase_.empty()) {
       const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
-      rc = sdbg_phrase_groups_topk_by_column_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), group_off_.data(),
-                                                group_neg_.data(), query_group_off, 1, excluded_.data(), excl_off, filter_.data(),
-                                                field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_, hits_.data(), &n);
-      what = "sdbg_phrase_groups_topk_by_column_batch: ";
+      rc = sdbg_phrase_groups_topk_by_column_batch_min(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
+                                                       group_off_.data(), group_neg_.data(), phrase_minimums(group_min_, group_neg_),
+                                                       query_group_off, 1, excluded_.data(), excl_off, filter_.data(), field_,
+                                                       desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_, hits_.data(), &n);
+      what = "sdbg_phrase_groups_topk_by_column_batch_min: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_topk_by_column_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                            filter_.data(), field_, desc_ ? 1 : 0, nulls_first_ ? 1 : 0, k_,
@@ -403,9 +416,10 @@ GpuMatchScan::GpuMatchScan(std::vector<sdbg_segment*> segments, std::vector<sdbg
       group_sizes_(group_sizes.empty() ? std::vector<uint32_t>{uint32_t(terms_.size())} : std::move(group_sizes)),
       group_min_(std::move(group_min_match)), phrase_(std::move(phrase_positions)), filter_(table_filter), k1_(k1), b_(b),
       scored_(scored) {
-  check_phrase(phrase_, terms_.size(), group_sizes_.size() > 1 || !group_min_.empty());
+  check_phrase(phrase_, terms_.size(), group_sizes_.size() > 1);
   phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
                  group_off_, group_neg_);
+  if (!phrase_.empty()) phrase_minimums(group_min_, group_neg_);
 }
 
 void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kPage - 1
@@ -420,10 +434,12 @@ void GpuMatchScan::Fetch() {   // the next page: matches offset_ .. offset_ + kP
     const std::vector<uint32_t> ids = term_ids(terms_);
     const std::vector<sdbg_bm25_term> stats = clause_stats(terms_, clause_off_, clause_neg_);
     const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
-    rc = sdbg_phrase_groups_scan_batch(segs_.data(), segs_.size(), ids.data(), phrase_.data(), clause_off_.data(), group_off_.data(), group_neg_.data(),
-                                    query_group_off, 1, excluded_.data(), excl_off, filter_.data(), scored_ ? stats.data() : nullptr,
-                                    k1_, b_, &offset_, kPage, scored_ ? 1 : 0, page_.data(), &n, &total_);
-    what = "sdbg_phrase_groups_scan_batch: ";
+    rc = sdbg_phrase_groups_scan_batch_min(segs_.data(), segs_.size(), ids.data(), phrase_.data(), clause_off_.data(),
+                                           group_off_.data(), group_neg_.data(), phrase_minimums(group_min_, group_neg_),
+                                           query_group_off, 1, excluded_.data(), excl_off, filter_.data(),
+                                           scored_ ? stats.data() : nullptr, k1_, b_, &offset_, kPage, scored_ ? 1 : 0,
+                                           page_.data(), &n, &total_);
+    what = "sdbg_phrase_groups_scan_batch_min: ";
   } else {
     rc = sdbg_match_scan_batch_groups_min(segs_.data(), segs_.size(), terms_.data(), group_off.data(), query_group_off,
                                           group_minimums(group_min_, group_sizes_.size()), 1, excluded_.data(), excl_off,
@@ -463,6 +479,7 @@ GpuFacetScan::GpuFacetScan(std::vector<sdbg_segment*> segments, int kind, std::v
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
   phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
                  group_off_, group_neg_);
+  if (!phrase_.empty()) phrase_minimums(group_min_, group_neg_);
 }
 
 void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
@@ -487,10 +504,11 @@ void GpuFacetScan::Scan(duckdb::DataChunkMock& output) {
     const char* what;
     if (!phrase_.empty()) {
       const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
-      rc = sdbg_phrase_groups_facet_counts_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), group_off_.data(),
-                                              group_neg_.data(), query_group_off, 1, excluded_.data(), excl_off, filter_.data(),
-                                              field_, lo, uint32_t(span), counts.data(), &nulls_);
-      what = "sdbg_phrase_groups_facet_counts_batch: ";
+      rc = sdbg_phrase_groups_facet_counts_batch_min(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
+                                                     group_off_.data(), group_neg_.data(), phrase_minimums(group_min_, group_neg_),
+                                                     query_group_off, 1, excluded_.data(), excl_off, filter_.data(), field_, lo,
+                                                     uint32_t(span), counts.data(), &nulls_);
+      what = "sdbg_phrase_groups_facet_counts_batch_min: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_facet_counts_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                          filter_.data(), field_, lo, uint32_t(span), counts.data(), &nulls_);
@@ -533,6 +551,7 @@ GpuMatchAggScan::GpuMatchAggScan(std::vector<sdbg_segment*> segments, int kind, 
   check_phrase(phrase_, terms_.size(), !group_sizes_.empty());
   phrase_clauses(phrase_, terms_.size(), clause_sizes, clause_negated, clause_group_sizes, clause_off_, clause_neg_,
                  group_off_, group_neg_);
+  if (!phrase_.empty()) phrase_minimums(group_min_, group_neg_);
 }
 
 void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
@@ -564,10 +583,11 @@ void GpuMatchAggScan::Scan(duckdb::DataChunkMock& output) {
     const char* what;
     if (!phrase_.empty()) {
       const uint32_t query_group_off[2] = {0, uint32_t(group_neg_.size())};
-      rc = sdbg_phrase_groups_aggregate_batch(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(), group_off_.data(),
-                                           group_neg_.data(), query_group_off, 1, excluded_.data(), excl_off, filter_.data(),
-                                           key_field_, lo, uint32_t(span), value_field_, cells.data(), &null_cell);
-      what = "sdbg_phrase_groups_aggregate_batch: ";
+      rc = sdbg_phrase_groups_aggregate_batch_min(segs_.data(), segs_.size(), terms_.data(), phrase_.data(), clause_off_.data(),
+                                                  group_off_.data(), group_neg_.data(), phrase_minimums(group_min_, group_neg_),
+                                                  query_group_off, 1, excluded_.data(), excl_off, filter_.data(), key_field_, lo,
+                                                  uint32_t(span), value_field_, cells.data(), &null_cell);
+      what = "sdbg_phrase_groups_aggregate_batch_min: ";
     } else if (group_sizes_.empty()) {
       rc = sdbg_match_aggregate_batch(segs_.data(), segs_.size(), kind_, terms_.data(), term_off, 1, excluded_.data(), excl_off,
                                       filter_.data(), key_field_, lo, uint32_t(span), value_field_, cells.data(),

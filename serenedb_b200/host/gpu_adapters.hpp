@@ -50,7 +50,9 @@ class GpuTopKIterator final : public irs::DocIterator {
                   const sdbg_col_pred* table_filter /* nullable: the ColFilter wrap */,
                   std::vector<uint32_t> excluded_terms = {} /* term ids of the And's Not children (irs exclusion.hpp) */,
                   std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */,
-                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1.
+                    With phrase_positions: one per clause group (per clause_group_sizes, or per clause when that is
+                    empty), 1..its clauses, 1 for a negated group; another size: GpuError(SDBG_EINVAL) */,
 
                   std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
                                                                  relative positions (0 first, increasing); needs k > 0 */,
@@ -137,7 +139,9 @@ class GpuCountScan {
   GpuCountScan(std::vector<sdbg_segment*> segments, int kind /* SDBG_QUERY_OR | SDBG_QUERY_AND */, std::vector<uint32_t> terms,
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors: consecutive OR groups over `terms`; empty = flat */,
-               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1.
+                 With phrase_positions: one per clause group (per clause_group_sizes, or per clause when that is
+                 empty), 1..its clauses, 1 for a negated group; another size: GpuError(SDBG_EINVAL) */,
 
                std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
                                                               relative positions (0 first, increasing) */,
@@ -170,7 +174,9 @@ class GpuSortedScan {
                 uint64_t sort_field, bool descending, bool nulls_first /* the plan's resolved OrderByNullType */,
                 uint32_t k /* LIMIT (+ OFFSET), 1..4096 */,
                 std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
-                std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+                std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1.
+                  With phrase_positions: one per clause group (per clause_group_sizes, or per clause when that is
+                  empty), 1..its clauses, 1 for a negated group; another size: GpuError(SDBG_EINVAL) */,
 
                 std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
                                                                relative positions (0 first, increasing) */,
@@ -208,7 +214,9 @@ class GpuMatchScan {
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
                float k1, float b, bool scored,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors over `terms`; empty = one group (a flat OR) */,
-               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1.
+                 With phrase_positions: one per clause group (per clause_group_sizes, or per clause when that is
+                 empty), 1..its clauses, 1 for a negated group; another size: GpuError(SDBG_EINVAL) */,
 
                std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
                                                               relative positions (0 first, increasing) */,
@@ -247,7 +255,9 @@ class GpuFacetScan {
                std::vector<uint32_t> excluded_terms /* the And's Not children */, const sdbg_col_pred* table_filter /* nullable */,
                uint64_t key_field /* int64 or int32 */,
                std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
-               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+               std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1.
+                 With phrase_positions: one per clause group (per clause_group_sizes, or per clause when that is
+                 empty), 1..its clauses, 1 for a negated group; another size: GpuError(SDBG_EINVAL) */,
 
                std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
                                                               relative positions (0 first, increasing) */,
@@ -287,7 +297,9 @@ class GpuMatchAggScan {
                   uint64_t key_field /* int64 or int32; UINT64_MAX: no GROUP BY */, uint64_t value_field,
                   sdbg_type value_type /* as staged: picks sum_f64 or the 128-bit sum for avg */,
                   std::vector<uint32_t> group_sizes = {} /* an And of Ors, as GpuCountScan takes it; kind is then unused */,
-                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1 */,
+                  std::vector<uint32_t> group_min_match = {} /* per group: Or::min_match_count, 1..its size; empty = all 1.
+                    With phrase_positions: one per clause group (per clause_group_sizes, or per clause when that is
+                    empty), 1..its clauses, 1 for a negated group; another size: GpuError(SDBG_EINVAL) */,
 
                   std::vector<uint32_t> phrase_positions = {} /* non-empty: `terms` are a by_phrase's slots at these
                                                                  relative positions (0 first, increasing) */,

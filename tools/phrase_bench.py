@@ -24,10 +24,12 @@ expansion produces: --queries queries each of `("w1 w2" | s) & t`, `"w1 w2" | s`
 s a token of another doc, t a token of the phrase's doc (s, w1 and t distinct), next to `"w1 w2" & t` (phrase-and) and
 `(w1 | s) & t` (the OR-group count, top-k and facets of sdbg_*_groups). The proxy candidates of `"w1 w2" | s` are the
 docs of w1 or w2 (the cheaper) or s, wider than the phrase's own AND.
+A fifth batch, "phrase-min", times minimum match counts over such groups (sdbg_phrase_groups_*_batch_min):
+`2 of ("w1 w2" | s | t)`, `2 of ("w1 w2" | s | t) & u` and `2 of ("w1 w2" | s | "w3 w4")`, count, top-1000 and facets.
 --batches picks the batches to run (comma-separated; all by default).
 Prints one JSON line with the GPU name and power limit read in the same run.
 
-    python tools/phrase_bench.py [--steps 5] [--warmup 2] [--docs 10000000] [--queries 4096] [--batches 2-word,phrase-and,phrase-groups]
+    python tools/phrase_bench.py [--steps 5] [--warmup 2] [--docs 10000000] [--queries 4096] [--batches 2-word,phrase-and,phrase-groups,phrase-min]
 """
 import argparse
 import json
@@ -174,6 +176,41 @@ def phrase_groups_rows(c, reader, ctx, scorer, n, rng, steps, warmup):
     return r
 
 
+def phrase_min_rows(c, reader, ctx, scorer, n, rng, steps, warmup):
+    """The "phrase-min" batch: `2 of ("w1 w2" | s | t)`, `2 of ("w1 w2" | s | t) & u` and `2 of ("w1 w2" | s | "w3 w4")`
+    (sdbg_phrase_groups_*_batch_min): s, t and u occur near the phrase in its doc, so the minimums are met often."""
+    terms, doc = c["terms"], c["doc"]
+    ph, near = [], []
+    while len(ph) < n:
+        i = int(rng.integers(0, len(terms) - 2))
+        if doc[i] != doc[i + 1]:
+            continue
+        same = np.flatnonzero(doc[max(0, i - 28):i + 30] == doc[i]) + max(0, i - 28)
+        s, t, u = (int(terms[int(same[int(rng.integers(0, len(same)))])]) for _ in range(3))
+        if len({int(terms[i]), int(terms[i + 1]), s, t, u}) < 5:
+            continue
+        ph.append([int(terms[i]), int(terms[i + 1])]); near.append((s, t, u))
+    w34 = phrases(c, n, 2, rng)
+    two = [[[p, [s], [t]]] for p, (s, t, _) in zip(ph, near)]
+    two_u = [[[p, [s], [t]], [[u]]] for p, (s, t, u) in zip(ph, near)]
+    two_ph = [[[p, [s], q]] for p, (s, _, _), q in zip(ph, near, w34)]
+    r = {}
+    for name, q, m in (("two", two, [[2]] * n), ("two_and_u", two_u, [[2, 1]] * n), ("two_phrases", two_ph, [[2]] * n)):
+        cnt = sdb.ExecutePhraseGroupsCountBatch(reader, q, min_match=m)
+        one = sdb.ExecutePhraseGroupsCountBatch(reader, q)
+        _, _, tt = sdb.ExecutePhraseGroupsTopKBatch(reader, q, scorer, 1000, min_match=m)
+        fac = sdb.ExecutePhraseGroupsFacetCountsBatch(reader, q, 2, 0, 100, min_match=m)
+        if not np.array_equal(tt, cnt) or not np.array_equal(fac["counts"].sum(1), cnt) or np.any(cnt > one):
+            raise SystemExit("phrase-min count / top-k / facet mismatch")
+        r[name + "_matches"] = int(cnt.sum())
+        r[name + "_count_ms"] = timed(ctx, lambda: sdb.ExecutePhraseGroupsCountBatch(reader, q, min_match=m), steps, warmup)
+        r[name + "_top1000_ms"] = timed(ctx, lambda: sdb.ExecutePhraseGroupsTopKBatch(reader, q, scorer, 1000, min_match=m), steps,
+                                        warmup)
+        r[name + "_facets_ms"] = timed(ctx, lambda: sdb.ExecutePhraseGroupsFacetCountsBatch(reader, q, 2, 0, 100, min_match=m), steps,
+                                       warmup)
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
@@ -181,7 +218,7 @@ def main():
     ap.add_argument("--docs", type=int, default=10_000_000)
     ap.add_argument("--vocab", type=int, default=100_000)
     ap.add_argument("--queries", type=int, default=4096)
-    ap.add_argument("--batches", default="2-word,3/4-word,phrase-and,phrase-groups")
+    ap.add_argument("--batches", default="2-word,3/4-word,phrase-and,phrase-groups,phrase-min")
     a = ap.parse_args()
     want = set(a.batches.split(","))
     c = corpus(a.docs, a.vocab, 7)
@@ -239,6 +276,8 @@ def main():
     if "phrase-groups" in want:
         out["batches"]["phrase-groups"] = phrase_groups_rows(c, reader, ctx, scorer, a.queries, np.random.default_rng(19), a.steps,
                                                              a.warmup)
+    if "phrase-min" in want:
+        out["batches"]["phrase-min"] = phrase_min_rows(c, reader, ctx, scorer, a.queries, np.random.default_rng(23), a.steps, a.warmup)
     print(json.dumps(out))
 
 
